@@ -32,14 +32,6 @@ METRIC = "training-step rays/sec at n_obj x n_rays x n_samples"
 IMAP_RAYS, IMAP_SAMPLES, IMAP_HIDDEN = 4800, 32, 256                # BASELINE configs[4]
 IMAP_FLOP_PER_POINT = 6 * (4 * IMAP_HIDDEN * IMAP_HIDDEN + 220 * IMAP_HIDDEN + 63)
 
-# tcgen05.mma cycles (M=128, K=16, both operands from shared memory) measured by tools/umma_bench2.cu on this pool's
-# B200 (profiles/r02_umma_bench2.txt), and the fused kernel's MMA mix per 128-lane tile (k_step_fused.cuh: forward 23 x
-# N32 + 4 x N16, dgrad 10 x N32 + 4 x N96 + 2 x N48, wgrad 40 x N32 + 16 x N16): the tensor-pipe time floor of THIS
-# decomposition, i.e. the shape-limited peak the achieved FLOP/s is also reported against.
-MMA_CYCLES = {16: 36.0, 32: 40.0, 48: 44.0, 96: 56.0}
-MMA_MIX = {32: 73, 16: 20, 96: 4, 48: 2}
-
-
 def log(msg):
     """Progress on stderr (stdout carries exactly one JSON line)."""
     print(f"[bench rank {os.environ.get('RANK', '0')}] {msg}", file=sys.stderr, flush=True)
@@ -50,30 +42,18 @@ def workload_name(world):
     return f"vMAP {N_OBJ} objects per GPU x {N_RAYS} rays x {N_SAMPLES} samples, hidden {HIDDEN} (BASELINE cfg 2 per GPU)"
 
 
-def k1_dram_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of the step kernel, from this round's committed
-    `ncu --set full` summary of the same command (a profiler cannot run inside the timed benchmark)."""
-    f = os.path.join(ROOT, "profiles", "r02_k_step_fused_ncu_summary.txt")
-    if not os.path.isfile(f):
-        return None
-    tot, seen = 0.0, 0
-    mult = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    for ln in open(f):
-        for key in ("dram__bytes_read.sum [", "dram__bytes_write.sum ["):
-            if ln.startswith(key):
-                unit = ln[len(key):ln.index("]")]
-                tot += float(ln.split("=")[1]) * mult.get(unit, 1.0)
-                seen += 1
-    return tot if seen == 2 else None
+# NVIDIA's data sheet for the H100 SXM (dense fp16 tensor TFLOP/s, HBM3 GB/s): the roofline denominators.  They are
+# data-sheet figures for a 700 W card, not rates this benchmark reached.
+H100_FP16_TFLOPS, H100_HBM_GBS = 989.0, 3350.0
 
 
-def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.isfile(p):
-        d = json.load(open(p))
-        return (d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0),
-                d.get("sm_max_mhz", 1965.0), "measured")
-    return 1590.0, 1400.0, 6650.0, 1965.0, "fallback"
+def dump_outputs(out_dir, ens):
+    """What the timed path handed its caller in its last step: the per-object loss terms and the updated parameter
+    block (float32, a few hundred KB), one .npy each."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss_terms.npy"), ens.loss_terms.detach().float().cpu().numpy())
+    np.save(os.path.join(out_dir, "params.npy"), ens.params.detach().float().cpu().numpy())
 
 
 class ClockSampler:
@@ -98,11 +78,16 @@ class ClockSampler:
         for ln in self.proc.stdout:
             self.lines.append((time.time(), ln.strip()))
 
+    def terminate(self):
+        if self.proc is not None and self.proc.poll() is None:
+            self.proc.terminate()
+            self.proc.wait()
+
     def stop(self, t0, t1):
         if self.proc is None:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.12)
-        self.proc.terminate()
+        self.terminate()
         rows = [l for (t, l) in self.lines if t0 - 0.05 <= t <= t1 + 0.05] or [l for _, l in self.lines]
         sm, mx, reasons = [], None, set()
         for l in rows:
@@ -387,16 +372,23 @@ def run_ours(args):
     sampler = ClockSampler(local)                 # runs for the whole process; windowed to the timed arms below
     if rank == 0:
         sampler.start()
+    try:
+        _run_ours_timed(args, torch, dist, vo, VmapEnsemble, world, rank, dev, impl, fused, sampler)
+    finally:
+        sampler.terminate()                       # never leave the nvidia-smi poller behind
+
+
+def _run_ours_timed(args, torch, dist, vo, VmapEnsemble, world, rank, dev, impl, fused, sampler):
     B, R, S = N_OBJ, N_RAYS, N_SAMPLES            # per GPU (weak scaling)
     params = vo.init_params(B, HIDDEN, seed=1000 + rank)
     ens = VmapEnsemble(B, hidden=HIDDEN, scale=2.0, device=dev, impl=impl)
     ens.load_stacked(params)
 
-    # input pool larger than L2 (126 MB): every step reads a different, cold batch.  One flat
+    # input pool larger than L2 (50 MB): every step reads a different, cold batch.  One flat
     # buffer per batch (pinned on the host) so a step's inputs move with a single H2D copy.
     from vmap_b200.ensemble import StepInputs
     step_bytes = B * R * S * 16 + B * R * 18
-    n_pool = max(8, int(140e6 // step_bytes) + 1)
+    n_pool = max(8, int(64e6 // step_bytes) + 1)
     host_pool = []
     for i in range(n_pool):
         host_pool.append(StepInputs(B, R, S, pinned=True).fill(vo.synthetic_batch(B, R, S, seed=rank * 100003 + i)))
@@ -447,6 +439,8 @@ def run_ours(args):
     ms_total = max_over_ranks(e0.elapsed_time(e1))
     ens.check_status()
     log(f"device-resident arm: {ms_total / K * 1e3:.1f} us/step")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ens)
 
     # ---- same steps launched eagerly with CUDA events around the step kernel (roofline) ----
     k1_events = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(K)]
@@ -508,17 +502,9 @@ def run_ours(args):
         barrier()
 
     if rank == 0:
-        bf16_burst, bf16_sust, hbm, sm_max_mhz, src = peaks()
         rays_total = world * B * R * K
         flop_k1 = FLOP_PER_POINT * B * R * S
         achieved = flop_k1 / (k1_avg_ms * 1e-3) / 1e12
-        # tensor-pipe floor of this decomposition: tiles/SM x MMA cycles per tile at the measured issue cost
-        rpw = 32 // S
-        tiles = B * ((R + 4 * rpw - 1) // (4 * rpw))
-        n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
-        cyc_tile = sum(MMA_CYCLES[n] * c for n, c in MMA_MIX.items())
-        floor_us = (tiles / n_sm) * cyc_tile / (sm_max_mhz * 1e6) * 1e6
-        peak_shape = flop_k1 / (floor_us * 1e-6) / 1e12
         line = {
             "metric": METRIC, "value": rays_total / (ms_total * 1e-3), "unit": "rays/s", "n_gpus": world,
             "steps": K, "warmup": W, "ms_per_step": ms_total / K, "higher_is_better": True, "scaling": "weak",
@@ -527,7 +513,7 @@ def run_ours(args):
                 "workload": workload_name(world),
                 "global_objects": world * B, "parallelism": f"object-sharded x{world}, no collective in the step",
                 "precision": "fp16 tensor-core operands, fp32 accumulate, fp32 master weights / Adam / render / loss",
-                "impl": impl, "l2": f"input pool of {n_pool} distinct batches ({n_pool * step_bytes / 1e6:.0f} MB > 126 MB L2)",
+                "impl": impl, "l2": f"input pool of {n_pool} distinct batches ({n_pool * step_bytes / 1e6:.0f} MB > 50 MB L2)",
                 "launch": ("CUDA graph of the step (one kernel) per input buffer" if fused else "CUDA graph of K0+K1+K2 per input buffer")
                           if use_graphs else "eager launches",
                 "d2h": "per-object loss terms copied to pinned host memory every step (async), one sync at the end",
@@ -536,20 +522,14 @@ def run_ours(args):
                     "h2d_bytes_per_step": host_pool[0].nbytes, "d2h_bytes_per_step": B * 16,
                     "pipeline": "double-buffered staging: H2D of step i+1 on a copy stream overlaps step i"},
             "gpu_launches": (1 if fused else 3) * K,
-            "roofline": {"bound": "tensor", "achieved": achieved, "peak": bf16_burst, "unit": "TFLOP/s",
-                         "frac": achieved / bf16_burst,
-                         "traffic": k1_dram_traffic() if fused and world == 1 else None,
-                         "traffic_source": "profiles/r02_k_step_fused_ncu_summary.txt (ncu --set full of this command)",
-                         "peak_source": src + " bf16 burst",
-                         "peak_sustained": bf16_sust, "kernel": "k_step_fused" if fused else ("k_step_fp32" if impl == "fp32" else "layer-wise"),
+            "roofline": {"bound": "tensor", "achieved": achieved, "peak": H100_FP16_TFLOPS, "unit": "TFLOP/s",
+                         "frac": achieved / H100_FP16_TFLOPS, "peak_source": "H100 SXM data sheet, dense fp16 at 700 W",
+                         "kernel": "k_step_fused" if fused else "k_step_fp32",
                          "kernel_does": "mask counts + PE + MLP + render + loss + backward + ordered gradient reduction + AdamW" if fused else "K1 only",
                          "kernel_us": k1_avg_ms * 1e3, "kernel_us_median": k1_ms[len(k1_ms) // 2] * 1e3,
                          "flop_per_launch": flop_k1,
-                         "peak_shape_limited": peak_shape, "frac_shape_limited": achieved / peak_shape,
-                         "shape_limited_note": f"{tiles} tiles of 128 lanes over {n_sm} SMs x {cyc_tile:.0f} tensor-pipe cycles per tile "
-                                               f"(tcgen05.mma M128 K16: N32 {MMA_CYCLES[32]:.0f}, N16 {MMA_CYCLES[16]:.0f}, N96 {MMA_CYCLES[96]:.0f}, N48 {MMA_CYCLES[48]:.0f} "
-                                               f"cycles, profiles/r02_umma_bench2.txt) at {sm_max_mhz:.0f} MHz = {floor_us:.1f} us floor",
-                         "hbm_algorithmic_GBps": (B * R * S * 16 + B * R * 18 + 24 * B * 11363) / (k1_avg_ms * 1e-3) / 1e9, "hbm_peak": hbm},
+                         "hbm_algorithmic_GBps": (B * R * S * 16 + B * R * 18 + 24 * B * 11363) / (k1_avg_ms * 1e-3) / 1e9,
+                         "hbm_peak": H100_HBM_GBS},
             "clocks": clocks,
         }
         line.update(extras)
@@ -571,8 +551,14 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-extras", action="store_true", help="skip the configs[4] / drop-in / frame-loop arms")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's loss terms and parameters (rank 0) to "
+                         "DIR/<name>.npy; they follow warmup + steps updates, so compare runs with the same --warmup and "
+                         "--steps.  Not available with --impl reference")
     args = ap.parse_args()
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs applies to the GPU arm only")
         run_reference(args)
     else:
         run_ours(args)

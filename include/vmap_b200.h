@@ -1,5 +1,5 @@
 /*
- * vmap_b200 -- C ABI of the B200-native vMAP training-step library (libvmap_b200.so).
+ * vmap_b200 -- C ABI of the H100-native (sm_90a) vMAP training-step library (libvmap_b200.so).
  *
  * The reference (kxhit/vMAP) is pure Python and has no FFI; its "operator interface"
  * for this path is the set of call sites in train.py.  Each entry point below replaces
@@ -40,9 +40,9 @@ enum {
 enum {
   VMB_IMPL_AUTO = 0,
   VMB_IMPL_FP32 = 1,    /* CUDA-core fp32 kernel, any hidden size (parity anchor)            */
-  VMB_IMPL_UMMA = 2,    /* tcgen05/TMEM fp16-operand fused kernel, hidden = 32 (the fast path): counts, step,
+  VMB_IMPL_UMMA = 2,    /* wgmma fp16-operand fused kernel, hidden = 32 (the fast path): counts, step,
                            gradient reduction and (with fuse_adam) AdamW in ONE launch, n_samples <= 32        */
-  VMB_IMPL_LAYERWISE = 3 /* tcgen05 GEMM per layer over all points, hidden = 64/128/256 (bg / iMAP) */
+  VMB_IMPL_LAYERWISE = 3 /* wgmma GEMM per layer over all points, hidden = 64/128/256 (bg / iMAP) */
 };
 
 /* status word bits (vmb_step_args.status / vmb_adam_args.status, device int[4]) */
@@ -176,8 +176,8 @@ typedef struct vmb_forward_args {
   float* alpha;  long long alpha_stride;
   float* colour; long long colour_stride;
   const void* image;   /* optional fp16 weight image (vmb_image_bytes per object, kept current by vmb_adam /
-                          vmb_build_image): hidden 32 then runs the forward half of the fused tcgen05 kernel,
-                          hidden 64/128/256 the layer-wise tcgen05 GEMMs; NULL = fp32 CUDA-core kernel          */
+                          vmb_build_image): hidden 32 then runs the forward half of the fused wgmma kernel,
+                          hidden 64/128/256 the layer-wise wgmma GEMMs; NULL = fp32 CUDA-core kernel          */
 } vmb_forward_args;
 
 int vmb_forward(vmb_handle* h, const vmb_forward_args* a, void* stream);
@@ -262,7 +262,7 @@ typedef struct vmb_ingest_args {
 int vmb_ingest_frame(vmb_handle* h, const vmb_ingest_args* a, void* stream);
 
 /* ---- bring-up / test hook (not part of the reference-facing surface) --------------------------- */
-/* Generic tcgen05 GEMM of the layer-wise wide-model path: D[M][N] = A[M][K1+K2] * B[N][K]^T, fp16 in,
+/* Generic wgmma GEMM of the layer-wise wide-model path: D[M][N] = A[M][K1+K2] * B[N][K]^T, fp16 in,
  * fp32 accumulate.  a_mn/b_mn = 0: operand stored [rows][ld] with K contiguous; 1: stored [K][ld] with
  * M/N contiguous.  epi 0: out16 = relu(acc*scale + bias); 2: out32 (=|+=) acc*scale; 3: atomicAdd;
  * epi + 16 selects the weight-stationary kernel (a_mn = 0, N <= 256).                                */

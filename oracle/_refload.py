@@ -1,4 +1,5 @@
-"""Import the UNMODIFIED reference modules from /root/reference (build container only).
+"""Import the UNMODIFIED reference modules from a checkout of the reference (golden generators only;
+set VMAP_REFERENCE_ROOT to its directory, default: ``reference`` beside this repository).
 
 TEST INFRASTRUCTURE ONLY.  The reference's non-numeric imports (open3d, trimesh,
 skimage, imgviz, bidict) are absent from this image; they are replaced by
@@ -14,7 +15,8 @@ import sys
 import types
 from unittest.mock import MagicMock
 
-REF_ROOT = os.environ.get("VMAP_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("VMAP_REFERENCE_ROOT") or os.path.join(
+    os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), "reference")
 
 
 def available() -> bool:

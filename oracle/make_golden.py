@@ -1,6 +1,6 @@
-"""Generate tests/golden/*.npz from the UNMODIFIED reference (build container only).
+"""Generate tests/golden/*.npz from the UNMODIFIED reference (needs a reference checkout, see oracle/_refload.py).
 
-Run:  python -m oracle.make_golden        (needs /root/reference; no GPU)
+Run:  python -m oracle.make_golden        (no GPU)
 
 The reference has no tests or golden vectors of its own (SURVEY.md section 4), so these
 fixtures are what pins parity: they are produced by the reference's own

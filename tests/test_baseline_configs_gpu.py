@@ -51,8 +51,8 @@ def test_cfg2_cfg3_many_objects_umma_vs_oracle(n_obj):
         ga, gu = g_ref[k].cuda(), u.view(k, u.grads)
         per_obj = ((ga - gu).flatten(1).norm(dim=1) / (ga.flatten(1).norm(dim=1) + 1e-20))
         # The losses are L1: d|x|/dx = sign(x) flips for rays whose residual is within the fp16 forward noise,
-        # so a few objects with few contributing rays show large relative differences (deterministic, see
-        # tools/diag160.py); the bulk must agree closely and the whole-stack gradient within the kernel's bar.
+        # so a few objects with few contributing rays show large relative differences (deterministic);
+        # the bulk must agree closely and the whole-stack gradient within the kernel's bar.
         q90 = float(per_obj.kthvalue(max(1, int(0.9 * n_obj))).values)
         print(k, 'per-object grad rel-L2: median', float(per_obj.median()), 'p90', q90, 'max', float(per_obj.max()),
               'stack', rel_l2(gu, ga))

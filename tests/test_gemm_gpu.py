@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 GEMMs (TMA-fed SWIZZLE_128B stages; generic tiled and weight-stationary kernels) of the
+"""GPU: the wgmma GEMMs (TMA-fed SWIZZLE_128B stages; generic tiled and weight-stationary kernels) of the
 layer-wise wide-model path against torch.matmul, for the operand layouts / epilogues the path uses."""
 import ctypes as C
 

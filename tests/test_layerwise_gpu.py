@@ -93,7 +93,7 @@ def test_layerwise_speed_vs_fp32_kernel_imap_shape():
 
 @pytest.mark.parametrize("H,N", [(128, 3000), (64, 300001), (256, 1000)])
 def test_eval_points_layerwise_forward_matches_oracle(H, N):
-    """Trainer.eval_points (trainer.py:77-90) on the layer-wise tcgen05 GEMMs; N = 300001 crosses the internal
+    """Trainer.eval_points (trainer.py:77-90) on the layer-wise wgmma GEMMs; N = 300001 crosses the internal
     262144-point chunking used to bound the activation workspace for 256^3 grids."""
     params = vo.init_params(1, H, seed=11)
     pts = (torch.rand(1, N, 3, generator=torch.Generator().manual_seed(2)) - 0.5) * 8

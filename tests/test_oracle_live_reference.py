@@ -1,204 +1,110 @@
-"""Oracle vs the UNMODIFIED reference modules, live (build container only: skipped where /root/reference is absent,
-e.g. on the GPU box).  The committed goldens pin a few fixed cases; this sweeps more shapes / seeds through the same
-harness train.py uses (functorch vmap over combine_state_for_ensemble, loss.step_batch_loss, torch.optim.AdamW)."""
+"""Oracle and host mirror vs the UNMODIFIED reference modules.  The reference side of every comparison was run once
+by oracle/make_reference_golden.py (the same harness train.py uses: functorch vmap over combine_state_for_ensemble,
+loss.step_batch_loss, torch.optim.AdamW; sceneObject.get_training_samples / append_keyframe; dataset.Replica) and is
+replayed here from tests/golden/ref_*.npz, so the comparison runs wherever the repository does."""
+import json
+import random
+import types
+
+import numpy as np
 import pytest
 import torch
 
-from oracle import _refload
+from oracle import make_reference_golden as mrg
 from oracle import vmap_oracle as vo
 from tests._util import rel_l2
 
-pytestmark = pytest.mark.skipif(not _refload.available(), reason="reference tree not mounted")
+
+def _golden(kind, *case):
+    return np.load(mrg.golden_path(kind, *case))
 
 
-def _reference_step(n_obj, hidden, n_rays, n_samples, scale, n_cam2surf, seed, n_steps):
-    model, embedding, render_rays, loss = _refload.load("model", "embedding", "render_rays", "loss")
-    from functorch import combine_state_for_ensemble, vmap
-    torch.manual_seed(seed)
-    e1, e2 = vo.emb_sizes(5)
-    fcs = [model.OccupancyMap(e1, e2, hidden_size=hidden).apply(model.init_weights) for _ in range(n_obj)]   # trainer.py:27-33
-    pes = [embedding.UniDirsEmbed(max_deg=5, scale=scale) for _ in range(n_obj)]
-    batch = vo.synthetic_batch(n_obj, n_rays, n_samples, seed=seed + 100, n_cam2surf=n_cam2surf)
-    opt = torch.optim.AdamW([torch.zeros(1, requires_grad=True)], lr=1e-3, weight_decay=0.013)             # train.py:67
-    fc_model, fc_param, fc_buffer = combine_state_for_ensemble(fcs)                                        # utils.py:31
-    pe_model, pe_param, pe_buffer = combine_state_for_ensemble(pes)
-    for p in list(fc_param) + list(pe_param):
-        p.requires_grad_()
-    opt.add_param_group({"params": fc_param}); opt.add_param_group({"params": pe_param})
-    names = [n for n, _ in fcs[0].named_parameters()]
-    init = {n: p.detach().clone() for n, p in zip(names, fc_param)}
-    init[vo.PE_KEY] = pe_param[0].detach().clone()
-
-    def fwd_loss():
-        emb = vmap(pe_model)(pe_param, pe_buffer, batch["pcs"])                                            # train.py:293
-        alpha, col = vmap(fc_model)(fc_param, fc_buffer, emb)                                              # train.py:294
-        return loss.step_batch_loss(alpha, col, batch["gt_depth"], batch["gt_colour"], batch["sem"],
-                                    batch["mask_depth"], batch["z"])[0]                                    # train.py:303
-    l0 = fwd_loss()
-    l0.backward()
-    grads = {n: p.grad.detach().clone() for n, p in zip(names, fc_param)}
-    grads[vo.PE_KEY] = pe_param[0].grad.detach().clone()
-    losses = [float(l0)]
-    for s in range(n_steps):
-        opt.step(); opt.zero_grad(set_to_none=True)
-        l = fwd_loss(); losses.append(float(l))
-        if s + 1 < n_steps:
-            l.backward()
-    final = {n: p.detach().clone() for n, p in zip(names, fc_param)}
-    final[vo.PE_KEY] = pe_param[0].detach().clone()
-    return batch, init, grads, losses, final
-
-
-@pytest.mark.parametrize("n_obj,hidden,n_rays,n_samples,scale,n1,seed", [
-    (1, 32, 17, 6, 2.0, 1, 21), (5, 32, 9, 10, 2.0, 1, 22), (2, 64, 13, 14, 5.0, 5, 23), (1, 128, 8, 10, 5.0, 5, 24),
-    (3, 32, 1, 10, 2.0, 1, 25)])
+@pytest.mark.parametrize("n_obj,hidden,n_rays,n_samples,scale,n1,seed", mrg.STEP_CASES)
 def test_oracle_matches_live_reference_step(n_obj, hidden, n_rays, n_samples, scale, n1, seed):
     n_steps = 2
-    batch, init, g_ref, l_ref, p_ref = _reference_step(n_obj, hidden, n_rays, n_samples, scale, n1, seed, n_steps)
+    G = _golden("step", seed)
+    init, batch = mrg.step_inputs(n_obj, hidden, n_rays, n_samples, n1, seed)
+    for k in vo.ALL_KEYS:                           # the regenerated inputs are the ones the reference ran on
+        assert torch.equal(mrg.sampled(init[k], k), torch.from_numpy(G["init_" + k])), k
+    l_ref = G["losses"]
+
+    def check(mine, prefix, tol, k):
+        ref_s, ref_n = torch.from_numpy(G[prefix + "_" + k]), float(G[prefix + "norm_" + k])
+        assert rel_l2(mrg.sampled(mine, k), ref_s) < tol, k
+        assert abs(float(mine.detach().double().norm()) - ref_n) <= tol * ref_n + 1e-12, k
+
     orc = vo.OracleEnsemble(init, scale)
     loss, grads = orc.grads(batch)
     assert abs(float(loss) - l_ref[0]) <= 2e-6 * abs(l_ref[0]) + 1e-7
     for k in vo.ALL_KEYS:
-        assert rel_l2(grads[k], g_ref[k]) < 2e-5, k
+        check(grads[k], "g", 2e-5, k)
     orc = vo.OracleEnsemble(init, scale)            # fresh optimiser state / no leftover .grad
     losses = [float(orc.step(batch)) for _ in range(n_steps)]
     for a, b in zip(losses, l_ref[:n_steps]):
         assert abs(a - b) <= 5e-6 * abs(b) + 1e-7
     for k in vo.ALL_KEYS:
-        assert rel_l2(orc.params[k], p_ref[k]) < 2e-6, k
+        check(orc.params[k], "p", 2e-6, k)
 
 
-@pytest.mark.parametrize("seed,n_kf,n_frames,n_samples,n1", [(31, 7, 9, 11, 1), (32, 3, 6, 5, 5), (33, 1, 4, 7, 1),
-                                                             (34, 8, 20, 3, 1), (35, 4, 5, 16, 5)])
+@pytest.mark.parametrize("seed,n_kf,n_frames,n_samples,n1", mrg.SAMPLER_CASES)
 def test_sampler_oracle_matches_live_reference(seed, n_kf, n_frames, n_samples, n1):
-    """sceneObject.get_training_samples (vmap.py:319-459) run live vs oracle/sampler_oracle.py with the reference's RNG
+    """sceneObject.get_training_samples (vmap.py:319-459) vs oracle/sampler_oracle.py with the reference's RNG
     call order reproduced: integer outputs and z bit-exact."""
-    import numpy as np
     from oracle import sampler_oracle as so
-    vmap_mod = _refload.load("vmap")
-    W, H, KF = 56, 40, 8
-    g = torch.Generator().manual_seed(seed)
-    rgbs = torch.randint(0, 256, (KF, W, H, 4), generator=g).to(torch.uint8)
-    rgbs[..., 3] = (torch.rand(KF, W, H, generator=g) * 3).long().clamp(0, 2).to(torch.uint8)
-    depth = torch.rand(KF, W, H, generator=g) * 4 + 0.5
-    depth[torch.rand(KF, W, H, generator=g) < 0.15] = 0.0
-    twc = torch.eye(4).repeat(KF, 1, 1)
-    twc[:, :3, 3] = torch.rand(KF, 3, generator=g) - 0.5
-    bbox = torch.empty(KF, 4)
-    bbox[:, 0] = torch.randint(0, W // 2, (KF,), generator=g).float()
-    bbox[:, 1] = bbox[:, 0] + torch.randint(4, W // 2, (KF,), generator=g).float()
-    bbox[:, 2] = torch.randint(0, H // 2, (KF,), generator=g).float()
-    bbox[:, 3] = bbox[:, 2] + torch.randint(4, H // 2, (KF,), generator=g).float()
-    rays = so.camera_ray_dirs(W, H, 60.0, 60.0, W / 2 - 0.5, H / 2 - 0.5)
-    latest = [n_kf - 2, n_kf - 1] if n_kf >= 2 else [0]
-    obj = object.__new__(vmap_mod.sceneObject)          # skip __init__ (builds a Trainer / open3d)
-    obj.n_keyframes, obj.data_device, obj.lastest_kf_queue = n_kf, "cpu", list(latest)
-    obj.bbox, obj.rgbs_batch, obj.depth_batch, obj.t_wc_batch = bbox, rgbs, depth, twc
-    obj.n_bins_cam2surface, obj.n_bins, obj.surface_eps, obj.stop_eps = n1, 9, 0.1, 0.05
-    obj.min_bound, obj.max_bound = 0.0, 8.0
-    obj.this_obj, obj.other_obj, obj.unknown_obj = 1, 0, 2
-    obj.obj_center = torch.tensor(0.0)
-    torch.manual_seed(seed + 1)
-    r_rgb, r_depth, r_valid, r_lab, r_pcs, r_z = obj.get_training_samples(n_frames, n_samples, rays)
+    G = _golden("sampler", seed)
+    rgbs, depth, twc, bbox, rays, latest = mrg.sampler_inputs(seed, n_kf)
     cfg = so.SamplerCfg(n_bins_cam2surface=n1)
     torch.manual_seed(seed + 1)
     rnd = so.draw_randoms_reference_order(None, n_kf, latest, n_frames, n_samples, bbox, rgbs, depth, cfg)
     rgb, dep, valid, lab, pcs, z = so.sample_from_randoms(rnd, rgbs, depth, twc, bbox, rays, cfg)
-    assert torch.equal(rgb, r_rgb) and torch.equal(dep, r_depth) and torch.equal(valid, r_valid) and torch.equal(lab, r_lab)
-    assert torch.equal(z, r_z)
-    np.testing.assert_allclose(pcs.numpy(), r_pcs.numpy(), rtol=0, atol=1e-6)
+    for name, t in (("rgb", rgb), ("depth", dep), ("valid", valid), ("lab", lab), ("z", z)):
+        ref = torch.from_numpy(G[name])
+        assert t.dtype == ref.dtype and torch.equal(t, ref), name
+    np.testing.assert_allclose(pcs.numpy(), G["pcs"], rtol=0, atol=1e-6)
 
 
-@pytest.mark.parametrize("kf_step,buf,n_frames_seen,seed", [(3, 6, 40, 1), (1, 4, 25, 2), (5, 8, 60, 3)])
+@pytest.mark.parametrize("kf_step,buf,n_frames_seen,seed", mrg.KEYFRAME_CASES)
 def test_keyframe_policy_matches_live_reference(kf_step, buf, n_frames_seen, seed, monkeypatch):
     """vmap_b200.vmap.sceneObject.append_keyframe / prune_keyframe vs the reference's (vmap.py:208-268), fed the same
     frames and the same ``random`` stream: slot choice, keyframe count, latest queue, id map and buffer contents."""
-    import random
-    import types
-    from oracle._refload import _Bidict
     from vmap_b200 import vmap as vm
-    ref_mod = _refload.load("vmap")
+    G = _golden("keyframes", seed)
     monkeypatch.setattr(vm.trainer_mod, "Trainer", lambda cfg: types.SimpleNamespace())
-    W, H = 6, 5
-    cfg = types.SimpleNamespace(do_bg=False, data_device="cpu", training_device="cpu", obj_scale=2.0, bg_scale=5.0,
-                                hidden_feature_size=32, hidden_feature_size_bg=128, n_bins_cam2surface=1,
-                                n_bins_cam2surface_bg=5, keyframe_step=kf_step, keyframe_step_bg=kf_step, min_depth=0.0,
-                                max_depth=8.0, n_bins=9, n_unidir_funcs=5, surface_eps=0.1, stop_eps=0.05,
-                                keyframe_buffer_size=buf)
-
-    def frame(fid):
-        g = torch.Generator().manual_seed(1000 * seed + fid)
-        return (torch.randint(0, 255, (W, H, 3), dtype=torch.uint8, generator=g), torch.rand(W, H, generator=g),
-                torch.randint(0, 3, (W, H), dtype=torch.uint8, generator=g), torch.tensor([0., float(fid % W), 0., float(fid % H)]),
-                torch.eye(4) * (fid + 1))
-
-    rgb, depth, mask, bbox, T = frame(0)
-    mine = vm.sceneObject(cfg, 7, rgb, depth, mask, bbox, T, 0)
-    ref = object.__new__(ref_mod.sceneObject)               # the reference __init__ builds a Trainer / needs open3d
-    ref.n_keyframes, ref.kf_pointer, ref.keyframe_buffer_size = 1, None, buf
-    ref.kf_id_dict, ref.kf_buffer_full, ref.frame_cnt, ref.lastest_kf_queue = _Bidict({0: 0}), False, 0, []
-    ref.keyframe_step, ref.rgb_idx, ref.state_idx = kf_step, slice(0, 3), slice(3, 4)
-    ref.bbox = torch.empty(buf, 4); ref.rgbs_batch = torch.empty(buf, W, H, 4, dtype=torch.uint8)
-    ref.depth_batch = torch.empty(buf, W, H); ref.t_wc_batch = torch.empty(buf, 4, 4)
-    ref.bbox[0] = bbox; ref.rgbs_batch[0, :, :, :3] = rgb; ref.rgbs_batch[0, :, :, 3:4] = mask[..., None]
-    ref.depth_batch[0] = depth; ref.t_wc_batch[0] = T
+    rgb, depth, mask, bbox, T = mrg.keyframe_frame(seed, 0)
+    mine = vm.sceneObject(mrg.keyframe_cfg(kf_step, buf), 7, rgb, depth, mask, bbox, T, 0)
+    assert G["scal"].shape[0] == n_frames_seen - 1
     for fid in range(1, n_frames_seen):
-        rgb, depth, mask, bbox, T = frame(fid)
+        rgb, depth, mask, bbox, T = mrg.keyframe_frame(seed, fid)
         random.seed(fid); mine.append_keyframe(rgb, depth, mask, bbox, T, fid)
-        random.seed(fid); ref.append_keyframe(rgb, depth, mask, bbox, T, fid)
-        assert mine.n_keyframes == ref.n_keyframes and mine.kf_pointer == ref.kf_pointer, fid
-        assert mine.lastest_kf_queue == ref.lastest_kf_queue and mine.frame_cnt == ref.frame_cnt
-        assert dict(mine.kf_id_dict) == dict(ref.kf_id_dict) and mine.kf_buffer_full == ref.kf_buffer_full
-        n = max(mine.n_keyframes, (mine.kf_pointer or 0) + 1)
-        assert torch.equal(mine.rgbs_batch[:n], ref.rgbs_batch[:n]) and torch.equal(mine.depth_batch[:n], ref.depth_batch[:n])
-        assert torch.equal(mine.t_wc_batch[:n], ref.t_wc_batch[:n]) and torch.equal(mine.bbox[:n], ref.bbox[:n])
+        st = mrg.keyframe_state(mine, buf)
+        for k, v in st.items():
+            assert np.array_equal(v, G[k][fid - 1]), (fid, k)
 
 
 def test_module_surface_matches_live_reference():
     """state_dict keys / shapes of OccupancyMap and UniDirsEmbed, the icosahedron directions, and cameraInfo's ray cache
-    against the live reference classes (model.py:17-52, embedding.py:44-80, vmap.py:494-524)."""
-    import types
+    against the reference classes (model.py:17-52, embedding.py:44-80, vmap.py:494-524)."""
     from vmap_b200 import embedding as my_emb, model as my_model, vmap as my_vmap
-    ref_model, ref_emb, ref_vmap = _refload.load("model", "embedding", "vmap")
+    G = _golden("surface")
+    sd = json.loads(str(G["occupancy_state_dict"]))
     for hidden in (32, 128, 256):
         a = my_model.OccupancyMap(87, 42, hidden_size=hidden).state_dict()
-        b = ref_model.OccupancyMap(87, 42, hidden_size=hidden).state_dict()
-        assert list(a) == list(b) and all(a[k].shape == b[k].shape for k in a)
-    pa, pb = my_emb.UniDirsEmbed(max_deg=5, scale=2.0), ref_emb.UniDirsEmbed(max_deg=5, scale=2.0)
-    assert list(pa.state_dict()) == list(pb.state_dict())
-    assert torch.equal(pa.B_layer.weight.detach(), pb.B_layer.weight.detach()) and float(pa.scale) == float(pb.scale)
-    cfg = types.SimpleNamespace(data_device="cpu", W=37, H=23, fx=31.5, fy=29.25, cx=18.0, cy=11.5)
-    assert torch.equal(my_vmap.cameraInfo(cfg).rays_dir_cache, ref_vmap.cameraInfo(cfg).rays_dir_cache)
+        assert [[k, list(v.shape)] for k, v in a.items()] == sd[str(hidden)]
+    pa = my_emb.UniDirsEmbed(max_deg=5, scale=2.0)
+    assert list(pa.state_dict()) == json.loads(str(G["pe_keys"]))
+    assert torch.equal(pa.B_layer.weight.detach(), torch.from_numpy(G["pe_weight"])) and float(pa.scale) == float(G["pe_scale"])
+    cfg = types.SimpleNamespace(**mrg.SURFACE_CAM)
+    assert torch.equal(my_vmap.cameraInfo(cfg).rays_dir_cache, torch.from_numpy(G["rays_dir_cache"]))
 
 
-@pytest.mark.parametrize("W,H,n_inst,seed", [(96, 64, 9, 41), (200, 150, 25, 42), (64, 96, 5, 43)])
+@pytest.mark.parametrize("W,H,n_inst,seed", mrg.LOADER_CASES)
 def test_ingest_oracle_matches_live_reference_loader(W, H, n_inst, seed):
-    """oracle/ingest_oracle.replica_frame vs dataset.Replica.__getitem__ (dataset.py:80-141) run live on a synthetic
-    Replica-format directory (written under the repo's scratch area and removed afterwards)."""
-    import os
-    import shutil
-    import tempfile
-    import types
-    import numpy as np
-    cv2 = pytest.importorskip("cv2")
+    """oracle/ingest_oracle.replica_frame vs dataset.Replica.__getitem__ (dataset.py:80-141) on a synthetic
+    Replica-format frame."""
     from oracle import ingest_oracle as io
-    dataset = _refload.load("dataset")
+    G = _golden("loader", seed)
     inst, cls = io.synthetic_instance_frame(W, H, n_inst, seed)
-    root = tempfile.mkdtemp(prefix="_ds_", dir=os.path.dirname(os.path.abspath(io.__file__)))
-    try:
-        for d in ("rgb", "depth", "semantic_instance", "semantic_class"):
-            os.makedirs(os.path.join(root, d))
-        rng = np.random.default_rng(seed)
-        cv2.imwrite(os.path.join(root, "rgb", "rgb_0.png"), rng.integers(0, 255, (H, W, 3), dtype=np.uint8))
-        cv2.imwrite(os.path.join(root, "depth", "depth_0.png"), rng.integers(500, 4000, (H, W)).astype(np.uint16))
-        cv2.imwrite(os.path.join(root, "semantic_instance", "semantic_instance_0.png"), inst.T.astype(np.uint16))
-        cv2.imwrite(os.path.join(root, "semantic_class", "semantic_class_0.png"), cls.T.astype(np.uint16))
-        np.savetxt(os.path.join(root, "traj_w_c.txt"), np.eye(4).reshape(1, 16), delimiter=" ")
-        ds = dataset.Replica(types.SimpleNamespace(imap_mode=False, dataset_dir=root, depth_scale=1000.0, max_depth=8.0))
-        sample = ds[0]
-    finally:
-        shutil.rmtree(root, ignore_errors=True)
-    ref_bbox = {int(k): [int(x) for x in np.asarray(v).reshape(-1)] for k, v in sample["bbox_dict"].items()}
-    bbox_dict, obj = io.replica_frame(inst, cls, set(ds.background_cls_list), ds.bbox_scale)
-    assert {k: v.tolist() for k, v in bbox_dict.items()} == ref_bbox
-    assert np.array_equal(obj, np.asarray(sample["obj"]).astype(np.int32))
+    bbox_dict, obj = io.replica_frame(inst, cls, set(int(c) for c in G["background_cls"]), float(G["bbox_scale"]))
+    ref_bbox = {int(k): [int(x) for x in row] for k, row in zip(G["bbox_keys"], G["bbox"])}
+    assert {int(k): [int(x) for x in np.asarray(v).reshape(-1)] for k, v in bbox_dict.items()} == ref_bbox
+    assert np.array_equal(obj, G["obj"])

@@ -1,5 +1,5 @@
 """Trained-quality parity on a consistent scene (BASELINE target: trained PSNR within +-0.2 dB of the
-reference on identical inputs): the CPU oracle (= the reference's fp32 functorch step) and the tcgen05
+reference on identical inputs): the CPU oracle (= the reference's fp32 functorch step) and the tensor-core
 path train on the same batch stream from the same init; quality is measured on held-out rays."""
 import pytest
 import torch
@@ -39,7 +39,7 @@ def test_trained_psnr_matches_oracle(impl, tol_db):
 
 def test_trained_psnr_20_objects_1000_steps():
     """SURVEY.md 8(c): identical-input 1000-step trajectory at the shipped shape (20 objects x 120 rays x 10 samples):
-    trained PSNR of the fused tcgen05 step within 0.2 dB of the oracle, object by object on average."""
+    trained PSNR of the fused tensor-core step within 0.2 dB of the oracle, object by object on average."""
     B, R, S, steps = 20, 120, 10, 1000
     params = vo.init_params(B, 32, seed=8)
     orc = vo.OracleEnsemble(params, 2.0)

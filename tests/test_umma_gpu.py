@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 (fp16-operand) step kernel: BASELINE bar is <= 1e-3 relative L2
+"""GPU parity of the tensor-core (fp16-operand) step kernel: BASELINE bar is <= 1e-3 relative L2
 on rendered depth / colour vs the reference on identical inputs."""
 import pytest
 import torch
@@ -89,7 +89,7 @@ def test_umma_training_tracks_fp32_kernel():
 
 @pytest.mark.parametrize("N", [1000, 70001])
 def test_eval_points_tensor_core_forward_matches_oracle(N):
-    """Trainer.eval_points (trainer.py:77-90) through the forward half of the fused tcgen05 kernel."""
+    """Trainer.eval_points (trainer.py:77-90) through the forward half of the fused tensor-core kernel."""
     B = 3
     params = vo.init_params(B, 32, seed=9)
     pts = (torch.rand(B, N, 3, generator=torch.Generator().manual_seed(1)) - 0.5) * 4
@@ -98,7 +98,7 @@ def test_eval_points_tensor_core_forward_matches_oracle(N):
     alpha, col = ens.eval_points(pts.cuda())
     a32, c32 = ens.eval_points(pts.cuda(), impl="fp32")
     assert rel_l2(a32, alpha_ref.view(B, N)) < 1e-5
-    print("eval_points tcgen05 vs oracle: alpha", rel_l2(alpha, alpha_ref.view(B, N)), "colour", rel_l2(col, col_ref.view(B, N, 3)))
+    print("eval_points tensor-core vs oracle: alpha", rel_l2(alpha, alpha_ref.view(B, N)), "colour", rel_l2(col, col_ref.view(B, N, 3)))
     assert rel_l2(alpha, alpha_ref.view(B, N)) < 2e-3
     assert rel_l2(col, col_ref.view(B, N, 3)) < 1e-3
 
@@ -123,16 +123,13 @@ def test_eval_points_throughput_grid():
     assert res["umma"] < res["fp32"]
 
 
-def test_step_is_reproducible(monkeypatch):
+def test_step_is_reproducible():
     """No floating-point atomics on the hidden-32 path: per-(CTA, object) gradient partials are reduced in segment
-    order by the last CTA to finish the object.  With VMB_DETERMINISTIC=1 (one point group per CTA, so every wgrad
-    accumulator sees a single in-order MMA stream) two runs from the same state give identical bits over 200 steps;
-    in the default mode (two groups interleave their wgrad MMAs in arrival order) a single step agrees to fp32
-    rounding of the summation order."""
+    order by the last CTA to finish the object, and every wgrad accumulator sees a single in-order MMA stream, so two
+    runs from the same state give identical bits over 200 steps."""
     B, R, S = 7, 301, 10                      # CTAs straddle objects, ragged last tile
     params = vo.init_params(B, 32, seed=3)
     batches = [to_dev(vo.synthetic_batch(B, R, S, seed=50 + i)) for i in range(4)]
-    monkeypatch.setenv("VMB_DETERMINISTIC", "1")
     outs = []
     for run in range(2):
         ens = make_ensemble(params, 2.0, 32, impl="umma")
@@ -150,7 +147,6 @@ def test_step_is_reproducible(monkeypatch):
         e1.step(batches[it % 4])
         e2.forward_backward(batches[it % 4]); e2.adam_step()
     assert torch.equal(e1.params, e2.params) and torch.equal(e1.image, e2.image)
-    monkeypatch.delenv("VMB_DETERMINISTIC")
     g = []
     for run in range(2):
         e = make_ensemble(params, 2.0, 32, impl="umma")

@@ -1,4 +1,4 @@
-"""vmap_b200 -- B200-native implementation of vMAP's vectorised per-object training step.
+"""vmap_b200 -- H100-native (sm_90a) implementation of vMAP's vectorised per-object training step.
 
 Only what the hot path needs lives here: the CUDA kernels + C ABI (csrc/, libvmap_b200.so),
 the packed ensemble / fused step driver (ensemble.py) and the host-side mirror of the

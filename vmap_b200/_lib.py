@@ -1,7 +1,7 @@
 """ctypes binding of libvmap_b200.so (C ABI declared in include/vmap_b200.h).
 
 There is deliberately NO fallback: if the CUDA library is missing or fails to
-load, every op raises.  ``build()`` compiles it in-tree with nvcc for sm_100a.
+load, every op raises.  ``build()`` compiles it in-tree with nvcc for sm_90a.
 """
 from __future__ import annotations
 
@@ -11,7 +11,7 @@ import subprocess
 import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("VMB_LIB") or os.path.join(_HERE, "libvmap_b200.so")   # VMB_LIB: profiling variants
+LIB_PATH = os.environ.get("VMB_LIB") or os.path.join(_HERE, "libvmap_b200.so")   # VMB_LIB: another build of the library
 CSRC = os.path.join(_HERE, "csrc")
 
 VMB_IMPL = {"auto": 0, "fp32": 1, "umma": 2, "layerwise": 3}
@@ -107,7 +107,7 @@ class VmbError(RuntimeError):
 
 
 def build(verbose: bool = False) -> str:
-    """Compile libvmap_b200.so in-tree (nvcc, -gencode arch=compute_100a,code=sm_100a)."""
+    """Compile libvmap_b200.so in-tree (nvcc, -gencode arch=compute_90a,code=sm_90a)."""
     r = subprocess.run(["make", "-C", CSRC], capture_output=True, text=True)
     if verbose or r.returncode != 0:
         print(r.stdout, r.stderr)

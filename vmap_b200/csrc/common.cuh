@@ -1,4 +1,4 @@
-// Shared definitions for the vmap_b200 kernels (sm_100a only).
+// Shared definitions for the vmap_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>

@@ -1,25 +1,29 @@
-// Generic tcgen05 GEMM used by the layer-wise path for wide models (hidden 128 / 256: background
-// model, iMAP whole-scene model), where one object's weights and a tile's activations no longer fit
-// in shared memory together and the layers run as separate launches over all points.
+// wgmma GEMMs of the layer-wise path for wide models (hidden 64 / 128 / 256: background model, iMAP whole-scene
+// model), where one object's weights and a tile's activations no longer fit in shared memory together and the layers
+// run as separate launches over all points.
 //
-//   D[M][N] (+)= A[M][K] * B[N][K]^T        fp16 operands, fp32 accumulate in TMEM
+//   D[M][N] (+)= A[M][K] * B[N][K]^T        fp16 operands from shared memory, fp32 accumulate in registers
 //
 // Two kernels share the operand conventions below:
-//   k_gemm_umma  generic persistent kernel: 128 x 128 output tiles, K in chunks of 64, 3-stage TMA -> mbarrier ->
-//                tcgen05.mma pipeline, warp 4 = TMA producer (one elected lane), warp 5 = MMA issuer, warps 0..3 =
-//                epilogue; two TMEM accumulators (2 x 128 columns) so tile i+1's MMAs overlap tile i's epilogue;
-//                107 KB of shared memory: two CTAs per SM.  Used for wgrad (split-K over points, atomics) and for the
-//                forward layers whose weights exceed the weight-stationary budget.
+//   k_gemm_umma  generic persistent kernel: 128 x 128 output tiles, K in chunks of 64, 4-stage TMA -> mbarrier ring,
+//                warp 8 = TMA producer (one elected lane), warps 0..7 = two consumer warpgroups.  Warpgroup g owns the
+//                tile's columns 64g .. 64g+63: two wgmma.m64n64k16 per K step (rows 0..63 and 64..127), then the
+//                epilogue on its own accumulators.  Used for wgrad (split-K over points, atomics) and for the forward
+//                layers whose weights exceed the weight-stationary budget.
 //   k_gemm_ws    weight-stationary kernel for the skinny forward / dgrad GEMMs (see its header further down).
-// * Operand stages use the 128-byte-swizzle canonical layouts, written by TMA (CU_TENSOR_MAP_SWIZZLE_128B,
-//   128-byte inner box so the TMA engine moves full lines; a first version with 16-byte inner boxes into the
-//   SWIZZLE_NONE layout was TMA-bound at ~150 TFLOP/s):
+// * Operand stages use the 128-byte-swizzle canonical layouts, written by TMA (CU_TENSOR_MAP_SWIZZLE_128B, 128-byte
+//   inner box so the TMA engine moves full lines):
 //     K-major  operand, global [rows][ld]  (K contiguous):  2-D box (64 k, 128 rows)  -> [128 rows][128 B]
-//        descriptor SWIZZLE_128B, SBO 1024 (8 rows), k-step +32 B inside the swizzle atom
+//        descriptor SWIZZLE_128B, SBO 1024 (8 rows), k-step +32 B inside the swizzle atom, 64 rows = +8192 B
 //     MN-major operand, global [K][ld]     (MN contiguous): two 2-D boxes (64 mn, 64 k) -> two [64 k][128 B] panels
-//        descriptor SWIZZLE_128B, LBO 8192 (next 64-wide panel), SBO 1024 (8 k-rows), k-step +2048 B
+//        descriptor SWIZZLE_128B, SBO 1024 (8 k-rows), k-step +2048 B, one panel per 64 rows / columns
 //   Out-of-range rows / columns are zero-filled by the TMA engine, so ragged edges need no branches.
 // * A may come from two sources concatenated along K (e.g. [fc2 | emb1] for cat_layer).
+// * Not pipelined yet: a consumer waits for each K chunk's wgmmas (wait_group 0) before it looks at the next stage, a
+//   tile's epilogue does not overlap the next tile's MMAs, and ptxas reports the wgmmas of both kernels as serialised
+//   (C7520; the build prints the count).  The TMA ring still runs ahead of the consumers.
+// * Epilogues work one output ROW per lane: a warp's accumulator fragments (rows 16w .. 16w+15 of both 64-row halves)
+//   are transposed through a per-warp shared-memory tile, 32 columns at a time.
 #pragma once
 #include "common.cuh"
 #include "umma_ptx.cuh"
@@ -28,10 +32,12 @@
 
 namespace lw {
 
-constexpr int BM = 128, BN = 128, BK = 64, NSTAGE = 3;
+constexpr int BM = 128, BN = 128, BK = 64, NSTAGE = 4;
 constexpr int STAGE_BYTES = (BM + BN) * BK * 2;             // 32 KB
-constexpr int GEMM_SMEM = NSTAGE * STAGE_BYTES + 1024 + 4 * 2560;      // + barriers + fp16 epilogue staging (4 warps)
-constexpr int GEMM_THREADS = 192;
+constexpr int N_CWARPS = 8;                                 // consumer warps (two warpgroups)
+constexpr int EPI_SCRATCH = 32 * 144;                       // per consumer warp: fragment transposition tile, then the epilogue's staging tile
+constexpr int GEMM_SMEM = NSTAGE * STAGE_BYTES + 1024 + N_CWARPS * EPI_SCRATCH;      // + barriers
+constexpr int GEMM_THREADS = 32 * (N_CWARPS + 1);
 constexpr float LS = 256.0f, INV_LS = 1.0f / 256.0f;
 
 enum Epi { EPI_RELU_F16 = 0, EPI_GATE_F16 = 1, EPI_F32 = 2, EPI_ATOMIC = 3 };
@@ -83,13 +89,38 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
       ::"r"(ptx::smem_u32(dst)), "l"(map), "r"(ptx::smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-// SWIZZLE_128B shared-memory descriptor (layout type 2)
+// SWIZZLE_128B shared-memory matrix descriptor
 __device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return ptx::smem_desc(saddr, lbo_bytes, sbo_bytes) | ((uint64_t)2 << 61);
+  return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | ((uint64_t)1 << 62);
+}
+
+// Row r (0..31) of a consumer warp's slice of a 128-row tile: rows 16w .. 16w+15 of each 64-row wgmma half
+// (m_base = tile row 0 + 16w).
+__device__ __forceinline__ int wrow(int m_base, int r) { return m_base + (r & 15) + ((r >> 4) << 6); }
+
+// Accumulator fragments of the two 64-row halves (m64n64: d[4j + 0..1] = row l/4, columns 8j + 2(l%4) + {0, 1};
+// d[4j + 2..3] = row + 8) -> v = columns 32 cq .. 32 cq + 31 of warp row `lane` (see wrow), through the warp's tile.
+template <int CQ>
+__device__ __forceinline__ void frag_rows(const float (&d0)[32], const float (&d1)[32], unsigned char* scratch, int lane, float (&v)[32]) {
+  float* t = reinterpret_cast<float*>(scratch);
+  const int r = lane >> 2, c = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int k = 4 * (4 * CQ + j);
+    t[r * 33 + 8 * j + c] = d0[k];             t[r * 33 + 8 * j + c + 1] = d0[k + 1];
+    t[(r + 8) * 33 + 8 * j + c] = d0[k + 2];   t[(r + 8) * 33 + 8 * j + c + 1] = d0[k + 3];
+    t[(r + 16) * 33 + 8 * j + c] = d1[k];      t[(r + 16) * 33 + 8 * j + c + 1] = d1[k + 1];
+    t[(r + 24) * 33 + 8 * j + c] = d1[k + 2];  t[(r + 24) * 33 + 8 * j + c + 1] = d1[k + 3];
+  }
+  __syncwarp();
+#pragma unroll
+  for (int j = 0; j < 32; ++j) v[j] = t[lane * 33 + j];
+  __syncwarp();
 }
 
 // Epilogue of one 32-column chunk for the 32 rows of a warp: v = accumulator values of columns nb .. nb+31 of
-// row m_base + lane.  A thread owns one output ROW (TMEM lane), so direct stores would touch 32 different
+// row wrow(m_base, lane).  A thread owns one output ROW, so direct stores would touch 32 different
 // cache lines per instruction (16 B each); the fp16 / fp32 paths therefore transpose through a per-warp
 // shared-memory tile so that each store (and each gate / accumulate load) instruction covers whole 64 B / 128 B
 // row segments (8 / 4 rows per instruction).  `stage` = per-warp scratch (EPI_STAGE_F16 / EPI_STAGE_F32 bytes),
@@ -106,7 +137,7 @@ __device__ __forceinline__ void stage_store_f16(unsigned char* stage, int lane, 
   const int piece = lane & 3;
 #pragma unroll
   for (int s4 = 0; s4 < 4; ++s4) {
-    const int r = 8 * s4 + (lane >> 2), m = m_base + r;
+    const int r = 8 * s4 + (lane >> 2), m = wrow(m_base, r);
     const uint4 val = *reinterpret_cast<const uint4*>(stage + r * 80 + piece * 16);
     if (m < M && nb + piece * 8 < N) *reinterpret_cast<uint4*>(out + (size_t)m * ldo + nb + piece * 8) = val;
   }
@@ -125,7 +156,7 @@ __device__ __forceinline__ uint32_t pack_sat(float lo, float hi) {
 template <int EPI, bool SMEM_VEC = false>
 __device__ __forceinline__ void epi_chunk(const GemmArgs& g, float (&v)[32], int m_base, int lane, int nb, const float* bias,
                                           unsigned char* stage, const uint4* gpre = nullptr, const float* r1col = nullptr) {
-  const int m = m_base + lane;
+  const int m = wrow(m_base, lane);
   if (EPI == EPI_RELU_F16) {
     uint32_t h[16];
     const __half2 zero2 = __float2half2_rn(0.f);
@@ -152,7 +183,7 @@ __device__ __forceinline__ void epi_chunk(const GemmArgs& g, float (&v)[32], int
       uint4 gv;
       if (gpre) gv = gpre[s4];
       else {
-        const int mr = m_base + r;
+        const int mr = wrow(m_base, r);
         gv = make_uint4(0u, 0u, 0u, 0u);
         if (mr < g.M && nb + piece * 8 < g.N) gv = *reinterpret_cast<const uint4*>(g.gate + (size_t)mr * g.ldg + nb + piece * 8);
       }
@@ -194,7 +225,7 @@ __device__ __forceinline__ void epi_chunk(const GemmArgs& g, float (&v)[32], int
       if (g.accumulate) {
 #pragma unroll
         for (int s8 = 0; s8 < 8; ++s8) {                            // coalesced read of the old values: 4 rows x 128 B
-          const int r = 4 * s8 + (lane >> 3), mr = m_base + r;
+          const int r = 4 * s8 + (lane >> 3), mr = wrow(m_base, r);
           float4 old = make_float4(0.f, 0.f, 0.f, 0.f);
           if (mr < g.M && nb + piece * 4 < g.N) old = *reinterpret_cast<const float4*>(g.out32 + (size_t)mr * g.ld32 + nb + piece * 4);
           *reinterpret_cast<float4*>(st + r * 36 + piece * 4) = old;
@@ -212,7 +243,7 @@ __device__ __forceinline__ void epi_chunk(const GemmArgs& g, float (&v)[32], int
       __syncwarp();
 #pragma unroll
       for (int s8 = 0; s8 < 8; ++s8) {
-        const int r = 4 * s8 + (lane >> 3), mr = m_base + r;
+        const int r = 4 * s8 + (lane >> 3), mr = wrow(m_base, r);
         if (mr < g.M && nb + piece * 4 < g.N)
           *reinterpret_cast<float4*>(g.out32 + (size_t)mr * g.ld32 + nb + piece * 4) = *reinterpret_cast<const float4*>(st + r * 36 + piece * 4);
       }
@@ -225,8 +256,8 @@ __device__ __forceinline__ void epi_chunk(const GemmArgs& g, float (&v)[32], int
       }
     }
   } else if (stage && g.ldgn == 1) {
-    // EPI_ATOMIC, unit column stride: a thread owns a ROW, so direct atomics would hit 32 different rows (32 L2
-    // transactions) per instruction.  Transpose 16 columns at a time through the per-warp tile ([32][17] floats) so
+    // EPI_ATOMIC, unit column stride: a thread owns a ROW, so direct atomics would hit 32 different rows
+    // per instruction.  Transpose 16 columns at a time through the per-warp tile ([32][17] floats) so
     // each reduction instruction covers two rows x 16 consecutive floats.
     float* stf = reinterpret_cast<float*>(stage);
     const int c = lane & 15, rsub = lane >> 4;
@@ -240,7 +271,7 @@ __device__ __forceinline__ void epi_chunk(const GemmArgs& g, float (&v)[32], int
       if (n_in || n_bias) {
 #pragma unroll 4
         for (int r2 = 0; r2 < 16; ++r2) {
-          const int r = r2 * 2 + rsub, mrow = m_base + r;
+          const int r = r2 * 2 + rsub, mrow = wrow(m_base, r);
           if (mrow < g.M) {
             const float val = stf[r * 17 + c];
             if (n_in) atomicAdd(g.gdst + (size_t)mrow * g.ldgd + n, val);
@@ -261,32 +292,23 @@ __device__ __forceinline__ void epi_chunk(const GemmArgs& g, float (&v)[32], int
 }
 
 template <int A_MN, int B_MN, int EPI>
-__global__ void __launch_bounds__(GEMM_THREADS, 2)
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 k_gemm_umma(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUtensorMap mapA2,
             const __grid_constant__ CUtensorMap mapB, GemmArgs g) {
   // Persistent: each CTA walks tiles  t = blockIdx.x, blockIdx.x + gridDim.x, ...  of the (z, m, n) tile space
-  // (n fastest, so the N-tiles of one row block run back to back and share A in L2).  Two TMEM accumulators
-  // (2 x 128 columns) let the MMAs of tile i+1 overlap the epilogue of tile i.
+  // (n fastest, so the N-tiles of one row block run back to back and share A in L2).
   extern __shared__ __align__(1024) unsigned char smem[];
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + NSTAGE * STAGE_BYTES);
   uint64_t* empty = full + NSTAGE;
-  uint64_t* tfull = empty + NSTAGE;          // [2] accumulator ready for the epilogue
-  uint64_t* tempty = tfull + 2;              // [2] accumulator drained by the epilogue
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n_tiles_total = g.mt * g.nt * g.zt;
   const int k_total = g.K1 + g.K2;
 
   if (tid == 0) {
-    for (int s = 0; s < NSTAGE; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { ptx::mbar_init(&tfull[s], 1); ptx::mbar_init(&tempty[s], 128); }
+    for (int s = 0; s < NSTAGE; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], N_CWARPS); }
     ptx::mbar_init_fence();
   }
-  if (warp == 5) { ptx::tmem_alloc(tmem_slot, 256); ptx::tmem_relinquish(); }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tm = *tmem_slot;
   ptx::pdl_wait();                 // everything above overlapped the predecessor's tail (programmatic dependent launch)
   ptx::pdl_launch_dependents();
 
@@ -297,7 +319,7 @@ k_gemm_umma(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ C
   const int k_end = g.ksplit > 0 ? min(k_total, k_begin + g.ksplit) : k_total;      \
   const int n_chunks = (k_end - k_begin + BK - 1) / BK;
 
-  if (warp == 4) {
+  if (warp == N_CWARPS) {
     // ===================== TMA producer =====================
     if (ptx::elect_one()) {
       uint32_t cc = 0;                        // running chunk counter across tiles
@@ -322,82 +344,59 @@ k_gemm_umma(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ C
         }
       }
     }
-  } else if (warp == 5) {
-    // ===================== MMA issuer =====================
-    if (ptx::elect_one()) {
-      constexpr uint32_t idesc = ptx::idesc_f16(BM, BN, A_MN, B_MN);
-      uint32_t cc = 0, it = 0;
-      for (int t = blockIdx.x; t < n_tiles_total; t += gridDim.x, ++it) {
-        TILE_COORDS(t)
-        (void)m0; (void)n0;
-        const uint32_t acc = it & 1u;
-        if (it >= 2) { ptx::mbar_wait(&tempty[acc], ((it >> 1) - 1) & 1); ptx::tc_fence_after(); }
-        for (int c = 0; c < n_chunks; ++c, ++cc) {
-          const int s = cc % NSTAGE;
-          ptx::mbar_wait(&full[s], (cc / NSTAGE) & 1);
-          ptx::tc_fence_after();
-          const uint32_t sa = ptx::smem_u32(smem + s * STAGE_BYTES), sb = sa + BM * BK * 2;
-          const int klen = min(BK, k_end - (k_begin + c * BK));
-#pragma unroll 1
-          for (int ks = 0; ks * 16 < klen; ++ks) {
-            const uint64_t ad = A_MN ? desc_sw128(sa + ks * 2048, 8192, 1024) : desc_sw128(sa + ks * 32, 16, 1024);
-            const uint64_t bd = B_MN ? desc_sw128(sb + ks * 2048, 8192, 1024) : desc_sw128(sb + ks * 32, 16, 1024);
-            ptx::umma_f16(tm + acc * BN, ad, bd, idesc, (c > 0 || ks > 0) ? 1u : 0u);
-          }
-          ptx::umma_commit(&empty[s]);
-        }
-        ptx::umma_commit(&tfull[acc]);
-      }
-    }
   } else {
-    // ===================== epilogue: TMEM lane = output row =====================
-    uint32_t it = 0;
-    for (int t = blockIdx.x; t < n_tiles_total; t += gridDim.x, ++it) {
-    TILE_COORDS(t)
-    (void)n_chunks; (void)k_end;
-    const uint32_t acc = it & 1u;
-    ptx::mbar_wait(&tfull[acc], (it >> 1) & 1);
-    ptx::tc_fence_after();
-    const uint32_t taddr = tm + ((uint32_t)(warp * 32) << 16) + acc * BN;
+    // ===================== consumers: warpgroup wg owns columns 64 wg .. 64 wg + 63 of the tile =====================
+    const int wg = warp >> 2, wq = warp & 3;
+    unsigned char* scratch = smem + NSTAGE * STAGE_BYTES + 1024 + warp * EPI_SCRATCH;
+    unsigned char* stage = (EPI == EPI_RELU_F16 || EPI == EPI_GATE_F16 || EPI == EPI_ATOMIC) ? scratch : nullptr;
+    float d0[32], d1[32];                     // rows 0..63 / 64..127 of the tile
+    uint32_t cc = 0;
+    for (int t = blockIdx.x; t < n_tiles_total; t += gridDim.x) {
+      TILE_COORDS(t)
+      for (int c = 0; c < n_chunks; ++c, ++cc) {
+        const int s = cc % NSTAGE;
+        ptx::mbar_wait(&full[s], (cc / NSTAGE) & 1);
+        const uint32_t sa = ptx::smem_u32(smem + s * STAGE_BYTES), sb = sa + BM * BK * 2 + wg * 8192;
+        const int klen = min(BK, k_end - (k_begin + c * BK));
+        ptx::wgmma_fence();
 #pragma unroll 1
-    for (int c32 = 0; c32 < BN; c32 += 32) {
-      if (n0 + c32 >= g.N) break;                           // warp-uniform
+        for (int ks = 0; ks * 16 < klen; ++ks) {
+          const uint32_t ao = A_MN ? ks * 2048 : ks * 32, bo = B_MN ? ks * 2048 : ks * 32;
+          const uint64_t bd = desc_sw128(sb + bo, 16, 1024);
+          const uint32_t acc = (c > 0 || ks > 0) ? 1u : 0u;
+          ptx::wgmma_n64<A_MN, B_MN>(d0, desc_sw128(sa + ao, 16, 1024), bd, acc);
+          ptx::wgmma_n64<A_MN, B_MN>(d1, desc_sw128(sa + 8192 + ao, 16, 1024), bd, acc);
+        }
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        if (lane == 0) ptx::mbar_arrive(&empty[s]);
+      }
       float v[32];
-      ptx::tmem_ld32(taddr + c32, v);
-      ptx::tmem_ld_wait();
-      epi_chunk<EPI>(g, v, m0 + warp * 32, tid & 31, n0 + c32, g.bias,
-                     (EPI == EPI_RELU_F16 || EPI == EPI_GATE_F16 || EPI == EPI_ATOMIC) ? smem + NSTAGE * STAGE_BYTES + 1024 + warp * EPI_STAGE_F16 : nullptr);
-    }
-    ptx::tc_fence_before();
-    ptx::mbar_arrive(&tempty[acc]);            // this thread has drained its lanes of the accumulator
+      const int nb = n0 + wg * 64;
+      if (nb < g.N) { frag_rows<0>(d0, d1, scratch, lane, v); epi_chunk<EPI>(g, v, m0 + 16 * wq, lane, nb, g.bias, stage); }
+      if (nb + 32 < g.N) { frag_rows<1>(d0, d1, scratch, lane, v); epi_chunk<EPI>(g, v, m0 + 16 * wq, lane, nb + 32, g.bias, stage); }
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 5) ptx::tmem_dealloc(tm, 256);
 #undef TILE_COORDS
 }
 
 // ---------------------------------------------------------------------------------------------
 // Weight-stationary variant for the skinny GEMMs of the forward / dgrad passes:
 //   D[M][N] = A[M][K] * B   with  M = all points (10^5..10^6),  N <= 256,  K <= 384.
-// The generic kernel above re-streams A and B for every 128 x 128 tile (160 KB through L2 per 8.4 MFLOP):
-// at H = 256 it is L2-bandwidth bound (~6.5 TB/s aggregate).  Here each persistent CTA (one per SM)
+// The generic kernel above re-streams A and B for every 128 x 128 tile.  Here each persistent CTA (one per SM)
 //   * loads the WHOLE B operand (all N, all K: <= 192 KB) into shared memory once,
 //   * streams only A through a deep TMA ring (16 KB stages),
-//   * issues M128 x N<=256 x K16 MMAs (one instruction covers every output column of the row block),
-//   * double-buffers the accumulator in TMEM (2 x 256 columns = all 512),
-//   * drains it with EIGHT epilogue warps (TMEM lane quadrant = warp % 4, column half = warp / 4).
-// Per 128-row block the SM now moves 128 x K x 2 B in and 128 x N x 2 B out: ~2.5x less L2 traffic.
+//   * covers every output column of a 128-row block with its two consumer warpgroups: warpgroup g owns NB blocks of
+//     64 columns starting at 64 NB g (NB = 1 for N <= 128, 2 for N <= 256), two wgmma.m64n64k16 per block and K step.
 // ---------------------------------------------------------------------------------------------
-constexpr int WS_THREADS = 320;            // warps 0..7 epilogue, 8 = TMA producer, 9 = MMA issuer
-constexpr int WS_SMEM = 232448;            // all of it: also pins one CTA per SM (the CTA allocates all of TMEM)
+constexpr int WS_THREADS = 32 * (N_CWARPS + 1);            // warps 0..7 consumers, 8 = TMA producer
+constexpr int WS_SMEM = 232448;            // 227 KB: all of it
 constexpr int WS_ASTAGE = BM * BK * 2;     // 16 KB
 constexpr int WS_MAXCHUNK = 8, WS_MAXSTAGE = 8;
 
-struct WsGeom { int n_mma, nb_bytes, n_chunks, n_stage; };
+struct WsGeom { int nb_bytes, n_chunks, n_stage; };
 
-template <int B_MN, int EPI>
+template <int B_MN, int EPI, int NB>
 __global__ void __launch_bounds__(WS_THREADS, 1)
 k_gemm_ws(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUtensorMap mapA2,
           const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapB2, GemmArgs g, WsGeom geo) {
@@ -408,31 +407,23 @@ k_gemm_ws(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
   uint64_t* full = reinterpret_cast<uint64_t*>(tail);              // [WS_MAXSTAGE]
   uint64_t* empty = full + WS_MAXSTAGE;                            // [WS_MAXSTAGE]
   uint64_t* bfull = empty + WS_MAXSTAGE;                           // [WS_MAXCHUNK] B chunk landed
-  uint64_t* tfull = bfull + WS_MAXCHUNK;                           // [2]
-  uint64_t* tempty = tfull + 2;                                    // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
   float* sbias = reinterpret_cast<float*>(tail + 256);             // [256]
-  unsigned char* sstage = tail + 256 + 1024;                       // [8 warps][EPI stage]
-  const int tid = threadIdx.x, warp = tid >> 5;
+  unsigned char* sstage = tail + 256 + 1024;                       // [8 warps][EPI_SCRATCH]
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int k_total = g.K1 + g.K2;
 
   if (tid == 0) {
-    for (int s = 0; s < geo.n_stage; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 1); }
+    for (int s = 0; s < geo.n_stage; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], N_CWARPS); }
     for (int c = 0; c < geo.n_chunks; ++c) ptx::mbar_init(&bfull[c], 1);
-    for (int s = 0; s < 2; ++s) { ptx::mbar_init(&tfull[s], 1); ptx::mbar_init(&tempty[s], 256); }
     ptx::mbar_init_fence();
   }
   if (EPI == EPI_RELU_F16 && tid < 256) sbias[tid] = tid < g.N ? g.bias[tid] : 0.f;
   if (EPI == EPI_GATE_F16 && g.r1_row && tid < 256) sbias[tid] = tid < g.N ? g.r1_col[tid] : 0.f;
-  if (warp == 9) { ptx::tmem_alloc(tmem_slot, 512); ptx::tmem_relinquish(); }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tm = *tmem_slot;
-  ptx::pdl_wait();                 // barrier init / TMEM alloc / bias staging (parameters: written launches ago) overlap the predecessor
+  ptx::pdl_wait();                 // barrier init / bias staging (parameters: written launches ago) overlap the predecessor
   ptx::pdl_launch_dependents();
 
-  if (warp == 8) {
+  if (warp == N_CWARPS) {
     // ===================== TMA producer: B once, then the A ring =====================
     if (ptx::elect_one()) {
       for (int c = 0; c < geo.n_chunks; ++c) {
@@ -463,75 +454,48 @@ k_gemm_ws(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
         }
       }
     }
-  } else if (warp == 9) {
-    // ===================== MMA issuer =====================
-    if (ptx::elect_one()) {
-      const uint32_t idesc = ptx::idesc_f16(BM, geo.n_mma, 0, B_MN);
-      uint32_t cc = 0, it = 0;
-      for (int t = blockIdx.x; t < g.mt; t += gridDim.x, ++it) {
-        const uint32_t acc = it & 1u;
-        if (it >= 2) { ptx::mbar_wait(&tempty[acc], ((it >> 1) - 1) & 1); ptx::tc_fence_after(); }
-        for (int c = 0; c < geo.n_chunks; ++c, ++cc) {
-          const int s = cc % geo.n_stage;
-          if (it == 0) ptx::mbar_wait(&bfull[c], 0);
-          ptx::mbar_wait(&full[s], (cc / geo.n_stage) & 1);
-          ptx::tc_fence_after();
-          const uint32_t sa = ptx::smem_u32(sA + s * WS_ASTAGE), sb = ptx::smem_u32(sB + c * geo.nb_bytes);
-          const int klen = min(BK, k_total - c * BK);
-#pragma unroll 1
-          for (int ks = 0; ks * 16 < klen; ++ks) {
-            const uint64_t ad = desc_sw128(sa + ks * 32, 16, 1024);
-            const uint64_t bd = B_MN ? desc_sw128(sb + ks * 2048, 8192, 1024) : desc_sw128(sb + ks * 32, 16, 1024);
-            ptx::umma_f16(tm + acc * 256, ad, bd, idesc, (c > 0 || ks > 0) ? 1u : 0u);
-          }
-          ptx::umma_commit(&empty[s]);
-        }
-        ptx::umma_commit(&tfull[acc]);
-      }
-    }
   } else {
-    // ===================== epilogue: 8 warps, lane quadrant = warp % 4, column half = warp / 4 =====================
-    const int quad = warp & 3, half = warp >> 2;
-    const int n_c32 = (g.N + 31) / 32, c_lo = half ? (n_c32 + 1) / 2 : 0, c_hi = half ? n_c32 : (n_c32 + 1) / 2;
-    uint32_t it = 0;
+    // ===================== consumers =====================
+    const int wg = warp >> 2, wq = warp & 3;
+    unsigned char* scratch = sstage + warp * EPI_SCRATCH;
+    float d[NB][2][32];
+    uint32_t cc = 0, it = 0;
     for (int t = blockIdx.x; t < g.mt; t += gridDim.x, ++it) {
-      const uint32_t acc = it & 1u;
-      const int m_base = t * BM + quad * 32, lane = tid & 31;
-      // the gate rows do not depend on the MMAs: the first chunk's are fetched (coalesced pattern) before waiting
-      // for the accumulator, each later chunk's one chunk ahead, so their latency hides behind other work
-      uint4 gpre[2][4];
-      auto gate_fetch = [&](int c, uint4 (&dst)[4]) {
+      for (int c = 0; c < geo.n_chunks; ++c, ++cc) {
+        const int s = cc % geo.n_stage;
+        if (it == 0) ptx::mbar_wait(&bfull[c], 0);
+        ptx::mbar_wait(&full[s], (cc / geo.n_stage) & 1);
+        const uint32_t sa = ptx::smem_u32(sA + s * WS_ASTAGE), sb = ptx::smem_u32(sB + c * geo.nb_bytes);
+        const int klen = min(BK, k_total - c * BK);
+        ptx::wgmma_fence();
+#pragma unroll 1
+        for (int ks = 0; ks * 16 < klen; ++ks) {
+          const uint32_t acc = (c > 0 || ks > 0) ? 1u : 0u;
+          const uint64_t ad0 = desc_sw128(sa + ks * 32, 16, 1024), ad1 = desc_sw128(sa + 8192 + ks * 32, 16, 1024);
 #pragma unroll
-        for (int s4 = 0; s4 < 4; ++s4) {
-          const int mr = m_base + 8 * s4 + (lane >> 2), col = c * 32 + (lane & 3) * 8;
-          dst[s4] = make_uint4(0u, 0u, 0u, 0u);
-          if (c < c_hi && mr < g.M && col < g.N) dst[s4] = *reinterpret_cast<const uint4*>(g.gate + (size_t)mr * g.ldg + col);
+          for (int q = 0; q < NB; ++q) {
+            const int col0 = (wg * NB + q) * 64;
+            if (col0 < g.N) {                                     // warpgroup-uniform
+              const uint64_t bd = desc_sw128(sb + (col0 >> 6) * 8192 + (B_MN ? ks * 2048 : ks * 32), 16, 1024);
+              ptx::wgmma_n64<0, B_MN>(d[q][0], ad0, bd, acc);
+              ptx::wgmma_n64<0, B_MN>(d[q][1], ad1, bd, acc);
+            }
+          }
         }
-      };
-      if (EPI == EPI_GATE_F16) gate_fetch(c_lo, gpre[0]);
-      ptx::mbar_wait(&tfull[acc], (it >> 1) & 1);
-      ptx::tc_fence_after();
-      const uint32_t taddr = tm + ((uint32_t)(quad * 32) << 16) + acc * 256;
-      float v[2][32];
-      if (c_lo < c_hi) ptx::tmem_ld32(taddr + c_lo * 32, v[0]);
-#pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {
-        const int c = c_lo + cc;
-        if (c < c_hi) {
-          ptx::tmem_ld_wait();
-          if (cc < 3 && c + 1 < c_hi) ptx::tmem_ld32(taddr + (c + 1) * 32, v[(cc + 1) & 1]);
-          if (EPI == EPI_GATE_F16 && cc < 3) gate_fetch(c + 1, gpre[(cc + 1) & 1]);
-          epi_chunk<EPI, true>(g, v[cc & 1], m_base, lane, c * 32, sbias, sstage + warp * (EPI == EPI_F32 ? EPI_STAGE_F32 : EPI_STAGE_F16),
-                               EPI == EPI_GATE_F16 ? gpre[cc & 1] : nullptr, sbias);
-        }
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        if (lane == 0) ptx::mbar_arrive(&empty[s]);
       }
-      ptx::tc_fence_before();
-      ptx::mbar_arrive(&tempty[acc]);
+      const int m_base = t * BM + 16 * wq;
+      float v[32];
+#pragma unroll
+      for (int q = 0; q < NB; ++q) {
+        const int nb = (wg * NB + q) * 64;
+        if (nb < g.N) { frag_rows<0>(d[q][0], d[q][1], scratch, lane, v); epi_chunk<EPI, true>(g, v, m_base, lane, nb, sbias, scratch, nullptr, sbias); }
+        if (nb + 32 < g.N) { frag_rows<1>(d[q][0], d[q][1], scratch, lane, v); epi_chunk<EPI, true>(g, v, m_base, lane, nb + 32, sbias, scratch, nullptr, sbias); }
+      }
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 9) ptx::tmem_dealloc(tm, 512);
 }
 
 // ---- host: tensor maps ----------------------------------------------------------------------
@@ -588,7 +552,7 @@ static cudaError_t launch_gemm(const Operand& a1, const Operand& a2, const Opera
   if (!n_sm[dev & 63]) cudaDeviceGetAttribute(&n_sm[dev & 63], cudaDevAttrMultiProcessorCount, dev);
   g.mt = m_tiles; g.nt = n_tiles; g.zt = z;
   const long long total = (long long)m_tiles * n_tiles * z;
-  const int grid = (int)std::min<long long>(total, 2LL * n_sm[dev & 63]);
+  const int grid = (int)std::min<long long>(total, (long long)n_sm[dev & 63]);
   return launch_k(k_gemm_umma<A_MN, B_MN, EPI>, dim3(grid), dim3(GEMM_THREADS), GEMM_SMEM, st, mA1, mA2, mB, g);
 }
 
@@ -599,20 +563,20 @@ static cudaError_t launch_gemm_ws(const Operand& a1, const Operand& a2, const Op
                                   const Operand* b2 = nullptr) {
   const int K = g.K1 + g.K2;
   WsGeom geo;
-  geo.n_mma = (g.N + 15) / 16 * 16;
   geo.nb_bytes = (g.N + 127) / 128 * 128 * 128;
   geo.n_chunks = (K + BK - 1) / BK;
-  const int avail = WS_SMEM - 2048 - 8 * (EPI == EPI_F32 ? EPI_STAGE_F32 : EPI_STAGE_F16) - geo.n_chunks * geo.nb_bytes;
+  const int avail = WS_SMEM - 2048 - N_CWARPS * EPI_SCRATCH - geo.n_chunks * geo.nb_bytes;
   geo.n_stage = std::min(WS_MAXSTAGE, avail / WS_ASTAGE);
   if (g.N > 256 || geo.n_chunks > WS_MAXCHUNK || geo.n_stage < 3 || g.ksplit > 0 || (g.K2 > 0 && g.K1 % BK != 0))
     return cudaErrorNotSupported;
-  static bool attr[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (!attr[dev & 63]) {
-    cudaError_t e = cudaFuncSetAttribute(k_gemm_ws<B_MN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, WS_SMEM);
+  auto kern = g.N > 128 ? k_gemm_ws<B_MN, EPI, 2> : k_gemm_ws<B_MN, EPI, 1>;
+  static bool attr[64][2] = {};
+  if (!attr[dev & 63][g.N > 128]) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, WS_SMEM);
     if (e != cudaSuccess) return e;
-    attr[dev & 63] = true;
+    attr[dev & 63][g.N > 128] = true;
   }
   CUtensorMap mA1, mA2, mB;
   if (!make_operand_map(&mA1, a1.base, a1.rows, a1.cols, a1.ld, 0)) return cudaErrorInvalidValue;
@@ -626,7 +590,7 @@ static cudaError_t launch_gemm_ws(const Operand& a1, const Operand& a2, const Op
   if (!n_sm[dev & 63]) cudaDeviceGetAttribute(&n_sm[dev & 63], cudaDevAttrMultiProcessorCount, dev);
   g.mt = m_tiles; g.nt = 1; g.zt = 1;
   const int grid = std::min(m_tiles, n_sm[dev & 63]);
-  return launch_k(k_gemm_ws<B_MN, EPI>, dim3(grid), dim3(WS_THREADS), WS_SMEM, st, mA1, mA2, mB, mB2, g, geo);
+  return launch_k(kern, dim3(grid), dim3(WS_THREADS), WS_SMEM, st, mA1, mA2, mB, mB2, g, geo);
 }
 
 // forward / dgrad GEMMs: weight-stationary when the shape fits, generic otherwise

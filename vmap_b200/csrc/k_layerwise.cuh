@@ -1,6 +1,6 @@
 // Layer-wise tensor-core path for wide models (hidden 64 / 128 / 256: the separate background model
 // and the iMAP whole-scene model).  One object's weights (up to 640 KB of fp16) and a tile's
-// activations no longer fit in shared memory together, so each layer runs as a tcgen05 GEMM
+// activations no longer fit in shared memory together, so each layer runs as a wgmma GEMM
 // (k_gemm_umma.cuh) over ALL points of the object, activations living in an L2-resident workspace;
 // the thin stages between the GEMMs (positional embedding, heads, volume render + loss, head
 // gradients, PE gradient) are small CUDA-core kernels.  Same arithmetic and the same reference lines
@@ -42,6 +42,15 @@ static void fill_image_index(const VmbLayout& L, int* idx) {
     for (int k = 0; k < H; ++k) idx[L.o_Wm2 + o * H + k] = (int)(off_m2(H) + (long long)o * H + k);
     for (int k = 0; k < H + L.e2; ++k) idx[L.o_Wcl + o * (H + L.e2) + k] = (int)(off_cl(H) + (long long)o * (H + 48) + k);
   }
+}
+
+// multiprocessors of the current device (launch sizing)
+static int sm_count() {
+  static int n[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (!n[dev & 63]) cudaDeviceGetAttribute(&n[dev & 63], cudaDevAttrMultiProcessorCount, dev);
+  return n[dev & 63] > 0 ? n[dev & 63] : 132;
 }
 
 struct Workspace {
@@ -533,16 +542,16 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
   }
   const int hr_per_sm = std::max(1, std::min(8, (int)(227 * 1024 / (hr_smem<H>() + 6 * 1024))));
   arm();
-  LW_TRY(launch_k(k_lw_heads_render<H>, dim3(std::min((sp.R + 3) / 4, 148 * hr_per_sm)), dim3(128), (size_t)hr_smem<H>(), st, ra,
+  LW_TRY(launch_k(k_lw_heads_render<H>, dim3(std::min((sp.R + 3) / 4, sm_count() * hr_per_sm)), dim3(128), (size_t)hr_smem<H>(), st, ra,
                   (const __half*)ws.X4, (const __half*)ws.XC, Pb, L, ws.dYc, ws.dh16, ws.dalpha_s, G));
   if (!sp.backward) return 0;
 
   // ---- backward ----
   // split over points: enough z slices that the widest weight-gradient GEMM (2 x 2 output tiles) fills the machine
-  // (148 SMs x 2 resident CTAs) at any point count, bounded below so a slice still amortises its pipeline fill
-  const int ksplit = (int)std::min<long long>(4096, std::max<long long>(512, ((np * 4 / 296 + BK - 1) / BK) * BK));
+  // (one resident CTA per SM) at any point count, bounded below so a slice still amortises its pipeline fill
+  const int ksplit = (int)std::min<long long>(4096, std::max<long long>(512, ((np * 4 / sm_count() + BK - 1) / BK) * BK));
   const int zs = (int)((np + ksplit - 1) / ksplit);
-  const int cs_rows = (int)std::max<long long>(64, (np + 591) / 592);       // bias column sums: ~4 blocks per SM
+  const int cs_rows = (int)std::max<long long>(64, (np + 4 * sm_count() - 1) / (4 * sm_count()));       // bias column sums: ~4 blocks per SM
   // weight gradient: G[o*ldm + n] += sum_p dY[p][o] * X[p][n]   (A = dY^T, B = X, both MN-major, split over points)
   LW_TRY(ws.ensure_streams());
   cudaStream_t sd = ws.side;

@@ -1,29 +1,23 @@
-// K1, round 2: ONE launch per optimisation step for hidden = 32.
+// K1: ONE launch per optimisation step for hidden = 32 (sm_90a: wgmma, bulk async copy, mbarrier).
 //   mask counts (render_rays.py:68,86) -> PE -> MLP -> volume render -> losses -> backward
 //   -> per-object gradient reduction in a fixed order -> AdamW + fp16 weight-image refresh
-// fp16 operands / fp32 accumulate on tcgen05 (TMEM accumulators), weights staged per object with one bulk
-// async copy.  CTA = 2 point groups x 256 threads; a group owns a tile of up to 128 sample points (whole rays; one TMEM
-// lane = one point, two threads per point split the accumulator columns / PE directions) and walks it through 12
-// dependent MMA stages (6 forward, 6 backward): threads write the stage's operands -> group barrier -> one elected
-// lane of the group's first warp issues the tcgen05.mma batch and commits to the group's mbarrier -> threads read the
-// accumulator back with tcgen05.ld.  The two groups are independent, so one group's epilogue overlaps the other's
-// MMAs.  Shared-memory operand layout: SWIZZLE_NONE 8x8 core matrices, an activation block is
-// [feature-group (8 feats)][point][8 feats] halves -- the same bytes serve as a K-major A operand (dgrad: M = points,
-// K = features) and as an MN-major operand (wgrad: M or N = features, K = points).  Weight gradients accumulate in
-// TMEM across all the tiles a CTA owns for an object.  What the round-1 / round-2 cycle traces showed to be on the
-// critical path is off it:
-//   * the forward MMAs read their A operand from TENSOR MEMORY (tcgen05.mma [d], [a_tmem], b_desc: 16 cycles at N = 32
-//     instead of 40, tools/umma_bench2.cu): PE and the layer epilogues tcgen05.st the fp16 rows beside the shared-memory
-//     copy the weight-gradient MMAs need later, and no generic->async proxy fence sits on the forward chain;
+// fp16 operands / fp32 accumulate on wgmma.mma_async (m64nNk16, both operands from shared memory, accumulators in
+// registers), weights staged per object with one bulk async copy.  CTA = 256 threads = two warpgroups; a tile is up to
+// 128 sample points (whole rays) and walks through 12 dependent MMA stages (6 forward, 6 backward): threads write the
+// stage's operands -> fence + CTA barrier -> each warpgroup issues the stage's wgmmas for its 64 points and waits ->
+// the hidden-layer epilogues run on the accumulator fragments in registers.  Shared-memory operand layout: no-swizzle
+// 8x8 core matrices, an activation block is [feature-group (8 feats)][point][8 feats] halves -- the same bytes serve
+// as a K-major A operand (forward / dgrad: M = points, K = features) and as an MN-major operand (wgrad: M or N =
+// features, K = points).  Weight gradients accumulate in REGISTERS across all the tiles a CTA owns for an object (each
+// warpgroup owns 64 of the up-to-128 feature rows of every gradient tile: 96 registers per thread).
+//   * PE, the heads, the volume render and PE backward work one thread (pair) per point; the heads' 4 columns and the
+//     144 embedding-gradient columns cross from the fragment layout to the point layout through shared memory;
 //   * rays never straddle a warp (32/S rays per warp), so transmittance, the five rendered sums, the variance and
-//     the backward suffix sum are warp-shuffle scans over the sample axis in registers -- no per-ray serial loop,
-//     no fp32 scratch rows in shared memory;
-//   * dY_l is no longer stored over h_l: one spare 8 KB block (Z) and the blocks whose readers have retired are
-//     rotated (dYc->Z, dY4->HC, dY3->FC4, dY2->HC, dY1->FC3), so a stage commits after its 1-4 dgrad MMAs and the
-//     8 wgrad MMAs of the layer are issued behind the commit and overlap the next epilogue;
+//     the backward suffix sum are warp-shuffle scans over the sample axis in registers;
+//   * dY_l is not stored over h_l: one spare 8 KB block (Z) and the blocks whose readers have retired are rotated
+//     (dYc->Z, dY4->HC, dY3->FC4, dY2->HC, dY1->FC3);
 //   * both head weight gradients and both head bias gradients come out of ONE wgrad ([fc4 | emb2 | hc] x dhead);
-//   * the PE-direction gradient dB = dproj^T [x y z] is a wgrad MMA too (fp16 dproj block x the coordinate columns
-//     of the embedding block) instead of a shared-memory reduction;
+//   * the PE-direction gradient dB = dproj^T [x y z] is a wgrad MMA too;
 //   * K0 (mask counts) runs in the prologue, K2 (AdamW) in the last CTA to finish an object: every (CTA, object)
 //     segment writes its gradient partial to its own row, the finisher adds the rows in segment order (bitwise
 //     reproducible -- no floating-point atomics anywhere) and applies AdamW exactly as k_adamw does.
@@ -37,19 +31,6 @@
 #include "k_step_fp32.cuh"
 #include "umma_ptx.cuh"
 #include "k_umma_image.cuh"     // column maps, weight-image layout, PE ladders, packed-half helpers (namespace um)
-
-// Optional cycle trace (profiling builds only: -DVMB_TRACE), same buffer as the round-1 kernel
-#ifdef VMB_TRACE
-#define TRF(row, slot) do { if (blockIdx.x == 0 && (slot) < 256) g_vmb_trace[row][slot] = clock64(); } while (0)
-#else
-#define TRF(row, slot) do { } while (0)
-#endif
-// finer stamps inside the PE-forward phase of group 0 (row 2), profiling builds with -DVMB_TRACE -DVMB_TRACE_E0
-#if defined(VMB_TRACE) && defined(VMB_TRACE_E0)
-#define TRE() do { if (tid == 0) { TRF(2, tre); ++tre; } } while (0)
-#else
-#define TRE() do { } while (0)
-#endif
 
 struct FusedExtra {
   float* partials;            // [(B + grid)][stride] per-(CTA, object) gradient partials, row = blockIdx + object
@@ -68,45 +49,36 @@ struct FusedExtra {
   float lr_wd, one_m_b1, b2, one_m_b2, eps;
   int guard_loss;
   int* status;
-  int single_group;           // 1: only point group 0 walks tiles -> one in-order wgrad MMA stream per SM -> bitwise reproducible
   int cooperative;            // 1: cooperative launch (all CTAs resident): an object's CTAs share its reduction + update
   float* loss_sum;            // optional: sum over objects of the weighted loss totals, written by the last CTA to leave
 };
 
 namespace uf {
 
-constexpr int GT = 256, NT = 512, FGB = 2048;
+constexpr int GT = 256, NT = 256, FGB = 2048;
 // feature-group index of each 8-feature block inside a group's activation region.  Contiguity that the MMAs rely on:
 // [FC1|FC2|E1] (mid1 bias row = E1's constant-1 column, cat_layer K = 128), [FC3|FC4|E2|HC] (mid2 / alpha bias rows =
 // E2's constant-1 column, color_linear K = 80, heads wgrad M = [fc4 | emb2 | hc]).
 constexpr int FG_DH = 0, FG_FC1 = 2, FG_FC2 = 6, FG_E1 = 10, FG_FC3 = 22, FG_FC4 = 26, FG_E2 = 30, FG_HC = 36, FG_Z = 40, FG_DPR = 44;
 constexpr int FG_TOTAL = 47;
-constexpr int ACT_BYTES = FG_TOTAL * FGB;                         // 96256 per group
-constexpr int SM_ACT0 = 0, SM_ACT1 = ACT_BYTES, SM_W = 2 * ACT_BYTES, SM_MISC = SM_W + um::IMG_BYTES;
+constexpr int ACT_BYTES = FG_TOTAL * FGB;                         // 96256
+// Embedding-gradient tile (fp32): [36 blocks of 4 columns][128 points][4]: blocks 0..23 = d_emb1 (96 columns),
+// 24..35 = d_emb2 (48 columns).  The warpgroups store their wgmma fragments here; PE backward reads a point's row.
+constexpr int EG_BLOCKS = 36, EG_E2 = 24, EG_BYTES = EG_BLOCKS * FGB;
+constexpr int HD_BYTES = 128 * 16;                                // heads tile: [128 points][alpha, r, g, b] fp32
+constexpr int SM_ACT0 = 0, SM_EG = ACT_BYTES, SM_W = SM_EG + EG_BYTES, SM_HD = SM_W + um::IMG_BYTES, SM_MISC = SM_HD + HD_BYTES;
 constexpr int MISC_BYTES = 512;
 constexpr int SM_CNT = SM_MISC + MISC_BYTES;                      // int [B][3] mask counts
-constexpr int SMEM_MAX = 232448;
-constexpr int MAX_OBJ_SMEM = (SMEM_MAX - SM_CNT) / 12;            // objects whose counts fit (1062)
-// TMEM columns: persistent wgrad accumulators, then per group 160 columns:
-//   backward: acc[0,48) | - | E[64,160) (embedding-gradient tile)
-//   forward : acc[0,32) | hA[32,48) activation A-operand | alpha tile[48,64) | emb1 A-operand[64,112) | emb2 A-operand
-//             [112,136) | colour tile[136,152)             (VMB_TS_FWD: the forward MMAs read A from tensor memory)
-#ifndef VMB_TS_FWD
-#define VMB_TS_FWD 1
-#endif
-constexpr int WG_IN = 0, WG_M1 = 32, WG_CAT = 64, WG_M2 = 96, WG_CL = 128, WG_HD = 160, WG_DB = 176;
-constexpr int ACC0 = 192, ACC_STRIDE = 160, ACC_E = 64;
-constexpr int TC_HA = 32, TC_E1A = 64, TC_E2A = 112;
-constexpr int TC_ALPHA = VMB_TS_FWD ? 48 : 64, TC_COL = VMB_TS_FWD ? 136 : 80;
+constexpr int SMEM_MAX = 232448;                                  // 227 KB: the most one block may have on sm_90
+constexpr int MAX_OBJ_SMEM = (SMEM_MAX - SM_CNT) / 12;            // objects whose counts fit
 constexpr float LS = um::LS, INV_LS = um::INV_LS;
 
 struct Misc {
-  uint64_t done[2], wb[2], wbar;
-  uint32_t tmem_base;
+  uint64_t wbar;
   int on[3];
   int fin, skip;
   float step_size, bc2_sqrt;
-  float lsum[8][4];
+  float lsum[4][4];
 };
 static_assert(sizeof(Misc) <= MISC_BYTES, "Misc");
 
@@ -116,9 +88,8 @@ __device__ __forceinline__ uint32_t pack_relu_h2(float lo, float hi) {
   asm("cvt.rn.relu.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }
-__device__ __forceinline__ void group_bar(int g) { asm volatile("bar.sync %0, 256;" ::"r"(1 + g) : "memory"); }
 
-// wgrad accumulator (block 0..4, lane) -> (param index of out-column 0, stride per out-column), or -1
+// wgrad accumulator (block 0..4, feature row) -> (param index of out-column 0, stride per out-column), or -1
 __device__ __forceinline__ int wg_base(const VmbLayout& L, int blk, int lane, int& ld) {
   ld = 1;
   switch (blk) {
@@ -153,140 +124,36 @@ __device__ __forceinline__ int wg_base(const VmbLayout& L, int blk, int lane, in
   }
 }
 
-// ---- MMA issue: one elected lane of the group's first warp ------------------------------------------------------
-struct Issuer {
-  uint32_t a16, w16, tm, acc;      // (activation base, weight base) >> 4, TMEM base, this group's accumulator base
+// ---- MMA issue: warpgroup-collective wgmma.  The CTA's two warpgroups split M: for the forward / dgrad GEMMs (M = points)
+// warpgroup h owns points 64h .. 64h+63 of the tile, for the weight-gradient GEMMs (M = features) features 64h .. 64h+63
+// of the A block.  Rows past the block's real features read neighbouring blocks (for the dB tile, the start of the
+// embedding-gradient tile), possibly while the other warpgroup's epilogue rewrites them: a race on rows whose
+// accumulators are never stored, and on no others.
+struct Mma {
+  uint32_t a16, w16;               // (activation base, weight base) >> 4
+  int mh;                          // this warpgroup's M half
 
+  // shared-memory matrix descriptor, no swizzle: start address, leading / stride byte offsets (all >> 4)
   static __device__ __forceinline__ uint64_t mk(uint32_t base16, uint32_t off, uint32_t lbo, uint32_t sbo) {
-    const uint32_t lo = base16 + (off >> 4) + ((lbo >> 4) << 16);
-    const uint32_t hi = (sbo >> 4) | 0x4000u;
-    return ((uint64_t)hi << 32) | lo;
+    const uint32_t lo = ((base16 + (off >> 4)) & 0x3FFFu) | ((lbo >> 4) << 16);
+    return ((uint64_t)(sbo >> 4) << 32) | lo;
   }
-  __device__ __forceinline__ uint64_t a_k(int fg, int ks) const { return mk(a16, fg * FGB + ks * 4096, 2048, 128); }   // K-major A: M = points
-  __device__ __forceinline__ uint64_t x_mn(int fg, int ks) const { return mk(a16, fg * FGB + ks * 256, 128, 2048); }   // MN-major: M/N = features, K = points
+  __device__ __forceinline__ uint64_t a_k(int fg, int ks) const { return mk(a16, fg * FGB + mh * 1024 + ks * 4096, 2048, 128); }   // K-major A: M = this half's points
+  __device__ __forceinline__ uint64_t xa_mn(int fg, int ks) const { return mk(a16, (fg + 8 * mh) * FGB + ks * 256, 128, 2048); }  // MN-major A: M = this half's features, K = points
+  __device__ __forceinline__ uint64_t xb_mn(int fg, int ks) const { return mk(a16, fg * FGB + ks * 256, 128, 2048); }             // MN-major B: N = features, K = points
   __device__ __forceinline__ uint64_t w_k(int off, int ks) const { return mk(w16, off + ks * 1024, 512, 128); }
   __device__ __forceinline__ uint64_t w16_k(int off, int ks) const { return mk(w16, off + ks * 512, 256, 128); }
   __device__ __forceinline__ uint64_t w_mn(int off, int ks) const { return mk(w16, off + ks * 256, 128, 512); }
   __device__ __forceinline__ uint64_t w16_mn(int off) const { return mk(w16, off, 128, 256); }
 
-  // dW (+)= X^T dY over the tile's 128 points: A = X block (features on M), B = dY block (features on N)
-  __device__ __forceinline__ void wgrad(int col, int fgX, int fgDY, uint32_t idesc) const {
+  // dW += X^T dY over the tile's 128 points: A = X block (features on M), B = dY block (features on N)
+  __device__ __forceinline__ void wgrad32(float (&d)[16], int fgX, int fgDY) const {
 #pragma unroll
-    for (int ks = 0; ks < 8; ++ks) ptx::umma_f16(tm + col, x_mn(fgX, ks), x_mn(fgDY, ks), idesc, 1u);
+    for (int ks = 0; ks < 8; ++ks) ptx::wgmma_n32<1, 1>(d, xa_mn(fgX, ks), xb_mn(fgDY, ks), 1u);
   }
-
-  // the MMAs a stage's epilogue waits for
-  __device__ __forceinline__ void stage(int st) const {
-    constexpr uint32_t KK32 = ptx::idesc_f16(128, 32, 0, 0), KK16 = ptx::idesc_f16(128, 16, 0, 0);
-    constexpr uint32_t KM32 = ptx::idesc_f16(128, 32, 0, 1), KM48 = ptx::idesc_f16(128, 48, 0, 1), KM96 = ptx::idesc_f16(128, 96, 0, 1);
-    const uint32_t A = acc, E = acc + ACC_E;
-    switch (st) {
-#if VMB_TS_FWD
-      case 0:   // in_layer: emb1 (K = 96), A from tensor memory
+  __device__ __forceinline__ void wgrad16(float (&d)[8], int fgX, int fgDY) const {
 #pragma unroll
-        for (int ks = 0; ks < 6; ++ks) ptx::umma_f16_ts(A, acc + TC_E1A + ks * 8, w_k(um::IMG_WIN, ks), KK32, ks > 0);
-        break;
-      case 1:   // mid1: fc1
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16_ts(A, acc + TC_HA + ks * 8, w_k(um::IMG_WM1, ks), KK32, ks > 0);
-        break;
-      case 2:   // cat_layer: [fc2 | emb1] (K = 128)
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks)
-          ptx::umma_f16_ts(A, ks < 2 ? acc + TC_HA + ks * 8 : acc + TC_E1A + (ks - 2) * 8, w_k(um::IMG_WCAT, ks), KK32, ks > 0);
-        break;
-      case 3:   // mid2: fc3
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16_ts(A, acc + TC_HA + ks * 8, w_k(um::IMG_WM2, ks), KK32, ks > 0);
-        break;
-      case 4:   // color_linear: [fc4 | emb2] (K = 80) -> A ; out_alpha: fc4 -> alpha tile column 0
-#pragma unroll
-        for (int ks = 0; ks < 5; ++ks)
-          ptx::umma_f16_ts(A, ks < 2 ? acc + TC_HA + ks * 8 : acc + TC_E2A + (ks - 2) * 8, w_k(um::IMG_WCL, ks), KK32, ks > 0);
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16_ts(acc + TC_ALPHA, acc + TC_HA + ks * 8, w16_k(um::IMG_WA16, ks), KK16, ks > 0);
-        break;
-      case 5:   // out_color: hc -> its own 16-column tile (columns 1..3), so alpha's tile can be read while this runs
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16_ts(acc + TC_COL, acc + TC_HA + ks * 8, w16_k(um::IMG_WOC16, ks), KK16, ks > 0);
-        break;
-#else
-      case 0:   // in_layer: emb1 (K = 96)
-#pragma unroll
-        for (int ks = 0; ks < 6; ++ks) ptx::umma_f16(A, a_k(FG_E1, ks), w_k(um::IMG_WIN, ks), KK32, ks > 0);
-        break;
-      case 1:   // mid1: fc1
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16(A, a_k(FG_FC1, ks), w_k(um::IMG_WM1, ks), KK32, ks > 0);
-        break;
-      case 2:   // cat_layer: [fc2 | emb1] (K = 128)
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks) ptx::umma_f16(A, a_k(FG_FC2, ks), w_k(um::IMG_WCAT, ks), KK32, ks > 0);
-        break;
-      case 3:   // mid2: fc3
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16(A, a_k(FG_FC3, ks), w_k(um::IMG_WM2, ks), KK32, ks > 0);
-        break;
-      case 4:   // color_linear: [fc4 | emb2] (K = 80) -> A ; out_alpha: fc4 -> alpha tile column 0
-#pragma unroll
-        for (int ks = 0; ks < 5; ++ks) ptx::umma_f16(A, a_k(FG_FC4, ks), w_k(um::IMG_WCL, ks), KK32, ks > 0);
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16(acc + TC_ALPHA, a_k(FG_FC4, ks), w16_k(um::IMG_WA16, ks), KK16, ks > 0);
-        break;
-      case 5:   // out_color: hc -> its own 16-column tile (columns 1..3), so alpha's tile can be read while this runs
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16(acc + TC_COL, a_k(FG_HC, ks), w16_k(um::IMG_WOC16, ks), KK16, ks > 0);
-        break;
-#endif
-      case 6:   // d_hc = dhead @ W_oc
-        ptx::umma_f16(A, a_k(FG_DH, 0), w16_mn(um::IMG_WOC16), KM32, 0u);
-        break;
-      case 7:   // d_fc4 = dYc @ W_cl[:, :32] + dhead @ W_a
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16(A, a_k(FG_Z, ks), w_mn(um::IMG_WCL, ks), KM32, ks > 0);
-        ptx::umma_f16(A, a_k(FG_DH, 0), w16_mn(um::IMG_WA16), KM32, 1u);
-        break;
-      case 8:   // d_fc3 = dY4 @ W_m2                      (dY4 lives in HC)
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16(A, a_k(FG_HC, ks), w_mn(um::IMG_WM2, ks), KM32, ks > 0);
-        break;
-      case 9:   // d_fc2 = dY3 @ W_cat[:, :32]             (dY3 lives in FC4)
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16(A, a_k(FG_FC4, ks), w_mn(um::IMG_WCAT, ks), KM32, ks > 0);
-        break;
-      case 10:  // d_fc1 = dY2 @ W_m1                      (dY2 lives in HC)
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16(A, a_k(FG_HC, ks), w_mn(um::IMG_WM1, ks), KM32, ks > 0);
-        break;
-      default:  // 11: d_emb1 += dY1 @ W_in (dY1 in FC3) -> E ; d_emb2 = dYc @ W_cl[:, 32:] (dYc in Z) -> A[0..48)
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16(E, a_k(FG_FC3, ks), w_mn(um::IMG_WIN, ks), KM96, 1u);
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16(A, a_k(FG_Z, ks), w_mn(um::IMG_WCL + 4 * 512, ks), KM48, ks > 0);
-        break;
-    }
-  }
-  // issued BEHIND the stage's commit: nothing waits for these before the next stage's commit (in-order pipe)
-  __device__ __forceinline__ void post(int st) const {
-    constexpr uint32_t KM96 = ptx::idesc_f16(128, 96, 0, 1);
-    constexpr uint32_t MM32 = ptx::idesc_f16(128, 32, 1, 1), MM16 = ptx::idesc_f16(128, 16, 1, 1);
-    switch (st) {
-      case 6:  wgrad(WG_HD, FG_FC4, FG_DH, MM16); break;            // out_alpha + out_color weights and biases
-      case 7:  wgrad(WG_CL, FG_FC4, FG_Z, MM32); break;             // color_linear: [fc4 | emb2] x dYc
-      case 8:  wgrad(WG_M2, FG_FC3, FG_HC, MM32); break;            // mid2: fc3 x dY4
-      case 9:                                                        // d_emb1 = dY3 @ W_cat[:, 32:] -> E ; cat_layer wgrad
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::umma_f16(acc + ACC_E, a_k(FG_FC4, ks), w_mn(um::IMG_WCAT + 4 * 512, ks), KM96, ks > 0);
-        wgrad(WG_CAT, FG_FC2, FG_FC4, MM32);
-        break;
-      case 10: wgrad(WG_M1, FG_FC1, FG_HC, MM32); break;            // mid1: fc1 x dY2
-      case 11: wgrad(WG_IN, FG_E1, FG_FC3, MM32); break;            // in_layer: emb1 x dY1
-      default: break;
-    }
-  }
-  __device__ __forceinline__ void dirs_wgrad() const {               // dB = dproj^T [1 x y z ...]
-    constexpr uint32_t MM16 = ptx::idesc_f16(128, 16, 1, 1);
-    wgrad(WG_DB, FG_DPR, FG_E1, MM16);
+    for (int ks = 0; ks < 8; ++ks) ptx::wgmma_n16<1, 1>(d, xa_mn(fgX, ks), xb_mn(fgDY, ks), 1u);
   }
 };
 
@@ -313,17 +180,12 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
   int* cnt = reinterpret_cast<int*>(smem + SM_CNT);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int S = SC ? SC : a.S, R = a.R;
-  if (tid == 0) TRF(3, 199);
 
   if (tid == 0) {
-    ptx::mbar_init(&misc->done[0], 1); ptx::mbar_init(&misc->done[1], 1);
-    ptx::mbar_init(&misc->wb[0], 1);   ptx::mbar_init(&misc->wb[1], 1);
     ptx::mbar_init(&misc->wbar, 1);
     misc->on[0] = misc->on[1] = misc->on[2] = 1;
     ptx::mbar_init_fence();
   }
-  if (warp == 15) { ptx::tmem_alloc(&misc->tmem_base, 512); ptx::tmem_relinquish(); }
-  if (tid == 0) TRF(3, 210);          // barriers initialised
   const int G = gridDim.x;
   const long long gt_begin = rg.begin[blockIdx.x], gt_end = rg.begin[blockIdx.x + 1];
   __syncthreads();
@@ -331,12 +193,11 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     ptx::mbar_arrive_expect_tx(&misc->wbar, um::IMG_BYTES);
     ptx::bulk_g2s(smem + SM_W, image + (size_t)(gt_begin / npo) * um::IMG_BYTES, um::IMG_BYTES, &misc->wbar);
   }
-  if (tid == 0) TRF(3, 211);          // TMEM allocated (first __syncthreads passed), first weight copy issued
   // ---- K0 in the prologue: mask counts of EVERY object (the any-empty early-out couples them, render_rays.py:68-73).
   // Cooperative launch: CTA c counts objects c, c + grid, ... ONCE and publishes counts + empty flags + a "published"
   // counter in global memory; every CTA starts its tiles at once and acquires the counts right before its first
-  // volume render (thousands of cycles later: the wait is free).  Otherwise every CTA counts everything (148-fold
-  // redundant reads of the label / mask bytes: ~3 us of L2 traffic on the launch's critical path).
+  // volume render (thousands of cycles later: the wait is free).  Otherwise every CTA counts everything (every CTA
+  // reads all the label / mask bytes).
   const bool pub_counts = x.cooperative && !x.counts_in && !a.fwd_only;
   unsigned int* gbar = x.obj_done + 2 * a.B;            // [0] arrive, [1] depart, [2] objects published, [3..5] empty flags
   if (pub_counts) {
@@ -382,7 +243,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
         if (c == 0) misc->on[i % 3] = 0;
       }
     } else {
-      // warp w counts objects w, w+16, ...; two objects at a time with every load of both in flight together (the
+      // warp w counts objects w, w + NT/32, ...; two objects at a time with every load of both in flight together (the
       // inputs are cold in HBM: one latency per pair of objects instead of one per 8 words)
       const int nw = R >> 2;
       auto finish = [&](int b, int nd, int no, int ns) {
@@ -441,46 +302,30 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       }
     }
   }
-  if (tid == 0) TRF(3, 212);          // this warp's mask counts done
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  if (tid == 0) TRF(3, 213);          // all counts done
-  const uint32_t tm = misc->tmem_base;
-  if (warp < 8) {                     // zero the persistent wgrad accumulators (192 columns x 128 lanes)
-    const uint32_t zb = tm + ((uint32_t)((warp & 3) * 32) << 16) + (warp >> 2) * 96;
-#pragma unroll
-    for (int c = 0; c < 6; ++c) ptx::tmem_st_zero16(zb + c * 16);
-    ptx::tmem_st_wait();
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (tid == 0) TRF(3, 200);
-  ptx::tc_fence_after();
 
   uint32_t wpar = 0;                  // weight-barrier parity (one completion per segment)
-  uint32_t ph = 0, wph = 0;           // parities of this thread's group barriers: stage commits / deferred MMAs
-  bool wb_pending = false;            // deferred MMAs of the previous tile not yet known complete
 
-  // thread roles inside a group
-  const int g = warp >> 3, tg = tid & (GT - 1);
-  const int p = tg & 127, hsel = tg >> 7;               // point slot (= TMEM lane), column / direction half
+  // thread roles: point layout (PE, heads, render: one thread pair per point) ...
+  const int p = tid & 127, hsel = tid >> 7;               // point slot, direction half (= warpgroup)
   const int quad = (warp & 3);
   const int rw = lane / S, sidx = lane - rw * S;        // ray of this warp, sample index
   const bool lane_used = rw < rpw;
   const int ray_in_tile = quad * rpw + rw;
   const int seg_lo = lane - sidx;                        // first lane of this ray
-  unsigned char* act = smem + (g ? SM_ACT1 : SM_ACT0);
+  unsigned char* act = smem + SM_ACT0;
+  unsigned char* eg = smem + SM_EG;
+  float* hd = reinterpret_cast<float*>(smem + SM_HD);
   const float* wf = reinterpret_cast<const float*>(smem + SM_W + um::IMG_F32);
   const float* Bd = wf + um::F_DIRS;
-  const uint32_t lane_base = (uint32_t)(quad * 32) << 16;
-  const uint32_t tA = tm + ACC0 + g * ACC_STRIDE + lane_base, tE = tA + ACC_E;
-  Issuer is;
-  is.a16 = ptx::smem_u32(act) >> 4;
-  is.w16 = ptx::smem_u32(smem + SM_W) >> 4;
-  is.tm = tm;
-  is.acc = tm + ACC0 + g * ACC_STRIDE;
-  const bool issuer_warp = (warp & 7) == 0;
+  // ... and accumulator-fragment layout (wgmma m64nN): this thread holds rows fr0 and fr0 + 8, columns 8j + 2 cq + {0, 1}
+  const int cq = lane & 3, fr0 = 64 * hsel + 16 * quad + (lane >> 2);
+  Mma mm;
+  mm.a16 = ptx::smem_u32(act) >> 4;
+  mm.w16 = ptx::smem_u32(smem + SM_W) >> 4;
+  mm.mh = hsel;
+  // persistent weight-gradient accumulators of the current object (this warpgroup's 64 feature rows)
+  float wIN[16] = {}, wM1[16] = {}, wCAT[16] = {}, wM2[16] = {}, wCL[16] = {}, wHD[8] = {}, wDB[8] = {};
   // loss weights of this thread's current object: (term enabled: no object has an empty mask) / (this object's mask count)
   const float on_d = misc->on[0] ? 1.f : 0.f, on_c = misc->on[1] ? 1.f : 0.f, on_o = misc->on[2] ? 1.f : 0.f;
   float w_d = 0.f, w_c = 0.f, w_o = 0.f;
@@ -596,9 +441,8 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     return sk;
   };
 
-  // The work list is in units of TILE PAIRS (the two point groups of a CTA advance in lock-step rounds, one tile each):
-  // every segment of an object is a whole number of rounds -- with a per-tile split a segment boundary inside a CTA
-  // cost it an extra round.
+  // The work list is in units of TILE PAIRS (two consecutive tiles of an object, run one after the other), which is
+  // the unit the host-side partition balances.
   for (long long gt = gt_begin; gt < gt_end;) {
     const int b = (int)(gt / npo);
     const int p0 = (int)(gt - (long long)b * npo);
@@ -608,14 +452,10 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
 
     // ---- this object's weight image (one bulk copy global -> shared, issued before the previous segment's flush) ----
     um::mbar_wait_or_trap(&misc->wbar, wpar);
-    if (tid == 0) TRF(3, 201);
     wpar ^= 1;
 
     float ls_d = 0.f, ls_c = 0.f, ls_o = 0.f;
-    const int t_step = x.single_group ? 1 : 2;
-    const int t_first = x.single_group ? (g == 0 ? t0 : t1) : t0 + g;
     {
-    // ===================== compute threads of point group g ============================================================
     const float isc = 1.0f / a.scale[b];
     bool seg_w = false;               // w_d / w_c / w_o hold this segment's object?
     if (!a.fwd_only && !pub_counts) {
@@ -625,72 +465,48 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       seg_w = true;
     }
 
-    // operands written -> fence for the async proxy -> group barrier -> the elected lane of the group's first warp issues
-    // the stage's MMAs, commits, then issues the layer's weight-gradient MMAs behind the commit -> wait for the accumulator
-    // FWD_HANDOFF: a forward stage's MMAs read their A operand from tensor memory (tcgen05.st by the epilogue, no
-    // generic->async proxy fence on the chain); the shared-memory copies written beside it are first read by
-    // weight-gradient MMAs after stage 6's fence.
-#if VMB_TS_FWD
-#define FWD_HANDOFF() ptx::tmem_st_wait()
-#else
-#define FWD_HANDOFF() ptx::fence_async_smem()
-#endif
-#define STAGE_BEGIN(ST)                                \
-  do {                                                 \
-    if ((ST) < 6) FWD_HANDOFF(); else ptx::fence_async_smem(); \
-    ptx::tc_fence_before();                            \
-    group_bar(g);                                      \
-    TRG();                                             \
-    if (issuer_warp) {                                 \
-      ptx::tc_fence_after();                           \
-      if (ptx::elect_one()) {                          \
-        is.stage(ST);                                  \
-        ptx::umma_commit(&misc->done[g]);              \
-        is.post(ST);                                   \
-      }                                                \
-      __syncwarp();                                    \
-    }                                                  \
-  } while (0)
-#define STAGE_END()                                    \
-  do {                                                 \
-    um::mbar_wait_or_trap(&misc->done[g], ph);         \
-    ph ^= 1;                                           \
-    ptx::tc_fence_after();                             \
-    TRG();                                             \
-  } while (0)
-#define STAGE(ST) do { STAGE_BEGIN(ST); STAGE_END(); } while (0)
-    // hidden-layer epilogue on this thread's 16 columns: acc + bias -> ReLU -> fp16 (2 x 16 B)
-#define EPI_RELU(BIAS_OFF, FG)                                                                 \
-  do {                                                                                         \
-    float v[16];                                                                               \
-    ptx::tmem_ld16(tA + 16 * hsel, v);                                                         \
-    const float4* bp = reinterpret_cast<const float4*>(wf + (BIAS_OFF) + 16 * hsel);           \
-    const float4 b0 = bp[0], b1 = bp[1], b2 = bp[2], b3 = bp[3];                               \
-    ptx::tmem_ld_wait();                                                                       \
-    uint32_t hh[8];                                                                            \
-    hh[0] = pack_relu_h2(v[0] + b0.x, v[1] + b0.y);   hh[1] = pack_relu_h2(v[2] + b0.z, v[3] + b0.w);     \
-    hh[2] = pack_relu_h2(v[4] + b1.x, v[5] + b1.y);   hh[3] = pack_relu_h2(v[6] + b1.z, v[7] + b1.w);     \
-    hh[4] = pack_relu_h2(v[8] + b2.x, v[9] + b2.y);   hh[5] = pack_relu_h2(v[10] + b2.z, v[11] + b2.w);   \
-    hh[6] = pack_relu_h2(v[12] + b3.x, v[13] + b3.y); hh[7] = pack_relu_h2(v[14] + b3.z, v[15] + b3.w);   \
-    if (VMB_TS_FWD) ptx::tmem_st8(tA + TC_HA + 8 * hsel, hh);      /* next layer's A operand */              \
-    uint4* dst = reinterpret_cast<uint4*>(act + ((FG) + 2 * hsel) * FGB + p * 16);   /* wgrad's copy */      \
-    dst[0] = make_uint4(hh[0], hh[1], hh[2], hh[3]);                                           \
-    dst[128] = make_uint4(hh[4], hh[5], hh[6], hh[7]);                                         \
-  } while (0)
-    // dgrad epilogue: dY = (h > 0) * acc; h is read from its own block (FG_H), dY goes to a block whose readers retired
-#define EPI_DGRAD(FG_H, FG_OUT)                                                                \
-  do {                                                                                         \
-    float v[16];                                                                               \
-    ptx::tmem_ld16(tA + 16 * hsel, v);                                                         \
-    const uint4* hsrc = reinterpret_cast<const uint4*>(act + ((FG_H) + 2 * hsel) * FGB + p * 16); \
-    const uint4 o0 = hsrc[0], o1 = hsrc[128];                                                  \
-    ptx::tmem_ld_wait();                                                                       \
-    uint4* dst = reinterpret_cast<uint4*>(act + ((FG_OUT) + 2 * hsel) * FGB + p * 16);         \
-    dst[0] = make_uint4(um::gate_h2(um::pack_h2(v[0], v[1]), o0.x), um::gate_h2(um::pack_h2(v[2], v[3]), o0.y),       \
-                        um::gate_h2(um::pack_h2(v[4], v[5]), o0.z), um::gate_h2(um::pack_h2(v[6], v[7]), o0.w));      \
-    dst[128] = make_uint4(um::gate_h2(um::pack_h2(v[8], v[9]), o1.x), um::gate_h2(um::pack_h2(v[10], v[11]), o1.y),   \
-                          um::gate_h2(um::pack_h2(v[12], v[13]), o1.z), um::gate_h2(um::pack_h2(v[14], v[15]), o1.w)); \
-  } while (0)
+    // A stage: operands written by generic stores -> fence for the async proxy -> CTA barrier -> each warpgroup issues
+    // the stage's wgmmas on its M half and, behind them, the layer's weight-gradient wgmmas into the persistent
+    // accumulators -> commit -> wait.
+#define OPERANDS_READY() do { ptx::fence_async_smem(); __syncthreads(); ptx::wgmma_fence(); } while (0)
+#define MMA_DONE() do { ptx::wgmma_commit(); ptx::wgmma_wait<0>(); } while (0)
+    // hidden-layer epilogue on the fragment: acc + bias -> ReLU -> fp16 into block FG
+    auto epi_relu = [&](const float (&v)[16], int bias_off, int fg) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 bb = *reinterpret_cast<const float2*>(wf + bias_off + 8 * j + 2 * cq);
+        unsigned char* dst = act + (fg + j) * FGB + fr0 * 16 + cq * 4;
+        *reinterpret_cast<uint32_t*>(dst) = pack_relu_h2(v[4 * j] + bb.x, v[4 * j + 1] + bb.y);
+        *reinterpret_cast<uint32_t*>(dst + 128) = pack_relu_h2(v[4 * j + 2] + bb.x, v[4 * j + 3] + bb.y);
+      }
+    };
+    // dgrad epilogue: dY = (h > 0) * acc; h is read from its own block, dY goes to a block whose readers retired
+    auto epi_dgrad = [&](const float (&v)[16], int fg_h, int fg_out) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int off = j * FGB + fr0 * 16 + cq * 4;
+        const uint32_t h0 = *reinterpret_cast<const uint32_t*>(act + fg_h * FGB + off);
+        const uint32_t h1 = *reinterpret_cast<const uint32_t*>(act + fg_h * FGB + off + 128);
+        *reinterpret_cast<uint32_t*>(act + fg_out * FGB + off) = um::gate_h2(um::pack_h2(v[4 * j], v[4 * j + 1]), h0);
+        *reinterpret_cast<uint32_t*>(act + fg_out * FGB + off + 128) = um::gate_h2(um::pack_h2(v[4 * j + 2], v[4 * j + 3]), h1);
+      }
+    };
+    // embedding-gradient fragment (8-column groups starting at 4-column block blk0) -> the shared fp32 tile
+    auto eg_store = [&](const auto& v, int blk0) {
+      constexpr int NJ = (int)(sizeof(v) / 16);
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) {
+        float* d = reinterpret_cast<float*>(eg + (blk0 + 2 * j + (cq >> 1)) * FGB + fr0 * 16 + (cq & 1) * 8);
+        *reinterpret_cast<float2*>(d) = make_float2(v[4 * j], v[4 * j + 1]);
+        *reinterpret_cast<float2*>(d + 32) = make_float2(v[4 * j + 2], v[4 * j + 3]);
+      }
+    };
+    // eight consecutive embedding-gradient columns of this thread's point
+    auto eg_load8 = [&](int blk, float (&o)[8]) {
+      const float4 u0 = *reinterpret_cast<const float4*>(eg + blk * FGB + p * 16);
+      const float4 u1 = *reinterpret_cast<const float4*>(eg + (blk + 1) * FGB + p * 16);
+      o[0] = u0.x; o[1] = u0.y; o[2] = u0.z; o[3] = u0.w; o[4] = u1.x; o[5] = u1.y; o[6] = u1.z; o[7] = u1.w;
+    };
 
     // prefetched inputs of the next tile (global-load latency overlaps the current tile)
     float nx = 0.f, ny = 0.f, nz = 0.f, nzv = 0.f, n_gd = 0.f, n_c0 = 0.f, n_c1 = 0.f, n_c2 = 0.f;
@@ -724,23 +540,17 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       }
       n_live = true;                                      // live point
     };
-    prefetch(t_first);
+    prefetch(t0);
 
-    int trs = 0;
-#define TRG() do { if (tg == 0) { TRF(g, trs); ++trs; } } while (0)
-    for (int t = t_first; t < t1; t += t_step) {
+    for (int t = t0; t < t1; ++t) {
       const int ray = t * nr + ray_in_tile;
-      TRG();                                            // tile start
       // ---- E0: positional embedding (embedding.py:82-91) ----------------------------------------------------
       const float t0x = nx * isc, t1x = ny * isc, t2x = nz * isc, zv = nzv;
       const uint64_t tp0 = um::pk2(t0x, t0x), tp1 = um::pk2(t1x, t1x), tp2 = um::pk2(t2x, t2x);
       const float gd = n_gd, gc0 = n_c0, gc1 = n_c1, gc2 = n_c2;
       const int sv = n_sem, mv = n_msk;
       const bool live = n_live;
-      [[maybe_unused]] int tre = 16 * ((t - t_first) / t_step);
-      TRE();
-      prefetch(t + t_step);
-      TRE();
+      prefetch(t + 1);
       {
         uint4* e1 = reinterpret_cast<uint4*>(act + FG_E1 * FGB + p * 16);
         uint4* e2 = reinterpret_cast<uint4*>(act + FG_E2 * FGB + p * 16);
@@ -764,20 +574,10 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
           }
           um::sin_doubling4_x2(s01, s23, c01, c23, sv);
           s01 = ns01; s23 = ns23; c01 = nc01; c23 = nc23;
-          TRE();
-          if (q == q0 && wb_pending) {                  // the previous tile's deferred MMAs still read E1 / DPR / FC3
-            um::mbar_wait_or_trap(&misc->wb[g], wph); wph ^= 1; wb_pending = false;
-          }
           const uint4 ua = make_uint4(um::pack_h2(sv[0][0], sv[0][1]), um::pack_h2(sv[0][2], sv[0][3]), um::pack_h2(sv[1][0], sv[1][1]), um::pack_h2(sv[1][2], sv[1][3]));
           const uint4 ub = make_uint4(um::pack_h2(sv[2][0], sv[2][1]), um::pack_h2(sv[2][2], sv[2][3]), um::pack_h2(sv[3][0], sv[3][1]), um::pack_h2(sv[3][2], sv[3][3]));
           const uint4 uc = make_uint4(um::pack_h2(sv[0][4], sv[0][5]), um::pack_h2(sv[1][4], sv[1][5]), um::pack_h2(sv[2][4], sv[2][5]), um::pack_h2(sv[3][4], sv[3][5]));
           e1[(2 * q + 1) * 128] = ua; e1[(2 * q + 2) * 128] = ub; e2[q * 128] = uc;
-          if (VMB_TS_FWD) {       // the same 8-feature chunks as A-operand columns (4 packed columns per chunk)
-            ptx::tmem_st4(tA + TC_E1A + (2 * q + 1) * 4, ua.x, ua.y, ua.z, ua.w);
-            ptx::tmem_st4(tA + TC_E1A + (2 * q + 2) * 4, ub.x, ub.y, ub.z, ub.w);
-            ptx::tmem_st4(tA + TC_E2A + q * 4, uc.x, uc.y, uc.z, uc.w);
-          }
-          TRE();
         }
         if (hsel) {
           // direction 20 shares chunk 0 of emb1 with [1, x, y, z] and chunk 5 of emb2 with the const-1 column
@@ -788,33 +588,47 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
           e1[0] = u0;
           e2[5 * 128] = u5;
           e1[11 * 128] = make_uint4(0u, 0u, 0u, 0u);
-          if (VMB_TS_FWD) {
-            ptx::tmem_st4(tA + TC_E1A, u0.x, u0.y, u0.z, u0.w);
-            ptx::tmem_st4(tA + TC_E2A + 20, u5.x, u5.y, u5.z, u5.w);
-            ptx::tmem_st4(tA + TC_E1A + 44, 0u, 0u, 0u, 0u);
-          }
           // zero this point's dhead row (cols 4..15 stay zero; 0..3 are written after the render)
           uint4* dh = reinterpret_cast<uint4*>(act + FG_DH * FGB + p * 16);
           dh[0] = make_uint4(0u, 0u, 0u, 0u); dh[128] = make_uint4(0u, 0u, 0u, 0u);
         }
       }
-      TRG();                                            // E0 done
-      STAGE(0);                                         // in_layer
-      EPI_RELU(um::F_BIN, FG_FC1);
-      TRG();
-      STAGE(1);                                         // mid1
-      EPI_RELU(um::F_BM1, FG_FC2);
-      TRG();
-      STAGE(2);                                         // cat_layer
-      EPI_RELU(um::F_BCAT, FG_FC3);
-      TRG();
-      STAGE(3);                                         // mid2
-      EPI_RELU(um::F_BM2, FG_FC4);
-      TRG();
-      STAGE(4);                                         // color_linear + out_alpha
-      EPI_RELU(um::F_BCL, FG_HC);
-      TRG();
-      STAGE_BEGIN(5);                                   // out_color runs while the alpha-only part of the render is computed
+      float acc[16], hacc[8];
+      OPERANDS_READY();                                 // in_layer: emb1 (K = 96)
+#pragma unroll
+      for (int ks = 0; ks < 6; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_E1, ks), mm.w_k(um::IMG_WIN, ks), ks > 0);
+      MMA_DONE();
+      epi_relu(acc, um::F_BIN, FG_FC1);
+      OPERANDS_READY();                                 // mid1: fc1
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_FC1, ks), mm.w_k(um::IMG_WM1, ks), ks > 0);
+      MMA_DONE();
+      epi_relu(acc, um::F_BM1, FG_FC2);
+      OPERANDS_READY();                                 // cat_layer: [fc2 | emb1] (K = 128)
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_FC2, ks), mm.w_k(um::IMG_WCAT, ks), ks > 0);
+      MMA_DONE();
+      epi_relu(acc, um::F_BCAT, FG_FC3);
+      OPERANDS_READY();                                 // mid2: fc3
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_FC3, ks), mm.w_k(um::IMG_WM2, ks), ks > 0);
+      MMA_DONE();
+      epi_relu(acc, um::F_BM2, FG_FC4);
+      OPERANDS_READY();                                 // color_linear: [fc4 | emb2] (K = 80) ; out_alpha: fc4 -> column 0
+#pragma unroll
+      for (int ks = 0; ks < 5; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_FC4, ks), mm.w_k(um::IMG_WCL, ks), ks > 0);
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16<0, 0>(hacc, mm.a_k(FG_FC4, ks), mm.w16_k(um::IMG_WA16, ks), ks > 0);
+      MMA_DONE();
+      epi_relu(acc, um::F_BCL, FG_HC);
+      if (cq == 0) { hd[fr0 * 4] = hacc[0]; hd[(fr0 + 8) * 4] = hacc[2]; }
+      OPERANDS_READY();                                 // out_color: hc -> columns 1..3
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16<0, 0>(hacc, mm.a_k(FG_HC, ks), mm.w16_k(um::IMG_WOC16, ks), ks > 0);
+      MMA_DONE();
+      if (cq == 0) { hd[fr0 * 4 + 1] = hacc[1]; hd[(fr0 + 8) * 4 + 1] = hacc[3]; }
+      if (cq == 1) { hd[fr0 * 4 + 2] = hacc[0]; hd[fr0 * 4 + 3] = hacc[1]; hd[(fr0 + 8) * 4 + 2] = hacc[2]; hd[(fr0 + 8) * 4 + 3] = hacc[3]; }
+      __syncthreads();                                  // heads tile: fragment layout -> point layout
       // ---- heads + volume render + losses + ray gradients, all in registers of the hsel == 0 warps ---------------
       // rays never straddle a warp: the scans over the sample axis are warp shuffles
       auto raysum = [&](float v) {                      // per-ray sum: guarded tree reduction to the ray's first lane, broadcast
@@ -825,7 +639,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
         return __shfl_sync(0xffffffffu, v, seg_lo);
       };
       float araw = 0.f, occ = 0.f, fr = 1.f, Tr = 1.f, w = 0.f, D = 0.f, O = 0.f, V = 0.f;
-      if (hsel == 0) {                                  // alpha's tile was complete with stage 4
+      if (hsel == 0) {
         if (!seg_w && pub_counts) {                     // cooperative launch: acquire the published mask counts (first render only)
           if (!cnt_ready) {
             const volatile unsigned int* pubd = gbar + 2;
@@ -841,10 +655,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
           w_o = (ef[2] ? 0.f : 1.f) / ((float)cp[2] + 1e-10f);
           seg_w = true;
         }
-        float hv[8];
-        um::tmem_ld8(tA + TC_ALPHA, hv);
-        ptx::tmem_ld_wait();
-        araw = (hv[0] + wf[um::F_BA]) * 10.0f;                                   // model.py:77
+        araw = (hd[p * 4] + wf[um::F_BA]) * 10.0f;                                   // model.py:77
         occ = um::fast_sigmoid(araw);                                            // render_rays.py:6
         if (!a.fwd_only) {
           if (!live) occ = 0.f;
@@ -863,13 +674,10 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
           V = raysum(w * dz * dz);                                                // render_rays.py:47-51 (detached)
         }
       }
-      STAGE_END();
       if (hsel == 0) {
-        float hv[8];
-        um::tmem_ld8(tA + TC_COL, hv);
-        ptx::tmem_ld_wait();
-        const float c0 = um::fast_sigmoid(hv[1] + wf[um::F_BOC + 0]), c1 = um::fast_sigmoid(hv[2] + wf[um::F_BOC + 1]),
-                    c2 = um::fast_sigmoid(hv[3] + wf[um::F_BOC + 2]);
+        const float4 hv = *reinterpret_cast<const float4*>(hd + p * 4);
+        const float c0 = um::fast_sigmoid(hv.y + wf[um::F_BOC + 0]), c1 = um::fast_sigmoid(hv.z + wf[um::F_BOC + 1]),
+                    c2 = um::fast_sigmoid(hv.w + wf[um::F_BOC + 2]);
         if (a.fwd_only) {                               // eval_points (trainer.py:77-90): raw alpha*10, sigmoid colour per point
           if (live) {
             const size_t n = (size_t)ray * S + sidx;
@@ -913,24 +721,58 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
           }
         }
       }
-      TRG();                                            // heads + render done
-      if (a.fwd_only || !a.backward) { group_bar(g); continue; }
-      STAGE(6);                                         // d_hc            (+ heads wgrad behind the commit)
-      EPI_DGRAD(FG_HC, FG_Z);                           // dYc -> Z
-      TRG();
-      STAGE(7);                                         // d_fc4           (+ wgrad color_linear)
-      EPI_DGRAD(FG_FC4, FG_HC);                         // dY4 -> HC
-      TRG();
-      STAGE(8);                                         // d_fc3           (+ wgrad mid2)
-      EPI_DGRAD(FG_FC3, FG_FC4);                        // dY3 -> FC4
-      TRG();
-      STAGE(9);                                         // d_fc2           (+ d_emb1 part 1, wgrad cat_layer)
-      EPI_DGRAD(FG_FC2, FG_HC);                         // dY2 -> HC
-      TRG();
-      STAGE(10);                                        // d_fc1           (+ wgrad mid1)
-      EPI_DGRAD(FG_FC1, FG_FC3);                        // dY1 -> FC3
-      TRG();
-      STAGE(11);                                        // d_emb1 part 2 -> E, d_emb2 -> A[0..48)   (+ wgrad in_layer)
+      if (a.fwd_only || !a.backward) { __syncthreads(); continue; }
+      OPERANDS_READY();                                 // d_hc = dhead @ W_oc ; heads wgrad (out_alpha + out_color, weights and biases)
+      ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_DH, 0), mm.w16_mn(um::IMG_WOC16), 0u);
+      mm.wgrad16(wHD, FG_FC4, FG_DH);
+      MMA_DONE();
+      epi_dgrad(acc, FG_HC, FG_Z);                      // dYc -> Z
+      OPERANDS_READY();                                 // d_fc4 = dYc @ W_cl[:, :32] + dhead @ W_a ; wgrad color_linear
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_Z, ks), mm.w_mn(um::IMG_WCL, ks), ks > 0);
+      ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_DH, 0), mm.w16_mn(um::IMG_WA16), 1u);
+      mm.wgrad32(wCL, FG_FC4, FG_Z);
+      MMA_DONE();
+      epi_dgrad(acc, FG_FC4, FG_HC);                    // dY4 -> HC
+      OPERANDS_READY();                                 // d_fc3 = dY4 @ W_m2 ; wgrad mid2
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_HC, ks), mm.w_mn(um::IMG_WM2, ks), ks > 0);
+      mm.wgrad32(wM2, FG_FC3, FG_HC);
+      MMA_DONE();
+      epi_dgrad(acc, FG_FC3, FG_FC4);                   // dY3 -> FC4
+      OPERANDS_READY();                                 // d_fc2 = dY3 @ W_cat[:, :32] ; wgrad cat_layer
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_FC4, ks), mm.w_mn(um::IMG_WCAT, ks), ks > 0);
+      mm.wgrad32(wCAT, FG_FC2, FG_FC4);
+      MMA_DONE();
+      epi_dgrad(acc, FG_FC2, FG_HC);                    // dY2 -> HC
+      OPERANDS_READY();                                 // d_fc1 = dY2 @ W_m1 ; wgrad mid1
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_HC, ks), mm.w_mn(um::IMG_WM1, ks), ks > 0);
+      mm.wgrad32(wM1, FG_FC1, FG_HC);
+      MMA_DONE();
+      epi_dgrad(acc, FG_FC1, FG_FC3);                   // dY1 -> FC3
+      // d_emb1 = dY3 @ W_cat[:, 32:] + dY1 @ W_in (32 columns at a time), d_emb2 = dYc @ W_cl[:, 32:] ; wgrad in_layer
+      OPERANDS_READY();
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_FC4, ks), mm.w_mn(um::IMG_WCAT + (4 + 4 * c) * 512, ks), ks > 0);
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_FC3, ks), mm.w_mn(um::IMG_WIN + 4 * c * 512, ks), 1u);
+        MMA_DONE();
+        eg_store(acc, 8 * c);
+        ptx::wgmma_fence();
+      }
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_Z, ks), mm.w_mn(um::IMG_WCL + 4 * 512, ks), ks > 0);
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16<0, 1>(hacc, mm.a_k(FG_Z, ks), mm.w_mn(um::IMG_WCL + 8 * 512, ks), ks > 0);
+      mm.wgrad32(wIN, FG_E1, FG_FC3);
+      MMA_DONE();
+      eg_store(acc, EG_E2);
+      eg_store(hacc, EG_E2 + 8);
+      __syncthreads();                                  // embedding-gradient tile: fragment layout -> point layout
       // ---- PE backward: dproj_d = pi * sum_k 2^k g_{k,d} cos(pi 2^k proj_d), written as an fp16 block --------------
       {
         const int q0 = hsel ? 3 : 0, q1 = hsel ? 5 : 3;
@@ -943,9 +785,9 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
 #pragma unroll 1
         for (int q = q0; q < q1; ++q) {
           float g1a[8], g1b[8], g2[8];
-          um::tmem_ld8(tE + 16 * q + 8, g1a);          // emb1 cols of directions 4q, 4q+1 (k = 0..3)
-          um::tmem_ld8(tE + 16 * q + 16, g1b);         //                          4q+2, 4q+3
-          um::tmem_ld8(tA + 8 * q, g2);                // emb2 cols (k = 4, 5)
+          eg_load8(4 * q + 2, g1a);                    // emb1 cols of directions 4q, 4q+1 (k = 0..3)
+          eg_load8(4 * q + 4, g1b);                    //                          4q+2, 4q+3
+          eg_load8(EG_E2 + 2 * q, g2);                 // emb2 cols (k = 4, 5)
           float cv[4][6], dp[4];
           uint64_t nc01 = 0, nc23 = 0;
           if (q + 1 < q1) {                            // next chunk's front half before this chunk's recurrence
@@ -955,7 +797,6 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
           }
           um::cos_doubling4_x2(c01, c23, cv);
           c01 = nc01; c23 = nc23;
-          ptx::tmem_ld_wait();
 #pragma unroll
           for (int dd = 0; dd < 4; ++dd) {
             const float* g1 = (dd < 2) ? (g1a + dd * 4) : (g1b + (dd - 2) * 4);
@@ -973,36 +814,26 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
         }
         if (hsel) {                                     // direction 20: emb1 cols 4..7, emb2 cols 40, 41
           float g1[8], g2[8], c[6];
-          um::tmem_ld8(tE, g1);
-          um::tmem_ld8(tA + 40, g2);
+          eg_load8(0, g1);
+          eg_load8(EG_E2 + 10, g2);
           um::cos_ladder(fmaf(Bd[2 * um::DIRS_PITCH + 20], t2x, fmaf(Bd[um::DIRS_PITCH + 20], t1x, Bd[20] * t0x)), c);
-          ptx::tmem_ld_wait();
           float d = g1[4] * c[0];
           d = fmaf(2.f * g1[5], c[1], d); d = fmaf(4.f * g1[6], c[2], d); d = fmaf(8.f * g1[7], c[3], d);
           d = fmaf(16.f * g2[0], c[4], d); d = fmaf(32.f * g2[1], c[5], d);
           *reinterpret_cast<uint2*>(act + (FG_DPR + 2) * FGB + p * 16 + 8) = make_uint2(um::pack_h2(d * VMB_PI_F, 0.f), 0u);
         }
       }
-      TRG();                                            // PE backward done
-      // dB (+)= dproj^T [x y z] as a wgrad MMA; its commit also covers wgrad in_layer issued behind stage 11
-      ptx::fence_async_smem();
-      ptx::tc_fence_before();
-      group_bar(g);
-      if (issuer_warp) {
-        ptx::tc_fence_after();
-        if (ptx::elect_one()) { is.dirs_wgrad(); ptx::umma_commit(&misc->wb[g]); }
-        __syncwarp();
-      }
-      wb_pending = true;
-      TRG();
+      // dB += dproj^T [1 x y z ...]: the 21 real feature rows are in the first warpgroup's half; the second issues the
+      // same instructions on rows that are never stored, which keeps the wgmma stream free of divergent branches
+      OPERANDS_READY();
+      mm.wgrad16(wDB, FG_DPR, FG_E1);
+      MMA_DONE();
+      __syncthreads();                                  // the next tile's PE overwrites E1 / E2 / DH
     }
-#undef TRG
-#undef STAGE
-#undef EPI_RELU
-#undef EPI_DGRAD
-    if (wb_pending) { um::mbar_wait_or_trap(&misc->wb[g], wph); wph ^= 1; wb_pending = false; }
+#undef OPERANDS_READY
+#undef MMA_DONE
     }   // compute threads
-    if (a.fwd_only) {                                   // nothing to reduce; the weight buffer is free once both groups are done
+    if (a.fwd_only) {                                   // nothing to reduce; the weight buffer is free once every warp is done
       __syncthreads();
       if (tid == 0 && gt < gt_end) {
         ptx::mbar_arrive_expect_tx(&misc->wbar, um::IMG_BYTES);
@@ -1012,61 +843,60 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     }
     // ---- segment end: this CTA's partial sums for object b -----------------------------------------------------
     ls_d = warp_sum(ls_d); ls_c = warp_sum(ls_c); ls_o = warp_sum(ls_o);
-    if (hsel == 0 && lane == 0) { float* l = misc->lsum[g * 4 + quad]; l[0] = ls_d; l[1] = ls_c; l[2] = ls_o; }
-    ptx::tc_fence_before();
+    if (hsel == 0 && lane == 0) { float* l = misc->lsum[quad]; l[0] = ls_d; l[1] = ls_c; l[2] = ls_o; }
     __syncthreads();
-    if (tid == 0) TRF(3, 202);
-    ptx::tc_fence_after();
     if (tid == 0 && gt < gt_end) {          // every MMA of this segment has completed: the weight buffer is free --
       ptx::mbar_arrive_expect_tx(&misc->wbar, um::IMG_BYTES);        // the next object's image lands during the flush
       ptx::bulk_g2s(smem + SM_W, image + (size_t)(gt / npo) * um::IMG_BYTES, um::IMG_BYTES, &misc->wbar);
     }
-    // the segment's gradient row is assembled in shared memory (group 0's activation region is idle now: the scattered
+    // the segment's gradient row is assembled in shared memory (the activation region is idle now: the scattered
     // 4-byte stores of the accumulator -> parameter-index mapping cost nothing there) and leaves as coalesced 16-byte stores
     float* Pr = reinterpret_cast<float*>(smem + SM_ACT0);
     if (tid < 3) {                                      // fixed summation order -> reproducible loss terms
       float s = 0.f;
 #pragma unroll
-      for (int w8 = 0; w8 < 8; ++w8) s += misc->lsum[w8][tid];
+      for (int w8 = 0; w8 < 4; ++w8) s += misc->lsum[w8][tid];
       Pr[L.P + tid] = s;
     }
-    if (a.backward && warp < 8) {
-      // TMEM -> registers -> this segment's row of the partial block (plain stores, no atomics)
-      const int q = warp & 3, half = warp >> 2, ln = q * 32 + lane;
-#pragma unroll 1
-      for (int cc = 0; cc < 3; ++cc) {
-        const int blk = half * 3 + cc;
-        float v[32];
-        ptx::tmem_ld32(tm + ((uint32_t)(q * 32) << 16) + blk * 32, v);
-        ptx::tmem_ld_wait();
-        if (blk < 5) {
+    if (a.backward) {
+      // accumulator fragments -> this segment's row of the partial block (plain stores, no atomics), then cleared for
+      // the next object
+      auto put = [&](float (&d)[16], int blk) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
           int ld;
-          const int base = wg_base(L, blk, ln, ld);
+          const int base = wg_base(L, blk, fr0 + 8 * i, ld);
           if (base >= 0) {
-            float* gp = Pr + base;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) gp[j * ld] = v[j] * INV_LS;
-          }
-        } else {    // heads tile: A = [fc4 | emb2 | hc], B = dhead (col 0 = alpha, 1..3 = colour); then the dB tile
-          if (ln < 32) {
-            Pr[L.o_Wa + ln] = v[0] * INV_LS;
-          } else if (ln == 32 + 42) {                   // emb2's constant-1 column: all four head biases
-            Pr[L.o_ba] = v[0] * INV_LS;
+            for (int j = 0; j < 4; ++j)
 #pragma unroll
-            for (int c = 0; c < 3; ++c) Pr[L.o_boc + c] = v[1 + c] * INV_LS;
-          } else if (ln >= 80 && ln < 112) {
-#pragma unroll
-            for (int c = 0; c < 3; ++c) Pr[L.o_Woc + c * 32 + (ln - 80)] = v[1 + c] * INV_LS;
-          }
-          if (ln < VMB_NDIRS) {                         // dB[d][i]: A = dproj block, B = emb1 cols [1, x, y, z, ...]
-#pragma unroll
-            for (int i = 0; i < 3; ++i) Pr[L.o_B + ln * 3 + i] = v[16 + 1 + i] * INV_LS;
+              for (int e = 0; e < 2; ++e) Pr[base + (8 * j + 2 * cq + e) * ld] = d[4 * j + 2 * i + e] * INV_LS;
           }
         }
-        ptx::tmem_st_zero16(tm + ((uint32_t)(q * 32) << 16) + blk * 32);       // ready for the next object
-        ptx::tmem_st_zero16(tm + ((uint32_t)(q * 32) << 16) + blk * 32 + 16);
+#pragma unroll
+        for (int k = 0; k < 16; ++k) d[k] = 0.f;
+      };
+      put(wIN, 0); put(wM1, 1); put(wCAT, 2); put(wM2, 3); put(wCL, 4);
+      // heads tile: A = [fc4 | emb2 | hc], B = dhead (col 0 = alpha, 1..3 = colour); dB tile: A = dproj, B = emb1 cols [1, x, y, z]
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int ln = fr0 + 8 * i;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = 2 * cq + e;
+          const float vh = wHD[2 * i + e] * INV_LS, vb = wDB[2 * i + e] * INV_LS;
+          if (col == 0) {
+            if (ln < 32) Pr[L.o_Wa + ln] = vh;
+            else if (ln == 32 + 42) Pr[L.o_ba] = vh;    // emb2's constant-1 column: the head biases
+          } else if (col < 4) {
+            if (ln == 32 + 42) Pr[L.o_boc + col - 1] = vh;
+            else if (ln >= 80 && ln < 112) Pr[L.o_Woc + (col - 1) * 32 + (ln - 80)] = vh;
+            if (ln < VMB_NDIRS) Pr[L.o_B + ln * 3 + col - 1] = vb;
+          }
+        }
       }
-      ptx::tmem_st_wait();
+#pragma unroll
+      for (int k = 0; k < 8; ++k) { wHD[k] = 0.f; wDB[k] = 0.f; }
     }
     __syncthreads();
     {
@@ -1092,10 +922,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
         }
       }
     }
-    ptx::tc_fence_before();
     __syncthreads();
-    if (tid == 0) TRF(3, 203);
-    ptx::tc_fence_after();
   }
 
   if (x.cooperative && !a.fwd_only) {
@@ -1112,9 +939,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     }
     __syncthreads();
     __threadfence();
-    if (tid == 0) TRF(3, 205);
     const int n4 = L.stride >> 2;
-    if (tid == 0) TRF(3, 206);
     const long long W = (long long)a.B * n4;
     const long long lo = (W * blockIdx.x) / G, hi = (W * (blockIdx.x + 1)) / G;
     for (int b = (int)(lo / n4); (long long)b * n4 < hi; ++b) {
@@ -1123,10 +948,8 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       const int skip = finish_rows(b, i_lo, i_hi, i_lo == 0);
       if (i_lo == 0 && tid == 0) x.obj_done[a.B + b] = (unsigned int)skip;
     }
-    if (tid == 0) TRF(3, 207);          // this CTA's slices reduced + updated
     __threadfence();
     __syncthreads();
-    if (tid == 0) TRF(3, 208);          // fenced
     if (tid == 0) misc->fin = (atomicAdd(&gbar[1], 1u) + 1u == (unsigned int)G) ? 1 : 0;
     __syncthreads();
     if (misc->fin) {                                    // the last CTA to leave: step numbers, re-arm the barrier
@@ -1144,8 +967,6 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     }
   }
 
-  if (tid == 0) TRF(3, 204);
-  if (warp == 15) ptx::tmem_dealloc(tm, 512);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1154,7 +975,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
 static int fused_rows_needed(int n_obj, int n_sm) { return n_obj + n_sm; }
 
 // Cost-aware split of B objects x npo tile pairs over G CTAs.  Starting a second object inside a CTA costs it a flush
-// of the gradient partial, a weight load and a pipeline refill (~0.4 of a round measured), so pairs are laid out on a
+// of the gradient partial, a weight load and a pipeline refill, so pairs are laid out on a
 // virtual axis x(p) = p + beta * (object of p) -- every object boundary is a gap of beta -- and that axis is split
 // evenly: a CTA whose range crosses a boundary gets correspondingly fewer pairs.  beta is the largest of {1, 0.7, 0.4, 0}
 // that does not raise the maximum number of rounds per CTA.

@@ -14,10 +14,6 @@
 #include "common.cuh"
 #include "umma_ptx.cuh"
 
-#ifdef VMB_TRACE
-__device__ long long g_vmb_trace[4][256];
-#endif
-
 namespace um {
 
 // weight image (bytes)
@@ -80,13 +76,6 @@ __device__ __forceinline__ uint32_t gate_h2(uint32_t dy, uint32_t h) {
   __half2 r = __hmul2(*reinterpret_cast<__half2*>(&dy), m);
   return *reinterpret_cast<uint32_t*>(&r);
 }
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr) : "memory");
-}
-
 // Bring-up safety net: a protocol bug traps (CUDA error) instead of hanging the GPU.
 #ifndef VMB_SPIN_LIMIT
 #define VMB_SPIN_LIMIT 50000000u
@@ -147,12 +136,24 @@ __device__ __forceinline__ void cos_ladder(float proj, float (&c)[6]) {
 }
 
 
-// ---- packed fp32 (FFMA2 / FMUL2 / FADD2, sm_100): two directions per instruction ------------------------------------
+// ---- fp32 pairs: two directions per value (plain fp32 arithmetic on each half) -------------------------------------
 __device__ __forceinline__ uint64_t pk2(float lo, float hi) { uint64_t r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
 __device__ __forceinline__ void upk2(uint64_t v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) { uint64_t d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
-__device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) { uint64_t d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) { uint64_t d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
+__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
+  float a0, a1, b0, b1, c0, c1;
+  upk2(a, a0, a1); upk2(b, b0, b1); upk2(c, c0, c1);
+  return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
+}
+__device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) {
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1); upk2(b, b0, b1);
+  return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
+}
+__device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) {
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1); upk2(b, b0, b1);
+  return pk2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
+}
 
 // Front half of the ladders: range reduction (sin/cos(pi x) have period 2) and the MUFU sin / cos of four directions
 // held as two packed pairs (d0,d1 | d2,d3).  Split from the doubling recurrence so that the caller can issue the next
@@ -178,7 +179,7 @@ __device__ __forceinline__ void cos4_x2(uint64_t pj01, uint64_t pj23, uint64_t& 
   }
   c01 = pk2(c[0], c[1]); c23 = pk2(c[2], c[3]);
 }
-// sin(pi 2^k x), k = 0..5: angle doubling on packed pairs (FADD2 / FMUL2 / FFMA2), same recurrence as sin_ladder4
+// sin(pi 2^k x), k = 0..5: angle doubling on pairs, same recurrence as sin_ladder4
 __device__ __forceinline__ void sin_doubling4_x2(uint64_t s01, uint64_t s23, uint64_t c01, uint64_t c23, float (&s)[4][6]) {
   const uint64_t one = pk2(1.0f, 1.0f), neg = pk2(-1.0f, -1.0f);
   upk2(s01, s[0][0], s[1][0]); upk2(s23, s[2][0], s[3][0]);

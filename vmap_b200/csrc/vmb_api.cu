@@ -30,8 +30,8 @@ struct vmb_handle {
   float2* d_bc;           // AdamW bias corrections per step number for (bc_b1, bc_b2), built on the host in double precision
   double bc_b1, bc_b2;
   int img_halves;
-  bool umma_ok;           // hidden 32: fused tcgen05 kernel + its pre-swizzled fp16 image
-  bool lw_ok;             // hidden 64/128/256: layer-wise tcgen05 GEMM path + row-major fp16 image
+  bool umma_ok;           // hidden 32: fused wgmma kernel + its pre-arranged fp16 image
+  bool lw_ok;             // hidden 64/128/256: layer-wise wgmma GEMM path + row-major fp16 image
   lw::Workspace ws;       // training-step activations (may be baked into a captured graph)
   lw::Workspace ws_fwd;   // forward-only queries (vmb_forward): separate, so eval_points never moves the step's buffers
   std::string err;
@@ -82,7 +82,7 @@ static int dispatch_fp32(vmb_handle* h, const StepParams& sp, cudaStream_t st) {
 
 extern "C" {
 
-const char* vmb_version(void) { return "vmap_b200 0.1 (sm_100a)"; }
+const char* vmb_version(void) { return "vmap_b200 0.1 (sm_90a)"; }
 
 int vmb_param_count(int hidden, int n_freq) {
   if (hidden <= 0 || n_freq < 4 || n_freq > VMB_MAX_FREQ) return VMB_E_ARG;
@@ -119,7 +119,7 @@ int vmb_create(vmb_handle** out, int device, int max_obj, int hidden, int n_freq
   CUDA_TRY(nullptr, cudaSetDevice(device));
   vmb_handle* h = new vmb_handle();
   h->device = device; h->max_obj = max_obj; h->H = hidden; h->nfreq = n_freq;
-  h->n_sm = 148;
+  h->n_sm = 132;
   cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, device);
   h->L = vmb_make_layout(hidden, n_freq);
   h->d_counts = nullptr; h->d_img_index = nullptr; h->d_ticket = nullptr; h->d_smax = nullptr; h->d_partials = nullptr; h->d_objdone = nullptr; h->d_bc = nullptr; h->bc_b1 = h->bc_b2 = -1.0; h->img_halves = 0; h->umma_ok = false; h->lw_ok = false;
@@ -204,14 +204,6 @@ static int fused_scratch(vmb_handle* h, cudaStream_t st) {
   if (e == cudaSuccess) e = cudaMemset(h->d_objdone, 0, sizeof(unsigned int) * (2 * (size_t)h->max_obj + 8));
   if (e != cudaSuccess) return fail(h, VMB_E_NOMEM, cudaGetErrorString(e));
   return VMB_OK;
-}
-
-// VMB_DETERMINISTIC=1: one point group per CTA walks the tiles, so every wgrad accumulator receives ONE in-order stream
-// of MMAs and the step is bitwise reproducible (default: two groups interleave their MMAs in arrival order -- still no
-// floating-point atomics, but the fp32 summation order of the two tile streams inside an SM varies from run to run)
-static bool deterministic_mode() {
-  const char* e = getenv("VMB_DETERMINISTIC");
-  return e && e[0] == '1';
 }
 
 // Device table of AdamW's bias corrections (1 - b1^t, sqrt(1 - b2^t)) for t < BC_N, computed in double precision like
@@ -316,7 +308,6 @@ int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
     memset(&fx, 0, sizeof(fx));
     fx.partials = h->d_partials; fx.obj_done = h->d_objdone; fx.counts_in = a->counts; fx.counts_pub = h->d_counts;
     fx.fuse_adam = a->fuse_adam ? 1 : 0;
-    fx.single_group = deterministic_mode() ? 1 : 0;
     if (a->fuse_adam) {
       fx.p = const_cast<float*>(a->params); fx.m = a->exp_avg; fx.v = a->exp_avg_sq;
       fx.image_out = (__half*)const_cast<void*>(a->image); fx.img_index = h->d_img_index; fx.img_halves = h->img_halves;
@@ -508,7 +499,7 @@ int vmb_ingest_frame(vmb_handle* h, const vmb_ingest_args* a, void* stream) {
   return VMB_OK;
 }
 
-// ---- bring-up / test hook for the generic tcgen05 GEMM of the layer-wise (wide model) path --------
+// ---- test hook for the generic wgmma GEMM of the layer-wise (wide model) path --------
 // a_mn / b_mn = 0: operand stored [M or N rows][ld] with K contiguous; 1: stored [K rows][ld] with M or N contiguous.
 // epi 0: out16 = relu(acc*scale + bias) (fp16);  epi 2: out32 (=|+=) acc*scale;  epi 3: atomicAdd(out32, acc*scale)
 int vmb_debug_gemm(int a_mn, int b_mn, int epi, int M, int N, int K1, int K2, const void* a1, long long a1_ld,
@@ -541,16 +532,5 @@ int vmb_debug_gemm(int a_mn, int b_mn, int epi, int M, int N, int K1, int K2, co
   if (e != cudaSuccess) return fail(nullptr, VMB_E_CUDA, std::string("vmb_debug_gemm: ") + cudaGetErrorString(e));
   return VMB_OK;
 }
-
-#ifdef VMB_TRACE
-// profiling builds only: copy the kernel's cycle trace to the host (4 x 256 clock64 stamps)
-int vmb_trace_read(long long* host_out) {
-  return cudaMemcpyFromSymbol(host_out, g_vmb_trace, sizeof(long long) * 4 * 256) == cudaSuccess ? 0 : -2;
-}
-int vmb_trace_clear(void) {
-  static long long z[4 * 256];
-  return cudaMemcpyToSymbol(g_vmb_trace, z, sizeof(z)) == cudaSuccess ? 0 : -2;
-}
-#endif
 
 }  // extern "C"

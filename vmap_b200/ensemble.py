@@ -266,7 +266,7 @@ class VmapEnsemble:
         ``vmb_forward`` with n_obj = 1, so meshing one object of a 160-object stack costs one object's work)
         -> alpha [N], colour [N,3].  ``chunk`` bounds the points per launch (the reference uses 100k chunks).
         ``impl="fp32"`` forces the CUDA-core kernel; otherwise hidden 32 runs the forward half of the fused
-        tcgen05 kernel and hidden 64/128/256 the layer-wise tcgen05 GEMMs, on the fp16 weight image."""
+        wgmma kernel and hidden 64/128/256 the layer-wise wgmma GEMMs, on the fp16 weight image."""
         if row is None:
             B, N, _ = points.shape
             assert B == self.n_obj
