@@ -261,6 +261,59 @@ typedef struct vmb_ingest_args {
 
 int vmb_ingest_frame(vmb_handle* h, const vmb_ingest_args* a, void* stream);
 
+/* ---- K5: meshing -----------------------------------------------------------------------------------
+ * Marching cubes on a dense fp32 volume.  Replaces skimage.measure.marching_cubes and the trimesh transforms of
+ * Trainer.meshing (trainer.py:53-64, vis.py:6-19).  Volume [nx][ny][nz] (z fastest, nx, ny, nz >= 2); a corner is
+ * inside when v > level; one vertex per crossed grid edge at a + t (b - a), t = (level - v_a) / (v_b - v_a), a the
+ * lower-index end; vertex normal = the negated central-difference gradient (one-sided at the border) interpolated
+ * along the edge, mapped by the inverse transpose of `affine` and normalised.  Triangles wind so that their
+ * right-hand normal points from inside to outside (after `affine`, when its determinant is positive).  Order:
+ * vertices by (grid-point linear index, edge axis x < y < z), faces by (cell linear index, case-table order).
+ * Two calls with ONE host sync between them:
+ *   vmb_mc_count  classifies the volume and writes the totals {vertices, faces} to totals[2];
+ *   vmb_mc_emit   writes vertices / normals / faces of the volume given to the last vmb_mc_count on this handle
+ *                 (same pointer and shape; VMB_E_ARG otherwise) into buffers sized from those totals.
+ * An empty result (no crossing) is a success with zero totals.                                          */
+typedef struct vmb_mc_args {
+  const float* volume;           /* [nx][ny][nz]                                                                 */
+  int nx, ny, nz;
+  float level;                   /* 0.5 in Trainer.meshing (vis.py:6)                                             */
+  float affine[12];              /* row-major 3x4 index -> world map (x_w = A[:, :3] x_i + A[:, 3]); host values   */
+  int* totals;                   /* count: out device int[2] = number of vertices, faces                          */
+  float* vertices;               /* emit: out [V][3]                                                              */
+  float* normals;                /* emit: optional out [V][3]                                                     */
+  int* faces;                    /* emit: out [F][3] vertex indices                                               */
+  long long max_vertices, max_faces;   /* emit: capacities of the buffers above (entries beyond are not written) */
+} vmb_mc_args;
+
+int vmb_mc_count(vmb_handle* h, const vmb_mc_args* a, void* stream);
+int vmb_mc_emit(vmb_handle* h, const vmb_mc_args* a, void* stream);
+
+/* Object-pixel unprojection.  Replaces the open3d point cloud of sceneObject.get_bound (vmap.py:270-286): every
+ * pixel of the object's first n_keyframes keyframes that belongs to the object and has depth > 0 becomes the world
+ * point t_wc . [(u-cx) z/fx, (v-cy) z/fy, z, 1] (u indexes W, v indexes H, as cameraInfo), compacted in
+ * (keyframe, u, v) order.  Per-object buffers: belongs = state byte rgbs[kf][u][v][3] == 1.  Shared keyframe store
+ * (store_depth != NULL): belongs = store_inst[kf_slot[kf]][u][v] == obj_id.  `count` always receives the number of
+ * selected pixels; `points` (optional) receives the first min(count, max_points) of them, so a caller that does
+ * not know the count calls once without `points`, syncs, and calls again.                                      */
+typedef struct vmb_unproject_args {
+  int width, height, n_keyframes;
+  float fx, fy, cx, cy;
+  const unsigned char* rgbs;     /* per-object: [KF][W][H][4] u8, state in byte 3                                 */
+  const float* depths;           /* per-object: [KF][W][H]                                                        */
+  const float* t_wc;             /* per-object: [KF][4][4]                                                        */
+  const float* store_depth;      /* store: [slots][W][H]                                                          */
+  const int* store_inst;         /* store: [slots][W][H]                                                          */
+  const float* store_t_wc;       /* store: [slots][4][4]                                                          */
+  const int* kf_slot;            /* store: [n_keyframes] slot of each keyframe                                    */
+  int obj_id;                    /* store: instance id of the object                                              */
+  int* count;                    /* out device int                                                                */
+  float* points;                 /* optional out [max_points][3]                                                  */
+  long long max_points;
+} vmb_unproject_args;
+
+int vmb_unproject(vmb_handle* h, const vmb_unproject_args* a, void* stream);
+
 /* ---- bring-up / test hook (not part of the reference-facing surface) --------------------------- */
 /* Generic wgmma GEMM of the layer-wise wide-model path: D[M][N] = A[M][K1+K2] * B[N][K]^T, fp16 in,
  * fp32 accumulate.  a_mn/b_mn = 0: operand stored [rows][ld] with K contiguous; 1: stored [K][ld] with

@@ -92,10 +92,29 @@ class IngestArgs(C.Structure):
     ]
 
 
+class McArgs(C.Structure):
+    _fields_ = [
+        ("volume", _vp), ("nx", C.c_int), ("ny", C.c_int), ("nz", C.c_int), ("level", C.c_float),
+        ("affine", C.c_float * 12), ("totals", _vp),
+        ("vertices", _vp), ("normals", _vp), ("faces", _vp), ("max_vertices", _ll), ("max_faces", _ll),
+    ]
+
+
+class UnprojectArgs(C.Structure):
+    _fields_ = [
+        ("width", C.c_int), ("height", C.c_int), ("n_keyframes", C.c_int),
+        ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
+        ("rgbs", _vp), ("depths", _vp), ("t_wc", _vp),
+        ("store_depth", _vp), ("store_inst", _vp), ("store_t_wc", _vp), ("kf_slot", _vp), ("obj_id", C.c_int),
+        ("count", _vp), ("points", _vp), ("max_points", _ll),
+    ]
+
+
 EXPORTS = (
     "vmb_version", "vmb_param_count", "vmb_param_stride", "vmb_param_offsets", "vmb_image_bytes",
     "vmb_create", "vmb_destroy", "vmb_last_error", "vmb_step", "vmb_mask_counts", "vmb_adam",
     "vmb_build_image", "vmb_forward", "vmb_sample", "vmb_ingest_frame", "vmb_debug_gemm",
+    "vmb_mc_count", "vmb_mc_emit", "vmb_unproject",
 )
 
 _lib = None
@@ -141,6 +160,9 @@ def lib():
         L.vmb_forward.argtypes = [_vp, C.POINTER(ForwardArgs), _vp]
         L.vmb_sample.argtypes = [_vp, C.POINTER(SampleArgs), _vp]
         L.vmb_ingest_frame.argtypes = [_vp, C.POINTER(IngestArgs), _vp]
+        L.vmb_mc_count.argtypes = [_vp, C.POINTER(McArgs), _vp]
+        L.vmb_mc_emit.argtypes = [_vp, C.POINTER(McArgs), _vp]
+        L.vmb_unproject.argtypes = [_vp, C.POINTER(UnprojectArgs), _vp]
         L.vmb_build_image.argtypes = [_vp, C.c_int, _vp, _vp, _vp]
         L.vmb_mask_counts.argtypes = [_vp, C.c_int, C.c_int, _vp, _ll, _vp, _ll, _vp, _vp]
         L.vmb_debug_gemm.argtypes = [C.c_int] * 7 + [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, C.c_int, _vp, C.c_int,

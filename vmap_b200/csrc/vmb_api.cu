@@ -16,6 +16,7 @@
 #include "k_step_fused.cuh"
 #include "k_gemm_umma.cuh"
 #include "k_layerwise.cuh"
+#include "k_mesh.cuh"
 
 struct vmb_handle {
   int device, max_obj, H, nfreq;
@@ -34,6 +35,7 @@ struct vmb_handle {
   bool lw_ok;             // hidden 64/128/256: layer-wise wgmma GEMM path + row-major fp16 image
   lw::Workspace ws;       // training-step activations (may be baked into a captured graph)
   lw::Workspace ws_fwd;   // forward-only queries (vmb_forward): separate, so eval_points never moves the step's buffers
+  mesh::Workspace ws_mesh;// marching cubes / unprojection scratch (grow-only)
   std::string err;
 };
 
@@ -161,6 +163,7 @@ void vmb_destroy(vmb_handle* h) {
   if (h->d_bc) cudaFree(h->d_bc);
   h->ws.release(); h->ws.destroy_streams();
   h->ws_fwd.release(); h->ws_fwd.destroy_streams();
+  h->ws_mesh.release();
   delete h;
 }
 
@@ -496,6 +499,106 @@ int vmb_ingest_frame(vmb_handle* h, const vmb_ingest_args* a, void* stream) {
     ing::k_ingest_write<<<4 * h->n_sm, 256, 0, st>>>(a->inst, a->rgb, a->depth, a->stats, a->max_id, n,
                                                      reinterpret_cast<uchar4*>(a->dst_rgbx), a->dst_depth, a->dst_inst);
   CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
+// ---- K5: meshing (marching cubes, object-pixel unprojection) ---------------------------------------
+static int mc_params(vmb_handle* h, const vmb_mc_args* a, mesh::McParams& q, const char* who) {
+  if (!h || !a || !a->volume || a->nx < 2 || a->ny < 2 || a->nz < 2)
+    return fail(h, VMB_E_ARG, std::string(who) + ": need a volume with nx, ny, nz >= 2");
+  memset(&q, 0, sizeof(q));
+  q.vol = a->volume; q.nx = a->nx; q.ny = a->ny; q.nz = a->nz; q.level = a->level;
+  q.n = (long long)a->nx * a->ny * a->nz;
+  if (3 * q.n >= 0x7fffffffLL || (long long)VMB_MC_MAX_TRI * q.n >= 0x7fffffffLL)
+    return fail(h, VMB_E_ARG, std::string(who) + ": volume too large for int32 vertex / face indices");
+  double A[9], det;
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) { A[3 * r + c] = a->affine[4 * r + c]; q.M[3 * r + c] = a->affine[4 * r + c]; }
+    q.o[r] = a->affine[4 * r + 3];
+  }
+  det = A[0] * (A[4] * A[8] - A[5] * A[7]) - A[1] * (A[3] * A[8] - A[5] * A[6]) + A[2] * (A[3] * A[7] - A[4] * A[6]);
+  if (!(std::fabs(det) > 0.0) || !std::isfinite(det)) return fail(h, VMB_E_ARG, std::string(who) + ": singular affine");
+  // M^-T = cofactor(M) / det
+  const double C[9] = {A[4] * A[8] - A[5] * A[7], A[5] * A[6] - A[3] * A[8], A[3] * A[7] - A[4] * A[6],
+                       A[2] * A[7] - A[1] * A[8], A[0] * A[8] - A[2] * A[6], A[1] * A[6] - A[0] * A[7],
+                       A[1] * A[5] - A[2] * A[4], A[2] * A[3] - A[0] * A[5], A[0] * A[4] - A[1] * A[3]};
+  for (int i = 0; i < 9; ++i) q.Nt[i] = (float)(C[i] / det);
+  return VMB_OK;
+}
+
+int vmb_mc_count(vmb_handle* h, const vmb_mc_args* a, void* stream) {
+  mesh::McParams q;
+  const int rc = mc_params(h, a, q, "vmb_mc_count");
+  if (rc != VMB_OK) return rc;
+  if (!a->totals) return fail(h, VMB_E_ARG, "vmb_mc_count: totals is NULL");
+  cudaStream_t st = (cudaStream_t)stream;
+  mesh::Workspace& w = h->ws_mesh;
+  const size_t n1 = (size_t)q.n + 1;
+  CUDA_TRY(h, mesh::Workspace::grow((void**)&w.mc_bytes, &w.mc_cap, 2 * n1 * sizeof(int) + 2 * (size_t)q.n));
+  q.pt_scan = reinterpret_cast<int*>(w.mc_bytes);
+  q.cell_scan = q.pt_scan + n1;
+  q.pt_mask = reinterpret_cast<unsigned char*>(q.cell_scan + n1);
+  q.cell_case = q.pt_mask + q.n;
+  mesh::k_mc_count<<<mesh::blocks_for((long long)n1), 256, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  CUDA_TRY(h, w.scan(q.pt_scan, (long long)n1, st));
+  CUDA_TRY(h, w.scan(q.cell_scan, (long long)n1, st));
+  mesh::k_mc_totals<<<1, 1, 0, st>>>(q.pt_scan, q.cell_scan, q.n, a->totals);
+  CUDA_TRY(h, cudaGetLastError());
+  w.last = q;
+  w.counted = true;
+  return VMB_OK;
+}
+
+int vmb_mc_emit(vmb_handle* h, const vmb_mc_args* a, void* stream) {
+  mesh::McParams q;
+  const int rc = mc_params(h, a, q, "vmb_mc_emit");
+  if (rc != VMB_OK) return rc;
+  const mesh::McParams& c = h->ws_mesh.last;
+  if (!h->ws_mesh.counted || c.vol != q.vol || c.nx != q.nx || c.ny != q.ny || c.nz != q.nz || c.level != q.level)
+    return fail(h, VMB_E_ARG, "vmb_mc_emit: no matching vmb_mc_count on this handle (same volume, shape and level)");
+  if ((a->max_vertices > 0 && !a->vertices) || (a->max_faces > 0 && !a->faces) || a->max_vertices < 0 || a->max_faces < 0)
+    return fail(h, VMB_E_ARG, "vmb_mc_emit: output buffers missing for the given capacities");
+  q.pt_scan = c.pt_scan; q.cell_scan = c.cell_scan; q.pt_mask = c.pt_mask; q.cell_case = c.cell_case;
+  q.verts = a->vertices; q.normals = a->normals; q.faces = a->faces;
+  q.max_verts = a->max_vertices; q.max_faces = a->max_faces;
+  mesh::k_mc_emit<<<mesh::blocks_for(q.n), 256, 0, (cudaStream_t)stream>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
+int vmb_unproject(vmb_handle* h, const vmb_unproject_args* a, void* stream) {
+  if (!h || !a || !a->count || a->width <= 0 || a->height <= 0 || a->n_keyframes < 0 || !(a->fx != 0.f) || !(a->fy != 0.f))
+    return fail(h, VMB_E_ARG, "vmb_unproject: bad arguments");
+  const bool store = a->store_depth != nullptr;
+  if (store && (!a->store_inst || !a->store_t_wc || (a->n_keyframes > 0 && !a->kf_slot)))
+    return fail(h, VMB_E_ARG, "vmb_unproject: shared keyframe store needs store_inst, store_t_wc and kf_slot");
+  if (!store && (!a->rgbs || !a->depths || !a->t_wc))
+    return fail(h, VMB_E_ARG, "vmb_unproject: per-object mode needs rgbs, depths and t_wc");
+  if (a->max_points < 0 || (a->max_points > 0 && !a->points))
+    return fail(h, VMB_E_ARG, "vmb_unproject: points missing for the given capacity");
+  mesh::UnprojParams q;
+  memset(&q, 0, sizeof(q));
+  q.W = a->width; q.H = a->height; q.n_kf = a->n_keyframes;
+  q.n = (long long)a->n_keyframes * a->width * a->height;
+  if (q.n + 1 >= 0x7fffffffLL) return fail(h, VMB_E_ARG, "vmb_unproject: too many pixels for int32 indices");
+  q.fx = a->fx; q.fy = a->fy; q.cx = a->cx; q.cy = a->cy;
+  q.rgbs = reinterpret_cast<const uchar4*>(a->rgbs); q.depths = a->depths; q.t_wc = a->t_wc;
+  q.st_depth = a->store_depth; q.st_inst = a->store_inst; q.st_twc = a->store_t_wc; q.kf_slot = a->kf_slot;
+  q.obj_id = a->obj_id;
+  q.out = a->points; q.max_points = a->points ? a->max_points : 0;
+  mesh::Workspace& w = h->ws_mesh;
+  cudaStream_t st = (cudaStream_t)stream;
+  CUDA_TRY(h, mesh::Workspace::grow((void**)&w.up_scan, &w.up_cap, (size_t)(q.n + 1) * sizeof(int)));
+  q.scan = w.up_scan;
+  mesh::k_unproj_flag<<<mesh::blocks_for(q.n + 1), 256, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  CUDA_TRY(h, w.scan(q.scan, q.n + 1, st));
+  CUDA_TRY(h, cudaMemcpyAsync(a->count, q.scan + q.n, sizeof(int), cudaMemcpyDeviceToDevice, st));
+  if (q.max_points > 0 && q.n > 0) {
+    mesh::k_unproj_emit<<<mesh::blocks_for(q.n), 256, 0, st>>>(q);
+    CUDA_TRY(h, cudaGetLastError());
+  }
   return VMB_OK;
 }
 

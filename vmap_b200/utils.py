@@ -1,11 +1,31 @@
-"""utils.update_vmap with the reference's signature (utils.py:30-34) and the ``vmap`` shim
-that replaces ``functorch.vmap`` at train.py:293-294."""
+"""utils.update_vmap with the reference's signature (utils.py:30-34), the ``vmap`` shim
+that replaces ``functorch.vmap`` at train.py:293-294, and the picklable ``BoundingBox`` that
+sceneObject.get_bound stores in checkpoints (utils.py:11-24)."""
 from __future__ import annotations
 
 import torch
 
 from .layout import FC_KEYS, PE_KEY
 from .lazy import LazyEmbedding, LazyHeads, bind_modules
+
+
+class BoundingBox:
+    """Oriented 3-D box (utils.py:11-18): ``center`` [3], ``R`` [3,3] (box axes as columns), ``extent`` [3]."""
+
+    def __init__(self):
+        self.extent = None
+        self.R = None
+        self.center = None
+        self.points3d = None    # (8,3)
+
+
+def bbox_open3d2bbox(bbox_o3d):
+    """utils.py:20-25: anything with .extent / .R / .center -> BoundingBox."""
+    bbox = BoundingBox()
+    bbox.extent = bbox_o3d.extent
+    bbox.R = bbox_o3d.R
+    bbox.center = bbox_o3d.center
+    return bbox
 
 
 class _Stack:

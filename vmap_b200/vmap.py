@@ -14,6 +14,7 @@ import random
 from time import perf_counter_ns
 from typing import Dict, List, Optional
 
+import numpy as np
 import torch
 
 from . import trainer as trainer_mod
@@ -240,7 +241,34 @@ class sceneObject:
                 o["z"][0].view(n_frames, n_samples, S))
 
     def get_bound(self, intrinsic_open3d):
-        raise NotImplementedError("3-D bounds use open3d/trimesh on the CPU (vmap.py:270-315): out of the hot path")
+        """Oriented 3-D bound of the object (vmap.py:270-315).  The object's pixels of its first ``n_keyframes``
+        keyframes with depth > 0 are unprojected on the GPU (K5); the minimum-volume box of their convex hull is fitted
+        on the host (mesh.oriented_bounds), extents clamped to >= 0.10.  Stores a picklable utils.BoundingBox in
+        ``self.bbox3d`` (it goes into checkpoints) and returns an open3d OrientedBoundingBox when open3d is installed
+        (train.py:367 adds it to the viewer), the BoundingBox otherwise; None when the points are too few or flat.
+        ``intrinsic_open3d``: an open3d PinholeCameraIntrinsic or a 3x3 matrix."""
+        from scipy.spatial import QhullError
+        from . import mesh, utils
+        pts = mesh.unproject_object(self, mesh.intrinsic_matrix(intrinsic_open3d)).cpu().numpy()
+        try:
+            center, R, extents = mesh.oriented_bounds(pts)
+        except (QhullError, ValueError):
+            print("too few pcs obj ")
+            return None
+        extents = np.maximum(extents, 0.10)                  # at least rendering 10cm (vmap.py:298-299, 306-307)
+        bbox = utils.BoundingBox()
+        bbox.center, bbox.R, bbox.extent = center, R, extents
+        self.bbox3d = bbox
+        print("obj ", self.obj_id)
+        print("bound ", f"center {center}, extent {extents}")
+        print("kf id dict ", self.kf_id_dict)
+        try:
+            import open3d
+        except ImportError:
+            return bbox
+        bbox3d = open3d.geometry.OrientedBoundingBox(center, R, extents)
+        bbox3d.color = (255, 0, 0)
+        return bbox3d
 
     def save_checkpoints(self, path, epoch):
         """Same file layout and keys as vmap.py:461-476."""
