@@ -314,6 +314,67 @@ typedef struct vmb_unproject_args {
 
 int vmb_unproject(vmb_handle* h, const vmb_unproject_args* a, void* stream);
 
+/* ---- K6: 3-D reconstruction metrics ----------------------------------------------------------------
+ * The arithmetic under metric/eval_3D_obj.py and eval_3D_scene.py: box crop, area-weighted surface sampling and exact
+ * nearest-neighbour distances.  Means and ratios over the distances are left to the caller.
+ *
+ * Box crop (trimesh slice_plane with the six faces of an oriented box): each face of an indexed mesh is clipped
+ * against the box's half-spaces (Sutherland-Hodgman in fp64, fp32 out, at most 9 vertices) and fan-triangulated from the first
+ * clipped vertex.  Output: a triangle soup [T][3][3] ordered by (input face, fan order).  Faces wholly inside are
+ * copied unchanged, faces wholly outside (or with an index outside [0, n_vertices)) give nothing.
+ * Two calls with ONE host sync between them, as marching cubes:
+ *   vmb_clip_count  writes T to *count (device int);
+ *   vmb_clip_emit   writes the soup of the mesh and box given to the last vmb_clip_count on this handle (same
+ *                   pointers, sizes and box; VMB_E_ARG otherwise) into a buffer sized from T.                 */
+typedef struct vmb_clip_args {
+  const float* vertices;         /* [V][3]                                                                       */
+  long long n_vertices;
+  const int* faces;              /* [F][3]                                                                       */
+  long long n_faces;
+  float center[3];               /* box center                                                                   */
+  float rotation[9];             /* row-major 3x3 with the box axes as columns                                   */
+  float extent[3];               /* full edge lengths along the three axes                                       */
+  int* count;                    /* count: out device int = T                                                    */
+  float* triangles;              /* emit: out [max_triangles][3][3]                                              */
+  long long max_triangles;
+} vmb_clip_args;
+
+int vmb_clip_count(vmb_handle* h, const vmb_clip_args* a, void* stream);
+int vmb_clip_emit(vmb_handle* h, const vmb_clip_args* a, void* stream);
+
+/* Surface sampling (trimesh.sample.sample_surface): face areas 0.5 |e1 x e2| and their inclusive prefix in fp64; per
+ * point face = searchsorted(prefix, u0 * total, side='left'), r = (u1, u2), r = |r - 1| when u1 + u2 > 1,
+ * p = v0 + (r1 (v1 - v0) + r2 (v2 - v0)).  Randoms: Philox4x32-10 keyed by (seed, point index), or `uniforms`.
+ * Syncs the stream once (to check the total area): a mesh of total area 0, or a face index outside [0, V), is
+ * VMB_E_ARG.  n_points == 0 is a no-op.                                                                     */
+typedef struct vmb_surface_sample_args {
+  const float* vertices;         /* [V][3]                                                                       */
+  long long n_vertices;
+  const int* faces;              /* [F][3]                                                                       */
+  long long n_faces;
+  long long n_points;
+  unsigned long long seed;
+  const double* uniforms;        /* optional [n_points][3] (u0, u1, u2) in [0, 1): replaces Philox               */
+  float* points;                 /* out [n_points][3]                                                            */
+  int* face_index;               /* optional out [n_points]                                                      */
+} vmb_surface_sample_args;
+
+int vmb_surface_sample(vmb_handle* h, const vmb_surface_sample_args* a, void* stream);
+
+/* Exact nearest neighbour: dist[i] = min_j |query_i - ref_j| (fp32 coordinates), index[i] = that j, ties to the lowest
+ * j.  Uniform grid over ref's bounding box in handle scratch, shell search per query; no host sync.
+ * n_ref == 0 is VMB_E_ARG; n_query == 0 is a no-op.                                                       */
+typedef struct vmb_nn_args {
+  const float* ref;              /* [n_ref][3]                                                                   */
+  long long n_ref;
+  const float* query;            /* [n_query][3]                                                                 */
+  long long n_query;
+  float* dist;                   /* out [n_query]                                                                */
+  int* index;                    /* optional out [n_query]                                                       */
+} vmb_nn_args;
+
+int vmb_nn_dist(vmb_handle* h, const vmb_nn_args* a, void* stream);
+
 /* ---- bring-up / test hook (not part of the reference-facing surface) --------------------------- */
 /* Generic wgmma GEMM of the layer-wise wide-model path: D[M][N] = A[M][K1+K2] * B[N][K]^T, fp16 in,
  * fp32 accumulate.  a_mn/b_mn = 0: operand stored [rows][ld] with K contiguous; 1: stored [K][ld] with

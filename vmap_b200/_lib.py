@@ -110,11 +110,33 @@ class UnprojectArgs(C.Structure):
     ]
 
 
+class ClipArgs(C.Structure):
+    _fields_ = [
+        ("vertices", _vp), ("n_vertices", _ll), ("faces", _vp), ("n_faces", _ll),
+        ("center", C.c_float * 3), ("rotation", C.c_float * 9), ("extent", C.c_float * 3),
+        ("count", _vp), ("triangles", _vp), ("max_triangles", _ll),
+    ]
+
+
+class SurfaceSampleArgs(C.Structure):
+    _fields_ = [
+        ("vertices", _vp), ("n_vertices", _ll), ("faces", _vp), ("n_faces", _ll),
+        ("n_points", _ll), ("seed", C.c_ulonglong), ("uniforms", _vp), ("points", _vp), ("face_index", _vp),
+    ]
+
+
+class NnArgs(C.Structure):
+    _fields_ = [
+        ("ref", _vp), ("n_ref", _ll), ("query", _vp), ("n_query", _ll), ("dist", _vp), ("index", _vp),
+    ]
+
+
 EXPORTS = (
     "vmb_version", "vmb_param_count", "vmb_param_stride", "vmb_param_offsets", "vmb_image_bytes",
     "vmb_create", "vmb_destroy", "vmb_last_error", "vmb_step", "vmb_mask_counts", "vmb_adam",
     "vmb_build_image", "vmb_forward", "vmb_sample", "vmb_ingest_frame", "vmb_debug_gemm",
     "vmb_mc_count", "vmb_mc_emit", "vmb_unproject",
+    "vmb_clip_count", "vmb_clip_emit", "vmb_surface_sample", "vmb_nn_dist",
 )
 
 _lib = None
@@ -163,6 +185,10 @@ def lib():
         L.vmb_mc_count.argtypes = [_vp, C.POINTER(McArgs), _vp]
         L.vmb_mc_emit.argtypes = [_vp, C.POINTER(McArgs), _vp]
         L.vmb_unproject.argtypes = [_vp, C.POINTER(UnprojectArgs), _vp]
+        L.vmb_clip_count.argtypes = [_vp, C.POINTER(ClipArgs), _vp]
+        L.vmb_clip_emit.argtypes = [_vp, C.POINTER(ClipArgs), _vp]
+        L.vmb_surface_sample.argtypes = [_vp, C.POINTER(SurfaceSampleArgs), _vp]
+        L.vmb_nn_dist.argtypes = [_vp, C.POINTER(NnArgs), _vp]
         L.vmb_build_image.argtypes = [_vp, C.c_int, _vp, _vp, _vp]
         L.vmb_mask_counts.argtypes = [_vp, C.c_int, C.c_int, _vp, _ll, _vp, _ll, _vp, _vp]
         L.vmb_debug_gemm.argtypes = [C.c_int] * 7 + [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, C.c_int, _vp, C.c_int,

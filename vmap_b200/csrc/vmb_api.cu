@@ -17,6 +17,7 @@
 #include "k_gemm_umma.cuh"
 #include "k_layerwise.cuh"
 #include "k_mesh.cuh"
+#include "k_eval.cuh"
 
 struct vmb_handle {
   int device, max_obj, H, nfreq;
@@ -36,6 +37,7 @@ struct vmb_handle {
   lw::Workspace ws;       // training-step activations (may be baked into a captured graph)
   lw::Workspace ws_fwd;   // forward-only queries (vmb_forward): separate, so eval_points never moves the step's buffers
   mesh::Workspace ws_mesh;// marching cubes / unprojection scratch (grow-only)
+  eval3d::Workspace ws_eval;// box crop / surface sampling / nearest-neighbour scratch (grow-only)
   std::string err;
 };
 
@@ -164,6 +166,7 @@ void vmb_destroy(vmb_handle* h) {
   h->ws.release(); h->ws.destroy_streams();
   h->ws_fwd.release(); h->ws_fwd.destroy_streams();
   h->ws_mesh.release();
+  h->ws_eval.release();
   delete h;
 }
 
@@ -599,6 +602,129 @@ int vmb_unproject(vmb_handle* h, const vmb_unproject_args* a, void* stream) {
     mesh::k_unproj_emit<<<mesh::blocks_for(q.n), 256, 0, st>>>(q);
     CUDA_TRY(h, cudaGetLastError());
   }
+  return VMB_OK;
+}
+
+// ---- K6: 3-D reconstruction metrics (box crop, surface sampling, nearest neighbour) ---------------
+static int clip_params(vmb_handle* h, const vmb_clip_args* a, eval3d::ClipParams& q, const char* who) {
+  if (!h || !a || !a->vertices || !a->faces || a->n_vertices <= 0 || a->n_faces <= 0)
+    return fail(h, VMB_E_ARG, std::string(who) + ": need a mesh with n_vertices, n_faces >= 1");
+  if (a->n_vertices > 0x7fffffffLL || 7 * a->n_faces + 1 >= 0x7fffffffLL)
+    return fail(h, VMB_E_ARG, std::string(who) + ": mesh too large for int32 indices");
+  memset(&q, 0, sizeof(q));
+  q.v = a->vertices; q.nv = a->n_vertices; q.f = a->faces; q.nf = a->n_faces;
+  for (int j = 0; j < 3; ++j) {
+    if (!(a->extent[j] >= 0.f)) return fail(h, VMB_E_ARG, std::string(who) + ": box extents must be >= 0");
+    q.c[j] = a->center[j];
+    q.half[j] = 0.5f * a->extent[j];
+    for (int r = 0; r < 3; ++r) q.ax[j][r] = a->rotation[3 * r + j];
+  }
+  return VMB_OK;
+}
+
+int vmb_clip_count(vmb_handle* h, const vmb_clip_args* a, void* stream) {
+  eval3d::ClipParams q;
+  const int rc = clip_params(h, a, q, "vmb_clip_count");
+  if (rc != VMB_OK) return rc;
+  if (!a->count) return fail(h, VMB_E_ARG, "vmb_clip_count: count is NULL");
+  cudaStream_t st = (cudaStream_t)stream;
+  eval3d::Workspace& w = h->ws_eval;
+  CUDA_TRY(h, eval3d::Workspace::grow((void**)&w.clip_scan, &w.clip_cap, (size_t)(q.nf + 1) * sizeof(int)));
+  q.scan = w.clip_scan;
+  eval3d::k_clip_count<<<eval3d::blocks_for(q.nf + 1, 128), 128, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  CUDA_TRY(h, w.exclusive_sum(q.scan, q.nf + 1, st));
+  CUDA_TRY(h, cudaMemcpyAsync(a->count, q.scan + q.nf, sizeof(int), cudaMemcpyDeviceToDevice, st));
+  w.last = q;
+  w.counted = true;
+  return VMB_OK;
+}
+
+int vmb_clip_emit(vmb_handle* h, const vmb_clip_args* a, void* stream) {
+  eval3d::ClipParams q;
+  const int rc = clip_params(h, a, q, "vmb_clip_emit");
+  if (rc != VMB_OK) return rc;
+  const eval3d::ClipParams& c = h->ws_eval.last;
+  if (!h->ws_eval.counted || c.v != q.v || c.nv != q.nv || c.f != q.f || c.nf != q.nf ||
+      memcmp(c.c, q.c, sizeof(q.c)) || memcmp(c.ax, q.ax, sizeof(q.ax)) || memcmp(c.half, q.half, sizeof(q.half)))
+    return fail(h, VMB_E_ARG, "vmb_clip_emit: no matching vmb_clip_count on this handle (same mesh and box)");
+  if (a->max_triangles < 0 || (a->max_triangles > 0 && !a->triangles))
+    return fail(h, VMB_E_ARG, "vmb_clip_emit: triangles missing for the given capacity");
+  q.scan = c.scan; q.out = a->triangles; q.max_tri = a->max_triangles;
+  eval3d::k_clip_emit<<<eval3d::blocks_for(q.nf, 128), 128, 0, (cudaStream_t)stream>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
+int vmb_surface_sample(vmb_handle* h, const vmb_surface_sample_args* a, void* stream) {
+  if (!h || !a || !a->vertices || !a->faces || a->n_vertices <= 0 || a->n_faces <= 0 || a->n_points < 0)
+    return fail(h, VMB_E_ARG, "vmb_surface_sample: need a mesh with n_vertices, n_faces >= 1 and n_points >= 0");
+  if (a->n_vertices > 0x7fffffffLL || a->n_faces >= 0x7fffffffLL)
+    return fail(h, VMB_E_ARG, "vmb_surface_sample: mesh too large for int32 indices");
+  if (a->n_points > 0 && !a->points) return fail(h, VMB_E_ARG, "vmb_surface_sample: points is NULL");
+  if (a->n_points == 0) return VMB_OK;
+  eval3d::SampleSurfParams q;
+  memset(&q, 0, sizeof(q));
+  q.v = a->vertices; q.nv = a->n_vertices; q.f = a->faces; q.nf = a->n_faces;
+  q.n = a->n_points; q.seed = a->seed; q.uniforms = a->uniforms; q.points = a->points; q.face_index = a->face_index;
+  cudaStream_t st = (cudaStream_t)stream;
+  eval3d::Workspace& w = h->ws_eval;
+  CUDA_TRY(h, eval3d::Workspace::grow((void**)&w.cum, &w.cum_cap, (size_t)q.nf * sizeof(double) + sizeof(double)));
+  q.cum = w.cum;
+  q.bad = reinterpret_cast<int*>(w.cum + q.nf);
+  CUDA_TRY(h, cudaMemsetAsync(q.bad, 0, sizeof(int), st));
+  eval3d::k_face_area<<<eval3d::blocks_for(q.nf, 256), 256, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  CUDA_TRY(h, w.inclusive_sum(q.cum, q.nf, st));
+  double total = 0.0;
+  int bad = 0;
+  CUDA_TRY(h, cudaMemcpyAsync(&total, q.cum + q.nf - 1, sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(h, cudaMemcpyAsync(&bad, q.bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(h, cudaStreamSynchronize(st));
+  if (bad) return fail(h, VMB_E_ARG, "vmb_surface_sample: a face index is outside [0, n_vertices)");
+  if (!(total > 0.0) || !std::isfinite(total))
+    return fail(h, VMB_E_ARG, "vmb_surface_sample: the mesh has no (finite) area");
+  eval3d::k_sample_surface<<<eval3d::blocks_for(q.n, 256), 256, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
+int vmb_nn_dist(vmb_handle* h, const vmb_nn_args* a, void* stream) {
+  if (!h || !a || !a->ref || a->n_ref <= 0 || a->n_query < 0)
+    return fail(h, VMB_E_ARG, "vmb_nn_dist: need n_ref >= 1 ref points and n_query >= 0");
+  if (a->n_ref >= 0x7fffffffLL) return fail(h, VMB_E_ARG, "vmb_nn_dist: too many ref points for int32 indices");
+  if (a->n_query > 0 && (!a->query || !a->dist)) return fail(h, VMB_E_ARG, "vmb_nn_dist: query / dist is NULL");
+  if (a->n_query == 0) return VMB_OK;
+  eval3d::NnParams q;
+  memset(&q, 0, sizeof(q));
+  q.ref = a->ref; q.n_ref = a->n_ref; q.query = a->query; q.n_q = a->n_query; q.dist = a->dist; q.index = a->index;
+  q.max_cells = std::min<long long>(std::max<long long>(a->n_ref, 1), eval3d::EVAL_MAX_CELLS);
+  // scratch: keys[6] (padded to 32 B) | Grid (padded to 64 B) | cell_start[max_cells+1] | pt_cell | pt_rank | sorted
+  const size_t off_grid = 32, off_cells = 96;
+  const size_t off_cell_pt = (off_cells + (size_t)(q.max_cells + 1) * sizeof(int) + 15) & ~(size_t)15;
+  const size_t off_rank = off_cell_pt + (size_t)q.n_ref * sizeof(int);
+  const size_t off_sorted = (off_rank + (size_t)q.n_ref * sizeof(int) + 15) & ~(size_t)15;
+  const size_t need = off_sorted + (size_t)q.n_ref * sizeof(float4);
+  eval3d::Workspace& w = h->ws_eval;
+  cudaStream_t st = (cudaStream_t)stream;
+  CUDA_TRY(h, eval3d::Workspace::grow((void**)&w.nn, &w.nn_cap, need));
+  q.keys = reinterpret_cast<unsigned int*>(w.nn);
+  q.grid = reinterpret_cast<eval3d::Grid*>(w.nn + off_grid);
+  q.cell_start = reinterpret_cast<int*>(w.nn + off_cells);
+  q.pt_cell = reinterpret_cast<int*>(w.nn + off_cell_pt);
+  q.pt_rank = reinterpret_cast<int*>(w.nn + off_rank);
+  q.sorted = reinterpret_cast<float4*>(w.nn + off_sorted);
+  CUDA_TRY(h, cudaMemsetAsync(q.keys, 0xff, 3 * sizeof(unsigned int), st));
+  CUDA_TRY(h, cudaMemsetAsync(q.keys + 3, 0, 3 * sizeof(unsigned int), st));
+  CUDA_TRY(h, cudaMemsetAsync(q.cell_start, 0, (size_t)(q.max_cells + 1) * sizeof(int), st));
+  eval3d::k_nn_bbox<<<eval3d::blocks_for(q.n_ref, 256), 256, 0, st>>>(q);
+  eval3d::k_nn_grid<<<1, 1, 0, st>>>(q);
+  eval3d::k_nn_count<<<eval3d::blocks_for(q.n_ref, 256), 256, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  CUDA_TRY(h, w.exclusive_sum(q.cell_start, q.max_cells + 1, st));
+  eval3d::k_nn_scatter<<<eval3d::blocks_for(q.n_ref, 256), 256, 0, st>>>(q);
+  eval3d::k_nn_query<<<eval3d::blocks_for(q.n_q, 128), 128, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
   return VMB_OK;
 }
 
