@@ -375,6 +375,62 @@ typedef struct vmb_nn_args {
 
 int vmb_nn_dist(vmb_handle* h, const vmb_nn_args* a, void* stream);
 
+/* ---- K7: ScanNet instance association --------------------------------------------------------------
+ * utils.box_filter (utils.py:112-208) and the per-label 2-D boxes of dataset.py:263-283 for one frame, in three calls
+ * on one handle, in this order, with the same args (images, max_id, tracks):
+ *   vmb_assoc_classify  per id: pixel count, class minimum (background when bg_class[min] is set), valid-depth points,
+ *                       eroded pixels (a pixel survives iff every in-image pixel within Chebyshev distance 6 has its
+ *                       id: cv2.erode(ones(5,5), iterations=3)), eroded points and, for tracked ids, points inside the
+ *                       tracked box (inclusive open3d test); then box_filter's branch in stats[id][6]
+ *                       (VMB_ASSOC_*).  Points are x = (u-cx) z/fx, y = (v-cy) z/fy, camera_pose . [x y z 1] in fp64
+ *                       with no FMA contraction.  No sync.
+ *   vmb_assoc_voxel     for every MERGE / NEW id: its previous cloud (pool, merged ids only) followed by the selected
+ *                       points in row-major (v, u) order, voxel-downsampled in fp64 (min_bound = min - voxel / 2,
+ *                       key = floor((p - min_bound) / voxel), mean summed in input order), emitted into cloud_out in
+ *                       ascending (id, kx, ky, kz) order; stats[id][7] = the id's output count.  Syncs the stream
+ *                       ONCE: a voxel key outside [0, 65536) is VMB_E_ARG.
+ *   vmb_assoc_finalize  labels from final_label (VMB_ASSOC_FINAL_*; an id labelled after a merge gets -1 on its
+ *                       valid-depth pixels outside the box), per-label pixel boxes for labels -1 .. max_id-1, enlarged
+ *                       as enlarge_bbox on python ints (margin = int((0.5 * bbox_scale) * extent) in fp64, clipped to
+ *                       W-1 / H-1); a label whose margin is 0 is relabelled 0.  No sync.                             */
+enum { VMB_ASSOC_ZERO = 0, VMB_ASSOC_MERGE = 1, VMB_ASSOC_NEW = 2, VMB_ASSOC_NEG = 3 };
+enum { VMB_ASSOC_FINAL_ZERO = 0, VMB_ASSOC_FINAL_ID = 1, VMB_ASSOC_FINAL_NEG = 2 };
+
+typedef struct vmb_assoc_args {
+  int width, height;
+  const int* inst;               /* [W][H] id per pixel (instance + 1, dataset.py:247); ids outside [1, max_id) are ignored */
+  const int* cls;                /* optional [W][H] semantic class                                               */
+  const float* depth;            /* [W][H] metres, <= 0 = no point                                               */
+  int max_id;                    /* 1 .. 65536                                                                   */
+  const unsigned char* bg_class; /* optional [n_class]: 1 = background class (dataset.py:187)                    */
+  int n_class;
+  double fx, fy, cx, cy;
+  double camera_pose[16];        /* row-major 4x4 camera -> world; host values                                   */
+  int min_pixels;                /* new ids need this many eroded pixels (dataset.py:184 uses 1500)              */
+  double voxel_size;             /* 0.01 (utils.py:112)                                                          */
+  double bbox_scale;             /* 0.2 (dataset.py:188)                                                         */
+  const double* boxes;           /* [max_id][16]: tracked flag, center[3], R[:,j] * extent[j] / 2 for j = 0..2,
+                                    then the three squared half-axis lengths                                     */
+  const double* pool;            /* [n_pool][3] previous clouds                                                  */
+  const int* cloud_off;          /* [max_id] first pool row of each id's cloud                                   */
+  const int* cloud_cnt;          /* [max_id] rows of each id's cloud (0 = none)                                  */
+  long long n_pool;
+  int* stats;                    /* out [max_id][8]: pixels, class min, points, eroded pixels, eroded points,
+                                    inside points, branch (VMB_ASSOC_*), voxelised points                        */
+  double* cloud_out;             /* voxel: out [max_cloud_out][3], max_cloud_out >= n_pool + W * H               */
+  long long max_cloud_out;
+  const int* final_label;        /* finalize: [max_id] VMB_ASSOC_FINAL_*                                          */
+  long long* labels;             /* finalize: out [W][H]                                                         */
+  long long* bbox;               /* finalize: out [max_id + 1][5] per label + 1: kept, u_lo, u_hi, v_lo, v_hi;
+                                    row 1 (label 0) is always the full frame [0, W, 0, H]                         */
+  int relabel;                   /* finalize: 1 = relabel labels whose box is None to 0 (dataset.py:269-270);
+                                    0 = leave box_filter's labels as they are                                    */
+} vmb_assoc_args;
+
+int vmb_assoc_classify(vmb_handle* h, const vmb_assoc_args* a, void* stream);
+int vmb_assoc_voxel(vmb_handle* h, const vmb_assoc_args* a, void* stream);
+int vmb_assoc_finalize(vmb_handle* h, const vmb_assoc_args* a, void* stream);
+
 /* ---- bring-up / test hook (not part of the reference-facing surface) --------------------------- */
 /* Generic wgmma GEMM of the layer-wise wide-model path: D[M][N] = A[M][K1+K2] * B[N][K]^T, fp16 in,
  * fp32 accumulate.  a_mn/b_mn = 0: operand stored [rows][ld] with K contiguous; 1: stored [K][ld] with

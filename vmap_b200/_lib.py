@@ -131,12 +131,25 @@ class NnArgs(C.Structure):
     ]
 
 
+class AssocArgs(C.Structure):
+    _fields_ = [
+        ("width", C.c_int), ("height", C.c_int), ("inst", _vp), ("cls", _vp), ("depth", _vp), ("max_id", C.c_int),
+        ("bg_class", _vp), ("n_class", C.c_int),
+        ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
+        ("camera_pose", C.c_double * 16), ("min_pixels", C.c_int), ("voxel_size", C.c_double),
+        ("bbox_scale", C.c_double), ("boxes", _vp), ("pool", _vp), ("cloud_off", _vp), ("cloud_cnt", _vp),
+        ("n_pool", _ll), ("stats", _vp), ("cloud_out", _vp), ("max_cloud_out", _ll),
+        ("final_label", _vp), ("labels", _vp), ("bbox", _vp), ("relabel", C.c_int),
+    ]
+
+
 EXPORTS = (
     "vmb_version", "vmb_param_count", "vmb_param_stride", "vmb_param_offsets", "vmb_image_bytes",
     "vmb_create", "vmb_destroy", "vmb_last_error", "vmb_step", "vmb_mask_counts", "vmb_adam",
     "vmb_build_image", "vmb_forward", "vmb_sample", "vmb_ingest_frame", "vmb_debug_gemm",
     "vmb_mc_count", "vmb_mc_emit", "vmb_unproject",
     "vmb_clip_count", "vmb_clip_emit", "vmb_surface_sample", "vmb_nn_dist",
+    "vmb_assoc_classify", "vmb_assoc_voxel", "vmb_assoc_finalize",
 )
 
 _lib = None
@@ -189,6 +202,8 @@ def lib():
         L.vmb_clip_emit.argtypes = [_vp, C.POINTER(ClipArgs), _vp]
         L.vmb_surface_sample.argtypes = [_vp, C.POINTER(SurfaceSampleArgs), _vp]
         L.vmb_nn_dist.argtypes = [_vp, C.POINTER(NnArgs), _vp]
+        for n in ("vmb_assoc_classify", "vmb_assoc_voxel", "vmb_assoc_finalize"):
+            getattr(L, n).argtypes = [_vp, C.POINTER(AssocArgs), _vp]
         L.vmb_build_image.argtypes = [_vp, C.c_int, _vp, _vp, _vp]
         L.vmb_mask_counts.argtypes = [_vp, C.c_int, C.c_int, _vp, _ll, _vp, _ll, _vp, _vp]
         L.vmb_debug_gemm.argtypes = [C.c_int] * 7 + [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, C.c_int, _vp, C.c_int,

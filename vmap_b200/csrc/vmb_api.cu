@@ -18,6 +18,7 @@
 #include "k_layerwise.cuh"
 #include "k_mesh.cuh"
 #include "k_eval.cuh"
+#include "k_assoc.cuh"
 
 struct vmb_handle {
   int device, max_obj, H, nfreq;
@@ -38,6 +39,7 @@ struct vmb_handle {
   lw::Workspace ws_fwd;   // forward-only queries (vmb_forward): separate, so eval_points never moves the step's buffers
   mesh::Workspace ws_mesh;// marching cubes / unprojection scratch (grow-only)
   eval3d::Workspace ws_eval;// box crop / surface sampling / nearest-neighbour scratch (grow-only)
+  assoc::Workspace ws_assoc;// ScanNet association scratch (grow-only)
   std::string err;
 };
 
@@ -167,6 +169,7 @@ void vmb_destroy(vmb_handle* h) {
   h->ws_fwd.release(); h->ws_fwd.destroy_streams();
   h->ws_mesh.release();
   h->ws_eval.release();
+  h->ws_assoc.release();
   delete h;
 }
 
@@ -724,6 +727,146 @@ int vmb_nn_dist(vmb_handle* h, const vmb_nn_args* a, void* stream) {
   CUDA_TRY(h, w.exclusive_sum(q.cell_start, q.max_cells + 1, st));
   eval3d::k_nn_scatter<<<eval3d::blocks_for(q.n_ref, 256), 256, 0, st>>>(q);
   eval3d::k_nn_query<<<eval3d::blocks_for(q.n_q, 128), 128, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
+// ---- K7: ScanNet instance association (classify -> voxel -> finalize) ------------------------------
+static int assoc_params(vmb_handle* h, const vmb_assoc_args* a, assoc::Params& q, const char* who) {
+  if (!h || !a || a->width <= 0 || a->height <= 0 || !a->inst || !a->depth || !a->stats || !a->boxes)
+    return fail(h, VMB_E_ARG, std::string(who) + ": bad arguments");
+  if (a->max_id < 1 || a->max_id > 65536) return fail(h, VMB_E_ARG, std::string(who) + ": max_id must be in [1, 65536]");
+  if ((long long)a->width * a->height >= 0x7fffffffLL) return fail(h, VMB_E_ARG, std::string(who) + ": image too large");
+  if (a->bg_class && (!a->cls || a->n_class <= 0))
+    return fail(h, VMB_E_ARG, std::string(who) + ": bg_class needs the class image and n_class");
+  if (!(a->fx != 0.0) || !(a->fy != 0.0) || !(a->voxel_size > 0.0) || !(a->bbox_scale >= 0.0))
+    return fail(h, VMB_E_ARG, std::string(who) + ": need fx, fy != 0, voxel_size > 0 and bbox_scale >= 0");
+  if (a->n_pool < 0 || (a->n_pool > 0 && (!a->pool || !a->cloud_off || !a->cloud_cnt)) || a->n_pool >= 0x7fffffffLL)
+    return fail(h, VMB_E_ARG, std::string(who) + ": pool needs cloud_off / cloud_cnt");
+  memset(&q, 0, sizeof(q));
+  q.W = a->width; q.H = a->height; q.max_id = a->max_id; q.n = (long long)a->width * a->height;
+  q.inst = a->inst; q.cls = a->cls; q.depth = a->depth; q.bg_class = a->bg_class; q.n_class = a->n_class;
+  q.fx = a->fx; q.fy = a->fy; q.cx = a->cx; q.cy = a->cy;
+  for (int i = 0; i < 12; ++i) q.P[i] = a->camera_pose[i];
+  q.min_pixels = a->min_pixels; q.voxel = a->voxel_size; q.half_voxel = a->voxel_size * 0.5;
+  q.half_scale = 0.5 * a->bbox_scale;
+  q.boxes = a->boxes; q.pool = a->pool; q.cloud_off = a->cloud_off; q.cloud_cnt = a->cloud_cnt;
+  q.stats = a->stats;
+  q.bound = a->n_pool + q.n;
+  // scratch carving (grow-only; pixel, id and element regions)
+  assoc::Workspace& w = h->ws_assoc;
+  const size_t n = (size_t)q.n, ni = (size_t)q.max_id + 1, nb = (size_t)q.bound;
+  const size_t o_row = assoc::align16(n), o_k = o_row + assoc::align16(n), o_ko = o_k + 4 * n, o_v = o_ko + 4 * n,
+               o_vo = o_v + 4 * n, pix_need = o_vo + 4 * n;
+  CUDA_TRY(h, assoc::Workspace::grow((void**)&w.pix, &w.pix_cap, pix_need));
+  q.flags = w.pix; q.rowok = w.pix + o_row;
+  q.sel_key = (int*)(w.pix + o_k); q.sel_key_out = (int*)(w.pix + o_ko);
+  q.sel_val = (int*)(w.pix + o_v); q.sel_val_out = (int*)(w.pix + o_vo);
+  const size_t i_seg = assoc::align16(4 * ni), i_min = i_seg + assoc::align16(4 * ni), i_st = i_min + 24 * ni,
+               i_ext = i_st + 16, ids_need = i_ext + 20 * ni;
+  CUDA_TRY(h, assoc::Workspace::grow((void**)&w.ids, &w.ids_cap, ids_need));
+  q.new_off = (int*)w.ids; q.seg_off = (int*)(w.ids + i_seg);
+  q.minb = (unsigned long long*)(w.ids + i_min); q.status = (int*)(w.ids + i_st);
+  const size_t e_k = 24 * nb, e_ko = e_k + 8 * nb, e_i = e_ko + 8 * nb, e_io = e_i + 4 * nb,
+               e_h = e_io + assoc::align16(4 * nb), el_need = e_h + 4 * (nb + 1);
+  CUDA_TRY(h, assoc::Workspace::grow((void**)&w.el, &w.el_cap, el_need));
+  q.elem = (double*)w.el; q.ekey = (unsigned long long*)(w.el + e_k); q.ekey_out = (unsigned long long*)(w.el + e_ko);
+  q.eidx = (int*)(w.el + e_i); q.eidx_out = (int*)(w.el + e_io); q.head = (int*)(w.el + e_h);
+  return VMB_OK;
+}
+
+static bool assoc_same(const assoc::Params& a, const assoc::Params& b) {
+  return a.W == b.W && a.H == b.H && a.max_id == b.max_id && a.inst == b.inst && a.depth == b.depth &&
+         a.stats == b.stats && a.boxes == b.boxes && a.pool == b.pool && a.bound == b.bound;
+}
+
+int vmb_assoc_classify(vmb_handle* h, const vmb_assoc_args* a, void* stream) {
+  assoc::Params q;
+  const int rc = assoc_params(h, a, q, "vmb_assoc_classify");
+  if (rc != VMB_OK) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const unsigned gi = assoc::grid_for(q.max_id + 1, 256, 1 << 20), gp = assoc::grid_for(q.n, 256, 8 * h->n_sm);
+  assoc::k_init<<<gi, 256, 0, st>>>(q);
+  assoc::k_stats<<<gp, 256, 0, st>>>(q);
+  assoc::k_erode_u<<<gp, 256, 0, st>>>(q);
+  assoc::k_classify<<<gp, 256, 0, st>>>(q);
+  assoc::k_decide<<<gi, 256, 0, st>>>(q);
+  assoc::k_select<<<gp, 256, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  int end_bit = 1;
+  while ((1 << end_bit) <= q.max_id) ++end_bit;
+  assoc::Workspace& w = h->ws_assoc;
+  size_t need = 0;
+  CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(nullptr, need, q.sel_key, q.sel_key_out, q.sel_val, q.sel_val_out,
+                                              (int)q.n, 0, end_bit, st));
+  CUDA_TRY(h, w.tmp(need));
+  CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(w.cub_tmp, need, q.sel_key, q.sel_key_out, q.sel_val, q.sel_val_out,
+                                              (int)q.n, 0, end_bit, st));
+  w.last = q;
+  w.classified = true;
+  return VMB_OK;
+}
+
+int vmb_assoc_voxel(vmb_handle* h, const vmb_assoc_args* a, void* stream) {
+  assoc::Params q;
+  const int rc = assoc_params(h, a, q, "vmb_assoc_voxel");
+  if (rc != VMB_OK) return rc;
+  assoc::Workspace& w = h->ws_assoc;
+  if (!w.classified || !assoc_same(w.last, q))
+    return fail(h, VMB_E_ARG, "vmb_assoc_voxel: no matching vmb_assoc_classify on this handle");
+  if (!a->cloud_out || a->max_cloud_out < q.bound)
+    return fail(h, VMB_E_ARG, "vmb_assoc_voxel: cloud_out must hold n_pool + width * height points");
+  cudaStream_t st = (cudaStream_t)stream;
+  const unsigned gi = assoc::grid_for(q.max_id + 1, 256, 1 << 20), ge = assoc::grid_for(q.bound, 256, 8 * h->n_sm);
+  assoc::k_seg_len<<<gi, 256, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  size_t need = 0;
+  CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(nullptr, need, q.seg_off, q.max_id + 1, st));
+  CUDA_TRY(h, w.tmp(need));
+  CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(w.cub_tmp, need, q.seg_off, q.max_id + 1, st));
+  CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(w.cub_tmp, need, q.new_off, q.max_id + 1, st));
+  assoc::k_elements<<<ge, 256, 0, st>>>(q);
+  assoc::k_keys<<<ge, 256, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  need = 0;
+  CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(nullptr, need, q.ekey, q.ekey_out, q.eidx, q.eidx_out, (int)q.bound, 0, 64, st));
+  CUDA_TRY(h, w.tmp(need));
+  CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(w.cub_tmp, need, q.ekey, q.ekey_out, q.eidx, q.eidx_out, (int)q.bound, 0, 64, st));
+  assoc::k_heads<<<ge, 256, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  need = 0;
+  CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(nullptr, need, q.head, (int)(q.bound + 1), st));
+  CUDA_TRY(h, w.tmp(need));
+  CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(w.cub_tmp, need, q.head, (int)(q.bound + 1), st));
+  assoc::k_voxel_mean<<<ge, 256, 0, st>>>(q, a->cloud_out);
+  CUDA_TRY(h, cudaGetLastError());
+  int status = 0;
+  CUDA_TRY(h, cudaMemcpyAsync(&status, q.status, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(h, cudaStreamSynchronize(st));
+  if (status) return fail(h, VMB_E_ARG, "vmb_assoc_voxel: a cloud spans more than 65536 voxels along an axis");
+  return VMB_OK;
+}
+
+int vmb_assoc_finalize(vmb_handle* h, const vmb_assoc_args* a, void* stream) {
+  assoc::Params q;
+  const int rc = assoc_params(h, a, q, "vmb_assoc_finalize");
+  if (rc != VMB_OK) return rc;
+  assoc::Workspace& w = h->ws_assoc;
+  if (!w.classified || !assoc_same(w.last, q))
+    return fail(h, VMB_E_ARG, "vmb_assoc_finalize: no matching vmb_assoc_classify on this handle");
+  if (!a->final_label || !a->labels || !a->bbox) return fail(h, VMB_E_ARG, "vmb_assoc_finalize: bad arguments");
+  assoc::FinParams f;
+  memset(&f, 0, sizeof(f));
+  f.W = q.W; f.H = q.H; f.max_id = q.max_id; f.n = q.n;
+  f.inst = q.inst; f.depth = q.depth; f.stats = q.stats; f.flags = q.flags; f.final_label = a->final_label;
+  f.labels = a->labels; f.bbox = a->bbox; f.half_scale = q.half_scale;
+  f.ext = (int*)(w.ids + ((size_t)((char*)q.status - (char*)w.ids) + 16));
+  cudaStream_t st = (cudaStream_t)stream;
+  const unsigned gi = assoc::grid_for(q.max_id + 1, 256, 1 << 20), gp = assoc::grid_for(q.n, 256, 8 * h->n_sm);
+  assoc::k_fin_init<<<gi, 256, 0, st>>>(f);
+  assoc::k_fin_label<<<gp, 256, 0, st>>>(f);
+  assoc::k_fin_box<<<gi, 256, 0, st>>>(f);
+  if (a->relabel) assoc::k_fin_relabel<<<gp, 256, 0, st>>>(f);
   CUDA_TRY(h, cudaGetLastError());
   return VMB_OK;
 }

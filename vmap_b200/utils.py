@@ -123,3 +123,10 @@ def vmap(fmodel, *args, **kwargs):
         raise TypeError("vmap_b200.vmap only maps the fused models returned by update_vmap "
                         "(no tracing / PyTorch fallback)")
     return fmodel.batched
+
+
+def box_filter(masks, classes, depth, inst_dict, intrinsic_open3d, T_CW, min_pixels=500, voxel_size=0.01):
+    """utils.box_filter (utils.py:112-208) with the reference's signature and return value (int64 [H, W]), run by
+    the GPU instance tracker of vmap_b200.scannet; the tracking state follows the ``inst_dict`` object."""
+    from .scannet import box_filter as _box_filter
+    return _box_filter(masks, classes, depth, inst_dict, intrinsic_open3d, T_CW, min_pixels, voxel_size)
