@@ -149,7 +149,7 @@ EXPORTS = (
     "vmb_build_image", "vmb_forward", "vmb_sample", "vmb_ingest_frame", "vmb_debug_gemm",
     "vmb_mc_count", "vmb_mc_emit", "vmb_unproject",
     "vmb_clip_count", "vmb_clip_emit", "vmb_surface_sample", "vmb_nn_dist",
-    "vmb_assoc_classify", "vmb_assoc_voxel", "vmb_assoc_finalize",
+    "vmb_assoc_classify", "vmb_assoc_voxel", "vmb_assoc_finalize", "vmb_step_cooperative",
 )
 
 _lib = None
@@ -187,6 +187,7 @@ def lib():
             getattr(L, n).argtypes = [C.c_int, C.c_int]
             getattr(L, n).restype = C.c_int
         L.vmb_param_offsets.argtypes = [C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+        L.vmb_step_cooperative.argtypes = [C.c_int]
         L.vmb_create.argtypes = [C.POINTER(_vp), C.c_int, C.c_int, C.c_int, C.c_int]
         L.vmb_destroy.argtypes = [_vp]
         L.vmb_destroy.restype = None

@@ -23,15 +23,33 @@ struct AdamParams {
   float eps;
   int zero_grads;
   // optional device-resident per-object step numbers (CUDA-graph replay): t_b = step_counter[b] + 1 is read by
-  // every block on entry; the last block to finish increments them all and resets the ticket.
+  // every block on entry; the last block to finish increments those of the updated objects and resets the ticket.
   int* step_counter; unsigned int* ticket;
   double lr, b1, b2d;
   float log_b1, log_b2;       // ln(beta1), ln(beta2)
   const float2* bc_table; int bc_n;   // [t] -> (1 - beta1^t, sqrt(1 - beta2^t)), host-built in double precision
 };
 
+// render_rays.py:88-90's guard on object b's loss terms (the reference aborts before the update): 1 = one of the three
+// terms above 1e5, 2 = any of the four values (terms and weighted total) non-finite or beyond 3e38; 0 when the guard is
+// off.  The fused hidden-32 finisher tests only the total for bit 2; a non-finite term always makes the total
+// non-finite, so both flag the same objects.
+__device__ __forceinline__ int adam_row_guard(const float* loss_terms, int b) {
+  if (!loss_terms) return 0;
+  int bad = 0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float l = loss_terms[b * 4 + i];
+    if (i != 3 && l > 100000.f) bad |= 1;
+    if (!(l == l) || fabsf(l) > 3.0e38f) bad |= 2;
+  }
+  return bad;
+}
+
+// The guard is per object: a row whose loss tripped it keeps its params, moments, image and step number and only has
+// its gradients zeroed; the other rows of the launch are updated.
 __global__ void __launch_bounds__(256) k_adamw(AdamParams a) {
-  __shared__ int s_skip;
+  __shared__ int s_skip[2];
   __shared__ float s_step_size[2], s_bc2_sqrt[2];
   // issue this thread's loads first: their latency overlaps the bias-correction prologue
   const long long i4 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4;
@@ -44,9 +62,12 @@ __global__ void __launch_bounds__(256) k_adamw(AdamParams a) {
   }
   // a block covers 1024 consecutive floats = at most two rows (row pitch >= 1024): per-object step numbers
   const int row0 = (int)(((long long)blockIdx.x * blockDim.x * 4) / a.stride);
-  if (threadIdx.x == 0) s_skip = 0;
   if (threadIdx.x < 2) {
     const int rb = row0 + threadIdx.x;
+    const int bad = rb < a.B ? adam_row_guard(a.loss_terms, rb) : 0;
+    s_skip[threadIdx.x] = bad;
+    // the block holding the row's first float reports it, so the status word gets each row's bits exactly once
+    if (bad && a.status && (long long)rb * a.stride / ((long long)blockDim.x * 4) == blockIdx.x) atomicOr(a.status, bad);
     if (a.step_counter && rb < a.B) {
       // bias corrections of step t from the host-built table (torch's double scalars, rounded once); beyond the table
       // 1 - beta^t = -expm1(t ln beta), fp32, cancellation-free (<= 3e-7 relative)
@@ -70,25 +91,12 @@ __global__ void __launch_bounds__(256) k_adamw(AdamParams a) {
     if (threadIdx.x == 32) *a.loss_sum = s;
   }
   __syncthreads();
-  if (a.loss_terms) {       // render_rays.py:88-90: the reference aborts before the update
-    int bad = 0;
-    for (int i = threadIdx.x; i < a.B * 4; i += blockDim.x) {
-      const float l = a.loss_terms[i];
-      if ((i & 3) != 3 && l > 100000.f) bad |= 1;
-      if (!(l == l) || fabsf(l) > 3.0e38f) bad |= 2;
-    }
-    if (bad) atomicOr(&s_skip, bad);
-    __syncthreads();
-    if (s_skip) {
-      // no update; the exploded gradients must not leak into the next step's accumulation
-      if (a.zero_grads && i4 < a.n) *reinterpret_cast<float4*>(a.g + i4) = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (blockIdx.x == 0 && threadIdx.x == 0 && a.status) atomicOr(a.status, s_skip);
-      return;
-    }
-  }
-  if (i4 < a.n) {
-  if (a.grad_scale) { const float gs = *a.grad_scale; g.x *= gs; g.y *= gs; g.z *= gs; g.w *= gs; }
   const int b = (int)(i4 / a.stride);
+  if (i4 < a.n && s_skip[b - row0]) {
+    // no update of this object; its exploded gradients must not leak into the next step's accumulation
+    if (a.zero_grads) *reinterpret_cast<float4*>(a.g + i4) = make_float4(0.f, 0.f, 0.f, 0.f);
+  } else if (i4 < a.n) {
+  if (a.grad_scale) { const float gs = *a.grad_scale; g.x *= gs; g.y *= gs; g.z *= gs; g.w *= gs; }
   const float step_size = s_step_size[b - row0], bc2_sqrt = s_bc2_sqrt[b - row0];
   float* pp = &p.x; float* gg = &g.x; float* mm = &m.x; float* vv = &v.x;
 #pragma unroll
@@ -126,7 +134,8 @@ __global__ void __launch_bounds__(256) k_adamw(AdamParams a) {
     }
     __syncthreads();
     if (s_last) {           // every block has read its step numbers: the last one to finish publishes t + 1
-      for (int i = threadIdx.x; i < a.B; i += blockDim.x) a.step_counter[i] += 1;
+      for (int i = threadIdx.x; i < a.B; i += blockDim.x)
+        if (!adam_row_guard(a.loss_terms, i)) a.step_counter[i] += 1;
       if (threadIdx.x == 0) *a.ticket = 0u;
     }
   }

@@ -1002,6 +1002,18 @@ static void fused_partition(int B, int npo, int G, uf::Ranges& rg) {
   while (c < G) rg.begin[++c] = (int)T;
 }
 
+// Whether a training step on device `dev` takes the cooperative (grid-wide) finish: the device supports cooperative
+// launch and VMB_NO_COOP is not set (read per call).  Otherwise each object's last CTA reduces and updates it.
+static bool fused_cooperative(int dev) {
+  static int coop_ok[64] = {};
+  if (coop_ok[dev & 63] == 0) {
+    int v = 0;
+    cudaDeviceGetAttribute(&v, cudaDevAttrCooperativeLaunch, dev);
+    coop_ok[dev & 63] = v ? 1 : -1;
+  }
+  return coop_ok[dev & 63] == 1 && getenv("VMB_NO_COOP") == nullptr;
+}
+
 static int fused_launch_step(const VmbLayout& L, const StepParams& sp, const FusedExtra& fx, const void* image, int n_sm,
                              cudaStream_t st, std::string& err, bool* cooperative = nullptr) {
   using namespace uf;
@@ -1035,13 +1047,7 @@ static int fused_launch_step(const VmbLayout& L, const StepParams& sp, const Fus
   FusedExtra fxl = fx;
   // every CTA is resident (grid <= #SMs, one CTA per SM) -- the cooperative attribute makes the runtime guarantee it,
   // which is what lets an object's CTAs wait for each other in the shared reduction
-  static int coop_ok[64] = {};
-  if (coop_ok[dev & 63] == 0) {
-    int v = 0;
-    cudaDeviceGetAttribute(&v, cudaDevAttrCooperativeLaunch, dev);
-    coop_ok[dev & 63] = v ? 1 : -1;
-  }
-  fxl.cooperative = (coop_ok[dev & 63] == 1 && !sp.fwd_only && getenv("VMB_NO_COOP") == nullptr) ? 1 : 0;
+  fxl.cooperative = (!sp.fwd_only && fused_cooperative(dev)) ? 1 : 0;
   if (cooperative) *cooperative = fxl.cooperative != 0;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));

@@ -379,6 +379,8 @@ int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
   return VMB_OK;
 }
 
+int vmb_step_cooperative(int device) { return fused_cooperative(device) ? 1 : 0; }
+
 int vmb_forward(vmb_handle* h, const vmb_forward_args* a, void* stream) {
   if (!h || !a || a->n_obj <= 0 || a->n_obj > h->max_obj || a->n_points <= 0 || !a->points || !a->params ||
       !a->scale || !a->alpha || !a->colour)
