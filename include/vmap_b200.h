@@ -436,6 +436,62 @@ int vmb_assoc_classify(vmb_handle* h, const vmb_assoc_args* a, void* stream);
 int vmb_assoc_voxel(vmb_handle* h, const vmb_assoc_args* a, void* stream);
 int vmb_assoc_finalize(vmb_handle* h, const vmb_assoc_args* a, void* stream);
 
+/* ---- K8: convex hulls and minimum-volume boxes -----------------------------------------------------
+ * vmb_hull      exact 3-D convex hull of n_sets point sets in one call.  Set s is the next set_size[s * size_stride]
+ *               points of `points` (negative sizes count as 0; the sizes are read and scanned on the device, so
+ *               stats[:, 7] of vmb_assoc_voxel feeds it directly).  A vertex is an extreme point: a point on a facet
+ *               or an edge is not one, and of several copies of an extreme point only the lowest index is flagged.
+ *               Every predicate is exact (fp64 orientation with a static error filter, expansion arithmetic when
+ *               the filter cannot decide).  status[s]: VMB_HULL_OK, TOO_FEW (fewer than 4 points), FLAT (all points
+ *               coplanar, collinear or identical), BAD (the set reaches past n_points); a set that is not OK has no
+ *               vertices and no facets.  Facets of set s are the rows 2 * (first point of s) + [0, facet_count[s]) of
+ *               `facets`: point-index triples (a, b, c) with the outward normal along (b - a) x (c - a), a
+ *               triangulation of the hull's boundary (its corners may include points that lie on a hull edge or
+ *               inside a flat face).  facet_nbr[row][j] is the facet (relative to the set's first row) across the edge
+ *               (v_j, v_j+1).  Vertices are compacted in (set, input order); vertex_offset[s] is set s's first
+ *               entry and vertex_offset[n_sets] the total.  No host sync.                                     */
+enum { VMB_HULL_OK = 0, VMB_HULL_TOO_FEW = 1, VMB_HULL_FLAT = 2, VMB_HULL_BAD = 3 };
+
+typedef struct vmb_hull_args {
+  const double* points;          /* [n_points][3], finite                                                         */
+  long long n_points;
+  const int* set_size;           /* device: size of set s at set_size[s * size_stride]                            */
+  int size_stride;               /* >= 1 (ints)                                                                   */
+  int n_sets;                    /* >= 1                                                                          */
+  unsigned char* is_vertex;      /* out [n_points] 1 = extreme point of its set                                   */
+  int* vertex_count;             /* out [n_sets]                                                                  */
+  int* vertex_offset;            /* optional out [n_sets + 1]; required with vertices                             */
+  int* vertices;                 /* optional out [n_points] extreme point indices, (set, input order)             */
+  int* status;                   /* out [n_sets] VMB_HULL_*                                                       */
+  int* facets;                   /* out [2 * n_points][3]                                                         */
+  int* facet_nbr;                /* optional out [2 * n_points][3]                                                */
+  int* facet_count;              /* out [n_sets]                                                                  */
+} vmb_hull_args;
+
+int vmb_hull(vmb_handle* h, const vmb_hull_args* a, void* stream);
+
+/* vmb_obb_minvol  minimum-volume oriented box of one set from its hull (trimesh.bounds.oriented_bounds as
+ *               vmap_b200/mesh.py restates it): for every distinct facet normal (unit, rounded to 1e-10) the height
+ *               along it and the minimum-area rectangle of the projected hull vertices over the projected silhouette
+ *               edge directions; the least volume wins, exact ties to the lexicographically smallest normal.  Pass
+ *               the set's rows of vmb_hull's facets / facet_nbr, its vertices, and device pointers to its counts and
+ *               status.  box = center[3], R[3][3] row-major (columns are the box axes, det +1), extent[3], fp64.
+ *               box_status = VMB_HULL_OK or the hull's status.  No host sync.                                    */
+typedef struct vmb_obb_args {
+  const double* points;          /* the points vmb_hull was given                                                 */
+  const int* facets;             /* [facet_count][3]                                                              */
+  const int* facet_nbr;          /* [facet_count][3]                                                              */
+  const int* facet_count;        /* device [1]                                                                    */
+  const int* vertices;           /* [vertex_count] extreme point indices                                          */
+  const int* vertex_count;       /* device [1]                                                                    */
+  const int* status;             /* device [1] the set's VMB_HULL_* status                                        */
+  long long max_facets;          /* upper bound of facet_count (sizes the scratch)                                */
+  double* box;                   /* out [15]                                                                      */
+  int* box_status;               /* out [1]                                                                       */
+} vmb_obb_args;
+
+int vmb_obb_minvol(vmb_handle* h, const vmb_obb_args* a, void* stream);
+
 /* ---- bring-up / test hook (not part of the reference-facing surface) --------------------------- */
 /* Generic wgmma GEMM of the layer-wise wide-model path: D[M][N] = A[M][K1+K2] * B[N][K]^T, fp16 in,
  * fp32 accumulate.  a_mn/b_mn = 0: operand stored [rows][ld] with K contiguous; 1: stored [K][ld] with

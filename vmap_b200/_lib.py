@@ -143,6 +143,23 @@ class AssocArgs(C.Structure):
     ]
 
 
+class HullArgs(C.Structure):
+    _fields_ = [
+        ("points", _vp), ("n_points", _ll), ("set_size", _vp), ("size_stride", C.c_int), ("n_sets", C.c_int),
+        ("is_vertex", _vp), ("vertex_count", _vp), ("vertex_offset", _vp), ("vertices", _vp), ("status", _vp),
+        ("facets", _vp), ("facet_nbr", _vp), ("facet_count", _vp),
+    ]
+
+
+class ObbArgs(C.Structure):
+    _fields_ = [
+        ("points", _vp), ("facets", _vp), ("facet_nbr", _vp), ("facet_count", _vp), ("vertices", _vp),
+        ("vertex_count", _vp), ("status", _vp), ("max_facets", _ll), ("box", _vp), ("box_status", _vp),
+    ]
+
+
+HULL_OK, HULL_TOO_FEW, HULL_FLAT, HULL_BAD = 0, 1, 2, 3       # VMB_HULL_*
+
 EXPORTS = (
     "vmb_version", "vmb_param_count", "vmb_param_stride", "vmb_param_offsets", "vmb_image_bytes",
     "vmb_create", "vmb_destroy", "vmb_last_error", "vmb_step", "vmb_mask_counts", "vmb_adam",
@@ -150,6 +167,7 @@ EXPORTS = (
     "vmb_mc_count", "vmb_mc_emit", "vmb_unproject",
     "vmb_clip_count", "vmb_clip_emit", "vmb_surface_sample", "vmb_nn_dist",
     "vmb_assoc_classify", "vmb_assoc_voxel", "vmb_assoc_finalize", "vmb_step_cooperative",
+    "vmb_hull", "vmb_obb_minvol",
 )
 
 _lib = None
@@ -205,6 +223,8 @@ def lib():
         L.vmb_nn_dist.argtypes = [_vp, C.POINTER(NnArgs), _vp]
         for n in ("vmb_assoc_classify", "vmb_assoc_voxel", "vmb_assoc_finalize"):
             getattr(L, n).argtypes = [_vp, C.POINTER(AssocArgs), _vp]
+        L.vmb_hull.argtypes = [_vp, C.POINTER(HullArgs), _vp]
+        L.vmb_obb_minvol.argtypes = [_vp, C.POINTER(ObbArgs), _vp]
         L.vmb_build_image.argtypes = [_vp, C.c_int, _vp, _vp, _vp]
         L.vmb_mask_counts.argtypes = [_vp, C.c_int, C.c_int, _vp, _ll, _vp, _ll, _vp, _vp]
         L.vmb_debug_gemm.argtypes = [C.c_int] * 7 + [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, C.c_int, _vp, C.c_int,

@@ -19,6 +19,7 @@
 #include "k_mesh.cuh"
 #include "k_eval.cuh"
 #include "k_assoc.cuh"
+#include "k_hull.cuh"
 
 struct vmb_handle {
   int device, max_obj, H, nfreq;
@@ -40,6 +41,7 @@ struct vmb_handle {
   mesh::Workspace ws_mesh;// marching cubes / unprojection scratch (grow-only)
   eval3d::Workspace ws_eval;// box crop / surface sampling / nearest-neighbour scratch (grow-only)
   assoc::Workspace ws_assoc;// ScanNet association scratch (grow-only)
+  hull::Workspace ws_hull;  // convex hull / minimum-volume box scratch (grow-only)
   std::string err;
 };
 
@@ -170,6 +172,7 @@ void vmb_destroy(vmb_handle* h) {
   h->ws_mesh.release();
   h->ws_eval.release();
   h->ws_assoc.release();
+  h->ws_hull.release();
   delete h;
 }
 
@@ -869,6 +872,114 @@ int vmb_assoc_finalize(vmb_handle* h, const vmb_assoc_args* a, void* stream) {
   assoc::k_fin_label<<<gp, 256, 0, st>>>(f);
   assoc::k_fin_box<<<gi, 256, 0, st>>>(f);
   if (a->relabel) assoc::k_fin_relabel<<<gp, 256, 0, st>>>(f);
+  CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
+// ---- K8: convex hulls and minimum-volume boxes ----------------------------------------------------
+static unsigned grid_of(long long n, int per, long long cap) {
+  long long g = (n + per - 1) / per;
+  if (g < 1) g = 1;
+  if (g > cap) g = cap;
+  return (unsigned)g;
+}
+
+int vmb_hull(vmb_handle* h, const vmb_hull_args* a, void* stream) {
+  using namespace hull;
+  if (!h || !a || a->n_points < 0 || (a->n_points > 0 && !a->points) || !a->set_size || a->size_stride < 1 ||
+      a->n_sets < 1 || !a->is_vertex || !a->vertex_count || !a->status || !a->facets || !a->facet_count ||
+      (a->vertices && !a->vertex_offset))
+    return fail(h, VMB_E_ARG, "vmb_hull: bad arguments");
+  if (a->n_points >= (1LL << 29)) return fail(h, VMB_E_ARG, "vmb_hull: too many points for int32 facet rows");
+  const long long n = a->n_points;
+  const int ns = a->n_sets;
+  const long long fcap = facet_cap(n, ns);
+  Params q;
+  memset(&q, 0, sizeof(q));
+  q.pts = a->points; q.n = n; q.set_size = a->set_size; q.size_stride = a->size_stride; q.n_sets = ns;
+  q.is_vertex = a->is_vertex; q.vertex_count = a->vertex_count; q.status = a->status;
+  q.facets = a->facets; q.facet_nbr = a->facet_nbr; q.facet_count = a->facet_count; q.fcap = fcap;
+  // scratch: per-set ints | per-point bytes and ints | facet work regions
+  const size_t si = align256(4 * (size_t)(ns + 1)), pb = align256((size_t)n + 1), pi = align256(4 * (size_t)n + 4),
+               fi = align256(4 * (size_t)fcap);
+  const size_t need = 11 * si + 256 + 2 * pb + 4 * pi + 12 * fi;
+  Workspace& w = h->ws_hull;
+  CUDA_TRY(h, Workspace::grow((void**)&w.buf, &w.cap, need));
+  unsigned char* c = w.buf;
+  auto take = [&](size_t bytes) { unsigned char* r = c; c += bytes; return r; };
+  q.size = (int*)take(si); q.start = (int*)take(si);
+  for (int k = 0; k < 3; ++k) q.cnt[k] = (int*)take(si);
+  for (int k = 0; k < 2; ++k) q.off[k] = (int*)take(si);
+  q.red = (int*)take(si); q.ntile = (int*)take(si); q.tile_start = (int*)take(si);
+  int* vcount1 = (int*)take(si);
+  q.n_sel = (int*)take(256);
+  q.mark = take(pb); q.keep = take(pb);
+  for (int k = 0; k < 2; ++k) q.list[k] = (int*)take(pi);
+  q.start_at = (int*)take(pi); q.end_at = (int*)take(pi);
+  q.fv = (int*)take(3 * fi); q.fn = (int*)take(3 * fi); q.fs = (int*)take(fi); q.vis = (int*)take(fi);
+  q.fre = (int*)take(fi); q.hz = (int*)take(3 * fi);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int ni = (int)std::max<long long>(n, 1);
+  size_t t1 = 0, t2 = 0, t3 = 0;
+  CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(nullptr, t1, q.size, q.start, ns + 1, st));
+  CUDA_TRY(h, cub::DeviceSelect::Flagged(nullptr, t2, q.list[0], q.keep, q.list[1], q.n_sel, ni, st));
+  CUDA_TRY(h, cub::DeviceSelect::Flagged(nullptr, t3, thrust::counting_iterator<int>(0), q.is_vertex, q.list[1],
+                                         q.n_sel, ni, st));
+  CUDA_TRY(h, Workspace::grow(&w.cub_tmp, &w.cub_cap, std::max(t1, std::max(t2, t3))));
+  size_t tb = w.cub_cap;
+  const unsigned gs = grid_of(ns + 1, 256, 4096), gn = grid_of(n, 256, 8 * (long long)h->n_sm);
+  k_sizes<<<gs, 256, 0, st>>>(q, q.cnt[0]);
+  CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(w.cub_tmp, tb, q.size, q.start, ns + 1, st));
+  k_init<<<gn, 256, 0, st>>>(q, q.cnt[0]);
+  CUDA_TRY(h, cudaGetLastError());
+  const int* cnt = q.cnt[0];
+  const int* prev = nullptr;
+  const int* off = q.start;
+  const int* list = q.list[0];
+  if (n > TILE)
+    for (int r = 0; r < ROUNDS; ++r) {
+      int* nxt = q.cnt[(r + 1) % 3];
+      int* off_n = q.off[r % 2];
+      int* list_n = q.list[(r + 1) % 2];
+      k_tiles<<<gs, 256, 0, st>>>(q, cnt, prev, q.red, nxt);
+      CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(w.cub_tmp, tb, q.ntile, q.tile_start, ns + 1, st));
+      k_tile<<<(unsigned)max_tiles(n, ns), NT, 0, st>>>(q, cnt, off, list, q.red, nxt);
+      k_keep<<<gn, 256, 0, st>>>(q, off, list);
+      CUDA_TRY(h, cudaGetLastError());
+      CUDA_TRY(h, cub::DeviceSelect::Flagged(w.cub_tmp, tb, list, q.keep, list_n, q.n_sel, ni, st));
+      CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(w.cub_tmp, tb, nxt, off_n, ns + 1, st));
+      prev = cnt; cnt = nxt; off = off_n; list = list_n;
+    }
+  k_final<<<ns, NT, 0, st>>>(q, cnt, off, list);
+  CUDA_TRY(h, cudaGetLastError());
+  if (a->vertex_offset) {
+    CUDA_TRY(h, cudaMemsetAsync(vcount1 + ns, 0, sizeof(int), st));
+    CUDA_TRY(h, cudaMemcpyAsync(vcount1, a->vertex_count, sizeof(int) * ns, cudaMemcpyDeviceToDevice, st));
+    CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(w.cub_tmp, tb, vcount1, a->vertex_offset, ns + 1, st));
+  }
+  if (a->vertices && n > 0)
+    CUDA_TRY(h, cub::DeviceSelect::Flagged(w.cub_tmp, tb, thrust::counting_iterator<int>(0), q.is_vertex,
+                                           a->vertices, q.n_sel, ni, st));
+  return VMB_OK;
+}
+
+int vmb_obb_minvol(vmb_handle* h, const vmb_obb_args* a, void* stream) {
+  using namespace hull;
+  if (!h || !a || !a->points || !a->facets || !a->facet_nbr || !a->facet_count || !a->vertices || !a->vertex_count ||
+      !a->status || !a->box || !a->box_status || a->max_facets < 0)
+    return fail(h, VMB_E_ARG, "vmb_obb_minvol: bad arguments");
+  const long long cap = std::max<long long>(a->max_facets, 1);
+  Workspace& w = h->ws_hull;
+  CUDA_TRY(h, Workspace::grow((void**)&w.obb, &w.obb_cap, 15 * sizeof(double) * (size_t)cap));
+  ObbParams q;
+  q.pts = a->points; q.facets = a->facets; q.facet_nbr = a->facet_nbr; q.facet_count = a->facet_count;
+  q.vertices = a->vertices; q.vertex_count = a->vertex_count; q.status = a->status;
+  q.box = a->box; q.box_status = a->box_status;
+  q.nr = w.obb; q.nu = w.obb + 3 * cap; q.res = w.obb + 6 * cap;
+  cudaStream_t st = (cudaStream_t)stream;
+  k_obb_normals<<<grid_of(cap, 256, 8 * (long long)h->n_sm), 256, 0, st>>>(q);
+  k_obb_eval<<<grid_of(cap, 1, 8 * (long long)h->n_sm), NT, 0, st>>>(q);
+  k_obb_pick<<<1, NT, 0, st>>>(q);
   CUDA_TRY(h, cudaGetLastError());
   return VMB_OK;
 }

@@ -1,16 +1,17 @@
 """Meshing path of train.py's visualisation block (train.py:343-368): object bounds (sceneObject.get_bound,
 vmap.py:270-315) and marching cubes (Trainer.meshing, trainer.py:35-75, vis.py:6-29).
 
-Per-pixel and per-voxel arithmetic runs in the library (K5, csrc/k_mesh.cuh): the object-pixel unprojection and
-marching cubes.  The host keeps what is small and sequential: the convex hull of the unprojected points
-(scipy.spatial.ConvexHull) and the minimum-volume box fitted to it, and the ``Mesh`` container that train.py
-exports.  There is no CPU fallback: without the library every call raises.
+Per-pixel and per-voxel arithmetic runs in the library: the object-pixel unprojection and marching cubes (K5,
+csrc/k_mesh.cuh), the exact convex hull of the unprojected points and the minimum-volume box fitted to it (K8,
+csrc/k_hull.cuh).  The host keeps the ``Mesh`` container that train.py exports, and ``oriented_bounds``, the host
+restatement of trimesh's box fit that the device fit is checked against.  There is no CPU fallback: without the
+library every device call raises.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Dict, Optional, Tuple
+from typing import Dict, List, NamedTuple, Optional, Tuple, Union
 
 import numpy as np
 import torch
@@ -206,3 +207,96 @@ def oriented_bounds(points: np.ndarray):
         R[:, 2] = -R[:, 2]
         mid[2] = -mid[2]
     return R @ mid, R, ext
+
+
+# ---- exact convex hull and minimum-volume box on the device (K8) ----------------------------------------------------
+class Hull(NamedTuple):
+    """Convex hull of one point set: ``vertices`` int64 [V] indices of the extreme points in input order (scipy's
+    ``ConvexHull.vertices`` order), ``facets`` int64 [F, 3] outward triangles (normal along (b - a) x (c - a)), both
+    on the points' device; ``status`` one of _lib.HULL_OK / HULL_TOO_FEW (< 4 points) / HULL_FLAT (coplanar,
+    collinear or identical points), with no vertices and no facets unless OK."""
+    vertices: torch.Tensor
+    facets: torch.Tensor
+    status: int
+
+
+def _as_points64(points, device=None) -> torch.Tensor:
+    t = torch.as_tensor(points)
+    if device is None:
+        device = t.device if t.is_cuda else torch.device("cuda", torch.cuda.current_device())
+    t = t.to(device=device, dtype=torch.float64).reshape(-1, 3).contiguous()
+    return t
+
+
+def _hull_launch(k: _Kernels, pts: torch.Tensor, sizes: torch.Tensor, stride: int, n_sets: int, nbr: bool = False):
+    """Enqueues vmb_hull on fp64 points [n, 3] split into n_sets sets (set s has sizes[s * stride] points); returns
+    the device outputs.  No host sync."""
+    dev, n = pts.device, pts.shape[0]
+    i32 = dict(dtype=torch.int32, device=dev)
+    o = {"is_vertex": torch.empty(max(n, 1), dtype=torch.uint8, device=dev),
+         "vertex_count": torch.empty(n_sets, **i32), "vertex_offset": torch.empty(n_sets + 1, **i32),
+         "vertices": torch.empty(max(n, 1), **i32), "status": torch.empty(n_sets, **i32),
+         "facets": torch.empty(max(2 * n, 1), 3, **i32), "facet_count": torch.empty(n_sets, **i32),
+         "facet_nbr": torch.empty(max(2 * n, 1), 3, **i32) if nbr else None}
+    a = _lib.HullArgs()
+    a.points, a.n_points, a.set_size, a.size_stride, a.n_sets = _p(pts) if n else None, n, _p(sizes), stride, n_sets
+    for f in ("is_vertex", "vertex_count", "vertex_offset", "vertices", "status", "facets", "facet_nbr",
+              "facet_count"):
+        setattr(a, f, _p(o[f]))
+    k.call("vmb_hull", a)
+    return o
+
+
+def convex_hull(points: Union[torch.Tensor, np.ndarray, List]) -> Union[Hull, List[Hull]]:
+    """Exact convex hull (K8) of one point set [n, 3], or of each set in a list (one launch for all).  Points are
+    taken in fp64 (fp32 converts exactly) on their CUDA device, or the current one for host input.  A vertex is an
+    extreme point: points on a facet or an edge are not vertices, and of several copies of an extreme point only the
+    lowest index is one.  Returns a Hull per set, indices relative to that set."""
+    single = torch.is_tensor(points) or isinstance(points, np.ndarray)
+    sets = [points] if single else list(points)
+    if not sets:
+        return []
+    first = torch.as_tensor(sets[0])
+    dev = first.device if first.is_cuda else torch.device("cuda", torch.cuda.current_device())
+    parts = [_as_points64(p, dev) for p in sets]
+    pts = torch.cat(parts) if len(parts) > 1 else parts[0]
+    counts = [int(p.shape[0]) for p in parts]
+    sizes = torch.tensor(counts, dtype=torch.int32, device=dev)
+    o = _hull_launch(_kernels(dev), pts, sizes, 1, len(parts))
+    meta = torch.cat([o["vertex_offset"], o["status"], o["facet_count"]]).cpu().numpy()
+    ns = len(parts)
+    vo, st, fc = meta[:ns + 1], meta[ns + 1:2 * ns + 1], meta[2 * ns + 1:]
+    out, start = [], 0
+    for s, c in enumerate(counts):
+        v = o["vertices"][int(vo[s]):int(vo[s + 1])].long() - start
+        f = o["facets"][2 * start:2 * start + int(fc[s])].long() - start
+        out.append(Hull(v, f, int(st[s])))
+        start += c
+    return out[0] if single else out
+
+
+def oriented_bounds_gpu(points):
+    """``oriented_bounds`` on the device: exact hull (K8), then the minimum-volume box over its distinct facet normals
+    (vmb_obb_minvol), with no host round trip of the points; only the 15 numbers of the box come back.  Returns
+    (center [3], R [3, 3] with the box axes as columns and det +1, extent [3]) as fp64 numpy.  Raises ValueError
+    when the points are fewer than 4 or flat (coplanar, collinear or identical)."""
+    pts = _as_points64(points)
+    dev, n = pts.device, pts.shape[0]
+    k = _kernels(dev)
+    sizes = torch.tensor([n], dtype=torch.int32, device=dev)
+    o = _hull_launch(k, pts, sizes, 1, 1, nbr=True)
+    box = torch.empty(16, dtype=torch.float64, device=dev)
+    status = torch.empty(1, dtype=torch.int32, device=dev)
+    a = _lib.ObbArgs()
+    a.points, a.facets, a.facet_nbr, a.facet_count = _p(pts) if n else _p(box), _p(o["facets"]), _p(o["facet_nbr"]), \
+        _p(o["facet_count"])
+    a.vertices, a.vertex_count, a.status = _p(o["vertices"]), _p(o["vertex_count"]), _p(o["status"])
+    a.max_facets, a.box, a.box_status = max(2 * n, 1), _p(box), _p(status)
+    k.call("vmb_obb_minvol", a)
+    box[15] = status[0].to(torch.float64)
+    b = box.cpu().numpy()
+    st = int(b[15])
+    if st != _lib.HULL_OK:
+        raise ValueError("oriented_bounds_gpu: " + ("fewer than 4 points" if st == _lib.HULL_TOO_FEW else
+                                                    "the points are flat (coplanar, collinear or identical)"))
+    return b[0:3].copy(), b[3:12].reshape(3, 3).copy(), b[12:15].copy()

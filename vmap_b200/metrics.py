@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .mesh import _kernels, _p, oriented_bounds
+from .mesh import _kernels, _p, oriented_bounds_gpu
 
 # the reference's background classes (eval_3D_obj.py:68)
 BACKGROUND_CLS = [5, 12, 30, 31, 40, 60, 92, 93, 95, 97, 98, 79]
@@ -165,8 +165,8 @@ def calc_3d_metric(mesh_rec, mesh_gt, N: int = 200000, crop_to_gt_box: bool = Fa
     dev = _device(device)
     if crop_to_gt_box:
         gt_v = mesh_gt[0] if isinstance(mesh_gt, (tuple, list)) else mesh_gt.vertices
-        gt_v = gt_v.detach().cpu().numpy() if torch.is_tensor(gt_v) else np.asarray(gt_v)
-        center, R, ext = oriented_bounds(np.asarray(gt_v, np.float64))
+        gt_v = gt_v.detach() if torch.is_tensor(gt_v) else torch.from_numpy(np.asarray(gt_v, np.float64))
+        center, R, ext = oriented_bounds_gpu(gt_v.to(dev))
         soup = crop_to_box(mesh_rec, center, R, ext / 0.9, device=dev)
         if soup is None:
             print("no mesh found")

@@ -242,17 +242,16 @@ class sceneObject:
 
     def get_bound(self, intrinsic_open3d):
         """Oriented 3-D bound of the object (vmap.py:270-315).  The object's pixels of its first ``n_keyframes``
-        keyframes with depth > 0 are unprojected on the GPU (K5); the minimum-volume box of their convex hull is fitted
-        on the host (mesh.oriented_bounds), extents clamped to >= 0.10.  Stores a picklable utils.BoundingBox in
+        keyframes with depth > 0 are unprojected on the GPU (K5); their exact convex hull and its minimum-volume box
+        are computed there too (K8, mesh.oriented_bounds_gpu), extents clamped to >= 0.10.  Stores a picklable utils.BoundingBox in
         ``self.bbox3d`` (it goes into checkpoints) and returns an open3d OrientedBoundingBox when open3d is installed
         (train.py:367 adds it to the viewer), the BoundingBox otherwise; None when the points are too few or flat.
         ``intrinsic_open3d``: an open3d PinholeCameraIntrinsic or a 3x3 matrix."""
-        from scipy.spatial import QhullError
         from . import mesh, utils
-        pts = mesh.unproject_object(self, mesh.intrinsic_matrix(intrinsic_open3d)).cpu().numpy()
+        pts = mesh.unproject_object(self, mesh.intrinsic_matrix(intrinsic_open3d))
         try:
-            center, R, extents = mesh.oriented_bounds(pts)
-        except (QhullError, ValueError):
+            center, R, extents = mesh.oriented_bounds_gpu(pts)
+        except ValueError:
             print("too few pcs obj ")
             return None
         extents = np.maximum(extents, 0.10)                  # at least rendering 10cm (vmap.py:298-299, 306-307)
