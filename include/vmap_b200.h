@@ -492,6 +492,62 @@ typedef struct vmb_obb_args {
 
 int vmb_obb_minvol(vmb_handle* h, const vmb_obb_args* a, void* stream);
 
+/* ---- K9: view rendering of the object map (vmap_b200/render.py; the rule is in csrc/k_render.cuh) ---------------
+ * Rays [ray0, ray0 + n_rays) of a width x height camera (pixel (u, v) = ray u*height + v) are culled against up to
+ * 1024 oriented boxes, sampled inside each hit box and composited front to back.  Per pass (0 coarse, 1 fine):
+ *   vmb_render_count      pass 0 writes the hit table (nearest 16 hits per ray by (t0, source)), hit counts and the
+ *                         overflow count; both passes write src_total, the samples of the pass per source.  Pass 1
+ *                         reads zstar.  The caller reads src_total (one host sync) to size the emit buffers.
+ *   vmb_render_emit       writes the pass's samples source-major (source, ray, k): points [sum][3] (world point minus
+ *                         the source's offset, fp32), z [sum], and base[ray][hit], the first sample of each entry.
+ *                         Must follow a count with the same arguments (VMB_E_ARG otherwise).
+ *   (the caller runs vmb_forward per source on its contiguous segment: alpha [sum], colour [sum][3])
+ *   vmb_render_composite  pass 0 writes zstar (-1 = none) and surf (merged index of the surface sample, -1 = none),
+ *                         and the images when n_fine == 0; pass 1 composites coarse + fine into the images.
+ * Images are full-view [width * height] device arrays; each call writes its rays only.  VMB_E_ARG on: width or
+ * height <= 0, n_src outside [1, 1024], n_coarse < 1, n_fine < 0, fx or fy == 0, a non-finite pose / intrinsic /
+ * box, a half-extent <= 0, near < 0 or far <= near.                                                                */
+typedef struct vmb_render_args {
+  int width, height;
+  double fx, fy, cx, cy;
+  double t_wc[12];               /* camera-to-world rows 0..2 of the 4x4, row-major; host values                   */
+  double near_depth, far_depth;  /* cfg.min_depth, cfg.max_depth                                                   */
+  double surface_eps;            /* fine band half-width (cfg.surface_eps)                                         */
+  int n_src;                     /* 1..1024                                                                        */
+  const double* boxes;           /* HOST [n_src][18]: center[3], R[3][3] row-major (columns = axes), half[3], offset[3] */
+  const int* obj_id;             /* HOST [n_src] instance id written for a source's surface                       */
+  long long ray0;
+  int n_rays;
+  int n_coarse, n_fine;          /* samples per hit box; per fine band (0 = coarse only)                           */
+  int pass;                      /* 0 coarse, 1 fine                                                               */
+  int* hit_src;                  /* [n_rays][16] source index, -1 past hit_count                                   */
+  double* hit_t;                 /* [n_rays][16][2] (t0, t1)                                                       */
+  int* hit_count;                /* [n_rays]                                                                       */
+  int* overflow;                 /* count pass 0: out [1] rays with more than 16 hits                             */
+  int* src_total;                /* count: out [n_src] samples of this pass per source                            */
+  float* zstar;                  /* [n_rays] surface depth of the coarse composite, -1 = none                     */
+  int* surf;                     /* [n_rays] merged index of the coarse surface sample, -1 = none                 */
+  float* points;                 /* emit: out [sum][3]                                                             */
+  float* z;                      /* emit: out [sum]                                                                */
+  int* base;                     /* emit: out [n_rays][16]                                                         */
+  const float* z_coarse;         /* composite: the coarse pass's z, alpha [sum], colour [sum][3], base             */
+  const float* alpha_coarse;
+  const float* colour_coarse;
+  const int* base_coarse;
+  const float* z_fine;           /* composite pass 1: the same for the fine pass                                   */
+  const float* alpha_fine;
+  const float* colour_fine;
+  const int* base_fine;
+  float* depth;                  /* out [width * height]                                                           */
+  float* colour;                 /* out [width * height][3]                                                        */
+  float* opacity;                /* out [width * height]                                                           */
+  int* instance;                 /* out [width * height] obj_id of the surface source, -1 = none                   */
+} vmb_render_args;
+
+int vmb_render_count(vmb_handle* h, const vmb_render_args* a, void* stream);
+int vmb_render_emit(vmb_handle* h, const vmb_render_args* a, void* stream);
+int vmb_render_composite(vmb_handle* h, const vmb_render_args* a, void* stream);
+
 /* ---- bring-up / test hook (not part of the reference-facing surface) --------------------------- */
 /* Generic wgmma GEMM of the layer-wise wide-model path: D[M][N] = A[M][K1+K2] * B[N][K]^T, fp16 in,
  * fp32 accumulate.  a_mn/b_mn = 0: operand stored [rows][ld] with K contiguous; 1: stored [K][ld] with

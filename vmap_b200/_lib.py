@@ -158,6 +158,23 @@ class ObbArgs(C.Structure):
     ]
 
 
+class RenderArgs(C.Structure):
+    _fields_ = [
+        ("width", C.c_int), ("height", C.c_int),
+        ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double), ("t_wc", C.c_double * 12),
+        ("near_depth", C.c_double), ("far_depth", C.c_double), ("surface_eps", C.c_double),
+        ("n_src", C.c_int), ("boxes", _vp), ("obj_id", _vp), ("ray0", _ll), ("n_rays", C.c_int),
+        ("n_coarse", C.c_int), ("n_fine", C.c_int), ("pass", C.c_int),
+        ("hit_src", _vp), ("hit_t", _vp), ("hit_count", _vp), ("overflow", _vp), ("src_total", _vp),
+        ("zstar", _vp), ("surf", _vp), ("points", _vp), ("z", _vp), ("base", _vp),
+        ("z_coarse", _vp), ("alpha_coarse", _vp), ("colour_coarse", _vp), ("base_coarse", _vp),
+        ("z_fine", _vp), ("alpha_fine", _vp), ("colour_fine", _vp), ("base_fine", _vp),
+        ("depth", _vp), ("colour", _vp), ("opacity", _vp), ("instance", _vp),
+    ]
+
+
+RENDER_MAX_HITS, RENDER_MAX_SRC, RENDER_BOX = 16, 1024, 18     # VMB_RENDER_MAX_HITS, VMB_RENDER_MAX_SRC, VMB_RENDER_BOX
+
 HULL_OK, HULL_TOO_FEW, HULL_FLAT, HULL_BAD = 0, 1, 2, 3       # VMB_HULL_*
 
 EXPORTS = (
@@ -167,7 +184,7 @@ EXPORTS = (
     "vmb_mc_count", "vmb_mc_emit", "vmb_unproject",
     "vmb_clip_count", "vmb_clip_emit", "vmb_surface_sample", "vmb_nn_dist",
     "vmb_assoc_classify", "vmb_assoc_voxel", "vmb_assoc_finalize", "vmb_step_cooperative",
-    "vmb_hull", "vmb_obb_minvol",
+    "vmb_hull", "vmb_obb_minvol", "vmb_render_count", "vmb_render_emit", "vmb_render_composite",
 )
 
 _lib = None
@@ -225,6 +242,8 @@ def lib():
             getattr(L, n).argtypes = [_vp, C.POINTER(AssocArgs), _vp]
         L.vmb_hull.argtypes = [_vp, C.POINTER(HullArgs), _vp]
         L.vmb_obb_minvol.argtypes = [_vp, C.POINTER(ObbArgs), _vp]
+        for n in ("vmb_render_count", "vmb_render_emit", "vmb_render_composite"):
+            getattr(L, n).argtypes = [_vp, C.POINTER(RenderArgs), _vp]
         L.vmb_build_image.argtypes = [_vp, C.c_int, _vp, _vp, _vp]
         L.vmb_mask_counts.argtypes = [_vp, C.c_int, C.c_int, _vp, _ll, _vp, _ll, _vp, _vp]
         L.vmb_debug_gemm.argtypes = [C.c_int] * 7 + [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, C.c_int, _vp, C.c_int,

@@ -20,6 +20,7 @@
 #include "k_eval.cuh"
 #include "k_assoc.cuh"
 #include "k_hull.cuh"
+#include "k_render.cuh"
 
 struct vmb_handle {
   int device, max_obj, H, nfreq;
@@ -42,6 +43,7 @@ struct vmb_handle {
   eval3d::Workspace ws_eval;// box crop / surface sampling / nearest-neighbour scratch (grow-only)
   assoc::Workspace ws_assoc;// ScanNet association scratch (grow-only)
   hull::Workspace ws_hull;  // convex hull / minimum-volume box scratch (grow-only)
+  render::Workspace ws_render;// view rendering: source table, entry sort / scan scratch (grow-only)
   std::string err;
 };
 
@@ -173,6 +175,7 @@ void vmb_destroy(vmb_handle* h) {
   h->ws_eval.release();
   h->ws_assoc.release();
   h->ws_hull.release();
+  h->ws_render.release();
   delete h;
 }
 
@@ -980,6 +983,153 @@ int vmb_obb_minvol(vmb_handle* h, const vmb_obb_args* a, void* stream) {
   k_obb_normals<<<grid_of(cap, 256, 8 * (long long)h->n_sm), 256, 0, st>>>(q);
   k_obb_eval<<<grid_of(cap, 1, 8 * (long long)h->n_sm), NT, 0, st>>>(q);
   k_obb_pick<<<1, NT, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
+// ---- K9: view rendering (ray / box cull, sample emission, compositing) -----------------------------
+static bool finite_all(const double* v, int n) {
+  for (int i = 0; i < n; ++i)
+    if (!std::isfinite(v[i])) return false;
+  return true;
+}
+
+// checks shared by the three render entry points; fills the geometry part of q and uploads the source table
+static int render_params(vmb_handle* h, const vmb_render_args* a, render::Params& q, const char* who) {
+  const std::string w(who);
+  if (!h || !a) return fail(h, VMB_E_ARG, w + ": null argument");
+  if (a->width <= 0 || a->height <= 0) return fail(h, VMB_E_ARG, w + ": width and height must be >= 1");
+  if (a->n_src < 1 || a->n_src > VMB_RENDER_MAX_SRC) return fail(h, VMB_E_ARG, w + ": n_src must be in [1, 1024]");
+  if (a->n_coarse < 1 || a->n_fine < 0) return fail(h, VMB_E_ARG, w + ": need n_coarse >= 1 and n_fine >= 0");
+  if (a->pass != 0 && a->pass != 1) return fail(h, VMB_E_ARG, w + ": pass must be 0 or 1");
+  if (a->pass == 1 && a->n_fine == 0) return fail(h, VMB_E_ARG, w + ": pass 1 needs n_fine >= 1");
+  const double intr[4] = {a->fx, a->fy, a->cx, a->cy};
+  if (!finite_all(intr, 4) || a->fx == 0.0 || a->fy == 0.0)
+    return fail(h, VMB_E_ARG, w + ": intrinsics must be finite with fx, fy != 0");
+  if (!finite_all(a->t_wc, 12)) return fail(h, VMB_E_ARG, w + ": non-finite pose");
+  if (!std::isfinite(a->near_depth) || !(a->near_depth >= 0.0) || !(a->far_depth > a->near_depth) ||
+      std::isnan(a->far_depth))
+    return fail(h, VMB_E_ARG, w + ": need 0 <= near < far");
+  if (a->n_fine > 0 && !(std::isfinite(a->surface_eps) && a->surface_eps > 0.0))
+    return fail(h, VMB_E_ARG, w + ": surface_eps must be finite and > 0");
+  const long long n_pix = (long long)a->width * a->height;
+  if (a->n_rays < 1 || a->ray0 < 0 || a->ray0 + a->n_rays > n_pix)
+    return fail(h, VMB_E_ARG, w + ": rays [ray0, ray0 + n_rays) must lie inside the view");
+  const long long n_e = (long long)a->n_rays * VMB_RENDER_MAX_HITS;
+  if (n_e * std::max(a->n_coarse, a->n_fine) >= 0x7fffffffLL)
+    return fail(h, VMB_E_ARG, w + ": n_rays * 16 * max(n_coarse, n_fine) exceeds int32 sample indices");
+  if (!a->boxes || !a->obj_id) return fail(h, VMB_E_ARG, w + ": boxes / obj_id missing");
+  for (int s = 0; s < a->n_src; ++s) {
+    const double* b = a->boxes + (size_t)s * VMB_RENDER_BOX;
+    if (!finite_all(b, VMB_RENDER_BOX)) return fail(h, VMB_E_ARG, w + ": non-finite box");
+    if (!(b[12] > 0.0 && b[13] > 0.0 && b[14] > 0.0)) return fail(h, VMB_E_ARG, w + ": box half-extents must be > 0");
+  }
+  if (!a->hit_src || !a->hit_t || !a->hit_count) return fail(h, VMB_E_ARG, w + ": hit table missing");
+  memset(&q, 0, sizeof(q));
+  q.W = a->width; q.H = a->height;
+  q.fx = a->fx; q.fy = a->fy; q.cx = a->cx; q.cy = a->cy;
+  for (int i = 0; i < 12; ++i) q.T[i] = a->t_wc[i];
+  q.near_ = a->near_depth; q.far_ = a->far_depth; q.eps = a->surface_eps;
+  q.n_src = a->n_src; q.ray0 = a->ray0; q.n_rays = a->n_rays;
+  q.n_coarse = a->n_coarse; q.n_fine = a->n_fine; q.pass = a->pass;
+  q.hit_src = a->hit_src; q.hit_t = a->hit_t; q.hit_count = a->hit_count;
+  q.overflow = a->overflow; q.src_total = a->src_total; q.zstar = a->zstar; q.surf = a->surf;
+  render::Workspace& ws = h->ws_render;
+  CUDA_TRY(h, render::Workspace::grow((void**)&ws.boxes, &ws.boxes_cap, (size_t)a->n_src * VMB_RENDER_BOX * sizeof(double)));
+  CUDA_TRY(h, render::Workspace::grow((void**)&ws.obj_id, &ws.id_cap, (size_t)a->n_src * sizeof(int)));
+  q.boxes = ws.boxes; q.obj_id = ws.obj_id;
+  return VMB_OK;
+}
+
+static int render_upload(vmb_handle* h, const vmb_render_args* a, cudaStream_t st) {
+  render::Workspace& ws = h->ws_render;
+  CUDA_TRY(h, cudaMemcpyAsync(ws.boxes, a->boxes, (size_t)a->n_src * VMB_RENDER_BOX * sizeof(double),
+                              cudaMemcpyHostToDevice, st));
+  CUDA_TRY(h, cudaMemcpyAsync(ws.obj_id, a->obj_id, (size_t)a->n_src * sizeof(int), cudaMemcpyHostToDevice, st));
+  return VMB_OK;
+}
+
+static bool render_same(const render::Params& x, const render::Params& y) {
+  return x.pass == y.pass && x.ray0 == y.ray0 && x.n_rays == y.n_rays && x.n_src == y.n_src && x.W == y.W &&
+         x.H == y.H && x.n_coarse == y.n_coarse && x.n_fine == y.n_fine && x.hit_src == y.hit_src &&
+         x.hit_t == y.hit_t && x.hit_count == y.hit_count && x.zstar == y.zstar && x.eps == y.eps &&
+         x.fx == y.fx && x.fy == y.fy && x.cx == y.cx && x.cy == y.cy && !memcmp(x.T, y.T, sizeof(x.T));
+}
+
+int vmb_render_count(vmb_handle* h, const vmb_render_args* a, void* stream) {
+  render::Params q;
+  int rc = render_params(h, a, q, "vmb_render_count");
+  if (rc != VMB_OK) return rc;
+  if (!a->overflow || !a->src_total) return fail(h, VMB_E_ARG, "vmb_render_count: overflow / src_total missing");
+  if (a->pass == 1 && !a->zstar) return fail(h, VMB_E_ARG, "vmb_render_count: pass 1 needs zstar");
+  cudaStream_t st = (cudaStream_t)stream;
+  if ((rc = render_upload(h, a, st)) != VMB_OK) return rc;
+  render::Workspace& ws = h->ws_render;
+  const long long n_e = (long long)q.n_rays * VMB_RENDER_MAX_HITS;
+  const size_t n1 = (size_t)n_e + 1;
+  CUDA_TRY(h, render::Workspace::grow((void**)&ws.ints, &ws.ints_cap, 7 * n1 * sizeof(int)));
+  q.keys = ws.ints; q.keys_alt = q.keys + n1; q.vals = q.keys_alt + n1; q.vals_alt = q.vals + n1;
+  q.cnt = q.vals_alt + n1;
+  int* scan = q.cnt + n1;
+  q.wbase = scan + n1;
+  if (q.pass == 0) {
+    CUDA_TRY(h, cudaMemsetAsync(q.overflow, 0, sizeof(int), st));
+    render::k_cull<<<render::blocks_for(q.n_rays, 128), 128, 0, st>>>(q);
+    CUDA_TRY(h, cudaGetLastError());
+  }
+  CUDA_TRY(h, cudaMemsetAsync(q.src_total, 0, (size_t)q.n_src * sizeof(int), st));
+  render::k_entry_counts<<<render::blocks_for(n_e + 1, 256), 256, 0, st>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  // stable sort of the entries by source: the source-major sample order (ties keep ray order)
+  size_t need = 0, need_scan = 0;
+  CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(nullptr, need, q.keys, q.keys_alt, q.vals, q.vals_alt, (int)n_e, 0, 11, st));
+  CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(nullptr, need_scan, scan, (int)n1, st));
+  CUDA_TRY(h, render::Workspace::grow(&ws.cub_tmp, &ws.cub_cap, std::max(need, need_scan)));
+  CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(ws.cub_tmp, need, q.keys, q.keys_alt, q.vals, q.vals_alt, (int)n_e, 0, 11, st));
+  render::k_gather_counts<<<render::blocks_for(n_e + 1, 256), 256, 0, st>>>(q, q.vals_alt, q.cnt, scan);
+  CUDA_TRY(h, cudaGetLastError());
+  CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(ws.cub_tmp, need_scan, scan, (int)n1, st));
+  render::k_scatter_base<<<render::blocks_for(n_e, 256), 256, 0, st>>>(q, q.vals_alt, scan, q.wbase);
+  CUDA_TRY(h, cudaGetLastError());
+  ws.last = q;
+  ws.counted = true;
+  return VMB_OK;
+}
+
+int vmb_render_emit(vmb_handle* h, const vmb_render_args* a, void* stream) {
+  render::Params q;
+  const int rc = render_params(h, a, q, "vmb_render_emit");
+  if (rc != VMB_OK) return rc;
+  render::Workspace& ws = h->ws_render;
+  if (!ws.counted || !render_same(q, ws.last))
+    return fail(h, VMB_E_ARG, "vmb_render_emit: no matching vmb_render_count on this handle (same rays, pass and tables)");
+  if (!a->points || !a->z || !a->base) return fail(h, VMB_E_ARG, "vmb_render_emit: points / z / base missing");
+  q.wbase = ws.last.wbase;
+  q.points = a->points; q.z = a->z; q.base = a->base;
+  const long long n_e = (long long)q.n_rays * VMB_RENDER_MAX_HITS;
+  render::k_emit<<<render::blocks_for(n_e, 128), 128, 0, (cudaStream_t)stream>>>(q);
+  CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
+int vmb_render_composite(vmb_handle* h, const vmb_render_args* a, void* stream) {
+  render::Params q;
+  int rc = render_params(h, a, q, "vmb_render_composite");
+  if (rc != VMB_OK) return rc;
+  const bool images = a->pass == 1 || a->n_fine == 0;
+  if (!a->z_coarse || !a->alpha_coarse || !a->colour_coarse || !a->base_coarse)
+    return fail(h, VMB_E_ARG, "vmb_render_composite: coarse samples missing");
+  if (a->pass == 1 && (!a->z_fine || !a->alpha_fine || !a->colour_fine || !a->base_fine))
+    return fail(h, VMB_E_ARG, "vmb_render_composite: fine samples missing");
+  if (!a->zstar || (a->pass == 0 && !a->surf)) return fail(h, VMB_E_ARG, "vmb_render_composite: zstar / surf missing");
+  if (images && (!a->depth || !a->colour || !a->opacity || !a->instance))
+    return fail(h, VMB_E_ARG, "vmb_render_composite: output images missing");
+  cudaStream_t st = (cudaStream_t)stream;
+  if ((rc = render_upload(h, a, st)) != VMB_OK) return rc;
+  q.z_c = a->z_coarse; q.alpha_c = a->alpha_coarse; q.colour_c = a->colour_coarse; q.base_c = a->base_coarse;
+  q.z_f = a->z_fine; q.alpha_f = a->alpha_fine; q.colour_f = a->colour_fine; q.base_f = a->base_fine;
+  q.depth = a->depth; q.colour = a->colour; q.opacity = a->opacity; q.instance = a->instance;
+  render::k_composite<<<render::blocks_for(q.n_rays, 128), 128, 0, st>>>(q);
   CUDA_TRY(h, cudaGetLastError());
   return VMB_OK;
 }

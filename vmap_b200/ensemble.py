@@ -259,14 +259,15 @@ class VmapEnsemble:
         return out["depth"], out["var"], out["colour"], out["opacity"]
 
     def eval_points(self, points: torch.Tensor, impl: Optional[str] = None, row: Optional[int] = None,
-                    chunk: int = 1 << 21):
+                    chunk: int = 1 << 21, out=None):
         """Forward only on raw points -> alpha (raw*10, model.py:77), colour (trainer.py:77-90).
         ``row=None``: points [B,N,3], every object evaluates its own set -> alpha [B,N], colour [B,N,3].
         ``row=r``: points [N,3] evaluated by object r ONLY (one-row views of the packed state are handed to
         ``vmb_forward`` with n_obj = 1, so meshing one object of a 160-object stack costs one object's work)
         -> alpha [N], colour [N,3].  ``chunk`` bounds the points per launch (the reference uses 100k chunks).
         ``impl="fp32"`` forces the CUDA-core kernel; otherwise hidden 32 runs the forward half of the fused
-        wgmma kernel and hidden 64/128/256 the layer-wise wgmma GEMMs, on the fp16 weight image."""
+        wgmma kernel and hidden 64/128/256 the layer-wise wgmma GEMMs, on the fp16 weight image.
+        ``out=(alpha, colour)``: contiguous fp32 device tensors of the result's shape to write into (and return)."""
         if row is None:
             B, N, _ = points.shape
             assert B == self.n_obj
@@ -278,8 +279,13 @@ class VmapEnsemble:
             params, scale = self.params[row:row + 1], self.scale[row:row + 1]
             image = self.image[row:row + 1] if self.image is not None else None
         assert points.is_contiguous() and points.dtype == torch.float32 and points.device == self.device
-        alpha = torch.empty(B, N, dtype=torch.float32, device=self.device)
-        colour = torch.empty(B, N, 3, dtype=torch.float32, device=self.device)
+        if out is None:
+            alpha = torch.empty(B, N, dtype=torch.float32, device=self.device)
+            colour = torch.empty(B, N, 3, dtype=torch.float32, device=self.device)
+        else:
+            alpha, colour = out[0].view(B, N), out[1].view(B, N, 3)
+            for t in (alpha, colour):
+                assert t.is_contiguous() and t.dtype == torch.float32 and t.device == self.device
         use_image = (impl or self.impl) != "fp32" and image is not None
         with torch.cuda.device(self.device):
             for n0 in range(0, N, chunk):

@@ -333,3 +333,29 @@ def frame_obj_ids(mesh_dir, frame: int) -> List[int]:
     """Object ids of the ``frame_{frame}_obj{id}.obj`` files train.py wrote into ``mesh_dir``, ascending."""
     pat = re.compile(r"^frame_%d_obj(\d+)\.obj$" % int(frame))
     return sorted(int(m.group(1)) for m in (pat.match(f) for f in os.listdir(mesh_dir)) if m)
+
+
+def view_metrics(colour, depth, gt_rgb, gt_depth, gt_inst=None) -> dict:
+    """2-D view metrics of a rendered view (vmap_b200.render.render_view) against ground truth, all images [W, H, ...].
+    The reference never published its eval_2D_view.py, so these definitions are the package's own:
+      psnr      over all pixels, colours in [0, 1], MSE in fp64;
+      depth_l1  mean |depth - gt| in metres over pixels with gt > 0 (nan when there are none);
+      obj_psnr  (with ``gt_inst``) the mean over GT instances != 0 of each instance's PSNR over its pixels."""
+    c = torch.as_tensor(colour).double()
+    g = torch.as_tensor(gt_rgb).double().to(c.device)
+    d = torch.as_tensor(depth).double().to(c.device)
+    gd = torch.as_tensor(gt_depth).double().to(c.device)
+
+    def psnr(mse):
+        return float(-10.0 * torch.log10(mse)) if float(mse) > 0 else float("inf")
+
+    se = ((c - g) ** 2).mean(-1)
+    out = {"psnr": psnr(se.mean())}
+    valid = gd > 0
+    out["depth_l1"] = float((d - gd).abs()[valid].mean()) if bool(valid.any()) else float("nan")
+    if gt_inst is not None:
+        gi = torch.as_tensor(gt_inst).to(c.device)
+        ids = [int(i) for i in torch.unique(gi).tolist() if int(i) != 0]
+        vals = [psnr(se[gi == i].mean()) for i in ids]
+        out["obj_psnr"] = float(np.mean(vals)) if vals else float("nan")
+    return out
