@@ -107,7 +107,7 @@ def unidir_embed(pcs: torch.Tensor, dirs: torch.Tensor, scale: torch.Tensor,
     B, R, S, _ = pcs.shape
     t = (pcs / scale.view(B, 1, 1, 1)).reshape(B, R * S, 3)                 # :83
     proj = _blinear(t, dirs, None)                                            # :84
-    freqs = 2.0 ** torch.linspace(0, max_deg, max_deg + 1, dtype=pcs.dtype)   # :78
+    freqs = 2.0 ** torch.linspace(0, max_deg, max_deg + 1, dtype=pcs.dtype, device=pcs.device)   # :78
     bands = proj.unsqueeze(-2) * freqs.view(1, 1, -1, 1)                      # :85
     feat = torch.sin(bands.reshape(B, R * S, -1) * math.pi)                   # :86-88
     return torch.cat([t, feat], dim=-1).reshape(B, R, S, -1)                  # :89
