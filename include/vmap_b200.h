@@ -212,7 +212,7 @@ typedef struct vmb_sample_args {
   const float* inj_u_w; const float* inj_u_h;   /* optional [B][n_frames][n_pix]           */
   const float* inj_u_z;                 /* optional [B][N][S]                              */
   const float* inj_nrm;                 /* optional [B][N][n2]  (already scaled by eps/3)  */
-  /* outputs, N = n_frames*n_pix rays per object                                           */
+  /* outputs, N = n_frames*n_pix rays per object (N < 2^29, VMB_E_ARG otherwise)            */
   float* pcs;                /* [B][N][S][3]                                               */
   float* z_vals;             /* [B][N][S]                                                  */
   float* gt_depth;           /* [B][N]                                                     */

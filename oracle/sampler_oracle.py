@@ -86,12 +86,18 @@ def draw_randoms_reference_order(gen: Optional[torch.Generator], n_keyframes: in
     return {"kf": kf, "u_w": u_w, "u_h": u_h, "u_z": u_z, "nrm": nrm}
 
 
-def pixel_indices(kf: torch.Tensor, u_w: torch.Tensor, u_h: torch.Tensor, bbox: torch.Tensor):
+def pixel_indices(kf: torch.Tensor, u_w: torch.Tensor, u_h: torch.Tensor, bbox: torch.Tensor, wh=None):
     """Uniforms -> integer pixel coordinates inside the keyframe's 2-D box
-    (vmap.py:346-351): fp32 ``u*(hi-lo)+lo`` then truncation."""
+    (vmap.py:346-351): fp32 ``u*(hi-lo)+lo`` then truncation.  ``wh`` = (W, H):
+    clamp to [0, W-1] x [0, H-1] as the CUDA sampler does for boxes that reach
+    past the image.  The reference does not clamp: past the high border it indexes
+    out of range, past the low border torch wraps the negative index to the
+    opposite edge."""
     b = bbox[kf]                                   # [n_frames, 4] = u_lo,u_hi,v_lo,v_hi
     iw = (u_w * (b[:, 1] - b[:, 0])[:, None] + b[:, 0][:, None]).long()
     ih = (u_h * (b[:, 3] - b[:, 2])[:, None] + b[:, 2][:, None]).long()
+    if wh is not None:
+        iw, ih = iw.clamp(0, wh[0] - 1), ih.clamp(0, wh[1] - 1)
     return iw, ih
 
 
@@ -114,7 +120,7 @@ def sample_from_randoms(rnd: Dict[str, torch.Tensor], rgbs_batch: torch.Tensor,
     F_, P_ = u_w.shape
     n1, n2 = cfg.n_bins_cam2surface, cfg.n_bins
     eps, oeps = cfg.surface_eps, cfg.stop_eps
-    iw, ih = pixel_indices(kf, u_w, u_h, bbox)
+    iw, ih = pixel_indices(kf, u_w, u_h, bbox, wh=rgbs_batch.shape[1:3])
     px = rgbs_batch[kf[:, None], iw, ih]                     # [F,P,4] u8      :353
     depth = depth_batch[kf[:, None], iw, ih]                 # [F,P]           :354
     dirs_c = rays_dir[iw, ih]                                # [F,P,3]         :357

@@ -9,8 +9,17 @@
 //
 // Index / bin arithmetic uses explicit round-to-nearest mul/add (no FMA contraction) so
 // that with injected randoms the integer outputs and z are bit-identical to torch's
-// separate fp32 ops.  Randoms come from Philox4x32-10 counters keyed by
-// (seed, object, stream, ray) unless injected.
+// separate fp32 ops.  Randoms come from Philox4x32-10 unless injected: key (k0, k1) = (low, high 32 bits of seed),
+// counter (c0, c1, c2, c3) = (index, stream, object b of the launch, low 32 bits of offset), with
+//   stream 0: c0 = keyframe draw f,    word 0 -> kf (only when n_kf <= 2 or f < n_frames - 2)
+//   stream 1: c0 = ray i,              words 0, 1 -> u_w, u_h
+//   stream 2: c0 = i * 8 + chunk c,    words 0-3 -> u_z[4c .. 4c+3]
+//   stream 3: c0 = i * 8 + chunk c,    words 0-3 -> Box-Muller normals 4c .. 4c+3 (this-object rays only)
+// so counters are distinct while S <= 32 (c < 8) and N < 2^29 (vmb_sample checks both).  Offsets past 2^32 repeat
+// the draws of offset mod 2^32.  The surface sampler of k_eval.cuh draws counter (i, i >> 32, 4, 0): with the same
+// seed that is this kernel's stream 0 of object 4 at offset 0, which is harmless (unrelated uses).
+// oracle/philox_oracle.py restates
+// the draws bit for bit (tests/test_sampler_philox.py, tests/test_sampler_exact_gpu.py).
 #pragma once
 #include "common.cuh"
 

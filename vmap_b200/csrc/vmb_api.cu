@@ -444,6 +444,8 @@ int vmb_sample(vmb_handle* h, const vmb_sample_args* a, void* stream) {
     return fail(h, VMB_E_ARG, "vmb_sample: bad arguments");
   if (a->n_bins_cam2surface < 1 || a->n_bins < 1 || a->n_bins_cam2surface + a->n_bins > 32)
     return fail(h, VMB_E_ARG, "vmb_sample: need 1 <= n1, n2 and n1+n2 <= 32");
+  if ((long long)a->n_frames * a->n_pix >= (1LL << 29))      // Philox counter word 0 is ray * 8 + chunk (k_sampler.cuh)
+    return fail(h, VMB_E_ARG, "vmb_sample: need n_frames * n_pix < 2^29 rays per object");
   const bool shared = a->store_rgbx != nullptr;
   if (shared && (!a->store_depth || !a->store_inst || !a->store_t_wc || !a->kf_slot || !a->kf_bbox || !a->obj_id ||
                  a->kf_stride <= 0))
