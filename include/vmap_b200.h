@@ -127,11 +127,6 @@ typedef struct vmb_step_args {
 
 int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream);
 
-/* 1 when a hidden-32 training step on `device` finishes cooperatively (all CTAs share the gradient reduction and
- * AdamW), 0 when each object's last CTA does it: the device lacks cooperative launch or VMB_NO_COOP is set.
- * Both give the same bits; the environment variable is read at every call and every step.                 */
-int vmb_step_cooperative(int device);
-
 /* Mask counts only (the normalisers of render_rays.py:68,86): out[B][4] int.
  * Exposed separately so that a ray-sharded run can all-reduce them before vmb_step.       */
 int vmb_mask_counts(vmb_handle* h, int n_obj, int n_rays,

@@ -283,19 +283,11 @@ def rays(batch, sl):
     return {k: v[:, sl] for k, v in batch.items()}
 
 
-@pytest.mark.parametrize("coop", ["cooperative", "fallback"])
 @pytest.mark.parametrize("case", ["unaligned_rows", "counts_in", "empty_object"])
-def test_edges(case, coop, monkeypatch):
-    """Label / mask rows that are not 4-byte aligned (an odd ray count and a slice starting at ray 1: the non-vector
-    count path), mask counts supplied from outside, and an object without object rays (the any-empty early-out turns
-    L_depth and L_colour off for every object), under the cooperative and the VMB_NO_COOP fallback finish."""
-    from vmap_b200 import _lib
-    if coop == "fallback":
-        monkeypatch.setenv("VMB_NO_COOP", "1")
-    else:
-        monkeypatch.delenv("VMB_NO_COOP", raising=False)
-        if not _lib.lib().vmb_step_cooperative(torch.cuda.current_device()):
-            pytest.skip("no cooperative launch on this device")
+def test_edges(case):
+    """Label / mask rows that are not 4-byte aligned (an odd ray count and a slice starting at ray 1: the scalar count
+    loop), mask counts supplied from outside, and an object without object rays (the any-empty early-out turns
+    L_depth and L_colour off for every object)."""
     params, db, ens = setup(5, 131, 10, 44)
     counts = None
     if case == "unaligned_rows":
@@ -306,7 +298,7 @@ def test_edges(case, coop, monkeypatch):
         counts = ens.mask_counts(full)
     else:
         db["sem"][2] = 0
-    check(ens, params, db, counts=counts, label=f"{case}, {coop} finish")
+    check(ens, params, db, counts=counts, label=case)
     if case == "empty_object":
         assert float(ens.loss_terms[:, :2].abs().max()) == 0.0
 

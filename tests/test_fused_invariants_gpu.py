@@ -4,8 +4,8 @@ guard on every path.
 The oracle bars of test_umma_gpu.py / test_baseline_configs_gpu.py must absorb fp16-operand noise and L1 sign flips,
 so a lost or double-counted tile, or a CTA's gradient partial reduced into the wrong row, stays inside them
 (test_dropped_tile_is_rejected shows it). Here the kernel is compared with itself where the exact answer is known:
-splitting the rays of a batch, permuting them, running an object alone, accumulating twice, and the cooperative vs the
-fallback finish. The only difference left is the fp32 reassociation of the per-CTA gradient partials, so the bars are
+splitting the rays of a batch, permuting them, running an object alone, accumulating twice, and training the same
+ensemble twice. The only difference left is the fp32 reassociation of the per-CTA gradient partials, so the bars are
 per object and per tensor. AdamW is compared per object with torch.optim.AdamW in fp64, at step numbers on both sides
 of the bias-correction table's edge. Run with -s to see every measured value next to its bar."""
 import pytest
@@ -227,7 +227,7 @@ def test_dropped_tile_is_rejected():
     assert worst_stack < 4e-2 and worst_cos > 0.999 and worst_obj < 0.6
 
 
-# ---- cooperative vs fallback finish --------------------------------------------------------------------------------------
+# ---- reproducible finish -------------------------------------------------------------------------------------------------
 
 def make_explode(params, batch, b):
     """Object b's depth loss exceeds 1e5: occupancy 1 at the first sample -> zero variance -> info weight 1e4."""
@@ -243,15 +243,10 @@ def explode_batch(batch, b):
 
 
 @pytest.mark.parametrize("explode", [False, True], ids=["clean", "object2_explodes"])
-def test_cooperative_and_fallback_finish_agree_bitwise(explode, monkeypatch):
-    """VMB_NO_COOP=1 selects the non-cooperative finish (the last CTA of each object reduces and updates it). Both
-    reduce the partial rows in segment order, so 50 steps must give identical bits."""
-    from vmap_b200 import _lib
+def test_finish_is_bitwise_reproducible(explode):
+    """The grid-wide finish reduces the partial rows in segment order, whichever CTA reaches the grid barrier first,
+    so two fresh ensembles trained for 50 steps on the same batches end with identical bits."""
     from vmap_b200.ensemble import LossExplode
-    dev = torch.cuda.current_device()
-    monkeypatch.delenv("VMB_NO_COOP", raising=False)
-    if not _lib.lib().vmb_step_cooperative(dev):
-        pytest.skip("the device has no cooperative launch: both runs would take the fallback finish")
     B, R, S = 7, 301, 10
     params = vo.init_params(B, 32, seed=3)
     batches = [vo.synthetic_batch(B, R, S, seed=50 + i) for i in range(4)]
@@ -260,31 +255,25 @@ def test_cooperative_and_fallback_finish_agree_bitwise(explode, monkeypatch):
         for bt in batches[1:]:
             explode_batch(bt, 2)
     batches = [to_dev(bt) for bt in batches]
-    runs = {}
-    for mode in ("cooperative", "fallback"):
-        if mode == "fallback":
-            monkeypatch.setenv("VMB_NO_COOP", "1")
-        else:
-            monkeypatch.delenv("VMB_NO_COOP", raising=False)
-        assert _lib.lib().vmb_step_cooperative(dev) == (mode == "cooperative")
+    runs = []
+    for _ in range(2):
         ens = make_ensemble(params, 2.0, 32, impl="umma")
         losses = torch.stack([ens.step(batches[it % 4]) for it in range(50)])
         torch.cuda.synchronize()
-        runs[mode] = dict(params=ens.params.clone(), exp_avg=ens.exp_avg.clone(), exp_avg_sq=ens.exp_avg_sq.clone(),
-                          image=ens.image.clone(), step_counter=ens.step_counter.clone(),
-                          loss_terms=ens.loss_terms.clone(), losses=losses)
+        runs.append(dict(params=ens.params.clone(), exp_avg=ens.exp_avg.clone(), exp_avg_sq=ens.exp_avg_sq.clone(),
+                         image=ens.image.clone(), step_counter=ens.step_counter.clone(),
+                         loss_terms=ens.loss_terms.clone(), losses=losses))
         if explode:
             with pytest.raises(LossExplode):
                 ens.check_status()
         else:
             ens.check_status()
-    monkeypatch.delenv("VMB_NO_COOP", raising=False)
-    for k, v in runs["cooperative"].items():
-        assert torch.equal(v, runs["fallback"][k]), k
+    for k, v in runs[0].items():
+        assert torch.equal(v, runs[1][k]), k
     want = torch.full((B,), 50, dtype=torch.int32, device="cuda")
     if explode:
         want[2] = 0
-    assert torch.equal(runs["cooperative"]["step_counter"], want)
+    assert torch.equal(runs[0]["step_counter"], want)
 
 
 # ---- per-object AdamW state ----------------------------------------------------------------------------------------------

@@ -183,7 +183,7 @@ EXPORTS = (
     "vmb_build_image", "vmb_forward", "vmb_sample", "vmb_ingest_frame", "vmb_debug_gemm",
     "vmb_mc_count", "vmb_mc_emit", "vmb_unproject",
     "vmb_clip_count", "vmb_clip_emit", "vmb_surface_sample", "vmb_nn_dist",
-    "vmb_assoc_classify", "vmb_assoc_voxel", "vmb_assoc_finalize", "vmb_step_cooperative",
+    "vmb_assoc_classify", "vmb_assoc_voxel", "vmb_assoc_finalize",
     "vmb_hull", "vmb_obb_minvol", "vmb_render_count", "vmb_render_emit", "vmb_render_composite",
 )
 
@@ -222,7 +222,6 @@ def lib():
             getattr(L, n).argtypes = [C.c_int, C.c_int]
             getattr(L, n).restype = C.c_int
         L.vmb_param_offsets.argtypes = [C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-        L.vmb_step_cooperative.argtypes = [C.c_int]
         L.vmb_create.argtypes = [C.POINTER(_vp), C.c_int, C.c_int, C.c_int, C.c_int]
         L.vmb_destroy.argtypes = [_vp]
         L.vmb_destroy.restype = None

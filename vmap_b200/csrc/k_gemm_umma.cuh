@@ -45,14 +45,9 @@ enum Epi { EPI_RELU_F16 = 0, EPI_GATE_F16 = 1, EPI_F32 = 2, EPI_ATOMIC = 3 };
 // Host side of programmatic dependent launch.  The orchestrator arms `t_pdl_next` right before a launch that directly
 // follows another kernel of the chain on the same stream; `launch_k` consumes it.  Every kernel of the layer-wise path
 // executes `ptx::pdl_wait()` before it touches anything its predecessor wrote, so an armed launch only overlaps its
-// prologue (and the launch latency itself) with the predecessor's tail.  VMB_NO_PDL=1 turns it off.
+// prologue (and the launch latency itself) with the predecessor's tail.
 static thread_local bool t_pdl_next = false;
-static bool pdl_enabled() {
-  static int on = -1;
-  if (on < 0) on = getenv("VMB_NO_PDL") == nullptr ? 1 : 0;
-  return on == 1;
-}
-static inline void pdl_arm() { t_pdl_next = pdl_enabled(); }
+static inline void pdl_arm() { t_pdl_next = true; }
 template <typename... KArgs, typename... Args>
 static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
   cudaLaunchConfig_t cfg = {};

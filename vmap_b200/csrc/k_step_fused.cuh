@@ -18,9 +18,10 @@
 //     (dYc->Z, dY4->HC, dY3->FC4, dY2->HC, dY1->FC3);
 //   * both head weight gradients and both head bias gradients come out of ONE wgrad ([fc4 | emb2 | hc] x dhead);
 //   * the PE-direction gradient dB = dproj^T [x y z] is a wgrad MMA too;
-//   * K0 (mask counts) runs in the prologue, K2 (AdamW) in the last CTA to finish an object: every (CTA, object)
-//     segment writes its gradient partial to its own row, the finisher adds the rows in segment order (bitwise
-//     reproducible -- no floating-point atomics anywhere) and applies AdamW exactly as k_adamw does.
+//   * K0 (mask counts) runs in the prologue, K2 (AdamW) after a grid barrier: every (CTA, object) segment writes its
+//     gradient partial to its own row, then the whole grid splits the reduction of all objects' rows, adds each
+//     object's rows in segment order (bitwise reproducible -- no floating-point atomics anywhere) and applies AdamW
+//     exactly as k_adamw does.  Training launches are cooperative: the grid barrier needs every CTA resident.
 //
 // Reference arithmetic: embedding.py:82-91, model.py:54-85, render_rays.py:4-96, loss.py:5-62, their autograd
 // backward (train.py:293-324) and torch.optim.AdamW.step + zero_grad (train.py:325-326).
@@ -34,10 +35,11 @@
 
 struct FusedExtra {
   float* partials;            // [(B + grid)][stride] per-(CTA, object) gradient partials, row = blockIdx + object
-  unsigned int* obj_done;     // [B] segments finished per object (non-cooperative), [B] skip flags, [2] grid arrive / depart (self-resetting)
+  unsigned int* finish_sync;  // [6] grid-barrier words (self-resetting), then [B] skip flags: the words' place must not
+                              // depend on B, or a launch with fewer objects would find a skip flag in them
   const int* counts_in;       // optional [B][4] external mask counts (ray-sharded iMAP: all-reduced by the caller)
-  int* counts_pub;            // [B][4] scratch: cooperative launches count each object ONCE (CTA b mod grid) and publish here
-  int fuse_adam;              // 1: the finisher applies AdamW; 0: it adds the reduced gradient into `grads`
+  int* counts_pub;            // [B][4] scratch: otherwise CTA c counts objects c, c + grid, ... ONCE and publishes here
+  int fuse_adam;              // 1: the grid-wide finish applies AdamW; 0: it adds the reduced gradient into `grads`
   float* p; float* m; float* v;
   __half* image_out; const int* img_index; int img_halves;
   int* step_counter;          // optional [B] device step numbers (t = counter + 1, incremented here)
@@ -49,7 +51,6 @@ struct FusedExtra {
   float lr_wd, one_m_b1, b2, one_m_b2, eps;
   int guard_loss;
   int* status;
-  int cooperative;            // 1: cooperative launch (all CTAs resident): an object's CTAs share its reduction + update
   float* loss_sum;            // optional: sum over objects of the weighted loss totals, written by the last CTA to leave
 };
 
@@ -194,12 +195,11 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     ptx::bulk_g2s(smem + SM_W, image + (size_t)(gt_begin / npo) * um::IMG_BYTES, um::IMG_BYTES, &misc->wbar);
   }
   // ---- K0 in the prologue: mask counts of EVERY object (the any-empty early-out couples them, render_rays.py:68-73).
-  // Cooperative launch: CTA c counts objects c, c + grid, ... ONCE and publishes counts + empty flags + a "published"
-  // counter in global memory; every CTA starts its tiles at once and acquires the counts right before its first
-  // volume render (thousands of cycles later: the wait is free).  Otherwise every CTA counts everything (every CTA
-  // reads all the label / mask bytes).
-  const bool pub_counts = x.cooperative && !x.counts_in && !a.fwd_only;
-  unsigned int* gbar = x.obj_done + 2 * a.B;            // [0] arrive, [1] depart, [2] objects published, [3..5] empty flags
+  // Training launch without counts_in: CTA c counts objects c, c + grid, ... ONCE and publishes counts + empty flags +
+  // a "published" counter in global memory; every CTA starts its tiles at once and acquires the counts right before
+  // its first volume render (thousands of cycles later: the wait is free).  With counts_in, every CTA copies them.
+  const bool pub_counts = !x.counts_in && !a.fwd_only;
+  unsigned int* gbar = x.finish_sync;                   // [0] arrive, [1] depart, [2] objects published, [3..5] empty flags
   if (pub_counts) {
     for (int b = blockIdx.x; b < a.B; b += G) {
       if (tid < 3) cnt[tid] = 0;
@@ -208,6 +208,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       const unsigned char* m = a.mask + (size_t)b * a.mask_stride;
       const bool vec = (((size_t)s | (size_t)m) & 3) == 0;
       const int nw = vec ? (R >> 2) : 0;
+      // one bit per byte: nonzero(x) folds a byte's bits into bit 0 (labels are 0 / 1 / 2, masks any nonzero = true)
       auto nzb = [](uint32_t v) { v |= v >> 4; v |= v >> 2; v |= v >> 1; return v & 0x01010101u; };
       int nd = 0, no = 0, ns = 0;
       for (int w = tid; w < nw; w += NT) {               // four rays per 32-bit load
@@ -235,71 +236,11 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       }
       __syncthreads();
     }
-  } else if (!a.fwd_only) {
-    if (x.counts_in) {
-      for (int i = tid; i < a.B * 3; i += NT) {
-        const int c = x.counts_in[(i / 3) * 4 + (i % 3)];
-        cnt[i] = c;
-        if (c == 0) misc->on[i % 3] = 0;
-      }
-    } else {
-      // warp w counts objects w, w + NT/32, ...; two objects at a time with every load of both in flight together (the
-      // inputs are cold in HBM: one latency per pair of objects instead of one per 8 words)
-      const int nw = R >> 2;
-      auto finish = [&](int b, int nd, int no, int ns) {
-        const unsigned char* s = a.sem + (size_t)b * a.sem_stride;
-        const unsigned char* m = a.mask + (size_t)b * a.mask_stride;
-        const bool vec = (((size_t)s | (size_t)m) & 3) == 0;
-        for (int r = (vec ? (nw << 2) : 0) + lane; r < R; r += 32) {      // tail rays, or everything when unaligned
-          const int sv = s[r], mo = sv != 0;
-          nd += (m[r] != 0) & mo; no += mo; ns += sv != 2;
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          nd += __shfl_xor_sync(0xffffffffu, nd, o); no += __shfl_xor_sync(0xffffffffu, no, o); ns += __shfl_xor_sync(0xffffffffu, ns, o);
-        }
-        if (lane == 0) {
-          cnt[b * 3] = nd; cnt[b * 3 + 1] = no; cnt[b * 3 + 2] = ns;
-          if (nd == 0) misc->on[0] = 0;
-          if (no == 0) misc->on[1] = 0;
-          if (ns == 0) misc->on[2] = 0;
-        }
-      };
-      // every CTA needs every object's counts: each starts at a different object, so the grid does not hit the same
-      // cache lines at the same moment
-      const int shift = (int)((blockIdx.x * 7u) % (unsigned)a.B);
-      for (int iA = warp; iA < a.B; iA += 2 * (NT / 32)) {
-        const int iB = iA + NT / 32;
-        const bool hasB = iB < a.B;
-        const int bA = (iA + shift) % a.B, bB = hasB ? (iB + shift) % a.B : bA;
-        const uint32_t* sA = reinterpret_cast<const uint32_t*>(a.sem + (size_t)bA * a.sem_stride);
-        const uint32_t* mA = reinterpret_cast<const uint32_t*>(a.mask + (size_t)bA * a.mask_stride);
-        const uint32_t* sB = reinterpret_cast<const uint32_t*>(a.sem + (size_t)(hasB ? bB : bA) * a.sem_stride);
-        const uint32_t* mB = reinterpret_cast<const uint32_t*>(a.mask + (size_t)(hasB ? bB : bA) * a.mask_stride);
-        const bool vA = (((size_t)sA | (size_t)mA) & 3) == 0, vB = hasB && (((size_t)sB | (size_t)mB) & 3) == 0;
-        int cA[3] = {0, 0, 0}, cB[3] = {0, 0, 0};
-        for (int w0 = 0; w0 < nw; w0 += 320) {                  // four rays per 32-bit load, ten loads per array per lane
-          uint32_t sa[10], ma[10], sb[10], mb[10];
-#pragma unroll
-          for (int u = 0; u < 10; ++u) {
-            const int w = w0 + u * 32 + lane;
-            const bool in = w < nw;
-            sa[u] = (in && vA) ? __ldg(sA + w) : 0u;  ma[u] = (in && vA) ? __ldg(mA + w) : 0u;
-            sb[u] = (in && vB) ? __ldg(sB + w) : 0u;  mb[u] = (in && vB) ? __ldg(mB + w) : 0u;
-          }
-          // one bit per byte: nonzero(x) folds a byte's bits into bit 0 (labels are 0 / 1 / 2, masks any nonzero = true)
-          auto nzb = [](uint32_t v) { v |= v >> 4; v |= v >> 2; v |= v >> 1; return v & 0x01010101u; };
-#pragma unroll
-          for (int u = 0; u < 10; ++u) {
-            const bool in = w0 + u * 32 + lane < nw;
-            const uint32_t oa = (in && vA) ? nzb(sa[u]) : 0u, ob = (in && vB) ? nzb(sb[u]) : 0u;
-            cA[1] += __popc(oa); cA[0] += __popc(oa & nzb(ma[u])); cA[2] += (in && vA) ? __popc(nzb(sa[u] ^ 0x02020202u)) : 0;
-            cB[1] += __popc(ob); cB[0] += __popc(ob & nzb(mb[u])); cB[2] += (in && vB) ? __popc(nzb(sb[u] ^ 0x02020202u)) : 0;
-          }
-        }
-        finish(bA, cA[0], cA[1], cA[2]);
-        if (hasB) finish(bB, cB[0], cB[1], cB[2]);
-      }
+  } else if (!a.fwd_only) {                             // counts_in given
+    for (int i = tid; i < a.B * 3; i += NT) {
+      const int c = x.counts_in[(i / 3) * 4 + (i % 3)];
+      cnt[i] = c;
+      if (c == 0) misc->on[i % 3] = 0;
     }
   }
   __syncthreads();
@@ -457,12 +398,11 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     float ls_d = 0.f, ls_c = 0.f, ls_o = 0.f;
     {
     const float isc = 1.0f / a.scale[b];
-    bool seg_w = false;               // w_d / w_c / w_o hold this segment's object?
-    if (!a.fwd_only && !pub_counts) {
+    bool seg_w = false;               // published counts: w_d / w_c / w_o hold this segment's object?
+    if (x.counts_in && !a.fwd_only) {
       w_d = on_d / ((float)cnt[b * 3 + 0] + 1e-10f);
       w_c = on_c / ((float)cnt[b * 3 + 1] + 1e-10f);
       w_o = on_o / ((float)cnt[b * 3 + 2] + 1e-10f);
-      seg_w = true;
     }
 
     // A stage: operands written by generic stores -> fence for the async proxy -> CTA barrier -> each warpgroup issues
@@ -640,7 +580,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       };
       float araw = 0.f, occ = 0.f, fr = 1.f, Tr = 1.f, w = 0.f, D = 0.f, O = 0.f, V = 0.f;
       if (hsel == 0) {
-        if (!seg_w && pub_counts) {                     // cooperative launch: acquire the published mask counts (first render only)
+        if (pub_counts && !seg_w) {                     // acquire the published mask counts (first render only)
           if (!cnt_ready) {
             const volatile unsigned int* pubd = gbar + 2;
             unsigned int spins = 0;
@@ -904,32 +844,14 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       const float4* src = reinterpret_cast<const float4*>(Pr);
       for (int i = tid; i < (L.stride >> 2); i += NT) dst[i] = src[i];
     }
-    // ---- reduce + update ---------------------------------------------------------------------------------------------
-    // cooperative launch: after the LAST segment (below, outside this loop), all CTAs share the reduction of all objects.
-    // otherwise: the last segment of the object to arrive reduces that object's rows here.
-    if (!x.cooperative) {
-      __threadfence();
-      __syncthreads();
-      const int c_first = cta_of_pair(rg, G, b * npo), c_last = cta_of_pair(rg, G, (b + 1) * npo - 1);
-      if (tid == 0) misc->fin = (atomicAdd(&x.obj_done[b], 1u) + 1u == (unsigned int)(c_last - c_first + 1)) ? 1 : 0;
-      __syncthreads();
-      if (misc->fin) {
-        __threadfence();
-        const int skip = finish_rows(b, 0, L.stride >> 2, true);
-        if (tid == 0) {
-          x.obj_done[b] = 0u;
-          if (x.fuse_adam && x.step_counter && a.backward && !skip) x.step_counter[b] += 1;
-        }
-      }
-    }
     __syncthreads();
   }
 
-  if (x.cooperative && !a.fwd_only) {
+  if (!a.fwd_only) {
     // ---- grid-wide finish: every CTA is resident (cooperative launch), all of them end their tiles within one round
     // of each other, and the reduction of ALL objects' partial rows + AdamW is split evenly over the grid (less than one
     // float4 of the parameter block per thread) instead of one object per SM on the kernel's tail.
-    // gbar[0] arrive, gbar[1] depart;  x.obj_done[B + b] = skip flag of object b
+    // gbar[0] arrive, gbar[1] depart;  gbar[6 + b] = skip flag of object b
     __threadfence();
     __syncthreads();
     if (tid == 0) {
@@ -946,7 +868,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       const int i_lo = (int)(max(lo, (long long)b * n4) - (long long)b * n4);
       const int i_hi = (int)(min(hi, (long long)(b + 1) * n4) - (long long)b * n4);
       const int skip = finish_rows(b, i_lo, i_hi, i_lo == 0);
-      if (i_lo == 0 && tid == 0) x.obj_done[a.B + b] = (unsigned int)skip;
+      if (i_lo == 0 && tid == 0) gbar[6 + b] = (unsigned int)skip;
     }
     __threadfence();
     __syncthreads();
@@ -955,7 +877,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     if (misc->fin) {                                    // the last CTA to leave: step numbers, re-arm the barrier
       __threadfence();
       if (x.fuse_adam && x.step_counter && a.backward)
-        for (int b = tid; b < a.B; b += NT) if (x.obj_done[a.B + b] == 0u) x.step_counter[b] += 1;
+        for (int b = tid; b < a.B; b += NT) if (gbar[6 + b] == 0u) x.step_counter[b] += 1;
       if (x.loss_sum && warp == 0) {                    // scalar loss of the step (loss.py:59-62), fixed summation order
         float s = 0.f;
         for (int b = lane; b < a.B; b += 32) s += __ldcg(a.loss_terms + b * 4 + 3);
@@ -1002,20 +924,8 @@ static void fused_partition(int B, int npo, int G, uf::Ranges& rg) {
   while (c < G) rg.begin[++c] = (int)T;
 }
 
-// Whether a training step on device `dev` takes the cooperative (grid-wide) finish: the device supports cooperative
-// launch and VMB_NO_COOP is not set (read per call).  Otherwise each object's last CTA reduces and updates it.
-static bool fused_cooperative(int dev) {
-  static int coop_ok[64] = {};
-  if (coop_ok[dev & 63] == 0) {
-    int v = 0;
-    cudaDeviceGetAttribute(&v, cudaDevAttrCooperativeLaunch, dev);
-    coop_ok[dev & 63] = v ? 1 : -1;
-  }
-  return coop_ok[dev & 63] == 1 && getenv("VMB_NO_COOP") == nullptr;
-}
-
 static int fused_launch_step(const VmbLayout& L, const StepParams& sp, const FusedExtra& fx, const void* image, int n_sm,
-                             cudaStream_t st, std::string& err, bool* cooperative = nullptr) {
+                             cudaStream_t st, std::string& err) {
   using namespace uf;
   if (L.H != 32 || L.nfreq != 6) { err = "fused step kernel: hidden must be 32 and n_freq 6"; return -4; }
   if (sp.S < 1 || sp.S > 32) { err = "fused step kernel: n_samples must be in [1, 32]"; return -4; }
@@ -1044,22 +954,19 @@ static int fused_launch_step(const VmbLayout& L, const StepParams& sp, const Fus
   Ranges rg;
   fused_partition(sp.B, npo, (int)grid, rg);
   const unsigned char* img = (const unsigned char*)image;
-  FusedExtra fxl = fx;
-  // every CTA is resident (grid <= #SMs, one CTA per SM) -- the cooperative attribute makes the runtime guarantee it,
-  // which is what lets an object's CTAs wait for each other in the shared reduction
-  fxl.cooperative = (!sp.fwd_only && fused_cooperative(dev)) ? 1 : 0;
-  if (cooperative) *cooperative = fxl.cooperative != 0;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(NT); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = st;
   cudaLaunchAttribute attr[1];
+  // a training launch ends in a grid barrier: every CTA must be resident (grid <= #SMs, one CTA per SM), and the
+  // cooperative attribute makes the runtime guarantee it
   attr[0].id = cudaLaunchAttributeCooperative;
-  attr[0].val.cooperative = fxl.cooperative;
+  attr[0].val.cooperative = sp.fwd_only ? 0 : 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
   cudaError_t e;
-  if (sp.S == 10)      e = cudaLaunchKernelEx(&cfg, k_step_fused<10>, sp, fxl, L, img, rg, tpo, npo, nr, rpw);
-  else if (sp.S == 14) e = cudaLaunchKernelEx(&cfg, k_step_fused<14>, sp, fxl, L, img, rg, tpo, npo, nr, rpw);
-  else                 e = cudaLaunchKernelEx(&cfg, k_step_fused<0>, sp, fxl, L, img, rg, tpo, npo, nr, rpw);
+  if (sp.S == 10)      e = cudaLaunchKernelEx(&cfg, k_step_fused<10>, sp, fx, L, img, rg, tpo, npo, nr, rpw);
+  else if (sp.S == 14) e = cudaLaunchKernelEx(&cfg, k_step_fused<14>, sp, fx, L, img, rg, tpo, npo, nr, rpw);
+  else                 e = cudaLaunchKernelEx(&cfg, k_step_fused<0>, sp, fx, L, img, rg, tpo, npo, nr, rpw);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { err = std::string("k_step_fused launch: ") + cudaGetErrorString(e); return -2; }
   return 0;

@@ -31,7 +31,7 @@ struct vmb_handle {
   unsigned int* d_ticket; // last-block ticket of the fused AdamW (device step counter mode)
   unsigned int* d_smax;   // [max_obj] sampler: per-object max sampled depth (order-preserving key)
   float* d_partials;      // fused step: [(max_obj + n_sm)][stride] per-(CTA, object) gradient partials (allocated on first use)
-  unsigned int* d_objdone;// fused step: [max_obj] finished-segment counters (self-resetting)
+  unsigned int* d_finish_sync; // fused step: [6] grid-barrier words (self-resetting) + [max_obj] skip flags
   float2* d_bc;           // AdamW bias corrections per step number for (bc_b1, bc_b2), built on the host in double precision
   double bc_b1, bc_b2;
   int img_halves;
@@ -132,7 +132,7 @@ int vmb_create(vmb_handle** out, int device, int max_obj, int hidden, int n_freq
   h->n_sm = 132;
   cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, device);
   h->L = vmb_make_layout(hidden, n_freq);
-  h->d_counts = nullptr; h->d_img_index = nullptr; h->d_ticket = nullptr; h->d_smax = nullptr; h->d_partials = nullptr; h->d_objdone = nullptr; h->d_bc = nullptr; h->bc_b1 = h->bc_b2 = -1.0; h->img_halves = 0; h->umma_ok = false; h->lw_ok = false;
+  h->d_counts = nullptr; h->d_img_index = nullptr; h->d_ticket = nullptr; h->d_smax = nullptr; h->d_partials = nullptr; h->d_finish_sync = nullptr; h->d_bc = nullptr; h->bc_b1 = h->bc_b2 = -1.0; h->img_halves = 0; h->umma_ok = false; h->lw_ok = false;
   cudaError_t e = cudaMalloc(&h->d_counts, sizeof(int) * 4 * max_obj);
   if (e == cudaSuccess) e = cudaMalloc(&h->d_ticket, sizeof(unsigned int));
   if (e == cudaSuccess) e = cudaMemset(h->d_ticket, 0, sizeof(unsigned int));
@@ -167,7 +167,7 @@ void vmb_destroy(vmb_handle* h) {
   if (h->d_ticket) cudaFree(h->d_ticket);
   if (h->d_smax) cudaFree(h->d_smax);
   if (h->d_partials) cudaFree(h->d_partials);
-  if (h->d_objdone) cudaFree(h->d_objdone);
+  if (h->d_finish_sync) cudaFree(h->d_finish_sync);
   if (h->d_bc) cudaFree(h->d_bc);
   h->ws.release(); h->ws.destroy_streams();
   h->ws_fwd.release(); h->ws_fwd.destroy_streams();
@@ -205,7 +205,7 @@ static AdamScalars adam_scalars(float lr_f, float b1_f, float b2_f, float wd_f, 
   return q;
 }
 
-// scratch of the fused step kernel (gradient partial rows + per-object arrival counters): allocated on first use,
+// scratch of the fused step kernel (gradient partial rows + grid-barrier words and skip flags): allocated on first use,
 // never while a stream capture is in progress (a captured graph bakes the pointers in)
 static int fused_scratch(vmb_handle* h, cudaStream_t st) {
   if (h->d_partials) return VMB_OK;
@@ -215,8 +215,9 @@ static int fused_scratch(vmb_handle* h, cudaStream_t st) {
     return fail(h, VMB_E_CUDA, "vmb_step: first fused step of a handle must run outside stream capture (scratch allocation)");
   const size_t rows = (size_t)fused_rows_needed(h->max_obj, h->n_sm);
   cudaError_t e = cudaMalloc(&h->d_partials, rows * h->L.stride * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->d_objdone, sizeof(unsigned int) * (2 * (size_t)h->max_obj + 8));
-  if (e == cudaSuccess) e = cudaMemset(h->d_objdone, 0, sizeof(unsigned int) * (2 * (size_t)h->max_obj + 8));
+  const size_t sync_bytes = sizeof(unsigned int) * (6 + (size_t)h->max_obj);
+  if (e == cudaSuccess) e = cudaMalloc(&h->d_finish_sync, sync_bytes);
+  if (e == cudaSuccess) e = cudaMemset(h->d_finish_sync, 0, sync_bytes);
   if (e != cudaSuccess) return fail(h, VMB_E_NOMEM, cudaGetErrorString(e));
   return VMB_OK;
 }
@@ -321,7 +322,7 @@ int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
     if (rc0 != VMB_OK) return rc0;
     FusedExtra fx;
     memset(&fx, 0, sizeof(fx));
-    fx.partials = h->d_partials; fx.obj_done = h->d_objdone; fx.counts_in = a->counts; fx.counts_pub = h->d_counts;
+    fx.partials = h->d_partials; fx.finish_sync = h->d_finish_sync; fx.counts_in = a->counts; fx.counts_pub = h->d_counts;
     fx.fuse_adam = a->fuse_adam ? 1 : 0;
     if (a->fuse_adam) {
       fx.p = const_cast<float*>(a->params); fx.m = a->exp_avg; fx.v = a->exp_avg_sq;
@@ -341,10 +342,8 @@ int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
     if (a->k1_start_event) cudaEventRecord((cudaEvent_t)a->k1_start_event, st);
     std::string err;
     fx.loss_sum = a->loss_sum;
-    bool coop = false;
-    const int rc = fused_launch_step(h->L, sp, fx, a->image, h->n_sm, st, err, &coop);
+    const int rc = fused_launch_step(h->L, sp, fx, a->image, h->n_sm, st, err);
     if (rc != VMB_OK) return fail(h, rc, err);
-    if (a->loss_sum && !coop) { k_loss_sum<<<1, 32, 0, st>>>(a->loss_terms, a->n_obj, a->loss_sum); CUDA_TRY(h, cudaGetLastError()); }
     return VMB_OK;
   }
 
@@ -384,8 +383,6 @@ int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
   if (a->loss_sum) { k_loss_sum<<<1, 32, 0, st>>>(a->loss_terms, a->n_obj, a->loss_sum); CUDA_TRY(h, cudaGetLastError()); }
   return VMB_OK;
 }
-
-int vmb_step_cooperative(int device) { return fused_cooperative(device) ? 1 : 0; }
 
 int vmb_forward(vmb_handle* h, const vmb_forward_args* a, void* stream) {
   if (!h || !a || a->n_obj <= 0 || a->n_obj > h->max_obj || a->n_points <= 0 || !a->points || !a->params ||
