@@ -543,6 +543,66 @@ int vmb_render_count(vmb_handle* h, const vmb_render_args* a, void* stream);
 int vmb_render_emit(vmb_handle* h, const vmb_render_args* a, void* stream);
 int vmb_render_composite(vmb_handle* h, const vmb_render_args* a, void* stream);
 
+/* ---- K10: camera tracking against the object map (vmap_b200/track.py; the rule is in csrc/k_track.cuh) -----------
+ * Adds what neither code base has: the pose of a new RGB-D frame estimated against the map.  The reference reads GT
+ * poses (dataset.py:135) or takes them from an external tracker in live mode (next_live_data); its unused
+ * optimizer.args.pose_lr is the rate here.  Per iteration of a frame:
+ *   vmb_track_step    once per group (one ensemble; hidden 32/64/128/256, same tiles and limits as the fp32 step):
+ *                     per-slice mask counts, forward, render, loss and the backward to the sample points, reduced into
+ *                     per-CTA fp64 partials of the 6-DoF pose gradient and the loss terms.  Reads the pose from `pose`
+ *                     and each object's weights from params row rows[b] (a subset of a packed stack, no repacking).
+ *   vmb_track_update  one small launch: sums every group's partials in a fixed order, runs Adam on the tangent and
+ *                     applies Exp; writes the pose, the iteration's scalar loss and the per-object loss terms.
+ * Everything stays on the device (no host sync), so a whole tracking loop can be captured as one CUDA graph.
+ * VMB_E_ARG: bad counts, hidden != the handle's, missing pointers, partials too small, n_iter < 1, iter outside
+ * [1, n_iter], bad rates; VMB_E_UNSUPPORTED: n_samples above the tile of the hidden size.  rows[] and the pose live on
+ * the device: a row outside [0, n_rows) contributes nothing and sets VMB_TRACK_ST_BAD_ROW, a non-finite pose, loss or
+ * gradient skips the update and sets VMB_ST_NONFINITE in `status`.                                                     */
+#define VMB_TRACK_MAX_GROUPS 8
+#define VMB_TRACK_PART 10              /* doubles per partial row: dL/dphi[3], dL/drho[3], L_d, L_c, L_o, 0           */
+enum { VMB_TRACK_ST_BAD_ROW = 4 };
+
+typedef struct vmb_track_group {
+  int hidden;                    /* the ensemble's hidden size (must match the handle of vmb_track_step)            */
+  int n_obj;                     /* B tracked objects                                                               */
+  int n_rows;                    /* rows of the packed stack `params` / `scale`                                    */
+  const int* rows;               /* device [B] params row of each tracked object                                   */
+  int n_rays, n_samples;         /* R rays of this iteration's slice, S samples per ray                             */
+  const float* pcs;          long long pcs_stride;        /* [B][R][S][3] camera-frame points q (identity-pose samples) */
+  const float* z_vals;       long long z_stride;          /* [B][R][S]                                              */
+  const float* gt_depth;     long long gt_depth_stride;   /* [B][R]                                                 */
+  const float* gt_colour;    long long gt_colour_stride;  /* [B][R][3]                                              */
+  const unsigned char* sem;  long long sem_stride;        /* [B][R]                                                 */
+  const unsigned char* mask_depth; long long mask_stride; /* [B][R]                                                 */
+  const float* params;           /* [n_rows][stride] fp32 weights                                                   */
+  const float* scale;            /* [n_rows] obj_scale                                                              */
+  double* partials;              /* [B * vmb_track_tiles(hidden, R, S)][VMB_TRACK_PART] scratch                     */
+  long long max_partials;        /* rows available in `partials`                                                    */
+  float* loss_terms;             /* optional [B][4] L_depth, L_colour, L_opacity, weighted total (written by update) */
+} vmb_track_group;
+
+typedef struct vmb_track_args {
+  int n_groups;                  /* 1 .. VMB_TRACK_MAX_GROUPS                                                       */
+  vmb_track_group group[VMB_TRACK_MAX_GROUPS];
+  int n_iter;                    /* iterations of the frame (>= 1)                                                  */
+  int iter;                      /* this iteration, 1-based (Adam's bias correction; moments restart at 1)          */
+  double* pose;                  /* device [4][4] fp64 T_wc, in/out                                                 */
+  double* adam;                  /* device [12] Adam moments m[6], v[6] of the tangent (phi, rho)                   */
+  double lr_rot, lr_trans;       /* cfg.pose_lr by default                                                          */
+  double beta1, beta2, eps;      /* 0.9, 0.999, 1e-8                                                                */
+  float colour_scaling;          /* 5.0  (loss.py:6)                                                                */
+  float opacity_scaling;         /* 10.0 (loss.py:6)                                                                */
+  double* loss;                  /* optional device [n_iter]: loss[iter-1] = the iteration's loss (before the update)*/
+  double* pose_hist;             /* optional device [n_iter+1][4][4]: the pose before iteration 1 and after each    */
+  double* grad_hist;             /* optional device [n_iter][6]: each iteration's gradient (phi, rho)               */
+  int* status;                   /* optional device int[4], bits OR-ed in                                           */
+} vmb_track_args;
+
+/* tiles (partial rows) per object of vmb_track_step for this shape, or a negative VMB_E_* code (host only)           */
+int vmb_track_tiles(int hidden, int n_rays, int n_samples);
+int vmb_track_step(vmb_handle* h, const vmb_track_args* a, int group, void* stream);
+int vmb_track_update(vmb_handle* h, const vmb_track_args* a, void* stream);
+
 /* ---- bring-up / test hook (not part of the reference-facing surface) --------------------------- */
 /* Generic wgmma GEMM of the layer-wise wide-model path: D[M][N] = A[M][K1+K2] * B[N][K]^T, fp16 in,
  * fp32 accumulate.  a_mn/b_mn = 0: operand stored [rows][ld] with K contiguous; 1: stored [K][ld] with

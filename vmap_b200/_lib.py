@@ -173,6 +173,34 @@ class RenderArgs(C.Structure):
     ]
 
 
+class TrackGroup(C.Structure):
+    _fields_ = [
+        ("hidden", C.c_int), ("n_obj", C.c_int), ("n_rows", C.c_int), ("rows", _vp),
+        ("n_rays", C.c_int), ("n_samples", C.c_int),
+        ("pcs", _vp), ("pcs_stride", _ll),
+        ("z_vals", _vp), ("z_stride", _ll),
+        ("gt_depth", _vp), ("gt_depth_stride", _ll),
+        ("gt_colour", _vp), ("gt_colour_stride", _ll),
+        ("sem", _vp), ("sem_stride", _ll),
+        ("mask_depth", _vp), ("mask_stride", _ll),
+        ("params", _vp), ("scale", _vp), ("partials", _vp), ("max_partials", _ll), ("loss_terms", _vp),
+    ]
+
+
+TRACK_MAX_GROUPS, TRACK_PART, TRACK_ST_BAD_ROW = 8, 10, 4     # VMB_TRACK_MAX_GROUPS, VMB_TRACK_PART, VMB_TRACK_ST_BAD_ROW
+
+
+class TrackArgs(C.Structure):
+    _fields_ = [
+        ("n_groups", C.c_int), ("group", TrackGroup * TRACK_MAX_GROUPS),
+        ("n_iter", C.c_int), ("iter", C.c_int), ("pose", _vp), ("adam", _vp),
+        ("lr_rot", C.c_double), ("lr_trans", C.c_double),
+        ("beta1", C.c_double), ("beta2", C.c_double), ("eps", C.c_double),
+        ("colour_scaling", C.c_float), ("opacity_scaling", C.c_float),
+        ("loss", _vp), ("pose_hist", _vp), ("grad_hist", _vp), ("status", _vp),
+    ]
+
+
 RENDER_MAX_HITS, RENDER_MAX_SRC, RENDER_BOX = 16, 1024, 18     # VMB_RENDER_MAX_HITS, VMB_RENDER_MAX_SRC, VMB_RENDER_BOX
 
 HULL_OK, HULL_TOO_FEW, HULL_FLAT, HULL_BAD = 0, 1, 2, 3       # VMB_HULL_*
@@ -185,6 +213,7 @@ EXPORTS = (
     "vmb_clip_count", "vmb_clip_emit", "vmb_surface_sample", "vmb_nn_dist",
     "vmb_assoc_classify", "vmb_assoc_voxel", "vmb_assoc_finalize",
     "vmb_hull", "vmb_obb_minvol", "vmb_render_count", "vmb_render_emit", "vmb_render_composite",
+    "vmb_track_tiles", "vmb_track_step", "vmb_track_update",
 )
 
 _lib = None
@@ -243,6 +272,10 @@ def lib():
         L.vmb_obb_minvol.argtypes = [_vp, C.POINTER(ObbArgs), _vp]
         for n in ("vmb_render_count", "vmb_render_emit", "vmb_render_composite"):
             getattr(L, n).argtypes = [_vp, C.POINTER(RenderArgs), _vp]
+        L.vmb_track_tiles.argtypes = [C.c_int, C.c_int, C.c_int]
+        L.vmb_track_tiles.restype = C.c_int
+        L.vmb_track_step.argtypes = [_vp, C.POINTER(TrackArgs), C.c_int, _vp]
+        L.vmb_track_update.argtypes = [_vp, C.POINTER(TrackArgs), _vp]
         L.vmb_build_image.argtypes = [_vp, C.c_int, _vp, _vp, _vp]
         L.vmb_mask_counts.argtypes = [_vp, C.c_int, C.c_int, _vp, _ll, _vp, _ll, _vp, _vp]
         L.vmb_debug_gemm.argtypes = [C.c_int] * 7 + [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, C.c_int, _vp, C.c_int,

@@ -4,6 +4,7 @@ from __future__ import annotations
 
 import json
 import os
+import weakref
 
 import numpy as np
 
@@ -12,7 +13,25 @@ def _load_matrix_txt(path):
     return np.loadtxt(path)
 
 
+_POSE_LR: "weakref.WeakKeyDictionary" = weakref.WeakKeyDictionary()
+
+
 class Config:
+    @property
+    def pose_lr(self) -> float:
+        """optimizer.args.pose_lr, the camera-tracking rate (vmap_b200/track.py).  Every shipped config carries it and
+        the reference never reads it, so it is kept out of the instance's attribute bag, which stays the reference's."""
+        return _POSE_LR.get(self, 0.001)
+
+    # pose_lr travels with copies and pickles of the config, outside the attribute bag
+    def __getstate__(self):
+        return dict(self.__dict__, _pose_lr=self.pose_lr)
+
+    def __setstate__(self, state):
+        state = dict(state)
+        _POSE_LR[self] = state.pop("_pose_lr", 0.001)
+        self.__dict__.update(state)
+
     def __init__(self, config_file=None, config_dict=None):
         if config_dict is None:
             with open(config_file) as f:
@@ -76,6 +95,7 @@ class Config:
         # optimiser (cfg.py:85-86)
         self.learning_rate = c["optimizer"]["args"]["lr"]
         self.weight_decay = c["optimizer"]["args"]["weight_decay"]
+        _POSE_LR[self] = float(c["optimizer"]["args"].get("pose_lr", 0.001))
         # vis (cfg.py:89-92)
         self.vis_device = vis["vis_device"]
         self.n_vis_iter = vis["n_vis_iter"]

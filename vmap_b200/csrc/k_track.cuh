@@ -1,0 +1,507 @@
+// K10: camera tracking against the object map -- pose gradient through every tracked object's network and an
+// on-device Adam / Exp pose optimiser.  CUDA-core fp32 for the networks (the layout and dense helpers of
+// k_step_fp32.cuh, no weight gradients), fp64 for the pose, the partial sums and the update.
+//
+// The rule (oracle/track_oracle.py restates it):
+//   Pose     camera-to-world T_wc = [R | t] (the reference's twc), fp64 [4][4] row-major in device memory.
+//   Samples  each tracked object samples the frame once with the frame's pose set to IDENTITY (K3, one keyframe: the
+//            new frame's slot and the object's 2-D box from this frame's ingest; the background, id 0, uses the full
+//            frame; n_bins_cam2surface 1 for objects, 5 for the background), so pcs holds camera-frame points
+//            q = d_c * z, with z, gt_depth, gt_colour, sem and mask_depth in the training rule (vmap.py:366-459).
+//            n_iter draws of n_pix rays; iteration i uses draw i (train.py:271).
+//   Points   p = R q + t - obj_center (obj_center = 0 in the package), in fp32 from an fp32 copy of the pose; the
+//            network sees p / scale (embedding.py:80).
+//   Loss     the training loss of every tracked object, sum_b (L_d + 5 L_c + 10 L_o) (loss.py:5-62,
+//            render_rays.py:53-96), var detached (loss.py:29), with each ray's render and loss in fp64.  Empty masks
+//            are handled PER OBJECT AND PER TERM: a term whose own mask count is 0 contributes 0 for that object only
+//            (the reference zeroes the term for the whole batch, render_rays.py:68-73, which would stop tracking whenever one small object has no valid ray).
+//   Gradient left perturbation R <- Exp(phi) R, t <- t + rho:
+//              dL/drho = sum g,  dL/dphi = sum (R q) x g,  g = dL/dp
+//              g = (1/scale) (dL/de_xyz + sum_{k,d} dL/de_{k,d} * pi 2^k cos(pi 2^k proj_d) * B_d)
+//            per-point terms in fp32, (R q) x g in fp64 from the fp64 pose; per-CTA partials summed in fp64 in point
+//            order, no floating-point atomics; the update sums every group's partials in (group, object, tile) order
+//            through a fixed tree.  Results are bitwise reproducible.
+//   Update   Adam on the tangent (phi, rho), no weight decay: m = b1 m + (1-b1) g, v = b2 v + (1-b2) g^2 (m = v = 0
+//            before iteration 1 of each frame), m^ = m / (1 - b1^i), v^ = v / (1 - b2^i),
+//            delta = -lr * m^ / (sqrt(v^) + eps) with lr = (lr_rot x 3, lr_trans x 3);
+//            R <- Exp(delta_phi) R, t <- t + delta_rho.  Exp = Rodrigues in fp64, I + [phi]x below |phi| = 1e-12.
+//            A non-finite loss, gradient or pose skips the iteration's update (moments included; at iteration 1 the
+//            moments are still reset to 0) and sets VMB_ST_NONFINITE.
+#pragma once
+#include "common.cuh"
+#include "k_step_fp32.cuh"
+
+// VMB_TRACK_PART (doubles per CTA partial row: dL/dphi[3], dL/drho[3], L_d, L_c, L_o, 0), VMB_TRACK_MAX_GROUPS and
+// VMB_TRACK_ST_BAD_ROW (a rows[] entry outside [0, n_rows); that object contributes nothing) are in vmap_b200.h.
+
+struct TrackParams {
+  int B, R, S, n_rows;
+  const int* rows;
+  const float* pcs;  long long pcs_stride;
+  const float* z;    long long z_stride;
+  const float* gt_depth;  long long gt_depth_stride;
+  const float* gt_colour; long long gt_colour_stride;
+  const unsigned char* sem;  long long sem_stride;
+  const unsigned char* mask; long long mask_stride;
+  const float* params;
+  const float* scale;
+  const double* pose;
+  double* partials;              // [B][tiles][VMB_TRACK_PART]
+  float cs, os;
+  int* status;
+};
+
+// rows [j0, j0 + OB) of d(loss)/d(embedding) for one point: acc[jj] = sum_o dy[o] W[o*ld + jj] (+ the second operand)
+// folded into d(loss)/d(t), t = p / scale.  Rows past `jend` are computed (they read inside the param row) and dropped.
+template <int OB>
+__device__ __forceinline__ void pe_input_grad(const float (&acc)[OB], int j0, int jend, const float* __restrict__ Bm,
+                                              float t0, float t1, float t2, float (&dt)[3]) {
+#pragma unroll
+  for (int jj = 0; jj < OB; ++jj) {
+    const int j = j0 + jj;
+    if (j >= jend) break;
+    if (j < 3) {                                              // xyz rows (constant indices keep dt in registers)
+      dt[0] += (j == 0) ? acc[jj] : 0.f; dt[1] += (j == 1) ? acc[jj] : 0.f; dt[2] += (j == 2) ? acc[jj] : 0.f;
+      continue;
+    }
+    const int k = (j - 3) / VMB_NDIRS, d = (j - 3) - k * VMB_NDIRS;
+    const float* Bd = Bm + d * 3;
+    const float b0 = __ldg(Bd), b1 = __ldg(Bd + 1), b2 = __ldg(Bd + 2);
+    const float proj = fmaf(b2, t2, fmaf(b1, t1, b0 * t0));          // embedding.py:88
+    const float fk = (float)(1 << k);
+    const float arg = (proj * fk) * VMB_PI_F;
+    const float c = (acc[jj] * cosf(arg) * VMB_PI_F) * fk;
+    dt[0] = fmaf(c, b0, dt[0]); dt[1] = fmaf(c, b1, dt[1]); dt[2] = fmaf(c, b2, dt[2]);
+  }
+}
+
+// One CTA (128 threads) = one tile of nr = TP / S whole rays of one tracked object (blockIdx.y), as k_step_fp32.
+template <int H, int TP>
+__global__ void __launch_bounds__(128, 1) k_track_step(TrackParams a, VmbLayout L) {
+  constexpr int NT = 128;
+  constexpr int PT = TP + 1;
+  constexpr int NOG = NT / TP;
+  constexpr int OPT = H / NOG;
+  constexpr int OB = 8;
+  static_assert(OPT % OB == 0, "feature split must be a multiple of the register block");
+
+  extern __shared__ float sm[];
+  float* sE = sm;                         // [E][PT] rows 0..2 = p/scale, then sin features
+  float* sA1 = sE + L.E * PT;             // fc1 / dY1
+  float* sA2 = sA1 + H * PT;              // fc2 / dY2
+  float* sA3 = sA2 + H * PT;              // fc3 / dY3
+  float* sA4 = sA3 + H * PT;              // fc4 / dY4
+  float* sAC = sA4 + H * PT;              // colour hidden / dYc
+  float* sHd = sAC + H * PT;              // 12 rows: alpha, col0..2, d_araw, d_rc0..2, z, occ, T, w; then dt partials
+  __shared__ double s_g[6][TP];           // per-point pose-gradient terms
+  __shared__ double s_l[3][TP];           // per-ray loss terms
+  __shared__ int s_cnt[3][NT / 32];
+
+  const int tid = threadIdx.x;
+  const int p = tid % TP, og = tid / TP;
+  const int b = blockIdx.y;
+  const int S = a.S, R = a.R;
+  const int nr = TP / S;
+  const int np = nr * S;
+  const int r0 = blockIdx.x * nr;
+  const int rl = p / S, sidx = p - rl * S;
+  const bool pvalid = (p < np) && (r0 + rl < R);
+  double* part = a.partials + ((size_t)b * gridDim.x + blockIdx.x) * VMB_TRACK_PART;
+  const int row = a.rows[b];
+  if (row < 0 || row >= a.n_rows) {                   // uniform over the CTA
+    if (tid < VMB_TRACK_PART) part[tid] = 0.0;
+    if (tid == 0 && a.status) atomicOr(a.status, VMB_TRACK_ST_BAD_ROW);
+    return;
+  }
+  const float* __restrict__ P = a.params + (size_t)row * L.stride;
+  const int o_lo = og * OPT;
+
+  // ---- per-object mask counts of this slice (loss.py:16-18,38): every CTA of the object counts the same rays --------
+  {
+    const unsigned char* sv = a.sem + (size_t)b * a.sem_stride;
+    const unsigned char* mv = a.mask + (size_t)b * a.mask_stride;
+    int nd = 0, no = 0, ns = 0;
+    for (int r = tid; r < R; r += NT) {
+      const int s = sv[r];
+      const int mo = s != 0;
+      nd += (mv[r] != 0) & mo; no += mo; ns += s != 2;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      nd += __shfl_xor_sync(0xffffffffu, nd, o);
+      no += __shfl_xor_sync(0xffffffffu, no, o);
+      ns += __shfl_xor_sync(0xffffffffu, ns, o);
+    }
+    if ((tid & 31) == 0) { s_cnt[0][tid >> 5] = nd; s_cnt[1][tid >> 5] = no; s_cnt[2][tid >> 5] = ns; }
+  }
+
+  // ---- A: point p = R q + t (fp32 copy of the fp64 pose), positional embedding of p / scale ---------------------------
+  const double* T = a.pose;
+  float q0 = 0.f, q1 = 0.f, q2 = 0.f, t0 = 0.f, t1 = 0.f, t2 = 0.f;
+  const float sc = a.scale[row];
+  if (pvalid) {
+    const size_t gi = (size_t)b * a.pcs_stride + ((size_t)(r0 + rl) * S + sidx) * 3;
+    q0 = a.pcs[gi]; q1 = a.pcs[gi + 1]; q2 = a.pcs[gi + 2];
+    const float x = fmaf((float)T[2], q2, fmaf((float)T[1], q1, (float)T[0] * q0)) + (float)T[3];
+    const float y = fmaf((float)T[6], q2, fmaf((float)T[5], q1, (float)T[4] * q0)) + (float)T[7];
+    const float w = fmaf((float)T[10], q2, fmaf((float)T[9], q1, (float)T[8] * q0)) + (float)T[11];
+    t0 = x / sc; t1 = y / sc; t2 = w / sc;
+  }
+  if (og == 0) {
+    sE[0 * PT + p] = t0; sE[1 * PT + p] = t1; sE[2 * PT + p] = t2;
+    sHd[8 * PT + p] = pvalid ? a.z[(size_t)b * a.z_stride + (size_t)(r0 + rl) * S + sidx] : 0.f;
+    sHd[4 * PT + p] = 0.f; sHd[5 * PT + p] = 0.f; sHd[6 * PT + p] = 0.f; sHd[7 * PT + p] = 0.f;
+  }
+  for (int d = og; d < VMB_NDIRS; d += NOG) {
+    const float* Bd = P + L.o_B + d * 3;
+    const float proj = fmaf(__ldg(Bd + 2), t2, fmaf(__ldg(Bd + 1), t1, __ldg(Bd) * t0));
+    for (int k = 0; k < L.nfreq; ++k) sE[(3 + k * VMB_NDIRS + d) * PT + p] = sinf((proj * (float)(1 << k)) * VMB_PI_F);
+  }
+  __syncthreads();
+
+  // ---- B: MLP forward (model.py:54-85), as k_step_fp32 ------------------------------------------------------------
+  for (int o = o_lo; o < o_lo + OPT; o += OB) {
+    float acc[OB];
+#pragma unroll
+    for (int j = 0; j < OB; ++j) acc[j] = __ldg(P + L.o_bin + o + j);
+    fwd_block<OB>(acc, P + L.o_Win + o * VMB_E1, VMB_E1, sE + p, VMB_E1, PT);
+#pragma unroll
+    for (int j = 0; j < OB; ++j) sA1[(o + j) * PT + p] = fmaxf(acc[j], 0.f);
+  }
+  __syncthreads();
+  for (int o = o_lo; o < o_lo + OPT; o += OB) {
+    float acc[OB];
+#pragma unroll
+    for (int j = 0; j < OB; ++j) acc[j] = __ldg(P + L.o_bm1 + o + j);
+    fwd_block<OB>(acc, P + L.o_Wm1 + o * H, H, sA1 + p, H, PT);
+#pragma unroll
+    for (int j = 0; j < OB; ++j) sA2[(o + j) * PT + p] = fmaxf(acc[j], 0.f);
+  }
+  __syncthreads();
+  {
+    const int ld = H + VMB_E1;
+    for (int o = o_lo; o < o_lo + OPT; o += OB) {
+      float acc[OB];
+#pragma unroll
+      for (int j = 0; j < OB; ++j) acc[j] = __ldg(P + L.o_bcat + o + j);
+      fwd_block<OB>(acc, P + L.o_Wcat + o * ld, ld, sA2 + p, H, PT);
+      fwd_block<OB>(acc, P + L.o_Wcat + o * ld + H, ld, sE + p, VMB_E1, PT);
+#pragma unroll
+      for (int j = 0; j < OB; ++j) sA3[(o + j) * PT + p] = fmaxf(acc[j], 0.f);
+    }
+  }
+  __syncthreads();
+  for (int o = o_lo; o < o_lo + OPT; o += OB) {
+    float acc[OB];
+#pragma unroll
+    for (int j = 0; j < OB; ++j) acc[j] = __ldg(P + L.o_bm2 + o + j);
+    fwd_block<OB>(acc, P + L.o_Wm2 + o * H, H, sA3 + p, H, PT);
+#pragma unroll
+    for (int j = 0; j < OB; ++j) sA4[(o + j) * PT + p] = fmaxf(acc[j], 0.f);
+  }
+  __syncthreads();
+  {
+    const int ld = H + L.e2;
+    for (int o = o_lo; o < o_lo + OPT; o += OB) {
+      float acc[OB];
+#pragma unroll
+      for (int j = 0; j < OB; ++j) acc[j] = __ldg(P + L.o_bcl + o + j);
+      fwd_block<OB>(acc, P + L.o_Wcl + o * ld, ld, sA4 + p, H, PT);
+      fwd_block<OB>(acc, P + L.o_Wcl + o * ld + H, ld, sE + VMB_E1 * PT + p, L.e2, PT);
+#pragma unroll
+      for (int j = 0; j < OB; ++j) sAC[(o + j) * PT + p] = fmaxf(acc[j], 0.f);
+    }
+    if (og == 0) {
+      float acc1[1] = {__ldg(P + L.o_ba)};
+      fwd_block<1>(acc1, P + L.o_Wa, H, sA4 + p, H, PT);
+      sHd[0 * PT + p] = acc1[0] * 10.0f;                    // model.py:77
+    }
+  }
+  __syncthreads();
+  if (og == 0) {
+    float acc3[3] = {__ldg(P + L.o_boc), __ldg(P + L.o_boc + 1), __ldg(P + L.o_boc + 2)};
+    fwd_block<3>(acc3, P + L.o_Woc, H, sAC + p, H, PT);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) sHd[(1 + c) * PT + p] = vmb_sigmoid(acc3[c]);
+  }
+  __syncthreads();
+
+  // ---- C: render + loss + d(loss)/d(alpha, colour), per-object per-term empty-mask rule ------------------------------
+  if (tid < TP) { s_l[0][tid] = 0.0; s_l[1][tid] = 0.0; s_l[2][tid] = 0.0; }
+  if (tid < nr && r0 + tid < R) {            // per-ray sums in fp64: depth and variance cancel when a ray's weight
+    const int ray = r0 + tid;                 // sits on one sample, and the depth weight 1/(sqrt(var)+1e-4) amplifies it
+    const int pb = tid * S;
+    double Tr = 1.0, D = 0.0, O = 0.0, C0 = 0.0, C1 = 0.0, C2 = 0.0;
+    for (int s = 0; s < S; ++s) {
+      const int qi = pb + s;
+      const float occ = vmb_sigmoid(sHd[0 * PT + qi]);      // render_rays.py:6
+      const double w = (double)occ * Tr;                    // render_rays.py:34
+      sHd[9 * PT + qi] = occ; sHd[10 * PT + qi] = (float)Tr; sHd[11 * PT + qi] = (float)w;
+      D += w * (double)sHd[8 * PT + qi]; O += w;
+      C0 += w * (double)sHd[1 * PT + qi]; C1 += w * (double)sHd[2 * PT + qi]; C2 += w * (double)sHd[3 * PT + qi];
+      Tr *= ((double)vmb_sigmoid(-sHd[0 * PT + qi]) + 1e-10);   // render_rays.py:29 with 1 - occ as sigmoid(-alpha):
+    }                                                       // no cancellation where occ rounds to 1 in fp32
+    double V = 0.0;
+    for (int s = 0; s < S; ++s) {
+      const double dz = (double)sHd[8 * PT + pb + s] - D;
+      V += (double)sHd[11 * PT + pb + s] * dz * dz;         // loss.py:28-29 (detached)
+    }
+    int cnt[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) cnt[c] = s_cnt[c][0] + s_cnt[c][1] + s_cnt[c][2] + s_cnt[c][3];
+    const int sv = a.sem[(size_t)b * a.sem_stride + ray];
+    const double m_o = (sv != 0) ? 1.0 : 0.0;
+    const double m_s = (sv != 2) ? 1.0 : 0.0;
+    const double m_d = (a.mask[(size_t)b * a.mask_stride + ray] != 0) ? m_o : 0.0;
+    const double gd = a.gt_depth[(size_t)b * a.gt_depth_stride + ray];
+    const float* gc = a.gt_colour + (size_t)b * a.gt_colour_stride + (size_t)ray * 3;
+    const double inv_nd = cnt[0] ? 1.0 / ((double)cnt[0] + 1e-10) : 0.0;
+    const double inv_no = cnt[1] ? 1.0 / ((double)cnt[1] + 1e-10) : 0.0;
+    const double inv_ns = cnt[2] ? 1.0 / ((double)cnt[2] + 1e-10) : 0.0;
+    const double info = 1.0 / (sqrt(V) + 1e-4);             // render_rays.py:74-79
+    const double e_d = D - gd, e_o = O - m_o;
+    const double e_c0 = C0 - (double)gc[0], e_c1 = C1 - (double)gc[1], e_c2 = C2 - (double)gc[2];
+    s_l[0][tid] = cnt[0] ? fabs(e_d) * m_d * info * inv_nd : 0.0;
+    s_l[1][tid] = cnt[1] ? (fabs(e_c0) + fabs(e_c1) + fabs(e_c2)) * m_o * inv_no : 0.0;
+    s_l[2][tid] = cnt[2] ? fabs(e_o) * m_s * inv_ns : 0.0;
+    const float gD = (float)(m_d * info * inv_nd) * vmb_sign((float)e_d);
+    const float kc = (float)((double)a.cs * m_o * inv_no);
+    const float gC0 = kc * vmb_sign((float)e_c0), gC1 = kc * vmb_sign((float)e_c1), gC2 = kc * vmb_sign((float)e_c2);
+    const float gO = (float)((double)a.os * m_s * inv_ns) * vmb_sign((float)e_o);
+    float suffix = 0.f;
+    for (int s = S - 1; s >= 0; --s) {
+      const int qi = pb + s;
+      const float occ = sHd[9 * PT + qi], Ts = sHd[10 * PT + qi], w = sHd[11 * PT + qi];
+      const float c0 = sHd[1 * PT + qi], c1 = sHd[2 * PT + qi], c2 = sHd[3 * PT + qi];
+      const float Gs = fmaf(gD, sHd[8 * PT + qi], fmaf(gC0, c0, fmaf(gC1, c1, fmaf(gC2, c2, gO))));
+      const float fr = vmb_sigmoid(-sHd[0 * PT + qi]);     // 1 - occ
+      const float f = fr + 1e-10f;
+      const float docc = Gs * Ts - suffix / f;
+      sHd[4 * PT + qi] = 10.0f * docc * occ * fr;
+      sHd[5 * PT + qi] = gC0 * w * c0 * (1.f - c0);
+      sHd[6 * PT + qi] = gC1 * w * c1 * (1.f - c1);
+      sHd[7 * PT + qi] = gC2 * w * c2 * (1.f - c2);
+      suffix = fmaf(Gs, w, suffix);
+    }
+  }
+  __syncthreads();
+
+  // ---- D: backward to the inputs only (no weight gradients) ----------------------------------------------------------
+  for (int o = o_lo; o < o_lo + OPT; ++o) {                 // dYc = relu'(hc) * (d_rawc @ W_oc)
+    float v = sHd[5 * PT + p] * __ldg(P + L.o_Woc + o);
+    v = fmaf(sHd[6 * PT + p], __ldg(P + L.o_Woc + H + o), v);
+    v = fmaf(sHd[7 * PT + p], __ldg(P + L.o_Woc + 2 * H + o), v);
+    sAC[o * PT + p] = (sAC[o * PT + p] > 0.f) ? v : 0.f;
+  }
+  __syncthreads();
+  {                                                         // dY4 = relu'(fc4) * (dYc @ W_cl[:, :H] + d_araw * W_a)
+    const int ld = H + L.e2;
+    for (int k = o_lo; k < o_lo + OPT; k += OB) {
+      float acc[OB];
+      const float da = sHd[4 * PT + p];
+#pragma unroll
+      for (int j = 0; j < OB; ++j) acc[j] = da * __ldg(P + L.o_Wa + k + j);
+      dgrad_block<OB>(acc, P + L.o_Wcl + k, ld, sAC + p, H, PT);
+#pragma unroll
+      for (int j = 0; j < OB; ++j) sA4[(k + j) * PT + p] = (sA4[(k + j) * PT + p] > 0.f) ? acc[j] : 0.f;
+    }
+  }
+  __syncthreads();
+  for (int k = o_lo; k < o_lo + OPT; k += OB) {             // dY3
+    float acc[OB];
+#pragma unroll
+    for (int j = 0; j < OB; ++j) acc[j] = 0.f;
+    dgrad_block<OB>(acc, P + L.o_Wm2 + k, H, sA4 + p, H, PT);
+#pragma unroll
+    for (int j = 0; j < OB; ++j) sA3[(k + j) * PT + p] = (sA3[(k + j) * PT + p] > 0.f) ? acc[j] : 0.f;
+  }
+  __syncthreads();
+  for (int k = o_lo; k < o_lo + OPT; k += OB) {             // dY2
+    float acc[OB];
+#pragma unroll
+    for (int j = 0; j < OB; ++j) acc[j] = 0.f;
+    dgrad_block<OB>(acc, P + L.o_Wcat + k, H + VMB_E1, sA3 + p, H, PT);
+#pragma unroll
+    for (int j = 0; j < OB; ++j) sA2[(k + j) * PT + p] = (sA2[(k + j) * PT + p] > 0.f) ? acc[j] : 0.f;
+  }
+  __syncthreads();
+  for (int k = o_lo; k < o_lo + OPT; k += OB) {             // dY1
+    float acc[OB];
+#pragma unroll
+    for (int j = 0; j < OB; ++j) acc[j] = 0.f;
+    dgrad_block<OB>(acc, P + L.o_Wm1 + k, H, sA2 + p, H, PT);
+#pragma unroll
+    for (int j = 0; j < OB; ++j) sA1[(k + j) * PT + p] = (sA1[(k + j) * PT + p] > 0.f) ? acc[j] : 0.f;
+  }
+  __syncthreads();
+
+  // d(loss)/d(t): embedding rows in blocks of OB, rows [0, 87) through in_layer + cat_layer, [87, E) through color_linear
+  {
+    float dt[3] = {0.f, 0.f, 0.f};
+    const int nb1 = (VMB_E1 + OB - 1) / OB, nb2 = (L.e2 + OB - 1) / OB;
+    const int ldc = H + VMB_E1, ldl = H + L.e2;
+    for (int blk = og; blk < nb1 + nb2; blk += NOG) {
+      float acc[OB];
+#pragma unroll
+      for (int j = 0; j < OB; ++j) acc[j] = 0.f;
+      if (blk < nb1) {
+        const int j0 = blk * OB;
+        dgrad_block<OB>(acc, P + L.o_Win + j0, VMB_E1, sA1 + p, H, PT);
+        dgrad_block<OB>(acc, P + L.o_Wcat + H + j0, ldc, sA3 + p, H, PT);
+        pe_input_grad<OB>(acc, j0, VMB_E1, P + L.o_B, t0, t1, t2, dt);
+      } else {
+        const int j0 = (blk - nb1) * OB;
+        dgrad_block<OB>(acc, P + L.o_Wcl + H + j0, ldl, sAC + p, H, PT);
+        pe_input_grad<OB>(acc, VMB_E1 + j0, L.E, P + L.o_B, t0, t1, t2, dt);
+      }
+    }
+    sHd[(og * 3 + 0) * PT + p] = dt[0]; sHd[(og * 3 + 1) * PT + p] = dt[1]; sHd[(og * 3 + 2) * PT + p] = dt[2];
+  }
+  __syncthreads();
+  if (og == 0) {
+    float d0 = 0.f, d1 = 0.f, d2 = 0.f;
+#pragma unroll
+    for (int g = 0; g < NOG; ++g) { d0 += sHd[(g * 3) * PT + p]; d1 += sHd[(g * 3 + 1) * PT + p]; d2 += sHd[(g * 3 + 2) * PT + p]; }
+    double c[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    if (pvalid) {
+      const double g0 = (double)(d0 / sc), g1 = (double)(d1 / sc), g2 = (double)(d2 / sc);
+      const double x0 = T[0] * q0 + T[1] * q1 + T[2] * q2;   // R q in fp64
+      const double x1 = T[4] * q0 + T[5] * q1 + T[6] * q2;
+      const double x2 = T[8] * q0 + T[9] * q1 + T[10] * q2;
+      c[0] = x1 * g2 - x2 * g1; c[1] = x2 * g0 - x0 * g2; c[2] = x0 * g1 - x1 * g0;
+      c[3] = g0; c[4] = g1; c[5] = g2;
+    }
+#pragma unroll
+    for (int i = 0; i < 6; ++i) s_g[i][p] = c[i];
+  }
+  __syncthreads();
+  if (tid < 6) {
+    double s = 0.0;
+    for (int i = 0; i < np; ++i) s += s_g[tid][i];
+    part[tid] = s;
+  } else if (tid < 9) {
+    double s = 0.0;
+    for (int i = 0; i < nr; ++i) s += s_l[tid - 6][i];
+    part[tid] = s;
+  } else if (tid == 9) {
+    part[9] = 0.0;
+  }
+}
+
+template <int H, int TP>
+static size_t track_smem(const VmbLayout& L) {
+  return sizeof(float) * (size_t)(L.E + 5 * H + 12) * (TP + 1);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Update: one CTA of 256 threads.  Thread k sums the objects k, k + 256, ... of the concatenated (group, object) list,
+// each object's tiles in order; a fixed tree joins the threads; thread 0 runs Adam + Exp.
+// ---------------------------------------------------------------------------------------------------------------------
+struct TrackGroupDev { const double* partials; int n_obj, tiles; float* loss_terms; };
+
+struct TrackUpdateParams {
+  int n_groups;
+  TrackGroupDev g[VMB_TRACK_MAX_GROUPS];
+  int iter;                      // 1-based iteration of this frame
+  double* pose;                  // [16] in/out
+  double* adam;                  // [12] m, v (not read at iter 1)
+  double lr[6], b1, b2, eps, bc1, bc2;
+  double cs, os;
+  double* loss;                  // optional [n_iter]: loss[iter-1]
+  double* pose_hist;             // optional [n_iter+1][16]
+  double* grad_hist;             // optional [n_iter][6]
+  int* status;
+};
+
+__device__ inline void track_exp(const double (&w)[3], double (&E)[9]) {
+  const double th2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
+  const double th = sqrt(th2);
+  double A, Bc;
+  if (th < 1e-12) { A = 1.0; Bc = 0.0; }
+  else { A = sin(th) / th; Bc = (1.0 - cos(th)) / th2; }
+  const double K[9] = {0.0, -w[2], w[1], w[2], 0.0, -w[0], -w[1], w[0], 0.0};
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      double k2 = 0.0;
+      for (int m = 0; m < 3; ++m) k2 += K[i * 3 + m] * K[m * 3 + j];
+      E[i * 3 + j] = (i == j ? 1.0 : 0.0) + A * K[i * 3 + j] + Bc * k2;
+    }
+}
+
+__global__ void __launch_bounds__(256) k_track_update(TrackUpdateParams a) {
+  constexpr int NC = 7;                                     // grad[6], loss
+  __shared__ double s_acc[NC][256];
+  const int tid = threadIdx.x;
+  double acc[NC];
+#pragma unroll
+  for (int c = 0; c < NC; ++c) acc[c] = 0.0;
+  int base = 0;
+  for (int gi = 0; gi < a.n_groups; ++gi) {
+    const TrackGroupDev G = a.g[gi];
+    for (int ob = ((tid - base) % 256 + 256) % 256; ob < G.n_obj; ob += 256) {
+      const double* pr = G.partials + (size_t)ob * G.tiles * VMB_TRACK_PART;
+      double s[9];
+#pragma unroll
+      for (int c = 0; c < 9; ++c) s[c] = 0.0;
+      for (int t = 0; t < G.tiles; ++t)
+#pragma unroll
+        for (int c = 0; c < 9; ++c) s[c] += pr[(size_t)t * VMB_TRACK_PART + c];
+      const double tot = s[6] + a.cs * s[7] + a.os * s[8];
+      if (G.loss_terms) {
+        float* lt = G.loss_terms + (size_t)ob * 4;
+        lt[0] = (float)s[6]; lt[1] = (float)s[7]; lt[2] = (float)s[8]; lt[3] = (float)tot;
+      }
+#pragma unroll
+      for (int c = 0; c < 6; ++c) acc[c] += s[c];
+      acc[6] += tot;
+    }
+    base += G.n_obj;
+  }
+#pragma unroll
+  for (int c = 0; c < NC; ++c) s_acc[c][tid] = acc[c];
+  __syncthreads();
+  for (int st = 128; st > 0; st >>= 1) {
+    if (tid < st)
+#pragma unroll
+      for (int c = 0; c < NC; ++c) s_acc[c][tid] += s_acc[c][tid + st];
+    __syncthreads();
+  }
+  if (tid != 0) return;
+
+  double g[6];
+  for (int c = 0; c < 6; ++c) g[c] = s_acc[c][0];
+  const double loss = s_acc[6][0];
+  if (a.loss) a.loss[a.iter - 1] = loss;
+  if (a.grad_hist) for (int c = 0; c < 6; ++c) a.grad_hist[(size_t)(a.iter - 1) * 6 + c] = g[c];
+  double T[16];
+  for (int i = 0; i < 16; ++i) T[i] = a.pose[i];
+  if (a.pose_hist && a.iter == 1) for (int i = 0; i < 16; ++i) a.pose_hist[i] = T[i];
+  bool ok = isfinite(loss);
+  for (int c = 0; c < 6; ++c) ok = ok && isfinite(g[c]);
+  for (int i = 0; i < 16; ++i) ok = ok && isfinite(T[i]);
+  if (ok) {
+    double d[6];
+    for (int c = 0; c < 6; ++c) {
+      const double m = (a.iter == 1 ? 0.0 : a.b1 * a.adam[c]) + (1.0 - a.b1) * g[c];
+      const double v = (a.iter == 1 ? 0.0 : a.b2 * a.adam[6 + c]) + (1.0 - a.b2) * g[c] * g[c];
+      a.adam[c] = m; a.adam[6 + c] = v;
+      d[c] = -a.lr[c] * (m / a.bc1) / (sqrt(v / a.bc2) + a.eps);
+    }
+    const double w[3] = {d[0], d[1], d[2]};
+    double E[9];
+    track_exp(w, E);
+    double Rn[9];
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j)
+        Rn[i * 3 + j] = E[i * 3 + 0] * T[0 * 4 + j] + E[i * 3 + 1] * T[1 * 4 + j] + E[i * 3 + 2] * T[2 * 4 + j];
+    for (int i = 0; i < 3; ++i) {
+      for (int j = 0; j < 3; ++j) T[i * 4 + j] = Rn[i * 3 + j];
+      T[i * 4 + 3] += d[3 + i];
+    }
+    for (int i = 0; i < 16; ++i) a.pose[i] = T[i];
+  } else {
+    if (a.iter == 1) for (int c = 0; c < 12; ++c) a.adam[c] = 0.0;   // a skipped first iteration still restarts the moments
+    if (a.status) atomicOr(a.status, VMB_ST_NONFINITE);
+  }
+  if (a.pose_hist) for (int i = 0; i < 16; ++i) a.pose_hist[(size_t)a.iter * 16 + i] = T[i];
+}

@@ -21,6 +21,7 @@
 #include "k_assoc.cuh"
 #include "k_hull.cuh"
 #include "k_render.cuh"
+#include "k_track.cuh"
 
 struct vmb_handle {
   int device, max_obj, H, nfreq;
@@ -1164,6 +1165,110 @@ int vmb_debug_gemm(int a_mn, int b_mn, int epi, int M, int N, int K1, int K2, co
   else if (a_mn == 0 && b_mn == 1 && epi == 2) e = launch_gemm<0, 1, EPI_F32>(A1, A2, B, g, mt, nt, z, st);
   else if (a_mn == 1 && b_mn == 1 && epi == 3) e = launch_gemm<1, 1, EPI_ATOMIC>(A1, A2, B, g, mt, nt, z, st);
   if (e != cudaSuccess) return fail(nullptr, VMB_E_CUDA, std::string("vmb_debug_gemm: ") + cudaGetErrorString(e));
+  return VMB_OK;
+}
+
+}  // extern "C"
+
+// ---- K10: tracking -------------------------------------------------------------------------------------------------
+static int track_tile(int hidden) { return hidden == 32 ? 128 : (hidden == 256 ? 32 : 64); }   // as dispatch_fp32
+
+template <int H, int TP>
+static int launch_track(vmb_handle* h, const TrackParams& tp, int tiles, cudaStream_t st) {
+  const size_t smem = track_smem<H, TP>(h->L);
+  static bool attr_set[64] = {};
+  if (!attr_set[h->device & 63]) {
+    CUDA_TRY(h, cudaFuncSetAttribute(k_track_step<H, TP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_set[h->device & 63] = true;
+  }
+  k_track_step<H, TP><<<dim3((unsigned)tiles, (unsigned)tp.B), 128, smem, st>>>(tp, h->L);
+  CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
+static int track_common(vmb_handle* h, const vmb_track_args* a, const char* who) {
+  if (!a) return fail(h, VMB_E_ARG, std::string(who) + ": null argument");
+  if (a->n_groups < 1 || a->n_groups > VMB_TRACK_MAX_GROUPS)
+    return fail(h, VMB_E_ARG, std::string(who) + ": n_groups must be in [1, 8]");
+  if (a->n_iter < 1 || a->iter < 1 || a->iter > a->n_iter)
+    return fail(h, VMB_E_ARG, std::string(who) + ": need n_iter >= 1 and 1 <= iter <= n_iter");
+  if (!a->pose) return fail(h, VMB_E_ARG, std::string(who) + ": pose is NULL");
+  return VMB_OK;
+}
+
+extern "C" {
+
+int vmb_track_tiles(int hidden, int n_rays, int n_samples) {
+  if (!(hidden == 32 || hidden == 64 || hidden == 128 || hidden == 256) || n_rays < 1 || n_samples < 1) return VMB_E_ARG;
+  const int TP = track_tile(hidden);
+  if (n_samples > TP || n_samples > 32) return VMB_E_UNSUPPORTED;
+  const int nr = TP / n_samples;
+  return (n_rays + nr - 1) / nr;
+}
+
+int vmb_track_step(vmb_handle* h, const vmb_track_args* a, int group, void* stream) {
+  if (!h) return fail(h, VMB_E_ARG, "vmb_track_step: null handle");
+  const int rc0 = track_common(h, a, "vmb_track_step");
+  if (rc0 != VMB_OK) return rc0;
+  if (group < 0 || group >= a->n_groups) return fail(h, VMB_E_ARG, "vmb_track_step: group index outside [0, n_groups)");
+  const vmb_track_group& g = a->group[group];
+  if (g.hidden != h->H) return fail(h, VMB_E_ARG, "vmb_track_step: group hidden size differs from the handle's");
+  if (g.n_obj < 1 || g.n_obj > 65535 || g.n_rows < 1 || g.n_rays < 1 || g.n_samples < 1)
+    return fail(h, VMB_E_ARG, "vmb_track_step: bad n_obj / n_rows / n_rays / n_samples");
+  if (!g.rows || !g.pcs || !g.z_vals || !g.gt_depth || !g.gt_colour || !g.sem || !g.mask_depth || !g.params ||
+      !g.scale || !g.partials)
+    return fail(h, VMB_E_ARG, "vmb_track_step: missing tensor pointer");
+  const int tiles = vmb_track_tiles(g.hidden, g.n_rays, g.n_samples);
+  if (tiles == VMB_E_UNSUPPORTED)
+    return fail(h, VMB_E_UNSUPPORTED, "vmb_track_step: n_samples exceeds the tile size for this hidden size");
+  if (tiles < 1) return fail(h, VMB_E_ARG, "vmb_track_step: bad shape");
+  if ((long long)tiles * g.n_obj > g.max_partials) return fail(h, VMB_E_ARG, "vmb_track_step: partials buffer too small");
+  TrackParams tp;
+  memset(&tp, 0, sizeof(tp));
+  tp.B = g.n_obj; tp.R = g.n_rays; tp.S = g.n_samples; tp.n_rows = g.n_rows; tp.rows = g.rows;
+  tp.pcs = g.pcs; tp.pcs_stride = g.pcs_stride; tp.z = g.z_vals; tp.z_stride = g.z_stride;
+  tp.gt_depth = g.gt_depth; tp.gt_depth_stride = g.gt_depth_stride;
+  tp.gt_colour = g.gt_colour; tp.gt_colour_stride = g.gt_colour_stride;
+  tp.sem = g.sem; tp.sem_stride = g.sem_stride; tp.mask = g.mask_depth; tp.mask_stride = g.mask_stride;
+  tp.params = g.params; tp.scale = g.scale; tp.pose = a->pose; tp.partials = g.partials;
+  tp.cs = a->colour_scaling; tp.os = a->opacity_scaling; tp.status = a->status;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (h->H) {
+    case 32:  return launch_track<32, 128>(h, tp, tiles, st);
+    case 64:  return launch_track<64, 64>(h, tp, tiles, st);
+    case 128: return launch_track<128, 64>(h, tp, tiles, st);
+    case 256: return launch_track<256, 32>(h, tp, tiles, st);
+  }
+  return fail(h, VMB_E_UNSUPPORTED, "vmb_track_step: unsupported hidden size");
+}
+
+int vmb_track_update(vmb_handle* h, const vmb_track_args* a, void* stream) {
+  if (!h) return fail(h, VMB_E_ARG, "vmb_track_update: null handle");
+  const int rc0 = track_common(h, a, "vmb_track_update");
+  if (rc0 != VMB_OK) return rc0;
+  if (!a->adam) return fail(h, VMB_E_ARG, "vmb_track_update: adam state is NULL");
+  if (!(std::isfinite(a->lr_rot) && a->lr_rot >= 0.0 && std::isfinite(a->lr_trans) && a->lr_trans >= 0.0 &&
+        a->beta1 >= 0.0 && a->beta1 < 1.0 && a->beta2 >= 0.0 && a->beta2 < 1.0 && a->eps > 0.0 && std::isfinite(a->eps)))
+    return fail(h, VMB_E_ARG, "vmb_track_update: need finite rates >= 0, betas in [0, 1) and eps > 0");
+  TrackUpdateParams u;
+  memset(&u, 0, sizeof(u));
+  u.n_groups = a->n_groups;
+  for (int i = 0; i < a->n_groups; ++i) {
+    const vmb_track_group& g = a->group[i];
+    const int tiles = vmb_track_tiles(g.hidden, g.n_rays, g.n_samples);
+    if (tiles < 1 || g.n_obj < 1 || !g.partials || (long long)tiles * g.n_obj > g.max_partials)
+      return fail(h, tiles == VMB_E_UNSUPPORTED ? VMB_E_UNSUPPORTED : VMB_E_ARG, "vmb_track_update: bad group");
+    u.g[i].partials = g.partials; u.g[i].n_obj = g.n_obj; u.g[i].tiles = tiles; u.g[i].loss_terms = g.loss_terms;
+  }
+  u.iter = a->iter; u.pose = a->pose; u.adam = a->adam;
+  for (int c = 0; c < 3; ++c) { u.lr[c] = a->lr_rot; u.lr[3 + c] = a->lr_trans; }
+  u.b1 = a->beta1; u.b2 = a->beta2; u.eps = a->eps;
+  u.bc1 = 1.0 - std::pow(a->beta1, (double)a->iter);
+  u.bc2 = 1.0 - std::pow(a->beta2, (double)a->iter);
+  u.cs = a->colour_scaling; u.os = a->opacity_scaling;
+  u.loss = a->loss; u.pose_hist = a->pose_hist; u.grad_hist = a->grad_hist; u.status = a->status;
+  k_track_update<<<1, 256, 0, (cudaStream_t)stream>>>(u);
+  CUDA_TRY(h, cudaGetLastError());
   return VMB_OK;
 }
 
