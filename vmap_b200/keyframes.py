@@ -91,6 +91,21 @@ class FrameStore:
             self.frame_id.pop(slot, None)
             self._free.append(slot)
 
+    def grow(self, capacity: int) -> None:
+        """Raise the capacity to ``capacity`` slots, keeping every stored frame in its slot.  The frame tensors are
+        reallocated, so a CUDA graph captured on this store reads freed memory afterwards: capture again."""
+        old = self.capacity
+        if capacity <= old:
+            return
+        extra = capacity - old
+        with torch.no_grad():
+            for name in ("rgbx", "depth", "inst", "t_wc"):
+                t = getattr(self, name)
+                setattr(self, name, torch.cat([t, torch.zeros((extra,) + t.shape[1:], dtype=t.dtype, device=t.device)]))
+        self.refcount += [0] * extra
+        self._free = list(range(capacity - 1, old - 1, -1)) + self._free
+        self.capacity = capacity
+
     # ---- writes ---------------------------------------------------------------------------------
     def put(self, rgb: torch.Tensor, depth: torch.Tensor, inst: torch.Tensor, t_wc: torch.Tensor, frame_id=None) -> int:
         """Store a frame whose instance image is already final (no ingest pass)."""

@@ -359,3 +359,82 @@ def view_metrics(colour, depth, gt_rgb, gt_depth, gt_inst=None) -> dict:
         vals = [psnr(se[gi == i].mean()) for i in ids]
         out["obj_psnr"] = float(np.mean(vals)) if vals else float("nan")
     return out
+
+
+# ---- trajectory metrics (TUM RGB-D benchmark definitions; host fp64, N <= a few thousand poses once per run) ---------
+
+def _poses(x) -> np.ndarray:
+    a = np.asarray(x.detach().cpu() if torch.is_tensor(x) else x, np.float64)
+    if a.ndim != 3 or a.shape[1:] != (4, 4):
+        raise ValueError(f"expected camera-to-world poses [N, 4, 4], got {a.shape}")
+    return a
+
+
+def _positions(x) -> np.ndarray:
+    a = np.asarray(x.detach().cpu() if torch.is_tensor(x) else x, np.float64)
+    if a.ndim == 3 and a.shape[1:] == (4, 4):
+        return a[:, :3, 3]
+    if a.ndim != 2 or a.shape[1] != 3:
+        raise ValueError(f"expected poses [N, 4, 4] or positions [N, 3], got {a.shape}")
+    return a
+
+
+def align_se3(est, gt) -> np.ndarray:
+    """The rigid transform S [4, 4] (rotation and translation, no scale) minimising sum_i |gt_i - S est_i|^2 over the
+    positions (poses [N, 4, 4] or positions [N, 3]), in closed form (Umeyama 1991, "Least-squares estimation of
+    transformation parameters between two point patterns", eqs. 38-42 with c = 1): with the centred cross-covariance
+    Sigma = 1/N sum (gt_i - mu_gt)(est_i - mu_est)^T = U D V^T, R = U diag(1, 1, s) V^T where s = -1 when
+    det(U) det(V) < 0 (the reflection guard) and 1 otherwise, and t = mu_gt - R mu_est.  The TUM benchmark's ATE uses
+    the same alignment (Horn's method)."""
+    e, g = _positions(est), _positions(gt)
+    if e.shape != g.shape or len(e) < 1:
+        raise ValueError("align_se3: est and gt need the same, non-zero number of poses")
+    me, mg = e.mean(0), g.mean(0)
+    sigma = (g - mg).T @ (e - me) / len(e)
+    U, _, Vt = np.linalg.svd(sigma)
+    s = np.eye(3)
+    if np.linalg.det(U) * np.linalg.det(Vt) < 0:
+        s[2, 2] = -1.0
+    S = np.eye(4)
+    S[:3, :3] = U @ s @ Vt
+    S[:3, 3] = mg - S[:3, :3] @ me
+    return S
+
+
+def ate(est, gt, align: bool = True) -> dict:
+    """Absolute trajectory error (Sturm et al. 2012, the TUM RGB-D benchmark, eq. 2): F_i = Q_i^-1 S P_i with P the
+    estimate, Q the ground truth and S = ``align_se3(P, Q)`` (identity with ``align=False``); the residual of frame i
+    is |trans(F_i)| = |q_i - S p_i| in metres.  Returns rmse, mean, median and max of the residuals (floats) and the
+    per-frame ``errors`` [N] (numpy)."""
+    e, g = _positions(est), _positions(gt)
+    S = align_se3(e, g) if align else np.eye(4)
+    err = np.linalg.norm(g - (e @ S[:3, :3].T + S[:3, 3]), axis=1)
+    return {"rmse": float(np.sqrt(np.mean(err ** 2))), "mean": float(err.mean()), "median": float(np.median(err)),
+            "max": float(err.max()), "errors": err}
+
+
+def _inv_se3(T: np.ndarray) -> np.ndarray:
+    inv = np.zeros_like(T)
+    inv[:, :3, :3] = T[:, :3, :3].transpose(0, 2, 1)
+    inv[:, :3, 3] = -np.einsum("nji,nj->ni", T[:, :3, :3], T[:, :3, 3])
+    inv[:, 3, 3] = 1.0
+    return inv
+
+
+def _rel(T: np.ndarray, delta: int) -> np.ndarray:
+    return _inv_se3(T[:-delta]) @ T[delta:]
+
+
+def rpe(est, gt, delta: int = 1) -> dict:
+    """Relative pose error (Sturm et al. 2012, eq. 1) over ``delta`` frames: E_i = (Q_i^-1 Q_{i+d})^-1 (P_i^-1 P_{i+d}).
+    Returns ``trans_rmse`` (metres), the RMSE of |trans(E_i)|, and ``rot_rmse_deg``, the RMSE of the rotation angle
+    arccos((trace(rot(E_i)) - 1) / 2) in degrees, plus the per-pair ``trans_errors`` / ``rot_errors_deg``."""
+    P, Q = _poses(est), _poses(gt)
+    if P.shape != Q.shape or not 1 <= delta < len(P):
+        raise ValueError("rpe: est and gt need the same number of poses, more than delta")
+    E = _inv_se3(_rel(Q, delta)) @ _rel(P, delta)
+    te = np.linalg.norm(E[:, :3, 3], axis=1)
+    c = np.clip((np.trace(E[:, :3, :3], axis1=1, axis2=2) - 1.0) / 2.0, -1.0, 1.0)
+    re = np.degrees(np.arccos(c))
+    return {"trans_rmse": float(np.sqrt(np.mean(te ** 2))), "rot_rmse_deg": float(np.sqrt(np.mean(re ** 2))),
+            "trans_errors": te, "rot_errors_deg": re}
