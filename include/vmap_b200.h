@@ -230,6 +230,12 @@ typedef struct vmb_sample_args {
   /* Optional device-resident draw counter: when set it replaces `offset`, so a captured CUDA graph of a whole
    * frame (sampler + its optimisation steps) draws fresh samples on every replay (the caller increments it). */
   const unsigned long long* offset_dev;
+  /* Optional, appended for bundle adjustment (csrc/k_ba.cuh); 0 / NULL leave every launch as it was.
+   * camera_frame != 0: take every keyframe's pose as identity (store and per-object mode), so pcs holds camera-frame
+   * points q = d_c * z.  kf_out: [B][n_frames] the keyframe index each draw used (latest-two rule and injected
+   * keyframes included).                                                                                           */
+  int camera_frame;
+  int* kf_out;
 } vmb_sample_args;
 
 int vmb_sample(vmb_handle* h, const vmb_sample_args* a, void* stream);
@@ -602,6 +608,77 @@ typedef struct vmb_track_args {
 int vmb_track_tiles(int hidden, int n_rays, int n_samples);
 int vmb_track_step(vmb_handle* h, const vmb_track_args* a, int group, void* stream);
 int vmb_track_update(vmb_handle* h, const vmb_track_args* a, void* stream);
+
+/* ---- K11: bundle adjustment of keyframe poses (vmap_b200/ba.py; the rule is in csrc/k_ba.cuh) ------------------
+ * Pose-only passes against a frozen map, between mapping frames: every keyframe pose the objects' keyframe tables hold
+ * is moved by the same loss the mapping frame minimises.  Per iteration of a pass:
+ *   vmb_ba_step    once per group (one ensemble; hidden 32/64/128/256, S as vmb_track_step): K10's forward, render,
+ *                  loss and backward to the sample points, with the pose of each ray read from the fp64 pose table at
+ *                  the frame its draw used; writes one fp64 row per ray (VMB_TRACK_PART doubles, as K10's partials).
+ *   vmb_ba_update  one small launch: sums the rows per (object, draw) and per window frame in a fixed order, runs one
+ *                  Adam on the stacked tangents of the window and applies Exp to each window pose in the table; after
+ *                  the last iteration writes each window pose in fp32 to the targets.
+ * VMB_E_ARG: bad counts, hidden != the handle's, missing pointers, rows or scratch too small, n_rays not a multiple of
+ * n_pix_draw, n_win outside [1, VMB_BA_MAX_WIN], iter outside [1, n_iter], bad rates.  On the device: a draw whose
+ * keyframe index or frame id is outside its table contributes nothing and sets VMB_BA_ST_BAD_FRAME (as does a window
+ * entry >= n_poses); a row outside [0, n_rows) sets VMB_TRACK_ST_BAD_ROW; a non-finite loss, gradient or window pose
+ * skips the iteration's update and sets VMB_ST_NONFINITE.  Window entries must be distinct.                         */
+#define VMB_BA_MAX_WIN 1024
+enum { VMB_BA_ST_BAD_FRAME = 8 };
+
+typedef struct vmb_ba_group {
+  int hidden;                    /* the ensemble's hidden size (must match the handle of vmb_ba_step)               */
+  int n_obj;                     /* B objects                                                                       */
+  int n_rows;                    /* rows of the packed stack `params` / `scale`                                    */
+  const int* rows;               /* device [B] params row of each object                                           */
+  int n_rays, n_samples;         /* R rays of this iteration's slice, S samples per ray                             */
+  const float* pcs;          long long pcs_stride;        /* [B][R][S][3] camera-frame points q                    */
+  const float* z_vals;       long long z_stride;          /* [B][R][S]                                              */
+  const float* gt_depth;     long long gt_depth_stride;   /* [B][R]                                                 */
+  const float* gt_colour;    long long gt_colour_stride;  /* [B][R][3]                                              */
+  const unsigned char* sem;  long long sem_stride;        /* [B][R]                                                 */
+  const unsigned char* mask_depth; long long mask_stride; /* [B][R]                                                 */
+  const float* params;           /* [n_rows][stride] fp32 weights                                                   */
+  const float* scale;            /* [n_rows] obj_scale                                                              */
+  int n_pix_draw;                /* rays per draw: ray r of the slice belongs to draw r / n_pix_draw                */
+  const int* kf_draw;  long long kf_draw_stride;          /* [B][R / n_pix_draw] keyframe index of each draw        */
+  const int* kf_frame; int kf_stride;                     /* [B][kf_stride] frame id of each keyframe index (-1: none) */
+  double* ray_rows;              /* [B][R][VMB_TRACK_PART] scratch: dL/dphi[3], dL/drho[3], L_d, L_c, L_o, 0       */
+  long long max_ray_rows;        /* rows available in `ray_rows`                                                    */
+} vmb_ba_group;
+
+typedef struct vmb_ba_target {
+  const int* frame_of;           /* device [n] frame id held by each entry (-1: none)                               */
+  float* t_wc;                   /* device [n][4][4] fp32 poses to refresh (NULL: no target)                        */
+  int n;
+} vmb_ba_target;
+
+typedef struct vmb_ba_args {
+  int n_groups;                  /* 1 .. VMB_TRACK_MAX_GROUPS                                                       */
+  vmb_ba_group group[VMB_TRACK_MAX_GROUPS];
+  int n_iter;                    /* iterations of the pass (>= 1)                                                   */
+  int iter;                      /* this iteration, 1-based (Adam's bias correction; moments restart at 1)          */
+  double* poses;                 /* device [n_poses][4][4] fp64 pose table T_wc, in/out                             */
+  int n_poses;
+  const int* window;             /* device [n_win] distinct frame ids the pass moves (-1: padding)                  */
+  int n_win;
+  int hold;                      /* a frame id that never moves (the anchor, 0), or -1                              */
+  double* adam;                  /* device [n_win][12] Adam moments m[6], v[6] per window entry                     */
+  double* scratch;               /* device, >= 8 * sum_groups(n_obj * n_rays / n_pix_draw) + 6 * n_win doubles      */
+  long long scratch_len;
+  double lr_rot, lr_trans;       /* cfg.pose_lr by default                                                          */
+  double beta1, beta2, eps;      /* 0.9, 0.999, 1e-8                                                                */
+  float colour_scaling;          /* 5.0  (loss.py:6)                                                                */
+  float opacity_scaling;         /* 10.0 (loss.py:6)                                                                */
+  double* loss;                  /* optional device [n_iter]: loss[iter-1] = the iteration's loss (before the update)*/
+  double* pose_hist;             /* optional device [n_iter+1][n_win][4][4]: poses before iteration 1 and after each */
+  double* grad_hist;             /* optional device [n_iter][n_win][6]: each iteration's gradient per window entry  */
+  vmb_ba_target target[2];       /* written after iteration n_iter                                                  */
+  int* status;                   /* optional device int[4], bits OR-ed in                                           */
+} vmb_ba_args;
+
+int vmb_ba_step(vmb_handle* h, const vmb_ba_args* a, int group, void* stream);
+int vmb_ba_update(vmb_handle* h, const vmb_ba_args* a, void* stream);
 
 /* ---- bring-up / test hook (not part of the reference-facing surface) --------------------------- */
 /* Generic wgmma GEMM of the layer-wise wide-model path: D[M][N] = A[M][K1+K2] * B[N][K]^T, fp16 in,

@@ -8,7 +8,10 @@ host bookkeeping the device waits for (keyframes, object insertion, sampler tabl
 frame.  Medians are over the frames after the last object insertion; insertion frames (re-stack, graph captures) are
 reported apart, and so is the tracking time of each tracking mode: a frame whose tracked set changed tracks eagerly,
 the next frame with that set captures the tracking graph (a warm-up frame, a synchronise and the capture) and later
-frames replay it.  The card's name and power limit are read in the same run."""
+frames replay it.  With ``--ba-every`` (one run per value; 0 = no bundle adjustment) the bundle-adjustment phase is
+reported too, by pass mode, and after the run the device time of one BA iteration per group (``vmb_ba_step`` on each
+ensemble) and of ``vmb_ba_update``, over repeated launches.  The card's name and power limit are read in the same
+run."""
 from __future__ import annotations
 
 import argparse
@@ -30,12 +33,50 @@ from vmap_b200.slam import Slam  # noqa: E402
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--frames", type=int, default=40)
+    ap.add_argument("--ba-every", default="0", help="comma-separated ba_every values, one run each")
+    ap.add_argument("--ba-iter", type=int, default=20)
     args = ap.parse_args(argv)
     assert torch.cuda.is_available(), "slam_time measures the GPU; there is no CPU number"
     cfg = Config(config_dict=replica_room0_dict())
     seq = synth.sphere_room_sequence(args.frames, cfg.W, cfg.H, cfg.fx, cfg.fy, cfg.cx, cfg.cy, n_extra=16)
+    for every in [int(x) for x in args.ba_every.split(",")]:
+        run(cfg, seq, args.frames, every, args.ba_iter)
+
+
+def ba_iteration_ms(slam, reps: int = 50) -> dict:
+    """Device time of one BA iteration's launches on the buffers of the last pass: vmb_ba_step per group and
+    vmb_ba_update (the poses it moves are not used afterwards)."""
+    import ctypes as C
+    from vmap_b200 import _lib
+    from vmap_b200.ensemble import _stream
+    ba = slam.ba
+    a = ba._args
+    out = {}
+    for gi, g in enumerate(ba.groups):
+        fn = lambda: _lib.check(g.ens._handle, g.ens.lib.vmb_ba_step(g.ens._handle, C.byref(a), gi, _stream()), "step")
+        out[f"step_h{g.ens.hidden}_x{len(g.rows)}"] = _event_ms(fn, reps)
+    e = ba.groups[0].ens
+    out["update"] = _event_ms(lambda: _lib.check(e._handle, e.lib.vmb_ba_update(e._handle, C.byref(a), _stream()),
+                                                 "update"), reps)
+    return out
+
+
+def _event_ms(fn, reps):
+    for _ in range(3):
+        fn()
+    s, t = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    s.record()
+    for _ in range(reps):
+        fn()
+    t.record()
+    torch.cuda.synchronize()
+    return round(s.elapsed_time(t) / reps, 4)
+
+
+def run(cfg, seq, frames, ba_every, ba_iter):
+    args = argparse.Namespace(frames=frames)
     slam = Slam(cfg, T_init=seq["poses"][0], background_cls=seq["background_cls"], max_frames=args.frames,
-                timing=True)
+                timing=True, ba_every=ba_every, n_ba_iter=ba_iter)
     for k in range(args.frames):
         slam.step(torch.from_numpy(seq["rgb"][k]), torch.from_numpy(seq["depth"][k].astype(np.float32)),
                   torch.from_numpy(seq["inst"][k]), torch.from_numpy(seq["cls"][k]))
@@ -56,7 +97,14 @@ def main(argv=None):
                                 for m in ("eager", "capture", "replay")
                                 for v in [[t["track"][i] for i, mm in enumerate(res["track_modes"]) if mm == m]] if v},
            "lost": int(res["lost"].sum()), "ate_rmse_m": ate["rmse"], "rpe_trans_rmse_m": rpe["trans_rmse"],
-           "rpe_rot_rmse_deg": rpe["rot_rmse_deg"]}
+           "rpe_rot_rmse_deg": rpe["rot_rmse_deg"], "ba_every": ba_every}
+    if ba_every:
+        out["ba_iters"] = ba_iter
+        out["ba_ms_by_mode"] = {m: {"frames": len(v), "median": round(float(np.median(v)), 3)}
+                                for m in ("eager", "capture", "replay")
+                                for v in [[t["ba"][i] for i, mm in enumerate(res["ba_modes"]) if mm == m]] if v}
+        out["ba_window_median"] = float(np.median([len(f) for f in res["ba_frames"] if f]))
+        out["ba_iteration_ms"] = ba_iteration_ms(slam)
     print(json.dumps(out))
 
 

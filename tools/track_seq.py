@@ -1,6 +1,6 @@
 """Track a whole Replica-layout sequence on the GPU and score the trajectory against its ``traj_w_c.txt``.
 
-    python tools/track_seq.py --config CFG --out DIR --slam [--frames a:b] [--n-iter N]
+    python tools/track_seq.py --config CFG --out DIR --slam [--frames a:b] [--n-iter N] [--ba-every N --ba-iter M]
     python tools/track_seq.py --config CFG --out DIR --ckpt-dir LOG/ckpt --frame F [--frames a:b] [--n-iter N]
 
 ``--slam`` runs online SLAM (``vmap_b200.slam.Slam``): frame a takes its GT pose as the anchor, every later frame is
@@ -62,6 +62,9 @@ def main(argv=None):
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--store-capacity", type=int, default=None,
                     help="initial frame-store slots (--slam; the store grows on demand)")
+    ap.add_argument("--ba-every", type=int, default=0,
+                    help="--slam: a bundle-adjustment pass after every N-th mapping frame (0: none)")
+    ap.add_argument("--ba-iter", type=int, default=20, help="bundle-adjustment iterations per pass")
     args = ap.parse_args(argv)
     cfg = Config(args.config)
     if cfg.dataset_format != "Replica":
@@ -80,7 +83,7 @@ def main(argv=None):
               bbox_scale=REPLICA_BBOX_SCALE, max_frames=len(frames), timing=True,
               store_capacity=args.store_capacity)
     if args.slam:
-        slam = Slam(cfg, T_init=gt_all[a], **kw)
+        slam = Slam(cfg, T_init=gt_all[a], ba_every=args.ba_every, n_ba_iter=args.ba_iter, **kw)
     else:
         sources, skipped = load_sources(args.ckpt_dir, args.frame, device=cfg.data_device)
         if skipped:
@@ -97,13 +100,15 @@ def main(argv=None):
            "ate_aligned": metrics.ate(est, gt, align=True), "ate_unaligned": metrics.ate(est, gt, align=False),
            "rpe": metrics.rpe(est, gt) if len(frames) > 1 else None,
            "lost": [f for f, l in zip(frames, res["lost"]) if l], "times_ms": times,
-           "tracked_ids": res["tracked_ids"], "inserted": res["inserted"], "track_modes": res["track_modes"]}
+           "tracked_ids": res["tracked_ids"], "inserted": res["inserted"], "track_modes": res["track_modes"],
+           "ba_loss": res["ba_loss"], "ba_frames": res["ba_frames"]}
     np.save(os.path.join(args.out, "metrics_traj.npy"), np.array(out, dtype=object), allow_pickle=True)
     line = {"mode": out["mode"], "frames": len(frames), "ate_rmse_m": out["ate_aligned"]["rmse"],
             "ate_rmse_unaligned_m": out["ate_unaligned"]["rmse"],
             "rpe_trans_rmse_m": out["rpe"]["trans_rmse"] if out["rpe"] else None,
             "rpe_rot_rmse_deg": out["rpe"]["rot_rmse_deg"] if out["rpe"] else None,
-            "lost": out["lost"], "frame_ms_median": float(np.median(times["frame"]))}
+            "lost": out["lost"], "frame_ms_median": float(np.median(times["frame"])),
+            "ba_passes": sum(1 for f in res["ba_frames"] if f)}
     print(json.dumps(line))
 
 

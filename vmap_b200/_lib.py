@@ -79,7 +79,7 @@ class SampleArgs(C.Structure):
         ("sem", _vp), ("mask_depth", _vp),
         ("store_rgbx", _vp), ("store_depth", _vp), ("store_inst", _vp), ("store_t_wc", _vp),
         ("kf_slot", _vp), ("kf_bbox", _vp), ("obj_id", _vp), ("kf_stride", C.c_int),
-        ("offset_dev", _vp),
+        ("offset_dev", _vp), ("camera_frame", C.c_int), ("kf_out", _vp),
     ]
 
 
@@ -201,6 +201,41 @@ class TrackArgs(C.Structure):
     ]
 
 
+BA_MAX_WIN, BA_ST_BAD_FRAME = 1024, 8                          # VMB_BA_MAX_WIN, VMB_BA_ST_BAD_FRAME
+
+
+class BaGroup(C.Structure):
+    _fields_ = [
+        ("hidden", C.c_int), ("n_obj", C.c_int), ("n_rows", C.c_int), ("rows", _vp),
+        ("n_rays", C.c_int), ("n_samples", C.c_int),
+        ("pcs", _vp), ("pcs_stride", _ll),
+        ("z_vals", _vp), ("z_stride", _ll),
+        ("gt_depth", _vp), ("gt_depth_stride", _ll),
+        ("gt_colour", _vp), ("gt_colour_stride", _ll),
+        ("sem", _vp), ("sem_stride", _ll),
+        ("mask_depth", _vp), ("mask_stride", _ll),
+        ("params", _vp), ("scale", _vp),
+        ("n_pix_draw", C.c_int), ("kf_draw", _vp), ("kf_draw_stride", _ll), ("kf_frame", _vp), ("kf_stride", C.c_int),
+        ("ray_rows", _vp), ("max_ray_rows", _ll),
+    ]
+
+
+class BaTarget(C.Structure):
+    _fields_ = [("frame_of", _vp), ("t_wc", _vp), ("n", C.c_int)]
+
+
+class BaArgs(C.Structure):
+    _fields_ = [
+        ("n_groups", C.c_int), ("group", BaGroup * TRACK_MAX_GROUPS),
+        ("n_iter", C.c_int), ("iter", C.c_int), ("poses", _vp), ("n_poses", C.c_int),
+        ("window", _vp), ("n_win", C.c_int), ("hold", C.c_int), ("adam", _vp), ("scratch", _vp), ("scratch_len", _ll),
+        ("lr_rot", C.c_double), ("lr_trans", C.c_double),
+        ("beta1", C.c_double), ("beta2", C.c_double), ("eps", C.c_double),
+        ("colour_scaling", C.c_float), ("opacity_scaling", C.c_float),
+        ("loss", _vp), ("pose_hist", _vp), ("grad_hist", _vp), ("target", BaTarget * 2), ("status", _vp),
+    ]
+
+
 RENDER_MAX_HITS, RENDER_MAX_SRC, RENDER_BOX = 16, 1024, 18     # VMB_RENDER_MAX_HITS, VMB_RENDER_MAX_SRC, VMB_RENDER_BOX
 
 HULL_OK, HULL_TOO_FEW, HULL_FLAT, HULL_BAD = 0, 1, 2, 3       # VMB_HULL_*
@@ -213,7 +248,7 @@ EXPORTS = (
     "vmb_clip_count", "vmb_clip_emit", "vmb_surface_sample", "vmb_nn_dist",
     "vmb_assoc_classify", "vmb_assoc_voxel", "vmb_assoc_finalize",
     "vmb_hull", "vmb_obb_minvol", "vmb_render_count", "vmb_render_emit", "vmb_render_composite",
-    "vmb_track_tiles", "vmb_track_step", "vmb_track_update",
+    "vmb_track_tiles", "vmb_track_step", "vmb_track_update", "vmb_ba_step", "vmb_ba_update",
 )
 
 _lib = None
@@ -276,6 +311,8 @@ def lib():
         L.vmb_track_tiles.restype = C.c_int
         L.vmb_track_step.argtypes = [_vp, C.POINTER(TrackArgs), C.c_int, _vp]
         L.vmb_track_update.argtypes = [_vp, C.POINTER(TrackArgs), _vp]
+        L.vmb_ba_step.argtypes = [_vp, C.POINTER(BaArgs), C.c_int, _vp]
+        L.vmb_ba_update.argtypes = [_vp, C.POINTER(BaArgs), _vp]
         L.vmb_build_image.argtypes = [_vp, C.c_int, _vp, _vp, _vp]
         L.vmb_mask_counts.argtypes = [_vp, C.c_int, C.c_int, _vp, _ll, _vp, _ll, _vp, _vp]
         L.vmb_debug_gemm.argtypes = [C.c_int] * 7 + [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, C.c_int, _vp, C.c_int,

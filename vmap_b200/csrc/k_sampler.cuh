@@ -43,7 +43,11 @@ struct SampleParams {
   const uchar4* st_rgbx; const float* st_depth; const int* st_inst; const float* st_twc;
   const int* kf_slot; const float* bbox_flat; const int* obj_id; int kf_stride;
   const unsigned long long* offset_dev;   // optional device-resident draw counter (CUDA-graph replay of a frame)
+  int camera_frame;                       // take every keyframe pose as identity: camera-frame points (K11)
+  int* kf_out;                            // optional [B][n_frames]: keyframe index of each draw
 };
+
+__device__ const float k_identity44[16] = {1.f, 0.f, 0.f, 0.f, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f, 1.f};
 
 __device__ __forceinline__ uint32_t sample_offset(const SampleParams& a) {
   return (uint32_t)(a.offset_dev ? *a.offset_dev : a.offset);
@@ -126,6 +130,7 @@ __global__ void __launch_bounds__(256) k_sample_gather(SampleParams a, unsigned 
   float mx = -3.0e38f;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < N; i += gridDim.x * blockDim.x) {
     const RayPick r = pick_pixel(a, b, i);
+    if (a.kf_out && i % a.n_pix == 0) a.kf_out[(size_t)b * a.n_frames + i / a.n_pix] = r.kf;
     uchar4 px;
     float d;
     if (a.st_rgbx) {
@@ -241,7 +246,8 @@ __global__ void __launch_bounds__(256) k_sample_points(SampleParams a, const uns
     }
 
     const float* dc = a.rays_dir + ((size_t)r.iw * a.Hh + r.ih) * 3;   // vmap.py:357
-    const float* T = a.st_rgbx ? a.st_twc + (size_t)a.kf_slot[(size_t)b * a.kf_stride + r.kf] * 16
+    const float* T = a.camera_frame ? k_identity44
+                   : a.st_rgbx ? a.st_twc + (size_t)a.kf_slot[(size_t)b * a.kf_stride + r.kf] * 16
                                : a.t_wc[b] + r.kf * 16;                // vmap.py:360
     const float dw0 = fmaf(T[2], dc[2], fmaf(T[1], dc[1], T[0] * dc[0]));      // vmap.py:37
     const float dw1 = fmaf(T[6], dc[2], fmaf(T[5], dc[1], T[4] * dc[0]));

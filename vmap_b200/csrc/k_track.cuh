@@ -4,9 +4,9 @@
 //
 // The rule (oracle/track_oracle.py restates it):
 //   Pose     camera-to-world T_wc = [R | t] (the reference's twc), fp64 [4][4] row-major in device memory.
-//   Samples  each tracked object samples the frame once with the frame's pose set to IDENTITY (K3, one keyframe: the
-//            new frame's slot and the object's 2-D box from this frame's ingest; the background, id 0, uses the full
-//            frame; n_bins_cam2surface 1 for objects, 5 for the background), so pcs holds camera-frame points
+//   Samples  each tracked object samples the frame once in the camera frame (K3's camera_frame mode: the points of an
+//            IDENTITY pose; one keyframe: the new frame's slot and the object's 2-D box from this frame's ingest; the
+//            background, id 0, uses the full frame; n_bins_cam2surface 1 for objects, 5 for the background), so pcs holds camera-frame points
 //            q = d_c * z, with z, gt_depth, gt_colour, sem and mask_depth in the training rule (vmap.py:366-459).
 //            n_iter draws of n_pix rays; iteration i uses draw i (train.py:271).
 //   Points   p = R q + t - obj_center (obj_center = 0 in the package), in fp32 from an fp32 copy of the pose; the
@@ -75,9 +75,28 @@ __device__ __forceinline__ void pe_input_grad(const float (&acc)[OB], int j0, in
   }
 }
 
+// K11's per-ray pose (k_ba.cuh): draw d of object b used keyframe index kf_draw[b][d], whose frame id (the row of the
+// fp64 pose table a.pose) is kf_frame[b][kf].  K10 does not read it.
+struct BaRays {
+  const int* kf_draw; long long kf_draw_stride;     // [B][draws of the slice]
+  const int* kf_frame; int kf_stride;               // [B][kf_stride], -1 = no frame
+  int n_pix_draw, n_poses;                          // rays per draw, rows of the pose table
+  double* rows;                                     // out [B][R][VMB_TRACK_PART] per-ray rows
+};
+
+// frame id of draw `d` of object `b`, or -1 when the keyframe index or the frame id is outside its table
+__device__ __forceinline__ int ba_draw_frame(const int* kf_draw, long long kf_draw_stride, const int* kf_frame,
+                                             int kf_stride, int n_poses, int b, int d) {
+  const int kf = kf_draw[(size_t)b * kf_draw_stride + d];
+  if (kf < 0 || kf >= kf_stride) return -1;
+  const int f = kf_frame[(size_t)b * kf_stride + kf];
+  return (f >= 0 && f < n_poses) ? f : -1;
+}
+
 // One CTA (128 threads) = one tile of nr = TP / S whole rays of one tracked object (blockIdx.y), as k_step_fp32.
-template <int H, int TP>
-__global__ void __launch_bounds__(128, 1) k_track_step(TrackParams a, VmbLayout L) {
+// BA = false is K10 (one pose, per-CTA partials); BA = true is K11 (a pose per ray, per-ray rows).
+template <int H, int TP, bool BA>
+__device__ __forceinline__ void track_step_body(const TrackParams& a, const VmbLayout& L, const BaRays& x) {
   constexpr int NT = 128;
   constexpr int PT = TP + 1;
   constexpr int NOG = NT / TP;
@@ -109,7 +128,12 @@ __global__ void __launch_bounds__(128, 1) k_track_step(TrackParams a, VmbLayout 
   double* part = a.partials + ((size_t)b * gridDim.x + blockIdx.x) * VMB_TRACK_PART;
   const int row = a.rows[b];
   if (row < 0 || row >= a.n_rows) {                   // uniform over the CTA
-    if (tid < VMB_TRACK_PART) part[tid] = 0.0;
+    if constexpr (BA) {
+      if (tid < nr && r0 + tid < R)
+        for (int c = 0; c < VMB_TRACK_PART; ++c) x.rows[((size_t)b * R + r0 + tid) * VMB_TRACK_PART + c] = 0.0;
+    } else if (tid < VMB_TRACK_PART) {
+      part[tid] = 0.0;
+    }
     if (tid == 0 && a.status) atomicOr(a.status, VMB_TRACK_ST_BAD_ROW);
     return;
   }
@@ -137,9 +161,16 @@ __global__ void __launch_bounds__(128, 1) k_track_step(TrackParams a, VmbLayout 
 
   // ---- A: point p = R q + t (fp32 copy of the fp64 pose), positional embedding of p / scale ---------------------------
   const double* T = a.pose;
+  bool pok = pvalid;                                  // K11: the ray's frame is in the pose table
+  if constexpr (BA) {
+    const int f = pvalid ? ba_draw_frame(x.kf_draw, x.kf_draw_stride, x.kf_frame, x.kf_stride, x.n_poses, b,
+                                         (r0 + rl) / x.n_pix_draw) : -1;
+    pok = f >= 0;
+    T = a.pose + (size_t)(pok ? f : 0) * 16;
+  }
   float q0 = 0.f, q1 = 0.f, q2 = 0.f, t0 = 0.f, t1 = 0.f, t2 = 0.f;
   const float sc = a.scale[row];
-  if (pvalid) {
+  if (pok) {
     const size_t gi = (size_t)b * a.pcs_stride + ((size_t)(r0 + rl) * S + sidx) * 3;
     q0 = a.pcs[gi]; q1 = a.pcs[gi + 1]; q2 = a.pcs[gi + 2];
     const float x = fmaf((float)T[2], q2, fmaf((float)T[1], q1, (float)T[0] * q0)) + (float)T[3];
@@ -250,8 +281,13 @@ __global__ void __launch_bounds__(128, 1) k_track_step(TrackParams a, VmbLayout 
 #pragma unroll
     for (int c = 0; c < 3; ++c) cnt[c] = s_cnt[c][0] + s_cnt[c][1] + s_cnt[c][2] + s_cnt[c][3];
     const int sv = a.sem[(size_t)b * a.sem_stride + ray];
-    const double m_o = (sv != 0) ? 1.0 : 0.0;
-    const double m_s = (sv != 2) ? 1.0 : 0.0;
+    bool rok = true;                          // K11: a ray whose frame is outside the pose table contributes nothing
+    if constexpr (BA) {
+      rok = ba_draw_frame(x.kf_draw, x.kf_draw_stride, x.kf_frame, x.kf_stride, x.n_poses, b, ray / x.n_pix_draw) >= 0;
+      if (!rok && a.status) atomicOr(a.status, VMB_BA_ST_BAD_FRAME);
+    }
+    const double m_o = (sv != 0 && rok) ? 1.0 : 0.0;
+    const double m_s = (sv != 2 && rok) ? 1.0 : 0.0;
     const double m_d = (a.mask[(size_t)b * a.mask_stride + ray] != 0) ? m_o : 0.0;
     const double gd = a.gt_depth[(size_t)b * a.gt_depth_stride + ray];
     const float* gc = a.gt_colour + (size_t)b * a.gt_colour_stride + (size_t)ray * 3;
@@ -363,7 +399,7 @@ __global__ void __launch_bounds__(128, 1) k_track_step(TrackParams a, VmbLayout 
 #pragma unroll
     for (int g = 0; g < NOG; ++g) { d0 += sHd[(g * 3) * PT + p]; d1 += sHd[(g * 3 + 1) * PT + p]; d2 += sHd[(g * 3 + 2) * PT + p]; }
     double c[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-    if (pvalid) {
+    if (pok) {
       const double g0 = (double)(d0 / sc), g1 = (double)(d1 / sc), g2 = (double)(d2 / sc);
       const double x0 = T[0] * q0 + T[1] * q1 + T[2] * q2;   // R q in fp64
       const double x1 = T[4] * q0 + T[5] * q1 + T[6] * q2;
@@ -375,7 +411,17 @@ __global__ void __launch_bounds__(128, 1) k_track_step(TrackParams a, VmbLayout 
     for (int i = 0; i < 6; ++i) s_g[i][p] = c[i];
   }
   __syncthreads();
-  if (tid < 6) {
+  if constexpr (BA) {                                       // per-ray rows: the ray's samples in order
+    if (tid < nr && r0 + tid < R) {
+      double* out = x.rows + ((size_t)b * R + r0 + tid) * VMB_TRACK_PART;
+      for (int c = 0; c < 6; ++c) {
+        double s = 0.0;
+        for (int i = 0; i < S; ++i) s += s_g[c][tid * S + i];
+        out[c] = s;
+      }
+      out[6] = s_l[0][tid]; out[7] = s_l[1][tid]; out[8] = s_l[2][tid]; out[9] = 0.0;
+    }
+  } else if (tid < 6) {
     double s = 0.0;
     for (int i = 0; i < np; ++i) s += s_g[tid][i];
     part[tid] = s;
@@ -386,6 +432,11 @@ __global__ void __launch_bounds__(128, 1) k_track_step(TrackParams a, VmbLayout 
   } else if (tid == 9) {
     part[9] = 0.0;
   }
+}
+
+template <int H, int TP>
+__global__ void __launch_bounds__(128, 1) k_track_step(TrackParams a, VmbLayout L) {
+  track_step_body<H, TP, false>(a, L, BaRays{});
 }
 
 template <int H, int TP>

@@ -22,6 +22,7 @@
 #include "k_hull.cuh"
 #include "k_render.cuh"
 #include "k_track.cuh"
+#include "k_ba.cuh"
 
 struct vmb_handle {
   int device, max_obj, H, nfreq;
@@ -464,6 +465,7 @@ int vmb_sample(vmb_handle* h, const vmb_sample_args* a, void* stream) {
   p.sem = a->sem; p.mask = a->mask_depth;
   p.st_rgbx = reinterpret_cast<const uchar4*>(a->store_rgbx); p.st_depth = a->store_depth; p.st_inst = a->store_inst;
   p.offset_dev = a->offset_dev;
+  p.camera_frame = a->camera_frame; p.kf_out = a->kf_out;
   p.st_twc = a->store_t_wc; p.kf_slot = a->kf_slot; p.bbox_flat = a->kf_bbox; p.obj_id = a->obj_id; p.kf_stride = a->kf_stride;
   if (a->n_obj > h->max_obj) return fail(h, VMB_E_ARG, "vmb_sample: n_obj exceeds the handle's max_obj");
   const int N = a->n_frames * a->n_pix;
@@ -1268,6 +1270,119 @@ int vmb_track_update(vmb_handle* h, const vmb_track_args* a, void* stream) {
   u.cs = a->colour_scaling; u.os = a->opacity_scaling;
   u.loss = a->loss; u.pose_hist = a->pose_hist; u.grad_hist = a->grad_hist; u.status = a->status;
   k_track_update<<<1, 256, 0, (cudaStream_t)stream>>>(u);
+  CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
+}  // extern "C"
+
+// ---- K11: bundle adjustment ------------------------------------------------------------------------------------------
+template <int H, int TP>
+static int launch_ba(vmb_handle* h, const TrackParams& tp, const BaRays& x, int tiles, cudaStream_t st) {
+  const size_t smem = track_smem<H, TP>(h->L);
+  static bool attr_set[64] = {};
+  if (!attr_set[h->device & 63]) {
+    CUDA_TRY(h, cudaFuncSetAttribute(k_ba_step<H, TP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_set[h->device & 63] = true;
+  }
+  k_ba_step<H, TP><<<dim3((unsigned)tiles, (unsigned)tp.B), 128, smem, st>>>(tp, h->L, x);
+  CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
+static int ba_common(vmb_handle* h, const vmb_ba_args* a, const char* who) {
+  if (!a) return fail(h, VMB_E_ARG, std::string(who) + ": null argument");
+  if (a->n_groups < 1 || a->n_groups > VMB_TRACK_MAX_GROUPS)
+    return fail(h, VMB_E_ARG, std::string(who) + ": n_groups must be in [1, 8]");
+  if (a->n_iter < 1 || a->iter < 1 || a->iter > a->n_iter)
+    return fail(h, VMB_E_ARG, std::string(who) + ": need n_iter >= 1 and 1 <= iter <= n_iter");
+  if (!a->poses || a->n_poses < 1) return fail(h, VMB_E_ARG, std::string(who) + ": need a pose table");
+  return VMB_OK;
+}
+
+static int ba_group_ok(const vmb_ba_group& g) {
+  if (g.n_obj < 1 || g.n_obj > 65535 || g.n_rows < 1 || g.n_rays < 1 || g.n_samples < 1 || g.n_pix_draw < 1 ||
+      g.n_rays % g.n_pix_draw != 0 || g.kf_stride < 1 || g.kf_draw_stride < g.n_rays / g.n_pix_draw)
+    return VMB_E_ARG;
+  if (!g.kf_draw || !g.kf_frame || !g.ray_rows || (long long)g.n_obj * g.n_rays > g.max_ray_rows) return VMB_E_ARG;
+  return VMB_OK;
+}
+
+extern "C" {
+
+int vmb_ba_step(vmb_handle* h, const vmb_ba_args* a, int group, void* stream) {
+  if (!h) return fail(h, VMB_E_ARG, "vmb_ba_step: null handle");
+  const int rc0 = ba_common(h, a, "vmb_ba_step");
+  if (rc0 != VMB_OK) return rc0;
+  if (group < 0 || group >= a->n_groups) return fail(h, VMB_E_ARG, "vmb_ba_step: group index outside [0, n_groups)");
+  const vmb_ba_group& g = a->group[group];
+  if (g.hidden != h->H) return fail(h, VMB_E_ARG, "vmb_ba_step: group hidden size differs from the handle's");
+  if (ba_group_ok(g) != VMB_OK)
+    return fail(h, VMB_E_ARG, "vmb_ba_step: bad counts, draw layout, keyframe tables or ray rows");
+  if (!g.rows || !g.pcs || !g.z_vals || !g.gt_depth || !g.gt_colour || !g.sem || !g.mask_depth || !g.params || !g.scale)
+    return fail(h, VMB_E_ARG, "vmb_ba_step: missing tensor pointer");
+  const int tiles = vmb_track_tiles(g.hidden, g.n_rays, g.n_samples);
+  if (tiles == VMB_E_UNSUPPORTED)
+    return fail(h, VMB_E_UNSUPPORTED, "vmb_ba_step: n_samples exceeds the tile size for this hidden size");
+  if (tiles < 1) return fail(h, VMB_E_ARG, "vmb_ba_step: bad shape");
+  TrackParams tp;
+  memset(&tp, 0, sizeof(tp));
+  tp.B = g.n_obj; tp.R = g.n_rays; tp.S = g.n_samples; tp.n_rows = g.n_rows; tp.rows = g.rows;
+  tp.pcs = g.pcs; tp.pcs_stride = g.pcs_stride; tp.z = g.z_vals; tp.z_stride = g.z_stride;
+  tp.gt_depth = g.gt_depth; tp.gt_depth_stride = g.gt_depth_stride;
+  tp.gt_colour = g.gt_colour; tp.gt_colour_stride = g.gt_colour_stride;
+  tp.sem = g.sem; tp.sem_stride = g.sem_stride; tp.mask = g.mask_depth; tp.mask_stride = g.mask_stride;
+  tp.params = g.params; tp.scale = g.scale; tp.pose = a->poses;
+  tp.cs = a->colour_scaling; tp.os = a->opacity_scaling; tp.status = a->status;
+  BaRays x;
+  x.kf_draw = g.kf_draw; x.kf_draw_stride = g.kf_draw_stride; x.kf_frame = g.kf_frame; x.kf_stride = g.kf_stride;
+  x.n_pix_draw = g.n_pix_draw; x.n_poses = a->n_poses; x.rows = g.ray_rows;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (h->H) {
+    case 32:  return launch_ba<32, 128>(h, tp, x, tiles, st);
+    case 64:  return launch_ba<64, 64>(h, tp, x, tiles, st);
+    case 128: return launch_ba<128, 64>(h, tp, x, tiles, st);
+    case 256: return launch_ba<256, 32>(h, tp, x, tiles, st);
+  }
+  return fail(h, VMB_E_UNSUPPORTED, "vmb_ba_step: unsupported hidden size");
+}
+
+int vmb_ba_update(vmb_handle* h, const vmb_ba_args* a, void* stream) {
+  if (!h) return fail(h, VMB_E_ARG, "vmb_ba_update: null handle");
+  const int rc0 = ba_common(h, a, "vmb_ba_update");
+  if (rc0 != VMB_OK) return rc0;
+  if (!a->adam || !a->window || !a->scratch) return fail(h, VMB_E_ARG, "vmb_ba_update: adam, window or scratch is NULL");
+  if (a->n_win < 1 || a->n_win > VMB_BA_MAX_WIN) return fail(h, VMB_E_ARG, "vmb_ba_update: n_win outside [1, 1024]");
+  if (!(std::isfinite(a->lr_rot) && a->lr_rot >= 0.0 && std::isfinite(a->lr_trans) && a->lr_trans >= 0.0 &&
+        a->beta1 >= 0.0 && a->beta1 < 1.0 && a->beta2 >= 0.0 && a->beta2 < 1.0 && a->eps > 0.0 && std::isfinite(a->eps)))
+    return fail(h, VMB_E_ARG, "vmb_ba_update: need finite rates >= 0, betas in [0, 1) and eps > 0");
+  BaUpdateParams u;
+  memset(&u, 0, sizeof(u));
+  u.n_groups = a->n_groups;
+  long long n_seg = 0;
+  for (int i = 0; i < a->n_groups; ++i) {
+    const vmb_ba_group& g = a->group[i];
+    if (ba_group_ok(g) != VMB_OK) return fail(h, VMB_E_ARG, "vmb_ba_update: bad group");
+    u.g[i].rows = g.ray_rows; u.g[i].n_obj = g.n_obj; u.g[i].n_rays = g.n_rays; u.g[i].n_pix_draw = g.n_pix_draw;
+    u.g[i].kf_draw = g.kf_draw; u.g[i].kf_draw_stride = g.kf_draw_stride;
+    u.g[i].kf_frame = g.kf_frame; u.g[i].kf_stride = g.kf_stride;
+    n_seg += (long long)g.n_obj * (g.n_rays / g.n_pix_draw);
+  }
+  if (8 * n_seg + 6LL * a->n_win > a->scratch_len) return fail(h, VMB_E_ARG, "vmb_ba_update: scratch too small");
+  for (int t = 0; t < 2; ++t) {
+    const vmb_ba_target& T = a->target[t];
+    if (T.t_wc && (!T.frame_of || T.n < 0)) return fail(h, VMB_E_ARG, "vmb_ba_update: target without frame_of");
+    u.tgt[t].frame_of = T.frame_of; u.tgt[t].t_wc = T.t_wc; u.tgt[t].n = T.t_wc ? T.n : 0;
+  }
+  u.iter = a->iter; u.n_iter = a->n_iter; u.n_poses = a->n_poses; u.n_win = a->n_win; u.hold = a->hold;
+  u.win = a->window; u.pose = a->poses; u.adam = a->adam; u.scratch = a->scratch;
+  for (int c = 0; c < 3; ++c) { u.lr[c] = a->lr_rot; u.lr[3 + c] = a->lr_trans; }
+  u.b1 = a->beta1; u.b2 = a->beta2; u.eps = a->eps;
+  u.bc1 = 1.0 - std::pow(a->beta1, (double)a->iter);
+  u.bc2 = 1.0 - std::pow(a->beta2, (double)a->iter);
+  u.cs = a->colour_scaling; u.os = a->opacity_scaling;
+  u.loss = a->loss; u.pose_hist = a->pose_hist; u.grad_hist = a->grad_hist; u.status = a->status;
+  k_ba_update<<<1, 256, 0, (cudaStream_t)stream>>>(u);
   CUDA_TRY(h, cudaGetLastError());
   return VMB_OK;
 }

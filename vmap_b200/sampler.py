@@ -71,8 +71,12 @@ class BatchedSampler:
             out["gt_rgb_u8"] = torch.empty(B, N, 3, dtype=torch.uint8, device=dev)
         return out
 
-    def _launch(self, a, out, B, n_frames, n_pix, W, H, rays_dir, seed, offset, inject, keep, offset_dev=None):
+    def _launch(self, a, out, B, n_frames, n_pix, W, H, rays_dir, seed, offset, inject, keep, offset_dev=None,
+                camera_frame=False, kf_out=None):
         dev = self.device
+        if kf_out is not None:
+            assert kf_out.dtype == torch.int32 and kf_out.shape == (B, n_frames) and kf_out.is_contiguous()
+        a.camera_frame, a.kf_out = int(bool(camera_frame)), _p(kf_out)
         a.n_obj, a.n_frames, a.n_pix = B, n_frames, n_pix
         a.n_bins_cam2surface, a.n_bins, a.width, a.height = self.n1, self.n2, W, H
         a.min_bound, a.surface_eps, a.stop_eps = self.min_bound, self.eps, self.oeps
@@ -95,12 +99,13 @@ class BatchedSampler:
 
     def sample(self, objects: List[KeyframeSet], n_frames: int, n_pix: int, rays_dir: torch.Tensor,
                seed: int = 0, offset: int = 0, inject: Optional[Dict[str, torch.Tensor]] = None,
-               want_u8: bool = False, tables: Optional["SamplerTables"] = None, out=None, offset_dev=None
-               ) -> Dict[str, torch.Tensor]:
+               want_u8: bool = False, tables: Optional["SamplerTables"] = None, out=None, offset_dev=None,
+               camera_frame: bool = False, kf_out: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
         """Per-object keyframe buffers (the reference's layout, vmap.py:137-176).
         ``tables`` / ``out`` / ``offset_dev``: persistent table + output buffers and a device draw counter, for
         CUDA-graph capture of a whole frame (frame.FrameLoop); with ``tables`` the caller has already filled and
-        uploaded them and ``objects`` is ignored."""
+        uploaded them and ``objects`` is ignored.  ``camera_frame``: take every keyframe pose as identity (camera-frame
+        points); ``kf_out`` [B, n_frames] int32: receives the keyframe index of each draw."""
         dev = self.device
         N, S = n_frames * n_pix, self.n1 + self.n2
         if tables is None:
@@ -112,14 +117,17 @@ class BatchedSampler:
         assert out["pcs"].shape == (B, N, S, 3) and out["sem"].shape == (B, N)
         a = _lib.SampleArgs()
         tables.bind(a)
-        return self._launch(a, out, B, n_frames, n_pix, W, H, rays_dir, seed, offset, inject, tables, offset_dev)
+        return self._launch(a, out, B, n_frames, n_pix, W, H, rays_dir, seed, offset, inject, tables, offset_dev,
+                            camera_frame, kf_out)
 
     def sample_store(self, store, tables, n_frames: int, n_pix: int, rays_dir: torch.Tensor,
                      seed: int = 0, offset: int = 0, inject: Optional[Dict[str, torch.Tensor]] = None,
-                     want_u8: bool = False, out=None, offset_dev=None) -> Dict[str, torch.Tensor]:
+                     want_u8: bool = False, out=None, offset_dev=None, camera_frame: bool = False,
+                     kf_out: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
         """Shared keyframe store (keyframes.FrameStore): frames stored once, per-object (slot, bbox) tables,
         pixel state derived from the instance image.  Same draws / outputs as ``sample`` on per-object copies.
-        ``tables``: a ``KeyframeTables`` (packed and uploaded here) or an already uploaded ``SamplerTables``."""
+        ``tables``: a ``KeyframeTables`` (packed and uploaded here) or an already uploaded ``SamplerTables``.
+        ``camera_frame`` / ``kf_out``: as ``sample``."""
         dev = self.device
         assert store.device == dev
         if isinstance(tables, KeyframeTables):
@@ -134,7 +142,8 @@ class BatchedSampler:
         a = _lib.SampleArgs()
         a.store_rgbx, a.store_depth, a.store_inst, a.store_t_wc = _p(store.rgbx), _p(store.depth), _p(store.inst), _p(store.t_wc)
         tables.bind(a)
-        return self._launch(a, out, B, n_frames, n_pix, store.W, store.H, rays_dir, seed, offset, inject, tables, offset_dev)
+        return self._launch(a, out, B, n_frames, n_pix, store.W, store.H, rays_dir, seed, offset, inject, tables, offset_dev,
+                            camera_frame, kf_out)
 
 
 class SamplerTables:

@@ -24,23 +24,33 @@ device synchronise and the capture) and later frames replay.  ``track_modes`` re
 
 The frame store starts small and doubles when a new frame finds no free slot, up to ``max_n_models *
 keyframe_buffer_size + 1`` slots: every object holds at most ``keyframe_buffer_size`` keyframe slots, and the live
-frame holds one.  Growing reallocates the frames, so both captured graphs are captured again.
+frame holds one.  Growing reallocates the frames, so the captured graphs are captured again.
+
+With ``ba_every`` > 0, every ``ba_every`` frames a bundle-adjustment pass (``ba.BundleAdjuster``, K11) runs after the
+mapping frame: ``n_ba_iter`` pose-only iterations against the frozen map move every keyframe pose the objects' keyframe
+tables hold (never frame 0, the anchor), and the refined poses go to ``poses``, the store and the background's
+copies, where the next mapping frames, the motion model, ``get_bound`` and meshing read them.  Its graph follows the
+same eager / capture / replay pattern (``ba_modes``).
 """
 from __future__ import annotations
 
 from typing import Dict, List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib
 from .frame import Background, FrameLoop
 from .keyframes import FrameStore
+from .ba import BundleAdjuster
 from .sampler import BatchedSampler
 from .track import Tracker, _rays_dir, groups_from_objects
 from .vmap import keyframe_tables, sceneObject
 
 # the tracker's sampler key: tracking frame k must not reuse the Philox streams that mapped frame k - 1
 _TRACK_SEED = 0x2545F491
+# the bundle adjuster's sampler key, distinct from the mapping frames' and the tracker's
+_BA_SEED = 0x61C88647
 
 
 def _inv_se3(T: torch.Tensor) -> torch.Tensor:
@@ -67,14 +77,21 @@ class Slam:
     map loaded from checkpoints).  ``graph``: replay the tracking frame and the mapping frame as CUDA graphs while the
     tracked set and the object set stay the same.  ``n_track_iter`` / ``lr_rot`` / ``lr_trans``: the tracker's
     iterations and rates (default ``cfg.pose_lr``).  ``store_capacity``: the frame store's initial number of slots (it
-    grows on demand).  ``timing``: record CUDA events at the phase boundaries of every frame (``phase_times``)."""
+    grows on demand).  ``timing``: record CUDA events at the phase boundaries of every frame (``phase_times``).
+    ``ba_every``: run a bundle-adjustment pass after the mapping frame of every ``ba_every``-th frame (0: never);
+    ``n_ba_iter`` / ``ba_lr_rot`` / ``ba_lr_trans``: its iterations and rates (default ``cfg.pose_lr``)."""
 
     def __init__(self, cfg, T_init=None, track: bool = True, map: bool = True, groups=None, graph: bool = True,
                  n_track_iter: int = 20, lr_rot: Optional[float] = None, lr_trans: Optional[float] = None,
                  seed: int = 0, max_frames: int = 100000, background_cls: Sequence[int] = (), bbox_scale: float = 0.2,
-                 store_capacity: Optional[int] = None, max_id: int = 4096, timing: bool = False):
+                 store_capacity: Optional[int] = None, max_id: int = 4096, timing: bool = False, ba_every: int = 0,
+                 n_ba_iter: int = 20, ba_lr_rot: Optional[float] = None, ba_lr_trans: Optional[float] = None):
         if not track and not map:
             raise ValueError("Slam: nothing to do with track=False and map=False")
+        if ba_every < 0 or n_ba_iter < 1:
+            raise ValueError("Slam: need ba_every >= 0 and n_ba_iter >= 1")
+        if ba_every and not map:
+            raise ValueError("Slam: bundle adjustment (ba_every > 0) refines the poses of a map being built: map=True")
         if not map and groups is None:
             raise ValueError("Slam(map=False) localises against a given map: pass groups")
         self.cfg, self.do_track, self.do_map, self.graph = cfg, track, map, graph
@@ -100,6 +117,15 @@ class Slam:
         self.inserted: Dict[int, int] = {}               # object id -> frame it was inserted at
         self.k = 0
         self.timing, self.events = timing, []
+        # bundle adjustment (off: nothing is allocated or launched)
+        self.ba_every = ba_every
+        self.ba_kw = dict(n_iter=n_ba_iter, lr_rot=ba_lr_rot, lr_trans=ba_lr_trans, seed=seed + _BA_SEED)
+        self.ba: Optional[BundleAdjuster] = None
+        self.ba_loss = torch.full((max_frames,), float("nan"), **f64) if ba_every else None
+        self.ba_frames: List[List[int]] = []
+        self.ba_modes: List[str] = []                    # per frame: "", "eager", "capture" or "replay"
+        self._ba_events: Dict[int, tuple] = {}
+        self._ba_seen = False
         # the map
         self.objects: Dict[int, sceneObject] = {}         # objects of the packed stack (the reference's obj_dict)
         self.scene_bg: Optional[sceneObject] = None
@@ -170,6 +196,11 @@ class Slam:
         self._mark()
         if self.do_map:
             self._map_frame(slot, k, visible, pose)
+        if self.ba_every:
+            self.ba_frames.append([])
+            self.ba_modes.append("")
+            if self.objects and (k + 1) % self.ba_every == 0:
+                self._bundle_adjust(k)
         store.release(slot)
         self._mark()
         self.k += 1
@@ -185,15 +216,19 @@ class Slam:
 
     def phase_times(self) -> dict:
         """With ``timing``: per frame, device milliseconds of ``ingest`` (with the keep-flag read), ``track``,
-        ``bookkeeping`` (keyframes, insertion, tables: host work the device waits for) and ``map``, and ``frame``."""
+        ``bookkeeping`` (keyframes, insertion, tables: host work the device waits for) and ``map``, ``ba`` (the
+        bundle-adjustment pass with its table fill; 0.0 where none ran) and ``frame``."""
         torch.cuda.synchronize(self.device)
-        out = {k: [] for k in ("ingest", "track", "bookkeeping", "map", "frame")}
-        for ev in self.events:
+        out = {k: [] for k in ("ingest", "track", "bookkeeping", "map", "ba", "frame")}
+        for k, ev in enumerate(self.events):
             d = [a.elapsed_time(b) for a, b in zip(ev[:-1], ev[1:])]
             if len(d) == 3:                                # no mapping mark (map=False)
                 d = d[:2] + [d[2], 0.0]
+            ba = self._ba_events[k][0].elapsed_time(self._ba_events[k][1]) if k in self._ba_events else 0.0
+            d[3] -= ba                                     # the pass runs inside the last interval, after the map
             for key, v in zip(("ingest", "track", "bookkeeping", "map"), d):
                 out[key].append(v)
+            out["ba"].append(ba)
             out["frame"].append(ev[0].elapsed_time(ev[-1]))
         return out
 
@@ -223,6 +258,8 @@ class Slam:
             self.loop.graph = None                        # FrameLoop.run captures again
         if self.tracker is not None:
             self.tracker.graph, self.tracker._graph_keep = None, None
+        if self.ba is not None:
+            self.ba.graph, self._ba_seen = None, False     # eager on the next pass, then captured again
 
     # ---- mapping (train.py:104-326 on the package's GPU path) --------------------------------------------------------
     def _map_frame(self, slot: int, k: int, visible: Dict[int, torch.Tensor], pose: torch.Tensor) -> None:
@@ -292,6 +329,13 @@ class Slam:
             self.loop.counter.copy_(old.counter)          # the sampler's draw counter runs on across re-stacks
         if self.do_track:
             self._rebuild_tracker()
+        if self.ba_every:
+            old = self.ba
+            self.ba = BundleAdjuster(groups_from_objects(self._ba_objects().values()), cfg, self._ba_objects(),
+                                     hold=0, **self.ba_kw)
+            if old is not None:
+                self.ba.counter.copy_(old.counter)        # the pass's draw counter runs on across re-stacks too
+            self._ba_seen = False
 
     def _rebuild_tracker(self) -> None:
         objs = list(self.objects.values()) + ([self.scene_bg] if self.scene_bg is not None else [])
@@ -303,14 +347,51 @@ class Slam:
         self._tracked_set = None
         self.mapped = {i for _, ids in groups for i in ids if i is not None}
 
+    # ---- bundle adjustment -------------------------------------------------------------------------------------------
+    def _ba_objects(self) -> Dict[int, sceneObject]:
+        objs = dict(self.objects)
+        if self.scene_bg is not None:
+            objs[0] = self.scene_bg
+        return objs
+
+    def _bundle_adjust(self, k: int) -> None:
+        """One pass after frame k's mapping frame: eager on the first pass of an object set, captured on the second,
+        replayed after that (with ``graph``)."""
+        ba, objs = self.ba, self._ba_objects()
+        if self.timing:
+            e0 = torch.cuda.Event(enable_timing=True)
+            e0.record()
+        if not self.graph or not self._ba_seen:
+            win = ba.run(self.store, self.poses, objs)
+            self._ba_seen, mode = True, "eager"
+        else:
+            mode = "replay"
+            if ba.graph is None or ba._cap != self.store.capacity:
+                ba.capture(self.store, self.poses, objs)
+                mode = "capture"
+            win = ba.replay(self.store, self.poses, objs)
+        if self.timing:
+            e1 = torch.cuda.Event(enable_timing=True)
+            e1.record()
+            self._ba_events[len(self.events) - 1] = (e0, e1)
+        if win:
+            self.ba_loss[k] = ba.losses[-1]
+            self.ba_frames[-1] = list(win)
+            self.ba_modes[-1] = mode
+
     # ---- the record --------------------------------------------------------------------------------------------------
     def result(self) -> dict:
         """The per-frame record read back (one copy at the end): ``poses`` [N, 4, 4] fp64, ``lost`` [N] bool,
         ``track_loss`` [N] fp64 (the tracker's last iteration; nan where not tracked), ``map_loss`` [N] (the last
-        mapping iteration; nan where not mapped), ``tracked_ids``, ``inserted`` {object id: frame}, ``track_modes``
-        and the frame store's final ``store_capacity``."""
+        mapping iteration; nan where not mapped), ``tracked_ids``, ``inserted`` {object id: frame}, ``track_modes``,
+        the frame store's final ``store_capacity``, ``ba_loss`` [N] fp64 (the last bundle-adjustment iteration's
+        loss at frames where a pass ran; nan elsewhere), ``ba_frames`` (per frame, the frame ids its pass moved) and
+        ``ba_modes``."""
         n = self.k
-        return {"poses": self.poses[:n].cpu().numpy(), "lost": self.lost[:n].cpu().numpy(),
+        ba_loss = self.ba_loss[:n].cpu().numpy() if self.ba_loss is not None else np.full(n, np.nan)
+        return {"ba_loss": ba_loss, "ba_frames": [list(f) for f in self.ba_frames] or [[] for _ in range(n)],
+                "ba_modes": list(self.ba_modes) or [""] * n,
+                "poses": self.poses[:n].cpu().numpy(), "lost": self.lost[:n].cpu().numpy(),
                 "track_loss": self.track_loss[:n].cpu().numpy(), "map_loss": self.map_loss[:n].cpu().numpy(),
                 "tracked_ids": [list(i) for i in self.tracked_ids], "inserted": dict(self.inserted),
                 "track_modes": list(self.track_modes), "store_capacity": self.store.capacity}

@@ -3,7 +3,7 @@
 The reference never estimates a pose: it reads GT poses (dataset.py:135) or takes them from an external tracker in
 live mode.  ``Tracker`` closes that loop with the networks the map already has.  Per frame:
 
-    K3 once per group on the new frame with an identity pose (one keyframe: the frame's slot and each object's box
+    K3 once per group on the new frame in the camera frame (one keyframe: the frame's slot and each object's box
       from this frame's ingest; the full frame for the background)  -> camera-frame points q
       -> n_iter x [ vmb_track_step per group on the iteration's ray slice -> vmb_track_update (Adam + Exp) ]
 
@@ -140,7 +140,6 @@ class Tracker:
         self.grad_hist = torch.zeros(n_iter, 6, **f64) if record else None
         self.counter = torch.zeros(1, dtype=torch.int64, device=dev)       # sampler draw counter, +1 per frame
         self.slot_dev = torch.zeros(1, dtype=torch.int64, device=dev)
-        self.eye32 = torch.eye(4, dtype=torch.float32, device=dev)[None]
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self._graph_keep = None
 
@@ -175,13 +174,12 @@ class Tracker:
     # ---- the frame ---------------------------------------------------------------------------------------------------
     def _enqueue(self, store, upload: bool = True) -> None:
         live = self._live()
-        store.t_wc.index_copy_(0, self.slot_dev, self.eye32)            # sample the frame with an identity pose
         for gi, g in enumerate(live):
             if upload:
                 g.tables.upload()
             g.boxes_to_device(store)
             g.smp.sample_store(store, g.tables, self.n_iter, g.n_pix, self.rays_dir, seed=self.seed + 0x9e3779b9 * gi,
-                               out=g.out, offset_dev=self.counter)
+                               out=g.out, offset_dev=self.counter, camera_frame=True)
         self.counter += 1
         self._args = _iterate(live, self.n_iter, self.pose, self.adam, self.lr_rot, self.lr_trans, self.losses,
                               self.status, self.pose_hist, self.grad_hist)
