@@ -680,6 +680,21 @@ typedef struct vmb_ba_args {
 int vmb_ba_step(vmb_handle* h, const vmb_ba_args* a, int group, void* stream);
 int vmb_ba_update(vmb_handle* h, const vmb_ba_args* a, void* stream);
 
+/* ---- K10 / K11 on the layer-wise tensor-core path (the rule is in csrc/k_track_lw.cuh) ------------------------------
+ * The same step as vmb_track_step / vmb_ba_step for the wide models (hidden 64/128/256, n_freq 6), with the network
+ * on the wgmma GEMMs of the layer-wise training path, reading each object's weights from the ensemble's fp16 image
+ * `image` ([n_rows][vmb_image_bytes], as the AdamW launch writes it; row rows[b] for object b, as params).  Writes the
+ * same rows as vmb_track_step (K10's partials: vmb_track_tiles rows per object) and vmb_ba_step (one row per ray), so
+ * vmb_track_update and vmb_ba_update run unchanged.  No floating-point atomics: bitwise reproducible.
+ * Argument checks as vmb_track_step / vmb_ba_step; VMB_E_ARG also for a NULL image; VMB_E_UNSUPPORTED for hidden 32
+ * (stays on vmb_track_step / vmb_ba_step) and n_samples > 32.  On the device, besides the bits of K10 / K11: a
+ * loss-scaled gradient that reaches the fp16 clamp (+-60000) sets VMB_TRACK_ST_CLAMP and adds to status[1] a lower
+ * bound on the number of clamped values (the colour-hidden gradient and the rank-1 alpha term; the saturating
+ * packs of the dY4..dY1 GEMMs are not counted).                                                                                              */
+enum { VMB_TRACK_ST_CLAMP = 16 };
+int vmb_track_step_lw(vmb_handle* h, const vmb_track_args* a, int group, const void* image, void* stream);
+int vmb_ba_step_lw(vmb_handle* h, const vmb_ba_args* a, int group, const void* image, void* stream);
+
 /* ---- bring-up / test hook (not part of the reference-facing surface) --------------------------- */
 /* Generic wgmma GEMM of the layer-wise wide-model path: D[M][N] = A[M][K1+K2] * B[N][K]^T, fp16 in,
  * fp32 accumulate.  a_mn/b_mn = 0: operand stored [rows][ld] with K contiguous; 1: stored [K][ld] with

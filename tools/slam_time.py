@@ -11,7 +11,8 @@ the next frame with that set captures the tracking graph (a warm-up frame, a syn
 frames replay it.  With ``--ba-every`` (one run per value; 0 = no bundle adjustment) the bundle-adjustment phase is
 reported too, by pass mode, and after the run the device time of one BA iteration per group (``vmb_ba_step`` on each
 ensemble) and of ``vmb_ba_update``, over repeated launches.  The card's name and power limit are read in the same
-run."""
+run.  ``--imap`` runs the iMAP settings instead (one hidden-256 scene model, every pixel instance 0);
+``--track-impl`` / ``--ba-impl`` choose ``fp32`` or ``layerwise`` (default: layer-wise in iMAP mode, fp32 otherwise)."""
 from __future__ import annotations
 
 import argparse
@@ -35,12 +36,15 @@ def main(argv=None):
     ap.add_argument("--frames", type=int, default=40)
     ap.add_argument("--ba-every", default="0", help="comma-separated ba_every values, one run each")
     ap.add_argument("--ba-iter", type=int, default=20)
+    ap.add_argument("--imap", action="store_true", help="the iMAP settings: one hidden-256 scene model")
+    ap.add_argument("--track-impl", choices=("fp32", "layerwise"), default=None)
+    ap.add_argument("--ba-impl", choices=("fp32", "layerwise"), default=None)
     args = ap.parse_args(argv)
     assert torch.cuda.is_available(), "slam_time measures the GPU; there is no CPU number"
-    cfg = Config(config_dict=replica_room0_dict())
+    cfg = Config(config_dict=replica_room0_dict(imap=args.imap))
     seq = synth.sphere_room_sequence(args.frames, cfg.W, cfg.H, cfg.fx, cfg.fy, cfg.cx, cfg.cy, n_extra=16)
     for every in [int(x) for x in args.ba_every.split(",")]:
-        run(cfg, seq, args.frames, every, args.ba_iter)
+        run(cfg, seq, args.frames, every, args.ba_iter, args.track_impl, args.ba_impl)
 
 
 def ba_iteration_ms(slam, reps: int = 50) -> dict:
@@ -49,12 +53,12 @@ def ba_iteration_ms(slam, reps: int = 50) -> dict:
     import ctypes as C
     from vmap_b200 import _lib
     from vmap_b200.ensemble import _stream
+    from vmap_b200.track import _step
     ba = slam.ba
     a = ba._args
     out = {}
     for gi, g in enumerate(ba.groups):
-        fn = lambda: _lib.check(g.ens._handle, g.ens.lib.vmb_ba_step(g.ens._handle, C.byref(a), gi, _stream()), "step")
-        out[f"step_h{g.ens.hidden}_x{len(g.rows)}"] = _event_ms(fn, reps)
+        out[f"step_h{g.ens.hidden}_x{len(g.rows)}"] = _event_ms(lambda g=g, gi=gi: _step(g, a, gi, ba=True), reps)
     e = ba.groups[0].ens
     out["update"] = _event_ms(lambda: _lib.check(e._handle, e.lib.vmb_ba_update(e._handle, C.byref(a), _stream()),
                                                  "update"), reps)
@@ -73,10 +77,10 @@ def _event_ms(fn, reps):
     return round(s.elapsed_time(t) / reps, 4)
 
 
-def run(cfg, seq, frames, ba_every, ba_iter):
+def run(cfg, seq, frames, ba_every, ba_iter, track_impl=None, ba_impl=None):
     args = argparse.Namespace(frames=frames)
     slam = Slam(cfg, T_init=seq["poses"][0], background_cls=seq["background_cls"], max_frames=args.frames,
-                timing=True, ba_every=ba_every, n_ba_iter=ba_iter)
+                timing=True, ba_every=ba_every, n_ba_iter=ba_iter, track_impl=track_impl, ba_impl=ba_impl)
     for k in range(args.frames):
         slam.step(torch.from_numpy(seq["rgb"][k]), torch.from_numpy(seq["depth"][k].astype(np.float32)),
                   torch.from_numpy(seq["inst"][k]), torch.from_numpy(seq["cls"][k]))
@@ -97,7 +101,8 @@ def run(cfg, seq, frames, ba_every, ba_iter):
                                 for m in ("eager", "capture", "replay")
                                 for v in [[t["track"][i] for i, mm in enumerate(res["track_modes"]) if mm == m]] if v},
            "lost": int(res["lost"].sum()), "ate_rmse_m": ate["rmse"], "rpe_trans_rmse_m": rpe["trans_rmse"],
-           "rpe_rot_rmse_deg": rpe["rot_rmse_deg"], "ba_every": ba_every}
+           "rpe_rot_rmse_deg": rpe["rot_rmse_deg"], "ba_every": ba_every, "imap": bool(cfg.imap_mode),
+           "track_impl": slam.track_kw["impl"], "ba_impl": slam.ba_kw["impl"]}
     if ba_every:
         out["ba_iters"] = ba_iter
         out["ba_ms_by_mode"] = {m: {"frames": len(v), "median": round(float(np.median(v)), 3)}

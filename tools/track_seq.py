@@ -65,6 +65,10 @@ def main(argv=None):
     ap.add_argument("--ba-every", type=int, default=0,
                     help="--slam: a bundle-adjustment pass after every N-th mapping frame (0: none)")
     ap.add_argument("--ba-iter", type=int, default=20, help="bundle-adjustment iterations per pass")
+    ap.add_argument("--track-impl", choices=("fp32", "layerwise"), default=None,
+                    help="tracking step (default: layerwise for iMAP configs, fp32 otherwise)")
+    ap.add_argument("--ba-impl", choices=("fp32", "layerwise"), default=None,
+                    help="bundle-adjustment step (default: layerwise for iMAP configs, fp32 otherwise)")
     args = ap.parse_args(argv)
     cfg = Config(args.config)
     if cfg.dataset_format != "Replica":
@@ -81,9 +85,9 @@ def main(argv=None):
     frames = list(range(a, min(b, n)))
     kw = dict(n_track_iter=args.n_iter, seed=args.seed, background_cls=REPLICA_BACKGROUND_CLS,
               bbox_scale=REPLICA_BBOX_SCALE, max_frames=len(frames), timing=True,
-              store_capacity=args.store_capacity)
+              store_capacity=args.store_capacity, track_impl=args.track_impl)
     if args.slam:
-        slam = Slam(cfg, T_init=gt_all[a], ba_every=args.ba_every, n_ba_iter=args.ba_iter, **kw)
+        slam = Slam(cfg, T_init=gt_all[a], ba_every=args.ba_every, n_ba_iter=args.ba_iter, ba_impl=args.ba_impl, **kw)
     else:
         sources, skipped = load_sources(args.ckpt_dir, args.frame, device=cfg.data_device)
         if skipped:

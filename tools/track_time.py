@@ -4,9 +4,13 @@
 synthetic 1200 x 680 frame ingested into a FrameStore.  Reports the sampler time, the per-iteration step time of each
 group and of the update, each launched alone (CUDA events over many launches), the whole frame eager (host clock around a synchronised
 frame) and as a graph replay, the FLOPs from shapes (forward plus the backward to the inputs, 4 (4H^2 + 220H + 63) per
-point) and their share of the H100 SXM fp32 data-sheet rate (67 TFLOP/s), with the card's name and power limit."""
+point) and their share of the H100 SXM fp32 data-sheet rate (67 TFLOP/s), with the card's name and power limit.
+
+``--impl layerwise`` times the tensor-core path for the hidden-128 background (hidden 32 stays on K10); ``--imap`` times
+the iMAP shape instead: one hidden-256 scene model, 4800 rays x 14 samples over the full frame."""
 from __future__ import annotations
 
+import argparse
 import json
 import os
 import subprocess
@@ -21,7 +25,7 @@ from oracle import vmap_oracle as vo  # noqa: E402
 from vmap_b200.cfg import Config, replica_room0_dict  # noqa: E402
 from vmap_b200.ensemble import VmapEnsemble  # noqa: E402
 from vmap_b200.keyframes import FrameStore  # noqa: E402
-from vmap_b200.track import Tracker, _iterate  # noqa: E402
+from vmap_b200.track import Tracker, _iterate, _step  # noqa: E402
 
 FP32_PEAK = 67e12
 
@@ -50,11 +54,15 @@ def ev_time(fn, n):
     return e0.elapsed_time(e1) * 1e3 / n          # us
 
 
-def main():
+def main(argv=None):
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("--impl", choices=("fp32", "layerwise"), default="fp32")
+    ap.add_argument("--imap", action="store_true", help="the iMAP shape: one hidden-256 model, 4800 x 14")
+    args = ap.parse_args(argv)
     assert torch.cuda.is_available(), "track_time measures the GPU; there is no CPU number"
     dev = "cuda:0"
-    cfg = Config(config_dict=replica_room0_dict())
-    n_iter, n_obj = 20, 20
+    cfg = Config(config_dict=replica_room0_dict(imap=args.imap))
+    n_iter, n_obj = 20, (0 if args.imap else 20)
     W, H = cfg.W, cfg.H
     g = torch.Generator().manual_seed(0)
     inst = torch.zeros(W, H, dtype=torch.int32)
@@ -65,15 +73,20 @@ def main():
     rgb = torch.randint(0, 256, (W, H, 3), generator=g, dtype=torch.uint8)
     store = FrameStore(W, H, 2, device=dev, max_id=64)
     slot, _, _ = store.ingest(rgb, depth, inst, torch.eye(4))
-    objs = VmapEnsemble(n_obj, hidden=32, scale=2.0, impl="fp32")
-    objs.load_stacked(vo.init_params(n_obj, 32, seed=1))
-    bg = VmapEnsemble(1, hidden=128, scale=5.0, impl="fp32")
-    bg.load_stacked(vo.init_params(1, 128, seed=2))
-    groups = [(objs, list(range(1, n_obj + 1))), (bg, [0])]
+    if args.imap:                                           # one scene model over the whole frame (dataset.py:95-96)
+        scene = VmapEnsemble(1, hidden=256, scale=cfg.obj_scale, impl="fp32")
+        scene.load_stacked(vo.init_params(1, 256, seed=2))
+        groups = [(scene, [0])]
+    else:
+        objs = VmapEnsemble(n_obj, hidden=32, scale=2.0, impl="fp32")
+        objs.load_stacked(vo.init_params(n_obj, 32, seed=1))
+        bg = VmapEnsemble(1, hidden=128, scale=5.0, impl="fp32")
+        bg.load_stacked(vo.init_params(1, 128, seed=2))
+        groups = [(objs, list(range(1, n_obj + 1))), (bg, [0])]
     T0 = np.eye(4)
     ids = list(range(n_obj + 1))
 
-    tr = Tracker(groups, cfg, n_iter=n_iter)
+    tr = Tracker(groups, cfg, n_iter=n_iter, impl=args.impl)
     tr.track(store, slot, T0, ids=ids)
     torch.cuda.synchronize()
     live = tr._live()
@@ -108,11 +121,16 @@ def main():
         tr.run(store, slot, T0)
     torch.cuda.synchronize()
     t_graph = (time.perf_counter() - t0) * 1e6 / reps
-    pts = {32: n_obj * cfg.n_per_optim * 10, 128: cfg.n_per_optim_bg * 14}
+    if args.imap:
+        pts = {256: cfg.n_per_optim * 14}
+        shape = {"scene": f"h256 x {cfg.n_per_optim} rays x 14", "n_iter": n_iter}
+    else:
+        pts = {32: n_obj * cfg.n_per_optim * 10, 128: cfg.n_per_optim_bg * 14}
+        shape = {"objects": f"{n_obj} x h32 x {cfg.n_per_optim} rays x 10",
+                 "background": f"h128 x {cfg.n_per_optim_bg} rays x 14", "n_iter": n_iter}
     flop_iter = sum(flops_per_point(h) * n for h, n in pts.items())
     out = {
-        "card": card(), "shape": {"objects": f"{n_obj} x h32 x {cfg.n_per_optim} rays x 10",
-                                  "background": f"h128 x {cfg.n_per_optim_bg} rays x 14", "n_iter": n_iter},
+        "card": card(), "impl": args.impl, "shape": shape,
         "sampler_us": round(t_sample, 2), "step_us": {k: round(v, 2) for k, v in step_us.items()},
         "update_us": round(t_update, 2), "iteration_us": round(t_iter, 2),
         "frame_eager_us": round(t_eager, 1), "frame_graph_us": round(t_graph, 1),
@@ -141,10 +159,9 @@ def _update_only(tr, live):
 
 
 def _iterate_one(tr, live, gi):
-    """vmb_track_step of group gi alone on iteration 0's slice (the update is timed with the whole iteration)."""
-    import ctypes as C
+    """The step of group gi alone on iteration 0's slice (the update is timed with the whole iteration)."""
     from vmap_b200 import _lib
-    from vmap_b200.ensemble import _ptr, _stream
+    from vmap_b200.ensemble import _ptr
     from vmap_b200.track import _Group
     a = _lib.TrackArgs()
     a.n_groups, a.n_iter, a.iter = len(live), tr.n_iter, 1
@@ -152,8 +169,7 @@ def _iterate_one(tr, live, gi):
     a.colour_scaling, a.opacity_scaling = 5.0, 10.0
     for k, gr in enumerate(live):
         _Group.bind(gr, a.group[k], 0)
-    e = live[gi].ens
-    _lib.check(e._handle, e.lib.vmb_track_step(e._handle, C.byref(a), gi, _stream()), "vmb_track_step")
+    _step(live[gi], a, gi, ba=False)
 
 
 if __name__ == "__main__":

@@ -8,7 +8,8 @@ pose-only passes against the frozen map: per pass
       -> the refined poses written to the fp64 pose table, the frame store's slots and the background's copies
 
 all on the device, so a pass can be captured as one CUDA graph (``capture`` / ``run``).  The rule is in
-``csrc/k_ba.cuh``; ``oracle/ba_oracle.py`` restates it.
+``csrc/k_ba.cuh``; ``oracle/ba_oracle.py`` restates it.  ``impl="layerwise"`` runs the step of every hidden-64/128/256
+group on the tensor-core path (``vmb_ba_step_lw``, ``csrc/k_track_lw.cuh``), as ``Tracker`` does.
 """
 from __future__ import annotations
 
@@ -21,17 +22,18 @@ import torch
 from . import _lib
 from .ensemble import VmapEnsemble, _ptr, _stream
 from .sampler import BatchedSampler, SamplerTables
-from .track import _rays_dir
+from .track import _rays_dir, _step, _use_lw
 
 
 class _BaGroup:
     """One ensemble's share of a pass: the shared-store objects of the mapping stack, or the ``do_bg`` background with
     its own keyframe copies.  Rows are those ``obj_ids`` names."""
 
-    def __init__(self, ens: VmapEnsemble, obj_ids: Sequence[Optional[int]], cfg, n_iter: int, bg: bool):
+    def __init__(self, ens: VmapEnsemble, obj_ids: Sequence[Optional[int]], cfg, n_iter: int, bg: bool,
+                 impl: str = "fp32"):
         ids = [None if i is None or int(i) < 0 else int(i) for i in obj_ids]
         assert len(ids) == ens.n_obj, "obj_ids must name every row of the ensemble (None / -1 = not an object)"
-        self.ens, self.ids, self.bg = ens, ids, bg
+        self.ens, self.ids, self.bg, self.lw = ens, ids, bg, _use_lw(ens, impl)
         self.rows = [r for r, i in enumerate(ids) if i is not None]
         B = len(self.rows)
         assert B > 0
@@ -100,17 +102,20 @@ class BundleAdjuster:
     for rows that are not objects), as ``track.groups_from_objects`` builds them; a group whose objects keep their own
     keyframe copies (the ``do_bg`` background) samples those.  ``n_iter`` iterations per pass in the mapping layout;
     rates default to ``cfg.pose_lr``; ``hold`` (the anchor frame) never moves.  ``record``: keep each pass's pose and
-    gradient history per window entry (``pose_hist`` [n_iter+1, max_win, 4, 4], ``grad_hist`` [n_iter, max_win, 6])."""
+    gradient history per window entry (``pose_hist`` [n_iter+1, max_win, 4, 4], ``grad_hist`` [n_iter, max_win, 6]).
+    ``impl``: ``"fp32"`` (K11 for every group) or ``"layerwise"`` (the tensor-core path for hidden 64/128/256)."""
 
     def __init__(self, groups: Sequence[Tuple[VmapEnsemble, Sequence[Optional[int]]]], cfg, objects: Dict[int, object],
                  n_iter: int = 20, lr_rot: Optional[float] = None, lr_trans: Optional[float] = None, seed: int = 0,
-                 hold: int = 0, record: bool = False):
+                 hold: int = 0, record: bool = False, impl: str = "fp32"):
         if not 1 <= len(groups) <= _lib.TRACK_MAX_GROUPS:
             raise _lib.VmbError(f"BundleAdjuster: 1 .. {_lib.TRACK_MAX_GROUPS} groups")
         self.groups = []
         for e, ids in groups:
             named = [int(i) for i in ids if i is not None and int(i) >= 0]
-            self.groups.append(_BaGroup(e, ids, cfg, n_iter, bg=getattr(objects[named[0]], "store", None) is None))
+            self.groups.append(_BaGroup(e, ids, cfg, n_iter, bg=getattr(objects[named[0]], "store", None) is None,
+                                        impl=impl))
+        self.impl = impl
         dev = self.groups[0].ens.device
         assert all(g.ens.device == dev for g in self.groups)
         self.device, self.cfg, self.n_iter, self.seed, self.hold = dev, cfg, n_iter, seed, hold
@@ -278,9 +283,7 @@ def _iterate(groups, kf_frames, n_iter, poses, window, n_win, hold, adam, scratc
         for gi, g in enumerate(groups):
             _BaGroup.bind(g, a.group[gi], it, kf_frames[gi])
         for gi, g in enumerate(groups):
-            with g.ens._on_device():
-                _lib.check(g.ens._handle, g.ens.lib.vmb_ba_step(g.ens._handle, C.byref(a), gi, _stream()),
-                           "vmb_ba_step")
+            _step(g, a, gi, ba=True)
         with e0._on_device():
             _lib.check(e0._handle, e0.lib.vmb_ba_update(e0._handle, C.byref(a), _stream()), "vmb_ba_update")
     return a
@@ -289,11 +292,12 @@ def _iterate(groups, kf_frames, n_iter, poses, window, n_win, hold, adam, scratc
 class BaSampleGroup:
     """A group fed with given samples instead of the sampler (tests, timing): ``batch`` holds [B, n_iter * R] rays of
     camera-frame points (``pcs`` [B,N,S,3]) and targets for the rows ``rows`` of ``ens``; ``kf_draw`` [B, N / n_pix_draw]
-    the keyframe index of each draw and ``kf_frame`` [B, KF] the frame id of each keyframe index (-1: none)."""
+    the keyframe index of each draw and ``kf_frame`` [B, KF] the frame id of each keyframe index (-1: none); ``impl``
+    as ``BundleAdjuster``'s."""
 
     def __init__(self, ens: VmapEnsemble, rows: Sequence[int], batch: Dict[str, torch.Tensor], n_iter: int,
-                 n_pix_draw: int, kf_draw, kf_frame):
-        self.ens, self.rows = ens, list(rows)
+                 n_pix_draw: int, kf_draw, kf_frame, impl: str = "fp32"):
+        self.ens, self.rows, self.lw = ens, list(rows), _use_lw(ens, impl)
         B, N, S = batch["pcs"].shape[:3]
         assert B == len(self.rows) and N % n_iter == 0 and (N // n_iter) % n_pix_draw == 0
         self.R, self.S, self.n_pix_draw = N // n_iter, S, n_pix_draw

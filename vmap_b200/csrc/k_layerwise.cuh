@@ -126,16 +126,8 @@ __device__ __forceinline__ void sincos_ladder6(float proj, float (&s)[6], float 
 // ---------------------------------------------------------------------------------------------
 // positional embedding: 128 points per block, rows assembled in shared memory, written coalesced
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_lw_pe(const float* __restrict__ pcs, const float* __restrict__ dirs,
-                                               const float* __restrict__ scale_ptr, long long P, __half* __restrict__ E) {
-  ptx::pdl_wait();
-  ptx::pdl_launch_dependents();
-  const float scale = *scale_ptr;
-  __shared__ __align__(16) __half row[128 * EW];
-  const long long p0 = (long long)blockIdx.x * 128, p = p0 + threadIdx.x;
-  __half* r = row + threadIdx.x * EW;
-  float t0 = 0.f, t1 = 0.f, t2 = 0.f;
-  if (p < P) { t0 = pcs[p * 3] / scale; t1 = pcs[p * 3 + 1] / scale; t2 = pcs[p * 3 + 2] / scale; }
+// one E row (EW halves) of the point t = p / scale: xyz, the sin bands, the constant-1 and zero columns
+__device__ __forceinline__ void pe_row(__half* r, float t0, float t1, float t2, const float* __restrict__ dirs) {
   r[0] = __float2half_rn(t0); r[1] = __float2half_rn(t1); r[2] = __float2half_rn(t2);
   for (int d = 0; d < VMB_NDIRS; ++d) {
     float s[6], c[6];
@@ -149,6 +141,19 @@ __global__ void __launch_bounds__(128) k_lw_pe(const float* __restrict__ pcs, co
   for (int j = ONES1 + 1; j < E1W; ++j) r[j] = __float2half_rn(0.f);
   r[E1W + ONES2] = __float2half_rn(1.0f);
   for (int j = E1W + ONES2 + 1; j < EW; ++j) r[j] = __float2half_rn(0.f);
+}
+
+__global__ void __launch_bounds__(128) k_lw_pe(const float* __restrict__ pcs, const float* __restrict__ dirs,
+                                               const float* __restrict__ scale_ptr, long long P, __half* __restrict__ E) {
+  ptx::pdl_wait();
+  ptx::pdl_launch_dependents();
+  const float scale = *scale_ptr;
+  __shared__ __align__(16) __half row[128 * EW];
+  const long long p0 = (long long)blockIdx.x * 128, p = p0 + threadIdx.x;
+  __half* r = row + threadIdx.x * EW;
+  float t0 = 0.f, t1 = 0.f, t2 = 0.f;
+  if (p < P) { t0 = pcs[p * 3] / scale; t1 = pcs[p * 3 + 1] / scale; t2 = pcs[p * 3 + 2] / scale; }
+  pe_row(r, t0, t1, t2, dirs);
   __syncthreads();
   // 128 rows x 288 B are contiguous in E
   const uint4* src = reinterpret_cast<const uint4*>(row);
@@ -408,8 +413,42 @@ __global__ void __launch_bounds__(256) k_lw_colsum(const __half* __restrict__ dY
 // ---------------------------------------------------------------------------------------------
 // PE backward: d/d(proj_d) = pi sum_k 2^k g[k,d] cos(pi 2^k proj_d);  dB[d][i] += dproj_d * t_i
 // ---------------------------------------------------------------------------------------------
+// d(loss)/d(proj_d) x 2^8 / pi from a dE row g: sum_k 2^k g[k,d] cos(pi 2^k proj_d), the cosines of sincos_ladder6
+__device__ __forceinline__ float pe_dproj(const float* g, int d, const float (&c)[6]) {
+  float dp = g[3 + d] * c[0];
+  dp = fmaf(2.f * g[3 + VMB_NDIRS + d], c[1], dp);
+  dp = fmaf(4.f * g[3 + 2 * VMB_NDIRS + d], c[2], dp);
+  dp = fmaf(8.f * g[3 + 3 * VMB_NDIRS + d], c[3], dp);
+  dp = fmaf(16.f * g[E1W + d], c[4], dp);
+  return fmaf(32.f * g[E1W + VMB_NDIRS + d], c[5], dp);
+}
 constexpr int PEB_LD = 145;      // odd row stride (floats): per-thread row reads are bank-conflict free
 constexpr int PEB_SMEM = 128 * PEB_LD * 4;
+// the dE rows of points [p0, p0 + 128) into shared memory [128][PEB_LD]: they are one contiguous 128 x 576 B span,
+// read as flat float4 loads, 12 in flight per thread
+__device__ __forceinline__ void stage_de_rows(float* sg, const float* __restrict__ dE, long long p0, long long P) {
+  const long long rows = min(128LL, P - p0);
+  const int n4 = (int)rows * (EW / 4);
+  const float4* src = reinterpret_cast<const float4*>(dE + p0 * EW);
+#pragma unroll 1
+  for (int base = 0; base < n4; base += 12 * 128) {
+    float4 q[12];
+#pragma unroll
+    for (int u = 0; u < 12; ++u) {
+      const int i = base + u * 128 + threadIdx.x;
+      q[u] = i < n4 ? src[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+#pragma unroll
+    for (int u = 0; u < 12; ++u) {
+      const int i = base + u * 128 + threadIdx.x;
+      if (i < n4) {
+        const int r = i / (EW / 4), c = (i - r * (EW / 4)) * 4;
+        float* d = sg + r * PEB_LD + c;
+        d[0] = q[u].x; d[1] = q[u].y; d[2] = q[u].z; d[3] = q[u].w;
+      }
+    }
+  }
+}
 __global__ void __launch_bounds__(128) k_lw_pe_bwd(const float* __restrict__ pcs, const float* __restrict__ dirs,
                                                    const float* __restrict__ scale_ptr, long long P,
                                                    const float* __restrict__ dE, float* __restrict__ gB) {
@@ -420,30 +459,7 @@ __global__ void __launch_bounds__(128) k_lw_pe_bwd(const float* __restrict__ pcs
   __shared__ float st[3][129];
   const long long p0 = (long long)blockIdx.x * 128;
   const long long p = p0 + threadIdx.x;
-  {
-    // the block's 128 dE rows are one contiguous 128 x 576 B span: flat float4 loads, 12 in flight per thread
-    const long long rows = min(128LL, P - p0);
-    const int n4 = (int)rows * (EW / 4);
-    const float4* src = reinterpret_cast<const float4*>(dE + p0 * EW);
-#pragma unroll 1
-    for (int base = 0; base < n4; base += 12 * 128) {
-      float4 q[12];
-#pragma unroll
-      for (int u = 0; u < 12; ++u) {
-        const int i = base + u * 128 + threadIdx.x;
-        q[u] = i < n4 ? src[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-#pragma unroll
-      for (int u = 0; u < 12; ++u) {
-        const int i = base + u * 128 + threadIdx.x;
-        if (i < n4) {
-          const int r = i / (EW / 4), c = (i - r * (EW / 4)) * 4;
-          float* d = sg + r * PEB_LD + c;
-          d[0] = q[u].x; d[1] = q[u].y; d[2] = q[u].z; d[3] = q[u].w;
-        }
-      }
-    }
-  }
+  stage_de_rows(sg, dE, p0, P);
   float t0 = 0.f, t1 = 0.f, t2 = 0.f;
   const bool ok = p < P;
   if (ok) { t0 = pcs[p * 3] / scale; t1 = pcs[p * 3 + 1] / scale; t2 = pcs[p * 3 + 2] / scale; }
@@ -457,13 +473,7 @@ __global__ void __launch_bounds__(128) k_lw_pe_bwd(const float* __restrict__ pcs
     if (ok) {
       float s[6], c[6];
       sincos_ladder6(fmaf(__ldg(dirs + d * 3 + 2), t2, fmaf(__ldg(dirs + d * 3 + 1), t1, __ldg(dirs + d * 3) * t0)), s, c);
-      dp = g[3 + d] * c[0];
-      dp = fmaf(2.f * g[3 + VMB_NDIRS + d], c[1], dp);
-      dp = fmaf(4.f * g[3 + 2 * VMB_NDIRS + d], c[2], dp);
-      dp = fmaf(8.f * g[3 + 3 * VMB_NDIRS + d], c[3], dp);
-      dp = fmaf(16.f * g[E1W + d], c[4], dp);
-      dp = fmaf(32.f * g[E1W + VMB_NDIRS + d], c[5], dp);
-      dp *= VMB_PI_F * INV_LS;
+      dp = pe_dproj(g, d, c) * (VMB_PI_F * INV_LS);
     }
     dpv[d] = dp;
   }
@@ -482,6 +492,71 @@ __global__ void __launch_bounds__(128) k_lw_pe_bwd(const float* __restrict__ pcs
 // ---------------------------------------------------------------------------------------------
 // host orchestration: one object at a time (wide ensembles have one or very few objects)
 // ---------------------------------------------------------------------------------------------
+// ---------------------------------------------------------------------------------------------
+// GEMM launches of one object, shared by the training step (step_object) and the tracking path (k_track_lw.cuh)
+// ---------------------------------------------------------------------------------------------
+// forward: the five layers E -> X1 -> X2 -> X3 -> X4 -> XC (model.py:54-85); Pb = the object's fp32 param row (biases),
+// Wi = its fp16 image.  Each launch follows its predecessor directly on `st` (k_lw_pe first): armed when pdl_ok.
+template <int H>
+static cudaError_t forward_gemms(Workspace& ws, const VmbLayout& L, const float* Pb, const __half* Wi, long long np, bool pdl_ok,
+                                 cudaStream_t st) {
+  const int mt = (int)((np + BM - 1) / BM);
+  const Operand none{nullptr, 0, 0, 0};
+  auto opX = [&](const __half* x) { return Operand{x, np, H, H}; };
+  const Operand opE1{ws.E, np, E1W, EW}, opE2{ws.E + E1W, np, E2W, EW};
+  auto fwd = [&](const Operand& a1, const Operand& a2, int K1, int K2, long long woff, int ldw, int boff, __half* out) {
+    GemmArgs g; memset(&g, 0, sizeof(g));
+    g.M = (int)np; g.N = H; g.K1 = K1; g.K2 = K2; g.bias = Pb + boff; g.out16 = out; g.ldo = H; g.scale = 1.0f;
+    if (pdl_ok) pdl_arm();                          // follows k_lw_pe / the previous layer directly on `st`
+    return launch_gemm_auto<0, EPI_RELU_F16>(a1, a2, Operand{Wi + woff, H, ldw, ldw}, g, mt, (H + BN - 1) / BN, st);
+  };
+  cudaError_t e = fwd(opE1, none, E1W, 0, 0, 96, L.o_bin, ws.X1);
+  if (e == cudaSuccess) e = fwd(opX(ws.X1), none, H, 0, off_m1(H), H, L.o_bm1, ws.X2);
+  if (e == cudaSuccess) e = fwd(opX(ws.X2), opE1, H, E1W, off_cat(H), H + 96, L.o_bcat, ws.X3);
+  if (e == cudaSuccess) e = fwd(opX(ws.X3), none, H, 0, off_m2(H), H, L.o_bm2, ws.X4);
+  if (e == cudaSuccess) e = fwd(opX(ws.X4), opE2, H, E2W, off_cl(H), H + 48, L.o_bcl, ws.XC);
+  return e;
+}
+
+// input gradient through a weight block: out = gate(x_prev) * (dY @ W[:, c0:c0+N] (+ rank-1 r1row x r1col))
+template <int H>
+static cudaError_t dgrad_gate_gemm(const __half* dY, const __half* Wi, long long woff, int ldw, long long np, const __half* xprev,
+                                   __half* out, const float* r1row, const float* r1col, cudaStream_t st) {
+  GemmArgs g; memset(&g, 0, sizeof(g));
+  g.M = (int)np; g.N = H; g.K1 = H; g.out16 = out; g.ldo = H; g.gate = xprev; g.ldg = H; g.r1_row = r1row; g.r1_col = r1col;
+  g.r1_stride = 1; g.scale = 1.0f;
+  const Operand none{nullptr, 0, 0, 0};
+  return launch_gemm_auto<1, EPI_GATE_F16>(Operand{dY, np, H, H}, none, Operand{Wi + woff, H, H, ldw}, g,
+                                           (int)((np + BM - 1) / BM), (H + BN - 1) / BN, st);
+}
+
+// input gradient into the fp32 embedding gradient: dE[:, ecol:ecol+N] (=|+=) dY @ W[:, c0:c0+N]
+template <int H>
+static cudaError_t dgrad_emb_gemm(Workspace& ws, const __half* dY, const __half* Wi, long long woff, int ldw, int N, int ecol,
+                                  int accumulate, long long np, cudaStream_t st) {
+  GemmArgs g; memset(&g, 0, sizeof(g));
+  g.M = (int)np; g.N = N; g.K1 = H; g.out32 = ws.dE + ecol; g.ld32 = EW; g.accumulate = accumulate; g.scale = 1.0f;
+  const Operand none{nullptr, 0, 0, 0};
+  return launch_gemm_auto<1, EPI_F32>(Operand{dY, np, H, H}, none, Operand{Wi + woff, H, N, ldw}, g, (int)((np + BM - 1) / BM), 1, st);
+}
+
+// d emb1 = dY3 @ W_cat[:, H:] + dY1 @ W_in in ONE launch: A = [dY3 | dY1] along K, B = the two weight blocks
+// (two launches, the second accumulating, where the weight-stationary kernel does not fit)
+template <int H>
+static cudaError_t demb1_gemm(Workspace& ws, const __half* dY3, const __half* dY1, const __half* Wi, long long np, cudaStream_t st) {
+  GemmArgs g; memset(&g, 0, sizeof(g));
+  g.M = (int)np; g.N = E1W; g.K1 = H; g.K2 = H; g.out32 = ws.dE; g.ld32 = EW; g.accumulate = 0; g.scale = 1.0f;
+  const Operand bcat{Wi + off_cat(H) + H, H, E1W, H + 96}, bin{Wi, H, E1W, 96};
+  cudaError_t e = launch_gemm_ws<1, EPI_F32>(Operand{dY3, np, H, H}, Operand{dY1, np, H, H}, bcat, g, (int)((np + BM - 1) / BM),
+                                              st, &bin);
+  if (e == cudaErrorNotSupported) {
+    (void)cudaGetLastError();
+    e = dgrad_emb_gemm<H>(ws, dY3, Wi, off_cat(H) + H, H + 96, E1W, 0, 0, np, st);
+    if (e == cudaSuccess) e = dgrad_emb_gemm<H>(ws, dY1, Wi, 0, 96, E1W, 0, 1, np, st);
+  }
+  return e;
+}
+
 #define LW_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return -2; } } while (0)
 
 template <int H>
@@ -489,7 +564,6 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
                        std::string& err, long long fwd_p0 = 0, long long fwd_np = 0) {
   // fwd_only (vmb_forward): points [fwd_p0, fwd_p0 + fwd_np) of object b, raw head outputs, no render
   const long long np = sp.fwd_only ? fwd_np : (long long)sp.R * sp.S;
-  const int mt = (int)((np + BM - 1) / BM);
   const float* Pb = sp.params + (size_t)b * L.stride;
   float* G = sp.grads ? sp.grads + (size_t)b * L.stride : nullptr;
   const __half* Wi = image + (size_t)b * img_halves(H);
@@ -508,17 +582,7 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
 
   // ---- forward ----
   LW_TRY(launch_k(k_lw_pe, dim3(nblk), dim3(128), 0, st, pcs, dirs, scale_p, np, ws.E));
-  auto fwd = [&](const Operand& a1, const Operand& a2, int K1, int K2, long long woff, int ldw, int boff, __half* out) {
-    GemmArgs g; memset(&g, 0, sizeof(g));
-    g.M = (int)np; g.N = H; g.K1 = K1; g.K2 = K2; g.bias = Pb + boff; g.out16 = out; g.ldo = H; g.scale = 1.0f;
-    arm();                                          // follows k_lw_pe / the previous layer directly on `st`
-    return launch_gemm_auto<0, EPI_RELU_F16>(a1, a2, Operand{Wi + woff, H, ldw, ldw}, g, mt, (H + BN - 1) / BN, st);
-  };
-  LW_TRY(fwd(opE1, none, E1W, 0, 0, 96, L.o_bin, ws.X1));
-  LW_TRY(fwd(opX(ws.X1), none, H, 0, off_m1(H), H, L.o_bm1, ws.X2));
-  LW_TRY(fwd(opX(ws.X2), opE1, H, E1W, off_cat(H), H + 96, L.o_bcat, ws.X3));
-  LW_TRY(fwd(opX(ws.X3), none, H, 0, off_m2(H), H, L.o_bm2, ws.X4));
-  LW_TRY(fwd(opX(ws.X4), opE2, H, E2W, off_cl(H), H + 48, L.o_bcl, ws.XC));
+  LW_TRY(forward_gemms<H>(ws, L, Pb, Wi, np, pdl_ok, st));
   if (sp.fwd_only) {
     arm();
     LW_TRY(launch_k(k_lw_heads<H>, dim3(nblk), dim3(128), 0, st, (const __half*)ws.X4, (const __half*)ws.XC, Pb, L, np,
@@ -562,17 +626,8 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
     g.n_valid = n_valid; g.ones_col = ones_col; g.gbias = boff >= 0 ? G + boff : nullptr; g.scale = INV_LS;
     return launch_gemm<1, 1, EPI_ATOMIC>(Operand{dY, np, H, H}, none, xb, g, (H + BM - 1) / BM, (N + BN - 1) / BN, zs, sd);
   };
-  // input gradient through a weight block: out = gate(x_prev) * (dY @ W[:, c0:c0+N] (+ rank-1))   or fp32 into dE
   auto dgrad_gate = [&](const __half* dY, long long woff, int ldw, const __half* xprev, __half* out, const float* r1row, const float* r1col) {
-    GemmArgs g; memset(&g, 0, sizeof(g));
-    g.M = (int)np; g.N = H; g.K1 = H; g.out16 = out; g.ldo = H; g.gate = xprev; g.ldg = H; g.r1_row = r1row; g.r1_col = r1col;
-    g.r1_stride = 1; g.scale = 1.0f;
-    return launch_gemm_auto<1, EPI_GATE_F16>(Operand{dY, np, H, H}, none, Operand{Wi + woff, H, H, ldw}, g, mt, (H + BN - 1) / BN, st);
-  };
-  auto dgrad_emb = [&](const __half* dY, long long woff, int ldw, int N, int ecol, int accumulate) {
-    GemmArgs g; memset(&g, 0, sizeof(g));
-    g.M = (int)np; g.N = N; g.K1 = H; g.out32 = ws.dE + ecol; g.ld32 = EW; g.accumulate = accumulate; g.scale = 1.0f;
-    return launch_gemm_auto<1, EPI_F32>(Operand{dY, np, H, H}, none, Operand{Wi + woff, H, N, ldw}, g, mt, 1, st);
+    return dgrad_gate_gemm<H>(dY, Wi, woff, ldw, np, xprev, out, r1row, r1col, st);
   };
   // heads: dW_a[o] = sum_p d_a fc4[p][o]; dW_oc[c][o] = sum_p d_rc[c] hc[p][o]   (B = dh16 [P][8], columns 0 / 1..3)
   {
@@ -590,7 +645,7 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
   LW_TRY(wgrad(ws.dYc, opX(ws.X4), H, L.o_Wcl, H + L.e2, H, -1, -1));
   arm();
   LW_TRY(wgrad(ws.dYc, opE2, E2W, L.o_Wcl + H, H + L.e2, L.e2, ONES2, L.o_bcl));
-  LW_TRY(dgrad_emb(ws.dYc, off_cl(H) + H, H + 48, E2W, E1W, 0));                // first kernel on `st` after the fork: not armed
+  LW_TRY(dgrad_emb_gemm<H>(ws, ws.dYc, Wi, off_cl(H) + H, H + 48, E2W, E1W, 0, np, st));          // first kernel on `st` after the fork: not armed
   arm();
   LW_TRY(dgrad_gate(ws.dYc, off_cl(H), H + 48, ws.X4, ws.dYa, ws.dalpha_s, Pb + L.o_Wa));          // dY4 -> dYa
   // mid2
@@ -617,18 +672,7 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
   LW_TRY(fork(4));
   LW_TRY(wgrad(ws.dYc, opE1, E1W, L.o_Win, VMB_E1, VMB_E1, ONES1, L.o_bin));
   LW_TRY(cudaEventRecord(ws.ev_side[1], sd));
-  // d emb1 = dY3 @ W_cat[:, H:] + dY1 @ W_in in ONE launch: A = [dY3 | dY1] along K, B = the two weight blocks
-  {
-    GemmArgs g; memset(&g, 0, sizeof(g));
-    g.M = (int)np; g.N = E1W; g.K1 = H; g.K2 = H; g.out32 = ws.dE; g.ld32 = EW; g.accumulate = 0; g.scale = 1.0f;
-    const Operand bcat{Wi + off_cat(H) + H, H, E1W, H + 96}, bin{Wi, H, E1W, 96};
-    cudaError_t e = launch_gemm_ws<1, EPI_F32>(Operand{ws.dYb, np, H, H}, Operand{ws.dYc, np, H, H}, bcat, g, mt, st, &bin);
-    if (e == cudaErrorNotSupported) {
-      (void)cudaGetLastError();
-      LW_TRY(dgrad_emb(ws.dYb, off_cat(H) + H, H + 96, E1W, 0, 0));
-      LW_TRY(dgrad_emb(ws.dYc, 0, 96, E1W, 0, 1));
-    } else LW_TRY(e);
-  }
+  LW_TRY(demb1_gemm<H>(ws, ws.dYb, ws.dYc, Wi, np, st));                                        // d emb1 (dY3, dY1)
   {
     static bool attr_set[64] = {};
     int dev = 0; cudaGetDevice(&dev);

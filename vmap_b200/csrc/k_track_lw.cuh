@@ -1,0 +1,504 @@
+// K10 / K11 on the layer-wise tensor-core path: the pose gradient of a wide model (hidden 64 / 128 / 256: the iMAP
+// whole-scene model, the vMAP background) through the wgmma GEMMs of k_layerwise.cuh instead of K10's fp32 CUDA cores.
+//
+// The rule is K10's (k_track.cuh) and, for the BA flavour, K11's (k_ba.cuh): same samples, same points, same loss with
+// the per-object, per-term empty-mask rule, same left-perturbation gradient, same output rows, so vmb_track_update and
+// vmb_ba_update run unchanged on what this path writes.  What differs is where the network runs and its precision:
+//   Weights  object b reads params row rows[b] and the fp16 image row rows[b] (as the AdamW launch writes it).  Both
+//            are copied on the device into this path's workspace first, so rows[] stays a device array (capturable);
+//            a row outside [0, n_rows) contributes nothing and sets VMB_TRACK_ST_BAD_ROW, as K10.
+//   Points   p = R q + t from an fp32 copy of the fp64 pose, K10's operation order, then p / scale; the embedding row
+//            is k_lw_pe's (fp16, sin by sincos_ladder6, constant-1 columns).  K11: the ray's pose is its draw's frame
+//            (ba_draw_frame); a ray whose frame is outside the table contributes nothing and sets VMB_BA_ST_BAD_FRAME.
+//   Network  the five forward GEMMs of step_object (fp16 operands, fp32 accumulation, fp16 activations).
+//   Render   one warp per ray, lane = sample (S <= 32): the heads in fp32 from the fp16 activations; the composite,
+//            render and loss in fp64 in sample order exactly as K10 (1 - occ as sigmoid(-alpha)); mask counts of this
+//            slice per object (integers); the backward to (raw alpha, raw colour) in fp32 as K10.  Each ray's three
+//            loss terms go to an fp64 per-ray buffer.  d(raw alpha) and dYc are loss-scaled by LS = 2^8 and clamped to
+//            the fp16 range +-60000 as in the training kernel.  status[1] gets a LOWER BOUND on the clamped values
+//            (and VMB_TRACK_ST_CLAMP is set when it is not 0): every clamped dYc element, plus every element where the
+//            rank-1 term LS d(raw alpha) W_a of dY4 passes 60000 on its own; the saturating packs of the dY4..dY1
+//            GEMM epilogues are not counted.  No head weight gradients.
+//   Backward the input-gradient GEMM chain of step_object only (colour-block dE, dY4 with the rank-1 d_alpha term, dY3,
+//            dY2, dY1, the fused dE GEMM): no weight-gradient GEMMs, no column sums, no side stream.
+//   Pose     per point dL/dt = INV_LS (dE_xyz + sum_{k,d} dE_{k,d} pi 2^k cos(pi 2^k proj_d) B_d) in fp32 (the cosines
+//            of sincos_ladder6, as k_lw_pe_bwd), g = dL/dt / scale, and the point's terms ((R q) x g, g) in fp64 from
+//            the fp64 pose.  Track flavour: the terms are summed in point order over the rays of each of K10's tiles
+//            (nr = TP / S rays, TP = vmb_track_tiles' tile), plus the per-ray loss terms in ray order: exactly K10's
+//            partial rows.  BA flavour: one row per ray (its samples in order), as K11.
+// No floating-point atomics anywhere on this path (the GEMM epilogues used here store): bitwise reproducible.
+// Registers (ptxas -v, sm_90a; track / BA flavour), no spills in any of them:
+//   k_tlw_gather 32; k_tlw_pe 74 / 74; k_tlw_render H 64: 71 / 68, H 128: 71 / 68, H 256: 68 / 68;
+//   k_tlw_pose 62 / 62; k_tlw_reduce 40 / 40.
+#pragma once
+#include "k_layerwise.cuh"
+#include "k_track.cuh"
+
+namespace lw {
+
+// the path's own buffers next to the training step's: grow-only, never moved once a captured graph holds them
+struct TrackWorkspace {
+  Workspace w;                 // E, X1..X4, XC, dYa..dYc, dalpha_s, dE (dh16 unused)
+  float* prow = nullptr;       // [stride] the object's fp32 param row
+  __half* wimg = nullptr;      // [img_halves] its fp16 image row
+  int* ctl = nullptr;          // [8]: mask counts nd, no, ns; row ok; scale (float bits)
+  double* lossr = nullptr;     // [R][3] per-ray loss terms
+  double* gpt = nullptr;       // [P][6] per-point pose terms
+  long long cap_rays = 0, cap_points = 0; int H = 0;
+  bool in_graph = false;
+  void release() {
+    void* ptrs[] = {prow, wimg, ctl, lossr, gpt};
+    for (void* q : ptrs) if (q) cudaFree(q);
+    prow = nullptr; wimg = nullptr; ctl = nullptr; lossr = nullptr; gpt = nullptr;
+    cap_rays = cap_points = 0; H = 0; in_graph = false;
+    w.release();
+    w.destroy_streams();
+  }
+  cudaError_t ensure(long long R, long long P, int H_, int stride, cudaStream_t st) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    cudaStreamIsCapturing(st, &cs);
+    const bool capturing = cs != cudaStreamCaptureStatusNone;
+    cudaError_t e = w.ensure(P, H_, st);
+    if (e != cudaSuccess) return e;
+    if (R <= cap_rays && P <= cap_points && H_ == H) { in_graph |= capturing; return cudaSuccess; }
+    if (capturing || in_graph) return cudaErrorStreamCaptureUnsupported;
+    void* ptrs[] = {prow, wimg, ctl, lossr, gpt};
+    for (void* q : ptrs) if (q) cudaFree(q);
+    prow = nullptr; wimg = nullptr; ctl = nullptr; lossr = nullptr; gpt = nullptr; cap_rays = cap_points = 0;
+    const long long Pp = (P + 127) / 128 * 128;
+    auto al = [&](void** q, size_t bytes) { if (e == cudaSuccess) e = cudaMalloc(q, bytes); };
+    al((void**)&prow, (size_t)stride * 4);
+    al((void**)&wimg, (size_t)img_halves(H_) * 2);
+    al((void**)&ctl, 8 * sizeof(int));
+    al((void**)&lossr, (size_t)R * 3 * sizeof(double));
+    al((void**)&gpt, (size_t)Pp * 6 * sizeof(double));
+    if (e != cudaSuccess) return e;
+    cap_rays = R; cap_points = Pp; H = H_;
+    return cudaSuccess;
+  }
+};
+
+// What the path reads for one object b of the group (TrackParams / BaRays of k_track.cuh carry the rest)
+struct TlwObj {
+  int b, R, S, n_rows, n_pix_draw, n_poses, kf_stride;
+  const int* rows;
+  const float* pcs;                  // object b's slice [R][S][3]
+  const double* pose;                // track: [16]; BA: the table [n_poses][16]
+  const int* kf_draw; const int* kf_frame;   // BA: object b's rows
+  int* status;
+};
+
+// frame id of ray r (BA) or 0 (track); -1 = outside the pose table
+template <bool BA>
+__device__ __forceinline__ int tlw_frame(const TlwObj& o, int r) {
+  if constexpr (BA) {
+    const int kf = o.kf_draw[r / o.n_pix_draw];
+    if (kf < 0 || kf >= o.kf_stride) return -1;
+    const int f = o.kf_frame[kf];
+    return (f >= 0 && f < o.n_poses) ? f : -1;
+  } else {
+    return 0;
+  }
+}
+
+// ---- 1: the object's weights into the workspace; block 0 also counts the slice's masks (loss.py:16-18,38) ----------
+__global__ void __launch_bounds__(256) k_tlw_gather(TlwObj o, const float* __restrict__ params, const float* __restrict__ scale,
+                                                    const __half* __restrict__ image, const unsigned char* __restrict__ sem,
+                                                    const unsigned char* __restrict__ mask, int stride, long long halves,
+                                                    float* __restrict__ prow, __half* __restrict__ wimg, int* __restrict__ ctl) {
+  ptx::pdl_wait();
+  ptx::pdl_launch_dependents();
+  const int row = o.rows[o.b];
+  const bool ok = row >= 0 && row < o.n_rows;
+  const long long n4 = halves / 8;                    // image rows are whole multiples of 16 B
+  const uint4* src = reinterpret_cast<const uint4*>(image + (size_t)(ok ? row : 0) * halves);
+  uint4* dst = reinterpret_cast<uint4*>(wimg);
+  const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
+  for (long long i = t0; i < n4; i += nt) dst[i] = ok ? src[i] : make_uint4(0u, 0u, 0u, 0u);
+  const float* P = params + (size_t)(ok ? row : 0) * stride;
+  for (long long i = t0; i < stride; i += nt) prow[i] = ok ? P[i] : 0.f;
+  if (blockIdx.x != 0) return;
+  __shared__ int s_cnt[3];
+  if (threadIdx.x < 3) s_cnt[threadIdx.x] = 0;
+  __syncthreads();
+  int nd = 0, no = 0, ns = 0;
+  for (int r = threadIdx.x; r < o.R; r += blockDim.x) {
+    const int s = sem[r];
+    const int mo = s != 0;
+    nd += (mask[r] != 0) & mo; no += mo; ns += s != 2;
+  }
+  atomicAdd(&s_cnt[0], nd); atomicAdd(&s_cnt[1], no); atomicAdd(&s_cnt[2], ns);
+  __syncthreads();
+  if (threadIdx.x < 3) ctl[threadIdx.x] = s_cnt[threadIdx.x];
+  if (threadIdx.x == 3) ctl[3] = ok ? 1 : 0;
+  if (threadIdx.x == 4) ctl[4] = __float_as_int(ok ? scale[row] : 1.0f);
+  if (threadIdx.x == 5 && !ok && o.status) atomicOr(o.status, VMB_TRACK_ST_BAD_ROW);
+}
+
+// p / scale of point p = ray r, sample s (K10's operation order); false where the ray has no pose
+template <bool BA>
+__device__ __forceinline__ bool tlw_point(const TlwObj& o, long long p, float sc, float& q0, float& q1, float& q2, float& t0,
+                                          float& t1, float& t2, const double*& T) {
+  const int f = tlw_frame<BA>(o, (int)(p / o.S));
+  q0 = q1 = q2 = t0 = t1 = t2 = 0.f;
+  T = o.pose + (size_t)(f > 0 ? f : 0) * 16;
+  if (f < 0) return false;
+  q0 = o.pcs[p * 3]; q1 = o.pcs[p * 3 + 1]; q2 = o.pcs[p * 3 + 2];
+  const float x = fmaf((float)T[2], q2, fmaf((float)T[1], q1, (float)T[0] * q0)) + (float)T[3];
+  const float y = fmaf((float)T[6], q2, fmaf((float)T[5], q1, (float)T[4] * q0)) + (float)T[7];
+  const float w = fmaf((float)T[10], q2, fmaf((float)T[9], q1, (float)T[8] * q0)) + (float)T[11];
+  t0 = x / sc; t1 = y / sc; t2 = w / sc;
+  return true;
+}
+
+// ---- 2: positional embedding at the pose, k_lw_pe's row layout ------------------------------------------------------
+template <bool BA>
+__global__ void __launch_bounds__(128) k_tlw_pe(TlwObj o, const float* __restrict__ prow, const int* __restrict__ ctl, int o_B,
+                                                __half* __restrict__ E) {
+  ptx::pdl_wait();
+  ptx::pdl_launch_dependents();
+  const long long P = (long long)o.R * o.S;
+  const float sc = __int_as_float(ctl[4]);
+  const float* dirs = prow + o_B;
+  __shared__ __align__(16) __half row[128 * EW];
+  const long long p0 = (long long)blockIdx.x * 128, p = p0 + threadIdx.x;
+  __half* r = row + threadIdx.x * EW;
+  float q0, q1, q2, t0 = 0.f, t1 = 0.f, t2 = 0.f;
+  const double* T;
+  if (p < P) tlw_point<BA>(o, p, sc, q0, q1, q2, t0, t1, t2, T);
+  pe_row(r, t0, t1, t2, dirs);                       // k_lw_pe's row
+  __syncthreads();
+  const uint4* src = reinterpret_cast<const uint4*>(row);
+  uint4* dst = reinterpret_cast<uint4*>(E + p0 * EW);
+  const long long n16 = min(128LL, P - p0) * (EW * 2 / 16);
+  for (long long i = threadIdx.x; i < n16; i += 128) dst[i] = src[i];
+}
+
+// ---- 3: heads + fp64 render + loss + d(raw alpha, raw colour) -> dalpha_s, dYc; one warp per ray, lane = sample ------
+struct TlwRender {
+  const float* z; const float* gt_depth; const float* gt_colour; const unsigned char* sem; const unsigned char* mask;
+  float cs, os;
+};
+template <int H, bool BA>
+__global__ void __launch_bounds__(128) k_tlw_render(TlwObj o, TlwRender a, const __half* __restrict__ X4, const __half* __restrict__ XC,
+                                                    const float* __restrict__ P, VmbLayout L, const int* __restrict__ ctl,
+                                                    __half* __restrict__ dYc, float* __restrict__ dalpha_s, double* __restrict__ lossr) {
+  ptx::pdl_wait();
+  ptx::pdl_launch_dependents();
+  extern __shared__ __align__(16) unsigned char hr_rows[];
+  __shared__ float w[4 * H];                          // [0,H) out_alpha row, [H,4H) out_color rows
+  constexpr int PITCH = hr_pitch<H>(), LPR = H / 8, RPP = 32 / LPR;
+  for (int i = threadIdx.x; i < H; i += 128) w[i] = P[L.o_Wa + i];
+  for (int i = threadIdx.x; i < 3 * H; i += 128) w[H + i] = P[L.o_Woc + i];
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, S = o.S;
+  const unsigned FULL = 0xffffffffu;
+  const float b_a = P[L.o_ba], b_c0 = P[L.o_boc], b_c1 = P[L.o_boc + 1], b_c2 = P[L.o_boc + 2];
+  const int cnt0 = ctl[0], cnt1 = ctl[1], cnt2 = ctl[2];
+  const double inv_nd = cnt0 ? 1.0 / ((double)cnt0 + 1e-10) : 0.0;
+  const double inv_no = cnt1 ? 1.0 / ((double)cnt1 + 1e-10) : 0.0;
+  const double inv_ns = cnt2 ? 1.0 / ((double)cnt2 + 1e-10) : 0.0;
+  const bool in = lane < S;
+  unsigned char* srow = hr_rows + warp * (32 * PITCH);
+  int n_clamp = 0;
+  auto stage_rows = [&](const __half* X, long long pb) {
+#pragma unroll 4
+    for (int r0 = 0; r0 < S; r0 += RPP) {
+      const int r = r0 + lane / LPR, cq = lane % LPR;
+      if (r < S) cp_async16(srow + r * PITCH + cq * 16, X + (pb + r) * H + cq * 8);
+    }
+    asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
+    __syncwarp();
+  };
+  const uint4* xrow = reinterpret_cast<const uint4*>(srow + lane * PITCH);
+  for (int ray = blockIdx.x * 4 + warp; ray < o.R; ray += gridDim.x * 4) {
+    const long long pb = (long long)ray * S, pi = pb + lane;
+    __syncwarp();
+    stage_rows(X4, pb);
+    float ha = 0.f, h0 = 0.f, h1 = 0.f, h2 = 0.f;
+    if (in) {
+      float hb = 0.f;
+#pragma unroll 4
+      for (int q = 0; q < H / 8; ++q) {
+        const uint4 u = xrow[q];
+        const __half* hu = reinterpret_cast<const __half*>(&u);
+#pragma unroll
+        for (int j = 0; j < 8; j += 2) {
+          ha = fmaf(__half2float(hu[j]), w[q * 8 + j], ha);
+          hb = fmaf(__half2float(hu[j + 1]), w[q * 8 + j + 1], hb);
+        }
+      }
+      ha += hb;
+    }
+    __syncwarp();
+    stage_rows(XC, pb);
+    float al = 0.f, oc = 0.f, zz = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f;
+    if (in) {
+#pragma unroll 4
+      for (int q = 0; q < H / 8; ++q) {
+        const uint4 v = xrow[q];
+        const __half* hv = reinterpret_cast<const __half*>(&v);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float fc = __half2float(hv[j]);
+          const int oo = q * 8 + j;
+          h0 = fmaf(fc, w[H + oo], h0); h1 = fmaf(fc, w[2 * H + oo], h1); h2 = fmaf(fc, w[3 * H + oo], h2);
+        }
+      }
+      al = (ha + b_a) * 10.0f;                        // model.py:77
+      oc = vmb_sigmoid(al);                           // render_rays.py:6
+      c0 = vmb_sigmoid(h0 + b_c0); c1 = vmb_sigmoid(h1 + b_c1); c2 = vmb_sigmoid(h2 + b_c2);
+      zz = a.z[pi];
+    }
+    // K10's per-ray render in fp64, samples in order (every lane runs the same sums)
+    double Tr = 1.0, D = 0.0, O = 0.0, C0 = 0.0, C1 = 0.0, C2 = 0.0;
+    float Ts = 0.f, wf = 0.f;
+    for (int s = 0; s < S; ++s) {
+      const float al_s = __shfl_sync(FULL, al, s), oc_s = __shfl_sync(FULL, oc, s), z_s = __shfl_sync(FULL, zz, s);
+      const float c0_s = __shfl_sync(FULL, c0, s), c1_s = __shfl_sync(FULL, c1, s), c2_s = __shfl_sync(FULL, c2, s);
+      const double wd = (double)oc_s * Tr;
+      if (lane == s) { Ts = (float)Tr; wf = (float)wd; }
+      D += wd * (double)z_s; O += wd;
+      C0 += wd * (double)c0_s; C1 += wd * (double)c1_s; C2 += wd * (double)c2_s;
+      Tr *= ((double)vmb_sigmoid(-al_s) + 1e-10);
+    }
+    double V = 0.0;
+    for (int s = 0; s < S; ++s) {
+      const double dz = (double)__shfl_sync(FULL, zz, s) - D;
+      V += (double)__shfl_sync(FULL, wf, s) * dz * dz;  // loss.py:28-29 (detached)
+    }
+    const int sv = a.sem[ray];
+    const bool rok = tlw_frame<BA>(o, ray) >= 0;
+    if (BA && !rok && lane == 0 && o.status) atomicOr(o.status, VMB_BA_ST_BAD_FRAME);
+    const double m_o = (sv != 0 && rok) ? 1.0 : 0.0;
+    const double m_s = (sv != 2 && rok) ? 1.0 : 0.0;
+    const double m_d = (a.mask[ray] != 0) ? m_o : 0.0;
+    const double gd = a.gt_depth[ray];
+    const float* gc = a.gt_colour + (size_t)ray * 3;
+    const double info = 1.0 / (sqrt(V) + 1e-4);      // render_rays.py:74-79
+    const double e_d = D - gd, e_o = O - m_o;
+    const double e_c0 = C0 - (double)gc[0], e_c1 = C1 - (double)gc[1], e_c2 = C2 - (double)gc[2];
+    if (lane == 0) {
+      lossr[(size_t)ray * 3 + 0] = cnt0 ? fabs(e_d) * m_d * info * inv_nd : 0.0;
+      lossr[(size_t)ray * 3 + 1] = cnt1 ? (fabs(e_c0) + fabs(e_c1) + fabs(e_c2)) * m_o * inv_no : 0.0;
+      lossr[(size_t)ray * 3 + 2] = cnt2 ? fabs(e_o) * m_s * inv_ns : 0.0;
+    }
+    const float gD = (float)(m_d * info * inv_nd) * vmb_sign((float)e_d);
+    const float kc = (float)((double)a.cs * m_o * inv_no);
+    const float gC0 = kc * vmb_sign((float)e_c0), gC1 = kc * vmb_sign((float)e_c1), gC2 = kc * vmb_sign((float)e_c2);
+    const float gO = (float)((double)a.os * m_s * inv_ns) * vmb_sign((float)e_o);
+    const float Gs = fmaf(gD, zz, fmaf(gC0, c0, fmaf(gC1, c1, fmaf(gC2, c2, gO))));
+    const float fr = vmb_sigmoid(-al);               // 1 - occ
+    float suffix = 0.f, docc = 0.f;                   // K10's suffix sum, samples from the last
+    for (int s = S - 1; s >= 0; --s) {
+      if (lane == s) docc = Gs * Ts - suffix / (fr + 1e-10f);
+      suffix = fmaf(__shfl_sync(FULL, Gs, s), __shfl_sync(FULL, wf, s), suffix);
+    }
+    if (in) {
+      const float dx = 10.0f * docc * oc * fr;
+      const float dy0 = gC0 * wf * c0 * (1.f - c0), dy1 = gC1 * wf * c1 * (1.f - c1), dy2 = gC2 * wf * c2 * (1.f - c2);
+      const float da = LS * dx;
+      dalpha_s[pi] = da;
+      uint4* xc = const_cast<uint4*>(xrow);           // the staged hc row, gated in place
+      const float d0 = LS * dy0, d1 = LS * dy1, d2 = LS * dy2;
+#pragma unroll 4
+      for (int q = 0; q < H / 8; ++q) {
+        const uint4 v = xc[q];
+        const __half* hv = reinterpret_cast<const __half*>(&v);
+        uint32_t r[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int oo = q * 8 + 2 * j;
+          float x0 = fmaf(d2, w[3 * H + oo], fmaf(d1, w[2 * H + oo], d0 * w[H + oo]));
+          float x1 = fmaf(d2, w[3 * H + oo + 1], fmaf(d1, w[2 * H + oo + 1], d0 * w[H + oo + 1]));
+          const bool g0 = __half2float(hv[2 * j]) > 0.f, g1 = __half2float(hv[2 * j + 1]) > 0.f;
+          n_clamp += (g0 && fabsf(x0) > 60000.f) + (g1 && fabsf(x1) > 60000.f);
+          n_clamp += (fabsf(da * w[oo]) > 60000.f) + (fabsf(da * w[oo + 1]) > 60000.f);
+          x0 = g0 ? fminf(fmaxf(x0, -60000.f), 60000.f) : 0.f;
+          x1 = g1 ? fminf(fmaxf(x1, -60000.f), 60000.f) : 0.f;
+          __half2 hh = __floats2half2_rn(x0, x1);
+          r[j] = *reinterpret_cast<uint32_t*>(&hh);
+        }
+        xc[q] = make_uint4(r[0], r[1], r[2], r[3]);
+      }
+    }
+    __syncwarp();
+#pragma unroll 4
+    for (int r0 = 0; r0 < S; r0 += RPP) {
+      const int r = r0 + lane / LPR, cq = lane % LPR;
+      if (r < S) *reinterpret_cast<uint4*>(dYc + (pb + r) * H + cq * 8) = *reinterpret_cast<const uint4*>(srow + r * PITCH + cq * 16);
+    }
+  }
+  for (int d = 16; d > 0; d >>= 1) n_clamp += __shfl_xor_sync(FULL, n_clamp, d);
+  if (lane == 0 && n_clamp && o.status) { atomicOr(o.status, VMB_TRACK_ST_CLAMP); atomicAdd(o.status + 1, n_clamp); }
+}
+
+// ---- 4: per-point pose terms ((R q) x g, g) in fp64 ------------------------------------------------------------------
+template <bool BA>
+__global__ void __launch_bounds__(128) k_tlw_pose(TlwObj o, const float* __restrict__ prow, const int* __restrict__ ctl, int o_B,
+                                                  const float* __restrict__ dE, double* __restrict__ gpt) {
+  ptx::pdl_wait();
+  ptx::pdl_launch_dependents();
+  extern __shared__ float sg[];                       // [128 points][PEB_LD]
+  const long long P = (long long)o.R * o.S;
+  const long long p0 = (long long)blockIdx.x * 128, p = p0 + threadIdx.x;
+  stage_de_rows(sg, dE, p0, P);
+  __syncthreads();
+  if (p >= P) return;
+  const float sc = __int_as_float(ctl[4]);
+  const float* dirs = prow + o_B;
+  float q0, q1, q2, t0, t1, t2;
+  const double* T;
+  const bool pok = tlw_point<BA>(o, p, sc, q0, q1, q2, t0, t1, t2, T);
+  const float* g = sg + threadIdx.x * PEB_LD;
+  float dt0 = g[0] * INV_LS, dt1 = g[1] * INV_LS, dt2 = g[2] * INV_LS;
+#pragma unroll 1
+  for (int d = 0; d < VMB_NDIRS; ++d) {
+    const float b0 = dirs[d * 3], b1 = dirs[d * 3 + 1], b2 = dirs[d * 3 + 2];
+    float s[6], c[6];
+    sincos_ladder6(fmaf(b2, t2, fmaf(b1, t1, b0 * t0)), s, c);
+    const float dp = pe_dproj(g, d, c) * (VMB_PI_F * INV_LS);       // as k_lw_pe_bwd
+    dt0 = fmaf(dp, b0, dt0); dt1 = fmaf(dp, b1, dt1); dt2 = fmaf(dp, b2, dt2);
+  }
+  double c6[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  if (pok && ctl[3]) {
+    const double g0 = (double)(dt0 / sc), g1 = (double)(dt1 / sc), g2 = (double)(dt2 / sc);
+    const double x0 = T[0] * q0 + T[1] * q1 + T[2] * q2;   // R q in fp64
+    const double x1 = T[4] * q0 + T[5] * q1 + T[6] * q2;
+    const double x2 = T[8] * q0 + T[9] * q1 + T[10] * q2;
+    c6[0] = x1 * g2 - x2 * g1; c6[1] = x2 * g0 - x0 * g2; c6[2] = x0 * g1 - x1 * g0;
+    c6[3] = g0; c6[4] = g1; c6[5] = g2;
+  }
+#pragma unroll
+  for (int i = 0; i < 6; ++i) gpt[p * 6 + i] = c6[i];
+}
+
+// ---- 5: fixed-order fp64 sums into K10's partial rows (track) or K11's per-ray rows (BA) -----------------------------
+template <bool BA>
+__global__ void __launch_bounds__(128) k_tlw_reduce(TlwObj o, int nr, int n_out, const int* __restrict__ ctl,
+                                                    const double* __restrict__ gpt, const double* __restrict__ lossr,
+                                                    double* __restrict__ out) {
+  ptx::pdl_wait();
+  ptx::pdl_launch_dependents();
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n_out) return;
+  double* dst = out + (size_t)j * VMB_TRACK_PART;
+  const int per = BA ? 1 : nr;                        // rays per output row
+  const int r0 = j * per, r1 = min(o.R, r0 + per);
+  double s[9] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  if (ctl[3]) {
+    const long long pe = (long long)r1 * o.S;
+    for (long long p = (long long)r0 * o.S; p < pe; ++p)
+#pragma unroll
+      for (int c = 0; c < 6; ++c) s[c] += gpt[p * 6 + c];
+    for (int r = r0; r < r1; ++r)
+#pragma unroll
+      for (int c = 0; c < 3; ++c) s[6 + c] += lossr[(size_t)r * 3 + c];
+  }
+#pragma unroll
+  for (int c = 0; c < 9; ++c) dst[c] = s[c];
+  dst[9] = 0.0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// host: one object at a time on `st`
+// ---------------------------------------------------------------------------------------------------------------------
+struct TlwGroup {
+  TrackParams tp;                // K10's group arguments (partials: track flavour output)
+  BaRays x;                      // K11's (BA flavour: rows = output, kf_* the draw tables)
+  const __half* image;           // [n_rows][img_halves(H)]
+  int nr;                        // track flavour: rays per K10 tile
+};
+
+#define TLW_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return -2; } } while (0)
+
+template <int H, bool BA>
+static int track_object_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGroup& G, int b, cudaStream_t st, std::string& err) {
+  const TrackParams& a = G.tp;
+  Workspace& ws = tw.w;
+  const long long np = (long long)a.R * a.S;
+  const int nblk = (int)((np + 127) / 128);
+  const bool pdl_ok = np <= 65536;                   // step_object's rule
+  auto arm = [&]() { if (pdl_ok) pdl_arm(); };
+  TlwObj o;
+  o.b = b; o.R = a.R; o.S = a.S; o.n_rows = a.n_rows; o.rows = a.rows;
+  o.pcs = a.pcs + (size_t)b * a.pcs_stride; o.pose = a.pose; o.status = a.status;
+  o.n_pix_draw = BA ? G.x.n_pix_draw : 1; o.n_poses = BA ? G.x.n_poses : 1; o.kf_stride = BA ? G.x.kf_stride : 0;
+  o.kf_draw = BA ? G.x.kf_draw + (size_t)b * G.x.kf_draw_stride : nullptr;
+  o.kf_frame = BA ? G.x.kf_frame + (size_t)b * G.x.kf_stride : nullptr;
+  const unsigned char* sem = a.sem + (size_t)b * a.sem_stride;
+  const unsigned char* mask = a.mask + (size_t)b * a.mask_stride;
+  const long long halves = img_halves(H);
+  TLW_TRY(launch_k(k_tlw_gather, dim3((unsigned)std::min<long long>(2 * sm_count(), (halves / 8 + 255) / 256)), dim3(256), 0, st, o,
+                   a.params, a.scale, G.image, sem, mask, L.stride, halves, tw.prow, tw.wimg, tw.ctl));
+  arm();
+  TLW_TRY(launch_k(k_tlw_pe<BA>, dim3(nblk), dim3(128), 0, st, o, (const float*)tw.prow, (const int*)tw.ctl, L.o_B, ws.E));
+  TLW_TRY(forward_gemms<H>(ws, L, tw.prow, tw.wimg, np, pdl_ok, st));
+  {
+    static bool attr_set[64] = {};
+    int dev = 0; cudaGetDevice(&dev);
+    if (!attr_set[dev & 63]) {
+      TLW_TRY(cudaFuncSetAttribute(k_tlw_render<H, BA>, cudaFuncAttributeMaxDynamicSharedMemorySize, hr_smem<H>()));
+      attr_set[dev & 63] = true;
+    }
+  }
+  TlwRender ra;
+  ra.z = a.z + (size_t)b * a.z_stride; ra.gt_depth = a.gt_depth + (size_t)b * a.gt_depth_stride;
+  ra.gt_colour = a.gt_colour + (size_t)b * a.gt_colour_stride; ra.sem = sem; ra.mask = mask; ra.cs = a.cs; ra.os = a.os;
+  const int hr_per_sm = std::max(1, std::min(8, (int)(227 * 1024 / (hr_smem<H>() + 6 * 1024))));
+  arm();
+  TLW_TRY(launch_k(k_tlw_render<H, BA>, dim3(std::min((a.R + 3) / 4, sm_count() * hr_per_sm)), dim3(128), (size_t)hr_smem<H>(), st,
+                   o, ra, (const __half*)ws.X4, (const __half*)ws.XC, (const float*)tw.prow, L, (const int*)tw.ctl, ws.dYc,
+                   ws.dalpha_s, tw.lossr));
+  // backward to the embedding only, the input-gradient chain of step_object
+  arm();
+  TLW_TRY(dgrad_emb_gemm<H>(ws, ws.dYc, tw.wimg, off_cl(H) + H, H + 48, E2W, E1W, 0, np, st));        // colour block of dE
+  arm();
+  TLW_TRY(dgrad_gate_gemm<H>(ws.dYc, tw.wimg, off_cl(H), H + 48, np, ws.X4, ws.dYa, ws.dalpha_s, tw.prow + L.o_Wa, st));  // dY4
+  arm();
+  TLW_TRY(dgrad_gate_gemm<H>(ws.dYa, tw.wimg, off_m2(H), H, np, ws.X3, ws.dYb, nullptr, nullptr, st));    // dY3 -> dYb
+  arm();
+  TLW_TRY(dgrad_gate_gemm<H>(ws.dYb, tw.wimg, off_cat(H), H + 96, np, ws.X2, ws.dYa, nullptr, nullptr, st));  // dY2 -> dYa
+  arm();
+  TLW_TRY(dgrad_gate_gemm<H>(ws.dYa, tw.wimg, off_m1(H), H, np, ws.X1, ws.dYc, nullptr, nullptr, st));    // dY1 -> dYc
+  arm();
+  TLW_TRY(demb1_gemm<H>(ws, ws.dYb, ws.dYc, tw.wimg, np, st));                                           // d emb1
+  {
+    static bool attr_set[64] = {};
+    int dev = 0; cudaGetDevice(&dev);
+    if (!attr_set[dev & 63]) {
+      TLW_TRY(cudaFuncSetAttribute(k_tlw_pose<BA>, cudaFuncAttributeMaxDynamicSharedMemorySize, PEB_SMEM));
+      attr_set[dev & 63] = true;
+    }
+  }
+  arm();
+  TLW_TRY(launch_k(k_tlw_pose<BA>, dim3(nblk), dim3(128), (size_t)PEB_SMEM, st, o, (const float*)tw.prow, (const int*)tw.ctl, L.o_B,
+                   (const float*)ws.dE, tw.gpt));
+  const int n_out = BA ? a.R : (a.R + G.nr - 1) / G.nr;
+  double* out = BA ? G.x.rows + (size_t)b * a.R * VMB_TRACK_PART : a.partials + (size_t)b * n_out * VMB_TRACK_PART;
+  arm();
+  TLW_TRY(launch_k(k_tlw_reduce<BA>, dim3((n_out + 127) / 128), dim3(128), 0, st, o, G.nr, n_out, (const int*)tw.ctl,
+                   (const double*)tw.gpt, (const double*)tw.lossr, out));
+  TLW_TRY(cudaGetLastError());
+  return 0;
+}
+
+template <bool BA>
+static int launch_track_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGroup& G, cudaStream_t st, std::string& err) {
+  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return -2; }
+  TLW_TRY(tw.ensure(G.tp.R, (long long)G.tp.R * G.tp.S, L.H, L.stride, st));
+  for (int b = 0; b < G.tp.B; ++b) {
+    int rc;
+    switch (L.H) {
+      case 64:  rc = track_object_lw<64, BA>(tw, L, G, b, st, err); break;
+      case 128: rc = track_object_lw<128, BA>(tw, L, G, b, st, err); break;
+      case 256: rc = track_object_lw<256, BA>(tw, L, G, b, st, err); break;
+      default: err = "layer-wise tracking: hidden must be 64, 128 or 256"; return -4;
+    }
+    if (rc) return rc;
+  }
+  return 0;
+}
+#undef TLW_TRY
+
+}  // namespace lw

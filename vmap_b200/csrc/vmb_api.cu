@@ -23,6 +23,7 @@
 #include "k_render.cuh"
 #include "k_track.cuh"
 #include "k_ba.cuh"
+#include "k_track_lw.cuh"
 
 struct vmb_handle {
   int device, max_obj, H, nfreq;
@@ -46,6 +47,8 @@ struct vmb_handle {
   assoc::Workspace ws_assoc;// ScanNet association scratch (grow-only)
   hull::Workspace ws_hull;  // convex hull / minimum-volume box scratch (grow-only)
   render::Workspace ws_render;// view rendering: source table, entry sort / scan scratch (grow-only)
+  lw::TrackWorkspace ws_track;// layer-wise tracking step: its own, so a tracking capture never pins the mapping step's
+  lw::TrackWorkspace ws_ba;   // layer-wise bundle-adjustment step: likewise (and tracking never moves a BA capture's)
   std::string err;
 };
 
@@ -178,6 +181,8 @@ void vmb_destroy(vmb_handle* h) {
   h->ws_assoc.release();
   h->ws_hull.release();
   h->ws_render.release();
+  h->ws_track.release();
+  h->ws_ba.release();
   delete h;
 }
 
@@ -1384,6 +1389,84 @@ int vmb_ba_update(vmb_handle* h, const vmb_ba_args* a, void* stream) {
   u.loss = a->loss; u.pose_hist = a->pose_hist; u.grad_hist = a->grad_hist; u.status = a->status;
   k_ba_update<<<1, 256, 0, (cudaStream_t)stream>>>(u);
   CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
+}  // extern "C"
+
+// ---- K10 / K11 on the layer-wise tensor-core path ---------------------------------------------------------------------
+extern "C" {
+
+int vmb_track_step_lw(vmb_handle* h, const vmb_track_args* a, int group, const void* image, void* stream) {
+  if (!h) return fail(h, VMB_E_ARG, "vmb_track_step_lw: null handle");
+  const int rc0 = track_common(h, a, "vmb_track_step_lw");
+  if (rc0 != VMB_OK) return rc0;
+  if (group < 0 || group >= a->n_groups) return fail(h, VMB_E_ARG, "vmb_track_step_lw: group index outside [0, n_groups)");
+  const vmb_track_group& g = a->group[group];
+  if (g.hidden != h->H) return fail(h, VMB_E_ARG, "vmb_track_step_lw: group hidden size differs from the handle's");
+  if (!h->lw_ok) return fail(h, VMB_E_UNSUPPORTED, "vmb_track_step_lw: the layer-wise path needs hidden 64/128/256 and n_freq 6");
+  if (g.n_obj < 1 || g.n_obj > 65535 || g.n_rows < 1 || g.n_rays < 1 || g.n_samples < 1)
+    return fail(h, VMB_E_ARG, "vmb_track_step_lw: bad n_obj / n_rows / n_rays / n_samples");
+  if (!g.rows || !g.pcs || !g.z_vals || !g.gt_depth || !g.gt_colour || !g.sem || !g.mask_depth || !g.params ||
+      !g.scale || !g.partials || !image)
+    return fail(h, VMB_E_ARG, "vmb_track_step_lw: missing tensor pointer");
+  const int tiles = vmb_track_tiles(g.hidden, g.n_rays, g.n_samples);
+  if (tiles == VMB_E_UNSUPPORTED || g.n_samples > 32)
+    return fail(h, VMB_E_UNSUPPORTED, "vmb_track_step_lw: n_samples above 32");
+  if (tiles < 1) return fail(h, VMB_E_ARG, "vmb_track_step_lw: bad shape");
+  if ((long long)tiles * g.n_obj > g.max_partials) return fail(h, VMB_E_ARG, "vmb_track_step_lw: partials buffer too small");
+  lw::TlwGroup G;
+  memset(&G, 0, sizeof(G));
+  TrackParams& tp = G.tp;
+  tp.B = g.n_obj; tp.R = g.n_rays; tp.S = g.n_samples; tp.n_rows = g.n_rows; tp.rows = g.rows;
+  tp.pcs = g.pcs; tp.pcs_stride = g.pcs_stride; tp.z = g.z_vals; tp.z_stride = g.z_stride;
+  tp.gt_depth = g.gt_depth; tp.gt_depth_stride = g.gt_depth_stride;
+  tp.gt_colour = g.gt_colour; tp.gt_colour_stride = g.gt_colour_stride;
+  tp.sem = g.sem; tp.sem_stride = g.sem_stride; tp.mask = g.mask_depth; tp.mask_stride = g.mask_stride;
+  tp.params = g.params; tp.scale = g.scale; tp.pose = a->pose; tp.partials = g.partials;
+  tp.cs = a->colour_scaling; tp.os = a->opacity_scaling; tp.status = a->status;
+  G.image = (const __half*)image;
+  G.nr = track_tile(g.hidden) / g.n_samples;
+  std::string err;
+  const int rc = lw::launch_track_lw<false>(h->ws_track, h->L, G, (cudaStream_t)stream, err);
+  if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, "vmb_track_step_lw: " + err);
+  return VMB_OK;
+}
+
+int vmb_ba_step_lw(vmb_handle* h, const vmb_ba_args* a, int group, const void* image, void* stream) {
+  if (!h) return fail(h, VMB_E_ARG, "vmb_ba_step_lw: null handle");
+  const int rc0 = ba_common(h, a, "vmb_ba_step_lw");
+  if (rc0 != VMB_OK) return rc0;
+  if (group < 0 || group >= a->n_groups) return fail(h, VMB_E_ARG, "vmb_ba_step_lw: group index outside [0, n_groups)");
+  const vmb_ba_group& g = a->group[group];
+  if (g.hidden != h->H) return fail(h, VMB_E_ARG, "vmb_ba_step_lw: group hidden size differs from the handle's");
+  if (!h->lw_ok) return fail(h, VMB_E_UNSUPPORTED, "vmb_ba_step_lw: the layer-wise path needs hidden 64/128/256 and n_freq 6");
+  if (ba_group_ok(g) != VMB_OK)
+    return fail(h, VMB_E_ARG, "vmb_ba_step_lw: bad counts, draw layout, keyframe tables or ray rows");
+  if (!g.rows || !g.pcs || !g.z_vals || !g.gt_depth || !g.gt_colour || !g.sem || !g.mask_depth || !g.params || !g.scale ||
+      !image)
+    return fail(h, VMB_E_ARG, "vmb_ba_step_lw: missing tensor pointer");
+  const int tiles = vmb_track_tiles(g.hidden, g.n_rays, g.n_samples);
+  if (tiles == VMB_E_UNSUPPORTED || g.n_samples > 32) return fail(h, VMB_E_UNSUPPORTED, "vmb_ba_step_lw: n_samples above 32");
+  if (tiles < 1) return fail(h, VMB_E_ARG, "vmb_ba_step_lw: bad shape");
+  lw::TlwGroup G;
+  memset(&G, 0, sizeof(G));
+  TrackParams& tp = G.tp;
+  tp.B = g.n_obj; tp.R = g.n_rays; tp.S = g.n_samples; tp.n_rows = g.n_rows; tp.rows = g.rows;
+  tp.pcs = g.pcs; tp.pcs_stride = g.pcs_stride; tp.z = g.z_vals; tp.z_stride = g.z_stride;
+  tp.gt_depth = g.gt_depth; tp.gt_depth_stride = g.gt_depth_stride;
+  tp.gt_colour = g.gt_colour; tp.gt_colour_stride = g.gt_colour_stride;
+  tp.sem = g.sem; tp.sem_stride = g.sem_stride; tp.mask = g.mask_depth; tp.mask_stride = g.mask_stride;
+  tp.params = g.params; tp.scale = g.scale; tp.pose = a->poses;
+  tp.cs = a->colour_scaling; tp.os = a->opacity_scaling; tp.status = a->status;
+  BaRays& x = G.x;
+  x.kf_draw = g.kf_draw; x.kf_draw_stride = g.kf_draw_stride; x.kf_frame = g.kf_frame; x.kf_stride = g.kf_stride;
+  x.n_pix_draw = g.n_pix_draw; x.n_poses = a->n_poses; x.rows = g.ray_rows;
+  G.image = (const __half*)image;
+  G.nr = 1;
+  std::string err;
+  const int rc = lw::launch_track_lw<true>(h->ws_ba, h->L, G, (cudaStream_t)stream, err);
+  if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, "vmb_ba_step_lw: " + err);
   return VMB_OK;
 }
 

@@ -31,6 +31,13 @@ mapping frame: ``n_ba_iter`` pose-only iterations against the frozen map move ev
 tables hold (never frame 0, the anchor), and the refined poses go to ``poses``, the store and the background's
 copies, where the next mapping frames, the motion model, ``get_bound`` and meshing read them.  Its graph follows the
 same eager / capture / replay pattern (``ba_modes``).
+
+In iMAP mode (``cfg.imap_mode``) every pixel of a frame is instance 0 (dataset.py:95-96) and id 0 is the one
+whole-scene network, an object of the stack as mapping builds it (``hidden_feature_size``, ``obj_scale``,
+``n_bins_cam2surface``, ``n_per_optim``); it is tracked like any other object from the frame after its insertion, with
+its box from the ingest.  ``track_impl`` / ``ba_impl`` choose the step of the tracker and the bundle adjuster:
+``"layerwise"`` (the tensor-core path for hidden 64/128/256, the default in iMAP mode) or ``"fp32"`` (K10 / K11, the
+default otherwise).
 """
 from __future__ import annotations
 
@@ -61,11 +68,11 @@ def _inv_se3(T: torch.Tensor) -> torch.Tensor:
     return out
 
 
-def tracker_groups(groups, do_bg: bool):
+def tracker_groups(groups, do_bg: bool, imap: bool = False):
     """``groups`` (``[(VmapEnsemble, obj_ids)]``) as the Tracker takes them.  The background (id 0) is tracked only as
     the separate background model of a ``do_bg`` map; with ``do_bg`` off it is an ordinary object network and its row
-    is left out."""
-    return [(e, [None if i is None or int(i) < 0 or (int(i) == 0 and not do_bg) else int(i) for i in ids])
+    is left out.  In iMAP mode (``imap``) id 0 is the whole-scene model, the only object, and it is kept."""
+    return [(e, [None if i is None or int(i) < 0 or (int(i) == 0 and not do_bg and not imap) else int(i) for i in ids])
             for e, ids in groups]
 
 
@@ -79,13 +86,16 @@ class Slam:
     iterations and rates (default ``cfg.pose_lr``).  ``store_capacity``: the frame store's initial number of slots (it
     grows on demand).  ``timing``: record CUDA events at the phase boundaries of every frame (``phase_times``).
     ``ba_every``: run a bundle-adjustment pass after the mapping frame of every ``ba_every``-th frame (0: never);
-    ``n_ba_iter`` / ``ba_lr_rot`` / ``ba_lr_trans``: its iterations and rates (default ``cfg.pose_lr``)."""
+    ``n_ba_iter`` / ``ba_lr_rot`` / ``ba_lr_trans``: its iterations and rates (default ``cfg.pose_lr``).
+    ``track_impl`` / ``ba_impl``: ``"fp32"`` or ``"layerwise"`` (see the module docstring; None: ``"layerwise"`` in iMAP
+    mode, ``"fp32"`` otherwise)."""
 
     def __init__(self, cfg, T_init=None, track: bool = True, map: bool = True, groups=None, graph: bool = True,
                  n_track_iter: int = 20, lr_rot: Optional[float] = None, lr_trans: Optional[float] = None,
                  seed: int = 0, max_frames: int = 100000, background_cls: Sequence[int] = (), bbox_scale: float = 0.2,
                  store_capacity: Optional[int] = None, max_id: int = 4096, timing: bool = False, ba_every: int = 0,
-                 n_ba_iter: int = 20, ba_lr_rot: Optional[float] = None, ba_lr_trans: Optional[float] = None):
+                 n_ba_iter: int = 20, ba_lr_rot: Optional[float] = None, ba_lr_trans: Optional[float] = None,
+                 track_impl: Optional[str] = None, ba_impl: Optional[str] = None):
         if not track and not map:
             raise ValueError("Slam: nothing to do with track=False and map=False")
         if ba_every < 0 or n_ba_iter < 1:
@@ -98,7 +108,10 @@ class Slam:
         self.device = torch.device(cfg.data_device)
         dev = self.device
         self.seed, self.n_track_iter = seed, n_track_iter
-        self.track_kw = dict(n_iter=n_track_iter, lr_rot=lr_rot, lr_trans=lr_trans, seed=seed + _TRACK_SEED)
+        self.imap = bool(cfg.imap_mode)
+        default_impl = "layerwise" if self.imap else "fp32"
+        self.track_kw = dict(n_iter=n_track_iter, lr_rot=lr_rot, lr_trans=lr_trans, seed=seed + _TRACK_SEED,
+                             impl=track_impl or default_impl)
         self.background_cls, self.bbox_scale = list(background_cls), bbox_scale
         # localisation holds only the live frame; mapping holds each object's keyframes (see the module docstring)
         self.max_slots = cfg.max_n_models * cfg.keyframe_buffer_size + 1 if map else 1
@@ -119,7 +132,8 @@ class Slam:
         self.timing, self.events = timing, []
         # bundle adjustment (off: nothing is allocated or launched)
         self.ba_every = ba_every
-        self.ba_kw = dict(n_iter=n_ba_iter, lr_rot=ba_lr_rot, lr_trans=ba_lr_trans, seed=seed + _BA_SEED)
+        self.ba_kw = dict(n_iter=n_ba_iter, lr_rot=ba_lr_rot, lr_trans=ba_lr_trans, seed=seed + _BA_SEED,
+                          impl=ba_impl or default_impl)
         self.ba: Optional[BundleAdjuster] = None
         self.ba_loss = torch.full((max_frames,), float("nan"), **f64) if ba_every else None
         self.ba_frames: List[List[int]] = []
@@ -134,7 +148,7 @@ class Slam:
         self.tracker: Optional[Tracker] = None
         self._tracked_set = None
         if not map:
-            groups = tracker_groups(groups, cfg.do_bg)
+            groups = tracker_groups(groups, cfg.do_bg, self.imap)
             self.tracker = Tracker(groups, cfg, **self.track_kw)
             self.mapped = {int(i) for _, ids in groups for i in ids if i is not None and int(i) >= 0}
         else:
@@ -158,8 +172,11 @@ class Slam:
 
     def step(self, rgb, depth, inst, cls=None, T_wc=None) -> int:
         """Process the next frame (images [W, H]: rgb uint8 [.., 3], depth metres, instance and class ids).  ``T_wc``:
-        the frame's pose when ``track=False`` (ignored otherwise).  Returns the frame index."""
+        the frame's pose when ``track=False`` (ignored otherwise).  In iMAP mode every pixel is instance 0 whatever
+        ``inst`` holds (it may be None).  Returns the frame index."""
         k, cfg, dev = self.k, self.cfg, self.device
+        if self.imap:
+            inst, cls = torch.zeros((cfg.W, cfg.H), dtype=torch.int32, device=dev), None
         if k >= self.poses.shape[0]:
             raise _lib.VmbError(f"Slam: more than max_frames={self.poses.shape[0]} frames")
         if not self.do_track:
@@ -339,7 +356,7 @@ class Slam:
 
     def _rebuild_tracker(self) -> None:
         objs = list(self.objects.values()) + ([self.scene_bg] if self.scene_bg is not None else [])
-        groups = tracker_groups(groups_from_objects(objs), self.cfg.do_bg)
+        groups = tracker_groups(groups_from_objects(objs), self.cfg.do_bg, self.imap)
         old = self.tracker
         self.tracker = Tracker(groups, self.cfg, **self.track_kw)
         if old is not None:

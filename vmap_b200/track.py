@@ -10,6 +10,10 @@ live mode.  ``Tracker`` closes that loop with the networks the map already has. 
 all on the device, so the loop can be captured as one CUDA graph (``capture`` / ``run``) as ``FrameLoop`` does for a
 mapping frame.  The rule (points, loss, per-object empty masks, gradient, update) is in ``csrc/k_track.cuh``;
 ``oracle/track_oracle.py`` restates it.
+
+``impl="layerwise"`` runs the step of every hidden-64/128/256 group on the tensor-core path instead
+(``vmb_track_step_lw``, ``csrc/k_track_lw.cuh``: the same rule, the network in fp16 on wgmma GEMMs); hidden-32 groups
+stay on K10.  In iMAP mode (``cfg.imap_mode``) id 0 is the whole-scene model and is sampled as an object.
 """
 from __future__ import annotations
 
@@ -22,6 +26,27 @@ import torch
 from . import _lib
 from .ensemble import VmapEnsemble, _ptr, _stream
 from .sampler import BatchedSampler, KeyframeTables, SamplerTables
+
+IMPLS = ("fp32", "layerwise")
+
+
+def _use_lw(ens: VmapEnsemble, impl: str) -> bool:
+    """True when ``impl`` sends this ensemble's step to the layer-wise tensor-core path (hidden 64/128/256)."""
+    if impl not in IMPLS:
+        raise ValueError(f"tracking impl must be one of {IMPLS}, not {impl!r}")
+    return impl == "layerwise" and ens.hidden != 32 and ens.image is not None
+
+
+def _step(g, a, gi: int, ba: bool) -> None:
+    """The step of group ``gi`` on K10 / K11 or, for a layer-wise group, on the tensor-core path."""
+    e = g.ens
+    with e._on_device():
+        if g.lw:
+            fn = e.lib.vmb_ba_step_lw if ba else e.lib.vmb_track_step_lw
+            _lib.check(e._handle, fn(e._handle, C.byref(a), gi, _ptr(e.image), _stream()), fn.__name__)
+        else:
+            fn = e.lib.vmb_ba_step if ba else e.lib.vmb_track_step
+            _lib.check(e._handle, fn(e._handle, C.byref(a), gi, _stream()), fn.__name__)
 
 
 def _rays_dir(cfg, device) -> torch.Tensor:
@@ -38,11 +63,11 @@ class _Group:
     """One ensemble's share of the tracking problem: its sampler, the rows tracked this frame and their buffers."""
 
     def __init__(self, ens: VmapEnsemble, obj_ids: Sequence[Optional[int]], cfg, n_pix: int, n_pix_bg: int,
-                 n_iter: int):
+                 n_iter: int, impl: str = "fp32"):
         ids = [None if i is None or int(i) < 0 else int(i) for i in obj_ids]
         assert len(ids) == ens.n_obj, "obj_ids must name every row of the ensemble (None / -1 = not an object)"
-        self.ens, self.ids = ens, ids
-        self.bg = 0 in ids
+        self.ens, self.ids, self.lw = ens, ids, _use_lw(ens, impl)
+        self.bg = 0 in ids and not getattr(cfg, "imap_mode", 0)     # iMAP: id 0 is the scene model, an object
         assert not self.bg or [i for i in ids if i is not None] == [0], "the background (id 0) is a group of its own"
         n1 = cfg.n_bins_cam2surface_bg if self.bg else cfg.n_bins_cam2surface
         self.smp = BatchedSampler(ens.device, n1, cfg.n_bins, cfg.surface_eps, cfg.stop_eps, cfg.min_depth)
@@ -115,16 +140,18 @@ class Tracker:
 
     ``groups``: ``[(VmapEnsemble, obj_ids), ...]`` with ``obj_ids[row]`` the instance id of each row (``None`` or -1
     for rows that are not objects); the background (id 0) is a group of its own.  ``n_iter`` iterations of ``n_pix``
-    rays per object (``n_pix_bg`` for the background); rates default to ``cfg.pose_lr``."""
+    rays per object (``n_pix_bg`` for the background); rates default to ``cfg.pose_lr``.  ``impl``: ``"fp32"`` (K10
+    for every group) or ``"layerwise"`` (the tensor-core path for hidden-64/128/256 groups, K10 for hidden 32)."""
 
     def __init__(self, groups: Sequence[Tuple[VmapEnsemble, Sequence[Optional[int]]]], cfg, n_iter: int = 20,
                  n_pix: Optional[int] = None, n_pix_bg: Optional[int] = None, lr_rot: Optional[float] = None,
-                 lr_trans: Optional[float] = None, seed: int = 0, record: bool = False):
+                 lr_trans: Optional[float] = None, seed: int = 0, record: bool = False, impl: str = "fp32"):
         if not 1 <= len(groups) <= _lib.TRACK_MAX_GROUPS:
             raise _lib.VmbError(f"Tracker: 1 .. {_lib.TRACK_MAX_GROUPS} groups")
         n_pix = cfg.n_per_optim if n_pix is None else n_pix
         n_pix_bg = cfg.n_per_optim_bg if n_pix_bg is None else n_pix_bg
-        self.groups = [_Group(e, ids, cfg, n_pix, n_pix_bg, n_iter) for e, ids in groups]
+        self.groups = [_Group(e, ids, cfg, n_pix, n_pix_bg, n_iter, impl) for e, ids in groups]
+        self.impl = impl
         dev = self.groups[0].ens.device
         assert all(g.ens.device == dev for g in self.groups)
         self.device, self.cfg, self.n_iter, self.seed = dev, cfg, n_iter, seed
@@ -252,9 +279,7 @@ def _iterate(live, n_iter, pose, adam, lr_rot, lr_trans, losses, status, pose_hi
         for gi, g in enumerate(live):
             _Group.bind(g, a.group[gi], it)
         for gi, g in enumerate(live):
-            with g.ens._on_device():
-                _lib.check(g.ens._handle, g.ens.lib.vmb_track_step(g.ens._handle, C.byref(a), gi, _stream()),
-                           "vmb_track_step")
+            _step(g, a, gi, ba=False)
         e = live[0].ens
         with e._on_device():
             _lib.check(e._handle, e.lib.vmb_track_update(e._handle, C.byref(a), _stream()), "vmb_track_update")
@@ -263,10 +288,12 @@ def _iterate(live, n_iter, pose, adam, lr_rot, lr_trans, losses, status, pose_hi
 
 class SampleGroup:
     """A group fed with given samples instead of the sampler (tests, timing): ``batch`` holds [B, n_iter * n_pix]
-    rays of camera-frame points (``pcs`` [B,N,S,3]) and targets for the rows ``rows`` of ``ens``."""
+    rays of camera-frame points (``pcs`` [B,N,S,3]) and targets for the rows ``rows`` of ``ens``; ``impl`` as
+    ``Tracker``'s."""
 
-    def __init__(self, ens: VmapEnsemble, rows: Sequence[int], batch: Dict[str, torch.Tensor], n_iter: int):
-        self.ens, self.active, self.n_iter = ens, list(rows), n_iter
+    def __init__(self, ens: VmapEnsemble, rows: Sequence[int], batch: Dict[str, torch.Tensor], n_iter: int,
+                 impl: str = "fp32"):
+        self.ens, self.active, self.n_iter, self.lw = ens, list(rows), n_iter, _use_lw(ens, impl)
         B, N, S = batch["pcs"].shape[:3]
         assert B == len(self.active) and N % n_iter == 0
         self.n_pix, self.S = N // n_iter, S
