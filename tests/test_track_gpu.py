@@ -169,7 +169,6 @@ def test_tracker_reproducible_and_graph_replay():
 
 def _args(sg, n_iter=1, it=1):
     from vmap_b200 import _lib
-    from vmap_b200.track import _Group
     a = _lib.TrackArgs()
     a.n_groups, a.n_iter, a.iter = 1, n_iter, it
     pose = torch.eye(4, dtype=torch.float64, device="cuda:0")
@@ -179,7 +178,7 @@ def _args(sg, n_iter=1, it=1):
     a.lr_rot = a.lr_trans = 1e-3
     a.beta1, a.beta2, a.eps = 0.9, 0.999, 1e-8
     a.colour_scaling, a.opacity_scaling = 5.0, 10.0
-    _Group.bind(sg, a.group[0], 0)
+    sg.bind(a.group[0], 0)
     return a, (pose, adam, status)
 
 

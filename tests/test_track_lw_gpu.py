@@ -186,7 +186,7 @@ def test_ba_bad_frame_and_empty_masks():
 
 def _bind_lw(ens, rows, batch, S_override=None):
     from vmap_b200 import _lib
-    from vmap_b200.track import SampleGroup, _Group
+    from vmap_b200.track import SampleGroup
     sg = SampleGroup(ens, rows, batch, 1)
     a = _lib.TrackArgs()
     a.n_groups, a.n_iter, a.iter = 1, 1, 1
@@ -194,7 +194,7 @@ def _bind_lw(ens, rows, batch, S_override=None):
     status = torch.zeros(4, dtype=torch.int32, device=DEV)
     a.pose, a.status = C.c_void_p(pose.data_ptr()), C.c_void_p(status.data_ptr())
     a.colour_scaling, a.opacity_scaling = 5.0, 10.0
-    _Group.bind(sg, a.group[0], 0)
+    sg.bind(a.group[0], 0)
     if S_override:
         a.group[0].n_samples = S_override
     keep = (sg, pose, status)

@@ -146,14 +146,13 @@ def _update_only(tr, live):
     import ctypes as C
     from vmap_b200 import _lib
     from vmap_b200.ensemble import _ptr, _stream
-    from vmap_b200.track import _Group
     a = _lib.TrackArgs()
     a.n_groups, a.n_iter, a.iter = len(live), tr.n_iter, 1
     a.pose, a.adam = _ptr(tr.pose), _ptr(tr.adam)
     a.beta1, a.beta2, a.eps = 0.9, 0.999, 1e-8
     a.colour_scaling, a.opacity_scaling = 5.0, 10.0
     for k, gr in enumerate(live):
-        _Group.bind(gr, a.group[k], 0)
+        gr.bind(a.group[k], 0)
     e = live[0].ens
     _lib.check(e._handle, e.lib.vmb_track_update(e._handle, C.byref(a), _stream()), "vmb_track_update")
 
@@ -162,13 +161,12 @@ def _iterate_one(tr, live, gi):
     """The step of group gi alone on iteration 0's slice (the update is timed with the whole iteration)."""
     from vmap_b200 import _lib
     from vmap_b200.ensemble import _ptr
-    from vmap_b200.track import _Group
     a = _lib.TrackArgs()
     a.n_groups, a.n_iter, a.iter = len(live), tr.n_iter, 1
     a.pose, a.adam = _ptr(tr.pose), _ptr(tr.adam)
     a.colour_scaling, a.opacity_scaling = 5.0, 10.0
     for k, gr in enumerate(live):
-        _Group.bind(gr, a.group[k], 0)
+        gr.bind(a.group[k], 0)
     _step(live[gi], a, gi, ba=False)
 
 

@@ -173,18 +173,22 @@ class RenderArgs(C.Structure):
     ]
 
 
+# the leading fields vmb_track_group and vmb_ba_group share: one iteration's sample slice and the network
+_POSE_GROUP_FIELDS = [
+    ("hidden", C.c_int), ("n_obj", C.c_int), ("n_rows", C.c_int), ("rows", _vp),
+    ("n_rays", C.c_int), ("n_samples", C.c_int),
+    ("pcs", _vp), ("pcs_stride", _ll),
+    ("z_vals", _vp), ("z_stride", _ll),
+    ("gt_depth", _vp), ("gt_depth_stride", _ll),
+    ("gt_colour", _vp), ("gt_colour_stride", _ll),
+    ("sem", _vp), ("sem_stride", _ll),
+    ("mask_depth", _vp), ("mask_stride", _ll),
+    ("params", _vp), ("scale", _vp),
+]
+
+
 class TrackGroup(C.Structure):
-    _fields_ = [
-        ("hidden", C.c_int), ("n_obj", C.c_int), ("n_rows", C.c_int), ("rows", _vp),
-        ("n_rays", C.c_int), ("n_samples", C.c_int),
-        ("pcs", _vp), ("pcs_stride", _ll),
-        ("z_vals", _vp), ("z_stride", _ll),
-        ("gt_depth", _vp), ("gt_depth_stride", _ll),
-        ("gt_colour", _vp), ("gt_colour_stride", _ll),
-        ("sem", _vp), ("sem_stride", _ll),
-        ("mask_depth", _vp), ("mask_stride", _ll),
-        ("params", _vp), ("scale", _vp), ("partials", _vp), ("max_partials", _ll), ("loss_terms", _vp),
-    ]
+    _fields_ = _POSE_GROUP_FIELDS + [("partials", _vp), ("max_partials", _ll), ("loss_terms", _vp)]
 
 
 TRACK_MAX_GROUPS, TRACK_PART, TRACK_ST_BAD_ROW = 8, 10, 4     # VMB_TRACK_MAX_GROUPS, VMB_TRACK_PART, VMB_TRACK_ST_BAD_ROW
@@ -206,16 +210,7 @@ TRACK_ST_CLAMP = 16                                            # VMB_TRACK_ST_CL
 
 
 class BaGroup(C.Structure):
-    _fields_ = [
-        ("hidden", C.c_int), ("n_obj", C.c_int), ("n_rows", C.c_int), ("rows", _vp),
-        ("n_rays", C.c_int), ("n_samples", C.c_int),
-        ("pcs", _vp), ("pcs_stride", _ll),
-        ("z_vals", _vp), ("z_stride", _ll),
-        ("gt_depth", _vp), ("gt_depth_stride", _ll),
-        ("gt_colour", _vp), ("gt_colour_stride", _ll),
-        ("sem", _vp), ("sem_stride", _ll),
-        ("mask_depth", _vp), ("mask_stride", _ll),
-        ("params", _vp), ("scale", _vp),
+    _fields_ = _POSE_GROUP_FIELDS + [
         ("n_pix_draw", C.c_int), ("kf_draw", _vp), ("kf_draw_stride", _ll), ("kf_frame", _vp), ("kf_stride", C.c_int),
         ("ray_rows", _vp), ("max_ray_rows", _ll),
     ]

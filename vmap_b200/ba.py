@@ -22,12 +22,14 @@ import torch
 from . import _lib
 from .ensemble import VmapEnsemble, _ptr, _stream
 from .sampler import BatchedSampler, SamplerTables
-from .track import _rays_dir, _step, _use_lw
+from .track import _rays_dir, _Slices, _step, _use_lw
+from .utils import capture_graph
 
 
-class _BaGroup:
+class _BaGroup(_Slices):
     """One ensemble's share of a pass: the shared-store objects of the mapping stack, or the ``do_bg`` background with
-    its own keyframe copies.  Rows are those ``obj_ids`` names."""
+    its own keyframe copies.  Rows are those ``obj_ids`` names; ``kf_frame`` is the device table of their keyframes'
+    frame ids, which ``BundleAdjuster`` provides."""
 
     def __init__(self, ens: VmapEnsemble, obj_ids: Sequence[Optional[int]], cfg, n_iter: int, bg: bool,
                  impl: str = "fp32"):
@@ -41,16 +43,19 @@ class _BaGroup:
         self.smp = BatchedSampler(ens.device, n1, cfg.n_bins, cfg.surface_eps, cfg.stop_eps, cfg.min_depth)
         self.win = cfg.win_size_bg if bg else cfg.win_size                     # draws per iteration (train.py:196-199)
         self.n_pix_draw = cfg.n_samples_per_frame_bg if bg else cfg.n_samples_per_frame
-        self.R, self.S, self.KF = self.win * self.n_pix_draw, n1 + cfg.n_bins, cfg.keyframe_buffer_size
+        self.n_pix, self.S, self.KF = self.win * self.n_pix_draw, n1 + cfg.n_bins, cfg.keyframe_buffer_size
         self.n_draws = n_iter * self.win
-        if ens.lib.vmb_track_tiles(ens.hidden, self.R, self.S) < 0:
-            raise _lib.VmbError(f"bundle adjustment: hidden {ens.hidden} does not support {self.S} samples per ray")
+        self._tiles("bundle adjustment")
         dev = ens.device
         self.rows_dev = torch.tensor(self.rows, dtype=torch.int32, device=dev)
         self.tables = SamplerTables(dev, B, kf_stride=0 if bg else self.KF)
         self.out = self.smp._outputs(B, self.n_draws * self.n_pix_draw, self.S, False)
         self.kf_out = torch.zeros(B, self.n_draws, dtype=torch.int32, device=dev)
-        self.ray_rows = torch.zeros(B * self.R, _lib.TRACK_PART, dtype=torch.float64, device=dev)
+        self._alloc_rows(B)
+
+    def _alloc_rows(self, B: int) -> None:
+        """The step's per-ray rows."""
+        self.ray_rows = torch.zeros(B * self.n_pix, _lib.TRACK_PART, dtype=torch.float64, device=self.ens.device)
 
     def fill(self, objects: Dict[int, object], store, kf_frame: np.ndarray) -> None:
         """The sampler tables and ``kf_frame`` [B, KF] (frame id of each keyframe index, -1: none) on the host."""
@@ -76,22 +81,13 @@ class _BaGroup:
         else:
             self.smp.sample_store(store, self.tables, self.n_draws, self.n_pix_draw, rays_dir, seed=seed, **kw)
 
-    def bind(self, g, it: int, kf_frame: torch.Tensor) -> None:
-        """vmb_ba_group for iteration ``it`` (0-based): rays [it * R, (it + 1) * R), draws [it * win, (it + 1) * win)."""
-        e, B, R, S, N = self.ens, len(self.rows), self.R, self.S, self.n_draws * self.n_pix_draw
-        o = self.out
-        g.hidden, g.n_obj, g.n_rows, g.rows = e.hidden, B, e.n_obj, _ptr(self.rows_dev)
-        g.n_rays, g.n_samples = R, S
-        g.pcs, g.pcs_stride = C.c_void_p(o["pcs"].data_ptr() + it * R * S * 12), N * S * 3
-        g.z_vals, g.z_stride = C.c_void_p(o["z"].data_ptr() + it * R * S * 4), N * S
-        g.gt_depth, g.gt_depth_stride = C.c_void_p(o["gt_depth"].data_ptr() + it * R * 4), N
-        g.gt_colour, g.gt_colour_stride = C.c_void_p(o["gt_colour"].data_ptr() + it * R * 12), N * 3
-        g.sem, g.sem_stride = C.c_void_p(o["sem"].data_ptr() + it * R), N
-        g.mask_depth, g.mask_stride = C.c_void_p(o["mask_depth"].data_ptr() + it * R), N
-        g.params, g.scale = _ptr(e.params), _ptr(e.scale)
+    def bind(self, g, it: int) -> None:
+        """vmb_ba_group for iteration ``it`` (0-based): rays [it * n_pix, (it + 1) * n_pix), draws
+        [it * win, (it + 1) * win)."""
+        super().bind(g, it)
         g.n_pix_draw = self.n_pix_draw
         g.kf_draw, g.kf_draw_stride = C.c_void_p(self.kf_out.data_ptr() + it * self.win * 4), self.n_draws
-        g.kf_frame, g.kf_stride = _ptr(kf_frame), self.KF
+        g.kf_frame, g.kf_stride = _ptr(self.kf_frame), self.KF
         g.ray_rows, g.max_ray_rows = _ptr(self.ray_rows), self.ray_rows.shape[0]
 
 
@@ -157,6 +153,8 @@ class BundleAdjuster:
             o += s
         self._cap = cap
         self._uploaded = None
+        for k, g in enumerate(self.groups):
+            g.kf_frame = self._d(k)
 
     def _h(self, k):
         o, s = self._views[k]
@@ -217,7 +215,7 @@ class BundleAdjuster:
         bg = [g for g in self.groups if g.bg]
         if bg:
             targets.append((self._d(ng + 2), objects[bg[0].ids[bg[0].rows[0]]].t_wc_batch, bg[0].KF))
-        a = _iterate(self.groups, [self._d(k) for k in range(ng)], self.n_iter, poses, self._d(ng), self.max_win,
+        a = _iterate(self.groups, self.n_iter, poses, self._d(ng), self.max_win,
                      self.hold, self.adam, self.scratch, self.lr_rot, self.lr_trans, self.losses, self.status,
                      self.pose_hist, self.grad_hist, targets)
         self._args = a
@@ -235,18 +233,8 @@ class BundleAdjuster:
         pose, no store pose and no draw counter."""
         self.prepare(store, objects)
         bg = [objects[g.ids[g.rows[0]]].t_wc_batch for g in self.groups if g.bg]
-        keep = [t.clone() for t in [poses, store.t_wc, self.counter] + bg]
-        st = torch.cuda.Stream(device=self.device)
-        st.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(st):
-            self._enqueue(store, poses, objects)
-        torch.cuda.current_stream(self.device).wait_stream(st)
-        torch.cuda.synchronize(self.device)
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self._enqueue(store, poses, objects, upload=False)
-        for dst, src in zip([poses, store.t_wc, self.counter] + bg, keep):
-            dst.copy_(src)
+        self.graph = capture_graph(self.device, lambda upload: self._enqueue(store, poses, objects, upload=upload),
+                                   [poses, store.t_wc, self.counter] + bg)
         self._graph_key = (store, store.t_wc.data_ptr(), poses.data_ptr())
 
     def replay(self, store, poses: torch.Tensor, objects: Dict[int, object]) -> List[int]:
@@ -263,7 +251,7 @@ class BundleAdjuster:
         return win
 
 
-def _iterate(groups, kf_frames, n_iter, poses, window, n_win, hold, adam, scratch, lr_rot, lr_trans, losses, status,
+def _iterate(groups, n_iter, poses, window, n_win, hold, adam, scratch, lr_rot, lr_trans, losses, status,
              pose_hist=None, grad_hist=None, targets=()):
     """n_iter x [vmb_ba_step per group -> vmb_ba_update] on the groups' sample buffers."""
     a = _lib.BaArgs()
@@ -281,7 +269,7 @@ def _iterate(groups, kf_frames, n_iter, poses, window, n_win, hold, adam, scratc
     for it in range(n_iter):
         a.iter = it + 1
         for gi, g in enumerate(groups):
-            _BaGroup.bind(g, a.group[gi], it, kf_frames[gi])
+            g.bind(a.group[gi], it)
         for gi, g in enumerate(groups):
             _step(g, a, gi, ba=True)
         with e0._on_device():
@@ -289,7 +277,7 @@ def _iterate(groups, kf_frames, n_iter, poses, window, n_win, hold, adam, scratc
     return a
 
 
-class BaSampleGroup:
+class BaSampleGroup(_BaGroup):
     """A group fed with given samples instead of the sampler (tests, timing): ``batch`` holds [B, n_iter * R] rays of
     camera-frame points (``pcs`` [B,N,S,3]) and targets for the rows ``rows`` of ``ens``; ``kf_draw`` [B, N / n_pix_draw]
     the keyframe index of each draw and ``kf_frame`` [B, KF] the frame id of each keyframe index (-1: none); ``impl``
@@ -300,19 +288,16 @@ class BaSampleGroup:
         self.ens, self.rows, self.lw = ens, list(rows), _use_lw(ens, impl)
         B, N, S = batch["pcs"].shape[:3]
         assert B == len(self.rows) and N % n_iter == 0 and (N // n_iter) % n_pix_draw == 0
-        self.R, self.S, self.n_pix_draw = N // n_iter, S, n_pix_draw
-        self.win, self.n_draws = self.R // n_pix_draw, N // n_pix_draw
+        self.n_pix, self.S, self.n_pix_draw = N // n_iter, S, n_pix_draw
+        self.win, self.n_draws = self.n_pix // n_pix_draw, N // n_pix_draw
+        self._upload(self.rows, batch)
         dev = ens.device
-        self.out = {k: v.to(dev).contiguous() for k, v in batch.items()}
-        self.out["mask_depth"] = self.out["mask_depth"].to(torch.uint8)
-        self.rows_dev = torch.tensor(self.rows, dtype=torch.int32, device=dev)
         self.kf_out = torch.as_tensor(kf_draw, dtype=torch.int32).to(dev).contiguous()
         self.kf_frame = torch.as_tensor(kf_frame, dtype=torch.int32).to(dev).contiguous()
         self.KF = self.kf_frame.shape[1]
         assert self.kf_out.shape == (B, self.n_draws) and self.kf_frame.shape[0] == B
-        if ens.lib.vmb_track_tiles(ens.hidden, self.R, S) < 0:
-            raise _lib.VmbError(f"bundle adjustment: hidden {ens.hidden} does not support {S} samples per ray")
-        self.ray_rows = torch.zeros(B * self.R, _lib.TRACK_PART, dtype=torch.float64, device=dev)
+        self._tiles("bundle adjustment")
+        self._alloc_rows(B)
 
 
 def ba_samples(groups: Sequence[BaSampleGroup], poses, window: Sequence[int], n_iter: int, lr_rot: float,
@@ -330,7 +315,7 @@ def ba_samples(groups: Sequence[BaSampleGroup], poses, window: Sequence[int], n_
         out["pose_hist"] = torch.zeros(n_iter + 1, n_win, 4, 4, **f64)
         out["grad_hist"] = torch.zeros(n_iter, n_win, 6, **f64)
     win = torch.tensor(list(window), dtype=torch.int32, device=dev)
-    _iterate(list(groups), [g.kf_frame for g in groups], n_iter, P, win, n_win, hold, torch.zeros(n_win, 12, **f64),
+    _iterate(list(groups), n_iter, P, win, n_win, hold, torch.zeros(n_win, 12, **f64),
              torch.zeros(8 * n_seg + 6 * n_win, **f64), lr_rot, lr_trans, out["losses"], out["status"],
              out.get("pose_hist"), out.get("grad_hist"))
     return out

@@ -1,6 +1,7 @@
 // K11: bundle adjustment of keyframe poses against the object map -- pose-only passes against a frozen map, run between
 // mapping frames.  The step is K10's (k_track.cuh) with a pose per ray; the update is one Adam / Exp over every frame
-// of the pass's window.
+// of the pass's window.  The parts of the rule K10 shares (frame lookup, point, per-ray loss, pose terms, Adam / Exp)
+// are the helpers of k_track.cuh.
 //
 // The rule (oracle/ba_oracle.py restates it):
 //   Samples  each object of the mapping stack samples its own keyframe table with K3 in the mapping layout,
@@ -19,7 +20,7 @@
 //            bitwise reproducible, eager or replayed.
 //   Update   one Adam over the stacked tangents of the window frames, no weight decay, moments reset at iteration 1
 //            of each pass, bias correction by the pass's iteration; a window frame no ray saw has gradient 0 (its
-//            momentum still moves it).  R_f <- Exp(dphi) R_f, t_f <- t_f + drho in fp64 (track_exp).  `hold` (frame
+//            momentum still moves it).  R_f <- Exp(dphi) R_f, t_f <- t_f + drho in fp64 (pose_adam_exp).  `hold` (frame
 //            0, the caller's anchor) never moves.  A non-finite loss, window gradient or window pose skips the whole
 //            iteration's update (at iteration 1 the moments are still reset) and sets VMB_ST_NONFINITE.
 //   Write-back after the last iteration, each window frame's pose goes in fp32 to every entry i of each target
@@ -53,8 +54,7 @@ struct BaUpdateParams {
   double* pose;                  // [n_poses][16] in/out
   double* adam;                  // [n_win][12]
   double* scratch;               // [segments][8] | [n_win][6]
-  double lr[6], b1, b2, eps, bc1, bc2;
-  double cs, os;
+  PoseUpdateScalars s;
   double* loss;                  // optional [n_iter]
   double* pose_hist;             // optional [n_iter+1][n_win][16]
   double* grad_hist;             // optional [n_iter][n_win][6]
@@ -92,7 +92,7 @@ __global__ void __launch_bounds__(256) k_ba_update(BaUpdateParams a) {
     const int f = ba_draw_frame(G.kf_draw, G.kf_draw_stride, G.kf_frame, G.kf_stride, a.n_poses, ob, d);
     double* o = seg + (size_t)s * 8;
     for (int c = 0; c < 6; ++c) o[c] = acc[c];
-    o[6] = acc[6] + a.cs * acc[7] + a.os * acc[8];
+    o[6] = acc[6] + a.s.cs * acc[7] + a.s.os * acc[8];
     o[7] = (double)f;
   }
   __syncthreads();
@@ -142,28 +142,10 @@ __global__ void __launch_bounds__(256) k_ba_update(BaUpdateParams a) {
       double* P = a.pose + (size_t)f * 16;
       double T[16];
       for (int i = 0; i < 16; ++i) T[i] = P[i];
-      double d[6];
-      for (int c = 0; c < 6; ++c) {
-        const double gc = gw[(size_t)w * 6 + c];
-        const double m = (a.iter == 1 ? 0.0 : a.b1 * A[c]) + (1.0 - a.b1) * gc;
-        const double v = (a.iter == 1 ? 0.0 : a.b2 * A[6 + c]) + (1.0 - a.b2) * gc * gc;
-        A[c] = m; A[6 + c] = v;
-        d[c] = -a.lr[c] * (m / a.bc1) / (sqrt(v / a.bc2) + a.eps);
-      }
-      const double wv[3] = {d[0], d[1], d[2]};
-      double E[9];
-      track_exp(wv, E);
-      double Rn[9];
-      for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 3; ++j)
-          Rn[i * 3 + j] = E[i * 3 + 0] * T[0 * 4 + j] + E[i * 3 + 1] * T[1 * 4 + j] + E[i * 3 + 2] * T[2 * 4 + j];
-      for (int i = 0; i < 3; ++i) {
-        for (int j = 0; j < 3; ++j) T[i * 4 + j] = Rn[i * 3 + j];
-        T[i * 4 + 3] += d[3 + i];
-      }
+      pose_adam_exp(T, A, gw + (size_t)w * 6, a.iter, a.s);
       for (int i = 0; i < 16; ++i) P[i] = T[i];
-    } else if (a.iter == 1) {
-      for (int c = 0; c < 12; ++c) A[c] = 0.0;
+    } else {
+      pose_adam_skip(A, a.iter);
     }
     if (!live) continue;
     const double* P = a.pose + (size_t)f * 16;

@@ -2,7 +2,9 @@
 // on-device Adam / Exp pose optimiser.  CUDA-core fp32 for the networks (the layout and dense helpers of
 // k_step_fp32.cuh, no weight gradients), fp64 for the pose, the partial sums and the update.
 //
-// The rule (oracle/track_oracle.py restates it):
+// The rule (oracle/track_oracle.py restates it).  The parts K11 (k_ba.cuh) and the layer-wise path (k_track_lw.cuh)
+// share are written once below, as the helpers ba_draw_frame, slice_mask_count, pose_point, ray_loss, pose_terms and
+// pose_adam_exp; each kernel keeps only its own reductions.
 //   Pose     camera-to-world T_wc = [R | t] (the reference's twc), fp64 [4][4] row-major in device memory.
 //   Samples  each tracked object samples the frame once in the camera frame (K3's camera_frame mode: the points of an
 //            IDENTITY pose; one keyframe: the new frame's slot and the object's 2-D box from this frame's ingest; the
@@ -84,6 +86,8 @@ struct BaRays {
   double* rows;                                     // out [B][R][VMB_TRACK_PART] per-ray rows
 };
 
+// ---- the pose rule, written once for K10, K11 (k_ba.cuh) and the layer-wise path (k_track_lw.cuh) -----------------
+
 // frame id of draw `d` of object `b`, or -1 when the keyframe index or the frame id is outside its table
 __device__ __forceinline__ int ba_draw_frame(const int* kf_draw, long long kf_draw_stride, const int* kf_frame,
                                              int kf_stride, int n_poses, int b, int d) {
@@ -91,6 +95,62 @@ __device__ __forceinline__ int ba_draw_frame(const int* kf_draw, long long kf_dr
   if (kf < 0 || kf >= kf_stride) return -1;
   const int f = kf_frame[(size_t)b * kf_stride + kf];
   return (f >= 0 && f < n_poses) ? f : -1;
+}
+
+// the slice's mask counts (loss.py:16-18,38), one ray's increment: depth (mask and object), object, not-unknown
+__device__ __forceinline__ void slice_mask_count(const unsigned char* sem, const unsigned char* mask, int r, int& nd,
+                                                 int& no, int& ns) {
+  const int s = sem[r];
+  const int mo = s != 0;
+  nd += (mask[r] != 0) & mo; no += mo; ns += s != 2;
+}
+
+// the network input of camera-frame point q: p = R q + t in fp32 from an fp32 copy of the fp64 pose T, then p / scale
+__device__ __forceinline__ float3 pose_point(const double* T, float3 q, float sc) {
+  const float x = fmaf((float)T[2], q.z, fmaf((float)T[1], q.y, (float)T[0] * q.x)) + (float)T[3];
+  const float y = fmaf((float)T[6], q.z, fmaf((float)T[5], q.y, (float)T[4] * q.x)) + (float)T[7];
+  const float w = fmaf((float)T[10], q.z, fmaf((float)T[9], q.y, (float)T[8] * q.x)) + (float)T[11];
+  return make_float3(x / sc, y / sc, w / sc);
+}
+
+// one point's pose terms c = ((R q) x g, g) in fp64 from the fp64 pose, g = dL/dt / scale (q: the fp32 point, widened)
+__device__ __forceinline__ void pose_terms(const double* T, double3 q, float3 dt, float sc, double (&c)[6]) {
+  const double g0 = (double)(dt.x / sc), g1 = (double)(dt.y / sc), g2 = (double)(dt.z / sc);
+  const double x0 = T[0] * q.x + T[1] * q.y + T[2] * q.z;     // R q in fp64
+  const double x1 = T[4] * q.x + T[5] * q.y + T[6] * q.z;
+  const double x2 = T[8] * q.x + T[9] * q.y + T[10] * q.z;
+  c[0] = x1 * g2 - x2 * g1; c[1] = x2 * g0 - x0 * g2; c[2] = x0 * g1 - x1 * g0;
+  c[3] = g0; c[4] = g1; c[5] = g2;
+}
+
+// One ray's loss from its fp64 render (depth D, opacity O, colour C, detached variance V): the three loss terms
+// L_d, L_c, L_o in fp64 and the fp32 upstream gradients d(loss)/d(D, C, O).  Empty masks are handled per object and per
+// term: cnt[] are the object's slice counts (nd, no, ns), and a term whose count is 0 contributes 0.  A ray without a
+// pose (rok false) is masked out of every term.
+struct RayLoss { double l[3]; float gD, gC0, gC1, gC2, gO; };
+
+__device__ __forceinline__ RayLoss ray_loss(double D, double O, double C0, double C1, double C2, double V, int sv,
+                                            bool md, float gt_d, const float* gc, bool rok, const int (&cnt)[3],
+                                            float cs, float os) {
+  RayLoss r;
+  const double m_o = (sv != 0 && rok) ? 1.0 : 0.0;
+  const double m_s = (sv != 2 && rok) ? 1.0 : 0.0;
+  const double m_d = md ? m_o : 0.0;
+  const double gd = gt_d;
+  const double inv_nd = cnt[0] ? 1.0 / ((double)cnt[0] + 1e-10) : 0.0;
+  const double inv_no = cnt[1] ? 1.0 / ((double)cnt[1] + 1e-10) : 0.0;
+  const double inv_ns = cnt[2] ? 1.0 / ((double)cnt[2] + 1e-10) : 0.0;
+  const double info = 1.0 / (sqrt(V) + 1e-4);               // render_rays.py:74-79
+  const double e_d = D - gd, e_o = O - m_o;
+  const double e_c0 = C0 - (double)gc[0], e_c1 = C1 - (double)gc[1], e_c2 = C2 - (double)gc[2];
+  r.l[0] = cnt[0] ? fabs(e_d) * m_d * info * inv_nd : 0.0;
+  r.l[1] = cnt[1] ? (fabs(e_c0) + fabs(e_c1) + fabs(e_c2)) * m_o * inv_no : 0.0;
+  r.l[2] = cnt[2] ? fabs(e_o) * m_s * inv_ns : 0.0;
+  r.gD = (float)(m_d * info * inv_nd) * vmb_sign((float)e_d);
+  const float kc = (float)((double)cs * m_o * inv_no);
+  r.gC0 = kc * vmb_sign((float)e_c0); r.gC1 = kc * vmb_sign((float)e_c1); r.gC2 = kc * vmb_sign((float)e_c2);
+  r.gO = (float)((double)os * m_s * inv_ns) * vmb_sign((float)e_o);
+  return r;
 }
 
 // One CTA (128 threads) = one tile of nr = TP / S whole rays of one tracked object (blockIdx.y), as k_step_fp32.
@@ -145,11 +205,7 @@ __device__ __forceinline__ void track_step_body(const TrackParams& a, const VmbL
     const unsigned char* sv = a.sem + (size_t)b * a.sem_stride;
     const unsigned char* mv = a.mask + (size_t)b * a.mask_stride;
     int nd = 0, no = 0, ns = 0;
-    for (int r = tid; r < R; r += NT) {
-      const int s = sv[r];
-      const int mo = s != 0;
-      nd += (mv[r] != 0) & mo; no += mo; ns += s != 2;
-    }
+    for (int r = tid; r < R; r += NT) slice_mask_count(sv, mv, r, nd, no, ns);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
       nd += __shfl_xor_sync(0xffffffffu, nd, o);
@@ -168,24 +224,21 @@ __device__ __forceinline__ void track_step_body(const TrackParams& a, const VmbL
     pok = f >= 0;
     T = a.pose + (size_t)(pok ? f : 0) * 16;
   }
-  float q0 = 0.f, q1 = 0.f, q2 = 0.f, t0 = 0.f, t1 = 0.f, t2 = 0.f;
+  float3 q = make_float3(0.f, 0.f, 0.f), t = q;
   const float sc = a.scale[row];
   if (pok) {
     const size_t gi = (size_t)b * a.pcs_stride + ((size_t)(r0 + rl) * S + sidx) * 3;
-    q0 = a.pcs[gi]; q1 = a.pcs[gi + 1]; q2 = a.pcs[gi + 2];
-    const float x = fmaf((float)T[2], q2, fmaf((float)T[1], q1, (float)T[0] * q0)) + (float)T[3];
-    const float y = fmaf((float)T[6], q2, fmaf((float)T[5], q1, (float)T[4] * q0)) + (float)T[7];
-    const float w = fmaf((float)T[10], q2, fmaf((float)T[9], q1, (float)T[8] * q0)) + (float)T[11];
-    t0 = x / sc; t1 = y / sc; t2 = w / sc;
+    q = make_float3(a.pcs[gi], a.pcs[gi + 1], a.pcs[gi + 2]);
+    t = pose_point(T, q, sc);
   }
   if (og == 0) {
-    sE[0 * PT + p] = t0; sE[1 * PT + p] = t1; sE[2 * PT + p] = t2;
+    sE[0 * PT + p] = t.x; sE[1 * PT + p] = t.y; sE[2 * PT + p] = t.z;
     sHd[8 * PT + p] = pvalid ? a.z[(size_t)b * a.z_stride + (size_t)(r0 + rl) * S + sidx] : 0.f;
     sHd[4 * PT + p] = 0.f; sHd[5 * PT + p] = 0.f; sHd[6 * PT + p] = 0.f; sHd[7 * PT + p] = 0.f;
   }
   for (int d = og; d < VMB_NDIRS; d += NOG) {
     const float* Bd = P + L.o_B + d * 3;
-    const float proj = fmaf(__ldg(Bd + 2), t2, fmaf(__ldg(Bd + 1), t1, __ldg(Bd) * t0));
+    const float proj = fmaf(__ldg(Bd + 2), t.z, fmaf(__ldg(Bd + 1), t.y, __ldg(Bd) * t.x));
     for (int k = 0; k < L.nfreq; ++k) sE[(3 + k * VMB_NDIRS + d) * PT + p] = sinf((proj * (float)(1 << k)) * VMB_PI_F);
   }
   __syncthreads();
@@ -286,24 +339,11 @@ __device__ __forceinline__ void track_step_body(const TrackParams& a, const VmbL
       rok = ba_draw_frame(x.kf_draw, x.kf_draw_stride, x.kf_frame, x.kf_stride, x.n_poses, b, ray / x.n_pix_draw) >= 0;
       if (!rok && a.status) atomicOr(a.status, VMB_BA_ST_BAD_FRAME);
     }
-    const double m_o = (sv != 0 && rok) ? 1.0 : 0.0;
-    const double m_s = (sv != 2 && rok) ? 1.0 : 0.0;
-    const double m_d = (a.mask[(size_t)b * a.mask_stride + ray] != 0) ? m_o : 0.0;
-    const double gd = a.gt_depth[(size_t)b * a.gt_depth_stride + ray];
-    const float* gc = a.gt_colour + (size_t)b * a.gt_colour_stride + (size_t)ray * 3;
-    const double inv_nd = cnt[0] ? 1.0 / ((double)cnt[0] + 1e-10) : 0.0;
-    const double inv_no = cnt[1] ? 1.0 / ((double)cnt[1] + 1e-10) : 0.0;
-    const double inv_ns = cnt[2] ? 1.0 / ((double)cnt[2] + 1e-10) : 0.0;
-    const double info = 1.0 / (sqrt(V) + 1e-4);             // render_rays.py:74-79
-    const double e_d = D - gd, e_o = O - m_o;
-    const double e_c0 = C0 - (double)gc[0], e_c1 = C1 - (double)gc[1], e_c2 = C2 - (double)gc[2];
-    s_l[0][tid] = cnt[0] ? fabs(e_d) * m_d * info * inv_nd : 0.0;
-    s_l[1][tid] = cnt[1] ? (fabs(e_c0) + fabs(e_c1) + fabs(e_c2)) * m_o * inv_no : 0.0;
-    s_l[2][tid] = cnt[2] ? fabs(e_o) * m_s * inv_ns : 0.0;
-    const float gD = (float)(m_d * info * inv_nd) * vmb_sign((float)e_d);
-    const float kc = (float)((double)a.cs * m_o * inv_no);
-    const float gC0 = kc * vmb_sign((float)e_c0), gC1 = kc * vmb_sign((float)e_c1), gC2 = kc * vmb_sign((float)e_c2);
-    const float gO = (float)((double)a.os * m_s * inv_ns) * vmb_sign((float)e_o);
+    const RayLoss ls = ray_loss(D, O, C0, C1, C2, V, sv,
+                                a.mask[(size_t)b * a.mask_stride + ray] != 0, a.gt_depth[(size_t)b * a.gt_depth_stride + ray],
+                                a.gt_colour + (size_t)b * a.gt_colour_stride + (size_t)ray * 3, rok, cnt, a.cs, a.os);
+    s_l[0][tid] = ls.l[0]; s_l[1][tid] = ls.l[1]; s_l[2][tid] = ls.l[2];
+    const float gD = ls.gD, gC0 = ls.gC0, gC1 = ls.gC1, gC2 = ls.gC2, gO = ls.gO;
     float suffix = 0.f;
     for (int s = S - 1; s >= 0; --s) {
       const int qi = pb + s;
@@ -384,11 +424,11 @@ __device__ __forceinline__ void track_step_body(const TrackParams& a, const VmbL
         const int j0 = blk * OB;
         dgrad_block<OB>(acc, P + L.o_Win + j0, VMB_E1, sA1 + p, H, PT);
         dgrad_block<OB>(acc, P + L.o_Wcat + H + j0, ldc, sA3 + p, H, PT);
-        pe_input_grad<OB>(acc, j0, VMB_E1, P + L.o_B, t0, t1, t2, dt);
+        pe_input_grad<OB>(acc, j0, VMB_E1, P + L.o_B, t.x, t.y, t.z, dt);
       } else {
         const int j0 = (blk - nb1) * OB;
         dgrad_block<OB>(acc, P + L.o_Wcl + H + j0, ldl, sAC + p, H, PT);
-        pe_input_grad<OB>(acc, VMB_E1 + j0, L.E, P + L.o_B, t0, t1, t2, dt);
+        pe_input_grad<OB>(acc, VMB_E1 + j0, L.E, P + L.o_B, t.x, t.y, t.z, dt);
       }
     }
     sHd[(og * 3 + 0) * PT + p] = dt[0]; sHd[(og * 3 + 1) * PT + p] = dt[1]; sHd[(og * 3 + 2) * PT + p] = dt[2];
@@ -399,14 +439,7 @@ __device__ __forceinline__ void track_step_body(const TrackParams& a, const VmbL
 #pragma unroll
     for (int g = 0; g < NOG; ++g) { d0 += sHd[(g * 3) * PT + p]; d1 += sHd[(g * 3 + 1) * PT + p]; d2 += sHd[(g * 3 + 2) * PT + p]; }
     double c[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-    if (pok) {
-      const double g0 = (double)(d0 / sc), g1 = (double)(d1 / sc), g2 = (double)(d2 / sc);
-      const double x0 = T[0] * q0 + T[1] * q1 + T[2] * q2;   // R q in fp64
-      const double x1 = T[4] * q0 + T[5] * q1 + T[6] * q2;
-      const double x2 = T[8] * q0 + T[9] * q1 + T[10] * q2;
-      c[0] = x1 * g2 - x2 * g1; c[1] = x2 * g0 - x0 * g2; c[2] = x0 * g1 - x1 * g0;
-      c[3] = g0; c[4] = g1; c[5] = g2;
-    }
+    if (pok) pose_terms(T, make_double3(q.x, q.y, q.z), make_float3(d0, d1, d2), sc, c);
 #pragma unroll
     for (int i = 0; i < 6; ++i) s_g[i][p] = c[i];
   }
@@ -444,11 +477,27 @@ static size_t track_smem(const VmbLayout& L) {
   return sizeof(float) * (size_t)(L.E + 5 * H + 12) * (TP + 1);
 }
 
+// host: raise kernel K's dynamic shared-memory limit to `bytes` on device `dev`, the first time only
+template <auto K>
+static cudaError_t pose_smem_limit(int dev, int bytes) {
+  static bool set[64] = {};      // per device (one process may drive several GPUs)
+  if (set[dev & 63]) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e == cudaSuccess) set[dev & 63] = true;
+  return e;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // Update: one CTA of 256 threads.  Thread k sums the objects k, k + 256, ... of the concatenated (group, object) list,
 // each object's tiles in order; a fixed tree joins the threads; thread 0 runs Adam + Exp.
 // ---------------------------------------------------------------------------------------------------------------------
 struct TrackGroupDev { const double* partials; int n_obj, tiles; float* loss_terms; };
+
+// Adam's rates, betas, eps and bias corrections 1 - b^iter for the iteration, and the loss weights
+struct PoseUpdateScalars {
+  double lr[6], b1, b2, eps, bc1, bc2;
+  double cs, os;
+};
 
 struct TrackUpdateParams {
   int n_groups;
@@ -456,15 +505,15 @@ struct TrackUpdateParams {
   int iter;                      // 1-based iteration of this frame
   double* pose;                  // [16] in/out
   double* adam;                  // [12] m, v (not read at iter 1)
-  double lr[6], b1, b2, eps, bc1, bc2;
-  double cs, os;
+  PoseUpdateScalars s;
   double* loss;                  // optional [n_iter]: loss[iter-1]
   double* pose_hist;             // optional [n_iter+1][16]
   double* grad_hist;             // optional [n_iter][6]
   int* status;
 };
 
-__device__ inline void track_exp(const double (&w)[3], double (&E)[9]) {
+// Exp of so(3) by Rodrigues in fp64, I + [w]x below |w| = 1e-12
+__device__ inline void pose_exp(const double (&w)[3], double (&E)[9]) {
   const double th2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
   const double th = sqrt(th2);
   double A, Bc;
@@ -477,6 +526,35 @@ __device__ inline void track_exp(const double (&w)[3], double (&E)[9]) {
       for (int m = 0; m < 3; ++m) k2 += K[i * 3 + m] * K[m * 3 + j];
       E[i * 3 + j] = (i == j ? 1.0 : 0.0) + A * K[i * 3 + j] + Bc * k2;
     }
+}
+
+// One Adam step on the tangent (phi, rho) with gradient g[6] and moments A = m[6], v[6] (not read at iteration 1), then
+// the left update R <- Exp(delta_phi) R, t <- t + delta_rho of the pose T (row-major [4][4]).
+__device__ __forceinline__ void pose_adam_exp(double (&T)[16], double* A, const double* g, int iter,
+                                              const PoseUpdateScalars& s) {
+  double d[6];
+  for (int c = 0; c < 6; ++c) {
+    const double m = (iter == 1 ? 0.0 : s.b1 * A[c]) + (1.0 - s.b1) * g[c];
+    const double v = (iter == 1 ? 0.0 : s.b2 * A[6 + c]) + (1.0 - s.b2) * g[c] * g[c];
+    A[c] = m; A[6 + c] = v;
+    d[c] = -s.lr[c] * (m / s.bc1) / (sqrt(v / s.bc2) + s.eps);
+  }
+  const double w[3] = {d[0], d[1], d[2]};
+  double E[9];
+  pose_exp(w, E);
+  double Rn[9];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j)
+      Rn[i * 3 + j] = E[i * 3 + 0] * T[0 * 4 + j] + E[i * 3 + 1] * T[1 * 4 + j] + E[i * 3 + 2] * T[2 * 4 + j];
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) T[i * 4 + j] = Rn[i * 3 + j];
+    T[i * 4 + 3] += d[3 + i];
+  }
+}
+
+// a skipped update still restarts the moments when it is the first iteration
+__device__ __forceinline__ void pose_adam_skip(double* A, int iter) {
+  if (iter == 1) for (int c = 0; c < 12; ++c) A[c] = 0.0;
 }
 
 __global__ void __launch_bounds__(256) k_track_update(TrackUpdateParams a) {
@@ -497,7 +575,7 @@ __global__ void __launch_bounds__(256) k_track_update(TrackUpdateParams a) {
       for (int t = 0; t < G.tiles; ++t)
 #pragma unroll
         for (int c = 0; c < 9; ++c) s[c] += pr[(size_t)t * VMB_TRACK_PART + c];
-      const double tot = s[6] + a.cs * s[7] + a.os * s[8];
+      const double tot = s[6] + a.s.cs * s[7] + a.s.os * s[8];
       if (G.loss_terms) {
         float* lt = G.loss_terms + (size_t)ob * 4;
         lt[0] = (float)s[6]; lt[1] = (float)s[7]; lt[2] = (float)s[8]; lt[3] = (float)tot;
@@ -531,27 +609,10 @@ __global__ void __launch_bounds__(256) k_track_update(TrackUpdateParams a) {
   for (int c = 0; c < 6; ++c) ok = ok && isfinite(g[c]);
   for (int i = 0; i < 16; ++i) ok = ok && isfinite(T[i]);
   if (ok) {
-    double d[6];
-    for (int c = 0; c < 6; ++c) {
-      const double m = (a.iter == 1 ? 0.0 : a.b1 * a.adam[c]) + (1.0 - a.b1) * g[c];
-      const double v = (a.iter == 1 ? 0.0 : a.b2 * a.adam[6 + c]) + (1.0 - a.b2) * g[c] * g[c];
-      a.adam[c] = m; a.adam[6 + c] = v;
-      d[c] = -a.lr[c] * (m / a.bc1) / (sqrt(v / a.bc2) + a.eps);
-    }
-    const double w[3] = {d[0], d[1], d[2]};
-    double E[9];
-    track_exp(w, E);
-    double Rn[9];
-    for (int i = 0; i < 3; ++i)
-      for (int j = 0; j < 3; ++j)
-        Rn[i * 3 + j] = E[i * 3 + 0] * T[0 * 4 + j] + E[i * 3 + 1] * T[1 * 4 + j] + E[i * 3 + 2] * T[2 * 4 + j];
-    for (int i = 0; i < 3; ++i) {
-      for (int j = 0; j < 3; ++j) T[i * 4 + j] = Rn[i * 3 + j];
-      T[i * 4 + 3] += d[3 + i];
-    }
+    pose_adam_exp(T, a.adam, g, a.iter, a.s);
     for (int i = 0; i < 16; ++i) a.pose[i] = T[i];
   } else {
-    if (a.iter == 1) for (int c = 0; c < 12; ++c) a.adam[c] = 0.0;   // a skipped first iteration still restarts the moments
+    pose_adam_skip(a.adam, a.iter);
     if (a.status) atomicOr(a.status, VMB_ST_NONFINITE);
   }
   if (a.pose_hist) for (int i = 0; i < 16; ++i) a.pose_hist[(size_t)a.iter * 16 + i] = T[i];

@@ -3,17 +3,19 @@
 //
 // The rule is K10's (k_track.cuh) and, for the BA flavour, K11's (k_ba.cuh): same samples, same points, same loss with
 // the per-object, per-term empty-mask rule, same left-perturbation gradient, same output rows, so vmb_track_update and
-// vmb_ba_update run unchanged on what this path writes.  What differs is where the network runs and its precision:
+// vmb_ba_update run unchanged on what this path writes.  The parts that do not depend on where the network runs are
+// the helpers of k_track.cuh that K10 and K11 call too: ba_draw_frame, slice_mask_count, pose_point, ray_loss and
+// pose_terms.  What differs is where the network runs and its precision:
 //   Weights  object b reads params row rows[b] and the fp16 image row rows[b] (as the AdamW launch writes it).  Both
 //            are copied on the device into this path's workspace first, so rows[] stays a device array (capturable);
 //            a row outside [0, n_rows) contributes nothing and sets VMB_TRACK_ST_BAD_ROW, as K10.
-//   Points   p = R q + t from an fp32 copy of the fp64 pose, K10's operation order, then p / scale; the embedding row
+//   Points   pose_point: p = R q + t from an fp32 copy of the fp64 pose, then p / scale; the embedding row
 //            is k_lw_pe's (fp16, sin by sincos_ladder6, constant-1 columns).  K11: the ray's pose is its draw's frame
 //            (ba_draw_frame); a ray whose frame is outside the table contributes nothing and sets VMB_BA_ST_BAD_FRAME.
 //   Network  the five forward GEMMs of step_object (fp16 operands, fp32 accumulation, fp16 activations).
 //   Render   one warp per ray, lane = sample (S <= 32): the heads in fp32 from the fp16 activations; the composite,
-//            render and loss in fp64 in sample order exactly as K10 (1 - occ as sigmoid(-alpha)); mask counts of this
-//            slice per object (integers); the backward to (raw alpha, raw colour) in fp32 as K10.  Each ray's three
+//            render in fp64 in sample order exactly as K10 (1 - occ as sigmoid(-alpha)) and ray_loss on it; mask counts
+//            of this slice per object (integers); the backward to (raw alpha, raw colour) in fp32 as K10.  Each ray's three
 //            loss terms go to an fp64 per-ray buffer.  d(raw alpha) and dYc are loss-scaled by LS = 2^8 and clamped to
 //            the fp16 range +-60000 as in the training kernel.  status[1] gets a LOWER BOUND on the clamped values
 //            (and VMB_TRACK_ST_CLAMP is set when it is not 0): every clamped dYc element, plus every element where the
@@ -22,13 +24,13 @@
 //   Backward the input-gradient GEMM chain of step_object only (colour-block dE, dY4 with the rank-1 d_alpha term, dY3,
 //            dY2, dY1, the fused dE GEMM): no weight-gradient GEMMs, no column sums, no side stream.
 //   Pose     per point dL/dt = INV_LS (dE_xyz + sum_{k,d} dE_{k,d} pi 2^k cos(pi 2^k proj_d) B_d) in fp32 (the cosines
-//            of sincos_ladder6, as k_lw_pe_bwd), g = dL/dt / scale, and the point's terms ((R q) x g, g) in fp64 from
-//            the fp64 pose.  Track flavour: the terms are summed in point order over the rays of each of K10's tiles
+//            of sincos_ladder6, as k_lw_pe_bwd), then pose_terms: ((R q) x g, g), g = dL/dt / scale, in fp64 from the
+//            fp64 pose.  Track flavour: the terms are summed in point order over the rays of each of K10's tiles
 //            (nr = TP / S rays, TP = vmb_track_tiles' tile), plus the per-ray loss terms in ray order: exactly K10's
 //            partial rows.  BA flavour: one row per ray (its samples in order), as K11.
 // No floating-point atomics anywhere on this path (the GEMM epilogues used here store): bitwise reproducible.
 // Registers (ptxas -v, sm_90a; track / BA flavour), no spills in any of them:
-//   k_tlw_gather 32; k_tlw_pe 74 / 74; k_tlw_render H 64: 71 / 68, H 128: 71 / 68, H 256: 68 / 68;
+//   k_tlw_gather 32; k_tlw_pe 74 / 74; k_tlw_render H 64: 67 / 68, H 128: 67 / 68, H 256: 67 / 68;
 //   k_tlw_pose 62 / 62; k_tlw_reduce 40 / 40.
 #pragma once
 #include "k_layerwise.cuh"
@@ -91,14 +93,7 @@ struct TlwObj {
 // frame id of ray r (BA) or 0 (track); -1 = outside the pose table
 template <bool BA>
 __device__ __forceinline__ int tlw_frame(const TlwObj& o, int r) {
-  if constexpr (BA) {
-    const int kf = o.kf_draw[r / o.n_pix_draw];
-    if (kf < 0 || kf >= o.kf_stride) return -1;
-    const int f = o.kf_frame[kf];
-    return (f >= 0 && f < o.n_poses) ? f : -1;
-  } else {
-    return 0;
-  }
+  return BA ? ba_draw_frame(o.kf_draw, 0, o.kf_frame, o.kf_stride, o.n_poses, 0, r / o.n_pix_draw) : 0;
 }
 
 // ---- 1: the object's weights into the workspace; block 0 also counts the slice's masks (loss.py:16-18,38) ----------
@@ -122,11 +117,7 @@ __global__ void __launch_bounds__(256) k_tlw_gather(TlwObj o, const float* __res
   if (threadIdx.x < 3) s_cnt[threadIdx.x] = 0;
   __syncthreads();
   int nd = 0, no = 0, ns = 0;
-  for (int r = threadIdx.x; r < o.R; r += blockDim.x) {
-    const int s = sem[r];
-    const int mo = s != 0;
-    nd += (mask[r] != 0) & mo; no += mo; ns += s != 2;
-  }
+  for (int r = threadIdx.x; r < o.R; r += blockDim.x) slice_mask_count(sem, mask, r, nd, no, ns);
   atomicAdd(&s_cnt[0], nd); atomicAdd(&s_cnt[1], no); atomicAdd(&s_cnt[2], ns);
   __syncthreads();
   if (threadIdx.x < 3) ctl[threadIdx.x] = s_cnt[threadIdx.x];
@@ -135,19 +126,15 @@ __global__ void __launch_bounds__(256) k_tlw_gather(TlwObj o, const float* __res
   if (threadIdx.x == 5 && !ok && o.status) atomicOr(o.status, VMB_TRACK_ST_BAD_ROW);
 }
 
-// p / scale of point p = ray r, sample s (K10's operation order); false where the ray has no pose
+// camera-frame point q and network input t = pose_point(q) of point p = ray r, sample s; false where the ray has no pose
 template <bool BA>
-__device__ __forceinline__ bool tlw_point(const TlwObj& o, long long p, float sc, float& q0, float& q1, float& q2, float& t0,
-                                          float& t1, float& t2, const double*& T) {
+__device__ __forceinline__ bool tlw_point(const TlwObj& o, long long p, float sc, float3& q, float3& t, const double*& T) {
   const int f = tlw_frame<BA>(o, (int)(p / o.S));
-  q0 = q1 = q2 = t0 = t1 = t2 = 0.f;
+  q = t = make_float3(0.f, 0.f, 0.f);
   T = o.pose + (size_t)(f > 0 ? f : 0) * 16;
   if (f < 0) return false;
-  q0 = o.pcs[p * 3]; q1 = o.pcs[p * 3 + 1]; q2 = o.pcs[p * 3 + 2];
-  const float x = fmaf((float)T[2], q2, fmaf((float)T[1], q1, (float)T[0] * q0)) + (float)T[3];
-  const float y = fmaf((float)T[6], q2, fmaf((float)T[5], q1, (float)T[4] * q0)) + (float)T[7];
-  const float w = fmaf((float)T[10], q2, fmaf((float)T[9], q1, (float)T[8] * q0)) + (float)T[11];
-  t0 = x / sc; t1 = y / sc; t2 = w / sc;
+  q = make_float3(o.pcs[p * 3], o.pcs[p * 3 + 1], o.pcs[p * 3 + 2]);
+  t = pose_point(T, q, sc);
   return true;
 }
 
@@ -163,10 +150,10 @@ __global__ void __launch_bounds__(128) k_tlw_pe(TlwObj o, const float* __restric
   __shared__ __align__(16) __half row[128 * EW];
   const long long p0 = (long long)blockIdx.x * 128, p = p0 + threadIdx.x;
   __half* r = row + threadIdx.x * EW;
-  float q0, q1, q2, t0 = 0.f, t1 = 0.f, t2 = 0.f;
+  float3 q, t = make_float3(0.f, 0.f, 0.f);
   const double* T;
-  if (p < P) tlw_point<BA>(o, p, sc, q0, q1, q2, t0, t1, t2, T);
-  pe_row(r, t0, t1, t2, dirs);                       // k_lw_pe's row
+  if (p < P) tlw_point<BA>(o, p, sc, q, t, T);
+  pe_row(r, t.x, t.y, t.z, dirs);                    // k_lw_pe's row
   __syncthreads();
   const uint4* src = reinterpret_cast<const uint4*>(row);
   uint4* dst = reinterpret_cast<uint4*>(E + p0 * EW);
@@ -194,10 +181,7 @@ __global__ void __launch_bounds__(128) k_tlw_render(TlwObj o, TlwRender a, const
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, S = o.S;
   const unsigned FULL = 0xffffffffu;
   const float b_a = P[L.o_ba], b_c0 = P[L.o_boc], b_c1 = P[L.o_boc + 1], b_c2 = P[L.o_boc + 2];
-  const int cnt0 = ctl[0], cnt1 = ctl[1], cnt2 = ctl[2];
-  const double inv_nd = cnt0 ? 1.0 / ((double)cnt0 + 1e-10) : 0.0;
-  const double inv_no = cnt1 ? 1.0 / ((double)cnt1 + 1e-10) : 0.0;
-  const double inv_ns = cnt2 ? 1.0 / ((double)cnt2 + 1e-10) : 0.0;
+  const int cnt[3] = {ctl[0], ctl[1], ctl[2]};
   const bool in = lane < S;
   unsigned char* srow = hr_rows + warp * (32 * PITCH);
   int n_clamp = 0;
@@ -267,26 +251,13 @@ __global__ void __launch_bounds__(128) k_tlw_render(TlwObj o, TlwRender a, const
       const double dz = (double)__shfl_sync(FULL, zz, s) - D;
       V += (double)__shfl_sync(FULL, wf, s) * dz * dz;  // loss.py:28-29 (detached)
     }
-    const int sv = a.sem[ray];
     const bool rok = tlw_frame<BA>(o, ray) >= 0;
     if (BA && !rok && lane == 0 && o.status) atomicOr(o.status, VMB_BA_ST_BAD_FRAME);
-    const double m_o = (sv != 0 && rok) ? 1.0 : 0.0;
-    const double m_s = (sv != 2 && rok) ? 1.0 : 0.0;
-    const double m_d = (a.mask[ray] != 0) ? m_o : 0.0;
-    const double gd = a.gt_depth[ray];
-    const float* gc = a.gt_colour + (size_t)ray * 3;
-    const double info = 1.0 / (sqrt(V) + 1e-4);      // render_rays.py:74-79
-    const double e_d = D - gd, e_o = O - m_o;
-    const double e_c0 = C0 - (double)gc[0], e_c1 = C1 - (double)gc[1], e_c2 = C2 - (double)gc[2];
-    if (lane == 0) {
-      lossr[(size_t)ray * 3 + 0] = cnt0 ? fabs(e_d) * m_d * info * inv_nd : 0.0;
-      lossr[(size_t)ray * 3 + 1] = cnt1 ? (fabs(e_c0) + fabs(e_c1) + fabs(e_c2)) * m_o * inv_no : 0.0;
-      lossr[(size_t)ray * 3 + 2] = cnt2 ? fabs(e_o) * m_s * inv_ns : 0.0;
-    }
-    const float gD = (float)(m_d * info * inv_nd) * vmb_sign((float)e_d);
-    const float kc = (float)((double)a.cs * m_o * inv_no);
-    const float gC0 = kc * vmb_sign((float)e_c0), gC1 = kc * vmb_sign((float)e_c1), gC2 = kc * vmb_sign((float)e_c2);
-    const float gO = (float)((double)a.os * m_s * inv_ns) * vmb_sign((float)e_o);
+    const RayLoss ls = ray_loss(D, O, C0, C1, C2, V, a.sem[ray], a.mask[ray] != 0, a.gt_depth[ray], a.gt_colour + (size_t)ray * 3,
+                                rok, cnt, a.cs, a.os);
+    if (lane == 0)
+      for (int c = 0; c < 3; ++c) lossr[(size_t)ray * 3 + c] = ls.l[c];
+    const float gD = ls.gD, gC0 = ls.gC0, gC1 = ls.gC1, gC2 = ls.gC2, gO = ls.gO;
     const float Gs = fmaf(gD, zz, fmaf(gC0, c0, fmaf(gC1, c1, fmaf(gC2, c2, gO))));
     const float fr = vmb_sigmoid(-al);               // 1 - occ
     float suffix = 0.f, docc = 0.f;                   // K10's suffix sum, samples from the last
@@ -347,28 +318,21 @@ __global__ void __launch_bounds__(128) k_tlw_pose(TlwObj o, const float* __restr
   if (p >= P) return;
   const float sc = __int_as_float(ctl[4]);
   const float* dirs = prow + o_B;
-  float q0, q1, q2, t0, t1, t2;
+  float3 q, t;
   const double* T;
-  const bool pok = tlw_point<BA>(o, p, sc, q0, q1, q2, t0, t1, t2, T);
+  const bool pok = tlw_point<BA>(o, p, sc, q, t, T);
   const float* g = sg + threadIdx.x * PEB_LD;
   float dt0 = g[0] * INV_LS, dt1 = g[1] * INV_LS, dt2 = g[2] * INV_LS;
 #pragma unroll 1
   for (int d = 0; d < VMB_NDIRS; ++d) {
     const float b0 = dirs[d * 3], b1 = dirs[d * 3 + 1], b2 = dirs[d * 3 + 2];
     float s[6], c[6];
-    sincos_ladder6(fmaf(b2, t2, fmaf(b1, t1, b0 * t0)), s, c);
+    sincos_ladder6(fmaf(b2, t.z, fmaf(b1, t.y, b0 * t.x)), s, c);
     const float dp = pe_dproj(g, d, c) * (VMB_PI_F * INV_LS);       // as k_lw_pe_bwd
     dt0 = fmaf(dp, b0, dt0); dt1 = fmaf(dp, b1, dt1); dt2 = fmaf(dp, b2, dt2);
   }
   double c6[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-  if (pok && ctl[3]) {
-    const double g0 = (double)(dt0 / sc), g1 = (double)(dt1 / sc), g2 = (double)(dt2 / sc);
-    const double x0 = T[0] * q0 + T[1] * q1 + T[2] * q2;   // R q in fp64
-    const double x1 = T[4] * q0 + T[5] * q1 + T[6] * q2;
-    const double x2 = T[8] * q0 + T[9] * q1 + T[10] * q2;
-    c6[0] = x1 * g2 - x2 * g1; c6[1] = x2 * g0 - x0 * g2; c6[2] = x0 * g1 - x1 * g0;
-    c6[3] = g0; c6[4] = g1; c6[5] = g2;
-  }
+  if (pok && ctl[3]) pose_terms(T, make_double3(q.x, q.y, q.z), make_float3(dt0, dt1, dt2), sc, c6);
 #pragma unroll
   for (int i = 0; i < 6; ++i) gpt[p * 6 + i] = c6[i];
 }
@@ -434,14 +398,9 @@ static int track_object_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGrou
   arm();
   TLW_TRY(launch_k(k_tlw_pe<BA>, dim3(nblk), dim3(128), 0, st, o, (const float*)tw.prow, (const int*)tw.ctl, L.o_B, ws.E));
   TLW_TRY(forward_gemms<H>(ws, L, tw.prow, tw.wimg, np, pdl_ok, st));
-  {
-    static bool attr_set[64] = {};
-    int dev = 0; cudaGetDevice(&dev);
-    if (!attr_set[dev & 63]) {
-      TLW_TRY(cudaFuncSetAttribute(k_tlw_render<H, BA>, cudaFuncAttributeMaxDynamicSharedMemorySize, hr_smem<H>()));
-      attr_set[dev & 63] = true;
-    }
-  }
+  int dev = 0;
+  cudaGetDevice(&dev);
+  TLW_TRY((pose_smem_limit<k_tlw_render<H, BA>>(dev, hr_smem<H>())));
   TlwRender ra;
   ra.z = a.z + (size_t)b * a.z_stride; ra.gt_depth = a.gt_depth + (size_t)b * a.gt_depth_stride;
   ra.gt_colour = a.gt_colour + (size_t)b * a.gt_colour_stride; ra.sem = sem; ra.mask = mask; ra.cs = a.cs; ra.os = a.os;
@@ -463,14 +422,7 @@ static int track_object_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGrou
   TLW_TRY(dgrad_gate_gemm<H>(ws.dYa, tw.wimg, off_m1(H), H, np, ws.X1, ws.dYc, nullptr, nullptr, st));    // dY1 -> dYc
   arm();
   TLW_TRY(demb1_gemm<H>(ws, ws.dYb, ws.dYc, tw.wimg, np, st));                                           // d emb1
-  {
-    static bool attr_set[64] = {};
-    int dev = 0; cudaGetDevice(&dev);
-    if (!attr_set[dev & 63]) {
-      TLW_TRY(cudaFuncSetAttribute(k_tlw_pose<BA>, cudaFuncAttributeMaxDynamicSharedMemorySize, PEB_SMEM));
-      attr_set[dev & 63] = true;
-    }
-  }
+  TLW_TRY(pose_smem_limit<k_tlw_pose<BA>>(dev, PEB_SMEM));
   arm();
   TLW_TRY(launch_k(k_tlw_pose<BA>, dim3(nblk), dim3(128), (size_t)PEB_SMEM, st, o, (const float*)tw.prow, (const int*)tw.ctl, L.o_B,
                    (const float*)ws.dE, tw.gpt));

@@ -4,6 +4,7 @@
 #include <cstring>
 #include <cmath>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/vmap_b200.h"
@@ -1177,29 +1178,139 @@ int vmb_debug_gemm(int a_mn, int b_mn, int epi, int M, int N, int K1, int K2, co
 
 }  // extern "C"
 
-// ---- K10: tracking -------------------------------------------------------------------------------------------------
+// ---- K10 / K11 and their layer-wise path: one host path for the four step entry points ------------------------------
 static int track_tile(int hidden) { return hidden == 32 ? 128 : (hidden == 256 ? 32 : 64); }   // as dispatch_fp32
 
-template <int H, int TP>
-static int launch_track(vmb_handle* h, const TrackParams& tp, int tiles, cudaStream_t st) {
+template <int H, int TP, bool BA>
+static int launch_pose(vmb_handle* h, const TrackParams& tp, const BaRays& x, int tiles, cudaStream_t st) {
   const size_t smem = track_smem<H, TP>(h->L);
-  static bool attr_set[64] = {};
-  if (!attr_set[h->device & 63]) {
-    CUDA_TRY(h, cudaFuncSetAttribute(k_track_step<H, TP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set[h->device & 63] = true;
+  const dim3 grid((unsigned)tiles, (unsigned)tp.B);
+  if constexpr (BA) {
+    CUDA_TRY(h, (pose_smem_limit<k_ba_step<H, TP>>(h->device, (int)smem)));
+    k_ba_step<H, TP><<<grid, 128, smem, st>>>(tp, h->L, x);
+  } else {
+    CUDA_TRY(h, (pose_smem_limit<k_track_step<H, TP>>(h->device, (int)smem)));
+    k_track_step<H, TP><<<grid, 128, smem, st>>>(tp, h->L);
   }
-  k_track_step<H, TP><<<dim3((unsigned)tiles, (unsigned)tp.B), 128, smem, st>>>(tp, h->L);
   CUDA_TRY(h, cudaGetLastError());
   return VMB_OK;
 }
 
-static int track_common(vmb_handle* h, const vmb_track_args* a, const char* who) {
+// the checks shared by every tracking (vmb_track_args) and bundle-adjustment (vmb_ba_args) entry point
+template <class Args>
+static int pose_args_ok(vmb_handle* h, const Args* a, const char* who) {
   if (!a) return fail(h, VMB_E_ARG, std::string(who) + ": null argument");
   if (a->n_groups < 1 || a->n_groups > VMB_TRACK_MAX_GROUPS)
     return fail(h, VMB_E_ARG, std::string(who) + ": n_groups must be in [1, 8]");
   if (a->n_iter < 1 || a->iter < 1 || a->iter > a->n_iter)
     return fail(h, VMB_E_ARG, std::string(who) + ": need n_iter >= 1 and 1 <= iter <= n_iter");
-  if (!a->pose) return fail(h, VMB_E_ARG, std::string(who) + ": pose is NULL");
+  if constexpr (std::is_same_v<Args, vmb_ba_args>) {
+    if (!a->poses || a->n_poses < 1) return fail(h, VMB_E_ARG, std::string(who) + ": need a pose table");
+  } else {
+    if (!a->pose) return fail(h, VMB_E_ARG, std::string(who) + ": pose is NULL");
+  }
+  return VMB_OK;
+}
+
+static int ba_group_ok(const vmb_ba_group& g) {
+  if (g.n_obj < 1 || g.n_obj > 65535 || g.n_rows < 1 || g.n_rays < 1 || g.n_samples < 1 || g.n_pix_draw < 1 ||
+      g.n_rays % g.n_pix_draw != 0 || g.kf_stride < 1 || g.kf_draw_stride < g.n_rays / g.n_pix_draw)
+    return VMB_E_ARG;
+  if (!g.kf_draw || !g.kf_frame || !g.ray_rows || (long long)g.n_obj * g.n_rays > g.max_ray_rows) return VMB_E_ARG;
+  return VMB_OK;
+}
+
+// Check group g, a vmb_track_group or vmb_ba_group (their leading fields share names), and fill the step's arguments
+// from it: the sample slice, the network, `pose` (the pose or the pose table), the loss weights and status of `a`.
+// Returns the group's tile count, or the VMB_E_* code of the failed check.
+template <class G, class Args>
+static int pose_group_params(vmb_handle* h, const G& g, const double* pose, const Args* a, const char* who, bool lw,
+                             const void* image, TrackParams& tp) {
+  constexpr bool BA = std::is_same_v<G, vmb_ba_group>;
+  const std::string w(who);
+  if (g.hidden != h->H) return fail(h, VMB_E_ARG, w + ": group hidden size differs from the handle's");
+  if (lw && !h->lw_ok) return fail(h, VMB_E_UNSUPPORTED, w + ": the layer-wise path needs hidden 64/128/256 and n_freq 6");
+  if constexpr (BA) {
+    if (ba_group_ok(g) != VMB_OK) return fail(h, VMB_E_ARG, w + ": bad counts, draw layout, keyframe tables or ray rows");
+  } else {
+    if (g.n_obj < 1 || g.n_obj > 65535 || g.n_rows < 1 || g.n_rays < 1 || g.n_samples < 1)
+      return fail(h, VMB_E_ARG, w + ": bad n_obj / n_rows / n_rays / n_samples");
+  }
+  bool missing = !g.rows || !g.pcs || !g.z_vals || !g.gt_depth || !g.gt_colour || !g.sem || !g.mask_depth || !g.params ||
+                 !g.scale || (lw && !image);
+  if constexpr (!BA) missing = missing || !g.partials;
+  if (missing) return fail(h, VMB_E_ARG, w + ": missing tensor pointer");
+  const int tiles = vmb_track_tiles(g.hidden, g.n_rays, g.n_samples);
+  if (lw && (tiles == VMB_E_UNSUPPORTED || g.n_samples > 32)) return fail(h, VMB_E_UNSUPPORTED, w + ": n_samples above 32");
+  if (tiles == VMB_E_UNSUPPORTED)
+    return fail(h, VMB_E_UNSUPPORTED, w + ": n_samples exceeds the tile size for this hidden size");
+  if (tiles < 1) return fail(h, VMB_E_ARG, w + ": bad shape");
+  memset(&tp, 0, sizeof(tp));
+  if constexpr (!BA) {
+    if ((long long)tiles * g.n_obj > g.max_partials) return fail(h, VMB_E_ARG, w + ": partials buffer too small");
+    tp.partials = g.partials;
+  }
+  tp.B = g.n_obj; tp.R = g.n_rays; tp.S = g.n_samples; tp.n_rows = g.n_rows; tp.rows = g.rows;
+  tp.pcs = g.pcs; tp.pcs_stride = g.pcs_stride; tp.z = g.z_vals; tp.z_stride = g.z_stride;
+  tp.gt_depth = g.gt_depth; tp.gt_depth_stride = g.gt_depth_stride;
+  tp.gt_colour = g.gt_colour; tp.gt_colour_stride = g.gt_colour_stride;
+  tp.sem = g.sem; tp.sem_stride = g.sem_stride; tp.mask = g.mask_depth; tp.mask_stride = g.mask_stride;
+  tp.params = g.params; tp.scale = g.scale; tp.pose = pose;
+  tp.cs = a->colour_scaling; tp.os = a->opacity_scaling; tp.status = a->status;
+  return tiles;
+}
+
+// The step of group `group`: K10 (vmb_track_args) or K11 (vmb_ba_args), on CUDA cores or on the layer-wise path (LW).
+template <bool LW, class Args>
+static int pose_step(vmb_handle* h, const Args* a, int group, const void* image, void* stream, const char* who) {
+  constexpr bool BA = std::is_same_v<Args, vmb_ba_args>;
+  if (!h) return fail(h, VMB_E_ARG, std::string(who) + ": null handle");
+  const int rc0 = pose_args_ok(h, a, who);
+  if (rc0 != VMB_OK) return rc0;
+  if (group < 0 || group >= a->n_groups) return fail(h, VMB_E_ARG, std::string(who) + ": group index outside [0, n_groups)");
+  const auto& g = a->group[group];
+  TrackParams tp;
+  BaRays x;
+  memset(&x, 0, sizeof(x));
+  int tiles;
+  if constexpr (BA) {
+    tiles = pose_group_params(h, g, a->poses, a, who, LW, image, tp);
+    if (tiles < 0) return tiles;
+    x.kf_draw = g.kf_draw; x.kf_draw_stride = g.kf_draw_stride; x.kf_frame = g.kf_frame; x.kf_stride = g.kf_stride;
+    x.n_pix_draw = g.n_pix_draw; x.n_poses = a->n_poses; x.rows = g.ray_rows;
+  } else {
+    tiles = pose_group_params(h, g, a->pose, a, who, LW, image, tp);
+    if (tiles < 0) return tiles;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  if constexpr (LW) {
+    const lw::TlwGroup G{tp, x, (const __half*)image, BA ? 1 : track_tile(g.hidden) / g.n_samples};
+    std::string err;
+    const int rc = lw::launch_track_lw<BA>(BA ? h->ws_ba : h->ws_track, h->L, G, st, err);
+    if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, std::string(who) + ": " + err);
+    return VMB_OK;
+  } else {
+    switch (h->H) {
+      case 32:  return launch_pose<32, 128, BA>(h, tp, x, tiles, st);
+      case 64:  return launch_pose<64, 64, BA>(h, tp, x, tiles, st);
+      case 128: return launch_pose<128, 64, BA>(h, tp, x, tiles, st);
+      case 256: return launch_pose<256, 32, BA>(h, tp, x, tiles, st);
+    }
+    return fail(h, VMB_E_UNSUPPORTED, std::string(who) + ": unsupported hidden size");
+  }
+}
+
+// the update's checks and Adam scalars, shared by vmb_track_update and vmb_ba_update
+template <class Args>
+static int pose_update_scalars(vmb_handle* h, const Args* a, const char* who, PoseUpdateScalars& s) {
+  if (!(std::isfinite(a->lr_rot) && a->lr_rot >= 0.0 && std::isfinite(a->lr_trans) && a->lr_trans >= 0.0 &&
+        a->beta1 >= 0.0 && a->beta1 < 1.0 && a->beta2 >= 0.0 && a->beta2 < 1.0 && a->eps > 0.0 && std::isfinite(a->eps)))
+    return fail(h, VMB_E_ARG, std::string(who) + ": need finite rates >= 0, betas in [0, 1) and eps > 0");
+  for (int c = 0; c < 3; ++c) { s.lr[c] = a->lr_rot; s.lr[3 + c] = a->lr_trans; }
+  s.b1 = a->beta1; s.b2 = a->beta2; s.eps = a->eps;
+  s.bc1 = 1.0 - std::pow(a->beta1, (double)a->iter);
+  s.bc2 = 1.0 - std::pow(a->beta2, (double)a->iter);
+  s.cs = a->colour_scaling; s.os = a->opacity_scaling;
   return VMB_OK;
 }
 
@@ -1214,51 +1325,30 @@ int vmb_track_tiles(int hidden, int n_rays, int n_samples) {
 }
 
 int vmb_track_step(vmb_handle* h, const vmb_track_args* a, int group, void* stream) {
-  if (!h) return fail(h, VMB_E_ARG, "vmb_track_step: null handle");
-  const int rc0 = track_common(h, a, "vmb_track_step");
-  if (rc0 != VMB_OK) return rc0;
-  if (group < 0 || group >= a->n_groups) return fail(h, VMB_E_ARG, "vmb_track_step: group index outside [0, n_groups)");
-  const vmb_track_group& g = a->group[group];
-  if (g.hidden != h->H) return fail(h, VMB_E_ARG, "vmb_track_step: group hidden size differs from the handle's");
-  if (g.n_obj < 1 || g.n_obj > 65535 || g.n_rows < 1 || g.n_rays < 1 || g.n_samples < 1)
-    return fail(h, VMB_E_ARG, "vmb_track_step: bad n_obj / n_rows / n_rays / n_samples");
-  if (!g.rows || !g.pcs || !g.z_vals || !g.gt_depth || !g.gt_colour || !g.sem || !g.mask_depth || !g.params ||
-      !g.scale || !g.partials)
-    return fail(h, VMB_E_ARG, "vmb_track_step: missing tensor pointer");
-  const int tiles = vmb_track_tiles(g.hidden, g.n_rays, g.n_samples);
-  if (tiles == VMB_E_UNSUPPORTED)
-    return fail(h, VMB_E_UNSUPPORTED, "vmb_track_step: n_samples exceeds the tile size for this hidden size");
-  if (tiles < 1) return fail(h, VMB_E_ARG, "vmb_track_step: bad shape");
-  if ((long long)tiles * g.n_obj > g.max_partials) return fail(h, VMB_E_ARG, "vmb_track_step: partials buffer too small");
-  TrackParams tp;
-  memset(&tp, 0, sizeof(tp));
-  tp.B = g.n_obj; tp.R = g.n_rays; tp.S = g.n_samples; tp.n_rows = g.n_rows; tp.rows = g.rows;
-  tp.pcs = g.pcs; tp.pcs_stride = g.pcs_stride; tp.z = g.z_vals; tp.z_stride = g.z_stride;
-  tp.gt_depth = g.gt_depth; tp.gt_depth_stride = g.gt_depth_stride;
-  tp.gt_colour = g.gt_colour; tp.gt_colour_stride = g.gt_colour_stride;
-  tp.sem = g.sem; tp.sem_stride = g.sem_stride; tp.mask = g.mask_depth; tp.mask_stride = g.mask_stride;
-  tp.params = g.params; tp.scale = g.scale; tp.pose = a->pose; tp.partials = g.partials;
-  tp.cs = a->colour_scaling; tp.os = a->opacity_scaling; tp.status = a->status;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (h->H) {
-    case 32:  return launch_track<32, 128>(h, tp, tiles, st);
-    case 64:  return launch_track<64, 64>(h, tp, tiles, st);
-    case 128: return launch_track<128, 64>(h, tp, tiles, st);
-    case 256: return launch_track<256, 32>(h, tp, tiles, st);
-  }
-  return fail(h, VMB_E_UNSUPPORTED, "vmb_track_step: unsupported hidden size");
+  return pose_step<false>(h, a, group, nullptr, stream, "vmb_track_step");
+}
+
+int vmb_ba_step(vmb_handle* h, const vmb_ba_args* a, int group, void* stream) {
+  return pose_step<false>(h, a, group, nullptr, stream, "vmb_ba_step");
+}
+
+int vmb_track_step_lw(vmb_handle* h, const vmb_track_args* a, int group, const void* image, void* stream) {
+  return pose_step<true>(h, a, group, image, stream, "vmb_track_step_lw");
+}
+
+int vmb_ba_step_lw(vmb_handle* h, const vmb_ba_args* a, int group, const void* image, void* stream) {
+  return pose_step<true>(h, a, group, image, stream, "vmb_ba_step_lw");
 }
 
 int vmb_track_update(vmb_handle* h, const vmb_track_args* a, void* stream) {
   if (!h) return fail(h, VMB_E_ARG, "vmb_track_update: null handle");
-  const int rc0 = track_common(h, a, "vmb_track_update");
+  const int rc0 = pose_args_ok(h, a, "vmb_track_update");
   if (rc0 != VMB_OK) return rc0;
   if (!a->adam) return fail(h, VMB_E_ARG, "vmb_track_update: adam state is NULL");
-  if (!(std::isfinite(a->lr_rot) && a->lr_rot >= 0.0 && std::isfinite(a->lr_trans) && a->lr_trans >= 0.0 &&
-        a->beta1 >= 0.0 && a->beta1 < 1.0 && a->beta2 >= 0.0 && a->beta2 < 1.0 && a->eps > 0.0 && std::isfinite(a->eps)))
-    return fail(h, VMB_E_ARG, "vmb_track_update: need finite rates >= 0, betas in [0, 1) and eps > 0");
   TrackUpdateParams u;
   memset(&u, 0, sizeof(u));
+  const int rc1 = pose_update_scalars(h, a, "vmb_track_update", u.s);
+  if (rc1 != VMB_OK) return rc1;
   u.n_groups = a->n_groups;
   for (int i = 0; i < a->n_groups; ++i) {
     const vmb_track_group& g = a->group[i];
@@ -1268,101 +1358,22 @@ int vmb_track_update(vmb_handle* h, const vmb_track_args* a, void* stream) {
     u.g[i].partials = g.partials; u.g[i].n_obj = g.n_obj; u.g[i].tiles = tiles; u.g[i].loss_terms = g.loss_terms;
   }
   u.iter = a->iter; u.pose = a->pose; u.adam = a->adam;
-  for (int c = 0; c < 3; ++c) { u.lr[c] = a->lr_rot; u.lr[3 + c] = a->lr_trans; }
-  u.b1 = a->beta1; u.b2 = a->beta2; u.eps = a->eps;
-  u.bc1 = 1.0 - std::pow(a->beta1, (double)a->iter);
-  u.bc2 = 1.0 - std::pow(a->beta2, (double)a->iter);
-  u.cs = a->colour_scaling; u.os = a->opacity_scaling;
   u.loss = a->loss; u.pose_hist = a->pose_hist; u.grad_hist = a->grad_hist; u.status = a->status;
   k_track_update<<<1, 256, 0, (cudaStream_t)stream>>>(u);
   CUDA_TRY(h, cudaGetLastError());
   return VMB_OK;
 }
 
-}  // extern "C"
-
-// ---- K11: bundle adjustment ------------------------------------------------------------------------------------------
-template <int H, int TP>
-static int launch_ba(vmb_handle* h, const TrackParams& tp, const BaRays& x, int tiles, cudaStream_t st) {
-  const size_t smem = track_smem<H, TP>(h->L);
-  static bool attr_set[64] = {};
-  if (!attr_set[h->device & 63]) {
-    CUDA_TRY(h, cudaFuncSetAttribute(k_ba_step<H, TP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set[h->device & 63] = true;
-  }
-  k_ba_step<H, TP><<<dim3((unsigned)tiles, (unsigned)tp.B), 128, smem, st>>>(tp, h->L, x);
-  CUDA_TRY(h, cudaGetLastError());
-  return VMB_OK;
-}
-
-static int ba_common(vmb_handle* h, const vmb_ba_args* a, const char* who) {
-  if (!a) return fail(h, VMB_E_ARG, std::string(who) + ": null argument");
-  if (a->n_groups < 1 || a->n_groups > VMB_TRACK_MAX_GROUPS)
-    return fail(h, VMB_E_ARG, std::string(who) + ": n_groups must be in [1, 8]");
-  if (a->n_iter < 1 || a->iter < 1 || a->iter > a->n_iter)
-    return fail(h, VMB_E_ARG, std::string(who) + ": need n_iter >= 1 and 1 <= iter <= n_iter");
-  if (!a->poses || a->n_poses < 1) return fail(h, VMB_E_ARG, std::string(who) + ": need a pose table");
-  return VMB_OK;
-}
-
-static int ba_group_ok(const vmb_ba_group& g) {
-  if (g.n_obj < 1 || g.n_obj > 65535 || g.n_rows < 1 || g.n_rays < 1 || g.n_samples < 1 || g.n_pix_draw < 1 ||
-      g.n_rays % g.n_pix_draw != 0 || g.kf_stride < 1 || g.kf_draw_stride < g.n_rays / g.n_pix_draw)
-    return VMB_E_ARG;
-  if (!g.kf_draw || !g.kf_frame || !g.ray_rows || (long long)g.n_obj * g.n_rays > g.max_ray_rows) return VMB_E_ARG;
-  return VMB_OK;
-}
-
-extern "C" {
-
-int vmb_ba_step(vmb_handle* h, const vmb_ba_args* a, int group, void* stream) {
-  if (!h) return fail(h, VMB_E_ARG, "vmb_ba_step: null handle");
-  const int rc0 = ba_common(h, a, "vmb_ba_step");
-  if (rc0 != VMB_OK) return rc0;
-  if (group < 0 || group >= a->n_groups) return fail(h, VMB_E_ARG, "vmb_ba_step: group index outside [0, n_groups)");
-  const vmb_ba_group& g = a->group[group];
-  if (g.hidden != h->H) return fail(h, VMB_E_ARG, "vmb_ba_step: group hidden size differs from the handle's");
-  if (ba_group_ok(g) != VMB_OK)
-    return fail(h, VMB_E_ARG, "vmb_ba_step: bad counts, draw layout, keyframe tables or ray rows");
-  if (!g.rows || !g.pcs || !g.z_vals || !g.gt_depth || !g.gt_colour || !g.sem || !g.mask_depth || !g.params || !g.scale)
-    return fail(h, VMB_E_ARG, "vmb_ba_step: missing tensor pointer");
-  const int tiles = vmb_track_tiles(g.hidden, g.n_rays, g.n_samples);
-  if (tiles == VMB_E_UNSUPPORTED)
-    return fail(h, VMB_E_UNSUPPORTED, "vmb_ba_step: n_samples exceeds the tile size for this hidden size");
-  if (tiles < 1) return fail(h, VMB_E_ARG, "vmb_ba_step: bad shape");
-  TrackParams tp;
-  memset(&tp, 0, sizeof(tp));
-  tp.B = g.n_obj; tp.R = g.n_rays; tp.S = g.n_samples; tp.n_rows = g.n_rows; tp.rows = g.rows;
-  tp.pcs = g.pcs; tp.pcs_stride = g.pcs_stride; tp.z = g.z_vals; tp.z_stride = g.z_stride;
-  tp.gt_depth = g.gt_depth; tp.gt_depth_stride = g.gt_depth_stride;
-  tp.gt_colour = g.gt_colour; tp.gt_colour_stride = g.gt_colour_stride;
-  tp.sem = g.sem; tp.sem_stride = g.sem_stride; tp.mask = g.mask_depth; tp.mask_stride = g.mask_stride;
-  tp.params = g.params; tp.scale = g.scale; tp.pose = a->poses;
-  tp.cs = a->colour_scaling; tp.os = a->opacity_scaling; tp.status = a->status;
-  BaRays x;
-  x.kf_draw = g.kf_draw; x.kf_draw_stride = g.kf_draw_stride; x.kf_frame = g.kf_frame; x.kf_stride = g.kf_stride;
-  x.n_pix_draw = g.n_pix_draw; x.n_poses = a->n_poses; x.rows = g.ray_rows;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (h->H) {
-    case 32:  return launch_ba<32, 128>(h, tp, x, tiles, st);
-    case 64:  return launch_ba<64, 64>(h, tp, x, tiles, st);
-    case 128: return launch_ba<128, 64>(h, tp, x, tiles, st);
-    case 256: return launch_ba<256, 32>(h, tp, x, tiles, st);
-  }
-  return fail(h, VMB_E_UNSUPPORTED, "vmb_ba_step: unsupported hidden size");
-}
-
 int vmb_ba_update(vmb_handle* h, const vmb_ba_args* a, void* stream) {
   if (!h) return fail(h, VMB_E_ARG, "vmb_ba_update: null handle");
-  const int rc0 = ba_common(h, a, "vmb_ba_update");
+  const int rc0 = pose_args_ok(h, a, "vmb_ba_update");
   if (rc0 != VMB_OK) return rc0;
   if (!a->adam || !a->window || !a->scratch) return fail(h, VMB_E_ARG, "vmb_ba_update: adam, window or scratch is NULL");
   if (a->n_win < 1 || a->n_win > VMB_BA_MAX_WIN) return fail(h, VMB_E_ARG, "vmb_ba_update: n_win outside [1, 1024]");
-  if (!(std::isfinite(a->lr_rot) && a->lr_rot >= 0.0 && std::isfinite(a->lr_trans) && a->lr_trans >= 0.0 &&
-        a->beta1 >= 0.0 && a->beta1 < 1.0 && a->beta2 >= 0.0 && a->beta2 < 1.0 && a->eps > 0.0 && std::isfinite(a->eps)))
-    return fail(h, VMB_E_ARG, "vmb_ba_update: need finite rates >= 0, betas in [0, 1) and eps > 0");
   BaUpdateParams u;
   memset(&u, 0, sizeof(u));
+  const int rc1 = pose_update_scalars(h, a, "vmb_ba_update", u.s);
+  if (rc1 != VMB_OK) return rc1;
   u.n_groups = a->n_groups;
   long long n_seg = 0;
   for (int i = 0; i < a->n_groups; ++i) {
@@ -1381,92 +1392,9 @@ int vmb_ba_update(vmb_handle* h, const vmb_ba_args* a, void* stream) {
   }
   u.iter = a->iter; u.n_iter = a->n_iter; u.n_poses = a->n_poses; u.n_win = a->n_win; u.hold = a->hold;
   u.win = a->window; u.pose = a->poses; u.adam = a->adam; u.scratch = a->scratch;
-  for (int c = 0; c < 3; ++c) { u.lr[c] = a->lr_rot; u.lr[3 + c] = a->lr_trans; }
-  u.b1 = a->beta1; u.b2 = a->beta2; u.eps = a->eps;
-  u.bc1 = 1.0 - std::pow(a->beta1, (double)a->iter);
-  u.bc2 = 1.0 - std::pow(a->beta2, (double)a->iter);
-  u.cs = a->colour_scaling; u.os = a->opacity_scaling;
   u.loss = a->loss; u.pose_hist = a->pose_hist; u.grad_hist = a->grad_hist; u.status = a->status;
   k_ba_update<<<1, 256, 0, (cudaStream_t)stream>>>(u);
   CUDA_TRY(h, cudaGetLastError());
-  return VMB_OK;
-}
-
-}  // extern "C"
-
-// ---- K10 / K11 on the layer-wise tensor-core path ---------------------------------------------------------------------
-extern "C" {
-
-int vmb_track_step_lw(vmb_handle* h, const vmb_track_args* a, int group, const void* image, void* stream) {
-  if (!h) return fail(h, VMB_E_ARG, "vmb_track_step_lw: null handle");
-  const int rc0 = track_common(h, a, "vmb_track_step_lw");
-  if (rc0 != VMB_OK) return rc0;
-  if (group < 0 || group >= a->n_groups) return fail(h, VMB_E_ARG, "vmb_track_step_lw: group index outside [0, n_groups)");
-  const vmb_track_group& g = a->group[group];
-  if (g.hidden != h->H) return fail(h, VMB_E_ARG, "vmb_track_step_lw: group hidden size differs from the handle's");
-  if (!h->lw_ok) return fail(h, VMB_E_UNSUPPORTED, "vmb_track_step_lw: the layer-wise path needs hidden 64/128/256 and n_freq 6");
-  if (g.n_obj < 1 || g.n_obj > 65535 || g.n_rows < 1 || g.n_rays < 1 || g.n_samples < 1)
-    return fail(h, VMB_E_ARG, "vmb_track_step_lw: bad n_obj / n_rows / n_rays / n_samples");
-  if (!g.rows || !g.pcs || !g.z_vals || !g.gt_depth || !g.gt_colour || !g.sem || !g.mask_depth || !g.params ||
-      !g.scale || !g.partials || !image)
-    return fail(h, VMB_E_ARG, "vmb_track_step_lw: missing tensor pointer");
-  const int tiles = vmb_track_tiles(g.hidden, g.n_rays, g.n_samples);
-  if (tiles == VMB_E_UNSUPPORTED || g.n_samples > 32)
-    return fail(h, VMB_E_UNSUPPORTED, "vmb_track_step_lw: n_samples above 32");
-  if (tiles < 1) return fail(h, VMB_E_ARG, "vmb_track_step_lw: bad shape");
-  if ((long long)tiles * g.n_obj > g.max_partials) return fail(h, VMB_E_ARG, "vmb_track_step_lw: partials buffer too small");
-  lw::TlwGroup G;
-  memset(&G, 0, sizeof(G));
-  TrackParams& tp = G.tp;
-  tp.B = g.n_obj; tp.R = g.n_rays; tp.S = g.n_samples; tp.n_rows = g.n_rows; tp.rows = g.rows;
-  tp.pcs = g.pcs; tp.pcs_stride = g.pcs_stride; tp.z = g.z_vals; tp.z_stride = g.z_stride;
-  tp.gt_depth = g.gt_depth; tp.gt_depth_stride = g.gt_depth_stride;
-  tp.gt_colour = g.gt_colour; tp.gt_colour_stride = g.gt_colour_stride;
-  tp.sem = g.sem; tp.sem_stride = g.sem_stride; tp.mask = g.mask_depth; tp.mask_stride = g.mask_stride;
-  tp.params = g.params; tp.scale = g.scale; tp.pose = a->pose; tp.partials = g.partials;
-  tp.cs = a->colour_scaling; tp.os = a->opacity_scaling; tp.status = a->status;
-  G.image = (const __half*)image;
-  G.nr = track_tile(g.hidden) / g.n_samples;
-  std::string err;
-  const int rc = lw::launch_track_lw<false>(h->ws_track, h->L, G, (cudaStream_t)stream, err);
-  if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, "vmb_track_step_lw: " + err);
-  return VMB_OK;
-}
-
-int vmb_ba_step_lw(vmb_handle* h, const vmb_ba_args* a, int group, const void* image, void* stream) {
-  if (!h) return fail(h, VMB_E_ARG, "vmb_ba_step_lw: null handle");
-  const int rc0 = ba_common(h, a, "vmb_ba_step_lw");
-  if (rc0 != VMB_OK) return rc0;
-  if (group < 0 || group >= a->n_groups) return fail(h, VMB_E_ARG, "vmb_ba_step_lw: group index outside [0, n_groups)");
-  const vmb_ba_group& g = a->group[group];
-  if (g.hidden != h->H) return fail(h, VMB_E_ARG, "vmb_ba_step_lw: group hidden size differs from the handle's");
-  if (!h->lw_ok) return fail(h, VMB_E_UNSUPPORTED, "vmb_ba_step_lw: the layer-wise path needs hidden 64/128/256 and n_freq 6");
-  if (ba_group_ok(g) != VMB_OK)
-    return fail(h, VMB_E_ARG, "vmb_ba_step_lw: bad counts, draw layout, keyframe tables or ray rows");
-  if (!g.rows || !g.pcs || !g.z_vals || !g.gt_depth || !g.gt_colour || !g.sem || !g.mask_depth || !g.params || !g.scale ||
-      !image)
-    return fail(h, VMB_E_ARG, "vmb_ba_step_lw: missing tensor pointer");
-  const int tiles = vmb_track_tiles(g.hidden, g.n_rays, g.n_samples);
-  if (tiles == VMB_E_UNSUPPORTED || g.n_samples > 32) return fail(h, VMB_E_UNSUPPORTED, "vmb_ba_step_lw: n_samples above 32");
-  if (tiles < 1) return fail(h, VMB_E_ARG, "vmb_ba_step_lw: bad shape");
-  lw::TlwGroup G;
-  memset(&G, 0, sizeof(G));
-  TrackParams& tp = G.tp;
-  tp.B = g.n_obj; tp.R = g.n_rays; tp.S = g.n_samples; tp.n_rows = g.n_rows; tp.rows = g.rows;
-  tp.pcs = g.pcs; tp.pcs_stride = g.pcs_stride; tp.z = g.z_vals; tp.z_stride = g.z_stride;
-  tp.gt_depth = g.gt_depth; tp.gt_depth_stride = g.gt_depth_stride;
-  tp.gt_colour = g.gt_colour; tp.gt_colour_stride = g.gt_colour_stride;
-  tp.sem = g.sem; tp.sem_stride = g.sem_stride; tp.mask = g.mask_depth; tp.mask_stride = g.mask_stride;
-  tp.params = g.params; tp.scale = g.scale; tp.pose = a->poses;
-  tp.cs = a->colour_scaling; tp.os = a->opacity_scaling; tp.status = a->status;
-  BaRays& x = G.x;
-  x.kf_draw = g.kf_draw; x.kf_draw_stride = g.kf_draw_stride; x.kf_frame = g.kf_frame; x.kf_stride = g.kf_stride;
-  x.n_pix_draw = g.n_pix_draw; x.n_poses = a->n_poses; x.rows = g.ray_rows;
-  G.image = (const __half*)image;
-  G.nr = 1;
-  std::string err;
-  const int rc = lw::launch_track_lw<true>(h->ws_ba, h->L, G, (cudaStream_t)stream, err);
-  if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, "vmb_ba_step_lw: " + err);
   return VMB_OK;
 }
 

@@ -20,6 +20,7 @@ import torch
 
 from .ensemble import VmapEnsemble
 from .sampler import BatchedSampler, KeyframeSet, KeyframeTables, SamplerTables
+from .utils import capture_graph
 
 
 class Background:
@@ -102,28 +103,13 @@ class FrameLoop:
     def capture(self) -> None:
         """Warm up once (kernel attributes, allocator) on a side stream, then capture.  The warm-up frame and the
         capture itself do not advance the optimiser or the draw counter."""
-        ens = self.ens
-        all_ens = [ens] + ([self.bg.ens] if self.bg is not None else [])
-        snap = [[t.clone() for t in (e.params, e.grads, e.exp_avg, e.exp_avg_sq, e.step_counter)] for e in all_ens]
-        imgs = [e.image.clone() if e.image is not None else None for e in all_ens]
+        all_ens = [self.ens] + ([self.bg.ens] if self.bg is not None else [])
+        keep = [t for e in all_ens for t in (e.params, e.grads, e.exp_avg, e.exp_avg_sq, e.step_counter)]
+        keep += [e.image for e in all_ens if e.image is not None] + [self.counter]
         counts = [e.step_count for e in all_ens]
-        draw = self.counter.clone()
-        st = torch.cuda.Stream(device=ens.device)
-        st.wait_stream(torch.cuda.current_stream(ens.device))
-        with torch.cuda.stream(st):
-            self._enqueue()
-        torch.cuda.current_stream(ens.device).wait_stream(st)
-        torch.cuda.synchronize(ens.device)
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self._enqueue(upload=False)
-        for e, sn, im, cn in zip(all_ens, snap, imgs, counts):
-            for dst, src in zip((e.params, e.grads, e.exp_avg, e.exp_avg_sq, e.step_counter), sn):
-                dst.copy_(src)
-            if im is not None:
-                e.image.copy_(im)
+        self.graph = capture_graph(self.ens.device, self._enqueue, keep)
+        for e, cn in zip(all_ens, counts):
             e.step_count = cn
-        self.counter.copy_(draw)
 
     def run(self) -> torch.Tensor:
         """Replay the captured frame; returns the per-iteration summed losses (device tensor [n_iter])."""

@@ -26,6 +26,7 @@ import torch
 from . import _lib
 from .ensemble import VmapEnsemble, _ptr, _stream
 from .sampler import BatchedSampler, KeyframeTables, SamplerTables
+from .utils import capture_graph
 
 IMPLS = ("fp32", "layerwise")
 
@@ -59,7 +60,41 @@ def _rays_dir(cfg, device) -> torch.Tensor:
     return d.contiguous()
 
 
-class _Group:
+class _Slices:
+    """One ensemble's rows ``rows_dev`` and their sample buffers ``out``: [B, N] rays in slices of ``n_pix`` rays of
+    ``S`` samples, one slice per iteration.  Shared by the tracking and the bundle-adjustment groups."""
+
+    def _tiles(self, what: str) -> int:
+        """Tiles per object of the step at this slice shape; raises when the hidden size cannot take S samples."""
+        tiles = self.ens.lib.vmb_track_tiles(self.ens.hidden, self.n_pix, self.S)
+        if tiles < 0:
+            raise _lib.VmbError(f"{what}: hidden {self.ens.hidden} does not support {self.S} samples per ray")
+        return tiles
+
+    def _upload(self, rows: Sequence[int], batch: Dict[str, torch.Tensor]) -> None:
+        """Given samples instead of the sampler's: ``batch`` for the ensemble rows ``rows`` to the device."""
+        dev = self.ens.device
+        self.out = {k: v.to(dev).contiguous() for k, v in batch.items()}
+        self.out["mask_depth"] = self.out["mask_depth"].to(torch.uint8)
+        self.rows_dev = torch.tensor(list(rows), dtype=torch.int32, device=dev)
+
+    def bind(self, g, it: int) -> None:
+        """The fields vmb_track_group and vmb_ba_group share, for iteration ``it`` (0-based): rays
+        [it * n_pix, (it + 1) * n_pix) of every row."""
+        e, o, R, S = self.ens, self.out, self.n_pix, self.S
+        B, N = o["pcs"].shape[:2]
+        g.hidden, g.n_obj, g.n_rows, g.rows = e.hidden, B, e.n_obj, _ptr(self.rows_dev)
+        g.n_rays, g.n_samples = R, S
+        g.pcs, g.pcs_stride = C.c_void_p(o["pcs"].data_ptr() + it * R * S * 12), N * S * 3
+        g.z_vals, g.z_stride = C.c_void_p(o["z"].data_ptr() + it * R * S * 4), N * S
+        g.gt_depth, g.gt_depth_stride = C.c_void_p(o["gt_depth"].data_ptr() + it * R * 4), N
+        g.gt_colour, g.gt_colour_stride = C.c_void_p(o["gt_colour"].data_ptr() + it * R * 12), N * 3
+        g.sem, g.sem_stride = C.c_void_p(o["sem"].data_ptr() + it * R), N
+        g.mask_depth, g.mask_stride = C.c_void_p(o["mask_depth"].data_ptr() + it * R), N
+        g.params, g.scale = _ptr(e.params), _ptr(e.scale)
+
+
+class _Group(_Slices):
     """One ensemble's share of the tracking problem: its sampler, the rows tracked this frame and their buffers."""
 
     def __init__(self, ens: VmapEnsemble, obj_ids: Sequence[Optional[int]], cfg, n_pix: int, n_pix_bg: int,
@@ -74,9 +109,7 @@ class _Group:
         self.n_pix = n_pix_bg if self.bg else n_pix
         self.S = n1 + cfg.n_bins
         self.n_iter = n_iter
-        self.tiles = ens.lib.vmb_track_tiles(ens.hidden, self.n_pix, self.S)
-        if self.tiles < 0:
-            raise _lib.VmbError(f"tracking: hidden {ens.hidden} does not support {self.S} samples per ray")
+        self.tiles = self._tiles("tracking")
         self.active: List[int] = []
 
     def set_active(self, rows: Sequence[int]) -> bool:
@@ -93,9 +126,14 @@ class _Group:
         self.ids_dev = torch.tensor([self.ids[r] for r in rows], dtype=torch.int64, device=dev)
         self.tables = SamplerTables(dev, B, kf_stride=1)
         self.out = self.smp._outputs(B, self.n_iter * self.n_pix, self.S, False)
-        self.partials = torch.zeros(B * self.tiles, _lib.TRACK_PART, dtype=torch.float64, device=dev)
-        self.loss_terms = torch.zeros(B, 4, dtype=torch.float32, device=dev)
+        self._alloc_rows(B)
         return True
+
+    def _alloc_rows(self, B: int) -> None:
+        """The step's partial rows (``tiles`` per object) and the update's per-object loss terms."""
+        dev = self.ens.device
+        self.partials = torch.zeros(max(B * self.tiles, 1), _lib.TRACK_PART, dtype=torch.float64, device=dev)
+        self.loss_terms = torch.zeros(B, 4, dtype=torch.float32, device=dev)
 
     def buffers(self):
         return (self.rows_dev, self.ids_dev, self.tables, self.out, self.partials, self.loss_terms)
@@ -120,17 +158,7 @@ class _Group:
 
     def bind(self, g, it: int) -> None:
         """vmb_track_group for iteration ``it`` (0-based): rays [it * n_pix, (it + 1) * n_pix)."""
-        e, B, R, S, N = self.ens, len(self.active), self.n_pix, self.S, self.n_iter * self.n_pix
-        o = self.out
-        g.hidden, g.n_obj, g.n_rows, g.rows = e.hidden, B, e.n_obj, _ptr(self.rows_dev)
-        g.n_rays, g.n_samples = R, S
-        g.pcs, g.pcs_stride = C.c_void_p(o["pcs"].data_ptr() + it * R * S * 12), N * S * 3
-        g.z_vals, g.z_stride = C.c_void_p(o["z"].data_ptr() + it * R * S * 4), N * S
-        g.gt_depth, g.gt_depth_stride = C.c_void_p(o["gt_depth"].data_ptr() + it * R * 4), N
-        g.gt_colour, g.gt_colour_stride = C.c_void_p(o["gt_colour"].data_ptr() + it * R * 12), N * 3
-        g.sem, g.sem_stride = C.c_void_p(o["sem"].data_ptr() + it * R), N
-        g.mask_depth, g.mask_stride = C.c_void_p(o["mask_depth"].data_ptr() + it * R), N
-        g.params, g.scale = _ptr(e.params), _ptr(e.scale)
+        super().bind(g, it)
         g.partials, g.max_partials = _ptr(self.partials), self.partials.shape[0]
         g.loss_terms = _ptr(self.loss_terms)
 
@@ -231,20 +259,9 @@ class Tracker:
         """Capture the frame (sampling + every iteration) as one CUDA graph for the current set of tracked rows.  The
         warm-up and the capture do not advance the draw counter."""
         self.select(store.visible_objects().keys() if ids is None else ids)
-        draw = self.counter.clone()
-        t_wc = store.t_wc[slot].clone()
         self._prepare(store, slot, T_init)
-        st = torch.cuda.Stream(device=self.device)
-        st.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(st):
-            self._enqueue(store)
-        torch.cuda.current_stream(self.device).wait_stream(st)
-        torch.cuda.synchronize(self.device)
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self._enqueue(store, upload=False)
-        self.counter.copy_(draw)
-        store.t_wc[slot] = t_wc
+        self.graph = capture_graph(self.device, lambda upload: self._enqueue(store, upload=upload),
+                                   [self.counter, store.t_wc[slot]])
         self._graph_store = store
         self._graph_keep = [g.buffers() for g in self._live()]     # alive as long as the graph that writes them
 
@@ -277,7 +294,7 @@ def _iterate(live, n_iter, pose, adam, lr_rot, lr_trans, losses, status, pose_hi
     for it in range(n_iter):
         a.iter = it + 1
         for gi, g in enumerate(live):
-            _Group.bind(g, a.group[gi], it)
+            g.bind(a.group[gi], it)
         for gi, g in enumerate(live):
             _step(g, a, gi, ba=False)
         e = live[0].ens
@@ -286,7 +303,7 @@ def _iterate(live, n_iter, pose, adam, lr_rot, lr_trans, losses, status, pose_hi
     return a
 
 
-class SampleGroup:
+class SampleGroup(_Group):
     """A group fed with given samples instead of the sampler (tests, timing): ``batch`` holds [B, n_iter * n_pix]
     rays of camera-frame points (``pcs`` [B,N,S,3]) and targets for the rows ``rows`` of ``ens``; ``impl`` as
     ``Tracker``'s."""
@@ -297,15 +314,9 @@ class SampleGroup:
         B, N, S = batch["pcs"].shape[:3]
         assert B == len(self.active) and N % n_iter == 0
         self.n_pix, self.S = N // n_iter, S
-        dev = ens.device
-        self.out = {k: v.to(dev).contiguous() for k, v in batch.items()}
-        self.out["mask_depth"] = self.out["mask_depth"].to(torch.uint8)
-        self.rows_dev = torch.tensor(self.active, dtype=torch.int32, device=dev)
-        tiles = ens.lib.vmb_track_tiles(ens.hidden, self.n_pix, S)
-        if tiles < 0:
-            raise _lib.VmbError(f"tracking: hidden {ens.hidden} does not support {S} samples per ray")
-        self.partials = torch.zeros(max(B * tiles, 1), _lib.TRACK_PART, dtype=torch.float64, device=dev)
-        self.loss_terms = torch.zeros(B, 4, dtype=torch.float32, device=dev)
+        self._upload(self.active, batch)
+        self.tiles = self._tiles("tracking")
+        self._alloc_rows(B)
 
 
 def track_samples(groups: Sequence[SampleGroup], T_init, n_iter: int, lr_rot: float, lr_trans: float,

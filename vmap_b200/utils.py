@@ -1,6 +1,7 @@
 """utils.update_vmap with the reference's signature (utils.py:30-34), the ``vmap`` shim
-that replaces ``functorch.vmap`` at train.py:293-294, and the picklable ``BoundingBox`` that
-sceneObject.get_bound stores in checkpoints (utils.py:11-24)."""
+that replaces ``functorch.vmap`` at train.py:293-294, the picklable ``BoundingBox`` that
+sceneObject.get_bound stores in checkpoints (utils.py:11-24), and ``capture_graph``, the warm-up and capture of the
+package's CUDA-graph loops (mapping frames, tracking, bundle adjustment)."""
 from __future__ import annotations
 
 import torch
@@ -123,6 +124,25 @@ def vmap(fmodel, *args, **kwargs):
         raise TypeError("vmap_b200.vmap only maps the fused models returned by update_vmap "
                         "(no tracing / PyTorch fallback)")
     return fmodel.batched
+
+
+def capture_graph(device, enqueue, keep) -> torch.cuda.CUDAGraph:
+    """One CUDA graph of ``enqueue``: a warm-up call ``enqueue(upload=True)`` on a side stream (kernel attributes, the
+    allocator's pools), a synchronise, then the capture of ``enqueue(upload=False)``.  The tensors in ``keep`` get back
+    the values they had before the warm-up, so neither run leaves a trace in them."""
+    snap = [t.clone() for t in keep]
+    st = torch.cuda.Stream(device=device)
+    st.wait_stream(torch.cuda.current_stream(device))
+    with torch.cuda.stream(st):
+        enqueue(upload=True)
+    torch.cuda.current_stream(device).wait_stream(st)
+    torch.cuda.synchronize(device)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        enqueue(upload=False)
+    for dst, src in zip(keep, snap):
+        dst.copy_(src)
+    return graph
 
 
 def box_filter(masks, classes, depth, inst_dict, intrinsic_open3d, T_CW, min_pixels=500, voxel_size=0.01):
