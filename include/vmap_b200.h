@@ -695,6 +695,27 @@ enum { VMB_TRACK_ST_CLAMP = 16 };
 int vmb_track_step_lw(vmb_handle* h, const vmb_track_args* a, int group, const void* image, void* stream);
 int vmb_ba_step_lw(vmb_handle* h, const vmb_ba_args* a, int group, const void* image, void* stream);
 
+/* ---- joint map-and-pose step on the layer-wise path (iMAP: network weights and keyframe poses together; the rule is
+ * in csrc/k_track_lw.cuh) ---------------------------------------------------------------------------------------------
+ * One mapping iteration that also yields K11's per-ray pose rows, from ONE forward and backward:
+ *   vmb_joint_step_lw  per object: world points p = R_f q + t_f (fp32 from an fp32 copy of the fp64 pose of the frame of
+ *                      the ray's draw, as K11) from the camera-frame samples s->pcs, then vmb_step's layer-wise step on p
+ *                      (mask counts, forward, render, loss, weight gradients accumulated into s->grads, loss_terms,
+ *                      loss_sum and the optional rendered outputs), then the pose terms of every point from that step's
+ *                      own embedding gradient and one row per ray into a->group[group].ray_rows (K11's layout; the loss
+ *                      columns are 0: the iteration's loss is the mapping loss in loss_terms / loss_sum).
+ * The caller then runs vmb_adam on the weights (the pose terms read the PE directions before it) and vmb_ba_update on
+ * the same vmb_ba_args (one Adam + Exp over the window).  `s`: as vmb_step, with fuse_adam = 0, backward = 1, grads and
+ * the fp16 image set, impl AUTO or LAYERWISE.  `a`: the pose table (poses, n_poses), status, and in group `group` the
+ * draw layout, keyframe tables and ray rows of the same objects, rays and samples (its other fields are not read here).
+ * pcs_world_out: optional [B][R][S][3] copy of the world points.  VMB_E_UNSUPPORTED for hidden 32; VMB_E_ARG as vmb_step
+ * and vmb_ba_step, and for a group that does not match `s`.  On the device: a ray whose draw's frame is outside its table
+ * is mapped at p = q, contributes nothing to the rows and sets VMB_BA_ST_BAD_FRAME.  No floating-point atomics on the
+ * pose side: the rows are bitwise reproducible for a given embedding gradient.
+ * Registers (ptxas -v, sm_90a), no spills: k_joint_world 32; k_tlw_pose and k_tlw_reduce as listed in k_track_lw.cuh. */
+int vmb_joint_step_lw(vmb_handle* h, const vmb_step_args* s, const vmb_ba_args* a, int group, float* pcs_world_out,
+                      void* stream);
+
 /* ---- bring-up / test hook (not part of the reference-facing surface) --------------------------- */
 /* Generic wgmma GEMM of the layer-wise wide-model path: D[M][N] = A[M][K1+K2] * B[N][K]^T, fp16 in,
  * fp32 accumulate.  a_mn/b_mn = 0: operand stored [rows][ld] with K contiguous; 1: stored [K][ld] with

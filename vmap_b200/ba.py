@@ -26,6 +26,111 @@ from .track import _rays_dir, _Slices, _step, _use_lw
 from .utils import capture_graph
 
 
+def fill_kf_frame(objs, store, kf_frame: np.ndarray, bg: bool = False) -> None:
+    """``kf_frame`` [B, KF] on the host: the frame id of each keyframe index of each object (-1: none), from the
+    shared-store objects' held slots or, for the ``do_bg`` background (``bg``), its own keyframe copies."""
+    kf_frame[:] = -1
+    for b, o in enumerate(objs):
+        if bg:
+            for f, j in o.kf_id_dict.items():
+                kf_frame[b, j] = int(f)
+        else:
+            for j in range(kf_frame.shape[1]):
+                if o._held[j]:
+                    kf_frame[b, j] = int(store.frame_id[o.kf_store_slot[j]])
+
+
+class PoseTables:
+    """The int32 tables of a window of keyframe poses, in one pinned host buffer and its device twin: ``kf_frame(k)``
+    [B_k, KF_k] of every group ``shapes[k] = (B_k, KF_k)``, the ``window`` (the distinct frame ids those hold without
+    ``hold``, padded with -1 to ``max_win``), ``frame_of`` (the frame id of every store slot) and, with ``bg_kf``, the
+    frame id of each of the ``do_bg`` background's keyframe copies.  Shared by ``BundleAdjuster`` and the joint mode of
+    ``FrameLoop``."""
+
+    def __init__(self, device, shapes: Sequence[Tuple[int, int]], max_win: int, bg_kf: int = 0):
+        self.device, self.shapes, self.max_win, self.bg_kf = device, list(shapes), max_win, bg_kf
+        self.cap = None
+        self.window: List[int] = []
+
+    def layout(self, store) -> bool:
+        """Size the buffers for the store's capacity; True when they were (re)allocated."""
+        cap = store.capacity
+        if self.cap == cap:
+            return False
+        sizes = [b * kf for b, kf in self.shapes] + [self.max_win, cap] + ([self.bg_kf] if self.bg_kf else [])
+        n = sum(sizes)
+        self._host = torch.zeros(n, dtype=torch.int32)
+        if torch.cuda.is_available():
+            self._host = self._host.pin_memory()
+        self._dev = torch.zeros(n, dtype=torch.int32, device=self.device)
+        self._views, o = [], 0
+        for s in sizes:
+            self._views.append((o, s))
+            o += s
+        self.cap = cap
+        self._uploaded = None
+        return True
+
+    def _h(self, k):
+        o, s = self._views[k]
+        return self._host[o:o + s]
+
+    def _d(self, k):
+        o, s = self._views[k]
+        return self._dev[o:o + s]
+
+    def kf_frame(self, k: int) -> torch.Tensor:
+        return self._d(k)
+
+    @property
+    def window_dev(self) -> torch.Tensor:
+        return self._d(len(self.shapes))
+
+    @property
+    def frame_of(self) -> torch.Tensor:
+        return self._d(len(self.shapes) + 1)
+
+    @property
+    def bg_frame_of(self) -> torch.Tensor:
+        return self._d(len(self.shapes) + 2)
+
+    def prepare(self, store, fills, hold: int = 0, bg_group: Optional[int] = None) -> List[int]:
+        """Fill every table on the host: ``fills[k](kf_frame)`` writes group k's [B_k, KF_k] table; the window and
+        ``frame_of`` follow from them and the store; ``bg_group``: the group whose first row the background's table
+        copies.  Returns the window (possibly empty).  Call ``layout`` first."""
+        if self._uploaded is not None:
+            self._uploaded.synchronize()       # the pinned buffer may still be the source of the last upload
+        frames = set()
+        for k, (b, kf) in enumerate(self.shapes):
+            t = self._h(k).numpy().reshape(b, kf)
+            fills[k](t)
+            frames.update(int(f) for f in t.reshape(-1) if f >= 0)
+        win = sorted(f for f in frames if f != hold)
+        if len(win) > self.max_win:
+            raise _lib.VmbError(f"pose window: {len(win)} frames exceed the window of {self.max_win}")
+        ng = len(self.shapes)
+        w = self._h(ng).numpy()
+        w[:] = -1
+        w[:len(win)] = win
+        fo = self._h(ng + 1).numpy()
+        fo[:] = -1
+        for s, f in store.frame_id.items():
+            if f is not None:
+                fo[s] = int(f)
+        if bg_group is not None:
+            b, kf = self.shapes[bg_group]
+            self._h(ng + 2).numpy()[:] = self._h(bg_group).numpy().reshape(b, kf)[0]
+        self.window = win
+        return win
+
+    def upload(self) -> None:
+        self._dev.copy_(self._host, non_blocking=True)
+        if not torch.cuda.is_current_stream_capturing():
+            if self._uploaded is None:
+                self._uploaded = torch.cuda.Event()
+            self._uploaded.record(torch.cuda.current_stream(self.device))
+
+
 class _BaGroup(_Slices):
     """One ensemble's share of a pass: the shared-store objects of the mapping stack, or the ``do_bg`` background with
     its own keyframe copies.  Rows are those ``obj_ids`` names; ``kf_frame`` is the device table of their keyframes'
@@ -60,19 +165,12 @@ class _BaGroup(_Slices):
     def fill(self, objects: Dict[int, object], store, kf_frame: np.ndarray) -> None:
         """The sampler tables and ``kf_frame`` [B, KF] (frame id of each keyframe index, -1: none) on the host."""
         objs = [objects[self.ids[r]] for r in self.rows]
-        kf_frame[:] = -1
         if self.bg:
             self.tables.fill_objects([o.keyframe_set() for o in objs])
-            for b, o in enumerate(objs):
-                for f, j in o.kf_id_dict.items():
-                    kf_frame[b, j] = int(f)
         else:
             from .vmap import keyframe_tables
             self.tables.fill_store(keyframe_tables(objs))
-            for b, o in enumerate(objs):
-                for j in range(self.KF):
-                    if o._held[j]:
-                        kf_frame[b, j] = int(store.frame_id[o.kf_store_slot[j]])
+        fill_kf_frame(objs, store, kf_frame, self.bg)
 
     def sample(self, store, rays_dir, seed: int, counter) -> None:
         kw = dict(out=self.out, offset_dev=counter, camera_frame=True, kf_out=self.kf_out)
@@ -129,79 +227,31 @@ class BundleAdjuster:
         self.grad_hist = torch.zeros(n_iter, self.max_win, 6, **f64) if record else None
         self.counter = torch.zeros(1, dtype=torch.int64, device=dev)       # sampler draw counter, +1 per pass
         self.window: List[int] = []
-        self._cap = None
+        bg = [g for g in self.groups if g.bg]
+        self.pose_tables = PoseTables(dev, [(len(g.rows), g.KF) for g in self.groups], self.max_win,
+                                      bg[0].KF if bg else 0)
         self.graph: Optional[torch.cuda.CUDAGraph] = None
 
-    # ---- the per-pass tables: one pinned int32 buffer and its device twin -------------------------------------------
+    # ---- the per-pass tables (PoseTables) ----------------------------------------------------------------------------
     def _layout(self, store) -> None:
-        cap = store.capacity
-        if self._cap == cap:
-            return
-        self.graph = None                      # a captured pass points at the old buffers
-        sizes = [len(g.rows) * g.KF for g in self.groups] + [self.max_win, cap]
-        bg = [g for g in self.groups if g.bg]
-        if bg:
-            sizes.append(bg[0].KF)
-        n = sum(sizes)
-        self._host = torch.zeros(n, dtype=torch.int32)
-        if torch.cuda.is_available():
-            self._host = self._host.pin_memory()
-        self._dev = torch.zeros(n, dtype=torch.int32, device=self.device)
-        self._views, o = [], 0
-        for s in sizes:
-            self._views.append((o, s))
-            o += s
-        self._cap = cap
-        self._uploaded = None
-        for k, g in enumerate(self.groups):
-            g.kf_frame = self._d(k)
-
-    def _h(self, k):
-        o, s = self._views[k]
-        return self._host[o:o + s]
-
-    def _d(self, k):
-        o, s = self._views[k]
-        return self._dev[o:o + s]
+        if self.pose_tables.layout(store):
+            self.graph = None                  # a captured pass points at the old buffers
+            for k, g in enumerate(self.groups):
+                g.kf_frame = self.pose_tables.kf_frame(k)
 
     def prepare(self, store, objects: Dict[int, object]) -> List[int]:
         """Fill every table of the next pass on the host from the objects' keyframe tables; returns the window (the
         distinct frame ids those tables hold, without ``hold``), which may be empty."""
         self._layout(store)
-        if self._uploaded is not None:
-            self._uploaded.synchronize()       # the pinned buffer may still be the source of the last upload
-        frames = set()
-        for k, g in enumerate(self.groups):
-            t = self._h(k).numpy().reshape(len(g.rows), g.KF)
-            g.fill(objects, store, t)
-            frames.update(int(f) for f in t.reshape(-1) if f >= 0)
-        win = sorted(f for f in frames if f != self.hold)
-        if len(win) > self.max_win:
-            raise _lib.VmbError(f"BundleAdjuster: {len(win)} frames exceed the window of {self.max_win}")
-        ng = len(self.groups)
-        w = self._h(ng).numpy()
-        w[:] = -1
-        w[:len(win)] = win
-        fo = self._h(ng + 1).numpy()
-        fo[:] = -1
-        for s, f in store.frame_id.items():
-            if f is not None:
-                fo[s] = int(f)
-        bg = [(k, g) for k, g in enumerate(self.groups) if g.bg]
-        if bg:
-            k, g = bg[0]
-            self._h(ng + 2).numpy()[:] = self._h(k).numpy().reshape(len(g.rows), g.KF)[0]
-        self.window = win
-        return win
+        bg = [k for k, g in enumerate(self.groups) if g.bg]
+        fills = [lambda t, g=g: g.fill(objects, store, t) for g in self.groups]
+        self.window = self.pose_tables.prepare(store, fills, self.hold, bg[0] if bg else None)
+        return self.window
 
     def _upload(self) -> None:
-        self._dev.copy_(self._host, non_blocking=True)
+        self.pose_tables.upload()
         for g in self.groups:
             g.tables.upload()
-        if not torch.cuda.is_current_stream_capturing():
-            if self._uploaded is None:
-                self._uploaded = torch.cuda.Event()
-            self._uploaded.record(torch.cuda.current_stream(self.device))
 
     # ---- the pass ----------------------------------------------------------------------------------------------------
     def _enqueue(self, store, poses: torch.Tensor, objects: Dict[int, object], upload: bool = True) -> None:
@@ -210,12 +260,12 @@ class BundleAdjuster:
         for gi, g in enumerate(self.groups):
             g.sample(store, self.rays_dir, self.seed + 0x9e3779b9 * gi, self.counter)
         self.counter += 1
-        ng = len(self.groups)
-        targets = [(self._d(ng + 1), store.t_wc, store.capacity)]
+        pt = self.pose_tables
+        targets = [(pt.frame_of, store.t_wc, store.capacity)]
         bg = [g for g in self.groups if g.bg]
         if bg:
-            targets.append((self._d(ng + 2), objects[bg[0].ids[bg[0].rows[0]]].t_wc_batch, bg[0].KF))
-        a = _iterate(self.groups, self.n_iter, poses, self._d(ng), self.max_win,
+            targets.append((pt.bg_frame_of, objects[bg[0].ids[bg[0].rows[0]]].t_wc_batch, bg[0].KF))
+        a = _iterate(self.groups, self.n_iter, poses, pt.window_dev, self.max_win,
                      self.hold, self.adam, self.scratch, self.lr_rot, self.lr_trans, self.losses, self.status,
                      self.pose_hist, self.grad_hist, targets)
         self._args = a
@@ -254,6 +304,28 @@ class BundleAdjuster:
 def _iterate(groups, n_iter, poses, window, n_win, hold, adam, scratch, lr_rot, lr_trans, losses, status,
              pose_hist=None, grad_hist=None, targets=()):
     """n_iter x [vmb_ba_step per group -> vmb_ba_update] on the groups' sample buffers."""
+    a = ba_args(groups, n_iter, poses, window, n_win, hold, adam, scratch, lr_rot, lr_trans, losses, status,
+                pose_hist, grad_hist, targets)
+    e0 = groups[0].ens
+    for it in range(n_iter):
+        a.iter = it + 1
+        for gi, g in enumerate(groups):
+            g.bind(a.group[gi], it)
+        for gi, g in enumerate(groups):
+            _step(g, a, gi, ba=True)
+        ba_update(e0, a)
+    return a
+
+
+def ba_update(ens: VmapEnsemble, a) -> None:
+    """vmb_ba_update: one Adam + Exp over the window from the rows the iteration's steps wrote."""
+    with ens._on_device():
+        _lib.check(ens._handle, ens.lib.vmb_ba_update(ens._handle, C.byref(a), _stream()), "vmb_ba_update")
+
+
+def ba_args(groups, n_iter, poses, window, n_win, hold, adam, scratch, lr_rot, lr_trans, losses, status,
+            pose_hist=None, grad_hist=None, targets=()):
+    """The vmb_ba_args of a pass over ``groups`` (each group's slice is bound per iteration by ``g.bind``)."""
     a = _lib.BaArgs()
     a.n_groups, a.n_iter = len(groups), n_iter
     a.poses, a.n_poses = _ptr(poses), poses.shape[0]
@@ -266,14 +338,6 @@ def _iterate(groups, n_iter, poses, window, n_win, hold, adam, scratch, lr_rot, 
     a.pose_hist, a.grad_hist = _ptr(pose_hist), _ptr(grad_hist)
     for t, (frame_of, t_wc, n) in enumerate(targets):
         a.target[t].frame_of, a.target[t].t_wc, a.target[t].n = _ptr(frame_of), _ptr(t_wc), n
-    for it in range(n_iter):
-        a.iter = it + 1
-        for gi, g in enumerate(groups):
-            g.bind(a.group[gi], it)
-        for gi, g in enumerate(groups):
-            _step(g, a, gi, ba=True)
-        with e0._on_device():
-            _lib.check(e0._handle, e0.lib.vmb_ba_update(e0._handle, C.byref(a), _stream()), "vmb_ba_update")
     return a
 
 

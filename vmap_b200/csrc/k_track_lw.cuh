@@ -31,7 +31,7 @@
 // No floating-point atomics anywhere on this path (the GEMM epilogues used here store): bitwise reproducible.
 // Registers (ptxas -v, sm_90a; track / BA flavour), no spills in any of them:
 //   k_tlw_gather 32; k_tlw_pe 74 / 74; k_tlw_render H 64: 67 / 68, H 128: 67 / 68, H 256: 67 / 68;
-//   k_tlw_pose 62 / 62; k_tlw_reduce 40 / 40.
+//   k_tlw_pose 62 / 62; k_tlw_reduce 40 / 40; the joint step's k_joint_world 32 (it runs k_tlw_pose / k_tlw_reduce<true>).
 #pragma once
 #include "k_layerwise.cuh"
 #include "k_track.cuh"
@@ -338,6 +338,7 @@ __global__ void __launch_bounds__(128) k_tlw_pose(TlwObj o, const float* __restr
 }
 
 // ---- 5: fixed-order fp64 sums into K10's partial rows (track) or K11's per-ray rows (BA) -----------------------------
+// lossr NULL (the joint step): the loss columns are written as 0
 template <bool BA>
 __global__ void __launch_bounds__(128) k_tlw_reduce(TlwObj o, int nr, int n_out, const int* __restrict__ ctl,
                                                     const double* __restrict__ gpt, const double* __restrict__ lossr,
@@ -355,9 +356,10 @@ __global__ void __launch_bounds__(128) k_tlw_reduce(TlwObj o, int nr, int n_out,
     for (long long p = (long long)r0 * o.S; p < pe; ++p)
 #pragma unroll
       for (int c = 0; c < 6; ++c) s[c] += gpt[p * 6 + c];
-    for (int r = r0; r < r1; ++r)
+    if (lossr)
+      for (int r = r0; r < r1; ++r)
 #pragma unroll
-      for (int c = 0; c < 3; ++c) s[6 + c] += lossr[(size_t)r * 3 + c];
+        for (int c = 0; c < 3; ++c) s[6 + c] += lossr[(size_t)r * 3 + c];
   }
 #pragma unroll
   for (int c = 0; c < 9; ++c) dst[c] = s[c];
@@ -446,6 +448,114 @@ static int launch_track_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGrou
       case 128: rc = track_object_lw<128, BA>(tw, L, G, b, st, err); break;
       case 256: rc = track_object_lw<256, BA>(tw, L, G, b, st, err); break;
       default: err = "layer-wise tracking: hidden must be 64, 128 or 256"; return -4;
+    }
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Joint map-and-pose step (vmb_joint_step_lw): the layer-wise MAPPING step fed from camera-frame samples, with K11's
+// per-ray rows taken from that step's own backward.  Per object b, in order on `st`:
+//   k_joint_world  p = pose_point(T_f, q, 1) per point, f = the frame of the ray's draw (ba_draw_frame); k_lw_pe's
+//                  t = p / scale is then bit-identical to the t that k_tlw_pose recomputes.  A ray whose frame is outside
+//                  its table keeps p = q (identity pose), gets zero rows and sets VMB_BA_ST_BAD_FRAME.  Writes ctl (row
+//                  ok = 1, scale[b]) for the pose kernels.
+//   step_object    the training step on p, unchanged (forward, render, loss, weight-gradient GEMMs, dE); no AdamW here,
+//                  because the pose terms read the PE directions from the fp32 param row and must see them before the update.
+//   k_tlw_pose / k_tlw_reduce (BA flavour) on the training workspace's dE: one row per ray, loss columns 0.
+// ---------------------------------------------------------------------------------------------------------------------
+struct JointWorkspace {        // grow-only, never moved once a captured graph holds it (as TrackWorkspace)
+  float* pw = nullptr;         // [P][3] world points of the current object
+  int* ctl = nullptr;          // [8] as TrackWorkspace::ctl (only row ok and scale are read)
+  double* gpt = nullptr;       // [P][6] per-point pose terms
+  long long cap_points = 0;
+  bool in_graph = false;
+  void release() {
+    void* ptrs[] = {pw, ctl, gpt};
+    for (void* q : ptrs) if (q) cudaFree(q);
+    pw = nullptr; ctl = nullptr; gpt = nullptr; cap_points = 0; in_graph = false;
+  }
+  cudaError_t ensure(long long P, cudaStream_t st) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    cudaStreamIsCapturing(st, &cs);
+    const bool capturing = cs != cudaStreamCaptureStatusNone;
+    if (P <= cap_points) { in_graph |= capturing; return cudaSuccess; }
+    if (capturing || in_graph) return cudaErrorStreamCaptureUnsupported;
+    release();
+    const long long Pp = (P + 127) / 128 * 128;
+    cudaError_t e = cudaSuccess;
+    auto al = [&](void** q, size_t bytes) { if (e == cudaSuccess) e = cudaMalloc(q, bytes); };
+    al((void**)&pw, (size_t)Pp * 3 * sizeof(float));
+    al((void**)&ctl, 8 * sizeof(int));
+    al((void**)&gpt, (size_t)Pp * 6 * sizeof(double));
+    if (e != cudaSuccess) { release(); return e; }
+    cap_points = Pp;
+    return cudaSuccess;
+  }
+};
+
+__global__ void __launch_bounds__(256) k_joint_world(TlwObj o, const float* __restrict__ scale, float* __restrict__ pw,
+                                                     float* __restrict__ pw_out, int* __restrict__ ctl) {
+  ptx::pdl_wait();
+  ptx::pdl_launch_dependents();
+  const long long P = (long long)o.R * o.S;
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p == 0) { ctl[3] = 1; ctl[4] = __float_as_int(scale[o.b]); }
+  if (p >= P) return;
+  const int f = tlw_frame<true>(o, (int)(p / o.S));
+  const float3 q = make_float3(o.pcs[p * 3], o.pcs[p * 3 + 1], o.pcs[p * 3 + 2]);
+  const float3 w = f >= 0 ? pose_point(o.pose + (size_t)f * 16, q, 1.0f) : q;
+  if (f < 0 && p % o.S == 0 && o.status) atomicOr(o.status, VMB_BA_ST_BAD_FRAME);
+  pw[p * 3] = w.x; pw[p * 3 + 1] = w.y; pw[p * 3 + 2] = w.z;
+  if (pw_out) { pw_out[p * 3] = w.x; pw_out[p * 3 + 1] = w.y; pw_out[p * 3 + 2] = w.z; }
+}
+
+// sp: the mapping step's arguments (pcs = camera-frame points); x: the per-draw pose tables and the output rows
+template <int H>
+static int joint_object_lw(Workspace& ws, JointWorkspace& jw, const VmbLayout& L, const StepParams& sp, const BaRays& x,
+                           const double* poses, int* status, const __half* image, int b, float* pw_out, cudaStream_t st,
+                           std::string& err) {
+  const long long np = (long long)sp.R * sp.S;
+  TlwObj o;
+  memset(&o, 0, sizeof(o));
+  o.b = b; o.R = sp.R; o.S = sp.S; o.n_rows = sp.B; o.pcs = sp.pcs + (size_t)b * sp.pcs_stride; o.pose = poses; o.status = status;
+  o.n_pix_draw = x.n_pix_draw; o.n_poses = x.n_poses; o.kf_stride = x.kf_stride;
+  o.kf_draw = x.kf_draw + (size_t)b * x.kf_draw_stride;
+  o.kf_frame = x.kf_frame + (size_t)b * x.kf_stride;
+  TLW_TRY(launch_k(k_joint_world, dim3((unsigned)((np + 255) / 256)), dim3(256), 0, st, o, sp.scale, jw.pw,
+                   pw_out ? pw_out + (size_t)b * np * 3 : nullptr, jw.ctl));
+  StepParams s1 = sp;
+  s1.pcs = jw.pw; s1.pcs_stride = 0;                // step_object reads object b's points at pcs + b * pcs_stride
+  const int rc = step_object<H>(ws, L, s1, image, b, st, err);
+  if (rc) return rc;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  TLW_TRY(pose_smem_limit<k_tlw_pose<true>>(dev, PEB_SMEM));
+  // after step_object's join with its side stream: an ordinary launch
+  TLW_TRY(launch_k(k_tlw_pose<true>, dim3((unsigned)((np + 127) / 128)), dim3(128), (size_t)PEB_SMEM, st, o,
+                   sp.params + (size_t)b * L.stride, (const int*)jw.ctl, L.o_B, (const float*)ws.dE, jw.gpt));
+  if (np <= 65536) pdl_arm();                       // step_object's rule
+  TLW_TRY(launch_k(k_tlw_reduce<true>, dim3((sp.R + 127) / 128), dim3(128), 0, st, o, 1, sp.R, (const int*)jw.ctl,
+                   (const double*)jw.gpt, (const double*)nullptr, x.rows + (size_t)b * sp.R * VMB_TRACK_PART));
+  TLW_TRY(cudaGetLastError());
+  return 0;
+}
+
+static int launch_joint_lw(Workspace& ws, JointWorkspace& jw, const VmbLayout& L, const StepParams& sp, const BaRays& x,
+                           const double* poses, int* status, const void* image, float* pw_out, cudaStream_t st,
+                           std::string& err) {
+  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return -2; }
+  const long long np = (long long)sp.R * sp.S;
+  TLW_TRY(ws.ensure(np, L.H, st));
+  TLW_TRY(jw.ensure(np, st));
+  for (int b = 0; b < sp.B; ++b) {
+    int rc;
+    switch (L.H) {
+      case 64:  rc = joint_object_lw<64>(ws, jw, L, sp, x, poses, status, (const __half*)image, b, pw_out, st, err); break;
+      case 128: rc = joint_object_lw<128>(ws, jw, L, sp, x, poses, status, (const __half*)image, b, pw_out, st, err); break;
+      case 256: rc = joint_object_lw<256>(ws, jw, L, sp, x, poses, status, (const __half*)image, b, pw_out, st, err); break;
+      default: err = "joint step: hidden must be 64, 128 or 256"; return -4;
     }
     if (rc) return rc;
   }

@@ -50,6 +50,7 @@ struct vmb_handle {
   render::Workspace ws_render;// view rendering: source table, entry sort / scan scratch (grow-only)
   lw::TrackWorkspace ws_track;// layer-wise tracking step: its own, so a tracking capture never pins the mapping step's
   lw::TrackWorkspace ws_ba;   // layer-wise bundle-adjustment step: likewise (and tracking never moves a BA capture's)
+  lw::JointWorkspace ws_joint;// joint map-and-pose step: world points and pose terms (the activations are the step's ws)
   std::string err;
 };
 
@@ -184,6 +185,7 @@ void vmb_destroy(vmb_handle* h) {
   h->ws_render.release();
   h->ws_track.release();
   h->ws_ba.release();
+  h->ws_joint.release();
   delete h;
 }
 
@@ -289,21 +291,16 @@ static int launch_adamw(vmb_handle* h, int n_obj, float* params, float* grads, f
   return VMB_OK;
 }
 
-int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
-  if (!h || !a) return fail(h, VMB_E_ARG, "vmb_step: null argument");
+// the argument checks of vmb_step (and of vmb_joint_step_lw, which takes the same struct) and the step's parameters
+static int step_params(vmb_handle* h, const vmb_step_args* a, StepParams& sp, const std::string& who) {
+  if (!h || !a) return fail(h, VMB_E_ARG, who + ": null argument");
   if (a->n_obj <= 0 || a->n_obj > h->max_obj || a->n_rays <= 0 || a->n_samples <= 0 || a->n_samples > 32)
-    return fail(h, VMB_E_ARG, "vmb_step: bad n_obj / n_rays / n_samples (1 <= S <= 32)");
+    return fail(h, VMB_E_ARG, who + ": bad n_obj / n_rays / n_samples (1 <= S <= 32)");
   if (!a->pcs || !a->z_vals || !a->gt_depth || !a->gt_colour || !a->sem || !a->mask_depth || !a->params ||
       !a->scale || !a->loss_terms || (a->backward && !a->grads && !a->fuse_adam))
-    return fail(h, VMB_E_ARG, "vmb_step: missing tensor pointer");
+    return fail(h, VMB_E_ARG, who + ": missing tensor pointer");
   if (a->fuse_adam && (!a->backward || !a->exp_avg || !a->exp_avg_sq || (a->step < 1 && !a->step_counter)))
-    return fail(h, VMB_E_ARG, "vmb_step: fuse_adam needs backward = 1, exp_avg / exp_avg_sq and a step number");
-  cudaStream_t st = (cudaStream_t)stream;
-  int impl = a->impl;
-  const bool umma_possible = h->umma_ok && a->image != nullptr;
-  const bool lw_possible = h->lw_ok && a->image != nullptr;
-  if (impl == VMB_IMPL_AUTO) impl = umma_possible ? VMB_IMPL_UMMA : (lw_possible ? VMB_IMPL_LAYERWISE : VMB_IMPL_FP32);
-  StepParams sp;
+    return fail(h, VMB_E_ARG, who + ": fuse_adam needs backward = 1, exp_avg / exp_avg_sq and a step number");
   memset(&sp, 0, sizeof(sp));
   sp.B = a->n_obj; sp.R = a->n_rays; sp.S = a->n_samples;
   sp.pcs = a->pcs; sp.pcs_stride = a->pcs_stride;
@@ -315,6 +312,33 @@ int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
   sp.params = a->params; sp.scale = a->scale; sp.grads = a->grads; sp.loss_terms = a->loss_terms;
   sp.r_depth = a->r_depth; sp.r_var = a->r_var; sp.r_colour = a->r_colour; sp.r_opacity = a->r_opacity;
   sp.cs = a->colour_scaling; sp.os = a->opacity_scaling; sp.backward = a->backward;
+  return VMB_OK;
+}
+
+// K0 of the non-fused paths: the mask counts (computed here unless the caller passes them) and zeroed loss terms
+static int step_counts(vmb_handle* h, const vmb_step_args* a, StepParams& sp, cudaStream_t st) {
+  const int* counts = a->counts;
+  if (!counts) {
+    k_mask_counts<<<a->n_obj, 256, 0, st>>>(a->n_rays, a->sem, a->sem_stride, a->mask_depth, a->mask_stride,
+                                            h->d_counts, a->loss_terms);
+    CUDA_TRY(h, cudaGetLastError());
+    counts = h->d_counts;
+  } else {
+    CUDA_TRY(h, cudaMemsetAsync(a->loss_terms, 0, sizeof(float) * 4 * a->n_obj, st));
+  }
+  sp.counts = counts;
+  return VMB_OK;
+}
+
+int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
+  StepParams sp;
+  const int rc0 = step_params(h, a, sp, "vmb_step");
+  if (rc0 != VMB_OK) return rc0;
+  cudaStream_t st = (cudaStream_t)stream;
+  int impl = a->impl;
+  const bool umma_possible = h->umma_ok && a->image != nullptr;
+  const bool lw_possible = h->lw_ok && a->image != nullptr;
+  if (impl == VMB_IMPL_AUTO) impl = umma_possible ? VMB_IMPL_UMMA : (lw_possible ? VMB_IMPL_LAYERWISE : VMB_IMPL_FP32);
   AdamScalars q;
   memset(&q, 0, sizeof(q));
   if (a->fuse_adam) q = adam_scalars(a->lr, a->beta1, a->beta2, a->weight_decay, a->step);
@@ -356,16 +380,8 @@ int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
   }
 
   // ---- other paths: K0 (mask counts) -> K1 -> [K2] ---------------------------------------------------------------
-  const int* counts = a->counts;
-  if (!counts) {
-    k_mask_counts<<<a->n_obj, 256, 0, st>>>(a->n_rays, a->sem, a->sem_stride, a->mask_depth, a->mask_stride,
-                                            h->d_counts, a->loss_terms);
-    CUDA_TRY(h, cudaGetLastError());
-    counts = h->d_counts;
-  } else {
-    CUDA_TRY(h, cudaMemsetAsync(a->loss_terms, 0, sizeof(float) * 4 * a->n_obj, st));
-  }
-  sp.counts = counts;
+  const int rcc = step_counts(h, a, sp, st);
+  if (rcc != VMB_OK) return rcc;
   if (a->backward && !a->grads) return fail(h, VMB_E_ARG, "vmb_step: this path needs the grads block");
   int rc = VMB_OK;
   {
@@ -1395,6 +1411,39 @@ int vmb_ba_update(vmb_handle* h, const vmb_ba_args* a, void* stream) {
   u.loss = a->loss; u.pose_hist = a->pose_hist; u.grad_hist = a->grad_hist; u.status = a->status;
   k_ba_update<<<1, 256, 0, (cudaStream_t)stream>>>(u);
   CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
+int vmb_joint_step_lw(vmb_handle* h, const vmb_step_args* s, const vmb_ba_args* a, int group, float* pcs_world_out,
+                      void* stream) {
+  const char* who = "vmb_joint_step_lw";
+  StepParams sp;
+  const int rc0 = step_params(h, s, sp, who);
+  if (rc0 != VMB_OK) return rc0;
+  if (!h->lw_ok)
+    return fail(h, VMB_E_UNSUPPORTED, "vmb_joint_step_lw: layer-wise path only (hidden 64/128/256, n_freq 6); hidden 32 has "
+                                      "no pose gradient from its mapping step");
+  if (!s->image || !s->grads || !s->backward || s->fuse_adam || (s->impl != VMB_IMPL_AUTO && s->impl != VMB_IMPL_LAYERWISE))
+    return fail(h, VMB_E_ARG, "vmb_joint_step_lw: needs an image, grads, backward = 1, fuse_adam = 0 and the layer-wise impl");
+  const int rc1 = pose_args_ok(h, a, who);
+  if (rc1 != VMB_OK) return rc1;
+  if (group < 0 || group >= a->n_groups) return fail(h, VMB_E_ARG, "vmb_joint_step_lw: group index outside [0, n_groups)");
+  const vmb_ba_group& g = a->group[group];
+  if (g.hidden != h->H || ba_group_ok(g) != VMB_OK || g.n_obj != s->n_obj || g.n_rays != s->n_rays ||
+      g.n_samples != s->n_samples)
+    return fail(h, VMB_E_ARG, "vmb_joint_step_lw: the pose group must describe the step's objects, rays and samples "
+                              "(draw layout, keyframe tables, ray rows)");
+  BaRays x;
+  memset(&x, 0, sizeof(x));
+  x.kf_draw = g.kf_draw; x.kf_draw_stride = g.kf_draw_stride; x.kf_frame = g.kf_frame; x.kf_stride = g.kf_stride;
+  x.n_pix_draw = g.n_pix_draw; x.n_poses = a->n_poses; x.rows = g.ray_rows;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int rcc = step_counts(h, s, sp, st);
+  if (rcc != VMB_OK) return rcc;
+  std::string err;
+  const int rc = lw::launch_joint_lw(h->ws, h->ws_joint, h->L, sp, x, a->poses, a->status, s->image, pcs_world_out, st, err);
+  if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, std::string(who) + ": " + err);
+  if (s->loss_sum) { k_loss_sum<<<1, 32, 0, st>>>(s->loss_terms, s->n_obj, s->loss_sum); CUDA_TRY(h, cudaGetLastError()); }
   return VMB_OK;
 }
 

@@ -238,6 +238,22 @@ class VmapEnsemble:
         self.step_count += 1
         return loss_out.view(-1)[0]
 
+    def joint_step(self, batch, ba_args, group: int = 0, loss_out: Optional[torch.Tensor] = None, outputs=None,
+                   pcs_world_out: Optional[torch.Tensor] = None) -> None:
+        """The step of one joint map-and-pose iteration (``vmb_joint_step_lw``, hidden 64/128/256): ``batch["pcs"]``
+        holds camera-frame points, moved to the world by the pose of each ray's draw (``ba_args``: the fp64 pose table
+        and, in ``group``, the draw layout, keyframe tables and ray rows); the layer-wise step on those points
+        accumulates into ``self.grads`` and overwrites ``self.loss_terms`` (``loss_out`` / ``outputs`` as in
+        ``step`` / ``render``), and the step's own embedding gradient gives the per-ray pose rows.  No optimiser update:
+        ``adam_step`` and ``vmb_ba_update`` follow.  ``pcs_world_out``: [B,R,S,3] float32 copy of the world points."""
+        a = self._step_args(batch, True, outputs, "layerwise", loss_out=loss_out)
+        if pcs_world_out is not None:
+            assert pcs_world_out.shape == batch["pcs"].shape and pcs_world_out.is_contiguous()
+            assert pcs_world_out.dtype == torch.float32 and pcs_world_out.device == self.device
+        with self._on_device():
+            _lib.check(self._handle, self.lib.vmb_joint_step_lw(self._handle, C.byref(a), C.byref(ba_args), group,
+                                                                _ptr(pcs_world_out), _stream()), "vmb_joint_step_lw")
+
     def capture_step(self, batch, impl: Optional[str] = None) -> "torch.cuda.CUDAGraph":
         """Capture the step (one launch at hidden 32) on ``batch``'s (fixed) buffers into a CUDA graph; refill the buffers
         and ``replay()`` for every step.  Removes the per-launch host overhead of the loop."""

@@ -11,6 +11,15 @@ enqueued right before the replay (outside the graph, so the pinned source buffer
 the host can fill the next frame's tables as soon as that copy -- not the whole frame -- has completed).  What changes between frames lives in device memory (Adam
 step counter, sampler draw counter) or in the pinned table buffer (keyframe slots / boxes / counts), so a replay
 draws fresh samples and continues the optimiser exactly as the eager loop would.
+
+Joint mode (``joint=JointPoses(...)``, iMAP, hidden 64/128/256): the keyframe poses are optimised with the weights.  The
+sampler draws the same Philox samples in the camera frame and records each draw's keyframe; per iteration
+
+    vmb_joint_step_lw (world points from each draw's pose, the mapping step, per-ray pose rows from its embedding
+      gradient) -> vmb_adam (weights) -> vmb_ba_update (one Adam + Exp over the window of keyframe poses)
+
+and after the last iteration the refined poses go in fp32 to the store's slots.  Frame 0 (the anchor) never moves; the
+pose Adam moments restart with every frame, as a bundle-adjustment pass's do.
 """
 from __future__ import annotations
 
@@ -18,6 +27,8 @@ from typing import List, Optional, Sequence
 
 import torch
 
+from . import _lib
+from .ba import PoseTables, _BaGroup, ba_args, ba_update, fill_kf_frame
 from .ensemble import VmapEnsemble
 from .sampler import BatchedSampler, KeyframeSet, KeyframeTables, SamplerTables
 from .utils import capture_graph
@@ -35,14 +46,38 @@ class Background:
         self.out = sampler._outputs(1, n_frames * n_pix, sampler.n1 + sampler.n2, False)
 
 
+class JointPoses:
+    """The opt-in joint mode of ``FrameLoop``: ``poses`` is the fp64 pose table [F, 4, 4] (row = frame id) whose keyframe
+    rows every mapping iteration moves with the weights, at rates ``lr_rot`` / ``lr_trans``; ``hold`` (the anchor frame)
+    never moves."""
+
+    def __init__(self, poses: torch.Tensor, lr_rot: float, lr_trans: float, hold: int = 0):
+        assert poses.dtype == torch.float64 and poses.dim() == 3 and poses.shape[1:] == (4, 4) and poses.is_contiguous()
+        self.poses, self.lr_rot, self.lr_trans, self.hold = poses, lr_rot, lr_trans, hold
+
+
+class _JointGroup(_BaGroup):
+    """The mapping stack as the one group of the joint step: FrameLoop's sample buffers, bound per iteration the way a
+    bundle-adjustment group is (``_BaGroup.bind``): ``n_pix`` rays of ``win`` draws of ``n_pix_draw`` pixels."""
+
+    def __init__(self, ens: VmapEnsemble, out, kf_out: torch.Tensor, n_pix: int, n_pix_draw: int, KF: int):
+        self.ens, self.out, self.kf_out, self.lw = ens, out, kf_out, True
+        self.n_pix, self.n_pix_draw, self.S, self.KF = n_pix, n_pix_draw, out["pcs"].shape[2], KF
+        self.win, self.n_draws = n_pix // n_pix_draw, kf_out.shape[1]
+        self.rows_dev = torch.arange(ens.n_obj, dtype=torch.int32, device=ens.device)
+        self._alloc_rows(ens.n_obj)
+
+
 class FrameLoop:
     def __init__(self, ens: VmapEnsemble, sampler: BatchedSampler, n_frames: int, n_pix: int, n_iter: int,
                  rays_dir: torch.Tensor, store=None, kf_stride: int = 0, seed: int = 0, first_offset: int = 0,
-                 background: Optional[Background] = None):
+                 background: Optional[Background] = None, joint: Optional[JointPoses] = None):
         """``n_frames * n_pix`` rays are drawn per object per frame and consumed in ``n_iter`` slices
         (train.py:198,270-277).  ``store``/``kf_stride``: shared keyframe store mode (keyframes.FrameStore).
         ``background``: the ``do_bg`` model, sampled and stepped inside the same graph; its loss is added to the
-        iteration's loss as train.py:308-316 does (`batch_loss += bg_loss`)."""
+        iteration's loss as train.py:308-316 does (`batch_loss += bg_loss`).  ``joint``: optimise the keyframe poses
+        with the weights (see the module docstring); needs the store, a layer-wise ensemble, no background and whole
+        draws per iteration.  Its tables come from ``set_joint_tables``."""
         assert (n_frames * n_pix) % n_iter == 0, "rays per frame must split evenly over the iterations"
         self.ens, self.smp, self.store = ens, sampler, store
         self.bg = background
@@ -59,6 +94,20 @@ class FrameLoop:
         self.counter = torch.full((1,), first_offset, dtype=torch.int64, device=dev)     # sampler draw counter
         self.losses = torch.zeros(n_iter, dtype=torch.float32, device=dev)
         self.graph: Optional[torch.cuda.CUDAGraph] = None
+        self.joint = joint
+        if joint is not None:
+            if store is None or background is not None or ens.hidden == 32 or ens.image is None:
+                raise ValueError("FrameLoop: joint poses need the frame store, a hidden-64/128/256 ensemble and no "
+                                 "background model")
+            assert n_frames % n_iter == 0, "joint poses: every iteration takes whole draws"
+            self.kf_out = torch.zeros(B, n_frames, dtype=torch.int32, device=dev)
+            self.jg = _JointGroup(ens, self.out, self.kf_out, n_frames * n_pix // n_iter, n_pix, kf_stride)
+            self.max_win = min(_lib.BA_MAX_WIN, B * kf_stride)
+            self.pose_tables = PoseTables(dev, [(B, kf_stride)], self.max_win)
+            f64 = dict(dtype=torch.float64, device=dev)
+            self.pose_adam = torch.zeros(self.max_win, 12, **f64)
+            self.pose_scratch = torch.zeros(8 * B * self.jg.win + 6 * self.max_win, **f64)
+            self.pose_status = torch.zeros(4, dtype=torch.int32, device=dev)
 
     # ---- per-frame host work: only the small tables ------------------------------------------------------
     def set_objects(self, sets: Sequence[KeyframeSet]) -> None:
@@ -69,6 +118,15 @@ class FrameLoop:
 
     def set_background(self, kf: KeyframeSet) -> None:
         self.bg.tables.fill_objects([kf])
+
+    def set_joint_tables(self, objects) -> List[int]:
+        """Joint mode: the frame id of every keyframe of ``objects`` (the stack's sceneObjects, row order) and the
+        window of poses this frame moves; returns the window.  A store that grew since the capture drops the graph."""
+        pt = self.pose_tables
+        if pt.layout(self.store):
+            self.graph = None                       # the captured frame points at the old tables
+            self.jg.kf_frame = pt.kf_frame(0)
+        return pt.prepare(self.store, [lambda t: fill_kf_frame(list(objects), self.store, t)], self.joint.hold)
 
     # ---- the frame -----------------------------------------------------------------------------------------
     def _enqueue(self, upload: bool = True) -> None:
@@ -82,6 +140,14 @@ class FrameLoop:
             bg.smp.sample(None, bg.n_frames, bg.n_pix, self.rays_dir, seed=self.seed + 0x5bd1e995,
                           tables=bg.tables, out=bg.out, offset_dev=self.counter)
             Rb = bg.n_frames * bg.n_pix // self.n_iter
+        if self.joint is not None:
+            if upload:
+                self.pose_tables.upload()
+            s.sample_store(self.store, self.tables, self.n_frames, self.n_pix, self.rays_dir, seed=self.seed,
+                           out=self.out, offset_dev=self.counter, camera_frame=True, kf_out=self.kf_out)
+            self.counter += 1
+            self._joint_iterations(R)
+            return
         if self.store is not None:
             s.sample_store(self.store, self.tables, self.n_frames, self.n_pix, self.rays_dir, seed=self.seed,
                            out=self.out, offset_dev=self.counter)
@@ -93,6 +159,19 @@ class FrameLoop:
             self.ens.step({k: v[:, it * R:(it + 1) * R] for k, v in self.out.items()}, loss_out=self.losses[it:it + 1])
             if bg is not None:  # train.py:308-316
                 self.losses[it] += bg.ens.step({k: v[:, it * Rb:(it + 1) * Rb] for k, v in bg.out.items()})
+
+    def _joint_iterations(self, R: int) -> None:
+        j, pt, g = self.joint, self.pose_tables, self.jg
+        a = ba_args([g], self.n_iter, j.poses, pt.window_dev, self.max_win, j.hold, self.pose_adam,
+                    self.pose_scratch, j.lr_rot, j.lr_trans, None, self.pose_status,
+                    targets=[(pt.frame_of, self.store.t_wc, self.store.capacity)])
+        for it in range(self.n_iter):
+            a.iter = it + 1
+            g.bind(a.group[0], it)
+            self.ens.joint_step({k: v[:, it * R:(it + 1) * R] for k, v in self.out.items()}, a, 0,
+                                loss_out=self.losses[it:it + 1])
+            self.ens.adam_step()
+            ba_update(self.ens, a)
 
     def run_eager(self) -> torch.Tensor:
         """The same frame without a graph (reference for tests / first frames)."""
@@ -106,6 +185,8 @@ class FrameLoop:
         all_ens = [self.ens] + ([self.bg.ens] if self.bg is not None else [])
         keep = [t for e in all_ens for t in (e.params, e.grads, e.exp_avg, e.exp_avg_sq, e.step_counter)]
         keep += [e.image for e in all_ens if e.image is not None] + [self.counter]
+        if self.joint is not None:
+            keep += [self.joint.poses, self.store.t_wc]
         counts = [e.step_count for e in all_ens]
         self.graph = capture_graph(self.ens.device, self._enqueue, keep)
         for e, cn in zip(all_ens, counts):
@@ -117,6 +198,8 @@ class FrameLoop:
             self.capture()
         self.ens.poll_status()            # raises LossExplode if an earlier frame tripped the device guard
         self.tables.upload()
+        if self.joint is not None:
+            self.pose_tables.upload()
         if self.bg is not None:
             self.bg.ens.poll_status()
             self.bg.tables.upload()

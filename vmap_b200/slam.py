@@ -38,6 +38,13 @@ whole-scene network, an object of the stack as mapping builds it (``hidden_featu
 its box from the ingest.  ``track_impl`` / ``ba_impl`` choose the step of the tracker and the bundle adjuster:
 ``"layerwise"`` (the tensor-core path for hidden 64/128/256, the default in iMAP mode) or ``"fp32"`` (K10 / K11, the
 default otherwise).
+
+With ``joint_poses`` (iMAP mode only) every mapping iteration also moves the keyframe poses, as iMAP optimises its
+network and keyframe poses together: the mapping frame runs ``FrameLoop``'s joint mode (``vmb_joint_step_lw``: the pose
+rows come from the mapping step's own backward, no second forward), one Adam + Exp over the window of every keyframe the
+model holds per iteration (never frame 0, the anchor), and the refined poses go to ``poses`` and the store, where the
+motion model, ``get_bound``, meshing and bundle adjustment read them.  The pose Adam moments restart with every mapping
+frame, as a bundle-adjustment pass's do.  vMAP mode is refused: its hidden-32 fused step has no pose gradient.
 """
 from __future__ import annotations
 
@@ -47,7 +54,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .frame import Background, FrameLoop
+from .frame import Background, FrameLoop, JointPoses
 from .keyframes import FrameStore
 from .ba import BundleAdjuster
 from .sampler import BatchedSampler
@@ -88,14 +95,22 @@ class Slam:
     ``ba_every``: run a bundle-adjustment pass after the mapping frame of every ``ba_every``-th frame (0: never);
     ``n_ba_iter`` / ``ba_lr_rot`` / ``ba_lr_trans``: its iterations and rates (default ``cfg.pose_lr``).
     ``track_impl`` / ``ba_impl``: ``"fp32"`` or ``"layerwise"`` (see the module docstring; None: ``"layerwise"`` in iMAP
-    mode, ``"fp32"`` otherwise)."""
+    mode, ``"fp32"`` otherwise).  ``joint_poses``: optimise the keyframe poses with the map in every mapping iteration
+    (iMAP mode only, see the module docstring); ``joint_lr_rot`` / ``joint_lr_trans``: its rates (default
+    ``cfg.pose_lr``)."""
 
     def __init__(self, cfg, T_init=None, track: bool = True, map: bool = True, groups=None, graph: bool = True,
                  n_track_iter: int = 20, lr_rot: Optional[float] = None, lr_trans: Optional[float] = None,
                  seed: int = 0, max_frames: int = 100000, background_cls: Sequence[int] = (), bbox_scale: float = 0.2,
                  store_capacity: Optional[int] = None, max_id: int = 4096, timing: bool = False, ba_every: int = 0,
                  n_ba_iter: int = 20, ba_lr_rot: Optional[float] = None, ba_lr_trans: Optional[float] = None,
-                 track_impl: Optional[str] = None, ba_impl: Optional[str] = None):
+                 track_impl: Optional[str] = None, ba_impl: Optional[str] = None, joint_poses: bool = False,
+                 joint_lr_rot: Optional[float] = None, joint_lr_trans: Optional[float] = None):
+        if joint_poses and not cfg.imap_mode:
+            raise ValueError("Slam: joint_poses needs iMAP mode (cfg.imap_mode): the vMAP objects' hidden-32 fused step "
+                             "has no pose gradient")
+        if joint_poses and not map:
+            raise ValueError("Slam: joint_poses refines the keyframe poses of a map being built: map=True")
         if not track and not map:
             raise ValueError("Slam: nothing to do with track=False and map=False")
         if ba_every < 0 or n_ba_iter < 1:
@@ -132,6 +147,8 @@ class Slam:
         self.timing, self.events = timing, []
         # bundle adjustment (off: nothing is allocated or launched)
         self.ba_every = ba_every
+        self.joint = JointPoses(self.poses, cfg.pose_lr if joint_lr_rot is None else joint_lr_rot,
+                                cfg.pose_lr if joint_lr_trans is None else joint_lr_trans) if joint_poses else None
         self.ba_kw = dict(n_iter=n_ba_iter, lr_rot=ba_lr_rot, lr_trans=ba_lr_trans, seed=seed + _BA_SEED,
                           impl=ba_impl or default_impl)
         self.ba: Optional[BundleAdjuster] = None
@@ -305,6 +322,8 @@ class Slam:
         if new:
             self._restack()
         self.loop.set_store_tables(keyframe_tables(list(self.objects.values())))
+        if self.joint is not None:
+            self.loop.set_joint_tables(self.objects.values())
         if self.loop.bg is not None:
             self.loop.set_background(self.scene_bg.keyframe_set())
         self._mark()
@@ -341,7 +360,7 @@ class Slam:
         old = self.loop
         self.loop = FrameLoop(self.ens, self.obj_sampler, cfg.n_iter_per_frame * cfg.win_size,
                               cfg.n_samples_per_frame, cfg.n_iter_per_frame, self.rays_dir, store=self.store,
-                              kf_stride=cfg.keyframe_buffer_size, seed=self.seed, background=bg)
+                              kf_stride=cfg.keyframe_buffer_size, seed=self.seed, background=bg, joint=self.joint)
         if old is not None:
             self.loop.counter.copy_(old.counter)          # the sampler's draw counter runs on across re-stacks
         if self.do_track:
@@ -383,7 +402,7 @@ class Slam:
             self._ba_seen, mode = True, "eager"
         else:
             mode = "replay"
-            if ba.graph is None or ba._cap != self.store.capacity:
+            if ba.graph is None or ba.pose_tables.cap != self.store.capacity:
                 ba.capture(self.store, self.poses, objs)
                 mode = "capture"
             win = ba.replay(self.store, self.poses, objs)
