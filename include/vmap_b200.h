@@ -716,6 +716,23 @@ int vmb_ba_step_lw(vmb_handle* h, const vmb_ba_args* a, int group, const void* i
 int vmb_joint_step_lw(vmb_handle* h, const vmb_step_args* s, const vmb_ba_args* a, int group, float* pcs_world_out,
                       void* stream);
 
+/* ---- joint map-and-pose step on the fused hidden-32 step (vMAP: the objects' weights and keyframe poses together; the
+ * rule is in csrc/k_step_fused.cuh and csrc/k_track_lw.cuh) ------------------------------------------------------------
+ *   vmb_joint_step_fused  world points of all B objects in one launch (k_joint_world, as vmb_joint_step_lw), then vmb_step's
+ *                      fused hidden-32 step on them (mask counts, forward, render, loss, backward, the ordered gradient
+ *                      reduction and, with fuse_adam = 1, AdamW), whose PE backward also forms every point's dL/dt from
+ *                      the pre-update directions, then one row per ray into a->group[group].ray_rows (K11's layout, loss
+ *                      columns 0).  The caller then runs vmb_ba_update.
+ * `s`: as vmb_step at hidden 32, with the image, backward = 1, impl AUTO or UMMA, fuse_adam 0 (gradients added into
+ * s->grads) or 1.  `a`, `group` and pcs_world_out as vmb_joint_step_lw.  VMB_E_UNSUPPORTED for hidden 64/128/256 (they
+ * take vmb_joint_step_lw); VMB_E_ARG as vmb_joint_step_lw.  The rows are the gradient of the mapping loss, so its
+ * whole-batch empty-mask rule applies (a term is off for every object when one object's count of it is 0).  No
+ * floating-point atomics on the pose side: the rows are bitwise reproducible.
+ * Registers (ptxas -v, sm_90a), no spills: k_joint_world 32, k_joint_rows 68; k_step_fused JOINT as listed in
+ * k_step_fused.cuh. */
+int vmb_joint_step_fused(vmb_handle* h, const vmb_step_args* s, const vmb_ba_args* a, int group, float* pcs_world_out,
+                         void* stream);
+
 /* ---- bring-up / test hook (not part of the reference-facing surface) --------------------------- */
 /* Generic wgmma GEMM of the layer-wise wide-model path: D[M][N] = A[M][K1+K2] * B[N][K]^T, fp16 in,
  * fp32 accumulate.  a_mn/b_mn = 0: operand stored [rows][ld] with K contiguous; 1: stored [K][ld] with

@@ -172,9 +172,16 @@ __device__ __forceinline__ int cta_of_pair(const Ranges& rg, int G, int pair) { 
 }  // namespace uf
 
 // ---------------------------------------------------------------------------------------------------------------
-template <int SC>
+// JOINT (the joint map-and-pose step, vmb_joint_step_fused): the PE backward also forms each point's pose gradient
+// dL/dt = INV_LS (dE_xyz + sum_d dproj_d B_d) in fp32 from the same cosines and the same pre-update directions Bd as the
+// dB wgrad (the rule of k_tlw_pose).  Each warpgroup sums its own directions (hsel 0: dE_xyz, then 0..11; hsel 1:
+// 12..20) and stores its half to jdt[b][point][hsel][3] (fp32, plain stores); k_joint_rows adds the halves in that
+// order.  jdt is read only under JOINT: the plain instantiations compile to the same SASS as without it.
+// Registers (ptxas -v, sm_90a), no spills: JOINT S = any / 10 / 14: 248 / 248 / 248 (plain: 245 / 248 / 248).
+template <int SC, bool JOINT>
 __global__ void __launch_bounds__(uf::NT, 1)
-k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image, const __grid_constant__ uf::Ranges rg, int tpo, int npo, int nr, int rpw) {
+k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image, const __grid_constant__ uf::Ranges rg, int tpo, int npo, int nr, int rpw,
+             float* jdt) {
   using namespace uf;
   extern __shared__ __align__(1024) unsigned char smem[];
   Misc* misc = reinterpret_cast<Misc*>(smem + SM_MISC);
@@ -716,6 +723,13 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       // ---- PE backward: dproj_d = pi * sum_k 2^k g_{k,d} cos(pi 2^k proj_d), written as an fp16 block --------------
       {
         const int q0 = hsel ? 3 : 0, q1 = hsel ? 5 : 3;
+        float jt0 = 0.f, jt1 = 0.f, jt2 = 0.f;         // JOINT: this half's dL/dt
+        if constexpr (JOINT) {
+          if (!hsel) {                                  // emb1 cols 1..3 = d/d[x y z]
+            const float4 e0 = *reinterpret_cast<const float4*>(eg + p * 16);
+            jt0 = e0.y * INV_LS; jt1 = e0.z * INV_LS; jt2 = e0.w * INV_LS;
+          }
+        }
         uint64_t c01, c23;
         {
           uint64_t pj01, pj23;
@@ -747,6 +761,11 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
             d = fmaf(16.f * g2[dd * 2], cv[dd][4], d);
             d = fmaf(32.f * g2[dd * 2 + 1], cv[dd][5], d);
             dp[dd] = d * VMB_PI_F;
+            if constexpr (JOINT) {
+              const int dir = 4 * q + dd;
+              const float g = dp[dd] * INV_LS;
+              jt0 = fmaf(g, Bd[dir], jt0); jt1 = fmaf(g, Bd[um::DIRS_PITCH + dir], jt1); jt2 = fmaf(g, Bd[2 * um::DIRS_PITCH + dir], jt2);
+            }
           }
           // directions 4q..4q+3 = columns (4q)%8.. of feature group q/2
           *reinterpret_cast<uint2*>(act + (FG_DPR + (q >> 1)) * FGB + p * 16 + (q & 1) * 8) =
@@ -761,6 +780,16 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
           d = fmaf(2.f * g1[5], c[1], d); d = fmaf(4.f * g1[6], c[2], d); d = fmaf(8.f * g1[7], c[3], d);
           d = fmaf(16.f * g2[0], c[4], d); d = fmaf(32.f * g2[1], c[5], d);
           *reinterpret_cast<uint2*>(act + (FG_DPR + 2) * FGB + p * 16 + 8) = make_uint2(um::pack_h2(d * VMB_PI_F, 0.f), 0u);
+          if constexpr (JOINT) {
+            const float g = (d * VMB_PI_F) * INV_LS;
+            jt0 = fmaf(g, Bd[20], jt0); jt1 = fmaf(g, Bd[um::DIRS_PITCH + 20], jt1); jt2 = fmaf(g, Bd[2 * um::DIRS_PITCH + 20], jt2);
+          }
+        }
+        if constexpr (JOINT) {
+          if (live) {
+            float* o = jdt + (((size_t)b * R + ray) * S + sidx) * 6 + 3 * hsel;
+            o[0] = jt0; o[1] = jt1; o[2] = jt2;
+          }
         }
       }
       // dB += dproj^T [1 x y z ...]: the 21 real feature rows are in the first warpgroup's half; the second issues the
@@ -924,20 +953,23 @@ static void fused_partition(int B, int npo, int G, uf::Ranges& rg) {
   while (c < G) rg.begin[++c] = (int)T;
 }
 
+// jdt: the joint step's [B][R * S][2][3] pose-gradient halves (JOINT instantiations), or nullptr (the plain step)
 static int fused_launch_step(const VmbLayout& L, const StepParams& sp, const FusedExtra& fx, const void* image, int n_sm,
-                             cudaStream_t st, std::string& err) {
+                             cudaStream_t st, std::string& err, float* jdt = nullptr) {
   using namespace uf;
   if (L.H != 32 || L.nfreq != 6) { err = "fused step kernel: hidden must be 32 and n_freq 6"; return -4; }
   if (sp.S < 1 || sp.S > 32) { err = "fused step kernel: n_samples must be in [1, 32]"; return -4; }
   if (!sp.fwd_only && sp.B > MAX_OBJ_SMEM) { err = "fused step kernel: too many objects for the in-kernel mask counts"; return -4; }
+  if (jdt && (sp.fwd_only || !sp.backward)) { err = "fused step kernel: the joint step needs the backward"; return -4; }
   static bool attr_set[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   const int smem_bytes = SM_CNT + (sp.fwd_only ? 0 : sp.B * 12) + 16;
   if (!attr_set[dev & 63]) {
-    cudaError_t e = cudaFuncSetAttribute(k_step_fused<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_step_fused<10>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_step_fused<14>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
+    cudaError_t e = cudaSuccess;
+    for (auto k : {k_step_fused<0, false>, k_step_fused<10, false>, k_step_fused<14, false>,
+                   k_step_fused<0, true>, k_step_fused<10, true>, k_step_fused<14, true>})
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
     if (e != cudaSuccess) { err = std::string("cudaFuncSetAttribute(k_step_fused): ") + cudaGetErrorString(e); return -2; }
     attr_set[dev & 63] = true;
   }
@@ -964,9 +996,9 @@ static int fused_launch_step(const VmbLayout& L, const StepParams& sp, const Fus
   attr[0].val.cooperative = sp.fwd_only ? 0 : 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
   cudaError_t e;
-  if (sp.S == 10)      e = cudaLaunchKernelEx(&cfg, k_step_fused<10>, sp, fx, L, img, rg, tpo, npo, nr, rpw);
-  else if (sp.S == 14) e = cudaLaunchKernelEx(&cfg, k_step_fused<14>, sp, fx, L, img, rg, tpo, npo, nr, rpw);
-  else                 e = cudaLaunchKernelEx(&cfg, k_step_fused<0>, sp, fx, L, img, rg, tpo, npo, nr, rpw);
+  auto kern = [&](auto k) { return cudaLaunchKernelEx(&cfg, k, sp, fx, L, img, rg, tpo, npo, nr, rpw, jdt); };
+  if (jdt) e = kern(sp.S == 10 ? k_step_fused<10, true> : sp.S == 14 ? k_step_fused<14, true> : k_step_fused<0, true>);
+  else     e = kern(sp.S == 10 ? k_step_fused<10, false> : sp.S == 14 ? k_step_fused<14, false> : k_step_fused<0, false>);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { err = std::string("k_step_fused launch: ") + cudaGetErrorString(e); return -2; }
   return 0;

@@ -466,15 +466,16 @@ static int launch_track_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGrou
 //   k_tlw_pose / k_tlw_reduce (BA flavour) on the training workspace's dE: one row per ray, loss columns 0.
 // ---------------------------------------------------------------------------------------------------------------------
 struct JointWorkspace {        // grow-only, never moved once a captured graph holds it (as TrackWorkspace)
-  float* pw = nullptr;         // [P][3] world points of the current object
+  float* pw = nullptr;         // [P][3] world points of the current object (fused step: of all B objects)
   int* ctl = nullptr;          // [8] as TrackWorkspace::ctl (only row ok and scale are read)
-  double* gpt = nullptr;       // [P][6] per-point pose terms
+  double* gpt = nullptr;       // [P][6] per-point pose terms (layer-wise step)
+  float* jdt = nullptr;        // [P][2][3] the fused step's per-point dL/dt halves
   long long cap_points = 0;
   bool in_graph = false;
   void release() {
-    void* ptrs[] = {pw, ctl, gpt};
+    void* ptrs[] = {pw, ctl, gpt, jdt};
     for (void* q : ptrs) if (q) cudaFree(q);
-    pw = nullptr; ctl = nullptr; gpt = nullptr; cap_points = 0; in_graph = false;
+    pw = nullptr; ctl = nullptr; gpt = nullptr; jdt = nullptr; cap_points = 0; in_graph = false;
   }
   cudaError_t ensure(long long P, cudaStream_t st) {
     cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
@@ -489,26 +490,74 @@ struct JointWorkspace {        // grow-only, never moved once a captured graph h
     al((void**)&pw, (size_t)Pp * 3 * sizeof(float));
     al((void**)&ctl, 8 * sizeof(int));
     al((void**)&gpt, (size_t)Pp * 6 * sizeof(double));
+    al((void**)&jdt, (size_t)Pp * 6 * sizeof(float));
     if (e != cudaSuccess) { release(); return e; }
     cap_points = Pp;
     return cudaSuccess;
   }
 };
 
-__global__ void __launch_bounds__(256) k_joint_world(TlwObj o, const float* __restrict__ scale, float* __restrict__ pw,
+// object o.b + blockIdx.y of a batched launch (the fused joint step: all B objects in one grid; the layer-wise step
+// launches one object with gridDim.y = 1): its slice of the samples and of the draw tables
+__device__ __forceinline__ TlwObj joint_obj(TlwObj o, long long pcs_stride, long long kf_draw_stride) {
+  const int y = blockIdx.y;
+  o.b += y; o.pcs += y * pcs_stride; o.kf_draw += y * kf_draw_stride; o.kf_frame += (size_t)y * o.kf_stride;
+  return o;
+}
+
+// pw / pw_out: [gridDim.y][P][3]; ctl (layer-wise step only) gets row ok = 1 and scale[o.b]
+__global__ void __launch_bounds__(256) k_joint_world(TlwObj o0, long long pcs_stride, long long kf_draw_stride,
+                                                     const float* __restrict__ scale, float* __restrict__ pw,
                                                      float* __restrict__ pw_out, int* __restrict__ ctl) {
   ptx::pdl_wait();
   ptx::pdl_launch_dependents();
+  const TlwObj o = joint_obj(o0, pcs_stride, kf_draw_stride);
   const long long P = (long long)o.R * o.S;
   const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p == 0) { ctl[3] = 1; ctl[4] = __float_as_int(scale[o.b]); }
+  if (p == 0 && ctl) { ctl[3] = 1; ctl[4] = __float_as_int(scale[o.b]); }
   if (p >= P) return;
+  pw += (size_t)blockIdx.y * P * 3;
+  if (pw_out) pw_out += (size_t)blockIdx.y * P * 3;
   const int f = tlw_frame<true>(o, (int)(p / o.S));
   const float3 q = make_float3(o.pcs[p * 3], o.pcs[p * 3 + 1], o.pcs[p * 3 + 2]);
   const float3 w = f >= 0 ? pose_point(o.pose + (size_t)f * 16, q, 1.0f) : q;
   if (f < 0 && p % o.S == 0 && o.status) atomicOr(o.status, VMB_BA_ST_BAD_FRAME);
   pw[p * 3] = w.x; pw[p * 3 + 1] = w.y; pw[p * 3 + 2] = w.z;
   if (pw_out) { pw_out[p * 3] = w.x; pw_out[p * 3 + 1] = w.y; pw_out[p * 3 + 2] = w.z; }
+}
+
+// The fused joint step's rows (vmb_joint_step_fused): one thread per ray of object blockIdx.y, its samples in order,
+// dL/dt = the two halves of jdt [B][R * S][2][3] added (hsel 0 + hsel 1), then pose_terms from the fp64 pose of the
+// draw's frame; K11's row layout with the loss columns and column 9 at 0.  A ray whose frame is outside its table gets a
+// zero row and sets VMB_BA_ST_BAD_FRAME.
+__global__ void __launch_bounds__(128) k_joint_rows(TlwObj o0, long long pcs_stride, long long kf_draw_stride,
+                                                    const float* __restrict__ scale, const float* __restrict__ jdt,
+                                                    double* __restrict__ rows) {
+  const TlwObj o = joint_obj(o0, pcs_stride, kf_draw_stride);
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= o.R) return;
+  const int f = tlw_frame<true>(o, r);
+  double s[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  if (f >= 0) {
+    const double* T = o.pose + (size_t)f * 16;
+    const float sc = scale[o.b];
+    const float* h = jdt + ((size_t)blockIdx.y * o.R + r) * o.S * 6;
+    for (int i = 0; i < o.S; ++i, h += 6) {
+      const long long p = (long long)r * o.S + i;
+      const float3 dt = make_float3(h[0] + h[3], h[1] + h[4], h[2] + h[5]);
+      double c6[6];
+      pose_terms(T, make_double3(o.pcs[p * 3], o.pcs[p * 3 + 1], o.pcs[p * 3 + 2]), dt, sc, c6);
+#pragma unroll
+      for (int c = 0; c < 6; ++c) s[c] += c6[c];
+    }
+  } else if (o.status) {
+    atomicOr(o.status, VMB_BA_ST_BAD_FRAME);
+  }
+  double* dst = rows + ((size_t)blockIdx.y * o.R + r) * VMB_TRACK_PART;
+#pragma unroll
+  for (int c = 0; c < 6; ++c) dst[c] = s[c];
+#pragma unroll
+  for (int c = 6; c < VMB_TRACK_PART; ++c) dst[c] = 0.0;
 }
 
 // sp: the mapping step's arguments (pcs = camera-frame points); x: the per-draw pose tables and the output rows
@@ -523,7 +572,7 @@ static int joint_object_lw(Workspace& ws, JointWorkspace& jw, const VmbLayout& L
   o.n_pix_draw = x.n_pix_draw; o.n_poses = x.n_poses; o.kf_stride = x.kf_stride;
   o.kf_draw = x.kf_draw + (size_t)b * x.kf_draw_stride;
   o.kf_frame = x.kf_frame + (size_t)b * x.kf_stride;
-  TLW_TRY(launch_k(k_joint_world, dim3((unsigned)((np + 255) / 256)), dim3(256), 0, st, o, sp.scale, jw.pw,
+  TLW_TRY(launch_k(k_joint_world, dim3((unsigned)((np + 255) / 256)), dim3(256), 0, st, o, 0LL, 0LL, sp.scale, jw.pw,
                    pw_out ? pw_out + (size_t)b * np * 3 : nullptr, jw.ctl));
   StepParams s1 = sp;
   s1.pcs = jw.pw; s1.pcs_stride = 0;                // step_object reads object b's points at pcs + b * pcs_stride

@@ -330,6 +330,32 @@ static int step_counts(vmb_handle* h, const vmb_step_args* a, StepParams& sp, cu
   return VMB_OK;
 }
 
+// the fused hidden-32 step's extra arguments (vmb_step and vmb_joint_step_fused): scratch, counts and the fused AdamW
+static int fused_extra(vmb_handle* h, const vmb_step_args* a, cudaStream_t st, FusedExtra& fx) {
+  const int rc0 = fused_scratch(h, st);
+  if (rc0 != VMB_OK) return rc0;
+  memset(&fx, 0, sizeof(fx));
+  fx.partials = h->d_partials; fx.finish_sync = h->d_finish_sync; fx.counts_in = a->counts; fx.counts_pub = h->d_counts;
+  fx.fuse_adam = a->fuse_adam ? 1 : 0;
+  if (a->fuse_adam) {
+    const AdamScalars q = adam_scalars(a->lr, a->beta1, a->beta2, a->weight_decay, a->step);
+    fx.p = const_cast<float*>(a->params); fx.m = a->exp_avg; fx.v = a->exp_avg_sq;
+    fx.image_out = (__half*)const_cast<void*>(a->image); fx.img_index = h->d_img_index; fx.img_halves = h->img_halves;
+    fx.step_counter = a->step_counter; fx.step_size = q.step_size; fx.bc2_sqrt = q.bc2_sqrt;
+    fx.lr = q.lr; fx.b1d = q.b1; fx.b2d = q.b2d;
+    fx.log_b1 = (float)std::log(q.b1); fx.log_b2 = (float)std::log(q.b2d);
+    if (a->step_counter) {
+      const int rcb = ensure_bc_table(h, q.b1, q.b2d, st);
+      if (rcb != VMB_OK) return rcb;
+      fx.bc_table = h->d_bc; fx.bc_n = BC_N;
+    }
+    fx.lr_wd = q.lr_wd; fx.one_m_b1 = q.one_m_b1; fx.b2 = q.b2; fx.one_m_b2 = q.one_m_b2; fx.eps = a->eps;
+    fx.guard_loss = a->guard_loss; fx.status = a->status;
+  }
+  fx.loss_sum = a->loss_sum;
+  return VMB_OK;
+}
+
 int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
   StepParams sp;
   const int rc0 = step_params(h, a, sp, "vmb_step");
@@ -339,9 +365,6 @@ int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
   const bool umma_possible = h->umma_ok && a->image != nullptr;
   const bool lw_possible = h->lw_ok && a->image != nullptr;
   if (impl == VMB_IMPL_AUTO) impl = umma_possible ? VMB_IMPL_UMMA : (lw_possible ? VMB_IMPL_LAYERWISE : VMB_IMPL_FP32);
-  AdamScalars q;
-  memset(&q, 0, sizeof(q));
-  if (a->fuse_adam) q = adam_scalars(a->lr, a->beta1, a->beta2, a->weight_decay, a->step);
   struct EvGuard {      // records the optional K1 timing events around whichever kernel runs
     cudaEvent_t stop; cudaStream_t st;
     ~EvGuard() { if (stop) cudaEventRecord(stop, st); }
@@ -350,30 +373,12 @@ int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
   // ---- hidden 32: ONE launch (counts + step + ordered gradient reduction (+ AdamW)) ----------------------------
   if (impl == VMB_IMPL_UMMA) {
     if (!umma_possible) return fail(h, VMB_E_UNSUPPORTED, "vmb_step: tensor-core path needs hidden=32, n_freq=6 and an image");
-    const int rc0 = fused_scratch(h, st);
-    if (rc0 != VMB_OK) return rc0;
     FusedExtra fx;
-    memset(&fx, 0, sizeof(fx));
-    fx.partials = h->d_partials; fx.finish_sync = h->d_finish_sync; fx.counts_in = a->counts; fx.counts_pub = h->d_counts;
-    fx.fuse_adam = a->fuse_adam ? 1 : 0;
-    if (a->fuse_adam) {
-      fx.p = const_cast<float*>(a->params); fx.m = a->exp_avg; fx.v = a->exp_avg_sq;
-      fx.image_out = (__half*)const_cast<void*>(a->image); fx.img_index = h->d_img_index; fx.img_halves = h->img_halves;
-      fx.step_counter = a->step_counter; fx.step_size = q.step_size; fx.bc2_sqrt = q.bc2_sqrt;
-      fx.lr = q.lr; fx.b1d = q.b1; fx.b2d = q.b2d;
-      fx.log_b1 = (float)std::log(q.b1); fx.log_b2 = (float)std::log(q.b2d);
-      if (a->step_counter) {
-        const int rcb = ensure_bc_table(h, q.b1, q.b2d, st);
-        if (rcb != VMB_OK) return rcb;
-        fx.bc_table = h->d_bc; fx.bc_n = BC_N;
-      }
-      fx.lr_wd = q.lr_wd; fx.one_m_b1 = q.one_m_b1; fx.b2 = q.b2; fx.one_m_b2 = q.one_m_b2; fx.eps = a->eps;
-      fx.guard_loss = a->guard_loss; fx.status = a->status;
-    }
+    const int rc0 = fused_extra(h, a, st, fx);
+    if (rc0 != VMB_OK) return rc0;
     EvGuard evg{(cudaEvent_t)a->k1_stop_event, st};
     if (a->k1_start_event) cudaEventRecord((cudaEvent_t)a->k1_start_event, st);
     std::string err;
-    fx.loss_sum = a->loss_sum;
     const int rc = fused_launch_step(h->L, sp, fx, a->image, h->n_sm, st, err);
     if (rc != VMB_OK) return fail(h, rc, err);
     return VMB_OK;
@@ -383,6 +388,9 @@ int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
   const int rcc = step_counts(h, a, sp, st);
   if (rcc != VMB_OK) return rcc;
   if (a->backward && !a->grads) return fail(h, VMB_E_ARG, "vmb_step: this path needs the grads block");
+  AdamScalars q;
+  memset(&q, 0, sizeof(q));
+  if (a->fuse_adam) q = adam_scalars(a->lr, a->beta1, a->beta2, a->weight_decay, a->step);
   int rc = VMB_OK;
   {
     EvGuard evg{(cudaEvent_t)a->k1_stop_event, st};
@@ -1414,6 +1422,22 @@ int vmb_ba_update(vmb_handle* h, const vmb_ba_args* a, void* stream) {
   return VMB_OK;
 }
 
+// the pose group of a joint step: it must describe the step's objects, rays and samples (both joint entry points)
+static int joint_group(vmb_handle* h, const vmb_step_args* s, const vmb_ba_args* a, int group, const char* who, BaRays& x) {
+  const int rc1 = pose_args_ok(h, a, who);
+  if (rc1 != VMB_OK) return rc1;
+  if (group < 0 || group >= a->n_groups) return fail(h, VMB_E_ARG, std::string(who) + ": group index outside [0, n_groups)");
+  const vmb_ba_group& g = a->group[group];
+  if (g.hidden != h->H || ba_group_ok(g) != VMB_OK || g.n_obj != s->n_obj || g.n_rays != s->n_rays ||
+      g.n_samples != s->n_samples)
+    return fail(h, VMB_E_ARG, std::string(who) + ": the pose group must describe the step's objects, rays and samples "
+                              "(draw layout, keyframe tables, ray rows)");
+  memset(&x, 0, sizeof(x));
+  x.kf_draw = g.kf_draw; x.kf_draw_stride = g.kf_draw_stride; x.kf_frame = g.kf_frame; x.kf_stride = g.kf_stride;
+  x.n_pix_draw = g.n_pix_draw; x.n_poses = a->n_poses; x.rows = g.ray_rows;
+  return VMB_OK;
+}
+
 int vmb_joint_step_lw(vmb_handle* h, const vmb_step_args* s, const vmb_ba_args* a, int group, float* pcs_world_out,
                       void* stream) {
   const char* who = "vmb_joint_step_lw";
@@ -1425,18 +1449,9 @@ int vmb_joint_step_lw(vmb_handle* h, const vmb_step_args* s, const vmb_ba_args* 
                                       "no pose gradient from its mapping step");
   if (!s->image || !s->grads || !s->backward || s->fuse_adam || (s->impl != VMB_IMPL_AUTO && s->impl != VMB_IMPL_LAYERWISE))
     return fail(h, VMB_E_ARG, "vmb_joint_step_lw: needs an image, grads, backward = 1, fuse_adam = 0 and the layer-wise impl");
-  const int rc1 = pose_args_ok(h, a, who);
-  if (rc1 != VMB_OK) return rc1;
-  if (group < 0 || group >= a->n_groups) return fail(h, VMB_E_ARG, "vmb_joint_step_lw: group index outside [0, n_groups)");
-  const vmb_ba_group& g = a->group[group];
-  if (g.hidden != h->H || ba_group_ok(g) != VMB_OK || g.n_obj != s->n_obj || g.n_rays != s->n_rays ||
-      g.n_samples != s->n_samples)
-    return fail(h, VMB_E_ARG, "vmb_joint_step_lw: the pose group must describe the step's objects, rays and samples "
-                              "(draw layout, keyframe tables, ray rows)");
   BaRays x;
-  memset(&x, 0, sizeof(x));
-  x.kf_draw = g.kf_draw; x.kf_draw_stride = g.kf_draw_stride; x.kf_frame = g.kf_frame; x.kf_stride = g.kf_stride;
-  x.n_pix_draw = g.n_pix_draw; x.n_poses = a->n_poses; x.rows = g.ray_rows;
+  const int rc1 = joint_group(h, s, a, group, who, x);
+  if (rc1 != VMB_OK) return rc1;
   cudaStream_t st = (cudaStream_t)stream;
   const int rcc = step_counts(h, s, sp, st);
   if (rcc != VMB_OK) return rcc;
@@ -1446,5 +1461,43 @@ int vmb_joint_step_lw(vmb_handle* h, const vmb_step_args* s, const vmb_ba_args* 
   if (s->loss_sum) { k_loss_sum<<<1, 32, 0, st>>>(s->loss_terms, s->n_obj, s->loss_sum); CUDA_TRY(h, cudaGetLastError()); }
   return VMB_OK;
 }
+
+int vmb_joint_step_fused(vmb_handle* h, const vmb_step_args* s, const vmb_ba_args* a, int group, float* pcs_world_out,
+                         void* stream) {
+  const char* who = "vmb_joint_step_fused";
+  StepParams sp;
+  const int rc0 = step_params(h, s, sp, who);
+  if (rc0 != VMB_OK) return rc0;
+  if (!h->umma_ok)
+    return fail(h, VMB_E_UNSUPPORTED, "vmb_joint_step_fused: the fused hidden-32 step only (hidden 32, n_freq 6); hidden "
+                                      "64/128/256 take vmb_joint_step_lw");
+  if (!s->image || !s->backward || (s->impl != VMB_IMPL_AUTO && s->impl != VMB_IMPL_UMMA))
+    return fail(h, VMB_E_ARG, "vmb_joint_step_fused: needs an image, backward = 1 and the fused (umma) impl");
+  BaRays x;
+  const int rc1 = joint_group(h, s, a, group, who, x);
+  if (rc1 != VMB_OK) return rc1;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long np = (long long)s->n_rays * s->n_samples;
+  CUDA_TRY(h, h->ws_joint.ensure(np * s->n_obj, st));
+  lw::TlwObj o;
+  memset(&o, 0, sizeof(o));
+  o.R = s->n_rays; o.S = s->n_samples; o.n_rows = s->n_obj; o.pcs = s->pcs; o.pose = a->poses; o.status = a->status;
+  o.n_pix_draw = x.n_pix_draw; o.n_poses = x.n_poses; o.kf_stride = x.kf_stride; o.kf_draw = x.kf_draw; o.kf_frame = x.kf_frame;
+  // world points of all B objects, then the fused step on them (pcs_stride: one dense [R][S][3] block per object)
+  CUDA_TRY(h, launch_k(lw::k_joint_world, dim3((unsigned)((np + 255) / 256), (unsigned)s->n_obj), dim3(256), 0, st, o,
+                       (long long)s->pcs_stride, (long long)x.kf_draw_stride, s->scale, h->ws_joint.pw, pcs_world_out,
+                       (int*)nullptr));
+  sp.pcs = h->ws_joint.pw; sp.pcs_stride = np * 3;
+  FusedExtra fx;
+  const int rc2 = fused_extra(h, s, st, fx);
+  if (rc2 != VMB_OK) return rc2;
+  std::string err;
+  const int rc = fused_launch_step(h->L, sp, fx, s->image, h->n_sm, st, err, h->ws_joint.jdt);
+  if (rc != VMB_OK) return fail(h, rc, std::string(who) + ": " + err);
+  CUDA_TRY(h, launch_k(lw::k_joint_rows, dim3((unsigned)((s->n_rays + 127) / 128), (unsigned)s->n_obj), dim3(128), 0, st, o,
+                       (long long)s->pcs_stride, (long long)x.kf_draw_stride, s->scale, (const float*)h->ws_joint.jdt, x.rows));
+  return VMB_OK;
+}
+
 
 }  // extern "C"

@@ -254,6 +254,24 @@ class VmapEnsemble:
             _lib.check(self._handle, self.lib.vmb_joint_step_lw(self._handle, C.byref(a), C.byref(ba_args), group,
                                                                 _ptr(pcs_world_out), _stream()), "vmb_joint_step_lw")
 
+    def joint_step_fused(self, batch, ba_args, group: int = 0, fuse_adam: bool = True,
+                         loss_out: Optional[torch.Tensor] = None, outputs=None,
+                         pcs_world_out: Optional[torch.Tensor] = None) -> None:
+        """The step of one joint map-and-pose iteration at hidden 32 (``vmb_joint_step_fused``): as ``joint_step``, on the
+        fused hidden-32 step, whose PE backward also gives every point's pose gradient.  ``fuse_adam`` (default): AdamW
+        runs inside the step, as ``step`` does (the pose terms read the directions before it); otherwise the gradients
+        accumulate into ``self.grads`` for ``adam_step``.  ``vmb_ba_update`` follows."""
+        a = self._step_args(batch, True, outputs, "umma", fuse_adam=fuse_adam, loss_out=loss_out)
+        if pcs_world_out is not None:
+            assert pcs_world_out.shape == batch["pcs"].shape and pcs_world_out.is_contiguous()
+            assert pcs_world_out.dtype == torch.float32 and pcs_world_out.device == self.device
+        with self._on_device():
+            _lib.check(self._handle, self.lib.vmb_joint_step_fused(self._handle, C.byref(a), C.byref(ba_args), group,
+                                                                   _ptr(pcs_world_out), _stream()),
+                       "vmb_joint_step_fused")
+        if fuse_adam:
+            self.step_count += 1
+
     def capture_step(self, batch, impl: Optional[str] = None) -> "torch.cuda.CUDAGraph":
         """Capture the step (one launch at hidden 32) on ``batch``'s (fixed) buffers into a CUDA graph; refill the buffers
         and ``replay()`` for every step.  Removes the per-launch host overhead of the loop."""

@@ -44,7 +44,10 @@ network and keyframe poses together: the mapping frame runs ``FrameLoop``'s join
 rows come from the mapping step's own backward, no second forward), one Adam + Exp over the window of every keyframe the
 model holds per iteration (never frame 0, the anchor), and the refined poses go to ``poses`` and the store, where the
 motion model, ``get_bound``, meshing and bundle adjustment read them.  The pose Adam moments restart with every mapping
-frame, as a bundle-adjustment pass's do.  vMAP mode is refused: its hidden-32 fused step has no pose gradient.
+frame, as a bundle-adjustment pass's do.  ``joint_impl`` chooses the joint step: ``"layerwise"`` (the default, iMAP
+mode) or ``"fused"`` (vMAP mode: ``vmb_joint_step_fused``, the objects' fused hidden-32 step with AdamW inside it, whose
+PE backward also gives the pose rows; with ``do_bg`` the background model's joint step is the update's second group and
+its keyframe copies receive the refined poses too).  In vMAP mode joint poses need ``joint_impl="fused"``.
 """
 from __future__ import annotations
 
@@ -96,8 +99,8 @@ class Slam:
     ``n_ba_iter`` / ``ba_lr_rot`` / ``ba_lr_trans``: its iterations and rates (default ``cfg.pose_lr``).
     ``track_impl`` / ``ba_impl``: ``"fp32"`` or ``"layerwise"`` (see the module docstring; None: ``"layerwise"`` in iMAP
     mode, ``"fp32"`` otherwise).  ``joint_poses``: optimise the keyframe poses with the map in every mapping iteration
-    (iMAP mode only, see the module docstring); ``joint_lr_rot`` / ``joint_lr_trans``: its rates (default
-    ``cfg.pose_lr``)."""
+    (see the module docstring); ``joint_lr_rot`` / ``joint_lr_trans``: its rates (default ``cfg.pose_lr``);
+    ``joint_impl``: ``None`` / ``"layerwise"`` (iMAP mode) or ``"fused"`` (vMAP mode)."""
 
     def __init__(self, cfg, T_init=None, track: bool = True, map: bool = True, groups=None, graph: bool = True,
                  n_track_iter: int = 20, lr_rot: Optional[float] = None, lr_trans: Optional[float] = None,
@@ -105,10 +108,15 @@ class Slam:
                  store_capacity: Optional[int] = None, max_id: int = 4096, timing: bool = False, ba_every: int = 0,
                  n_ba_iter: int = 20, ba_lr_rot: Optional[float] = None, ba_lr_trans: Optional[float] = None,
                  track_impl: Optional[str] = None, ba_impl: Optional[str] = None, joint_poses: bool = False,
-                 joint_lr_rot: Optional[float] = None, joint_lr_trans: Optional[float] = None):
-        if joint_poses and not cfg.imap_mode:
-            raise ValueError("Slam: joint_poses needs iMAP mode (cfg.imap_mode): the vMAP objects' hidden-32 fused step "
-                             "has no pose gradient")
+                 joint_lr_rot: Optional[float] = None, joint_lr_trans: Optional[float] = None,
+                 joint_impl: Optional[str] = None):
+        if joint_impl not in (None, "layerwise", "fused"):
+            raise ValueError(f"Slam: joint_impl must be None, 'layerwise' or 'fused', not {joint_impl!r}")
+        if joint_impl == "fused" and cfg.imap_mode:
+            raise ValueError("Slam: joint_impl='fused' is the vMAP objects' hidden-32 step; iMAP mode takes 'layerwise'")
+        if joint_poses and not cfg.imap_mode and joint_impl != "fused":
+            raise ValueError("Slam: joint_poses in vMAP mode needs joint_impl=\"fused\": the layer-wise joint step "
+                             "runs the iMAP model, the vMAP objects' hidden-32 step is the fused one")
         if joint_poses and not map:
             raise ValueError("Slam: joint_poses refines the keyframe poses of a map being built: map=True")
         if not track and not map:
@@ -323,7 +331,7 @@ class Slam:
             self._restack()
         self.loop.set_store_tables(keyframe_tables(list(self.objects.values())))
         if self.joint is not None:
-            self.loop.set_joint_tables(self.objects.values())
+            self.loop.set_joint_tables(self.objects.values(), self.scene_bg)
         if self.loop.bg is not None:
             self.loop.set_background(self.scene_bg.keyframe_set())
         self._mark()
