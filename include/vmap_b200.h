@@ -267,6 +267,23 @@ typedef struct vmb_ingest_args {
 
 int vmb_ingest_frame(vmb_handle* h, const vmb_ingest_args* a, void* stream);
 
+/* ScanNet relabel of a stored frame: the association's output (K7, vmb_assoc_finalize) replaces what the ingest wrote.
+ * One launch, no sync: dst_inst[p] = labels[p] (int32; -1 = unknown), and for every id i in [0, max_id) the ingest's
+ * tables are rebuilt: stats[i] = 0 except keep = (i < assoc_max_id and assoc_bbox[i + 1][0] != 0), bbox[i] = that
+ * label's box [u_lo, u_hi, v_lo, v_hi] as f32 where kept, 0 elsewhere.                                          */
+typedef struct vmb_relabel_args {
+  int width, height;
+  const long long* labels;       /* [W][H] int64 labels of vmb_assoc_finalize                                    */
+  const long long* assoc_bbox;   /* [assoc_max_id + 1][5] its per-label box table (row r = label r - 1)          */
+  int assoc_max_id;              /* the association's max_id, 1 .. max_id                                        */
+  int max_id;                    /* rows of stats / bbox                                                         */
+  int* stats;                    /* out [max_id][8] as vmb_ingest_args.stats (only keep is set)                  */
+  float* bbox;                   /* out [max_id][4] as vmb_ingest_args.bbox                                      */
+  int* dst_inst;                 /* out [W][H] the store slot's instance image                                   */
+} vmb_relabel_args;
+
+int vmb_store_relabel(vmb_handle* h, const vmb_relabel_args* a, void* stream);
+
 /* ---- K5: meshing -----------------------------------------------------------------------------------
  * Marching cubes on a dense fp32 volume.  Replaces skimage.measure.marching_cubes and the trimesh transforms of
  * Trainer.meshing (trainer.py:53-64, vis.py:6-19).  Volume [nx][ny][nz] (z fastest, nx, ny, nz >= 2); a corner is

@@ -1,4 +1,4 @@
-"""Track a whole Replica-layout sequence on the GPU and score the trajectory against its ``traj_w_c.txt``.
+"""Track a whole Replica- or ScanNet-layout sequence on the GPU and score the trajectory against its GT poses.
 
     python tools/track_seq.py --config CFG --out DIR --slam [--frames a:b] [--n-iter N] [--ba-every N --ba-iter M]
     python tools/track_seq.py --config CFG --out DIR --ckpt-dir LOG/ckpt --frame F [--frames a:b] [--n-iter N]
@@ -7,7 +7,11 @@
 tracked against the map of the frames before it and then mapped from the tracked pose.  ``--ckpt-dir`` localises every
 frame against the map of ``save_checkpoints`` files of frame F (loaded as ``tools/eval_2d.py`` loads them); frame a
 starts from its GT pose, every later frame from the constant-velocity prediction of the two before it, never from GT.
-Only the Replica layout (``rgb/``, ``depth/``, ``semantic_instance/``, ``semantic_class/``, ``traj_w_c.txt``) is read.
+Replica layout: ``rgb/``, ``depth/``, ``semantic_instance/``, ``semantic_class/`` and ``traj_w_c.txt``.  ScanNet layout
+(``--slam`` only): every frame in order through ``scannet.read_sequence``; vMAP configs run with the instance
+association (``Slam(assoc=...)``, one association state for the sequence), iMAP configs without.  The anchor is the
+first frame of ``--frames`` with a finite GT pose (frames before it are not run); ATE and RPE are computed over the
+frames whose GT pose is finite, and the others are listed as ``gt_invalid``.
 
 Writes ``traj_est.txt`` (``traj_w_c.txt`` format, one row per frame), ``metrics_traj.npy`` (a dict: ATE aligned and
 unaligned, RPE, lost frames, per-frame device milliseconds) and prints one JSON line.
@@ -26,7 +30,7 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 from eval_2d import load_sources, replica_gt  # noqa: E402
-from vmap_b200 import metrics  # noqa: E402
+from vmap_b200 import metrics, scannet  # noqa: E402
 from vmap_b200.cfg import Config  # noqa: E402
 from vmap_b200.slam import Slam  # noqa: E402
 
@@ -71,21 +75,42 @@ def main(argv=None):
                     help="bundle-adjustment step (default: layerwise for iMAP configs, fp32 otherwise)")
     args = ap.parse_args(argv)
     cfg = Config(args.config)
-    if cfg.dataset_format != "Replica":
-        raise SystemExit("track_seq.py reads the Replica layout only")
+    if cfg.dataset_format not in ("Replica", "ScanNet"):
+        raise SystemExit("track_seq.py reads the Replica and ScanNet layouts only")
+    is_scannet = cfg.dataset_format == "ScanNet"
+    if args.ckpt_dir and is_scannet:
+        raise SystemExit("track_seq.py: --ckpt-dir (localisation against a saved map) reads Replica sequences only; "
+                         "use --slam on ScanNet")
     if args.ckpt_dir and args.frame is None:
         raise SystemExit("--ckpt-dir needs --frame")
     os.makedirs(args.out, exist_ok=True)
-    gt_all = np.loadtxt(os.path.join(cfg.dataset_dir, "traj_w_c.txt"), delimiter=" ").reshape(-1, 4, 4)
+    if is_scannet:
+        gt_all = np.stack(scannet.ScanNet(cfg, n_trackers=0).poses)
+    else:
+        gt_all = np.loadtxt(os.path.join(cfg.dataset_dir, "traj_w_c.txt"), delimiter=" ").reshape(-1, 4, 4)
     n = len(os.listdir(os.path.join(cfg.dataset_dir, "depth")))
     a, b = 0, n
     if args.frames:
         lo, hi = args.frames.split(":")
         a, b = int(lo or 0), int(hi or n)
     frames = list(range(a, min(b, n)))
-    kw = dict(n_track_iter=args.n_iter, seed=args.seed, background_cls=REPLICA_BACKGROUND_CLS,
-              bbox_scale=REPLICA_BBOX_SCALE, max_frames=len(frames), timing=True,
+    if is_scannet:                                        # the anchor: the first frame with a finite GT pose
+        finite = [i for i in frames if np.all(np.isfinite(gt_all[i]))]
+        if not finite:
+            raise SystemExit("track_seq.py: no frame in --frames has a finite GT pose to anchor the trajectory")
+        frames = frames[frames.index(finite[0]):]
+        a = frames[0]
+    kw = dict(n_track_iter=args.n_iter, seed=args.seed, max_frames=len(frames), timing=True,
               store_capacity=args.store_capacity, track_impl=args.track_impl)
+    if is_scannet:
+        assoc = None
+        if not cfg.imap_mode:
+            assoc = scannet.InstanceTracker(cfg.fx, cfg.fy, cfg.cx, cfg.cy, cfg.data_device,
+                                            bbox_scale=scannet.BBOX_SCALE)
+        kw.update(background_cls=[c for c in scannet.BG_CLASSES if c >= 0], bbox_scale=scannet.BBOX_SCALE,
+                  assoc=assoc)
+    else:
+        kw.update(background_cls=REPLICA_BACKGROUND_CLS, bbox_scale=REPLICA_BBOX_SCALE)
     if args.slam:
         slam = Slam(cfg, T_init=gt_all[a], ba_every=args.ba_every, n_ba_iter=args.ba_iter, ba_impl=args.ba_impl, **kw)
     else:
@@ -93,16 +118,26 @@ def main(argv=None):
         if skipped:
             print("objects without a box in their checkpoint, not tracked:", skipped)
         slam = Slam(cfg, T_init=gt_all[a], map=False, groups=groups_from_sources(sources), **kw)
-    for i in frames:
-        rgb, depth, _, inst, cls = replica_frame(cfg, i)
-        slam.step(torch.from_numpy(rgb), torch.from_numpy(depth), torch.from_numpy(inst), torch.from_numpy(cls))
+    if is_scannet:
+        for f in scannet.read_sequence(cfg, frames):
+            slam.step(f["rgb"], f["depth"], f["inst"], f["cls"])
+    else:
+        for i in frames:
+            rgb, depth, _, inst, cls = replica_frame(cfg, i)
+            slam.step(torch.from_numpy(rgb), torch.from_numpy(depth), torch.from_numpy(inst), torch.from_numpy(cls))
     res = slam.result()
     times = slam.phase_times()
     est, gt = res["poses"], gt_all[frames]
     np.savetxt(os.path.join(args.out, "traj_est.txt"), est.reshape(-1, 16), delimiter=" ")
+    # ScanNet: score the frames with a finite GT pose only (metrics.ate / rpe with valid=)
+    valid = np.ones(len(frames), bool) if is_scannet else None
+    gt_ok = np.isfinite(gt.reshape(len(frames), -1)).all(1)
+    has_pair = bool(np.any(gt_ok[:-1] & gt_ok[1:])) if len(frames) > 1 else False
     out = {"mode": "slam" if args.slam else "localise", "frames": frames,
-           "ate_aligned": metrics.ate(est, gt, align=True), "ate_unaligned": metrics.ate(est, gt, align=False),
-           "rpe": metrics.rpe(est, gt) if len(frames) > 1 else None,
+           "ate_aligned": metrics.ate(est, gt, align=True, valid=valid),
+           "ate_unaligned": metrics.ate(est, gt, align=False, valid=valid),
+           "rpe": metrics.rpe(est, gt, valid=valid) if has_pair else None,
+           "gt_invalid": [f for f, ok in zip(frames, gt_ok) if not ok],
            "lost": [f for f, l in zip(frames, res["lost"]) if l], "times_ms": times,
            "tracked_ids": res["tracked_ids"], "inserted": res["inserted"], "track_modes": res["track_modes"],
            "ba_loss": res["ba_loss"], "ba_frames": res["ba_frames"]}
@@ -111,7 +146,7 @@ def main(argv=None):
             "ate_rmse_unaligned_m": out["ate_unaligned"]["rmse"],
             "rpe_trans_rmse_m": out["rpe"]["trans_rmse"] if out["rpe"] else None,
             "rpe_rot_rmse_deg": out["rpe"]["rot_rmse_deg"] if out["rpe"] else None,
-            "lost": out["lost"], "frame_ms_median": float(np.median(times["frame"])),
+            "lost": out["lost"], "gt_invalid": out["gt_invalid"], "frame_ms_median": float(np.median(times["frame"])),
             "ba_passes": sum(1 for f in res["ba_frames"] if f)}
     print(json.dumps(line))
 

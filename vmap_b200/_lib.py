@@ -92,6 +92,13 @@ class IngestArgs(C.Structure):
     ]
 
 
+class RelabelArgs(C.Structure):
+    _fields_ = [
+        ("width", C.c_int), ("height", C.c_int), ("labels", _vp), ("assoc_bbox", _vp), ("assoc_max_id", C.c_int),
+        ("max_id", C.c_int), ("stats", _vp), ("bbox", _vp), ("dst_inst", _vp),
+    ]
+
+
 class McArgs(C.Structure):
     _fields_ = [
         ("volume", _vp), ("nx", C.c_int), ("ny", C.c_int), ("nz", C.c_int), ("level", C.c_float),
@@ -239,7 +246,7 @@ HULL_OK, HULL_TOO_FEW, HULL_FLAT, HULL_BAD = 0, 1, 2, 3       # VMB_HULL_*
 EXPORTS = (
     "vmb_version", "vmb_param_count", "vmb_param_stride", "vmb_param_offsets", "vmb_image_bytes",
     "vmb_create", "vmb_destroy", "vmb_last_error", "vmb_step", "vmb_mask_counts", "vmb_adam",
-    "vmb_build_image", "vmb_forward", "vmb_sample", "vmb_ingest_frame", "vmb_debug_gemm",
+    "vmb_build_image", "vmb_forward", "vmb_sample", "vmb_ingest_frame", "vmb_store_relabel", "vmb_debug_gemm",
     "vmb_mc_count", "vmb_mc_emit", "vmb_unproject",
     "vmb_clip_count", "vmb_clip_emit", "vmb_surface_sample", "vmb_nn_dist",
     "vmb_assoc_classify", "vmb_assoc_voxel", "vmb_assoc_finalize",
@@ -291,6 +298,7 @@ def lib():
         L.vmb_forward.argtypes = [_vp, C.POINTER(ForwardArgs), _vp]
         L.vmb_sample.argtypes = [_vp, C.POINTER(SampleArgs), _vp]
         L.vmb_ingest_frame.argtypes = [_vp, C.POINTER(IngestArgs), _vp]
+        L.vmb_store_relabel.argtypes = [_vp, C.POINTER(RelabelArgs), _vp]
         L.vmb_mc_count.argtypes = [_vp, C.POINTER(McArgs), _vp]
         L.vmb_mc_emit.argtypes = [_vp, C.POINTER(McArgs), _vp]
         L.vmb_unproject.argtypes = [_vp, C.POINTER(UnprojectArgs), _vp]

@@ -126,4 +126,28 @@ __global__ void __launch_bounds__(256) k_ingest_write(const int* __restrict__ in
   }
 }
 
+// ScanNet relabel: the slot's instance image and the per-id tables from K7's output (vmb_assoc_finalize) instead of
+// the ingest's.  One grid-stride pass over max(n, max_id): pixel p takes its label (int64 -> int32, -1 stays
+// "unknown"); id i < max_id gets keep = the label has a box (abox row i + 1 = label i, column 0) and that box as f32
+// (integers below 2^24: exact), every other stats / bbox entry 0.  Ids at or past assoc_max_id have no row: keep 0.
+__global__ void __launch_bounds__(256) k_store_relabel(const long long* __restrict__ labels,
+                                                       const long long* __restrict__ abox, int assoc_max_id,
+                                                       long long n, int max_id, int* dst_inst, int* stats,
+                                                       float* bbox) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long m = n > (long long)max_id ? n : (long long)max_id;
+  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < m; p += stride) {
+    if (p < n) dst_inst[p] = (int)labels[p];
+    if (p < max_id) {
+      const long long* r = abox + (p + 1) * 5;
+      const int keep = p < assoc_max_id && r[0] != 0;
+      int* s = stats + p * ST;
+      for (int c = 0; c < ST; ++c) s[c] = 0;
+      s[S_KEEP] = keep;
+      float* bb = bbox + p * 4;
+      for (int c = 0; c < 4; ++c) bb[c] = keep ? (float)r[1 + c] : 0.f;
+    }
+  }
+}
+
 }  // namespace ing

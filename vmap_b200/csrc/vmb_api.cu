@@ -548,6 +548,23 @@ int vmb_ingest_frame(vmb_handle* h, const vmb_ingest_args* a, void* stream) {
   return VMB_OK;
 }
 
+int vmb_store_relabel(vmb_handle* h, const vmb_relabel_args* a, void* stream) {
+  if (!h || !a || a->width <= 0 || a->height <= 0 || a->max_id <= 0 || !a->labels || !a->assoc_bbox || !a->stats ||
+      !a->bbox || !a->dst_inst)
+    return fail(h, VMB_E_ARG, "vmb_store_relabel: bad arguments");
+  if (a->assoc_max_id < 1 || a->assoc_max_id > a->max_id)
+    return fail(h, VMB_E_ARG, "vmb_store_relabel: need 1 <= assoc_max_id <= max_id (labels must fit the store's tables)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long n = (long long)a->width * a->height;
+  const long long m = n > a->max_id ? n : a->max_id;
+  long long g = (m + 255) / 256;
+  if (g > 4 * h->n_sm) g = 4 * h->n_sm;
+  ing::k_store_relabel<<<(unsigned)g, 256, 0, st>>>(a->labels, a->assoc_bbox, a->assoc_max_id, n, a->max_id,
+                                                    a->dst_inst, a->stats, a->bbox);
+  CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
+}
+
 // ---- K5: meshing (marching cubes, object-pixel unprojection) ---------------------------------------
 static int mc_params(vmb_handle* h, const vmb_mc_args* a, mesh::McParams& q, const char* who) {
   if (!h || !a || !a->volume || a->nx < 2 || a->ny < 2 || a->nz < 2)

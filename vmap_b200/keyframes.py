@@ -157,6 +157,27 @@ class FrameStore:
         self._keep = (rgb, depth, inst, cls, bg)         # alive until the next call (async launches)
         return slot, self.stats, self.bbox
 
+    def relabel(self, slot: int, labels: torch.Tensor, assoc_bbox: torch.Tensor):
+        """ScanNet: replace the ingest's output for ``slot`` with the instance association's (``InstanceTracker.frame``,
+        K7).  ``labels`` [W, H] int64 become the slot's instance image (-1 = unknown), and ``stats`` / ``bbox`` are
+        rebuilt from ``assoc_bbox`` [assoc max_id + 1, 5] int64 (row r = label r - 1: kept, u_lo, u_hi, v_lo, v_hi;
+        the 2-D box rule of dataset.py:263-283): ``keep`` for the labels >= 0 that have a box, their boxes as f32,
+        every other entry 0.  One launch, no host read.  Returns ``(stats, bbox)`` as ``ingest`` does."""
+        dev = self.device
+        labels = labels.to(dev, torch.int64).contiguous()
+        assoc_bbox = assoc_bbox.to(dev, torch.int64).contiguous()
+        assert labels.shape == (self.W, self.H) and assoc_bbox.ndim == 2 and assoc_bbox.shape[1] == 5
+        assert self.refcount[slot] > 0, "relabel of a free slot"
+        a = _lib.RelabelArgs()
+        a.width, a.height, a.labels, a.assoc_bbox = self.W, self.H, _p(labels), _p(assoc_bbox)
+        a.assoc_max_id, a.max_id = assoc_bbox.shape[0] - 1, self.max_id
+        a.stats, a.bbox, a.dst_inst = _p(self.stats), _p(self.bbox), _p(self.inst[slot])
+        with torch.cuda.device(dev):
+            _lib.check(self._handle, self.lib.vmb_store_relabel(
+                self._handle, C.byref(a), C.c_void_p(torch.cuda.current_stream().cuda_stream)), "vmb_store_relabel")
+        self._keep = (labels, assoc_bbox)                 # alive until the next call (async launch)
+        return self.stats, self.bbox
+
     def visible_objects(self):
         """Host view of the last ingest: {instance id: bbox tensor [4] (device)} for kept instances
         (the reference's ``bbox_dict``, dataset.py:126,131).  One small device->host read per frame."""

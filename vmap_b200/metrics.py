@@ -401,11 +401,28 @@ def align_se3(est, gt) -> np.ndarray:
     return S
 
 
-def ate(est, gt, align: bool = True) -> dict:
+def _valid(valid, gt: np.ndarray) -> np.ndarray:
+    """The frames a metric keeps: ``valid`` [N] (bool) and a GT pose (or position) with every entry finite."""
+    v = np.asarray(valid, bool).reshape(-1)
+    if v.shape[0] != len(gt):
+        raise ValueError(f"valid needs one flag per frame ({len(gt)}), got {v.shape[0]}")
+    return v & np.isfinite(gt.reshape(len(gt), -1)).all(1)
+
+
+def ate(est, gt, align: bool = True, valid=None) -> dict:
     """Absolute trajectory error (Sturm et al. 2012, the TUM RGB-D benchmark, eq. 2): F_i = Q_i^-1 S P_i with P the
     estimate, Q the ground truth and S = ``align_se3(P, Q)`` (identity with ``align=False``); the residual of frame i
     is |trans(F_i)| = |q_i - S p_i| in metres.  Returns rmse, mean, median and max of the residuals (floats) and the
-    per-frame ``errors`` [N] (numpy)."""
+    per-frame ``errors`` [N] (numpy).  ``valid`` (optional [N] bool, e.g. all True): score only the frames it flags
+    whose GT pose has no non-finite entry (ScanNet marks frames without a GT pose with inf); the result is the metric
+    of that subset, and ``errors`` holds its frames only."""
+    if valid is not None:
+        g = np.asarray(gt.detach().cpu() if torch.is_tensor(gt) else gt, np.float64)
+        e = np.asarray(est.detach().cpu() if torch.is_tensor(est) else est, np.float64)
+        m = _valid(valid, g)
+        if not m.any():
+            raise ValueError("ate: no frame with a valid GT pose")
+        return ate(e[m], g[m], align=align)
     e, g = _positions(est), _positions(gt)
     S = align_se3(e, g) if align else np.eye(4)
     err = np.linalg.norm(g - (e @ S[:3, :3].T + S[:3, 3]), axis=1)
@@ -425,14 +442,23 @@ def _rel(T: np.ndarray, delta: int) -> np.ndarray:
     return _inv_se3(T[:-delta]) @ T[delta:]
 
 
-def rpe(est, gt, delta: int = 1) -> dict:
+def rpe(est, gt, delta: int = 1, valid=None) -> dict:
     """Relative pose error (Sturm et al. 2012, eq. 1) over ``delta`` frames: E_i = (Q_i^-1 Q_{i+d})^-1 (P_i^-1 P_{i+d}).
     Returns ``trans_rmse`` (metres), the RMSE of |trans(E_i)|, and ``rot_rmse_deg``, the RMSE of the rotation angle
-    arccos((trace(rot(E_i)) - 1) / 2) in degrees, plus the per-pair ``trans_errors`` / ``rot_errors_deg``."""
+    arccos((trace(rot(E_i)) - 1) / 2) in degrees, plus the per-pair ``trans_errors`` / ``rot_errors_deg``.  ``valid``
+    (optional [N] bool): keep only the pairs (i, i + d) whose two frames it flags and whose two GT poses have no
+    non-finite entry, as ``ate`` does per frame."""
     P, Q = _poses(est), _poses(gt)
     if P.shape != Q.shape or not 1 <= delta < len(P):
         raise ValueError("rpe: est and gt need the same number of poses, more than delta")
-    E = _inv_se3(_rel(Q, delta)) @ _rel(P, delta)
+    if valid is not None:
+        m = _valid(valid, Q)
+        i = np.nonzero(m[:-delta] & m[delta:])[0]
+        if len(i) == 0:
+            raise ValueError("rpe: no pair of frames with valid GT poses")
+        E = _inv_se3(_inv_se3(Q[i]) @ Q[i + delta]) @ (_inv_se3(P[i]) @ P[i + delta])
+    else:
+        E = _inv_se3(_rel(Q, delta)) @ _rel(P, delta)
     te = np.linalg.norm(E[:, :3, 3], axis=1)
     c = np.clip((np.trace(E[:, :3, :3], axis1=1, axis2=2) - 1.0) / 2.0, -1.0, 1.0)
     re = np.degrees(np.arccos(c))

@@ -13,6 +13,9 @@ depth scale / filter stay on the host with the reference's cv2 / numpy calls; as
 threads.  By default it reproduces the reference's 4-worker DataLoader, where each worker has its own ``inst_dict``:
 frame i is associated by tracker i % 4.  ``multi_worker=False`` uses one tracker, as the single-worker loader does;
 ``shared_tracker=True`` is the opt-in deviation that tracks all frames with one tracker.
+
+``read_sequence(cfg)`` is the reader for online SLAM (``slam.Slam(assoc=...)``): every frame in order with its GT pose,
+which may be inf, and no association (the SLAM loop runs it at the tracked pose).
 """
 from __future__ import annotations
 
@@ -125,6 +128,7 @@ class InstanceTracker:
         self.bg[bg] = 1
         self.bg = self.bg.to(self.device)
         self.inst_dict = {} if inst_dict is None else inst_dict
+        self.last_bbox = None       # the last frame's device box table [max_id + 1, 5] int64 (FrameStore.relabel)
         self._k = _Kernels(self.device)
         self.times = {"classify": 0.0, "voxel": 0.0, "hull": 0.0, "finalize": 0.0}
         self.timing = False
@@ -233,6 +237,7 @@ class InstanceTracker:
         final_d = final.to(dev)
         a.final_label = _p(final_d)
         self._k.call("vmb_assoc_finalize", a)
+        self.last_bbox = bbox
         if not relabel:
             self._tick("finalize", t0)
             return labels, None
@@ -272,7 +277,7 @@ class ScanNet:
         self.bbox_scale = BBOX_SCALE
         self.trackers = [InstanceTracker(self.fx, self.fy, self.cx, self.cy, self.device, self.min_pixels,
                                          bbox_scale=self.bbox_scale) for _ in range(n_trackers)]
-        self.inst_dict = self.trackers[0].inst_dict
+        self.inst_dict = self.trackers[0].inst_dict if self.trackers else {}
 
     def load_poses(self, path):
         self.poses = []
@@ -290,6 +295,10 @@ class ScanNet:
             if index + 1 == self.n_img:
                 return None
             index += 1
+        return self.decode_at(index)
+
+    def decode_at(self, index):
+        """``decode`` of frame ``index`` itself, whatever its pose (which may be non-finite)."""
         color = cv2.imread(self.color_paths[index]).astype(np.uint8)
         color = cv2.cvtColor(color, cv2.COLOR_BGR2RGB)
         depth = cv2.imread(self.depth_paths[index], cv2.IMREAD_UNCHANGED).astype(np.float32)
@@ -366,6 +375,40 @@ def init_loader(cfg, multi_worker=True, shared_tracker=False):
         raise ValueError(f"vmap_b200.scannet.init_loader handles ScanNet configs, not {cfg.dataset_format}")
     n = N_WORKERS if multi_worker and not shared_tracker else 1
     return _Loader(ScanNet(cfg, n_trackers=n), n)
+
+
+def read_sequence(cfg, frames=None, prefetch=4):
+    """The frames of a ScanNet sequence in order, for online SLAM (``slam.Slam(assoc=...)``): no association, and no
+    inf-pose skip (GT is only used to score a trajectory, so a frame whose GT pose is invalid is still a frame).  Host
+    decode as ``ScanNet.decode`` (resize, edge crop, depth scale / filter), ``prefetch`` frames ahead on threads.
+    Yields per frame a dict: ``index``, ``rgb`` [W, H, 3] uint8, ``depth`` [W, H] f32 metres, ``inst`` [W, H] int32
+    raw ids (instance + 1, dataset.py:247) and ``cls`` [W, H] int32 classes (both None in iMAP mode), and ``T`` the
+    GT camera-to-world pose [4, 4] fp64, which may hold non-finite entries.  Tensors are on the host."""
+    if cfg.dataset_format != "ScanNet":
+        raise ValueError(f"vmap_b200.scannet.read_sequence reads ScanNet configs, not {cfg.dataset_format}")
+    ds = ScanNet(cfg, n_trackers=0)
+    frames = list(range(len(ds))) if frames is None else list(frames)
+
+    def load(i):
+        color, depth, T, inst, sem = ds.decode_at(i)
+        out = {"index": i, "rgb": torch.from_numpy(np.ascontiguousarray(color.transpose(1, 0, 2))),
+               "depth": torch.from_numpy(np.ascontiguousarray(depth.T)), "T": np.asarray(T, np.float64),
+               "inst": None, "cls": None}
+        if inst is not None:
+            out["inst"] = torch.from_numpy(np.ascontiguousarray(inst.T))
+            semc = np.clip(sem.astype(np.int64), -1, None).astype(np.int32)      # as ScanNet.associate passes it
+            out["cls"] = torch.from_numpy(np.ascontiguousarray(semc.T))
+        return out
+
+    with ThreadPoolExecutor(max_workers=max(prefetch, 1)) as pool:
+        futs = {}
+        for j in range(min(prefetch, len(frames))):
+            futs[j] = pool.submit(load, frames[j])
+        for j in range(len(frames)):
+            nxt = j + prefetch
+            if nxt < len(frames):
+                futs[nxt] = pool.submit(load, frames[nxt])
+            yield futs.pop(j).result() if j in futs else load(frames[j])
 
 
 _BOX_FILTER_TRACKERS = {}

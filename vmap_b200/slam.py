@@ -48,6 +48,21 @@ frame, as a bundle-adjustment pass's do.  ``joint_impl`` chooses the joint step:
 mode) or ``"fused"`` (vMAP mode: ``vmb_joint_step_fused``, the objects' fused hidden-32 step with AdamW inside it, whose
 PE backward also gives the pose rows; with ``do_bg`` the background model's joint step is the update's second group and
 its keyframe copies receive the refined poses too).  In vMAP mode joint poses need ``joint_impl="fused"``.
+
+On ScanNet sequences (``assoc``: one ``scannet.InstanceTracker`` for the whole sequence, vMAP mode with ``map=True``)
+a frame's instance image comes from the instance association (utils.box_filter), which needs the frame's pose.  The
+ids of the objects already mapped are known before the pose is, so per frame:
+
+1. the prediction, and ``FrameStore.ingest`` of the **raw** ids (instance + 1) with the ScanNet background classes:
+   the provisional labels;
+2. tracking of the kept and mapped ids against the map, as above (each tracked object's full raw mask: no erosion and
+   no -1 "unsure" pixels);
+3. the association at the frame's final pose (the tracked one, the kept prediction of a lost frame, or the given pose
+   with ``track=False``): the only call that changes the association state;
+4. ``FrameStore.relabel`` of the slot from its labels and 2-D boxes (dataset.py:263-283), then keyframes, insertion,
+   the background state image and mapping as above.
+
+The association's clouds keep the poses they were merged at: bundle adjustment and joint poses do not re-pose them.
 """
 from __future__ import annotations
 
@@ -100,7 +115,9 @@ class Slam:
     ``track_impl`` / ``ba_impl``: ``"fp32"`` or ``"layerwise"`` (see the module docstring; None: ``"layerwise"`` in iMAP
     mode, ``"fp32"`` otherwise).  ``joint_poses``: optimise the keyframe poses with the map in every mapping iteration
     (see the module docstring); ``joint_lr_rot`` / ``joint_lr_trans``: its rates (default ``cfg.pose_lr``);
-    ``joint_impl``: ``None`` / ``"layerwise"`` (iMAP mode) or ``"fused"`` (vMAP mode)."""
+    ``joint_impl``: ``None`` / ``"layerwise"`` (iMAP mode) or ``"fused"`` (vMAP mode).  ``assoc``: a
+    ``scannet.InstanceTracker``, the one association state of a ScanNet sequence (see the module docstring); ``step``
+    then takes raw ScanNet ids and classes, and ``background_cls`` defaults to ``scannet.BG_CLASSES``."""
 
     def __init__(self, cfg, T_init=None, track: bool = True, map: bool = True, groups=None, graph: bool = True,
                  n_track_iter: int = 20, lr_rot: Optional[float] = None, lr_trans: Optional[float] = None,
@@ -109,7 +126,13 @@ class Slam:
                  n_ba_iter: int = 20, ba_lr_rot: Optional[float] = None, ba_lr_trans: Optional[float] = None,
                  track_impl: Optional[str] = None, ba_impl: Optional[str] = None, joint_poses: bool = False,
                  joint_lr_rot: Optional[float] = None, joint_lr_trans: Optional[float] = None,
-                 joint_impl: Optional[str] = None):
+                 joint_impl: Optional[str] = None, assoc=None):
+        if assoc is not None and cfg.imap_mode:
+            raise ValueError("Slam: assoc is the ScanNet instance association; in iMAP mode every pixel is instance 0 "
+                             "and there is nothing to associate")
+        if assoc is not None and not map:
+            raise ValueError("Slam: assoc relabels the frames of a map being built: map=True (localisation on "
+                             "ScanNet, map=False, is not supported)")
         if joint_impl not in (None, "layerwise", "fused"):
             raise ValueError(f"Slam: joint_impl must be None, 'layerwise' or 'fused', not {joint_impl!r}")
         if joint_impl == "fused" and cfg.imap_mode:
@@ -135,6 +158,10 @@ class Slam:
         default_impl = "layerwise" if self.imap else "fp32"
         self.track_kw = dict(n_iter=n_track_iter, lr_rot=lr_rot, lr_trans=lr_trans, seed=seed + _TRACK_SEED,
                              impl=track_impl or default_impl)
+        self.assoc = assoc
+        if assoc is not None and not len(background_cls):
+            from .scannet import BG_CLASSES
+            background_cls = [c for c in BG_CLASSES if c >= 0]
         self.background_cls, self.bbox_scale = list(background_cls), bbox_scale
         # localisation holds only the live frame; mapping holds each object's keyframes (see the module docstring)
         self.max_slots = cfg.max_n_models * cfg.keyframe_buffer_size + 1 if map else 1
@@ -198,7 +225,8 @@ class Slam:
     def step(self, rgb, depth, inst, cls=None, T_wc=None) -> int:
         """Process the next frame (images [W, H]: rgb uint8 [.., 3], depth metres, instance and class ids).  ``T_wc``:
         the frame's pose when ``track=False`` (ignored otherwise).  In iMAP mode every pixel is instance 0 whatever
-        ``inst`` holds (it may be None).  Returns the frame index."""
+        ``inst`` holds (it may be None).  With ``assoc``, ``inst`` holds the raw ScanNet ids (instance + 1, as
+        ``scannet.read_sequence`` yields them) and ``cls`` the classes.  Returns the frame index."""
         k, cfg, dev = self.k, self.cfg, self.device
         if self.imap:
             inst, cls = torch.zeros((cfg.W, cfg.H), dtype=torch.int32, device=dev), None
@@ -236,6 +264,9 @@ class Slam:
             store.t_wc[slot] = pose.to(torch.float32)       # every consumer of the frame reads the store's pose
         self.poses[k] = pose
         self._mark()
+        if self.assoc is not None:
+            visible = self._associate(slot, inst, depth, cls, pose)
+            self._mark()
         if self.do_map:
             self._map_frame(slot, k, visible, pose)
         if self.ba_every:
@@ -248,6 +279,20 @@ class Slam:
         self.k += 1
         return k
 
+    def _associate(self, slot: int, inst, depth, cls, pose: torch.Tensor) -> Dict[int, torch.Tensor]:
+        """ScanNet: the instance association at the frame's final pose (its only state change), then the slot and the
+        store's tables relabelled from its output.  Returns the relabelled frame's kept labels and boxes."""
+        store, dev = self.store, self.device
+        inst = torch.as_tensor(inst).to(dev, torch.int32)
+        max_id = int(inst.max()) + 1 if inst.numel() else 1          # as the loader sets it (ScanNet.associate)
+        if max_id > store.max_id:
+            raise _lib.VmbError(f"Slam: instance id {max_id - 1} does not fit the frame store's max_id={store.max_id}")
+        labels, _ = self.assoc.frame(inst, torch.as_tensor(depth).to(dev, torch.float32),
+                                     T=pose.cpu().numpy(), sem=cls, max_id=max_id)
+        store.relabel(slot, labels, self.assoc.last_bbox)
+        kb = torch.cat([store.stats[:, 7:8].float(), store.bbox], 1).cpu()
+        return {int(i): kb[i, 1:] for i in torch.nonzero(kb[:, 0]).flatten().tolist()}
+
     def _mark(self, new_frame: bool = False) -> None:
         if self.timing:
             if new_frame:
@@ -258,17 +303,19 @@ class Slam:
 
     def phase_times(self) -> dict:
         """With ``timing``: per frame, device milliseconds of ``ingest`` (with the keep-flag read), ``track``,
-        ``bookkeeping`` (keyframes, insertion, tables: host work the device waits for) and ``map``, ``ba`` (the
-        bundle-adjustment pass with its table fill; 0.0 where none ran) and ``frame``."""
+        ``assoc`` (only with ``assoc``: the association, the relabel and its table read), ``bookkeeping`` (keyframes,
+        insertion, tables: host work the device waits for) and ``map``, ``ba`` (the bundle-adjustment pass with its
+        table fill; 0.0 where none ran) and ``frame``."""
         torch.cuda.synchronize(self.device)
-        out = {k: [] for k in ("ingest", "track", "bookkeeping", "map", "ba", "frame")}
+        phases = ("ingest", "track") + (("assoc",) if self.assoc is not None else ()) + ("bookkeeping", "map")
+        out = {k: [] for k in phases + ("ba", "frame")}
         for k, ev in enumerate(self.events):
             d = [a.elapsed_time(b) for a, b in zip(ev[:-1], ev[1:])]
-            if len(d) == 3:                                # no mapping mark (map=False)
-                d = d[:2] + [d[2], 0.0]
+            if len(d) == len(phases) - 1:                  # no mapping mark (map=False, or no object yet)
+                d = d + [0.0]
             ba = self._ba_events[k][0].elapsed_time(self._ba_events[k][1]) if k in self._ba_events else 0.0
-            d[3] -= ba                                     # the pass runs inside the last interval, after the map
-            for key, v in zip(("ingest", "track", "bookkeeping", "map"), d):
+            d[-1] -= ba                                    # the pass runs inside the last interval, after the map
+            for key, v in zip(phases, d):
                 out[key].append(v)
             out["ba"].append(ba)
             out["frame"].append(ev[0].elapsed_time(ev[-1]))

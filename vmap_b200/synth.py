@@ -6,8 +6,8 @@ trainer.py:32, embedding.py:51-76) and training batches whose sample depths foll
 depth-guided strategy (vmap.py:366-459) in closed form.  No oracle code is imported here.
 
 ``sphere_room_sequence`` renders a posed RGB-D + instance + class sequence of spheres in a room in closed form (fp64,
-on the host) for SLAM tests and timing, and ``write_replica`` stores it in the directory layout ``dataset.Replica``
-reads.
+on the host) for SLAM tests and timing; ``write_replica`` stores it in the directory layout ``dataset.Replica``
+reads and ``write_scannet`` in the one ``dataset.ScanNet`` reads.
 """
 from __future__ import annotations
 
@@ -184,7 +184,7 @@ def sphere_room_sequence(n_frames: int, W: int, H: int, fx: float, fy: float, cx
     [N, W, H, 3] uint8 (the colour rounded), ``inst`` / ``cls`` [N, W, H] int32, ``spheres`` and the room's
     ``background_cls``.  Spheres are instances 1-4 of class ``SPHERE_CLASS``; the room's planes are instances 20-25 of
     background classes, which the ingest relabels to the background (0).  Sphere 4 comes into view partway;
-    ``n_extra`` adds small spheres (``sphere_room_scene``)."""
+    ``n_extra`` adds small spheres (``sphere_room_scene``).  ``intrinsics`` is (fx, fy, cx, cy)."""
     spheres = sphere_room_scene(math.atan((W / 2) / fx), n_extra)
     poses = sphere_room_path(n_frames, yaw_deg)
     out = {k: [] for k in ("depth", "rgb", "inst", "cls")}
@@ -195,7 +195,7 @@ def sphere_room_sequence(n_frames: int, W: int, H: int, fx: float, fy: float, cx
         out["inst"].append(inst)
         out["cls"].append(cls)
     seq = {k: np.stack(v) for k, v in out.items()}
-    seq.update(poses=poses, spheres=spheres, background_cls=sorted(set(ROOM_CLASSES)))
+    seq.update(poses=poses, spheres=spheres, background_cls=sorted(set(ROOM_CLASSES)), intrinsics=(fx, fy, cx, cy))
     return seq
 
 
@@ -216,3 +216,50 @@ def write_replica(root: str, seq: dict, depth_scale: float = 1.0 / 1000.0) -> No
                     seq["inst"][i].astype(np.uint16).T)
         cv2.imwrite(os.path.join(root, "semantic_class", f"semantic_class_{i}.png"), seq["cls"][i].astype(np.uint16).T)
     np.savetxt(os.path.join(root, "traj_w_c.txt"), np.asarray(seq["poses"]).reshape(-1, 16), delimiter=" ")
+
+
+# ScanNet classes of the scene (dataset.py:187's background list holds 1, 3 and 41; 5 is not in it)
+SCANNET_ROOM_CLASSES = (1, 1, 41, 3, 1, 1)          # wall, wall, ceiling, floor, wall, wall
+SCANNET_SPHERE_CLASS = 5
+
+
+def scannet_classes(inst: np.ndarray) -> np.ndarray:
+    """The ScanNet class image ``write_scannet`` writes for the instance image ``inst`` of the sphere room."""
+    cls = np.full(inst.shape, SCANNET_SPHERE_CLASS, np.int32)
+    for i, c in zip(ROOM_IDS, SCANNET_ROOM_CLASSES):
+        cls[inst == i] = c
+    return cls
+
+
+def write_scannet(root: str, seq: dict, mw: int = 10, inf_frames=(), depth_scale: float = 1.0 / 1000.0,
+                  color_size=(1296, 968)) -> None:
+    """Write the sphere-room sequence ``seq`` (``sphere_room_sequence``) in the layout ``dataset.ScanNet`` reads
+    (dataset.py:150-262): every frame is rendered again at (W + 2 mw) x (H + 2 mw) with the principal point moved by
+    ``mw``, so the loader's edge crop of ``mw`` pixels gives back ``seq``'s camera and images.  Files: ``color/{i}.jpg``
+    at ``color_size`` (the loader resizes it to the depth size), ``depth/{i}.png`` uint16 in units of ``depth_scale``
+    metres, ``instance-filt/{i}.png`` the instance id - 1 (the loader adds 1, so its ids are ``seq``'s),
+    ``label-filt/{i}.png`` the ScanNet class (``scannet_classes``: the room's planes get background classes, the
+    spheres a class that is not one), ``pose/{i}.txt`` the camera-to-world pose (every entry inf for the frames in
+    ``inf_frames``, as ScanNet marks frames without a pose) and ``intrinsic/intrinsic_depth.txt`` (4 x 4)."""
+    import cv2
+    fx, fy, cx, cy = seq["intrinsics"]
+    W, H = seq["depth"].shape[1:3]
+    Wf, Hf = W + 2 * mw, H + 2 * mw
+    for d in ("color", "depth", "instance-filt", "label-filt", "pose", "intrinsic"):
+        os.makedirs(os.path.join(root, d), exist_ok=True)
+    K = np.eye(4)
+    K[0, 0], K[1, 1], K[0, 2], K[1, 2] = fx, fy, cx + mw, cy + mw
+    np.savetxt(os.path.join(root, "intrinsic", "intrinsic_depth.txt"), K)
+    inf_frames = set(int(i) for i in inf_frames)
+    for i, T in enumerate(seq["poses"]):
+        depth, col, inst, _ = render_sphere_room(T, Wf, Hf, fx, fy, cx + mw, cy + mw, seq["spheres"])
+        rgb = np.clip(np.round(col * 255.0), 0, 255).astype(np.uint8)
+        bgr = cv2.cvtColor(rgb.transpose(1, 0, 2), cv2.COLOR_RGB2BGR)
+        cv2.imwrite(os.path.join(root, "color", f"{i}.jpg"), cv2.resize(bgr, color_size, interpolation=cv2.INTER_LINEAR))
+        dq = np.clip(np.round(depth / depth_scale), 0, 65535).astype(np.uint16)
+        cv2.imwrite(os.path.join(root, "depth", f"{i}.png"), dq.T)
+        cv2.imwrite(os.path.join(root, "instance-filt", f"{i}.png"), np.maximum(inst - 1, 0).astype(np.uint16).T)
+        cv2.imwrite(os.path.join(root, "label-filt", f"{i}.png"), scannet_classes(inst).astype(np.uint16).T)
+        P = np.full((4, 4), np.inf) if i in inf_frames else np.asarray(T, np.float64)
+        with open(os.path.join(root, "pose", f"{i}.txt"), "w") as f:
+            f.write("\n".join(" ".join(repr(float(x)) for x in row) for row in P) + "\n")
