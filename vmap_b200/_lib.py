@@ -245,7 +245,7 @@ HULL_OK, HULL_TOO_FEW, HULL_FLAT, HULL_BAD = 0, 1, 2, 3       # VMB_HULL_*
 
 EXPORTS = (
     "vmb_version", "vmb_param_count", "vmb_param_stride", "vmb_param_offsets", "vmb_image_bytes",
-    "vmb_create", "vmb_destroy", "vmb_last_error", "vmb_step", "vmb_mask_counts", "vmb_adam",
+    "vmb_create", "vmb_destroy", "vmb_last_error", "vmb_step", "vmb_step_trace", "vmb_mask_counts", "vmb_adam",
     "vmb_build_image", "vmb_forward", "vmb_sample", "vmb_ingest_frame", "vmb_store_relabel", "vmb_debug_gemm",
     "vmb_mc_count", "vmb_mc_emit", "vmb_unproject",
     "vmb_clip_count", "vmb_clip_emit", "vmb_surface_sample", "vmb_nn_dist",
@@ -294,6 +294,7 @@ def lib():
         L.vmb_destroy.argtypes = [_vp]
         L.vmb_destroy.restype = None
         L.vmb_step.argtypes = [_vp, C.POINTER(StepArgs), _vp]
+        L.vmb_step_trace.argtypes = [_vp, C.POINTER(StepArgs), _vp, _ll, _vp]
         L.vmb_adam.argtypes = [_vp, C.POINTER(AdamArgs), _vp]
         L.vmb_forward.argtypes = [_vp, C.POINTER(ForwardArgs), _vp]
         L.vmb_sample.argtypes = [_vp, C.POINTER(SampleArgs), _vp]

@@ -1,11 +1,15 @@
 // K1: ONE launch per optimisation step for hidden = 32 (sm_90a: wgmma, bulk async copy, mbarrier).
 //   mask counts (render_rays.py:68,86) -> PE -> MLP -> volume render -> losses -> backward
 //   -> per-object gradient reduction in a fixed order -> AdamW + fp16 weight-image refresh
-// fp16 operands / fp32 accumulate on wgmma.mma_async (m64nNk16, both operands from shared memory, accumulators in
-// registers), weights staged per object with one bulk async copy.  CTA = 256 threads = two warpgroups; a tile is up to
-// 128 sample points (whole rays) and walks through 12 dependent MMA stages (6 forward, 6 backward): threads write the
-// stage's operands -> fence + CTA barrier -> each warpgroup issues the stage's wgmmas for its 64 points and waits ->
-// the hidden-layer epilogues run on the accumulator fragments in registers.  Shared-memory operand layout: no-swizzle
+// fp16 operands / fp32 accumulate on wgmma.mma_async (m64nNk16, accumulators in registers), weights staged per object
+// with one bulk async copy.  CTA = 256 threads = two warpgroups; a tile is up to 128 sample points (whole rays) and
+// walks through 12 dependent MMA stages (6 forward, 6 backward): threads write the stage's operands -> fence + CTA
+// barrier -> each warpgroup issues the stage's wgmmas for its 64 points and waits -> the hidden-layer epilogues run on
+// the accumulator fragments in registers.  B (weights) always comes from shared memory.  A comes from REGISTERS (RS
+// form) wherever it is a hidden activation or a gated dY of this warpgroup's own 64 points: an m64n32 fp32 fragment
+// packed to f16x2 by the epilogue IS the A fragment of two k16 steps, so the next stage reads the epilogue's registers
+// (the same fp16 values it also stores for the weight-gradient MMAs).  A stays in shared memory (SS form) for the
+// embedding blocks, dhead and the weight-gradient MMAs (K = points of both warpgroups).  Shared-memory operand layout: no-swizzle
 // 8x8 core matrices, an activation block is [feature-group (8 feats)][point][8 feats] halves -- the same bytes serve
 // as a K-major A operand (forward / dgrad: M = points, K = features) and as an MN-major operand (wgrad: M or N =
 // features, K = points).  Weight gradients accumulate in REGISTERS across all the tiles a CTA owns for an object (each
@@ -163,6 +167,14 @@ struct Mma {
 // pipeline fill -- gets correspondingly fewer pairs: no CTA's cost exceeds the even share by more than one pair.
 constexpr int MAX_CTAS = 192;
 struct Ranges { int begin[MAX_CTAS + 1]; };
+
+// Phase trace (TRACE instantiation only, vmb_step_trace): thread 0 of each warpgroup stamps clock64() into its own
+// row of TR_STRIDE words, row = 2 * CTA + warpgroup.  Header: [0] kernel start, [1] prologue done, [2] last segment
+// done, [3] grid barrier passed, [4] kernel end, [5] tiles run, [6] cycles in segment flushes, [7] segments.  Then
+// TR_NST stamps for each of the first TR_TILES tiles: [0] tile start and [k] the end of phase k (1..18: PE, in_layer,
+// mid1, cat_layer, mid2, color_linear + alpha, out_color, heads transpose, render + loss, d_hc, d_fc4, d_fc3, d_fc2,
+// d_fc1, d_emb, EG store, PE backward, dB).
+constexpr int TR_HDR = 8, TR_NST = 20, TR_TILES = 64, TR_STRIDE = TR_HDR + TR_TILES * TR_NST;
 __device__ __forceinline__ int cta_of_pair(const Ranges& rg, int G, int pair) {        // largest c with begin[c] <= pair
   int lo = 0, hi = G - 1;
   while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (rg.begin[mid] <= pair) lo = mid; else hi = mid - 1; }
@@ -177,17 +189,28 @@ __device__ __forceinline__ int cta_of_pair(const Ranges& rg, int G, int pair) { 
 // dB wgrad (the rule of k_tlw_pose).  Each warpgroup sums its own directions (hsel 0: dE_xyz, then 0..11; hsel 1:
 // 12..20) and stores its half to jdt[b][point][hsel][3] (fp32, plain stores); k_joint_rows adds the halves in that
 // order.  jdt is read only under JOINT: the plain instantiations compile to the same SASS as without it.
-// Registers (ptxas -v, sm_90a), no spills: JOINT S = any / 10 / 14: 248 / 248 / 248 (plain: 245 / 248 / 248).
-template <int SC, bool JOINT>
+// Registers (ptxas -v, sm_90a), no spills: JOINT S = any / 10 / 14: 249 / 249 / 249 (plain: 251 / 251 / 251; TRACE
+// S = 10: 254).
+// TRACE (phase-stamped build, S = 10 only): `trace` as uf::TR_STRIDE describes; the other instantiations ignore it and
+// contain no trace code.
+template <int SC, bool JOINT, bool TRACE = false>
 __global__ void __launch_bounds__(uf::NT, 1)
 k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image, const __grid_constant__ uf::Ranges rg, int tpo, int npo, int nr, int rpw,
-             float* jdt) {
+             float* jdt, unsigned long long* trace) {
   using namespace uf;
   extern __shared__ __align__(1024) unsigned char smem[];
   Misc* misc = reinterpret_cast<Misc*>(smem + SM_MISC);
   int* cnt = reinterpret_cast<int*>(smem + SM_CNT);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int S = SC ? SC : a.S, R = a.R;
+  unsigned long long* tr = nullptr;
+  const bool tr_on = TRACE && (tid & 127) == 0;
+  int tr_t = 0, tr_nseg = 0;
+  long long tr_flush = 0, tr_f0 = 0;
+  if constexpr (TRACE) tr = trace + (size_t)(2 * blockIdx.x + (tid >> 7)) * TR_STRIDE;
+#define TR_STAMP(slot) do { if constexpr (TRACE) { if (tr_on) tr[slot] = clock64(); } } while (0)
+#define TR_TILE(k) do { if constexpr (TRACE) { if (tr_on && tr_t < TR_TILES) tr[TR_HDR + tr_t * TR_NST + (k)] = clock64(); } } while (0)
+  TR_STAMP(0);
 
   if (tid == 0) {
     ptx::mbar_init(&misc->wbar, 1);
@@ -251,6 +274,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     }
   }
   __syncthreads();
+  TR_STAMP(1);
 
   uint32_t wpar = 0;                  // weight-barrier parity (one completion per segment)
 
@@ -417,25 +441,31 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     // accumulators -> commit -> wait.
 #define OPERANDS_READY() do { ptx::fence_async_smem(); __syncthreads(); ptx::wgmma_fence(); } while (0)
 #define MMA_DONE() do { ptx::wgmma_commit(); ptx::wgmma_wait<0>(); } while (0)
-    // hidden-layer epilogue on the fragment: acc + bias -> ReLU -> fp16 into block FG
-    auto epi_relu = [&](const float (&v)[16], int bias_off, int fg) {
+    // hidden-layer epilogue on the fragment: acc + bias -> ReLU -> fp16 into block FG, and into u: the A operand
+    // (ptx::wgmma_n32_rs) of the next stage's two k-steps over these 32 features
+    auto epi_relu = [&](const float (&v)[16], int bias_off, int fg, uint32_t (&u)[8]) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const float2 bb = *reinterpret_cast<const float2*>(wf + bias_off + 8 * j + 2 * cq);
         unsigned char* dst = act + (fg + j) * FGB + fr0 * 16 + cq * 4;
-        *reinterpret_cast<uint32_t*>(dst) = pack_relu_h2(v[4 * j] + bb.x, v[4 * j + 1] + bb.y);
-        *reinterpret_cast<uint32_t*>(dst + 128) = pack_relu_h2(v[4 * j + 2] + bb.x, v[4 * j + 3] + bb.y);
+        u[2 * j] = pack_relu_h2(v[4 * j] + bb.x, v[4 * j + 1] + bb.y);
+        u[2 * j + 1] = pack_relu_h2(v[4 * j + 2] + bb.x, v[4 * j + 3] + bb.y);
+        *reinterpret_cast<uint32_t*>(dst) = u[2 * j];
+        *reinterpret_cast<uint32_t*>(dst + 128) = u[2 * j + 1];
       }
     };
-    // dgrad epilogue: dY = (h > 0) * acc; h is read from its own block, dY goes to a block whose readers retired
-    auto epi_dgrad = [&](const float (&v)[16], int fg_h, int fg_out) {
+    // dgrad epilogue: dY = (h > 0) * acc; h is read from its own block, dY goes to a block whose readers retired and
+    // into u (the A operand of the dgrad GEMMs that read dY)
+    auto epi_dgrad = [&](const float (&v)[16], int fg_h, int fg_out, uint32_t (&u)[8]) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const int off = j * FGB + fr0 * 16 + cq * 4;
         const uint32_t h0 = *reinterpret_cast<const uint32_t*>(act + fg_h * FGB + off);
         const uint32_t h1 = *reinterpret_cast<const uint32_t*>(act + fg_h * FGB + off + 128);
-        *reinterpret_cast<uint32_t*>(act + fg_out * FGB + off) = um::gate_h2(um::pack_h2(v[4 * j], v[4 * j + 1]), h0);
-        *reinterpret_cast<uint32_t*>(act + fg_out * FGB + off + 128) = um::gate_h2(um::pack_h2(v[4 * j + 2], v[4 * j + 3]), h1);
+        u[2 * j] = um::gate_h2(um::pack_h2(v[4 * j], v[4 * j + 1]), h0);
+        u[2 * j + 1] = um::gate_h2(um::pack_h2(v[4 * j + 2], v[4 * j + 3]), h1);
+        *reinterpret_cast<uint32_t*>(act + fg_out * FGB + off) = u[2 * j];
+        *reinterpret_cast<uint32_t*>(act + fg_out * FGB + off + 128) = u[2 * j + 1];
       }
     };
     // embedding-gradient fragment (8-column groups starting at 4-column block blk0) -> the shared fp32 tile
@@ -490,6 +520,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     prefetch(t0);
 
     for (int t = t0; t < t1; ++t) {
+      TR_TILE(0);
       const int ray = t * nr + ray_in_tile;
       // ---- E0: positional embedding (embedding.py:82-91) ----------------------------------------------------
       const float t0x = nx * isc, t1x = ny * isc, t2x = nz * isc, zv = nzv;
@@ -540,42 +571,55 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
           dh[0] = make_uint4(0u, 0u, 0u, 0u); dh[128] = make_uint4(0u, 0u, 0u, 0u);
         }
       }
+      TR_TILE(1);
       float acc[16], hacc[8];
+      uint32_t ua[8];                                   // the last epilogue's fp16 output: A of the next stage (RS)
       OPERANDS_READY();                                 // in_layer: emb1 (K = 96)
 #pragma unroll
       for (int ks = 0; ks < 6; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_E1, ks), mm.w_k(um::IMG_WIN, ks), ks > 0);
       MMA_DONE();
-      epi_relu(acc, um::F_BIN, FG_FC1);
+      epi_relu(acc, um::F_BIN, FG_FC1, ua);
+      TR_TILE(2);
       OPERANDS_READY();                                 // mid1: fc1
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_FC1, ks), mm.w_k(um::IMG_WM1, ks), ks > 0);
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WM1, ks), ks > 0);
       MMA_DONE();
-      epi_relu(acc, um::F_BM1, FG_FC2);
+      epi_relu(acc, um::F_BM1, FG_FC2, ua);
+      TR_TILE(3);
       OPERANDS_READY();                                 // cat_layer: [fc2 | emb1] (K = 128)
 #pragma unroll
-      for (int ks = 0; ks < 8; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_FC2, ks), mm.w_k(um::IMG_WCAT, ks), ks > 0);
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WCAT, ks), ks > 0);
+#pragma unroll
+      for (int ks = 2; ks < 8; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_FC2, ks), mm.w_k(um::IMG_WCAT, ks), 1u);
       MMA_DONE();
-      epi_relu(acc, um::F_BCAT, FG_FC3);
+      epi_relu(acc, um::F_BCAT, FG_FC3, ua);
+      TR_TILE(4);
       OPERANDS_READY();                                 // mid2: fc3
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_FC3, ks), mm.w_k(um::IMG_WM2, ks), ks > 0);
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WM2, ks), ks > 0);
       MMA_DONE();
-      epi_relu(acc, um::F_BM2, FG_FC4);
+      epi_relu(acc, um::F_BM2, FG_FC4, ua);
+      TR_TILE(5);
       OPERANDS_READY();                                 // color_linear: [fc4 | emb2] (K = 80) ; out_alpha: fc4 -> column 0
 #pragma unroll
-      for (int ks = 0; ks < 5; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_FC4, ks), mm.w_k(um::IMG_WCL, ks), ks > 0);
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WCL, ks), ks > 0);
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16<0, 0>(hacc, mm.a_k(FG_FC4, ks), mm.w16_k(um::IMG_WA16, ks), ks > 0);
+      for (int ks = 2; ks < 5; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_FC4, ks), mm.w_k(um::IMG_WCL, ks), 1u);
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<0>(hacc, ua + 4 * ks, mm.w16_k(um::IMG_WA16, ks), ks > 0);
       MMA_DONE();
-      epi_relu(acc, um::F_BCL, FG_HC);
+      epi_relu(acc, um::F_BCL, FG_HC, ua);
       if (cq == 0) { hd[fr0 * 4] = hacc[0]; hd[(fr0 + 8) * 4] = hacc[2]; }
+      TR_TILE(6);
       OPERANDS_READY();                                 // out_color: hc -> columns 1..3
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16<0, 0>(hacc, mm.a_k(FG_HC, ks), mm.w16_k(um::IMG_WOC16, ks), ks > 0);
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<0>(hacc, ua + 4 * ks, mm.w16_k(um::IMG_WOC16, ks), ks > 0);
       MMA_DONE();
       if (cq == 0) { hd[fr0 * 4 + 1] = hacc[1]; hd[(fr0 + 8) * 4 + 1] = hacc[3]; }
       if (cq == 1) { hd[fr0 * 4 + 2] = hacc[0]; hd[fr0 * 4 + 3] = hacc[1]; hd[(fr0 + 8) * 4 + 2] = hacc[2]; hd[(fr0 + 8) * 4 + 3] = hacc[3]; }
+      TR_TILE(7);
       __syncthreads();                                  // heads tile: fragment layout -> point layout
+      TR_TILE(8);
       // ---- heads + volume render + losses + ray gradients, all in registers of the hsel == 0 warps ---------------
       // rays never straddle a warp: the scans over the sample axis are warp shuffles
       auto raysum = [&](float v) {                      // per-ray sum: guarded tree reduction to the ray's first lane, broadcast
@@ -668,58 +712,69 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
           }
         }
       }
+      TR_TILE(9);
       if (a.fwd_only || !a.backward) { __syncthreads(); continue; }
+      // dgrad chain: A = dhead (point layout, written by the render) from shared memory, every gated dY from the
+      // registers of the epilogue that made it; dYc and dY3 stay in registers until the d_emb stage reads them
+      uint32_t uyc[8], uy3[8];
       OPERANDS_READY();                                 // d_hc = dhead @ W_oc ; heads wgrad (out_alpha + out_color, weights and biases)
       ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_DH, 0), mm.w16_mn(um::IMG_WOC16), 0u);
       mm.wgrad16(wHD, FG_FC4, FG_DH);
       MMA_DONE();
-      epi_dgrad(acc, FG_HC, FG_Z);                      // dYc -> Z
+      epi_dgrad(acc, FG_HC, FG_Z, uyc);                 // dYc -> Z
+      TR_TILE(10);
       OPERANDS_READY();                                 // d_fc4 = dYc @ W_cl[:, :32] + dhead @ W_a ; wgrad color_linear
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_Z, ks), mm.w_mn(um::IMG_WCL, ks), ks > 0);
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, uyc + 4 * ks, mm.w_mn(um::IMG_WCL, ks), ks > 0);
       ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_DH, 0), mm.w16_mn(um::IMG_WA16), 1u);
       mm.wgrad32(wCL, FG_FC4, FG_Z);
       MMA_DONE();
-      epi_dgrad(acc, FG_FC4, FG_HC);                    // dY4 -> HC
+      epi_dgrad(acc, FG_FC4, FG_HC, ua);                // dY4 -> HC
+      TR_TILE(11);
       OPERANDS_READY();                                 // d_fc3 = dY4 @ W_m2 ; wgrad mid2
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_HC, ks), mm.w_mn(um::IMG_WM2, ks), ks > 0);
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, ua + 4 * ks, mm.w_mn(um::IMG_WM2, ks), ks > 0);
       mm.wgrad32(wM2, FG_FC3, FG_HC);
       MMA_DONE();
-      epi_dgrad(acc, FG_FC3, FG_FC4);                   // dY3 -> FC4
+      epi_dgrad(acc, FG_FC3, FG_FC4, uy3);              // dY3 -> FC4
+      TR_TILE(12);
       OPERANDS_READY();                                 // d_fc2 = dY3 @ W_cat[:, :32] ; wgrad cat_layer
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_FC4, ks), mm.w_mn(um::IMG_WCAT, ks), ks > 0);
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, uy3 + 4 * ks, mm.w_mn(um::IMG_WCAT, ks), ks > 0);
       mm.wgrad32(wCAT, FG_FC2, FG_FC4);
       MMA_DONE();
-      epi_dgrad(acc, FG_FC2, FG_HC);                    // dY2 -> HC
+      epi_dgrad(acc, FG_FC2, FG_HC, ua);                // dY2 -> HC
+      TR_TILE(13);
       OPERANDS_READY();                                 // d_fc1 = dY2 @ W_m1 ; wgrad mid1
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_HC, ks), mm.w_mn(um::IMG_WM1, ks), ks > 0);
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, ua + 4 * ks, mm.w_mn(um::IMG_WM1, ks), ks > 0);
       mm.wgrad32(wM1, FG_FC1, FG_HC);
       MMA_DONE();
-      epi_dgrad(acc, FG_FC1, FG_FC3);                   // dY1 -> FC3
+      epi_dgrad(acc, FG_FC1, FG_FC3, ua);               // dY1 -> FC3
+      TR_TILE(14);
       // d_emb1 = dY3 @ W_cat[:, 32:] + dY1 @ W_in (32 columns at a time), d_emb2 = dYc @ W_cl[:, 32:] ; wgrad in_layer
       OPERANDS_READY();
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
 #pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_FC4, ks), mm.w_mn(um::IMG_WCAT + (4 + 4 * c) * 512, ks), ks > 0);
+        for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, uy3 + 4 * ks, mm.w_mn(um::IMG_WCAT + (4 + 4 * c) * 512, ks), ks > 0);
 #pragma unroll
-        for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_FC3, ks), mm.w_mn(um::IMG_WIN + 4 * c * 512, ks), 1u);
+        for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, ua + 4 * ks, mm.w_mn(um::IMG_WIN + 4 * c * 512, ks), 1u);
         MMA_DONE();
         eg_store(acc, 8 * c);
         ptx::wgmma_fence();
       }
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_Z, ks), mm.w_mn(um::IMG_WCL + 4 * 512, ks), ks > 0);
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, uyc + 4 * ks, mm.w_mn(um::IMG_WCL + 4 * 512, ks), ks > 0);
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16<0, 1>(hacc, mm.a_k(FG_Z, ks), mm.w_mn(um::IMG_WCL + 8 * 512, ks), ks > 0);
+      for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<1>(hacc, uyc + 4 * ks, mm.w_mn(um::IMG_WCL + 8 * 512, ks), ks > 0);
       mm.wgrad32(wIN, FG_E1, FG_FC3);
       MMA_DONE();
+      TR_TILE(15);
       eg_store(acc, EG_E2);
       eg_store(hacc, EG_E2 + 8);
       __syncthreads();                                  // embedding-gradient tile: fragment layout -> point layout
+      TR_TILE(16);
       // ---- PE backward: dproj_d = pi * sum_k 2^k g_{k,d} cos(pi 2^k proj_d), written as an fp16 block --------------
       {
         const int q0 = hsel ? 3 : 0, q1 = hsel ? 5 : 3;
@@ -792,16 +847,20 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
           }
         }
       }
+      TR_TILE(17);
       // dB += dproj^T [1 x y z ...]: the 21 real feature rows are in the first warpgroup's half; the second issues the
       // same instructions on rows that are never stored, which keeps the wgmma stream free of divergent branches
       OPERANDS_READY();
       mm.wgrad16(wDB, FG_DPR, FG_E1);
       MMA_DONE();
       __syncthreads();                                  // the next tile's PE overwrites E1 / E2 / DH
+      TR_TILE(18);
+      if constexpr (TRACE) ++tr_t;
     }
 #undef OPERANDS_READY
 #undef MMA_DONE
     }   // compute threads
+    if constexpr (TRACE) tr_f0 = clock64();
     if (a.fwd_only) {                                   // nothing to reduce; the weight buffer is free once every warp is done
       __syncthreads();
       if (tid == 0 && gt < gt_end) {
@@ -874,6 +933,11 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       for (int i = tid; i < (L.stride >> 2); i += NT) dst[i] = src[i];
     }
     __syncthreads();
+    if constexpr (TRACE) { tr_flush += clock64() - tr_f0; ++tr_nseg; }
+  }
+  TR_STAMP(2);
+  if constexpr (TRACE) {
+    if (tr_on) { tr[5] = (unsigned long long)tr_t; tr[6] = (unsigned long long)tr_flush; tr[7] = (unsigned long long)tr_nseg; }
   }
 
   if (!a.fwd_only) {
@@ -890,6 +954,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     }
     __syncthreads();
     __threadfence();
+    TR_STAMP(3);
     const int n4 = L.stride >> 2;
     const long long W = (long long)a.B * n4;
     const long long lo = (W * blockIdx.x) / G, hi = (W * (blockIdx.x + 1)) / G;
@@ -917,7 +982,9 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       if (tid == 0) { gbar[0] = 0u; gbar[1] = 0u; gbar[2] = 0u; gbar[3] = 0u; gbar[4] = 0u; gbar[5] = 0u; }
     }
   }
-
+  TR_STAMP(4);
+#undef TR_STAMP
+#undef TR_TILE
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -953,14 +1020,18 @@ static void fused_partition(int B, int npo, int G, uf::Ranges& rg) {
   while (c < G) rg.begin[++c] = (int)T;
 }
 
-// jdt: the joint step's [B][R * S][2][3] pose-gradient halves (JOINT instantiations), or nullptr (the plain step)
+// jdt: the joint step's [B][R * S][2][3] pose-gradient halves (JOINT instantiations), or nullptr (the plain step).
+// trace: [2 * grid][uf::TR_STRIDE] phase stamps (the TRACE instantiation, training step at S = 10 only), or nullptr
 static int fused_launch_step(const VmbLayout& L, const StepParams& sp, const FusedExtra& fx, const void* image, int n_sm,
-                             cudaStream_t st, std::string& err, float* jdt = nullptr) {
+                             cudaStream_t st, std::string& err, float* jdt = nullptr, unsigned long long* trace = nullptr) {
   using namespace uf;
   if (L.H != 32 || L.nfreq != 6) { err = "fused step kernel: hidden must be 32 and n_freq 6"; return -4; }
   if (sp.S < 1 || sp.S > 32) { err = "fused step kernel: n_samples must be in [1, 32]"; return -4; }
   if (!sp.fwd_only && sp.B > MAX_OBJ_SMEM) { err = "fused step kernel: too many objects for the in-kernel mask counts"; return -4; }
   if (jdt && (sp.fwd_only || !sp.backward)) { err = "fused step kernel: the joint step needs the backward"; return -4; }
+  if (trace && (jdt || sp.fwd_only || !sp.backward || sp.S != 10)) {
+    err = "fused step kernel: the phase trace covers the training step at n_samples 10 only"; return -4;
+  }
   static bool attr_set[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
@@ -968,7 +1039,7 @@ static int fused_launch_step(const VmbLayout& L, const StepParams& sp, const Fus
   if (!attr_set[dev & 63]) {
     cudaError_t e = cudaSuccess;
     for (auto k : {k_step_fused<0, false>, k_step_fused<10, false>, k_step_fused<14, false>,
-                   k_step_fused<0, true>, k_step_fused<10, true>, k_step_fused<14, true>})
+                   k_step_fused<0, true>, k_step_fused<10, true>, k_step_fused<14, true>, k_step_fused<10, false, true>})
       if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
     if (e != cudaSuccess) { err = std::string("cudaFuncSetAttribute(k_step_fused): ") + cudaGetErrorString(e); return -2; }
     attr_set[dev & 63] = true;
@@ -996,8 +1067,9 @@ static int fused_launch_step(const VmbLayout& L, const StepParams& sp, const Fus
   attr[0].val.cooperative = sp.fwd_only ? 0 : 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
   cudaError_t e;
-  auto kern = [&](auto k) { return cudaLaunchKernelEx(&cfg, k, sp, fx, L, img, rg, tpo, npo, nr, rpw, jdt); };
-  if (jdt) e = kern(sp.S == 10 ? k_step_fused<10, true> : sp.S == 14 ? k_step_fused<14, true> : k_step_fused<0, true>);
+  auto kern = [&](auto k) { return cudaLaunchKernelEx(&cfg, k, sp, fx, L, img, rg, tpo, npo, nr, rpw, jdt, trace); };
+  if (trace) e = kern(k_step_fused<10, false, true>);
+  else if (jdt) e = kern(sp.S == 10 ? k_step_fused<10, true> : sp.S == 14 ? k_step_fused<14, true> : k_step_fused<0, true>);
   else     e = kern(sp.S == 10 ? k_step_fused<10, false> : sp.S == 14 ? k_step_fused<14, false> : k_step_fused<0, false>);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { err = std::string("k_step_fused launch: ") + cudaGetErrorString(e); return -2; }

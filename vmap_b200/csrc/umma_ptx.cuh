@@ -1,5 +1,6 @@
 // Thin inline-PTX wrappers for the sm_90a features the step kernel uses:
-// wgmma (warpgroup MMA, operands in shared memory, accumulators in registers), mbarrier, bulk async copy.
+// wgmma (warpgroup MMA, B in shared memory, A in shared memory or registers, accumulators in registers), mbarrier,
+// bulk async copy.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -87,6 +88,34 @@ __device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t adesc, uint64_
       "{%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
       : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB)
+      : "memory");
+}
+// RS form: A from registers, B from shared memory.  A fragment of one k16 step (f16x2 pairs, low half = lower column):
+// a[0] = row 16w + l/4, columns 2(l%4) + {0, 1};  a[1] = row + 8;  a[2], a[3] = the same rows, columns + 8.  That is
+// the accumulator fragment above packed in order: the m64n32 fragment d[0..15] of one GEMM, packed pairwise to
+// u[i] = f16x2(d[2i], d[2i + 1]), is the A operand of the two k16 steps of the next, u[0..3] for k = 0..15 and u[4..7]
+// for k = 16..31 -- `a` points at u + 4 ks.
+template <int TB>
+__device__ __forceinline__ void wgmma_n32_rs(float (&d)[16], const uint32_t* a, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, %22;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate), "n"(TB)
+      : "memory");
+}
+template <int TB>
+__device__ __forceinline__ void wgmma_n16_rs(float (&d)[8], const uint32_t* a, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, %14;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate), "n"(TB)
       : "memory");
 }
 template <int TA, int TB>

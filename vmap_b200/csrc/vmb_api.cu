@@ -416,6 +416,26 @@ int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream) {
   return VMB_OK;
 }
 
+int vmb_step_trace(vmb_handle* h, const vmb_step_args* a, unsigned long long* trace, long long trace_words, void* stream) {
+  StepParams sp;
+  const int rc0 = step_params(h, a, sp, "vmb_step_trace");
+  if (rc0 != VMB_OK) return rc0;
+  if (!h->umma_ok || !a->image || a->impl == VMB_IMPL_FP32 || a->impl == VMB_IMPL_LAYERWISE)
+    return fail(h, VMB_E_UNSUPPORTED, "vmb_step_trace: the fused hidden-32 step only (hidden 32, n_freq 6, an image)");
+  static_assert(VMB_TRACE_STRIDE == uf::TR_STRIDE, "trace row layout");
+  const int max_grid = h->n_sm < uf::MAX_CTAS ? h->n_sm : uf::MAX_CTAS;
+  if (!trace || trace_words < 2LL * max_grid * uf::TR_STRIDE)
+    return fail(h, VMB_E_ARG, "vmb_step_trace: the trace needs 2 * min(#SMs, 192) rows of VMB_TRACE_STRIDE words");
+  cudaStream_t st = (cudaStream_t)stream;
+  FusedExtra fx;
+  const int rc1 = fused_extra(h, a, st, fx);
+  if (rc1 != VMB_OK) return rc1;
+  std::string err;
+  const int rc = fused_launch_step(h->L, sp, fx, a->image, h->n_sm, st, err, nullptr, trace);
+  if (rc != VMB_OK) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, err);
+  return VMB_OK;
+}
+
 int vmb_forward(vmb_handle* h, const vmb_forward_args* a, void* stream) {
   if (!h || !a || a->n_obj <= 0 || a->n_obj > h->max_obj || a->n_points <= 0 || !a->points || !a->params ||
       !a->scale || !a->alpha || !a->colour)
