@@ -1,10 +1,10 @@
 // K10: camera tracking against the object map -- pose gradient through every tracked object's network and an
-// on-device Adam / Exp pose optimiser.  CUDA-core fp32 for the networks (the layout and dense helpers of
-// k_step_fp32.cuh, no weight gradients), fp64 for the pose, the partial sums and the update.
+// on-device Adam / Exp pose optimiser.  CUDA-core fp32 for the networks: K1 fp32's network (NetTile of k_step_fp32.cuh:
+// tile, embedding, forward and input gradients), no weight gradients; fp64 for the pose, the partial sums and the update.
 //
 // The rule (oracle/track_oracle.py restates it).  The parts K11 (k_ba.cuh) and the layer-wise path (k_track_lw.cuh)
-// share are written once below, as the helpers ba_draw_frame, slice_mask_count, pose_point, ray_loss, pose_terms and
-// pose_adam_exp; each kernel keeps only its own reductions.
+// share are written once below, as the helpers ba_draw_frame, pose_point, ray_loss, pose_terms and pose_adam_exp, with
+// the mask counts of k_step_fp32.cuh (slice_mask_count); each kernel keeps only its own reductions.
 //   Pose     camera-to-world T_wc = [R | t] (the reference's twc), fp64 [4][4] row-major in device memory.
 //   Samples  each tracked object samples the frame once in the camera frame (K3's camera_frame mode: the points of an
 //            IDENTITY pose; one keyframe: the new frame's slot and the object's 2-D box from this frame's ingest; the
@@ -97,14 +97,6 @@ __device__ __forceinline__ int ba_draw_frame(const int* kf_draw, long long kf_dr
   return (f >= 0 && f < n_poses) ? f : -1;
 }
 
-// the slice's mask counts (loss.py:16-18,38), one ray's increment: depth (mask and object), object, not-unknown
-__device__ __forceinline__ void slice_mask_count(const unsigned char* sem, const unsigned char* mask, int r, int& nd,
-                                                 int& no, int& ns) {
-  const int s = sem[r];
-  const int mo = s != 0;
-  nd += (mask[r] != 0) & mo; no += mo; ns += s != 2;
-}
-
 // the network input of camera-frame point q: p = R q + t in fp32 from an fp32 copy of the fp64 pose T, then p / scale
 __device__ __forceinline__ float3 pose_point(const double* T, float3 q, float sc) {
   const float x = fmaf((float)T[2], q.z, fmaf((float)T[1], q.y, (float)T[0] * q.x)) + (float)T[3];
@@ -153,44 +145,28 @@ __device__ __forceinline__ RayLoss ray_loss(double D, double O, double C0, doubl
   return r;
 }
 
-// One CTA (128 threads) = one tile of nr = TP / S whole rays of one tracked object (blockIdx.y), as k_step_fp32.
+// One CTA = one tile of whole rays of one tracked object (blockIdx.y): NetTile's tile, embedding, forward and input
+// gradients (k_step_fp32.cuh), so the pose gradient is that of the network K1 fp32 trains.
 // BA = false is K10 (one pose, per-CTA partials); BA = true is K11 (a pose per ray, per-ray rows).
 template <int H, int TP, bool BA>
 __device__ __forceinline__ void track_step_body(const TrackParams& a, const VmbLayout& L, const BaRays& x) {
-  constexpr int NT = 128;
-  constexpr int PT = TP + 1;
-  constexpr int NOG = NT / TP;
-  constexpr int OPT = H / NOG;
-  constexpr int OB = 8;
-  static_assert(OPT % OB == 0, "feature split must be a multiple of the register block");
-
+  using Net = NetTile<H, TP>;
+  constexpr int NT = Net::NT, PT = Net::PT, NOG = Net::NOG, OB = Net::OB;
   extern __shared__ float sm[];
-  float* sE = sm;                         // [E][PT] rows 0..2 = p/scale, then sin features
-  float* sA1 = sE + L.E * PT;             // fc1 / dY1
-  float* sA2 = sA1 + H * PT;              // fc2 / dY2
-  float* sA3 = sA2 + H * PT;              // fc3 / dY3
-  float* sA4 = sA3 + H * PT;              // fc4 / dY4
-  float* sAC = sA4 + H * PT;              // colour hidden / dYc
-  float* sHd = sAC + H * PT;              // 12 rows: alpha, col0..2, d_araw, d_rc0..2, z, occ, T, w; then dt partials
+  const Net net(sm, L, a.S, a.R);         // net.sHd's 12 rows are followed by the dt partials
   __shared__ double s_g[6][TP];           // per-point pose-gradient terms
   __shared__ double s_l[3][TP];           // per-ray loss terms
   __shared__ int s_cnt[3][NT / 32];
 
   const int tid = threadIdx.x;
-  const int p = tid % TP, og = tid / TP;
   const int b = blockIdx.y;
   const int S = a.S, R = a.R;
-  const int nr = TP / S;
-  const int np = nr * S;
-  const int r0 = blockIdx.x * nr;
-  const int rl = p / S, sidx = p - rl * S;
-  const bool pvalid = (p < np) && (r0 + rl < R);
   double* part = a.partials + ((size_t)b * gridDim.x + blockIdx.x) * VMB_TRACK_PART;
   const int row = a.rows[b];
   if (row < 0 || row >= a.n_rows) {                   // uniform over the CTA
     if constexpr (BA) {
-      if (tid < nr && r0 + tid < R)
-        for (int c = 0; c < VMB_TRACK_PART; ++c) x.rows[((size_t)b * R + r0 + tid) * VMB_TRACK_PART + c] = 0.0;
+      if (tid < net.nr && net.r0 + tid < R)
+        for (int c = 0; c < VMB_TRACK_PART; ++c) x.rows[((size_t)b * R + net.r0 + tid) * VMB_TRACK_PART + c] = 0.0;
     } else if (tid < VMB_TRACK_PART) {
       part[tid] = 0.0;
     }
@@ -198,7 +174,6 @@ __device__ __forceinline__ void track_step_body(const TrackParams& a, const VmbL
     return;
   }
   const float* __restrict__ P = a.params + (size_t)row * L.stride;
-  const int o_lo = og * OPT;
 
   // ---- per-object mask counts of this slice (loss.py:16-18,38): every CTA of the object counts the same rays --------
   {
@@ -206,129 +181,54 @@ __device__ __forceinline__ void track_step_body(const TrackParams& a, const VmbL
     const unsigned char* mv = a.mask + (size_t)b * a.mask_stride;
     int nd = 0, no = 0, ns = 0;
     for (int r = tid; r < R; r += NT) slice_mask_count(sv, mv, r, nd, no, ns);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      nd += __shfl_xor_sync(0xffffffffu, nd, o);
-      no += __shfl_xor_sync(0xffffffffu, no, o);
-      ns += __shfl_xor_sync(0xffffffffu, ns, o);
-    }
-    if ((tid & 31) == 0) { s_cnt[0][tid >> 5] = nd; s_cnt[1][tid >> 5] = no; s_cnt[2][tid >> 5] = ns; }
+    warp_mask_counts(tid, nd, no, ns, s_cnt);
   }
 
   // ---- A: point p = R q + t (fp32 copy of the fp64 pose), positional embedding of p / scale ---------------------------
   const double* T = a.pose;
-  bool pok = pvalid;                                  // K11: the ray's frame is in the pose table
+  bool pok = net.pvalid;                              // K11: the ray's frame is in the pose table
   if constexpr (BA) {
-    const int f = pvalid ? ba_draw_frame(x.kf_draw, x.kf_draw_stride, x.kf_frame, x.kf_stride, x.n_poses, b,
-                                         (r0 + rl) / x.n_pix_draw) : -1;
+    const int f = net.pvalid ? ba_draw_frame(x.kf_draw, x.kf_draw_stride, x.kf_frame, x.kf_stride, x.n_poses, b,
+                                             (net.r0 + net.rl) / x.n_pix_draw) : -1;
     pok = f >= 0;
     T = a.pose + (size_t)(pok ? f : 0) * 16;
   }
   float3 q = make_float3(0.f, 0.f, 0.f), t = q;
   const float sc = a.scale[row];
   if (pok) {
-    const size_t gi = (size_t)b * a.pcs_stride + ((size_t)(r0 + rl) * S + sidx) * 3;
+    const size_t gi = (size_t)b * a.pcs_stride + ((size_t)(net.r0 + net.rl) * S + net.sidx) * 3;
     q = make_float3(a.pcs[gi], a.pcs[gi + 1], a.pcs[gi + 2]);
     t = pose_point(T, q, sc);
   }
-  if (og == 0) {
-    sE[0 * PT + p] = t.x; sE[1 * PT + p] = t.y; sE[2 * PT + p] = t.z;
-    sHd[8 * PT + p] = pvalid ? a.z[(size_t)b * a.z_stride + (size_t)(r0 + rl) * S + sidx] : 0.f;
-    sHd[4 * PT + p] = 0.f; sHd[5 * PT + p] = 0.f; sHd[6 * PT + p] = 0.f; sHd[7 * PT + p] = 0.f;
+  if (net.og == 0) {
+    net.sE[0 * PT + net.p] = t.x; net.sE[1 * PT + net.p] = t.y; net.sE[2 * PT + net.p] = t.z;
+    net.sHd[8 * PT + net.p] = net.pvalid ? a.z[(size_t)b * a.z_stride + (size_t)(net.r0 + net.rl) * S + net.sidx] : 0.f;
+    net.sHd[4 * PT + net.p] = 0.f; net.sHd[5 * PT + net.p] = 0.f; net.sHd[6 * PT + net.p] = 0.f; net.sHd[7 * PT + net.p] = 0.f;
   }
-  for (int d = og; d < VMB_NDIRS; d += NOG) {
-    const float* Bd = P + L.o_B + d * 3;
-    const float proj = fmaf(__ldg(Bd + 2), t.z, fmaf(__ldg(Bd + 1), t.y, __ldg(Bd) * t.x));
-    for (int k = 0; k < L.nfreq; ++k) sE[(3 + k * VMB_NDIRS + d) * PT + p] = sinf((proj * (float)(1 << k)) * VMB_PI_F);
-  }
-  __syncthreads();
+  net.embed(P, L, t);
 
-  // ---- B: MLP forward (model.py:54-85), as k_step_fp32 ------------------------------------------------------------
-  for (int o = o_lo; o < o_lo + OPT; o += OB) {
-    float acc[OB];
-#pragma unroll
-    for (int j = 0; j < OB; ++j) acc[j] = __ldg(P + L.o_bin + o + j);
-    fwd_block<OB>(acc, P + L.o_Win + o * VMB_E1, VMB_E1, sE + p, VMB_E1, PT);
-#pragma unroll
-    for (int j = 0; j < OB; ++j) sA1[(o + j) * PT + p] = fmaxf(acc[j], 0.f);
-  }
-  __syncthreads();
-  for (int o = o_lo; o < o_lo + OPT; o += OB) {
-    float acc[OB];
-#pragma unroll
-    for (int j = 0; j < OB; ++j) acc[j] = __ldg(P + L.o_bm1 + o + j);
-    fwd_block<OB>(acc, P + L.o_Wm1 + o * H, H, sA1 + p, H, PT);
-#pragma unroll
-    for (int j = 0; j < OB; ++j) sA2[(o + j) * PT + p] = fmaxf(acc[j], 0.f);
-  }
-  __syncthreads();
-  {
-    const int ld = H + VMB_E1;
-    for (int o = o_lo; o < o_lo + OPT; o += OB) {
-      float acc[OB];
-#pragma unroll
-      for (int j = 0; j < OB; ++j) acc[j] = __ldg(P + L.o_bcat + o + j);
-      fwd_block<OB>(acc, P + L.o_Wcat + o * ld, ld, sA2 + p, H, PT);
-      fwd_block<OB>(acc, P + L.o_Wcat + o * ld + H, ld, sE + p, VMB_E1, PT);
-#pragma unroll
-      for (int j = 0; j < OB; ++j) sA3[(o + j) * PT + p] = fmaxf(acc[j], 0.f);
-    }
-  }
-  __syncthreads();
-  for (int o = o_lo; o < o_lo + OPT; o += OB) {
-    float acc[OB];
-#pragma unroll
-    for (int j = 0; j < OB; ++j) acc[j] = __ldg(P + L.o_bm2 + o + j);
-    fwd_block<OB>(acc, P + L.o_Wm2 + o * H, H, sA3 + p, H, PT);
-#pragma unroll
-    for (int j = 0; j < OB; ++j) sA4[(o + j) * PT + p] = fmaxf(acc[j], 0.f);
-  }
-  __syncthreads();
-  {
-    const int ld = H + L.e2;
-    for (int o = o_lo; o < o_lo + OPT; o += OB) {
-      float acc[OB];
-#pragma unroll
-      for (int j = 0; j < OB; ++j) acc[j] = __ldg(P + L.o_bcl + o + j);
-      fwd_block<OB>(acc, P + L.o_Wcl + o * ld, ld, sA4 + p, H, PT);
-      fwd_block<OB>(acc, P + L.o_Wcl + o * ld + H, ld, sE + VMB_E1 * PT + p, L.e2, PT);
-#pragma unroll
-      for (int j = 0; j < OB; ++j) sAC[(o + j) * PT + p] = fmaxf(acc[j], 0.f);
-    }
-    if (og == 0) {
-      float acc1[1] = {__ldg(P + L.o_ba)};
-      fwd_block<1>(acc1, P + L.o_Wa, H, sA4 + p, H, PT);
-      sHd[0 * PT + p] = acc1[0] * 10.0f;                    // model.py:77
-    }
-  }
-  __syncthreads();
-  if (og == 0) {
-    float acc3[3] = {__ldg(P + L.o_boc), __ldg(P + L.o_boc + 1), __ldg(P + L.o_boc + 2)};
-    fwd_block<3>(acc3, P + L.o_Woc, H, sAC + p, H, PT);
-#pragma unroll
-    for (int c = 0; c < 3; ++c) sHd[(1 + c) * PT + p] = vmb_sigmoid(acc3[c]);
-  }
-  __syncthreads();
+  // ---- B: MLP forward (model.py:54-85) -------------------------------------------------------------------------------
+  net.forward(P, L);
 
   // ---- C: render + loss + d(loss)/d(alpha, colour), per-object per-term empty-mask rule ------------------------------
   if (tid < TP) { s_l[0][tid] = 0.0; s_l[1][tid] = 0.0; s_l[2][tid] = 0.0; }
-  if (tid < nr && r0 + tid < R) {            // per-ray sums in fp64: depth and variance cancel when a ray's weight
-    const int ray = r0 + tid;                 // sits on one sample, and the depth weight 1/(sqrt(var)+1e-4) amplifies it
+  if (tid < net.nr && net.r0 + tid < R) {    // per-ray sums in fp64: depth and variance cancel when a ray's weight
+    const int ray = net.r0 + tid;             // sits on one sample, and the depth weight 1/(sqrt(var)+1e-4) amplifies it
     const int pb = tid * S;
     double Tr = 1.0, D = 0.0, O = 0.0, C0 = 0.0, C1 = 0.0, C2 = 0.0;
     for (int s = 0; s < S; ++s) {
       const int qi = pb + s;
-      const float occ = vmb_sigmoid(sHd[0 * PT + qi]);      // render_rays.py:6
+      const float occ = vmb_sigmoid(net.sHd[0 * PT + qi]);  // render_rays.py:6
       const double w = (double)occ * Tr;                    // render_rays.py:34
-      sHd[9 * PT + qi] = occ; sHd[10 * PT + qi] = (float)Tr; sHd[11 * PT + qi] = (float)w;
-      D += w * (double)sHd[8 * PT + qi]; O += w;
-      C0 += w * (double)sHd[1 * PT + qi]; C1 += w * (double)sHd[2 * PT + qi]; C2 += w * (double)sHd[3 * PT + qi];
-      Tr *= ((double)vmb_sigmoid(-sHd[0 * PT + qi]) + 1e-10);   // render_rays.py:29 with 1 - occ as sigmoid(-alpha):
+      net.sHd[9 * PT + qi] = occ; net.sHd[10 * PT + qi] = (float)Tr; net.sHd[11 * PT + qi] = (float)w;
+      D += w * (double)net.sHd[8 * PT + qi]; O += w;
+      C0 += w * (double)net.sHd[1 * PT + qi]; C1 += w * (double)net.sHd[2 * PT + qi]; C2 += w * (double)net.sHd[3 * PT + qi];
+      Tr *= ((double)vmb_sigmoid(-net.sHd[0 * PT + qi]) + 1e-10);  // render_rays.py:29, 1 - occ as sigmoid(-alpha):
     }                                                       // no cancellation where occ rounds to 1 in fp32
     double V = 0.0;
     for (int s = 0; s < S; ++s) {
-      const double dz = (double)sHd[8 * PT + pb + s] - D;
-      V += (double)sHd[11 * PT + pb + s] * dz * dz;         // loss.py:28-29 (detached)
+      const double dz = (double)net.sHd[8 * PT + pb + s] - D;
+      V += (double)net.sHd[11 * PT + pb + s] * dz * dz;     // loss.py:28-29 (detached)
     }
     int cnt[3];
 #pragma unroll
@@ -347,106 +247,68 @@ __device__ __forceinline__ void track_step_body(const TrackParams& a, const VmbL
     float suffix = 0.f;
     for (int s = S - 1; s >= 0; --s) {
       const int qi = pb + s;
-      const float occ = sHd[9 * PT + qi], Ts = sHd[10 * PT + qi], w = sHd[11 * PT + qi];
-      const float c0 = sHd[1 * PT + qi], c1 = sHd[2 * PT + qi], c2 = sHd[3 * PT + qi];
-      const float Gs = fmaf(gD, sHd[8 * PT + qi], fmaf(gC0, c0, fmaf(gC1, c1, fmaf(gC2, c2, gO))));
-      const float fr = vmb_sigmoid(-sHd[0 * PT + qi]);     // 1 - occ
+      const float occ = net.sHd[9 * PT + qi], Ts = net.sHd[10 * PT + qi], w = net.sHd[11 * PT + qi];
+      const float c0 = net.sHd[1 * PT + qi], c1 = net.sHd[2 * PT + qi], c2 = net.sHd[3 * PT + qi];
+      const float Gs = fmaf(gD, net.sHd[8 * PT + qi], fmaf(gC0, c0, fmaf(gC1, c1, fmaf(gC2, c2, gO))));
+      const float fr = vmb_sigmoid(-net.sHd[0 * PT + qi]); // 1 - occ
       const float f = fr + 1e-10f;
       const float docc = Gs * Ts - suffix / f;
-      sHd[4 * PT + qi] = 10.0f * docc * occ * fr;
-      sHd[5 * PT + qi] = gC0 * w * c0 * (1.f - c0);
-      sHd[6 * PT + qi] = gC1 * w * c1 * (1.f - c1);
-      sHd[7 * PT + qi] = gC2 * w * c2 * (1.f - c2);
+      net.sHd[4 * PT + qi] = 10.0f * docc * occ * fr;
+      net.sHd[5 * PT + qi] = gC0 * w * c0 * (1.f - c0);
+      net.sHd[6 * PT + qi] = gC1 * w * c1 * (1.f - c1);
+      net.sHd[7 * PT + qi] = gC2 * w * c2 * (1.f - c2);
       suffix = fmaf(Gs, w, suffix);
     }
   }
   __syncthreads();
 
   // ---- D: backward to the inputs only (no weight gradients) ----------------------------------------------------------
-  for (int o = o_lo; o < o_lo + OPT; ++o) {                 // dYc = relu'(hc) * (d_rawc @ W_oc)
-    float v = sHd[5 * PT + p] * __ldg(P + L.o_Woc + o);
-    v = fmaf(sHd[6 * PT + p], __ldg(P + L.o_Woc + H + o), v);
-    v = fmaf(sHd[7 * PT + p], __ldg(P + L.o_Woc + 2 * H + o), v);
-    sAC[o * PT + p] = (sAC[o * PT + p] > 0.f) ? v : 0.f;
-  }
-  __syncthreads();
-  {                                                         // dY4 = relu'(fc4) * (dYc @ W_cl[:, :H] + d_araw * W_a)
-    const int ld = H + L.e2;
-    for (int k = o_lo; k < o_lo + OPT; k += OB) {
-      float acc[OB];
-      const float da = sHd[4 * PT + p];
-#pragma unroll
-      for (int j = 0; j < OB; ++j) acc[j] = da * __ldg(P + L.o_Wa + k + j);
-      dgrad_block<OB>(acc, P + L.o_Wcl + k, ld, sAC + p, H, PT);
-#pragma unroll
-      for (int j = 0; j < OB; ++j) sA4[(k + j) * PT + p] = (sA4[(k + j) * PT + p] > 0.f) ? acc[j] : 0.f;
-    }
-  }
-  __syncthreads();
-  for (int k = o_lo; k < o_lo + OPT; k += OB) {             // dY3
-    float acc[OB];
-#pragma unroll
-    for (int j = 0; j < OB; ++j) acc[j] = 0.f;
-    dgrad_block<OB>(acc, P + L.o_Wm2 + k, H, sA4 + p, H, PT);
-#pragma unroll
-    for (int j = 0; j < OB; ++j) sA3[(k + j) * PT + p] = (sA3[(k + j) * PT + p] > 0.f) ? acc[j] : 0.f;
-  }
-  __syncthreads();
-  for (int k = o_lo; k < o_lo + OPT; k += OB) {             // dY2
-    float acc[OB];
-#pragma unroll
-    for (int j = 0; j < OB; ++j) acc[j] = 0.f;
-    dgrad_block<OB>(acc, P + L.o_Wcat + k, H + VMB_E1, sA3 + p, H, PT);
-#pragma unroll
-    for (int j = 0; j < OB; ++j) sA2[(k + j) * PT + p] = (sA2[(k + j) * PT + p] > 0.f) ? acc[j] : 0.f;
-  }
-  __syncthreads();
-  for (int k = o_lo; k < o_lo + OPT; k += OB) {             // dY1
-    float acc[OB];
-#pragma unroll
-    for (int j = 0; j < OB; ++j) acc[j] = 0.f;
-    dgrad_block<OB>(acc, P + L.o_Wm1 + k, H, sA2 + p, H, PT);
-#pragma unroll
-    for (int j = 0; j < OB; ++j) sA1[(k + j) * PT + p] = (sA1[(k + j) * PT + p] > 0.f) ? acc[j] : 0.f;
-  }
-  __syncthreads();
+  net.dyc(P, L);
+  net.dy4(P, L);
+  net.dgrad(net.sA3, net.sA4, P + L.o_Wm2, H);                                // dY3
+  net.dgrad(net.sA2, net.sA3, P + L.o_Wcat, H + VMB_E1);                      // dY2
+  net.dgrad(net.sA1, net.sA2, P + L.o_Wm1, H);                                // dY1
 
   // d(loss)/d(t): embedding rows in blocks of OB, rows [0, 87) through in_layer + cat_layer, [87, E) through color_linear
   {
     float dt[3] = {0.f, 0.f, 0.f};
     const int nb1 = (VMB_E1 + OB - 1) / OB, nb2 = (L.e2 + OB - 1) / OB;
     const int ldc = H + VMB_E1, ldl = H + L.e2;
-    for (int blk = og; blk < nb1 + nb2; blk += NOG) {
+    for (int blk = net.og; blk < nb1 + nb2; blk += NOG) {
       float acc[OB];
 #pragma unroll
       for (int j = 0; j < OB; ++j) acc[j] = 0.f;
       if (blk < nb1) {
         const int j0 = blk * OB;
-        dgrad_block<OB>(acc, P + L.o_Win + j0, VMB_E1, sA1 + p, H, PT);
-        dgrad_block<OB>(acc, P + L.o_Wcat + H + j0, ldc, sA3 + p, H, PT);
+        dgrad_block<OB>(acc, P + L.o_Win + j0, VMB_E1, net.sA1 + net.p, H, PT);
+        dgrad_block<OB>(acc, P + L.o_Wcat + H + j0, ldc, net.sA3 + net.p, H, PT);
         pe_input_grad<OB>(acc, j0, VMB_E1, P + L.o_B, t.x, t.y, t.z, dt);
       } else {
         const int j0 = (blk - nb1) * OB;
-        dgrad_block<OB>(acc, P + L.o_Wcl + H + j0, ldl, sAC + p, H, PT);
+        dgrad_block<OB>(acc, P + L.o_Wcl + H + j0, ldl, net.sAC + net.p, H, PT);
         pe_input_grad<OB>(acc, VMB_E1 + j0, L.E, P + L.o_B, t.x, t.y, t.z, dt);
       }
     }
-    sHd[(og * 3 + 0) * PT + p] = dt[0]; sHd[(og * 3 + 1) * PT + p] = dt[1]; sHd[(og * 3 + 2) * PT + p] = dt[2];
+    net.sHd[(net.og * 3 + 0) * PT + net.p] = dt[0];
+    net.sHd[(net.og * 3 + 1) * PT + net.p] = dt[1];
+    net.sHd[(net.og * 3 + 2) * PT + net.p] = dt[2];
   }
   __syncthreads();
-  if (og == 0) {
+  if (net.og == 0) {
     float d0 = 0.f, d1 = 0.f, d2 = 0.f;
 #pragma unroll
-    for (int g = 0; g < NOG; ++g) { d0 += sHd[(g * 3) * PT + p]; d1 += sHd[(g * 3 + 1) * PT + p]; d2 += sHd[(g * 3 + 2) * PT + p]; }
+    for (int g = 0; g < NOG; ++g) {
+      d0 += net.sHd[(g * 3) * PT + net.p]; d1 += net.sHd[(g * 3 + 1) * PT + net.p]; d2 += net.sHd[(g * 3 + 2) * PT + net.p];
+    }
     double c[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
     if (pok) pose_terms(T, make_double3(q.x, q.y, q.z), make_float3(d0, d1, d2), sc, c);
 #pragma unroll
-    for (int i = 0; i < 6; ++i) s_g[i][p] = c[i];
+    for (int i = 0; i < 6; ++i) s_g[i][net.p] = c[i];
   }
   __syncthreads();
   if constexpr (BA) {                                       // per-ray rows: the ray's samples in order
-    if (tid < nr && r0 + tid < R) {
-      double* out = x.rows + ((size_t)b * R + r0 + tid) * VMB_TRACK_PART;
+    if (tid < net.nr && net.r0 + tid < R) {
+      double* out = x.rows + ((size_t)b * R + net.r0 + tid) * VMB_TRACK_PART;
       for (int c = 0; c < 6; ++c) {
         double s = 0.0;
         for (int i = 0; i < S; ++i) s += s_g[c][tid * S + i];
@@ -456,11 +318,11 @@ __device__ __forceinline__ void track_step_body(const TrackParams& a, const VmbL
     }
   } else if (tid < 6) {
     double s = 0.0;
-    for (int i = 0; i < np; ++i) s += s_g[tid][i];
+    for (int i = 0; i < net.np; ++i) s += s_g[tid][i];
     part[tid] = s;
   } else if (tid < 9) {
     double s = 0.0;
-    for (int i = 0; i < nr; ++i) s += s_l[tid - 6][i];
+    for (int i = 0; i < net.nr; ++i) s += s_l[tid - 6][i];
     part[tid] = s;
   } else if (tid == 9) {
     part[9] = 0.0;
@@ -470,21 +332,6 @@ __device__ __forceinline__ void track_step_body(const TrackParams& a, const VmbL
 template <int H, int TP>
 __global__ void __launch_bounds__(128, 1) k_track_step(TrackParams a, VmbLayout L) {
   track_step_body<H, TP, false>(a, L, BaRays{});
-}
-
-template <int H, int TP>
-static size_t track_smem(const VmbLayout& L) {
-  return sizeof(float) * (size_t)(L.E + 5 * H + 12) * (TP + 1);
-}
-
-// host: raise kernel K's dynamic shared-memory limit to `bytes` on device `dev`, the first time only
-template <auto K>
-static cudaError_t pose_smem_limit(int dev, int bytes) {
-  static bool set[64] = {};      // per device (one process may drive several GPUs)
-  if (set[dev & 63]) return cudaSuccess;
-  const cudaError_t e = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) set[dev & 63] = true;
-  return e;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

@@ -4,8 +4,8 @@
 // The rule is K10's (k_track.cuh) and, for the BA flavour, K11's (k_ba.cuh): same samples, same points, same loss with
 // the per-object, per-term empty-mask rule, same left-perturbation gradient, same output rows, so vmb_track_update and
 // vmb_ba_update run unchanged on what this path writes.  The parts that do not depend on where the network runs are
-// the helpers of k_track.cuh that K10 and K11 call too: ba_draw_frame, slice_mask_count, pose_point, ray_loss and
-// pose_terms.  What differs is where the network runs and its precision:
+// the helpers that K10 and K11 call too: ba_draw_frame, pose_point, ray_loss and pose_terms of k_track.cuh and
+// slice_mask_count of k_step_fp32.cuh.  What differs is where the network runs and its precision:
 //   Weights  object b reads params row rows[b] and the fp16 image row rows[b] (as the AdamW launch writes it).  Both
 //            are copied on the device into this path's workspace first, so rows[] stays a device array (capturable);
 //            a row outside [0, n_rows) contributes nothing and sets VMB_TRACK_ST_BAD_ROW, as K10.
@@ -402,7 +402,7 @@ static int track_object_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGrou
   TLW_TRY(forward_gemms<H>(ws, L, tw.prow, tw.wimg, np, pdl_ok, st));
   int dev = 0;
   cudaGetDevice(&dev);
-  TLW_TRY((pose_smem_limit<k_tlw_render<H, BA>>(dev, hr_smem<H>())));
+  TLW_TRY((smem_limit_once<k_tlw_render<H, BA>>(dev, hr_smem<H>())));
   TlwRender ra;
   ra.z = a.z + (size_t)b * a.z_stride; ra.gt_depth = a.gt_depth + (size_t)b * a.gt_depth_stride;
   ra.gt_colour = a.gt_colour + (size_t)b * a.gt_colour_stride; ra.sem = sem; ra.mask = mask; ra.cs = a.cs; ra.os = a.os;
@@ -424,7 +424,7 @@ static int track_object_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGrou
   TLW_TRY(dgrad_gate_gemm<H>(ws.dYa, tw.wimg, off_m1(H), H, np, ws.X1, ws.dYc, nullptr, nullptr, st));    // dY1 -> dYc
   arm();
   TLW_TRY(demb1_gemm<H>(ws, ws.dYb, ws.dYc, tw.wimg, np, st));                                           // d emb1
-  TLW_TRY(pose_smem_limit<k_tlw_pose<BA>>(dev, PEB_SMEM));
+  TLW_TRY(smem_limit_once<k_tlw_pose<BA>>(dev, PEB_SMEM));
   arm();
   TLW_TRY(launch_k(k_tlw_pose<BA>, dim3(nblk), dim3(128), (size_t)PEB_SMEM, st, o, (const float*)tw.prow, (const int*)tw.ctl, L.o_B,
                    (const float*)ws.dE, tw.gpt));
@@ -580,7 +580,7 @@ static int joint_object_lw(Workspace& ws, JointWorkspace& jw, const VmbLayout& L
   if (rc) return rc;
   int dev = 0;
   cudaGetDevice(&dev);
-  TLW_TRY(pose_smem_limit<k_tlw_pose<true>>(dev, PEB_SMEM));
+  TLW_TRY(smem_limit_once<k_tlw_pose<true>>(dev, PEB_SMEM));
   // after step_object's join with its side stream: an ordinary launch
   TLW_TRY(launch_k(k_tlw_pose<true>, dim3((unsigned)((np + 127) / 128)), dim3(128), (size_t)PEB_SMEM, st, o,
                    sp.params + (size_t)b * L.stride, (const int*)jw.ctl, L.o_B, (const float*)ws.dE, jw.gpt));

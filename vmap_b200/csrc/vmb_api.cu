@@ -68,14 +68,13 @@ static int fail(vmb_handle* h, int code, const std::string& msg) {
       return fail(h, VMB_E_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e_));      \
   } while (0)
 
+// points per tile (TP) of the CUDA-core fp32 network (NetTile) for hidden size H: K1 fp32, K10 and K11
+static constexpr int fp32_tile(int H) { return H == 32 ? 128 : (H == 256 ? 32 : 64); }
+
 template <int H, int TP>
 static int launch_fp32(vmb_handle* h, const StepParams& sp, long long n_tiles_x, cudaStream_t st) {
-  const size_t smem = step_fp32_smem<H, TP>(h->L);
-  static bool attr_set[64] = {};          // per device (one process may drive several GPUs)
-  if (!attr_set[h->device & 63]) {
-    CUDA_TRY(h, cudaFuncSetAttribute(k_step_fp32<H, TP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set[h->device & 63] = true;
-  }
+  const size_t smem = NetTile<H, TP>::smem(h->L, VMB_NDIRS);    // then the kernel's sDp rows
+  CUDA_TRY(h, (smem_limit_once<k_step_fp32<H, TP>>(h->device, (int)smem)));
   dim3 grid((unsigned)n_tiles_x, (unsigned)sp.B);
   k_step_fp32<H, TP><<<grid, 128, smem, st>>>(sp, h->L);
   CUDA_TRY(h, cudaGetLastError());
@@ -83,16 +82,16 @@ static int launch_fp32(vmb_handle* h, const StepParams& sp, long long n_tiles_x,
 }
 
 static int dispatch_fp32(vmb_handle* h, const StepParams& sp, cudaStream_t st) {
-  const int TP = (h->H == 32) ? 128 : (h->H == 256 ? 32 : 64);
+  const int TP = fp32_tile(h->H);
   if (sp.S > TP) return fail(h, VMB_E_UNSUPPORTED, "fp32 step kernel: n_samples exceeds the tile size for this hidden size");
   const int nr = TP / sp.S;
   const long long tiles = ((long long)sp.R + nr - 1) / nr;
   if (tiles > 0x7fffffffLL || sp.B > 65535) return fail(h, VMB_E_ARG, "grid too large");
   switch (h->H) {
-    case 32:  return launch_fp32<32, 128>(h, sp, tiles, st);
-    case 64:  return launch_fp32<64, 64>(h, sp, tiles, st);
-    case 128: return launch_fp32<128, 64>(h, sp, tiles, st);
-    case 256: return launch_fp32<256, 32>(h, sp, tiles, st);
+    case 32:  return launch_fp32<32, fp32_tile(32)>(h, sp, tiles, st);
+    case 64:  return launch_fp32<64, fp32_tile(64)>(h, sp, tiles, st);
+    case 128: return launch_fp32<128, fp32_tile(128)>(h, sp, tiles, st);
+    case 256: return launch_fp32<256, fp32_tile(256)>(h, sp, tiles, st);
   }
   return fail(h, VMB_E_UNSUPPORTED, "unsupported hidden size");
 }
@@ -1240,17 +1239,15 @@ int vmb_debug_gemm(int a_mn, int b_mn, int epi, int M, int N, int K1, int K2, co
 }  // extern "C"
 
 // ---- K10 / K11 and their layer-wise path: one host path for the four step entry points ------------------------------
-static int track_tile(int hidden) { return hidden == 32 ? 128 : (hidden == 256 ? 32 : 64); }   // as dispatch_fp32
-
 template <int H, int TP, bool BA>
 static int launch_pose(vmb_handle* h, const TrackParams& tp, const BaRays& x, int tiles, cudaStream_t st) {
-  const size_t smem = track_smem<H, TP>(h->L);
+  const size_t smem = NetTile<H, TP>::smem(h->L, 0);
   const dim3 grid((unsigned)tiles, (unsigned)tp.B);
   if constexpr (BA) {
-    CUDA_TRY(h, (pose_smem_limit<k_ba_step<H, TP>>(h->device, (int)smem)));
+    CUDA_TRY(h, (smem_limit_once<k_ba_step<H, TP>>(h->device, (int)smem)));
     k_ba_step<H, TP><<<grid, 128, smem, st>>>(tp, h->L, x);
   } else {
-    CUDA_TRY(h, (pose_smem_limit<k_track_step<H, TP>>(h->device, (int)smem)));
+    CUDA_TRY(h, (smem_limit_once<k_track_step<H, TP>>(h->device, (int)smem)));
     k_track_step<H, TP><<<grid, 128, smem, st>>>(tp, h->L);
   }
   CUDA_TRY(h, cudaGetLastError());
@@ -1345,17 +1342,17 @@ static int pose_step(vmb_handle* h, const Args* a, int group, const void* image,
   }
   cudaStream_t st = (cudaStream_t)stream;
   if constexpr (LW) {
-    const lw::TlwGroup G{tp, x, (const __half*)image, BA ? 1 : track_tile(g.hidden) / g.n_samples};
+    const lw::TlwGroup G{tp, x, (const __half*)image, BA ? 1 : fp32_tile(g.hidden) / g.n_samples};
     std::string err;
     const int rc = lw::launch_track_lw<BA>(BA ? h->ws_ba : h->ws_track, h->L, G, st, err);
     if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, std::string(who) + ": " + err);
     return VMB_OK;
   } else {
     switch (h->H) {
-      case 32:  return launch_pose<32, 128, BA>(h, tp, x, tiles, st);
-      case 64:  return launch_pose<64, 64, BA>(h, tp, x, tiles, st);
-      case 128: return launch_pose<128, 64, BA>(h, tp, x, tiles, st);
-      case 256: return launch_pose<256, 32, BA>(h, tp, x, tiles, st);
+      case 32:  return launch_pose<32, fp32_tile(32), BA>(h, tp, x, tiles, st);
+      case 64:  return launch_pose<64, fp32_tile(64), BA>(h, tp, x, tiles, st);
+      case 128: return launch_pose<128, fp32_tile(128), BA>(h, tp, x, tiles, st);
+      case 256: return launch_pose<256, fp32_tile(256), BA>(h, tp, x, tiles, st);
     }
     return fail(h, VMB_E_UNSUPPORTED, std::string(who) + ": unsupported hidden size");
   }
@@ -1379,7 +1376,7 @@ extern "C" {
 
 int vmb_track_tiles(int hidden, int n_rays, int n_samples) {
   if (!(hidden == 32 || hidden == 64 || hidden == 128 || hidden == 256) || n_rays < 1 || n_samples < 1) return VMB_E_ARG;
-  const int TP = track_tile(hidden);
+  const int TP = fp32_tile(hidden);
   if (n_samples > TP || n_samples > 32) return VMB_E_UNSUPPORTED;
   const int nr = TP / n_samples;
   return (n_rays + nr - 1) / nr;
