@@ -128,10 +128,11 @@ typedef struct vmb_step_args {
 int vmb_step(vmb_handle* h, const vmb_step_args* a, void* stream);
 
 /* Profiling build of vmb_step's fused hidden-32 training step (n_samples 10, impl AUTO / UMMA): the same launch and
- * results, with one thread per warpgroup stamping clock64() at every phase boundary of each tile into `trace`
+ * results, with one thread per warpgroup stamping clock64() at every phase boundary of each tile (and %globaltimer at
+ * kernel entry, last segment, finish start and exit) into `trace`
  * (device, 2 * min(#SMs, 192) rows of VMB_TRACE_STRIDE unsigned 64-bit words, row = 2 * CTA + warpgroup; the row
  * layout is described at uf::TR_STRIDE in k_step_fused.cuh).  For tools/step_phase_time.py.                         */
-#define VMB_TRACE_STRIDE (8 + 64 * 20)
+#define VMB_TRACE_STRIDE (16 + 64 * 20)
 int vmb_step_trace(vmb_handle* h, const vmb_step_args* a, unsigned long long* trace, long long trace_words, void* stream);
 
 /* Mask counts only (the normalisers of render_rays.py:68,86): out[B][4] int.

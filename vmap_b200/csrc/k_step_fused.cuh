@@ -22,10 +22,17 @@
 //     (dYc->Z, dY4->HC, dY3->FC4, dY2->HC, dY1->FC3);
 //   * both head weight gradients and both head bias gradients come out of ONE wgrad ([fc4 | emb2 | hc] x dhead);
 //   * the PE-direction gradient dB = dproj^T [x y z] is a wgrad MMA too;
-//   * K0 (mask counts) runs in the prologue, K2 (AdamW) after a grid barrier: every (CTA, object) segment writes its
-//     gradient partial to its own row, then the whole grid splits the reduction of all objects' rows, adds each
-//     object's rows in segment order (bitwise reproducible -- no floating-point atomics anywhere) and applies AdamW
-//     exactly as k_adamw does.  Training launches are cooperative: the grid barrier needs every CTA resident.
+//   * K0 (mask counts) runs in the prologue, K2 (AdamW) per object as soon as the object is complete: every (CTA,
+//     object) segment writes its gradient partial to its own row and then counts itself into the object's readiness
+//     word.  A CTA that has run all its tiles claims finish chunks (object, float4 column range; object order) from a
+//     ticket counter, issues the chunk's p / m / v loads, waits for the object's readiness word to reach its segment
+//     count, adds the object's rows in segment order (bitwise reproducible whichever CTA runs the chunk -- no
+//     floating-point atomics anywhere) and applies AdamW exactly as k_adamw does.  Training launches are cooperative:
+//     a waiting CTA needs every CTA that still runs tiles resident.
+//   * Updating an object while other CTAs still run tiles is safe because no CTA loads object b's weight image (its
+//     only read of b's parameters) once all of b's segments have flushed: a CTA's copy of b's image completes before
+//     its first tile of b, which is before its segment of b flushes.  The finish writes p / m / v and the image of b
+//     only after all of b's segments are counted.
 //
 // Reference arithmetic: embedding.py:82-91, model.py:54-85, render_rays.py:4-96, loss.py:5-62, their autograd
 // backward (train.py:293-324) and torch.optim.AdamW.step + zero_grad (train.py:325-326).
@@ -39,11 +46,12 @@
 
 struct FusedExtra {
   float* partials;            // [(B + grid)][stride] per-(CTA, object) gradient partials, row = blockIdx + object
-  unsigned int* finish_sync;  // [6] grid-barrier words (self-resetting), then [B] skip flags: the words' place must not
-                              // depend on B, or a launch with fewer objects would find a skip flag in them
+  unsigned int* finish_sync;  // [SY_OBJ + 2 * B] sync words (uf::SY_*), all but the skip flags re-armed by the last CTA
+                              // to leave: an object's words sit at the same place whatever B is, so a launch with
+                              // more objects never finds a skip flag in a readiness counter
   const int* counts_in;       // optional [B][4] external mask counts (ray-sharded iMAP: all-reduced by the caller)
   int* counts_pub;            // [B][4] scratch: otherwise CTA c counts objects c, c + grid, ... ONCE and publishes here
-  int fuse_adam;              // 1: the grid-wide finish applies AdamW; 0: it adds the reduced gradient into `grads`
+  int fuse_adam;              // 1: the finish applies AdamW; 0: it adds the reduced gradient into `grads`
   float* p; float* m; float* v;
   __half* image_out; const int* img_index; int img_halves;
   int* step_counter;          // optional [B] device step numbers (t = counter + 1, incremented here)
@@ -75,13 +83,15 @@ constexpr int SM_ACT0 = 0, SM_EG = ACT_BYTES, SM_W = SM_EG + EG_BYTES, SM_HD = S
 constexpr int MISC_BYTES = 512;
 constexpr int SM_CNT = SM_MISC + MISC_BYTES;                      // int [B][3] mask counts
 constexpr int SMEM_MAX = 232448;                                  // 227 KB: the most one block may have on sm_90
-constexpr int MAX_OBJ_SMEM = (SMEM_MAX - SM_CNT) / 12;            // objects whose counts fit
+constexpr int SMEM_SLACK = 16;                                   // the launch's dynamic shared memory: SM_CNT + 12 B + slack
+constexpr int MAX_OBJ_SMEM = (SMEM_MAX - SM_CNT - SMEM_SLACK) / 12;   // objects whose counts fit
 constexpr float LS = um::LS, INV_LS = um::INV_LS;
 
 struct Misc {
   uint64_t wbar;
   int on[3];
-  int fin, skip;
+  int fin;
+  unsigned int ticket[2];      // finish: the chunk claimed for this round and the next
   float step_size, bc2_sqrt;
   float lsum[4][4];
 };
@@ -162,22 +172,32 @@ struct Mma {
   }
 };
 
-// Work partition: CTA c owns tile pairs [begin[c], begin[c+1]) of the global list (object-major).  Built on the host
-// (fused_partition) so that a CTA whose range crosses an object boundary -- it pays a second flush / weight load /
-// pipeline fill -- gets correspondingly fewer pairs: no CTA's cost exceeds the even share by more than one pair.
+// Work partition: CTA c owns tiles [begin[c], begin[c+1]) of the global list (object-major).  Built on the host
+// (fused_partition): a CTA whose range crosses an object boundary -- it pays a second flush / weight load / pipeline
+// fill -- gets correspondingly fewer tiles, and the CTAs with the most tiles sit on the last objects.
 constexpr int MAX_CTAS = 192;
+// finish_sync words: [SY_TICKET] next finish chunk, [SY_DEPART] CTAs done, [SY_PUB] objects whose mask counts are
+// published, [SY_EMPTY + 0..2] any-empty flags, then per object b: [SY_OBJ + 2b] segments whose partial row is out,
+// [SY_OBJ + 2b + 1] skip flag (loss guard) of the step
+constexpr int SY_TICKET = 0, SY_DEPART = 1, SY_PUB = 2, SY_EMPTY = 3, SY_OBJ = 6;
 struct Ranges { int begin[MAX_CTAS + 1]; };
 
 // Phase trace (TRACE instantiation only, vmb_step_trace): thread 0 of each warpgroup stamps clock64() into its own
 // row of TR_STRIDE words, row = 2 * CTA + warpgroup.  Header: [0] kernel start, [1] prologue done, [2] last segment
-// done, [3] grid barrier passed, [4] kernel end, [5] tiles run, [6] cycles in segment flushes, [7] segments.  Then
-// TR_NST stamps for each of the first TR_TILES tiles: [0] tile start and [k] the end of phase k (1..18: PE, in_layer,
-// mid1, cat_layer, mid2, color_linear + alpha, out_color, heads transpose, render + loss, d_hc, d_fc4, d_fc3, d_fc2,
-// d_fc1, d_emb, EG store, PE backward, dB).
-constexpr int TR_HDR = 8, TR_NST = 20, TR_TILES = 64, TR_STRIDE = TR_HDR + TR_TILES * TR_NST;
-__device__ __forceinline__ int cta_of_pair(const Ranges& rg, int G, int pair) {        // largest c with begin[c] <= pair
+// done, [3] finish start, [4] kernel end, [5] tiles run, [6] cycles in segment flushes, [7] segments, [8..11]
+// %globaltimer (ns) at [0], [2], [3], [4], and in warpgroup 0's row only: [12] cycles waiting for other CTAs, [13]
+// finish calls.  Then TR_NST stamps for each of the first TR_TILES tiles: [0] tile start and [k] the end of phase k
+// (1..18: PE, in_layer, mid1, cat_layer, mid2, color_linear + alpha, out_color, heads transpose, render + loss, d_hc,
+// d_fc4, d_fc3, d_fc2, d_fc1, d_emb, EG store, PE backward, dB).
+constexpr int TR_HDR = 16, TR_NST = 20, TR_TILES = 64, TR_STRIDE = TR_HDR + TR_TILES * TR_NST;
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ int cta_of_tile(const Ranges& rg, int G, int tile) {        // largest c with begin[c] <= tile
   int lo = 0, hi = G - 1;
-  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (rg.begin[mid] <= pair) lo = mid; else hi = mid - 1; }
+  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (rg.begin[mid] <= tile) lo = mid; else hi = mid - 1; }
   return lo;
 }
 
@@ -190,12 +210,12 @@ __device__ __forceinline__ int cta_of_pair(const Ranges& rg, int G, int pair) { 
 // 12..20) and stores its half to jdt[b][point][hsel][3] (fp32, plain stores); k_joint_rows adds the halves in that
 // order.  jdt is read only under JOINT: the plain instantiations compile to the same SASS as without it.
 // Registers (ptxas -v, sm_90a), no spills: JOINT S = any / 10 / 14: 249 / 249 / 249 (plain: 251 / 251 / 251; TRACE
-// S = 10: 254).
+// S = 10: 252).
 // TRACE (phase-stamped build, S = 10 only): `trace` as uf::TR_STRIDE describes; the other instantiations ignore it and
 // contain no trace code.
 template <int SC, bool JOINT, bool TRACE = false>
 __global__ void __launch_bounds__(uf::NT, 1)
-k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image, const __grid_constant__ uf::Ranges rg, int tpo, int npo, int nr, int rpw,
+k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image, const __grid_constant__ uf::Ranges rg, int tpo, int nr, int rpw,
              float* jdt, unsigned long long* trace) {
   using namespace uf;
   extern __shared__ __align__(1024) unsigned char smem[];
@@ -208,9 +228,12 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
   int tr_t = 0, tr_nseg = 0;
   long long tr_flush = 0, tr_f0 = 0;
   if constexpr (TRACE) tr = trace + (size_t)(2 * blockIdx.x + (tid >> 7)) * TR_STRIDE;
+  long long tr_wait = 0;
+  int tr_calls = 0;
 #define TR_STAMP(slot) do { if constexpr (TRACE) { if (tr_on) tr[slot] = clock64(); } } while (0)
+#define TR_STAMP2(slot, gslot) do { if constexpr (TRACE) { if (tr_on) { tr[slot] = clock64(); tr[gslot] = globaltimer(); } } } while (0)
 #define TR_TILE(k) do { if constexpr (TRACE) { if (tr_on && tr_t < TR_TILES) tr[TR_HDR + tr_t * TR_NST + (k)] = clock64(); } } while (0)
-  TR_STAMP(0);
+  TR_STAMP2(0, 8);
 
   if (tid == 0) {
     ptx::mbar_init(&misc->wbar, 1);
@@ -222,14 +245,14 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
   __syncthreads();
   if (tid == 0 && gt_begin < gt_end) {     // first object's weight image: in flight while the mask counts run
     ptx::mbar_arrive_expect_tx(&misc->wbar, um::IMG_BYTES);
-    ptx::bulk_g2s(smem + SM_W, image + (size_t)(gt_begin / npo) * um::IMG_BYTES, um::IMG_BYTES, &misc->wbar);
+    ptx::bulk_g2s(smem + SM_W, image + (size_t)(gt_begin / tpo) * um::IMG_BYTES, um::IMG_BYTES, &misc->wbar);
   }
   // ---- K0 in the prologue: mask counts of EVERY object (the any-empty early-out couples them, render_rays.py:68-73).
   // Training launch without counts_in: CTA c counts objects c, c + grid, ... ONCE and publishes counts + empty flags +
   // a "published" counter in global memory; every CTA starts its tiles at once and acquires the counts right before
   // its first volume render (thousands of cycles later: the wait is free).  With counts_in, every CTA copies them.
   const bool pub_counts = !x.counts_in && !a.fwd_only;
-  unsigned int* gbar = x.finish_sync;                   // [0] arrive, [1] depart, [2] objects published, [3..5] empty flags
+  unsigned int* gbar = x.finish_sync;                   // words as uf::SY_* describes
   if (pub_counts) {
     for (int b = blockIdx.x; b < a.B; b += G) {
       if (tid < 3) cnt[tid] = 0;
@@ -259,10 +282,10 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       if (tid == 0) {
         for (int k = 0; k < 3; ++k) {
           x.counts_pub[b * 4 + k] = cnt[k];
-          if (cnt[k] == 0) atomicOr(&gbar[3 + k], 1u);
+          if (cnt[k] == 0) atomicOr(&gbar[SY_EMPTY + k], 1u);
         }
         __threadfence();
-        atomicAdd(&gbar[2], 1u);
+        atomicAdd(&gbar[SY_PUB], 1u);
       }
       __syncthreads();
     }
@@ -303,124 +326,11 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
   float w_d = 0.f, w_c = 0.f, w_o = 0.f;
   bool cnt_ready = !pub_counts;       // published counts acquired?
 
-  // Reduce object b's partial rows over float4 columns [i_lo, i_hi) in segment order (the same sum every run) and either
-  // apply AdamW (fuse_adam) or add the reduced gradient into `grads`.  `owner` writes the object's loss terms / status.
-  // Called by all threads of the CTA; returns the object's skip flag (loss explosion guard, render_rays.py:88-90).
-  auto finish_rows = [&](int b, int i_lo, int i_hi, bool owner) -> int {
-    const int c_first = cta_of_pair(rg, G, b * npo), c_last = cta_of_pair(rg, G, (b + 1) * npo - 1);
-    const int nseg = c_last - c_first + 1;
-    const float* P0 = x.partials + (size_t)(c_first + b) * L.stride;
-    const size_t row = (size_t)b * L.stride;
-    const int n4 = L.stride >> 2;
-    const bool upd = a.backward != 0;
-    // (1) the object's loss terms (segment order), the explosion guard and the bias corrections
-    if (warp == 0) {
-      float s = 0.f;
-      if (nseg <= 10) {                                 // up to ten segments are loaded by 30 lanes at once
-        const int k = lane / 3, j = lane - 3 * k;
-        const float v = (k < nseg) ? __ldcg(P0 + (size_t)k * L.stride + L.P + j) : 0.f;
-        for (int kk = 0; kk < nseg; ++kk) s += __shfl_sync(0xffffffffu, v, kk * 3 + (lane < 3 ? lane : 0));
-      } else if (lane < 3) {
-        for (int k = 0; k < nseg; ++k) s += __ldcg(P0 + (size_t)k * L.stride + L.P + lane);
-      }
-      const float l_d = __shfl_sync(0xffffffffu, s, 0), l_c = __shfl_sync(0xffffffffu, s, 1), l_o = __shfl_sync(0xffffffffu, s, 2);
-      if (lane == 0) {
-        const float tot = l_d + a.cs * l_c + a.os * l_o;
-        if (owner) { float* lt = a.loss_terms + b * 4; lt[0] = l_d; lt[1] = l_c; lt[2] = l_o; lt[3] = tot; }
-        int bad = 0;                                    // render_rays.py:88-90: the reference aborts before the update
-        if (x.guard_loss) {
-          if (l_d > 100000.f || l_c > 100000.f || l_o > 100000.f) bad |= 1;
-          if (!(tot == tot) || fabsf(tot) > 3.0e38f) bad |= 2;
-          if (bad && x.status && owner) atomicOr(x.status, bad);
-        }
-        misc->skip = bad;
-        if (x.fuse_adam && x.step_counter) {
-          // bias corrections of step t from the host-built table (torch's double-precision scalars, rounded once);
-          // beyond the table: 1 - beta^t = -expm1(t ln beta) in fp32 (cancellation-free, <= 3e-7 relative)
-          const int t = x.step_counter[b] + 1;
-          if (t < x.bc_n) {
-            const float2 bc = x.bc_table[t];
-            misc->step_size = (float)x.lr / bc.x;
-            misc->bc2_sqrt = bc.y;
-          } else {
-            misc->step_size = (float)x.lr / (-expm1f((float)t * x.log_b1));
-            misc->bc2_sqrt = sqrtf(-expm1f((float)t * x.log_b2));
-          }
-        } else {
-          misc->step_size = x.step_size; misc->bc2_sqrt = x.bc2_sqrt;
-        }
-      }
-    }
-    __syncthreads();
-    const int sk = misc->skip;
-    // (2) reduce + update this CTA's columns (normally at most one float4 column per thread).  Deliberately compact
-    //     code: it runs once per launch out of a cold instruction cache, where instruction fetch, not data, is the cost
-    if (upd && !(sk && x.fuse_adam)) {
-      const float step_size = misc->step_size, bc2_sqrt = misc->bc2_sqrt;
-      for (int c4 = i_lo + tid; c4 < i_hi; c4 += NT) {
-        const float4* src = reinterpret_cast<const float4*>(P0) + c4;
-        float4 pp, mm = make_float4(0.f, 0.f, 0.f, 0.f), vv = mm;
-        if (x.fuse_adam) {
-          pp = *(reinterpret_cast<const float4*>(x.p + row) + c4);
-          mm = *(reinterpret_cast<const float4*>(x.m + row) + c4);
-          vv = *(reinterpret_cast<const float4*>(x.v + row) + c4);
-        } else {
-          pp = *(reinterpret_cast<const float4*>(a.grads + row) + c4);
-        }
-        // segment order = CTA order: the same sum every run; four rows in flight per batch
-        float4 gsum = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 1
-        for (int k0 = 0; k0 < nseg; k0 += 4) {
-          float4 u[4];
-#pragma unroll
-          for (int k = 0; k < 4; ++k) u[k] = (k0 + k < nseg) ? __ldcg(src + (size_t)(k0 + k) * n4) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            if (k0 + k < nseg) { gsum.x += u[k].x; gsum.y += u[k].y; gsum.z += u[k].z; gsum.w += u[k].w; }
-        }
-        const int e = c4 * 4;
-        if (!x.fuse_adam) {
-          float4 o = pp;
-          o.x += gsum.x; o.y += gsum.y; o.z += gsum.z; o.w += gsum.w;
-          if (e + 3 >= L.P) { if (e + 0 >= L.P) o.x = 0.f; if (e + 1 >= L.P) o.y = 0.f; if (e + 2 >= L.P) o.z = 0.f; o.w = 0.f; }
-          *(reinterpret_cast<float4*>(a.grads + row) + c4) = o;
-          continue;
-        }
-        // torch.optim.AdamW._single_tensor_adamw, op for op as k_adamw restates it
-        float* pj = &pp.x; float* mj = &mm.x; float* vj = &vv.x; const float* gj = &gsum.x;
-        __half* img = x.image_out ? x.image_out + (size_t)b * x.img_halves : nullptr;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          if (e + j >= L.P) continue;
-          float pw = pj[j] * x.lr_wd;
-          const float m1 = mj[j] + (gj[j] - mj[j]) * x.one_m_b1;
-          const float v1 = vj[j] * x.b2 + (x.one_m_b2 * gj[j]) * gj[j];
-          const float denom = sqrtf(v1) / bc2_sqrt + x.eps;
-          pw = pw - step_size * (m1 / denom);
-          pj[j] = pw; mj[j] = m1; vj[j] = v1;
-          if (img) {
-            const int t = x.img_index[e + j];
-            if (t >= 0) img[t] = __float2half_rn(pw);
-            else if (t <= -2) reinterpret_cast<float*>(img)[-(t + 2)] = pw;
-          }
-        }
-        *(reinterpret_cast<float4*>(x.p + row) + c4) = pp;
-        *(reinterpret_cast<float4*>(x.m + row) + c4) = mm;
-        *(reinterpret_cast<float4*>(x.v + row) + c4) = vv;
-      }
-    }
-    __syncthreads();                                    // the next call's warp 0 overwrites misc->skip
-    return sk;
-  };
-
-  // The work list is in units of TILE PAIRS (two consecutive tiles of an object, run one after the other), which is
-  // the unit the host-side partition balances.
   for (long long gt = gt_begin; gt < gt_end;) {
-    const int b = (int)(gt / npo);
-    const int p0 = (int)(gt - (long long)b * npo);
-    const int p1 = (int)min((long long)npo, (long long)p0 + (gt_end - gt));
-    gt += p1 - p0;
-    const int t0 = 2 * p0, t1 = min(2 * p1, tpo);       // this segment's tiles of object b
+    const int b = (int)(gt / tpo);
+    const int t0 = (int)(gt - (long long)b * tpo);
+    const int t1 = (int)min((long long)tpo, (long long)t0 + (gt_end - gt));   // this segment's tiles of object b
+    gt += t1 - t0;
 
     // ---- this object's weight image (one bulk copy global -> shared, issued before the previous segment's flush) ----
     um::mbar_wait_or_trap(&misc->wbar, wpar);
@@ -633,13 +543,13 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       if (hsel == 0) {
         if (pub_counts && !seg_w) {                     // acquire the published mask counts (first render only)
           if (!cnt_ready) {
-            const volatile unsigned int* pubd = gbar + 2;
+            const volatile unsigned int* pubd = gbar + SY_PUB;
             unsigned int spins = 0;
             while (*pubd < (unsigned int)a.B) { if (++spins > 2000000000u) __trap(); }
             __threadfence();
             cnt_ready = true;
           }
-          const volatile unsigned int* ef = gbar + 3;
+          const volatile unsigned int* ef = gbar + SY_EMPTY;
           const volatile int* cp = x.counts_pub + b * 4;
           w_d = (ef[0] ? 0.f : 1.f) / ((float)cp[0] + 1e-10f);
           w_c = (ef[1] ? 0.f : 1.f) / ((float)cp[1] + 1e-10f);
@@ -865,7 +775,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       __syncthreads();
       if (tid == 0 && gt < gt_end) {
         ptx::mbar_arrive_expect_tx(&misc->wbar, um::IMG_BYTES);
-        ptx::bulk_g2s(smem + SM_W, image + (size_t)(gt / npo) * um::IMG_BYTES, um::IMG_BYTES, &misc->wbar);
+        ptx::bulk_g2s(smem + SM_W, image + (size_t)(gt / tpo) * um::IMG_BYTES, um::IMG_BYTES, &misc->wbar);
       }
       continue;
     }
@@ -875,7 +785,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     __syncthreads();
     if (tid == 0 && gt < gt_end) {          // every MMA of this segment has completed: the weight buffer is free --
       ptx::mbar_arrive_expect_tx(&misc->wbar, um::IMG_BYTES);        // the next object's image lands during the flush
-      ptx::bulk_g2s(smem + SM_W, image + (size_t)(gt / npo) * um::IMG_BYTES, um::IMG_BYTES, &misc->wbar);
+      ptx::bulk_g2s(smem + SM_W, image + (size_t)(gt / tpo) * um::IMG_BYTES, um::IMG_BYTES, &misc->wbar);
     }
     // the segment's gradient row is assembled in shared memory (the activation region is idle now: the scattered
     // 4-byte stores of the accumulator -> parameter-index mapping cost nothing there) and leaves as coalesced 16-byte stores
@@ -933,57 +843,173 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       for (int i = tid; i < (L.stride >> 2); i += NT) dst[i] = src[i];
     }
     __syncthreads();
+    if (tid == 0) {                                     // the row is out: one more of object b's segments is ready
+      __threadfence();
+      atomicAdd(&gbar[SY_OBJ + 2 * b], 1u);
+    }
     if constexpr (TRACE) { tr_flush += clock64() - tr_f0; ++tr_nseg; }
   }
-  TR_STAMP(2);
+  TR_STAMP2(2, 9);
   if constexpr (TRACE) {
     if (tr_on) { tr[5] = (unsigned long long)tr_t; tr[6] = (unsigned long long)tr_flush; tr[7] = (unsigned long long)tr_nseg; }
   }
 
   if (!a.fwd_only) {
-    // ---- grid-wide finish: every CTA is resident (cooperative launch), all of them end their tiles within one round
-    // of each other, and the reduction of ALL objects' partial rows + AdamW is split evenly over the grid (less than one
-    // float4 of the parameter block per thread) instead of one object per SM on the kernel's tail.
-    // gbar[0] arrive, gbar[1] depart;  gbar[6 + b] = skip flag of object b
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) {
-      atomicAdd(&gbar[0], 1u);
-      unsigned int spins = 0;
-      while (atomicAdd(&gbar[0], 0u) < (unsigned int)G) { __nanosleep(32); if (++spins > 400000000u) __trap(); }
-    }
-    __syncthreads();
-    __threadfence();
-    TR_STAMP(3);
+    // ---- finish: the reduction of every object's partial rows + AdamW, as a list of chunks (object, float4 column
+    // range) in object order, handed out by a ticket counter to CTAs that have run all their tiles.  A chunk waits only
+    // for ITS object's segments (ready count == segments), not for the whole grid: early objects are updated while
+    // other CTAs still run tiles.  Each thread owns at most one float4 column of a chunk.
     const int n4 = L.stride >> 2;
-    const long long W = (long long)a.B * n4;
-    const long long lo = (W * blockIdx.x) / G, hi = (W * (blockIdx.x + 1)) / G;
-    for (int b = (int)(lo / n4); (long long)b * n4 < hi; ++b) {
-      const int i_lo = (int)(max(lo, (long long)b * n4) - (long long)b * n4);
-      const int i_hi = (int)(min(hi, (long long)(b + 1) * n4) - (long long)b * n4);
-      const int skip = finish_rows(b, i_lo, i_hi, i_lo == 0);
-      if (i_lo == 0 && tid == 0) gbar[6 + b] = (unsigned int)skip;
+    const int ncp = (n4 + NT - 1) / NT, csz = (n4 + ncp - 1) / ncp;   // chunks per object, columns per chunk
+    const int nchunk = a.B * ncp;
+    const bool upd = a.backward != 0;
+    if (tid == 0) misc->ticket[0] = atomicAdd(&gbar[SY_TICKET], 1u);
+    __syncthreads();
+    TR_STAMP2(3, 10);
+    for (int it = 0;; ++it) {
+      const int k = (int)misc->ticket[it & 1];          // slot it & 1 was written before the last barrier
+      if (k >= nchunk) break;
+      const int b = k / ncp, i_lo = (k - b * ncp) * csz, i_hi = min(n4, i_lo + csz);
+      const int c4 = i_lo + tid;
+      const bool col = upd && c4 < i_hi, owner = i_lo == 0;
+      const size_t row = (size_t)b * L.stride;
+      // (1) everything that does not depend on other CTAs goes out before the wait: p / m / v (or grads) and the bias
+      //     corrections of step t from the host-built table (torch's double-precision scalars, rounded once); beyond
+      //     the table: 1 - beta^t = -expm1(t ln beta) in fp32 (cancellation-free, <= 3e-7 relative)
+      float4 pp = make_float4(0.f, 0.f, 0.f, 0.f), mm = pp, vv = pp;
+      if (col) {
+        if (x.fuse_adam) {
+          pp = *(reinterpret_cast<const float4*>(x.p + row) + c4);
+          mm = *(reinterpret_cast<const float4*>(x.m + row) + c4);
+          vv = *(reinterpret_cast<const float4*>(x.v + row) + c4);
+        } else {
+          pp = *(reinterpret_cast<const float4*>(a.grads + row) + c4);
+        }
+      }
+      float step_size = x.step_size, bc2_sqrt = x.bc2_sqrt;
+      if (x.fuse_adam && x.step_counter) {
+        const int t = x.step_counter[b] + 1;
+        if (t < x.bc_n) {
+          const float2 bc = x.bc_table[t];
+          step_size = (float)x.lr / bc.x;
+          bc2_sqrt = bc.y;
+        } else {
+          step_size = (float)x.lr / (-expm1f((float)t * x.log_b1));
+          bc2_sqrt = sqrtf(-expm1f((float)t * x.log_b2));
+        }
+      }
+      const int c_first = cta_of_tile(rg, G, b * tpo), c_last = cta_of_tile(rg, G, (b + 1) * tpo - 1);
+      const int nseg = c_last - c_first + 1;
+      const float* P0 = x.partials + (size_t)(c_first + b) * L.stride;
+      // (2) the next ticket, then wait until all of object b's segments have flushed their rows
+      if (tid == 0) {
+        misc->ticket[(it + 1) & 1] = atomicAdd(&gbar[SY_TICKET], 1u);
+        long long w0 = 0;
+        if constexpr (TRACE) w0 = clock64();
+        const unsigned int* rdy = gbar + SY_OBJ + 2 * b;
+        unsigned int spins = 0, r;
+        for (;;) {
+          asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(r) : "l"(rdy) : "memory");
+          if (r >= (unsigned int)nseg) break;
+          __nanosleep(64);
+          if (++spins > 400000000u) __trap();
+        }
+        if constexpr (TRACE) { tr_wait += clock64() - w0; ++tr_calls; }
+      }
+      __syncthreads();
+      // (3) the object's loss terms and explosion guard (render_rays.py:88-90: the reference aborts before the
+      //     update), and this column's rows, all loads in flight at once; both summed in segment order = CTA order,
+      //     the same sums every run whichever CTA runs the chunk
+      float l_d = 0.f, l_c = 0.f, l_o = 0.f;
+      float4 gsum = make_float4(0.f, 0.f, 0.f, 0.f);
+      const float4* src = reinterpret_cast<const float4*>(P0) + c4;
+#pragma unroll 1
+      for (int k0 = 0; k0 < nseg; k0 += 8) {
+        float4 u[8];
+        float lv[8][3];
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {
+          const bool in = k0 + kk < nseg;
+          u[kk] = (in && col) ? __ldcg(src + (size_t)(k0 + kk) * n4) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+          for (int j = 0; j < 3; ++j) lv[kk][j] = in ? __ldcg(P0 + (size_t)(k0 + kk) * L.stride + L.P + j) : 0.f;
+        }
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk)
+          if (k0 + kk < nseg) {
+            gsum.x += u[kk].x; gsum.y += u[kk].y; gsum.z += u[kk].z; gsum.w += u[kk].w;
+            l_d += lv[kk][0]; l_c += lv[kk][1]; l_o += lv[kk][2];
+          }
+      }
+      const float tot = l_d + a.cs * l_c + a.os * l_o;
+      int bad = 0;
+      if (x.guard_loss) {
+        if (l_d > 100000.f || l_c > 100000.f || l_o > 100000.f) bad |= 1;
+        if (!(tot == tot) || fabsf(tot) > 3.0e38f) bad |= 2;
+      }
+      if (owner && tid == 0) {
+        float* lt = a.loss_terms + b * 4; lt[0] = l_d; lt[1] = l_c; lt[2] = l_o; lt[3] = tot;
+        if (bad && x.status) atomicOr(x.status, bad);
+        gbar[SY_OBJ + 2 * b + 1] = (unsigned int)bad;   // skip flag: the step number stays
+      }
+      // (4) update this thread's column: AdamW (fuse_adam; skipped for an exploded object) or grads += gradient
+      if (col && !(bad && x.fuse_adam)) {
+        const int e = c4 * 4;
+        if (!x.fuse_adam) {
+          float4 o = pp;
+          o.x += gsum.x; o.y += gsum.y; o.z += gsum.z; o.w += gsum.w;
+          if (e + 3 >= L.P) { if (e + 0 >= L.P) o.x = 0.f; if (e + 1 >= L.P) o.y = 0.f; if (e + 2 >= L.P) o.z = 0.f; o.w = 0.f; }
+          *(reinterpret_cast<float4*>(a.grads + row) + c4) = o;
+        } else {
+          // torch.optim.AdamW._single_tensor_adamw, op for op as k_adamw restates it
+          float* pj = &pp.x; float* mj = &mm.x; float* vj = &vv.x; const float* gj = &gsum.x;
+          __half* img = x.image_out ? x.image_out + (size_t)b * x.img_halves : nullptr;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            if (e + j >= L.P) continue;
+            float pw = pj[j] * x.lr_wd;
+            const float m1 = mj[j] + (gj[j] - mj[j]) * x.one_m_b1;
+            const float v1 = vj[j] * x.b2 + (x.one_m_b2 * gj[j]) * gj[j];
+            const float denom = sqrtf(v1) / bc2_sqrt + x.eps;
+            pw = pw - step_size * (m1 / denom);
+            pj[j] = pw; mj[j] = m1; vj[j] = v1;
+            if (img) {
+              const int t = x.img_index[e + j];
+              if (t >= 0) img[t] = __float2half_rn(pw);
+              else if (t <= -2) reinterpret_cast<float*>(img)[-(t + 2)] = pw;
+            }
+          }
+          *(reinterpret_cast<float4*>(x.p + row) + c4) = pp;
+          *(reinterpret_cast<float4*>(x.m + row) + c4) = mm;
+          *(reinterpret_cast<float4*>(x.v + row) + c4) = vv;
+        }
+      }
     }
+    // ---- departure: the last CTA to leave has seen every chunk finish
     __threadfence();
     __syncthreads();
-    if (tid == 0) misc->fin = (atomicAdd(&gbar[1], 1u) + 1u == (unsigned int)G) ? 1 : 0;
+    if (tid == 0) misc->fin = (atomicAdd(&gbar[SY_DEPART], 1u) + 1u == (unsigned int)G) ? 1 : 0;
     __syncthreads();
-    if (misc->fin) {                                    // the last CTA to leave: step numbers, re-arm the barrier
+    if (misc->fin) {                                    // the last CTA to leave: step numbers, re-arm the sync words
       __threadfence();
       if (x.fuse_adam && x.step_counter && a.backward)
-        for (int b = tid; b < a.B; b += NT) if (gbar[6 + b] == 0u) x.step_counter[b] += 1;
+        for (int b = tid; b < a.B; b += NT) if (gbar[SY_OBJ + 2 * b + 1] == 0u) x.step_counter[b] += 1;
       if (x.loss_sum && warp == 0) {                    // scalar loss of the step (loss.py:59-62), fixed summation order
         float s = 0.f;
         for (int b = lane; b < a.B; b += 32) s += __ldcg(a.loss_terms + b * 4 + 3);
         s = warp_sum(s);
         if (lane == 0) *x.loss_sum = s;
       }
-      __syncthreads();
-      if (tid == 0) { gbar[0] = 0u; gbar[1] = 0u; gbar[2] = 0u; gbar[3] = 0u; gbar[4] = 0u; gbar[5] = 0u; }
+      for (int b = tid; b < a.B; b += NT) gbar[SY_OBJ + 2 * b] = 0u;
+      if (tid < SY_OBJ) gbar[tid] = 0u;
     }
   }
-  TR_STAMP(4);
+  TR_STAMP2(4, 11);
+  if constexpr (TRACE) {
+    if (tid == 0) { tr[12] = (unsigned long long)tr_wait; tr[13] = (unsigned long long)tr_calls; }
+  }
 #undef TR_STAMP
+#undef TR_STAMP2
 #undef TR_TILE
 }
 
@@ -992,32 +1018,33 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
 // ---------------------------------------------------------------------------------------------------------------
 static int fused_rows_needed(int n_obj, int n_sm) { return n_obj + n_sm; }
 
-// Cost-aware split of B objects x npo tile pairs over G CTAs.  Starting a second object inside a CTA costs it a flush
-// of the gradient partial, a weight load and a pipeline refill, so pairs are laid out on a
-// virtual axis x(p) = p + beta * (object of p) -- every object boundary is a gap of beta -- and that axis is split
-// evenly: a CTA whose range crosses a boundary gets correspondingly fewer pairs.  beta is the largest of {1, 0.7, 0.4, 0}
-// that does not raise the maximum number of rounds per CTA.
-static void fused_partition(int B, int npo, int G, uf::Ranges& rg) {
-  const long long T = (long long)B * npo;
-  double beta = 0.0;
-  if (T >= 2LL * G) {
-    const long long rounds = (T + G - 1) / G;
-    for (double cand : {1.0, 0.7, 0.4}) {
-      if ((long long)std::ceil(((double)T + cand * (B - 1)) / G - 1e-9) <= rounds) { beta = cand; break; }
+// Cost-aware split of B objects x tpo tiles over G CTAs, the CTAs with less work on the lowest object indices.
+// Starting a second object inside a CTA costs it a flush of the gradient partial, a weight load and a pipeline refill,
+// so tiles are laid out on a virtual axis x(t) = t + beta * (object of t) -- every object boundary is a gap of beta --
+// and the axis is split from its end: CTA c, from the last down, takes the tiles that fit in ceil(rest / (c + 1)) of it,
+// rest being the axis left for CTAs 0..c.  Rounding up puts the CTAs with one tile more on the last objects, so the
+// first objects are complete, and their finish chunks run, while those CTAs run their last tile.  beta is the largest
+// of {1, 0.7, 0.4, 0} whose split keeps every CTA at the fewest tiles possible, ceil(tiles / G).
+static void fused_partition(int B, int tpo, int G, uf::Ranges& rg) {
+  const long long T = (long long)B * tpo;
+  const long long rounds = (T + G - 1) / G;
+  for (double beta : {1.0, 0.7, 0.4, 0.0}) {
+    if (beta > 0.0 && T < 2LL * G) continue;
+    auto x = [&](long long t) { return (double)t + beta * (double)(t / tpo); };
+    rg.begin[G] = (int)T;
+    long long most = 0;
+    for (int c = G - 1; c > 0; --c) {                   // G <= T: every CTA keeps at least one tile
+      const long long end = rg.begin[c + 1];
+      const double top = x(end - 1) + 1.0, cap = std::ceil(top / (c + 1) - 1e-9);
+      long long p = end - 1;
+      while (p - 1 >= c && top - x(p - 1) <= cap) --p;
+      rg.begin[c] = (int)p;
+      most = std::max(most, end - p);
     }
+    rg.begin[0] = 0;
+    most = std::max(most, (long long)rg.begin[1]);
+    if (most <= rounds) return;
   }
-  const double V = (double)T + beta * (B - 1);
-  int c = 0;
-  rg.begin[0] = 0;
-  for (long long p = 0; p < T; ++p) {
-    const double x = (double)p + beta * (double)(p / npo);
-    while (c < G - 1 && x >= V * (c + 1) / G && p > rg.begin[c] && T - p >= G - 1 - c) rg.begin[++c] = (int)p;
-    if (T - p - 1 == G - 1 - c && c < G - 1) {            // one pair left per remaining CTA
-      for (long long q = p + 1; q < T; ++q) rg.begin[++c] = (int)q;
-      break;
-    }
-  }
-  while (c < G) rg.begin[++c] = (int)T;
 }
 
 // jdt: the joint step's [B][R * S][2][3] pose-gradient halves (JOINT instantiations), or nullptr (the plain step).
@@ -1035,7 +1062,7 @@ static int fused_launch_step(const VmbLayout& L, const StepParams& sp, const Fus
   static bool attr_set[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
-  const int smem_bytes = SM_CNT + (sp.fwd_only ? 0 : sp.B * 12) + 16;
+  const int smem_bytes = SM_CNT + (sp.fwd_only ? 0 : sp.B * 12) + SMEM_SLACK;
   if (!attr_set[dev & 63]) {
     cudaError_t e = cudaSuccess;
     for (auto k : {k_step_fused<0, false>, k_step_fused<10, false>, k_step_fused<14, false>,
@@ -1047,27 +1074,26 @@ static int fused_launch_step(const VmbLayout& L, const StepParams& sp, const Fus
   const int rpw = 32 / sp.S;                  // whole rays per warp: the sample axis never crosses a warp
   const int nr = 4 * rpw;
   const int tpo = (sp.R + nr - 1) / nr;       // tiles per object
-  const int npo = (tpo + 1) / 2;              // rounds (tile pairs) per object
-  const long long T = (long long)npo * sp.B;
+  const long long T = (long long)tpo * sp.B;
   if (T > 0x7fffffffLL) { err = "fused step kernel: too many tiles"; return -1; }
   long long grid = T;
   if (grid > n_sm) grid = n_sm;
   if (grid > MAX_CTAS) grid = MAX_CTAS;
   if (grid < 1) grid = 1;
   Ranges rg;
-  fused_partition(sp.B, npo, (int)grid, rg);
+  fused_partition(sp.B, tpo, (int)grid, rg);
   const unsigned char* img = (const unsigned char*)image;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(NT); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = st;
   cudaLaunchAttribute attr[1];
-  // a training launch ends in a grid barrier: every CTA must be resident (grid <= #SMs, one CTA per SM), and the
-  // cooperative attribute makes the runtime guarantee it
+  // a training launch's finish waits on other CTAs' segments: every CTA must be resident (grid <= #SMs, one CTA per
+  // SM), and the cooperative attribute makes the runtime guarantee it
   attr[0].id = cudaLaunchAttributeCooperative;
   attr[0].val.cooperative = sp.fwd_only ? 0 : 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
   cudaError_t e;
-  auto kern = [&](auto k) { return cudaLaunchKernelEx(&cfg, k, sp, fx, L, img, rg, tpo, npo, nr, rpw, jdt, trace); };
+  auto kern = [&](auto k) { return cudaLaunchKernelEx(&cfg, k, sp, fx, L, img, rg, tpo, nr, rpw, jdt, trace); };
   if (trace) e = kern(k_step_fused<10, false, true>);
   else if (jdt) e = kern(sp.S == 10 ? k_step_fused<10, true> : sp.S == 14 ? k_step_fused<14, true> : k_step_fused<0, true>);
   else     e = kern(sp.S == 10 ? k_step_fused<10, false> : sp.S == 14 ? k_step_fused<14, false> : k_step_fused<0, false>);

@@ -35,7 +35,7 @@ struct vmb_handle {
   unsigned int* d_ticket; // last-block ticket of the fused AdamW (device step counter mode)
   unsigned int* d_smax;   // [max_obj] sampler: per-object max sampled depth (order-preserving key)
   float* d_partials;      // fused step: [(max_obj + n_sm)][stride] per-(CTA, object) gradient partials (allocated on first use)
-  unsigned int* d_finish_sync; // fused step: [6] grid-barrier words (self-resetting) + [max_obj] skip flags
+  unsigned int* d_finish_sync; // fused step: finish sync words + per-object readiness counts and skip flags (uf::SY_*)
   float2* d_bc;           // AdamW bias corrections per step number for (bc_b1, bc_b2), built on the host in double precision
   double bc_b1, bc_b2;
   int img_halves;
@@ -214,7 +214,7 @@ static AdamScalars adam_scalars(float lr_f, float b1_f, float b2_f, float wd_f, 
   return q;
 }
 
-// scratch of the fused step kernel (gradient partial rows + grid-barrier words and skip flags): allocated on first use,
+// scratch of the fused step kernel (gradient partial rows + finish sync words and skip flags): allocated on first use,
 // never while a stream capture is in progress (a captured graph bakes the pointers in)
 static int fused_scratch(vmb_handle* h, cudaStream_t st) {
   if (h->d_partials) return VMB_OK;
@@ -224,7 +224,7 @@ static int fused_scratch(vmb_handle* h, cudaStream_t st) {
     return fail(h, VMB_E_CUDA, "vmb_step: first fused step of a handle must run outside stream capture (scratch allocation)");
   const size_t rows = (size_t)fused_rows_needed(h->max_obj, h->n_sm);
   cudaError_t e = cudaMalloc(&h->d_partials, rows * h->L.stride * sizeof(float));
-  const size_t sync_bytes = sizeof(unsigned int) * (6 + (size_t)h->max_obj);
+  const size_t sync_bytes = sizeof(unsigned int) * (uf::SY_OBJ + 2 * (size_t)h->max_obj);
   if (e == cudaSuccess) e = cudaMalloc(&h->d_finish_sync, sync_bytes);
   if (e == cudaSuccess) e = cudaMemset(h->d_finish_sync, 0, sync_bytes);
   if (e != cudaSuccess) return fail(h, VMB_E_NOMEM, cudaGetErrorString(e));
