@@ -720,6 +720,21 @@ enum { VMB_TRACK_ST_CLAMP = 16 };
 int vmb_track_step_lw(vmb_handle* h, const vmb_track_args* a, int group, const void* image, void* stream);
 int vmb_ba_step_lw(vmb_handle* h, const vmb_ba_args* a, int group, const void* image, void* stream);
 
+/* ---- K10 / K11 at hidden 32 on the fused wgmma tile (the rule is in csrc/k_track_fused.cuh) -------------------------
+ * The same step as vmb_track_step / vmb_ba_step for the hidden-32 object models (n_freq 6), with the network on the
+ * tile of the fused training step: one launch per call covers every object of the group, each object reading its fp16
+ * weight image row rows[b] of `image` ([n_rows][vmb_image_bytes], as the AdamW launch writes it).  The forward and the
+ * input-gradient chain only (no weight gradients); render, loss and pose terms in fp64 as K10.  Writes the same rows as
+ * vmb_track_step (K10's partials: vmb_track_tiles rows per object, the per-ray terms summed per K10 tile in ray order)
+ * and vmb_ba_step (one row per ray), so vmb_track_update and vmb_ba_update run unchanged.  No floating-point atomics:
+ * bitwise reproducible.  Argument checks as the _lw pair; VMB_E_ARG also for a NULL image and a partials or ray-rows
+ * buffer that is too small; VMB_E_UNSUPPORTED for hidden != 32 or n_freq != 6 (hidden 64/128/256 take the _lw pair) and
+ * n_samples > 32.  On the device, besides the bits of K10 / K11: a loss-scaled head gradient (LS d(raw alpha),
+ * LS d(raw colour)) past the fp16 clamp (+-60000) sets VMB_TRACK_ST_CLAMP and adds to status[1] the number of such
+ * values, a lower bound on the clamped values (the saturating packs of the d_hc .. d_fc1 epilogues are not counted). */
+int vmb_track_step_fused(vmb_handle* h, const vmb_track_args* a, int group, const void* image, void* stream);
+int vmb_ba_step_fused(vmb_handle* h, const vmb_ba_args* a, int group, const void* image, void* stream);
+
 /* ---- joint map-and-pose step on the layer-wise path (iMAP: network weights and keyframe poses together; the rule is
  * in csrc/k_track_lw.cuh) ---------------------------------------------------------------------------------------------
  * One mapping iteration that also yields K11's per-ray pose rows, from ONE forward and backward:

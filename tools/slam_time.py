@@ -12,7 +12,8 @@ frames replay it.  With ``--ba-every`` (one run per value; 0 = no bundle adjustm
 reported too, by pass mode, and after the run the device time of one BA iteration per group (``vmb_ba_step`` on each
 ensemble) and of ``vmb_ba_update``, over repeated launches.  The card's name and power limit are read in the same
 run.  ``--imap`` runs the iMAP settings instead (one hidden-256 scene model, every pixel instance 0);
-``--track-impl`` / ``--ba-impl`` choose ``fp32`` or ``layerwise`` (default: layer-wise in iMAP mode, fp32 otherwise)."""
+``--track-impl`` / ``--ba-impl`` choose ``fp32``, ``layerwise`` or ``fused`` (default: layer-wise in iMAP mode, fp32
+otherwise)."""
 from __future__ import annotations
 
 import argparse
@@ -37,8 +38,8 @@ def main(argv=None):
     ap.add_argument("--ba-every", default="0", help="comma-separated ba_every values, one run each")
     ap.add_argument("--ba-iter", type=int, default=20)
     ap.add_argument("--imap", action="store_true", help="the iMAP settings: one hidden-256 scene model")
-    ap.add_argument("--track-impl", choices=("fp32", "layerwise"), default=None)
-    ap.add_argument("--ba-impl", choices=("fp32", "layerwise"), default=None)
+    ap.add_argument("--track-impl", choices=("fp32", "layerwise", "fused"), default=None)
+    ap.add_argument("--ba-impl", choices=("fp32", "layerwise", "fused"), default=None)
     args = ap.parse_args(argv)
     assert torch.cuda.is_available(), "slam_time measures the GPU; there is no CPU number"
     cfg = Config(config_dict=replica_room0_dict(imap=args.imap))

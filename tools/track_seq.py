@@ -69,9 +69,9 @@ def main(argv=None):
     ap.add_argument("--ba-every", type=int, default=0,
                     help="--slam: a bundle-adjustment pass after every N-th mapping frame (0: none)")
     ap.add_argument("--ba-iter", type=int, default=20, help="bundle-adjustment iterations per pass")
-    ap.add_argument("--track-impl", choices=("fp32", "layerwise"), default=None,
+    ap.add_argument("--track-impl", choices=("fp32", "layerwise", "fused"), default=None,
                     help="tracking step (default: layerwise for iMAP configs, fp32 otherwise)")
-    ap.add_argument("--ba-impl", choices=("fp32", "layerwise"), default=None,
+    ap.add_argument("--ba-impl", choices=("fp32", "layerwise", "fused"), default=None,
                     help="bundle-adjustment step (default: layerwise for iMAP configs, fp32 otherwise)")
     args = ap.parse_args(argv)
     cfg = Config(args.config)

@@ -6,8 +6,10 @@ group and of the update, each launched alone (CUDA events over many launches), t
 frame) and as a graph replay, the FLOPs from shapes (forward plus the backward to the inputs, 4 (4H^2 + 220H + 63) per
 point) and their share of the H100 SXM fp32 data-sheet rate (67 TFLOP/s), with the card's name and power limit.
 
-``--impl layerwise`` times the tensor-core path for the hidden-128 background (hidden 32 stays on K10); ``--imap`` times
-the iMAP shape instead: one hidden-256 scene model, 4800 rays x 14 samples over the full frame."""
+``--impl layerwise`` times the tensor-core path for the hidden-128 background (hidden 32 stays on K10); ``--impl fused``
+also runs the hidden-32 objects on the fused wgmma tile (``vmb_track_step_fused``).  ``--kernels`` adds, from a
+``torch.profiler`` run of its own after the timed ones, the device time per launch of each kernel of one iteration.
+``--imap`` times the iMAP shape instead: one hidden-256 scene model, 4800 rays x 14 samples over the full frame."""
 from __future__ import annotations
 
 import argparse
@@ -56,8 +58,9 @@ def ev_time(fn, n):
 
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
-    ap.add_argument("--impl", choices=("fp32", "layerwise"), default="fp32")
+    ap.add_argument("--impl", choices=("fp32", "layerwise", "fused"), default="fp32")
     ap.add_argument("--imap", action="store_true", help="the iMAP shape: one hidden-256 model, 4800 x 14")
+    ap.add_argument("--kernels", action="store_true", help="per-kernel device time of one iteration (torch.profiler)")
     args = ap.parse_args(argv)
     assert torch.cuda.is_available(), "track_time measures the GPU; there is no CPU number"
     dev = "cuda:0"
@@ -138,7 +141,25 @@ def main(argv=None):
         "fp32_share_of_peak_per_iteration": round(flop_iter / (t_iter * 1e-6) / FP32_PEAK, 4),
         "fp32_share_of_peak_frame_graph": round(flop_iter * n_iter / (t_graph * 1e-6) / FP32_PEAK, 4),
     }
+    if args.kernels:
+        out["kernel_us"] = kernel_times(lambda: _iterate(live, 1, pose, adam, 0.0, 0.0, losses, status), 50)
     print(json.dumps(out))
+
+
+def kernel_times(fn, n):
+    """Device time per launch of each kernel ``fn`` launches (mean over ``n`` calls), from torch.profiler."""
+    from torch.profiler import ProfilerActivity, profile
+    fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(n):
+            fn()
+        torch.cuda.synchronize()
+    out = {}
+    for e in prof.key_averages():
+        if e.device_type.name == "CUDA" and e.count:
+            out[e.key[:60]] = {"us": round(e.device_time_total / e.count, 2), "launches": e.count}
+    return out
 
 
 def _update_only(tr, live):

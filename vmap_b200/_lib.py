@@ -252,7 +252,8 @@ EXPORTS = (
     "vmb_assoc_classify", "vmb_assoc_voxel", "vmb_assoc_finalize",
     "vmb_hull", "vmb_obb_minvol", "vmb_render_count", "vmb_render_emit", "vmb_render_composite",
     "vmb_track_tiles", "vmb_track_step", "vmb_track_update", "vmb_ba_step", "vmb_ba_update",
-    "vmb_track_step_lw", "vmb_ba_step_lw", "vmb_joint_step_lw", "vmb_joint_step_fused",
+    "vmb_track_step_lw", "vmb_ba_step_lw", "vmb_track_step_fused", "vmb_ba_step_fused", "vmb_joint_step_lw",
+    "vmb_joint_step_fused",
 )
 
 _lib = None
@@ -321,6 +322,8 @@ def lib():
         L.vmb_ba_update.argtypes = [_vp, C.POINTER(BaArgs), _vp]
         L.vmb_track_step_lw.argtypes = [_vp, C.POINTER(TrackArgs), C.c_int, _vp, _vp]
         L.vmb_ba_step_lw.argtypes = [_vp, C.POINTER(BaArgs), C.c_int, _vp, _vp]
+        L.vmb_track_step_fused.argtypes = [_vp, C.POINTER(TrackArgs), C.c_int, _vp, _vp]
+        L.vmb_ba_step_fused.argtypes = [_vp, C.POINTER(BaArgs), C.c_int, _vp, _vp]
         L.vmb_joint_step_lw.argtypes = [_vp, C.POINTER(StepArgs), C.POINTER(BaArgs), C.c_int, _vp, _vp]
         L.vmb_joint_step_fused.argtypes = [_vp, C.POINTER(StepArgs), C.POINTER(BaArgs), C.c_int, _vp, _vp]
         L.vmb_build_image.argtypes = [_vp, C.c_int, _vp, _vp, _vp]

@@ -9,7 +9,8 @@ pose-only passes against the frozen map: per pass
 
 all on the device, so a pass can be captured as one CUDA graph (``capture`` / ``run``).  The rule is in
 ``csrc/k_ba.cuh``; ``oracle/ba_oracle.py`` restates it.  ``impl="layerwise"`` runs the step of every hidden-64/128/256
-group on the tensor-core path (``vmb_ba_step_lw``, ``csrc/k_track_lw.cuh``), as ``Tracker`` does.
+group on the tensor-core path (``vmb_ba_step_lw``, ``csrc/k_track_lw.cuh``), as ``Tracker`` does; ``impl="fused"``
+also runs every hidden-32 group on the fused tile (``vmb_ba_step_fused``, ``csrc/k_track_fused.cuh``).
 """
 from __future__ import annotations
 
@@ -22,7 +23,7 @@ import torch
 from . import _lib
 from .ensemble import VmapEnsemble, _ptr, _stream
 from .sampler import BatchedSampler, SamplerTables
-from .track import _rays_dir, _Slices, _step, _use_lw
+from .track import _path, _rays_dir, _Slices, _step
 from .utils import capture_graph
 
 
@@ -140,7 +141,8 @@ class _BaGroup(_Slices):
                  impl: str = "fp32"):
         ids = [None if i is None or int(i) < 0 else int(i) for i in obj_ids]
         assert len(ids) == ens.n_obj, "obj_ids must name every row of the ensemble (None / -1 = not an object)"
-        self.ens, self.ids, self.bg, self.lw = ens, ids, bg, _use_lw(ens, impl)
+        self.ens, self.ids, self.bg, self.path = ens, ids, bg, _path(ens, impl)
+        self.lw = self.path == "layerwise"      # the group runs on the layer-wise path
         self.rows = [r for r, i in enumerate(ids) if i is not None]
         B = len(self.rows)
         assert B > 0
@@ -197,7 +199,8 @@ class BundleAdjuster:
     keyframe copies (the ``do_bg`` background) samples those.  ``n_iter`` iterations per pass in the mapping layout;
     rates default to ``cfg.pose_lr``; ``hold`` (the anchor frame) never moves.  ``record``: keep each pass's pose and
     gradient history per window entry (``pose_hist`` [n_iter+1, max_win, 4, 4], ``grad_hist`` [n_iter, max_win, 6]).
-    ``impl``: ``"fp32"`` (K11 for every group) or ``"layerwise"`` (the tensor-core path for hidden 64/128/256)."""
+    ``impl``: ``"fp32"`` (K11 for every group), ``"layerwise"`` (the tensor-core path for hidden 64/128/256) or
+    ``"fused"`` (as ``"layerwise"``, and the fused tile for hidden 32)."""
 
     def __init__(self, groups: Sequence[Tuple[VmapEnsemble, Sequence[Optional[int]]]], cfg, objects: Dict[int, object],
                  n_iter: int = 20, lr_rot: Optional[float] = None, lr_trans: Optional[float] = None, seed: int = 0,
@@ -349,7 +352,8 @@ class BaSampleGroup(_BaGroup):
 
     def __init__(self, ens: VmapEnsemble, rows: Sequence[int], batch: Dict[str, torch.Tensor], n_iter: int,
                  n_pix_draw: int, kf_draw, kf_frame, impl: str = "fp32"):
-        self.ens, self.rows, self.lw = ens, list(rows), _use_lw(ens, impl)
+        self.ens, self.rows, self.path = ens, list(rows), _path(ens, impl)
+        self.lw = self.path == "layerwise"      # the group runs on the layer-wise path
         B, N, S = batch["pcs"].shape[:3]
         assert B == len(self.rows) and N % n_iter == 0 and (N // n_iter) % n_pix_draw == 0
         self.n_pix, self.S, self.n_pix_draw = N // n_iter, S, n_pix_draw

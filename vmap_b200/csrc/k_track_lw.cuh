@@ -338,22 +338,15 @@ __global__ void __launch_bounds__(128) k_tlw_pose(TlwObj o, const float* __restr
 }
 
 // ---- 5: fixed-order fp64 sums into K10's partial rows (track) or K11's per-ray rows (BA) -----------------------------
-// lossr NULL (the joint step): the loss columns are written as 0
-template <bool BA>
-__global__ void __launch_bounds__(128) k_tlw_reduce(TlwObj o, int nr, int n_out, const int* __restrict__ ctl,
-                                                    const double* __restrict__ gpt, const double* __restrict__ lossr,
-                                                    double* __restrict__ out) {
-  ptx::pdl_wait();
-  ptx::pdl_launch_dependents();
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n_out) return;
-  double* dst = out + (size_t)j * VMB_TRACK_PART;
-  const int per = BA ? 1 : nr;                        // rays per output row
-  const int r0 = j * per, r1 = min(o.R, r0 + per);
+// Row j of R rays of S points: the points' terms of rays [j per, (j + 1) per) in point order, their loss terms in ray
+// order (0 when !ok, loss columns 0 when lossr is NULL).  Also the rule of the fused path's k_tf_reduce (S = 1).
+__device__ __forceinline__ void tlw_reduce_row(int R, int S, int per, int j, bool ok, const double* __restrict__ gpt,
+                                               const double* __restrict__ lossr, double* __restrict__ dst) {
+  const int r0 = j * per, r1 = min(R, r0 + per);
   double s[9] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-  if (ctl[3]) {
-    const long long pe = (long long)r1 * o.S;
-    for (long long p = (long long)r0 * o.S; p < pe; ++p)
+  if (ok) {
+    const long long pe = (long long)r1 * S;
+    for (long long p = (long long)r0 * S; p < pe; ++p)
 #pragma unroll
       for (int c = 0; c < 6; ++c) s[c] += gpt[p * 6 + c];
     if (lossr)
@@ -364,6 +357,18 @@ __global__ void __launch_bounds__(128) k_tlw_reduce(TlwObj o, int nr, int n_out,
 #pragma unroll
   for (int c = 0; c < 9; ++c) dst[c] = s[c];
   dst[9] = 0.0;
+}
+
+// lossr NULL (the joint step): the loss columns are written as 0
+template <bool BA>
+__global__ void __launch_bounds__(128) k_tlw_reduce(TlwObj o, int nr, int n_out, const int* __restrict__ ctl,
+                                                    const double* __restrict__ gpt, const double* __restrict__ lossr,
+                                                    double* __restrict__ out) {
+  ptx::pdl_wait();
+  ptx::pdl_launch_dependents();
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n_out) return;
+  tlw_reduce_row(o.R, o.S, BA ? 1 : nr, j, ctl[3] != 0, gpt, lossr, out + (size_t)j * VMB_TRACK_PART);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

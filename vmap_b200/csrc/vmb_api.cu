@@ -25,6 +25,7 @@
 #include "k_track.cuh"
 #include "k_ba.cuh"
 #include "k_track_lw.cuh"
+#include "k_track_fused.cuh"
 
 struct vmb_handle {
   int device, max_obj, H, nfreq;
@@ -51,6 +52,7 @@ struct vmb_handle {
   lw::TrackWorkspace ws_track;// layer-wise tracking step: its own, so a tracking capture never pins the mapping step's
   lw::TrackWorkspace ws_ba;   // layer-wise bundle-adjustment step: likewise (and tracking never moves a BA capture's)
   lw::JointWorkspace ws_joint;// joint map-and-pose step: world points and pose terms (the activations are the step's ws)
+  tf::Workspace ws_tf;        // fused hidden-32 tracking step: per-ray rows before K10's tile sums (BA writes its rows)
   std::string err;
 };
 
@@ -185,6 +187,7 @@ void vmb_destroy(vmb_handle* h) {
   h->ws_track.release();
   h->ws_ba.release();
   h->ws_joint.release();
+  h->ws_tf.release();
   delete h;
 }
 
@@ -1238,7 +1241,11 @@ int vmb_debug_gemm(int a_mn, int b_mn, int epi, int M, int N, int K1, int K2, co
 
 }  // extern "C"
 
-// ---- K10 / K11 and their layer-wise path: one host path for the four step entry points ------------------------------
+// ---- K10 / K11, their layer-wise path and their fused hidden-32 path: one host path for the six step entry points ----
+// which network runs the step: K10 / K11 on CUDA cores, the layer-wise wgmma GEMMs (hidden 64/128/256) or the fused
+// hidden-32 wgmma tile
+enum PosePath { POSE_FP32 = 0, POSE_LW = 1, POSE_FUSED = 2 };
+
 template <int H, int TP, bool BA>
 static int launch_pose(vmb_handle* h, const TrackParams& tp, const BaRays& x, int tiles, cudaStream_t st) {
   const size_t smem = NetTile<H, TP>::smem(h->L, 0);
@@ -1282,12 +1289,14 @@ static int ba_group_ok(const vmb_ba_group& g) {
 // from it: the sample slice, the network, `pose` (the pose or the pose table), the loss weights and status of `a`.
 // Returns the group's tile count, or the VMB_E_* code of the failed check.
 template <class G, class Args>
-static int pose_group_params(vmb_handle* h, const G& g, const double* pose, const Args* a, const char* who, bool lw,
+static int pose_group_params(vmb_handle* h, const G& g, const double* pose, const Args* a, const char* who, int path,
                              const void* image, TrackParams& tp) {
   constexpr bool BA = std::is_same_v<G, vmb_ba_group>;
   const std::string w(who);
   if (g.hidden != h->H) return fail(h, VMB_E_ARG, w + ": group hidden size differs from the handle's");
-  if (lw && !h->lw_ok) return fail(h, VMB_E_UNSUPPORTED, w + ": the layer-wise path needs hidden 64/128/256 and n_freq 6");
+  const bool lw = path != POSE_FP32;                  // a tensor-core path: reads the image, S <= 32
+  if (path == POSE_LW && !h->lw_ok) return fail(h, VMB_E_UNSUPPORTED, w + ": the layer-wise path needs hidden 64/128/256 and n_freq 6");
+  if (path == POSE_FUSED && !h->umma_ok) return fail(h, VMB_E_UNSUPPORTED, w + ": the fused path needs hidden 32 and n_freq 6");
   if constexpr (BA) {
     if (ba_group_ok(g) != VMB_OK) return fail(h, VMB_E_ARG, w + ": bad counts, draw layout, keyframe tables or ray rows");
   } else {
@@ -1318,8 +1327,8 @@ static int pose_group_params(vmb_handle* h, const G& g, const double* pose, cons
   return tiles;
 }
 
-// The step of group `group`: K10 (vmb_track_args) or K11 (vmb_ba_args), on CUDA cores or on the layer-wise path (LW).
-template <bool LW, class Args>
+// The step of group `group`: K10 (vmb_track_args) or K11 (vmb_ba_args), on the network path PATH (PosePath).
+template <int PATH, class Args>
 static int pose_step(vmb_handle* h, const Args* a, int group, const void* image, void* stream, const char* who) {
   constexpr bool BA = std::is_same_v<Args, vmb_ba_args>;
   if (!h) return fail(h, VMB_E_ARG, std::string(who) + ": null handle");
@@ -1332,16 +1341,22 @@ static int pose_step(vmb_handle* h, const Args* a, int group, const void* image,
   memset(&x, 0, sizeof(x));
   int tiles;
   if constexpr (BA) {
-    tiles = pose_group_params(h, g, a->poses, a, who, LW, image, tp);
+    tiles = pose_group_params(h, g, a->poses, a, who, PATH, image, tp);
     if (tiles < 0) return tiles;
     x.kf_draw = g.kf_draw; x.kf_draw_stride = g.kf_draw_stride; x.kf_frame = g.kf_frame; x.kf_stride = g.kf_stride;
     x.n_pix_draw = g.n_pix_draw; x.n_poses = a->n_poses; x.rows = g.ray_rows;
   } else {
-    tiles = pose_group_params(h, g, a->pose, a, who, LW, image, tp);
+    tiles = pose_group_params(h, g, a->pose, a, who, PATH, image, tp);
     if (tiles < 0) return tiles;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  if constexpr (LW) {
+  if constexpr (PATH == POSE_FUSED) {
+    std::string err;
+    const int rc = tf::launch_track_fused<BA>(h->ws_tf, h->L, tp, x, image, fp32_tile(32) / g.n_samples, h->max_obj,
+                                              st, err);
+    if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, std::string(who) + ": " + err);
+    return VMB_OK;
+  } else if constexpr (PATH == POSE_LW) {
     const lw::TlwGroup G{tp, x, (const __half*)image, BA ? 1 : fp32_tile(g.hidden) / g.n_samples};
     std::string err;
     const int rc = lw::launch_track_lw<BA>(BA ? h->ws_ba : h->ws_track, h->L, G, st, err);
@@ -1383,19 +1398,27 @@ int vmb_track_tiles(int hidden, int n_rays, int n_samples) {
 }
 
 int vmb_track_step(vmb_handle* h, const vmb_track_args* a, int group, void* stream) {
-  return pose_step<false>(h, a, group, nullptr, stream, "vmb_track_step");
+  return pose_step<POSE_FP32>(h, a, group, nullptr, stream, "vmb_track_step");
 }
 
 int vmb_ba_step(vmb_handle* h, const vmb_ba_args* a, int group, void* stream) {
-  return pose_step<false>(h, a, group, nullptr, stream, "vmb_ba_step");
+  return pose_step<POSE_FP32>(h, a, group, nullptr, stream, "vmb_ba_step");
 }
 
 int vmb_track_step_lw(vmb_handle* h, const vmb_track_args* a, int group, const void* image, void* stream) {
-  return pose_step<true>(h, a, group, image, stream, "vmb_track_step_lw");
+  return pose_step<POSE_LW>(h, a, group, image, stream, "vmb_track_step_lw");
 }
 
 int vmb_ba_step_lw(vmb_handle* h, const vmb_ba_args* a, int group, const void* image, void* stream) {
-  return pose_step<true>(h, a, group, image, stream, "vmb_ba_step_lw");
+  return pose_step<POSE_LW>(h, a, group, image, stream, "vmb_ba_step_lw");
+}
+
+int vmb_track_step_fused(vmb_handle* h, const vmb_track_args* a, int group, const void* image, void* stream) {
+  return pose_step<POSE_FUSED>(h, a, group, image, stream, "vmb_track_step_fused");
+}
+
+int vmb_ba_step_fused(vmb_handle* h, const vmb_ba_args* a, int group, const void* image, void* stream) {
+  return pose_step<POSE_FUSED>(h, a, group, image, stream, "vmb_ba_step_fused");
 }
 
 int vmb_track_update(vmb_handle* h, const vmb_track_args* a, void* stream) {

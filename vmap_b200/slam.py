@@ -36,8 +36,9 @@ In iMAP mode (``cfg.imap_mode``) every pixel of a frame is instance 0 (dataset.p
 whole-scene network, an object of the stack as mapping builds it (``hidden_feature_size``, ``obj_scale``,
 ``n_bins_cam2surface``, ``n_per_optim``); it is tracked like any other object from the frame after its insertion, with
 its box from the ingest.  ``track_impl`` / ``ba_impl`` choose the step of the tracker and the bundle adjuster:
-``"layerwise"`` (the tensor-core path for hidden 64/128/256, the default in iMAP mode) or ``"fp32"`` (K10 / K11, the
-default otherwise).
+``"layerwise"`` (the tensor-core path for hidden 64/128/256, the default in iMAP mode), ``"fp32"`` (K10 / K11, the
+default otherwise) or ``"fused"`` (as ``"layerwise"``, and the vMAP objects' hidden-32 models on the fused wgmma tile;
+in iMAP mode, which has no hidden-32 model, the same as ``"layerwise"``).
 
 With ``joint_poses`` (iMAP mode only) every mapping iteration also moves the keyframe poses, as iMAP optimises its
 network and keyframe poses together: the mapping frame runs ``FrameLoop``'s joint mode (``vmb_joint_step_lw``: the pose
@@ -112,8 +113,8 @@ class Slam:
     grows on demand).  ``timing``: record CUDA events at the phase boundaries of every frame (``phase_times``).
     ``ba_every``: run a bundle-adjustment pass after the mapping frame of every ``ba_every``-th frame (0: never);
     ``n_ba_iter`` / ``ba_lr_rot`` / ``ba_lr_trans``: its iterations and rates (default ``cfg.pose_lr``).
-    ``track_impl`` / ``ba_impl``: ``"fp32"`` or ``"layerwise"`` (see the module docstring; None: ``"layerwise"`` in iMAP
-    mode, ``"fp32"`` otherwise).  ``joint_poses``: optimise the keyframe poses with the map in every mapping iteration
+    ``track_impl`` / ``ba_impl``: ``"fp32"``, ``"layerwise"`` or ``"fused"`` (see the module docstring; None:
+    ``"layerwise"`` in iMAP mode, ``"fp32"`` otherwise).  ``joint_poses``: optimise the keyframe poses with the map in every mapping iteration
     (see the module docstring); ``joint_lr_rot`` / ``joint_lr_trans``: its rates (default ``cfg.pose_lr``);
     ``joint_impl``: ``None`` / ``"layerwise"`` (iMAP mode) or ``"fused"`` (vMAP mode).  ``assoc``: a
     ``scannet.InstanceTracker``, the one association state of a ScanNet sequence (see the module docstring); ``step``

@@ -13,7 +13,9 @@ mapping frame.  The rule (points, loss, per-object empty masks, gradient, update
 
 ``impl="layerwise"`` runs the step of every hidden-64/128/256 group on the tensor-core path instead
 (``vmb_track_step_lw``, ``csrc/k_track_lw.cuh``: the same rule, the network in fp16 on wgmma GEMMs); hidden-32 groups
-stay on K10.  In iMAP mode (``cfg.imap_mode``) id 0 is the whole-scene model and is sampled as an object.
+stay on K10.  ``impl="fused"`` does the same for hidden 64/128/256 and runs every hidden-32 group on the fused wgmma
+tile (``vmb_track_step_fused``, ``csrc/k_track_fused.cuh``: the same rule, one launch for all the group's objects).  In
+iMAP mode (``cfg.imap_mode``) id 0 is the whole-scene model and is sampled as an object.
 """
 from __future__ import annotations
 
@@ -28,22 +30,35 @@ from .ensemble import VmapEnsemble, _ptr, _stream
 from .sampler import BatchedSampler, KeyframeTables, SamplerTables
 from .utils import capture_graph
 
-IMPLS = ("fp32", "layerwise")
+IMPLS = ("fp32", "layerwise", "fused")
 
 
-def _use_lw(ens: VmapEnsemble, impl: str) -> bool:
-    """True when ``impl`` sends this ensemble's step to the layer-wise tensor-core path (hidden 64/128/256)."""
+def _path(ens: VmapEnsemble, impl: str) -> str:
+    """Where ``impl`` runs this ensemble's step: ``"fp32"`` (K10 / K11), ``"layerwise"`` (hidden 64/128/256 on the
+    layer-wise tensor-core path, with "layerwise" or "fused") or ``"fused"`` (hidden 32 on the fused tile, with
+    "fused").  A hidden-32 ensemble without its fp16 image cannot take the fused path: that raises."""
     if impl not in IMPLS:
         raise ValueError(f"tracking impl must be one of {IMPLS}, not {impl!r}")
-    return impl == "layerwise" and ens.hidden != 32 and ens.image is not None
+    if impl == "fp32":
+        return "fp32"
+    if ens.hidden == 32:
+        if impl == "layerwise":
+            return "fp32"
+        if ens.image is None:
+            raise _lib.VmbError("tracking impl 'fused': the hidden-32 ensemble has no fp16 weight image")
+        return "fused"
+    return "layerwise" if ens.image is not None else "fp32"
 
 
 def _step(g, a, gi: int, ba: bool) -> None:
-    """The step of group ``gi`` on K10 / K11 or, for a layer-wise group, on the tensor-core path."""
+    """The step of group ``gi`` on K10 / K11 or on the group's tensor-core path."""
     e = g.ens
     with e._on_device():
-        if g.lw:
-            fn = e.lib.vmb_ba_step_lw if ba else e.lib.vmb_track_step_lw
+        if g.path != "fp32":
+            if g.path == "fused":
+                fn = e.lib.vmb_ba_step_fused if ba else e.lib.vmb_track_step_fused
+            else:
+                fn = e.lib.vmb_ba_step_lw if ba else e.lib.vmb_track_step_lw
             _lib.check(e._handle, fn(e._handle, C.byref(a), gi, _ptr(e.image), _stream()), fn.__name__)
         else:
             fn = e.lib.vmb_ba_step if ba else e.lib.vmb_track_step
@@ -101,7 +116,8 @@ class _Group(_Slices):
                  n_iter: int, impl: str = "fp32"):
         ids = [None if i is None or int(i) < 0 else int(i) for i in obj_ids]
         assert len(ids) == ens.n_obj, "obj_ids must name every row of the ensemble (None / -1 = not an object)"
-        self.ens, self.ids, self.lw = ens, ids, _use_lw(ens, impl)
+        self.ens, self.ids, self.path = ens, ids, _path(ens, impl)
+        self.lw = self.path == "layerwise"      # the group runs on the layer-wise path
         self.bg = 0 in ids and not getattr(cfg, "imap_mode", 0)     # iMAP: id 0 is the scene model, an object
         assert not self.bg or [i for i in ids if i is not None] == [0], "the background (id 0) is a group of its own"
         n1 = cfg.n_bins_cam2surface_bg if self.bg else cfg.n_bins_cam2surface
@@ -169,7 +185,8 @@ class Tracker:
     ``groups``: ``[(VmapEnsemble, obj_ids), ...]`` with ``obj_ids[row]`` the instance id of each row (``None`` or -1
     for rows that are not objects); the background (id 0) is a group of its own.  ``n_iter`` iterations of ``n_pix``
     rays per object (``n_pix_bg`` for the background); rates default to ``cfg.pose_lr``.  ``impl``: ``"fp32"`` (K10
-    for every group) or ``"layerwise"`` (the tensor-core path for hidden-64/128/256 groups, K10 for hidden 32)."""
+    for every group), ``"layerwise"`` (the tensor-core path for hidden-64/128/256 groups, K10 for hidden 32) or
+    ``"fused"`` (as ``"layerwise"``, and the fused tile for hidden-32 groups)."""
 
     def __init__(self, groups: Sequence[Tuple[VmapEnsemble, Sequence[Optional[int]]]], cfg, n_iter: int = 20,
                  n_pix: Optional[int] = None, n_pix_bg: Optional[int] = None, lr_rot: Optional[float] = None,
@@ -310,7 +327,8 @@ class SampleGroup(_Group):
 
     def __init__(self, ens: VmapEnsemble, rows: Sequence[int], batch: Dict[str, torch.Tensor], n_iter: int,
                  impl: str = "fp32"):
-        self.ens, self.active, self.n_iter, self.lw = ens, list(rows), n_iter, _use_lw(ens, impl)
+        self.ens, self.active, self.n_iter, self.path = ens, list(rows), n_iter, _path(ens, impl)
+        self.lw = self.path == "layerwise"      # the group runs on the layer-wise path
         B, N, S = batch["pcs"].shape[:3]
         assert B == len(self.active) and N % n_iter == 0
         self.n_pix, self.S = N // n_iter, S
