@@ -735,6 +735,34 @@ int vmb_ba_step_lw(vmb_handle* h, const vmb_ba_args* a, int group, const void* i
 int vmb_track_step_fused(vmb_handle* h, const vmb_track_args* a, int group, const void* image, void* stream);
 int vmb_ba_step_fused(vmb_handle* h, const vmb_ba_args* a, int group, const void* image, void* stream);
 
+/* ---- relocalisation: the tracking loss of many candidate poses at once and their top K (vmap_b200/reloc.py; the rule
+ * is in csrc/k_reloc.cuh) ---------------------------------------------------------------------------------------------
+ *   vmb_reloc_score   hidden 32: for each hypothesis h of the device table hyps [n_hyp][4][4] (fp64 T_wc), K10's loss
+ *                     of group `group` of `a` at T_h on the group's slice (its camera-frame points, targets and masks as
+ *                     vmb_track_step reads them; the mask counts are counted once and shared by every hypothesis), from
+ *                     the fused tile's forward on the fp16 image `image` (as vmb_track_step_fused), summed in K10's order
+ *                     (rays within each vmb_track_tiles tile, tiles, then the objects by vmb_track_update's tree), ADDED
+ *                     to scores[h] (device [n_hyp] fp64: zero it before the first group).  On one group scores[h] is, bit
+ *                     for bit, the loss vmb_track_update reports for an iteration from T_h on the same slice.  terms:
+ *                     optional device [n_hyp][n_obj][4] fp64 per-object L_depth, L_colour, L_opacity, weighted total.
+ *                     Reads a's colour_scaling, opacity_scaling and status (not its pose, adam or iteration fields); the
+ *                     group's partials are checked as vmb_track_step checks them and not written.
+ *   vmb_reloc_select  the k smallest of the device scores [n] on the device: idx [k] (int) ascending by score, ties to
+ *                     the lower index, a non-finite score after every finite one; poses (optional) [k][4][4] the
+ *                     matching rows of hyps.  No host read.
+ * VMB_E_ARG: as vmb_track_step_fused, n_hyp outside [1, VMB_RELOC_MAX_HYP], k outside [1, min(n, VMB_RELOC_MAX_K)],
+ * a NULL image, hyps, scores or idx.  VMB_E_UNSUPPORTED: hidden != 32 or n_freq != 6, n_samples > 32.  On the device: a
+ * row outside [0, n_rows) contributes 0 and sets VMB_TRACK_ST_BAD_ROW.  No floating-point atomics: bitwise reproducible,
+ * and a hypothesis's score does not depend on n_hyp.  The per-ray scratch ([n_hyp][n_obj][n_rays][3] fp64 on the
+ * handle) grows on demand and is never moved once a captured graph holds it: after a capture, a call with a larger
+ * n_hyp * n_obj * n_rays fails with VMB_E_CUDA (run the largest shape eagerly first).  Registers as in k_reloc.cuh. */
+#define VMB_RELOC_MAX_HYP 4096
+#define VMB_RELOC_MAX_K 64
+int vmb_reloc_score(vmb_handle* h, const vmb_track_args* a, int group, int n_hyp, const double* hyps, double* scores,
+                    double* terms, const void* image, void* stream);
+int vmb_reloc_select(vmb_handle* h, int n, const double* scores, const double* hyps, int k, int* idx, double* poses,
+                     void* stream);
+
 /* ---- joint map-and-pose step on the layer-wise path (iMAP: network weights and keyframe poses together; the rule is
  * in csrc/k_track_lw.cuh) ---------------------------------------------------------------------------------------------
  * One mapping iteration that also yields K11's per-ray pose rows, from ONE forward and backward:

@@ -214,6 +214,7 @@ class TrackArgs(C.Structure):
 
 BA_MAX_WIN, BA_ST_BAD_FRAME = 1024, 8                          # VMB_BA_MAX_WIN, VMB_BA_ST_BAD_FRAME
 TRACK_ST_CLAMP = 16                                            # VMB_TRACK_ST_CLAMP (the count is in status[1])
+RELOC_MAX_HYP, RELOC_MAX_K = 4096, 64                          # VMB_RELOC_MAX_HYP, VMB_RELOC_MAX_K
 
 
 class BaGroup(C.Structure):
@@ -253,7 +254,7 @@ EXPORTS = (
     "vmb_hull", "vmb_obb_minvol", "vmb_render_count", "vmb_render_emit", "vmb_render_composite",
     "vmb_track_tiles", "vmb_track_step", "vmb_track_update", "vmb_ba_step", "vmb_ba_update",
     "vmb_track_step_lw", "vmb_ba_step_lw", "vmb_track_step_fused", "vmb_ba_step_fused", "vmb_joint_step_lw",
-    "vmb_joint_step_fused",
+    "vmb_joint_step_fused", "vmb_reloc_score", "vmb_reloc_select",
 )
 
 _lib = None
@@ -324,6 +325,8 @@ def lib():
         L.vmb_ba_step_lw.argtypes = [_vp, C.POINTER(BaArgs), C.c_int, _vp, _vp]
         L.vmb_track_step_fused.argtypes = [_vp, C.POINTER(TrackArgs), C.c_int, _vp, _vp]
         L.vmb_ba_step_fused.argtypes = [_vp, C.POINTER(BaArgs), C.c_int, _vp, _vp]
+        L.vmb_reloc_score.argtypes = [_vp, C.POINTER(TrackArgs), C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]
+        L.vmb_reloc_select.argtypes = [_vp, C.c_int, _vp, _vp, C.c_int, _vp, _vp, _vp]
         L.vmb_joint_step_lw.argtypes = [_vp, C.POINTER(StepArgs), C.POINTER(BaArgs), C.c_int, _vp, _vp]
         L.vmb_joint_step_fused.argtypes = [_vp, C.POINTER(StepArgs), C.POINTER(BaArgs), C.c_int, _vp, _vp]
         L.vmb_build_image.argtypes = [_vp, C.c_int, _vp, _vp, _vp]

@@ -92,6 +92,165 @@ __device__ __forceinline__ uint32_t pack_relu_h2(float lo, float hi) {
   return r;
 }
 
+// E0 and the six forward stages of one tile (the fused step's code, layout and fp16 rounding points) at this thread's
+// network input t: the embedding blocks and hidden activations to `act`, the heads (raw alpha, raw colour[3]) in point
+// layout to `hd` and zeroed dhead rows.  The weight image is in shared memory.  Ends before the CTA barrier that makes
+// the heads tile visible.  Shared by k_track_fused and the forward-only relocalisation tile (k_reloc.cuh).
+__device__ __forceinline__ void forward_tile(unsigned char* act, float* hd, const float* wf, const float* Bd,
+                                             const uf::Mma& mm, float3 t, int p, int hsel, int cq, int fr0,
+                                             uint32_t (&ua)[8]) {
+  const float t0x = t.x, t1x = t.y, t2x = t.z;
+  const uint64_t tp0 = um::pk2(t0x, t0x), tp1 = um::pk2(t1x, t1x), tp2 = um::pk2(t2x, t2x);
+  // ---- E0: positional embedding (embedding.py:82-91), the fused step's code and layout ------------------------------
+  {
+    uint4* e1 = reinterpret_cast<uint4*>(act + uf::FG_E1 * FGB + p * 16);
+    uint4* e2 = reinterpret_cast<uint4*>(act + uf::FG_E2 * FGB + p * 16);
+    const int q0 = hsel ? 3 : 0, q1 = hsel ? 5 : 3;
+    uint64_t s01, s23, c01, c23;
+    {
+      uint64_t pj01, pj23;
+      um::project4(Bd, q0, tp0, tp1, tp2, pj01, pj23);
+      um::sincos4_x2(pj01, pj23, s01, s23, c01, c23);
+    }
+#pragma unroll 1
+    for (int qq = q0; qq < q1; ++qq) {                 // directions 4qq .. 4qq+3
+      float sv[4][6];
+      uint64_t ns01 = 0, ns23 = 0, nc01 = 0, nc23 = 0;
+      if (qq + 1 < q1) {
+        uint64_t pj01, pj23;
+        um::project4(Bd, qq + 1, tp0, tp1, tp2, pj01, pj23);
+        um::sincos4_x2(pj01, pj23, ns01, ns23, nc01, nc23);
+      }
+      um::sin_doubling4_x2(s01, s23, c01, c23, sv);
+      s01 = ns01; s23 = ns23; c01 = nc01; c23 = nc23;
+      const uint4 ua = make_uint4(um::pack_h2(sv[0][0], sv[0][1]), um::pack_h2(sv[0][2], sv[0][3]), um::pack_h2(sv[1][0], sv[1][1]), um::pack_h2(sv[1][2], sv[1][3]));
+      const uint4 ub = make_uint4(um::pack_h2(sv[2][0], sv[2][1]), um::pack_h2(sv[2][2], sv[2][3]), um::pack_h2(sv[3][0], sv[3][1]), um::pack_h2(sv[3][2], sv[3][3]));
+      const uint4 uc = make_uint4(um::pack_h2(sv[0][4], sv[0][5]), um::pack_h2(sv[1][4], sv[1][5]), um::pack_h2(sv[2][4], sv[2][5]), um::pack_h2(sv[3][4], sv[3][5]));
+      e1[(2 * qq + 1) * 128] = ua; e1[(2 * qq + 2) * 128] = ub; e2[qq * 128] = uc;
+    }
+    if (hsel) {
+      // direction 20 shares chunk 0 of emb1 with [1, x, y, z] and chunk 5 of emb2 with the const-1 column
+      float s[6];
+      um::sin_ladder(fmaf(Bd[2 * um::DIRS_PITCH + 20], t2x, fmaf(Bd[um::DIRS_PITCH + 20], t1x, Bd[20] * t0x)), s);
+      e1[0] = make_uint4(um::pack_h2(1.0f, t0x), um::pack_h2(t1x, t2x), um::pack_h2(s[0], s[1]), um::pack_h2(s[2], s[3]));
+      e2[5 * 128] = make_uint4(um::pack_h2(s[4], s[5]), um::pack_h2(1.0f, 0.f), 0u, 0u);
+      e1[11 * 128] = make_uint4(0u, 0u, 0u, 0u);
+      uint4* dh = reinterpret_cast<uint4*>(act + uf::FG_DH * FGB + p * 16);   // this point's dhead row: 0 until the render
+      dh[0] = make_uint4(0u, 0u, 0u, 0u); dh[128] = make_uint4(0u, 0u, 0u, 0u);
+    }
+  }
+
+  // hidden-layer epilogue on the fragment: acc + bias -> ReLU -> fp16 into block fg (read back by the dgrad gates) and
+  // into u, the A operand of the next stage
+  auto epi_relu = [&](const float (&v)[16], int bias_off, int fg, uint32_t (&u)[8]) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 bb = *reinterpret_cast<const float2*>(wf + bias_off + 8 * j + 2 * cq);
+      unsigned char* dst = act + (fg + j) * FGB + fr0 * 16 + cq * 4;
+      u[2 * j] = pack_relu_h2(v[4 * j] + bb.x, v[4 * j + 1] + bb.y);
+      u[2 * j + 1] = pack_relu_h2(v[4 * j + 2] + bb.x, v[4 * j + 3] + bb.y);
+      *reinterpret_cast<uint32_t*>(dst) = u[2 * j];
+      *reinterpret_cast<uint32_t*>(dst + 128) = u[2 * j + 1];
+    }
+  };
+#define MMA_DONE() do { ptx::wgmma_commit(); ptx::wgmma_wait<0>(); } while (0)
+
+  // ---- forward: the fused step's six stages.  Only the embedding blocks cross warpgroups (SS A operand): one CTA
+  // barrier; every later A operand is this warpgroup's own registers (RS) or the embedding blocks again -------------
+  float acc[16], hacc[8];
+  ptx::fence_async_smem();
+  __syncthreads();
+  ptx::wgmma_fence();                                 // in_layer: emb1 (K = 96)
+#pragma unroll
+  for (int ks = 0; ks < 6; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(uf::FG_E1, ks), mm.w_k(um::IMG_WIN, ks), ks > 0);
+  MMA_DONE();
+  epi_relu(acc, um::F_BIN, uf::FG_FC1, ua);
+  ptx::wgmma_fence();                                 // mid1: fc1
+#pragma unroll
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WM1, ks), ks > 0);
+  MMA_DONE();
+  epi_relu(acc, um::F_BM1, uf::FG_FC2, ua);
+  ptx::wgmma_fence();                                 // cat_layer: [fc2 | emb1] (K = 128)
+#pragma unroll
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WCAT, ks), ks > 0);
+#pragma unroll
+  for (int ks = 2; ks < 8; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(uf::FG_FC2, ks), mm.w_k(um::IMG_WCAT, ks), 1u);
+  MMA_DONE();
+  epi_relu(acc, um::F_BCAT, uf::FG_FC3, ua);
+  ptx::wgmma_fence();                                 // mid2: fc3
+#pragma unroll
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WM2, ks), ks > 0);
+  MMA_DONE();
+  epi_relu(acc, um::F_BM2, uf::FG_FC4, ua);
+  ptx::wgmma_fence();                                 // color_linear: [fc4 | emb2] (K = 80) ; out_alpha: fc4 -> column 0
+#pragma unroll
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WCL, ks), ks > 0);
+#pragma unroll
+  for (int ks = 2; ks < 5; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(uf::FG_FC4, ks), mm.w_k(um::IMG_WCL, ks), 1u);
+#pragma unroll
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<0>(hacc, ua + 4 * ks, mm.w16_k(um::IMG_WA16, ks), ks > 0);
+  MMA_DONE();
+  epi_relu(acc, um::F_BCL, uf::FG_HC, ua);
+  if (cq == 0) { hd[fr0 * 4] = hacc[0]; hd[(fr0 + 8) * 4] = hacc[2]; }
+  ptx::wgmma_fence();                                 // out_color: hc -> columns 1..3
+#pragma unroll
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<0>(hacc, ua + 4 * ks, mm.w16_k(um::IMG_WOC16, ks), ks > 0);
+  MMA_DONE();
+  if (cq == 0) { hd[fr0 * 4 + 1] = hacc[1]; hd[(fr0 + 8) * 4 + 1] = hacc[3]; }
+  if (cq == 1) { hd[fr0 * 4 + 2] = hacc[0]; hd[fr0 * 4 + 3] = hacc[1]; hd[(fr0 + 8) * 4 + 2] = hacc[2]; hd[(fr0 + 8) * 4 + 3] = hacc[3]; }
+#undef MMA_DONE
+}
+
+// One sample's heads (point layout, from forward_tile) rendered along its ray by K10's rule, one lane per sample, the
+// ray's lanes [seg_lo, seg_lo + S) adjacent in the warp (every lane of the ray runs the sums): the heads' sigmoids in
+// fp32, then the fp64 render in sample order (1 - occ as sigmoid(-alpha)) and the detached depth variance.  Also this
+// sample's transmittance and weight in fp32 (the backward's).
+struct RayRender {
+  float al, oc, c0, c1, c2, Ts, wgt;
+  double D, O, C0, C1, C2, V;
+};
+
+__device__ __forceinline__ RayRender render_ray(const float* hd, const float* wf, float zv, int p, int S, int sidx,
+                                                int seg_lo) {
+  const unsigned FULL = 0xffffffffu;
+  RayRender r;
+  const float4 hv = *reinterpret_cast<const float4*>(hd + p * 4);
+  const float al = (hv.x + wf[um::F_BA]) * 10.0f;  // model.py:77
+  const float oc = vmb_sigmoid(al);                 // render_rays.py:6
+  const float c0 = vmb_sigmoid(hv.y + wf[um::F_BOC]), c1 = vmb_sigmoid(hv.z + wf[um::F_BOC + 1]),
+              c2 = vmb_sigmoid(hv.w + wf[um::F_BOC + 2]);
+  double Tr = 1.0, D = 0.0, O = 0.0, C0 = 0.0, C1 = 0.0, C2 = 0.0;
+  float Ts = 0.f, wgt = 0.f;
+  for (int s = 0; s < S; ++s) {                     // the ray's samples in order
+    const int src = seg_lo + s;
+    const float al_s = __shfl_sync(FULL, al, src), oc_s = __shfl_sync(FULL, oc, src), z_s = __shfl_sync(FULL, zv, src);
+    const float c0_s = __shfl_sync(FULL, c0, src), c1_s = __shfl_sync(FULL, c1, src), c2_s = __shfl_sync(FULL, c2, src);
+    const double wd = (double)oc_s * Tr;
+    if (sidx == s) { Ts = (float)Tr; wgt = (float)wd; }
+    D += wd * (double)z_s; O += wd;
+    C0 += wd * (double)c0_s; C1 += wd * (double)c1_s; C2 += wd * (double)c2_s;
+    Tr *= ((double)vmb_sigmoid(-al_s) + 1e-10);
+  }
+  double V = 0.0;
+  for (int s = 0; s < S; ++s) {
+    const double dz = (double)__shfl_sync(FULL, zv, seg_lo + s) - D;
+    V += (double)__shfl_sync(FULL, wgt, seg_lo + s) * dz * dz;   // loss.py:28-29 (detached)
+  }
+  r.al = al; r.oc = oc; r.c0 = c0; r.c1 = c1; r.c2 = c2; r.Ts = Ts; r.wgt = wgt;
+  r.D = D; r.O = O; r.C0 = C0; r.C1 = C1; r.C2 = C2; r.V = V;
+  return r;
+}
+
+// the object's slice mask counts (nd, no, ns) from warp_mask_counts' per-warp sums
+__device__ __forceinline__ void red_counts(const int (&red)[3][NT / 32], int (&cnt)[3]) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    cnt[c] = 0;
+#pragma unroll
+    for (int w = 0; w < NT / 32; ++w) cnt[c] += red[c][w];
+  }
+}
+
 // One CTA = tile blockIdx.x of object blockIdx.y.  nr = 4 rpw rays per tile, rpw = 32 / S rays per warp.
 // BA = false: per-ray terms to gray / lray (k_tf_reduce forms K10's partials); BA = true: K11's rows x.rows.
 template <bool BA>
@@ -167,60 +326,10 @@ __global__ void __launch_bounds__(NT, 2) k_track_fused(TrackParams a, BaRays x, 
   mm.mh = hsel;
   um::mbar_wait_or_trap(wbar, 0);
 
-  // ---- E0: positional embedding (embedding.py:82-91), the fused step's code and layout ------------------------------
   const float t0x = t.x, t1x = t.y, t2x = t.z;
   const uint64_t tp0 = um::pk2(t0x, t0x), tp1 = um::pk2(t1x, t1x), tp2 = um::pk2(t2x, t2x);
-  {
-    uint4* e1 = reinterpret_cast<uint4*>(act + uf::FG_E1 * FGB + p * 16);
-    uint4* e2 = reinterpret_cast<uint4*>(act + uf::FG_E2 * FGB + p * 16);
-    const int q0 = hsel ? 3 : 0, q1 = hsel ? 5 : 3;
-    uint64_t s01, s23, c01, c23;
-    {
-      uint64_t pj01, pj23;
-      um::project4(Bd, q0, tp0, tp1, tp2, pj01, pj23);
-      um::sincos4_x2(pj01, pj23, s01, s23, c01, c23);
-    }
-#pragma unroll 1
-    for (int qq = q0; qq < q1; ++qq) {                 // directions 4qq .. 4qq+3
-      float sv[4][6];
-      uint64_t ns01 = 0, ns23 = 0, nc01 = 0, nc23 = 0;
-      if (qq + 1 < q1) {
-        uint64_t pj01, pj23;
-        um::project4(Bd, qq + 1, tp0, tp1, tp2, pj01, pj23);
-        um::sincos4_x2(pj01, pj23, ns01, ns23, nc01, nc23);
-      }
-      um::sin_doubling4_x2(s01, s23, c01, c23, sv);
-      s01 = ns01; s23 = ns23; c01 = nc01; c23 = nc23;
-      const uint4 ua = make_uint4(um::pack_h2(sv[0][0], sv[0][1]), um::pack_h2(sv[0][2], sv[0][3]), um::pack_h2(sv[1][0], sv[1][1]), um::pack_h2(sv[1][2], sv[1][3]));
-      const uint4 ub = make_uint4(um::pack_h2(sv[2][0], sv[2][1]), um::pack_h2(sv[2][2], sv[2][3]), um::pack_h2(sv[3][0], sv[3][1]), um::pack_h2(sv[3][2], sv[3][3]));
-      const uint4 uc = make_uint4(um::pack_h2(sv[0][4], sv[0][5]), um::pack_h2(sv[1][4], sv[1][5]), um::pack_h2(sv[2][4], sv[2][5]), um::pack_h2(sv[3][4], sv[3][5]));
-      e1[(2 * qq + 1) * 128] = ua; e1[(2 * qq + 2) * 128] = ub; e2[qq * 128] = uc;
-    }
-    if (hsel) {
-      // direction 20 shares chunk 0 of emb1 with [1, x, y, z] and chunk 5 of emb2 with the const-1 column
-      float s[6];
-      um::sin_ladder(fmaf(Bd[2 * um::DIRS_PITCH + 20], t2x, fmaf(Bd[um::DIRS_PITCH + 20], t1x, Bd[20] * t0x)), s);
-      e1[0] = make_uint4(um::pack_h2(1.0f, t0x), um::pack_h2(t1x, t2x), um::pack_h2(s[0], s[1]), um::pack_h2(s[2], s[3]));
-      e2[5 * 128] = make_uint4(um::pack_h2(s[4], s[5]), um::pack_h2(1.0f, 0.f), 0u, 0u);
-      e1[11 * 128] = make_uint4(0u, 0u, 0u, 0u);
-      uint4* dh = reinterpret_cast<uint4*>(act + uf::FG_DH * FGB + p * 16);   // this point's dhead row: 0 until the render
-      dh[0] = make_uint4(0u, 0u, 0u, 0u); dh[128] = make_uint4(0u, 0u, 0u, 0u);
-    }
-  }
-
-  // hidden-layer epilogue on the fragment: acc + bias -> ReLU -> fp16 into block fg (read back by the dgrad gates) and
-  // into u, the A operand of the next stage
-  auto epi_relu = [&](const float (&v)[16], int bias_off, int fg, uint32_t (&u)[8]) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 bb = *reinterpret_cast<const float2*>(wf + bias_off + 8 * j + 2 * cq);
-      unsigned char* dst = act + (fg + j) * FGB + fr0 * 16 + cq * 4;
-      u[2 * j] = pack_relu_h2(v[4 * j] + bb.x, v[4 * j + 1] + bb.y);
-      u[2 * j + 1] = pack_relu_h2(v[4 * j + 2] + bb.x, v[4 * j + 3] + bb.y);
-      *reinterpret_cast<uint32_t*>(dst) = u[2 * j];
-      *reinterpret_cast<uint32_t*>(dst + 128) = u[2 * j + 1];
-    }
-  };
+  uint32_t ua[8];
+  forward_tile(act, hd, wf, Bd, mm, t, p, hsel, cq, fr0, ua);
   // dgrad epilogue: dY = (h > 0) * fp16(acc), h from its block; dY only in registers (no weight gradient reads it)
   auto epi_dgrad = [&](const float (&v)[16], int fg_h, uint32_t (&u)[8]) {
 #pragma unroll
@@ -247,84 +356,16 @@ __global__ void __launch_bounds__(NT, 2) k_track_fused(TrackParams a, BaRays x, 
     o[0] = u0.x; o[1] = u0.y; o[2] = u0.z; o[3] = u0.w; o[4] = u1.x; o[5] = u1.y; o[6] = u1.z; o[7] = u1.w;
   };
 #define MMA_DONE() do { ptx::wgmma_commit(); ptx::wgmma_wait<0>(); } while (0)
-
-  // ---- forward: the fused step's six stages.  Only the embedding blocks cross warpgroups (SS A operand): one CTA
-  // barrier; every later A operand is this warpgroup's own registers (RS) or the embedding blocks again -------------
   float acc[16], hacc[8];
-  uint32_t ua[8];
-  ptx::fence_async_smem();
-  __syncthreads();
-  ptx::wgmma_fence();                                 // in_layer: emb1 (K = 96)
-#pragma unroll
-  for (int ks = 0; ks < 6; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(uf::FG_E1, ks), mm.w_k(um::IMG_WIN, ks), ks > 0);
-  MMA_DONE();
-  epi_relu(acc, um::F_BIN, uf::FG_FC1, ua);
-  ptx::wgmma_fence();                                 // mid1: fc1
-#pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WM1, ks), ks > 0);
-  MMA_DONE();
-  epi_relu(acc, um::F_BM1, uf::FG_FC2, ua);
-  ptx::wgmma_fence();                                 // cat_layer: [fc2 | emb1] (K = 128)
-#pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WCAT, ks), ks > 0);
-#pragma unroll
-  for (int ks = 2; ks < 8; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(uf::FG_FC2, ks), mm.w_k(um::IMG_WCAT, ks), 1u);
-  MMA_DONE();
-  epi_relu(acc, um::F_BCAT, uf::FG_FC3, ua);
-  ptx::wgmma_fence();                                 // mid2: fc3
-#pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WM2, ks), ks > 0);
-  MMA_DONE();
-  epi_relu(acc, um::F_BM2, uf::FG_FC4, ua);
-  ptx::wgmma_fence();                                 // color_linear: [fc4 | emb2] (K = 80) ; out_alpha: fc4 -> column 0
-#pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WCL, ks), ks > 0);
-#pragma unroll
-  for (int ks = 2; ks < 5; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(uf::FG_FC4, ks), mm.w_k(um::IMG_WCL, ks), 1u);
-#pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<0>(hacc, ua + 4 * ks, mm.w16_k(um::IMG_WA16, ks), ks > 0);
-  MMA_DONE();
-  epi_relu(acc, um::F_BCL, uf::FG_HC, ua);
-  if (cq == 0) { hd[fr0 * 4] = hacc[0]; hd[(fr0 + 8) * 4] = hacc[2]; }
-  ptx::wgmma_fence();                                 // out_color: hc -> columns 1..3
-#pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<0>(hacc, ua + 4 * ks, mm.w16_k(um::IMG_WOC16, ks), ks > 0);
-  MMA_DONE();
-  if (cq == 0) { hd[fr0 * 4 + 1] = hacc[1]; hd[(fr0 + 8) * 4 + 1] = hacc[3]; }
-  if (cq == 1) { hd[fr0 * 4 + 2] = hacc[0]; hd[fr0 * 4 + 3] = hacc[1]; hd[(fr0 + 8) * 4 + 2] = hacc[2]; hd[(fr0 + 8) * 4 + 3] = hacc[3]; }
   __syncthreads();                                    // heads tile (fragment layout -> point layout); mask counts
 
   // ---- render + loss + d(raw alpha, raw colour): K10's rule, one lane per sample in the warps of warpgroup 0 ---------
   if (hsel == 0) {                                    // warp-uniform
-    const float4 hv = *reinterpret_cast<const float4*>(hd + p * 4);
-    const float al = (hv.x + wf[um::F_BA]) * 10.0f;  // model.py:77
-    const float oc = vmb_sigmoid(al);                 // render_rays.py:6
-    const float c0 = vmb_sigmoid(hv.y + wf[um::F_BOC]), c1 = vmb_sigmoid(hv.z + wf[um::F_BOC + 1]),
-                c2 = vmb_sigmoid(hv.w + wf[um::F_BOC + 2]);
-    double Tr = 1.0, D = 0.0, O = 0.0, C0 = 0.0, C1 = 0.0, C2 = 0.0;
-    float Ts = 0.f, wgt = 0.f;
-    for (int s = 0; s < S; ++s) {                     // the ray's samples in order (every lane of the ray runs the sums)
-      const int src = seg_lo + s;
-      const float al_s = __shfl_sync(FULL, al, src), oc_s = __shfl_sync(FULL, oc, src), z_s = __shfl_sync(FULL, zv, src);
-      const float c0_s = __shfl_sync(FULL, c0, src), c1_s = __shfl_sync(FULL, c1, src), c2_s = __shfl_sync(FULL, c2, src);
-      const double wd = (double)oc_s * Tr;
-      if (sidx == s) { Ts = (float)Tr; wgt = (float)wd; }
-      D += wd * (double)z_s; O += wd;
-      C0 += wd * (double)c0_s; C1 += wd * (double)c1_s; C2 += wd * (double)c2_s;
-      Tr *= ((double)vmb_sigmoid(-al_s) + 1e-10);
-    }
-    double V = 0.0;
-    for (int s = 0; s < S; ++s) {
-      const double dz = (double)__shfl_sync(FULL, zv, seg_lo + s) - D;
-      V += (double)__shfl_sync(FULL, wgt, seg_lo + s) * dz * dz;   // loss.py:28-29 (detached)
-    }
+    const RayRender rr = render_ray(hd, wf, zv, p, S, sidx, seg_lo);
+    const float al = rr.al, oc = rr.oc, c0 = rr.c0, c1 = rr.c1, c2 = rr.c2, Ts = rr.Ts, wgt = rr.wgt;
+    const double D = rr.D, O = rr.O, C0 = rr.C0, C1 = rr.C1, C2 = rr.C2, V = rr.V;
     int cnt[3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      cnt[c] = 0;
-#pragma unroll
-      for (int w = 0; w < NT / 32; ++w) cnt[c] += red[c][w];
-    }
+    red_counts(red, cnt);
     RayLoss ls = {{0.0, 0.0, 0.0}, 0.f, 0.f, 0.f, 0.f, 0.f};
     if (live) {
       if (BA && !pok && sidx == 0 && a.status) atomicOr(a.status, VMB_BA_ST_BAD_FRAME);

@@ -26,6 +26,7 @@
 #include "k_ba.cuh"
 #include "k_track_lw.cuh"
 #include "k_track_fused.cuh"
+#include "k_reloc.cuh"
 
 struct vmb_handle {
   int device, max_obj, H, nfreq;
@@ -53,6 +54,7 @@ struct vmb_handle {
   lw::TrackWorkspace ws_ba;   // layer-wise bundle-adjustment step: likewise (and tracking never moves a BA capture's)
   lw::JointWorkspace ws_joint;// joint map-and-pose step: world points and pose terms (the activations are the step's ws)
   tf::Workspace ws_tf;        // fused hidden-32 tracking step: per-ray rows before K10's tile sums (BA writes its rows)
+  rl::Workspace ws_reloc;     // relocalisation scoring: per-(hypothesis, ray) loss terms before K10's tile sums
   std::string err;
 };
 
@@ -188,6 +190,7 @@ void vmb_destroy(vmb_handle* h) {
   h->ws_ba.release();
   h->ws_joint.release();
   h->ws_tf.release();
+  h->ws_reloc.release();
   delete h;
 }
 
@@ -1419,6 +1422,36 @@ int vmb_track_step_fused(vmb_handle* h, const vmb_track_args* a, int group, cons
 
 int vmb_ba_step_fused(vmb_handle* h, const vmb_ba_args* a, int group, const void* image, void* stream) {
   return pose_step<POSE_FUSED>(h, a, group, image, stream, "vmb_ba_step_fused");
+}
+
+int vmb_reloc_score(vmb_handle* h, const vmb_track_args* a, int group, int n_hyp, const double* hyps, double* scores,
+                    double* terms, const void* image, void* stream) {
+  const char* who = "vmb_reloc_score";
+  if (!h) return fail(h, VMB_E_ARG, std::string(who) + ": null handle");
+  if (!a || a->n_groups < 1 || a->n_groups > VMB_TRACK_MAX_GROUPS || group < 0 || group >= a->n_groups)
+    return fail(h, VMB_E_ARG, std::string(who) + ": null arguments or group index outside [0, n_groups)");
+  if (n_hyp < 1 || n_hyp > VMB_RELOC_MAX_HYP || !hyps || !scores)
+    return fail(h, VMB_E_ARG, std::string(who) + ": need 1 <= n_hyp <= VMB_RELOC_MAX_HYP, hyps and scores");
+  const auto& g = a->group[group];
+  TrackParams tp;
+  const int tiles = pose_group_params(h, g, hyps, a, who, POSE_FUSED, image, tp);
+  if (tiles < 0) return tiles;
+  std::string err;
+  const int rc = rl::launch_reloc_fused(h->ws_reloc, h->L, tp, image, hyps, n_hyp, scores, terms,
+                                        fp32_tile(32) / g.n_samples, h->n_sm, (cudaStream_t)stream, err);
+  if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, std::string(who) + ": " + err);
+  return VMB_OK;
+}
+
+int vmb_reloc_select(vmb_handle* h, int n, const double* scores, const double* hyps, int k, int* idx, double* poses,
+                     void* stream) {
+  if (n < 1 || n > VMB_RELOC_MAX_HYP || k < 1 || k > VMB_RELOC_MAX_K || k > n || !scores || !idx || (poses && !hyps))
+    return fail(h, VMB_E_ARG, "vmb_reloc_select: need 1 <= k <= min(n, VMB_RELOC_MAX_K), n <= VMB_RELOC_MAX_HYP, "
+                              "scores, idx, and hyps when poses are asked for");
+  rl::k_reloc_select<<<(unsigned)((n + 255) / 256), 256, (size_t)n * sizeof(double), (cudaStream_t)stream>>>(
+      n, scores, hyps, k, idx, poses);
+  CUDA_TRY(h, cudaGetLastError());
+  return VMB_OK;
 }
 
 int vmb_track_update(vmb_handle* h, const vmb_track_args* a, void* stream) {
