@@ -5,7 +5,7 @@
 //   Samples  the frame's camera-frame points q of one ray slice (the tracker's own draw), shared by every hypothesis:
 //            nothing is sampled per hypothesis.  The mask counts depend on the pixels only, so each CTA counts its
 //            object's once and every hypothesis it scores uses them.
-//   Forward  forward_tile and render_ray of k_track_fused.cuh, unchanged: pose_point with T_h, E0 and the six forward
+//   Forward  load_object, forward_tile and render_ray of k_track_fused.cuh: pose_point with T_h, E0 and the six forward
 //            wgmma stages from the object's fp16 image row, the heads, the fp64 render and ray_loss (per-object,
 //            per-term empty masks, weights 1 / colour_scaling / opacity_scaling).  No input-gradient chain, no pose
 //            terms.  One CTA = one fused tile of one object (blockIdx.y) and a chunk of hypotheses (blockIdx.z): the
@@ -76,20 +76,7 @@ __global__ void __launch_bounds__(NT, 2) k_reloc_fused(TrackParams a, const unsi
     if (tid == 0 && a.status) atomicOr(a.status, VMB_TRACK_ST_BAD_ROW);
     return;
   }
-  uint64_t* wbar = reinterpret_cast<uint64_t*>(smem + SM_BAR);
-  if (tid == 0) { ptx::mbar_init(wbar, 1); ptx::mbar_init_fence(); }
-  __syncthreads();
-  if (tid == 0) {                                     // the object's weight image: in flight while the mask counts run
-    ptx::mbar_arrive_expect_tx(wbar, um::IMG_BYTES);
-    ptx::bulk_g2s(smem + SM_W, image + (size_t)row * um::IMG_BYTES, um::IMG_BYTES, wbar);
-  }
-  {                                                   // the object's mask counts of this slice, once per CTA
-    const unsigned char* sv = a.sem + (size_t)b * a.sem_stride;
-    const unsigned char* mv = a.mask + (size_t)b * a.mask_stride;
-    int nd = 0, no = 0, ns = 0;
-    for (int r = tid; r < R; r += NT) slice_mask_count(sv, mv, r, nd, no, ns);
-    warp_mask_counts(tid, nd, no, ns, red);
-  }
+  const uf::Tile tl = load_object(smem, image, row, a, red, quad);
   const float sc = a.scale[row];
   float3 q = make_float3(0.f, 0.f, 0.f);
   if (live) {
@@ -99,27 +86,18 @@ __global__ void __launch_bounds__(NT, 2) k_reloc_fused(TrackParams a, const unsi
   float zv = 0.f;
   if (hsel == 0 && live) zv = a.z[(size_t)b * a.z_stride + (size_t)ray * S + sidx];
 
-  unsigned char* act = smem + SM_ACT;
-  float* hd = reinterpret_cast<float*>(smem + SM_HD);
-  const float* wf = reinterpret_cast<const float*>(smem + SM_W + um::IMG_F32);
-  const float* Bd = wf + um::F_DIRS;
-  const int cq = lane & 3, fr0 = 64 * hsel + 16 * quad + (lane >> 2);
-  uf::Mma mm;
-  mm.a16 = ptx::smem_u32(act) >> 4;
-  mm.w16 = ptx::smem_u32(smem + SM_W) >> 4;
-  mm.mh = hsel;
-  um::mbar_wait_or_trap(wbar, 0);
+  image_ready(smem);
 
   // No barrier closes an iteration: after the heads barrier only warpgroup 0's render reads shared memory, and only
   // the heads tile, which the next iteration writes after forward_tile's own barrier.
 #pragma unroll 1
   for (int h = h0; h < h1; ++h) {
-    const float3 t = live ? pose_point(hyps + (size_t)h * 16, q, sc) : make_float3(0.f, 0.f, 0.f);
+    const uf::PeIn tin(live ? pose_point(hyps + (size_t)h * 16, q, sc) : make_float3(0.f, 0.f, 0.f));
     uint32_t ua[8];
-    forward_tile(act, hd, wf, Bd, mm, t, p, hsel, cq, fr0, ua);
+    forward_tile(tl, tin, ua);
     __syncthreads();                                  // heads tile (fragment layout -> point layout); mask counts
     if (hsel == 0) {                                  // warp-uniform
-      const RayRender rr = render_ray(hd, wf, zv, p, S, sidx, seg_lo);
+      const RayRender rr = render_ray(tl.hd, tl.wf, zv, p, S, sidx, seg_lo);
       int cnt[3];
       red_counts(red, cnt);
       if (live && sidx == 0) {

@@ -201,6 +201,205 @@ __device__ __forceinline__ int cta_of_tile(const Ranges& rg, int G, int tile) { 
   return lo;
 }
 
+// a point's network input t and, for the PE's paired fp32 arithmetic (um::project4), each coordinate twice
+struct PeIn {
+  float3 t;
+  uint64_t p0, p1, p2;
+  __device__ __forceinline__ explicit PeIn(float3 v)
+      : t(v), p0(um::pk2(v.x, v.x)), p1(um::pk2(v.y, v.y)), p2(um::pk2(v.z, v.z)) {}
+};
+
+// ---- The network on one tile as the training step (k_step_fused), the pose step (k_track_fused.cuh) and
+// relocalisation scoring (k_reloc.cuh) run it: the tile's shared-memory blocks, the two thread layouts and the wgmma
+// descriptors, with one copy of the positional embedding, the hidden-layer and dgrad epilogues, the embedding-gradient
+// tile's stores and loads and the PE backward -- their operand layout and fp16 rounding points.
+struct Tile {
+  unsigned char* act;              // activation blocks (FG_*)
+  unsigned char* eg;               // fp32 embedding-gradient tile (EG_*)
+  float* hd;                       // heads tile: [128 points][alpha, r, g, b]
+  const float* wf;                 // fp32 part of the weight image: biases, heads, PE directions
+  const float* Bd;
+  Mma mm;
+  // point layout (PE, heads, render: one thread pair per point): point slot, direction half (= warpgroup) ...
+  int p, hsel;
+  // ... and accumulator-fragment layout (wgmma m64nN): this thread holds rows fr0 and fr0 + 8, columns 8j + 2 cq + {0, 1}
+  int cq, fr0;
+
+  // quad: this thread's warp within its warpgroup
+  __device__ __forceinline__ Tile(unsigned char* act_, unsigned char* eg_, unsigned char* w, float* hd_, int quad)
+      : act(act_), eg(eg_), hd(hd_), wf(reinterpret_cast<const float*>(w + um::IMG_F32)), Bd(wf + um::F_DIRS) {
+    const int tid = threadIdx.x, lane = tid & 31;
+    p = tid & 127; hsel = tid >> 7;
+    cq = lane & 3; fr0 = 64 * hsel + 16 * quad + (lane >> 2);
+    mm.a16 = ptx::smem_u32(act) >> 4;
+    mm.w16 = ptx::smem_u32(w) >> 4;
+    mm.mh = hsel;
+  }
+
+  // E0: positional embedding (embedding.py:82-91) of this thread's network input into E1 / E2, and this point's
+  // dhead row zeroed (cols 4..15 stay zero; 0..3 are written after the render)
+  __device__ __forceinline__ void embed(const PeIn& in) const {
+    const float3 t = in.t;
+    uint4* e1 = reinterpret_cast<uint4*>(act + FG_E1 * FGB + p * 16);
+    uint4* e2 = reinterpret_cast<uint4*>(act + FG_E2 * FGB + p * 16);
+    const int q0 = hsel ? 3 : 0, q1 = hsel ? 5 : 3;
+    // software pipeline over the 4-direction chunks: the NEXT chunk's projections, range reduction and MUFU
+    // sin / cos are issued before the CURRENT chunk's doubling recurrence, which hides their latency
+    uint64_t s01, s23, c01, c23;
+    {
+      uint64_t pj01, pj23;
+      um::project4(Bd, q0, in.p0, in.p1, in.p2, pj01, pj23);
+      um::sincos4_x2(pj01, pj23, s01, s23, c01, c23);
+    }
+#pragma unroll 1
+    for (int q = q0; q < q1; ++q) {                    // directions 4q .. 4q+3
+      float sv[4][6];
+      uint64_t ns01 = 0, ns23 = 0, nc01 = 0, nc23 = 0;
+      if (q + 1 < q1) {
+        uint64_t pj01, pj23;
+        um::project4(Bd, q + 1, in.p0, in.p1, in.p2, pj01, pj23);
+        um::sincos4_x2(pj01, pj23, ns01, ns23, nc01, nc23);
+      }
+      um::sin_doubling4_x2(s01, s23, c01, c23, sv);
+      s01 = ns01; s23 = ns23; c01 = nc01; c23 = nc23;
+      const uint4 ua = make_uint4(um::pack_h2(sv[0][0], sv[0][1]), um::pack_h2(sv[0][2], sv[0][3]), um::pack_h2(sv[1][0], sv[1][1]), um::pack_h2(sv[1][2], sv[1][3]));
+      const uint4 ub = make_uint4(um::pack_h2(sv[2][0], sv[2][1]), um::pack_h2(sv[2][2], sv[2][3]), um::pack_h2(sv[3][0], sv[3][1]), um::pack_h2(sv[3][2], sv[3][3]));
+      const uint4 uc = make_uint4(um::pack_h2(sv[0][4], sv[0][5]), um::pack_h2(sv[1][4], sv[1][5]), um::pack_h2(sv[2][4], sv[2][5]), um::pack_h2(sv[3][4], sv[3][5]));
+      e1[(2 * q + 1) * 128] = ua; e1[(2 * q + 2) * 128] = ub; e2[q * 128] = uc;
+    }
+    if (hsel) {
+      // direction 20 shares chunk 0 of emb1 with [1, x, y, z] and chunk 5 of emb2 with the const-1 column
+      float s[6];
+      um::sin_ladder(fmaf(Bd[2 * um::DIRS_PITCH + 20], t.z, fmaf(Bd[um::DIRS_PITCH + 20], t.y, Bd[20] * t.x)), s);
+      const uint4 u0 = make_uint4(um::pack_h2(1.0f, t.x), um::pack_h2(t.y, t.z), um::pack_h2(s[0], s[1]), um::pack_h2(s[2], s[3]));
+      const uint4 u5 = make_uint4(um::pack_h2(s[4], s[5]), um::pack_h2(1.0f, 0.f), 0u, 0u);
+      e1[0] = u0;
+      e2[5 * 128] = u5;
+      e1[11 * 128] = make_uint4(0u, 0u, 0u, 0u);
+      uint4* dh = reinterpret_cast<uint4*>(act + FG_DH * FGB + p * 16);
+      dh[0] = make_uint4(0u, 0u, 0u, 0u); dh[128] = make_uint4(0u, 0u, 0u, 0u);
+    }
+  }
+
+  // hidden-layer epilogue on the fragment: acc + bias -> ReLU -> fp16 into block fg (read back by the dgrad gates), and
+  // into u: the A operand (ptx::wgmma_n32_rs) of the next stage's two k-steps over these 32 features
+  __device__ __forceinline__ void epi_relu(const float (&v)[16], int bias_off, int fg, uint32_t (&u)[8]) const {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 bb = *reinterpret_cast<const float2*>(wf + bias_off + 8 * j + 2 * cq);
+      unsigned char* dst = act + (fg + j) * FGB + fr0 * 16 + cq * 4;
+      u[2 * j] = pack_relu_h2(v[4 * j] + bb.x, v[4 * j + 1] + bb.y);
+      u[2 * j + 1] = pack_relu_h2(v[4 * j + 2] + bb.x, v[4 * j + 3] + bb.y);
+      *reinterpret_cast<uint32_t*>(dst) = u[2 * j];
+      *reinterpret_cast<uint32_t*>(dst + 128) = u[2 * j + 1];
+    }
+  }
+  // dgrad epilogue: dY = (h > 0) * fp16(acc); h is read from its own block, dY goes into u (the A operand of the dgrad
+  // GEMMs that read dY) and, under STORE (the training step), to block fg_out, whose readers have retired, for the
+  // weight-gradient GEMMs
+  template <bool STORE>
+  __device__ __forceinline__ void epi_dgrad(const float (&v)[16], int fg_h, int fg_out, uint32_t (&u)[8]) const {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int off = j * FGB + fr0 * 16 + cq * 4;
+      const uint32_t h0 = *reinterpret_cast<const uint32_t*>(act + fg_h * FGB + off);
+      const uint32_t h1 = *reinterpret_cast<const uint32_t*>(act + fg_h * FGB + off + 128);
+      u[2 * j] = um::gate_h2(um::pack_h2(v[4 * j], v[4 * j + 1]), h0);
+      u[2 * j + 1] = um::gate_h2(um::pack_h2(v[4 * j + 2], v[4 * j + 3]), h1);
+      if constexpr (STORE) {
+        *reinterpret_cast<uint32_t*>(act + fg_out * FGB + off) = u[2 * j];
+        *reinterpret_cast<uint32_t*>(act + fg_out * FGB + off + 128) = u[2 * j + 1];
+      }
+    }
+  }
+  // embedding-gradient fragment (8-column groups starting at 4-column block blk0) -> the shared fp32 tile
+  template <int N>
+  __device__ __forceinline__ void eg_store(const float (&v)[N], int blk0) const {
+#pragma unroll
+    for (int j = 0; j < N / 4; ++j) {
+      float* d = reinterpret_cast<float*>(eg + (blk0 + 2 * j + (cq >> 1)) * FGB + fr0 * 16 + (cq & 1) * 8);
+      *reinterpret_cast<float2*>(d) = make_float2(v[4 * j], v[4 * j + 1]);
+      *reinterpret_cast<float2*>(d + 32) = make_float2(v[4 * j + 2], v[4 * j + 3]);
+    }
+  }
+  // eight consecutive embedding-gradient columns of this thread's point
+  __device__ __forceinline__ void eg_load8(int blk, float (&o)[8]) const {
+    const float4 u0 = *reinterpret_cast<const float4*>(eg + blk * FGB + p * 16);
+    const float4 u1 = *reinterpret_cast<const float4*>(eg + (blk + 1) * FGB + p * 16);
+    o[0] = u0.x; o[1] = u0.y; o[2] = u0.z; o[3] = u0.w; o[4] = u1.x; o[5] = u1.y; o[6] = u1.z; o[7] = u1.w;
+  }
+
+  // PE backward from the eg tile: dproj_d = pi * sum_k 2^k g_{k,d} cos(pi 2^k proj_d) for this warpgroup's directions
+  // (hsel 0: 0..11, hsel 1: 12..20), under DPROJ written as the fp16 dproj block (A of the dB wgrad).  Returns this
+  // warpgroup's half of the point's dL/dt = INV_LS (dE_xyz + sum_d dproj_d B_d) in fp32 (the rule of k_tlw_pose),
+  // summed in a fixed order: hsel 0 dE_xyz, then directions 0..11; hsel 1 directions 12..20.  A caller that does not
+  // read it does not compute it.  The pose tile has no dproj block (DPROJ = false).
+  template <bool DPROJ>
+  __device__ __forceinline__ float3 pe_backward(const PeIn& in) const {
+    const float3 t = in.t;
+    const int q0 = hsel ? 3 : 0, q1 = hsel ? 5 : 3;
+    float jt0 = 0.f, jt1 = 0.f, jt2 = 0.f;
+    if (!hsel) {                                      // emb1 cols 1..3 = d/d[x y z]
+      const float4 e0 = *reinterpret_cast<const float4*>(eg + p * 16);
+      jt0 = e0.y * INV_LS; jt1 = e0.z * INV_LS; jt2 = e0.w * INV_LS;
+    }
+    uint64_t c01, c23;
+    {
+      uint64_t pj01, pj23;
+      um::project4(Bd, q0, in.p0, in.p1, in.p2, pj01, pj23);
+      um::cos4_x2(pj01, pj23, c01, c23);
+    }
+#pragma unroll 1
+    for (int q = q0; q < q1; ++q) {
+      float g1a[8], g1b[8], g2[8];
+      eg_load8(4 * q + 2, g1a);                      // emb1 cols of directions 4q, 4q+1 (k = 0..3)
+      eg_load8(4 * q + 4, g1b);                      //                          4q+2, 4q+3
+      eg_load8(EG_E2 + 2 * q, g2);                   // emb2 cols (k = 4, 5)
+      float cv[4][6], dp[4];
+      uint64_t nc01 = 0, nc23 = 0;
+      if (q + 1 < q1) {                              // next chunk's front half before this chunk's recurrence
+        uint64_t pj01, pj23;
+        um::project4(Bd, q + 1, in.p0, in.p1, in.p2, pj01, pj23);
+        um::cos4_x2(pj01, pj23, nc01, nc23);
+      }
+      um::cos_doubling4_x2(c01, c23, cv);
+      c01 = nc01; c23 = nc23;
+#pragma unroll
+      for (int dd = 0; dd < 4; ++dd) {
+        const float* g1 = (dd < 2) ? (g1a + dd * 4) : (g1b + (dd - 2) * 4);
+        float d = g1[0] * cv[dd][0];
+        d = fmaf(2.f * g1[1], cv[dd][1], d);
+        d = fmaf(4.f * g1[2], cv[dd][2], d);
+        d = fmaf(8.f * g1[3], cv[dd][3], d);
+        d = fmaf(16.f * g2[dd * 2], cv[dd][4], d);
+        d = fmaf(32.f * g2[dd * 2 + 1], cv[dd][5], d);
+        dp[dd] = d * VMB_PI_F;
+        const int dir = 4 * q + dd;
+        const float g = dp[dd] * INV_LS;
+        jt0 = fmaf(g, Bd[dir], jt0); jt1 = fmaf(g, Bd[um::DIRS_PITCH + dir], jt1); jt2 = fmaf(g, Bd[2 * um::DIRS_PITCH + dir], jt2);
+      }
+      // directions 4q..4q+3 = columns (4q)%8.. of feature group q/2
+      if constexpr (DPROJ)
+        *reinterpret_cast<uint2*>(act + (FG_DPR + (q >> 1)) * FGB + p * 16 + (q & 1) * 8) =
+            make_uint2(um::pack_h2(dp[0], dp[1]), um::pack_h2(dp[2], dp[3]));
+    }
+    if (hsel) {                                       // direction 20: emb1 cols 4..7, emb2 cols 40, 41
+      float g1[8], g2[8], c[6];
+      eg_load8(0, g1);
+      eg_load8(EG_E2 + 10, g2);
+      um::cos_ladder(fmaf(Bd[2 * um::DIRS_PITCH + 20], t.z, fmaf(Bd[um::DIRS_PITCH + 20], t.y, Bd[20] * t.x)), c);
+      float d = g1[4] * c[0];
+      d = fmaf(2.f * g1[5], c[1], d); d = fmaf(4.f * g1[6], c[2], d); d = fmaf(8.f * g1[7], c[3], d);
+      d = fmaf(16.f * g2[0], c[4], d); d = fmaf(32.f * g2[1], c[5], d);
+      if constexpr (DPROJ)
+        *reinterpret_cast<uint2*>(act + (FG_DPR + 2) * FGB + p * 16 + 8) = make_uint2(um::pack_h2(d * VMB_PI_F, 0.f), 0u);
+      const float g = (d * VMB_PI_F) * INV_LS;
+      jt0 = fmaf(g, Bd[20], jt0); jt1 = fmaf(g, Bd[um::DIRS_PITCH + 20], jt1); jt2 = fmaf(g, Bd[2 * um::DIRS_PITCH + 20], jt2);
+    }
+    return make_float3(jt0, jt1, jt2);
+  }
+};
+
 }  // namespace uf
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -312,13 +511,13 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
   unsigned char* eg = smem + SM_EG;
   float* hd = reinterpret_cast<float*>(smem + SM_HD);
   const float* wf = reinterpret_cast<const float*>(smem + SM_W + um::IMG_F32);
-  const float* Bd = wf + um::F_DIRS;
   // ... and accumulator-fragment layout (wgmma m64nN): this thread holds rows fr0 and fr0 + 8, columns 8j + 2 cq + {0, 1}
   const int cq = lane & 3, fr0 = 64 * hsel + 16 * quad + (lane >> 2);
   Mma mm;
   mm.a16 = ptx::smem_u32(act) >> 4;
   mm.w16 = ptx::smem_u32(smem + SM_W) >> 4;
   mm.mh = hsel;
+  const Tile tl(act, eg, smem + SM_W, hd, quad);
   // persistent weight-gradient accumulators of the current object (this warpgroup's 64 feature rows)
   float wIN[16] = {}, wM1[16] = {}, wCAT[16] = {}, wM2[16] = {}, wCL[16] = {}, wHD[8] = {}, wDB[8] = {};
   // loss weights of this thread's current object: (term enabled: no object has an empty mask) / (this object's mask count)
@@ -351,50 +550,6 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
     // accumulators -> commit -> wait.
 #define OPERANDS_READY() do { ptx::fence_async_smem(); __syncthreads(); ptx::wgmma_fence(); } while (0)
 #define MMA_DONE() do { ptx::wgmma_commit(); ptx::wgmma_wait<0>(); } while (0)
-    // hidden-layer epilogue on the fragment: acc + bias -> ReLU -> fp16 into block FG, and into u: the A operand
-    // (ptx::wgmma_n32_rs) of the next stage's two k-steps over these 32 features
-    auto epi_relu = [&](const float (&v)[16], int bias_off, int fg, uint32_t (&u)[8]) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 bb = *reinterpret_cast<const float2*>(wf + bias_off + 8 * j + 2 * cq);
-        unsigned char* dst = act + (fg + j) * FGB + fr0 * 16 + cq * 4;
-        u[2 * j] = pack_relu_h2(v[4 * j] + bb.x, v[4 * j + 1] + bb.y);
-        u[2 * j + 1] = pack_relu_h2(v[4 * j + 2] + bb.x, v[4 * j + 3] + bb.y);
-        *reinterpret_cast<uint32_t*>(dst) = u[2 * j];
-        *reinterpret_cast<uint32_t*>(dst + 128) = u[2 * j + 1];
-      }
-    };
-    // dgrad epilogue: dY = (h > 0) * acc; h is read from its own block, dY goes to a block whose readers retired and
-    // into u (the A operand of the dgrad GEMMs that read dY)
-    auto epi_dgrad = [&](const float (&v)[16], int fg_h, int fg_out, uint32_t (&u)[8]) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int off = j * FGB + fr0 * 16 + cq * 4;
-        const uint32_t h0 = *reinterpret_cast<const uint32_t*>(act + fg_h * FGB + off);
-        const uint32_t h1 = *reinterpret_cast<const uint32_t*>(act + fg_h * FGB + off + 128);
-        u[2 * j] = um::gate_h2(um::pack_h2(v[4 * j], v[4 * j + 1]), h0);
-        u[2 * j + 1] = um::gate_h2(um::pack_h2(v[4 * j + 2], v[4 * j + 3]), h1);
-        *reinterpret_cast<uint32_t*>(act + fg_out * FGB + off) = u[2 * j];
-        *reinterpret_cast<uint32_t*>(act + fg_out * FGB + off + 128) = u[2 * j + 1];
-      }
-    };
-    // embedding-gradient fragment (8-column groups starting at 4-column block blk0) -> the shared fp32 tile
-    auto eg_store = [&](const auto& v, int blk0) {
-      constexpr int NJ = (int)(sizeof(v) / 16);
-#pragma unroll
-      for (int j = 0; j < NJ; ++j) {
-        float* d = reinterpret_cast<float*>(eg + (blk0 + 2 * j + (cq >> 1)) * FGB + fr0 * 16 + (cq & 1) * 8);
-        *reinterpret_cast<float2*>(d) = make_float2(v[4 * j], v[4 * j + 1]);
-        *reinterpret_cast<float2*>(d + 32) = make_float2(v[4 * j + 2], v[4 * j + 3]);
-      }
-    };
-    // eight consecutive embedding-gradient columns of this thread's point
-    auto eg_load8 = [&](int blk, float (&o)[8]) {
-      const float4 u0 = *reinterpret_cast<const float4*>(eg + blk * FGB + p * 16);
-      const float4 u1 = *reinterpret_cast<const float4*>(eg + (blk + 1) * FGB + p * 16);
-      o[0] = u0.x; o[1] = u0.y; o[2] = u0.z; o[3] = u0.w; o[4] = u1.x; o[5] = u1.y; o[6] = u1.z; o[7] = u1.w;
-    };
-
     // prefetched inputs of the next tile (global-load latency overlaps the current tile)
     float nx = 0.f, ny = 0.f, nz = 0.f, nzv = 0.f, n_gd = 0.f, n_c0 = 0.f, n_c1 = 0.f, n_c2 = 0.f;
     // (nothing computes on the loaded values here: the first use of a load stalls the warp for the memory latency)
@@ -434,53 +589,12 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       const int ray = t * nr + ray_in_tile;
       // ---- E0: positional embedding (embedding.py:82-91) ----------------------------------------------------
       const float t0x = nx * isc, t1x = ny * isc, t2x = nz * isc, zv = nzv;
-      const uint64_t tp0 = um::pk2(t0x, t0x), tp1 = um::pk2(t1x, t1x), tp2 = um::pk2(t2x, t2x);
+      const PeIn tin(make_float3(t0x, t1x, t2x));
       const float gd = n_gd, gc0 = n_c0, gc1 = n_c1, gc2 = n_c2;
       const int sv = n_sem, mv = n_msk;
       const bool live = n_live;
       prefetch(t + 1);
-      {
-        uint4* e1 = reinterpret_cast<uint4*>(act + FG_E1 * FGB + p * 16);
-        uint4* e2 = reinterpret_cast<uint4*>(act + FG_E2 * FGB + p * 16);
-        const int q0 = hsel ? 3 : 0, q1 = hsel ? 5 : 3;
-        // software pipeline over the 4-direction chunks: the NEXT chunk's projections, range reduction and MUFU
-        // sin / cos are issued before the CURRENT chunk's doubling recurrence, which hides their latency
-        uint64_t s01, s23, c01, c23;
-        {
-          uint64_t pj01, pj23;
-          um::project4(Bd, q0, tp0, tp1, tp2, pj01, pj23);
-          um::sincos4_x2(pj01, pj23, s01, s23, c01, c23);
-        }
-#pragma unroll 1
-        for (int q = q0; q < q1; ++q) {                // directions 4q .. 4q+3
-          float sv[4][6];
-          uint64_t ns01 = 0, ns23 = 0, nc01 = 0, nc23 = 0;
-          if (q + 1 < q1) {
-            uint64_t pj01, pj23;
-            um::project4(Bd, q + 1, tp0, tp1, tp2, pj01, pj23);
-            um::sincos4_x2(pj01, pj23, ns01, ns23, nc01, nc23);
-          }
-          um::sin_doubling4_x2(s01, s23, c01, c23, sv);
-          s01 = ns01; s23 = ns23; c01 = nc01; c23 = nc23;
-          const uint4 ua = make_uint4(um::pack_h2(sv[0][0], sv[0][1]), um::pack_h2(sv[0][2], sv[0][3]), um::pack_h2(sv[1][0], sv[1][1]), um::pack_h2(sv[1][2], sv[1][3]));
-          const uint4 ub = make_uint4(um::pack_h2(sv[2][0], sv[2][1]), um::pack_h2(sv[2][2], sv[2][3]), um::pack_h2(sv[3][0], sv[3][1]), um::pack_h2(sv[3][2], sv[3][3]));
-          const uint4 uc = make_uint4(um::pack_h2(sv[0][4], sv[0][5]), um::pack_h2(sv[1][4], sv[1][5]), um::pack_h2(sv[2][4], sv[2][5]), um::pack_h2(sv[3][4], sv[3][5]));
-          e1[(2 * q + 1) * 128] = ua; e1[(2 * q + 2) * 128] = ub; e2[q * 128] = uc;
-        }
-        if (hsel) {
-          // direction 20 shares chunk 0 of emb1 with [1, x, y, z] and chunk 5 of emb2 with the const-1 column
-          float s[6];
-          um::sin_ladder(fmaf(Bd[2 * um::DIRS_PITCH + 20], t2x, fmaf(Bd[um::DIRS_PITCH + 20], t1x, Bd[20] * t0x)), s);
-          const uint4 u0 = make_uint4(um::pack_h2(1.0f, t0x), um::pack_h2(t1x, t2x), um::pack_h2(s[0], s[1]), um::pack_h2(s[2], s[3]));
-          const uint4 u5 = make_uint4(um::pack_h2(s[4], s[5]), um::pack_h2(1.0f, 0.f), 0u, 0u);
-          e1[0] = u0;
-          e2[5 * 128] = u5;
-          e1[11 * 128] = make_uint4(0u, 0u, 0u, 0u);
-          // zero this point's dhead row (cols 4..15 stay zero; 0..3 are written after the render)
-          uint4* dh = reinterpret_cast<uint4*>(act + FG_DH * FGB + p * 16);
-          dh[0] = make_uint4(0u, 0u, 0u, 0u); dh[128] = make_uint4(0u, 0u, 0u, 0u);
-        }
-      }
+      tl.embed(tin);
       TR_TILE(1);
       float acc[16], hacc[8];
       uint32_t ua[8];                                   // the last epilogue's fp16 output: A of the next stage (RS)
@@ -488,13 +602,13 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
 #pragma unroll
       for (int ks = 0; ks < 6; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_E1, ks), mm.w_k(um::IMG_WIN, ks), ks > 0);
       MMA_DONE();
-      epi_relu(acc, um::F_BIN, FG_FC1, ua);
+      tl.epi_relu(acc, um::F_BIN, FG_FC1, ua);
       TR_TILE(2);
       OPERANDS_READY();                                 // mid1: fc1
 #pragma unroll
       for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WM1, ks), ks > 0);
       MMA_DONE();
-      epi_relu(acc, um::F_BM1, FG_FC2, ua);
+      tl.epi_relu(acc, um::F_BM1, FG_FC2, ua);
       TR_TILE(3);
       OPERANDS_READY();                                 // cat_layer: [fc2 | emb1] (K = 128)
 #pragma unroll
@@ -502,13 +616,13 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
 #pragma unroll
       for (int ks = 2; ks < 8; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(FG_FC2, ks), mm.w_k(um::IMG_WCAT, ks), 1u);
       MMA_DONE();
-      epi_relu(acc, um::F_BCAT, FG_FC3, ua);
+      tl.epi_relu(acc, um::F_BCAT, FG_FC3, ua);
       TR_TILE(4);
       OPERANDS_READY();                                 // mid2: fc3
 #pragma unroll
       for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WM2, ks), ks > 0);
       MMA_DONE();
-      epi_relu(acc, um::F_BM2, FG_FC4, ua);
+      tl.epi_relu(acc, um::F_BM2, FG_FC4, ua);
       TR_TILE(5);
       OPERANDS_READY();                                 // color_linear: [fc4 | emb2] (K = 80) ; out_alpha: fc4 -> column 0
 #pragma unroll
@@ -518,7 +632,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
 #pragma unroll
       for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<0>(hacc, ua + 4 * ks, mm.w16_k(um::IMG_WA16, ks), ks > 0);
       MMA_DONE();
-      epi_relu(acc, um::F_BCL, FG_HC, ua);
+      tl.epi_relu(acc, um::F_BCL, FG_HC, ua);
       if (cq == 0) { hd[fr0 * 4] = hacc[0]; hd[(fr0 + 8) * 4] = hacc[2]; }
       TR_TILE(6);
       OPERANDS_READY();                                 // out_color: hc -> columns 1..3
@@ -631,7 +745,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_DH, 0), mm.w16_mn(um::IMG_WOC16), 0u);
       mm.wgrad16(wHD, FG_FC4, FG_DH);
       MMA_DONE();
-      epi_dgrad(acc, FG_HC, FG_Z, uyc);                 // dYc -> Z
+      tl.epi_dgrad<true>(acc, FG_HC, FG_Z, uyc);                 // dYc -> Z
       TR_TILE(10);
       OPERANDS_READY();                                 // d_fc4 = dYc @ W_cl[:, :32] + dhead @ W_a ; wgrad color_linear
 #pragma unroll
@@ -639,28 +753,28 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       ptx::wgmma_n32<0, 1>(acc, mm.a_k(FG_DH, 0), mm.w16_mn(um::IMG_WA16), 1u);
       mm.wgrad32(wCL, FG_FC4, FG_Z);
       MMA_DONE();
-      epi_dgrad(acc, FG_FC4, FG_HC, ua);                // dY4 -> HC
+      tl.epi_dgrad<true>(acc, FG_FC4, FG_HC, ua);                // dY4 -> HC
       TR_TILE(11);
       OPERANDS_READY();                                 // d_fc3 = dY4 @ W_m2 ; wgrad mid2
 #pragma unroll
       for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, ua + 4 * ks, mm.w_mn(um::IMG_WM2, ks), ks > 0);
       mm.wgrad32(wM2, FG_FC3, FG_HC);
       MMA_DONE();
-      epi_dgrad(acc, FG_FC3, FG_FC4, uy3);              // dY3 -> FC4
+      tl.epi_dgrad<true>(acc, FG_FC3, FG_FC4, uy3);              // dY3 -> FC4
       TR_TILE(12);
       OPERANDS_READY();                                 // d_fc2 = dY3 @ W_cat[:, :32] ; wgrad cat_layer
 #pragma unroll
       for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, uy3 + 4 * ks, mm.w_mn(um::IMG_WCAT, ks), ks > 0);
       mm.wgrad32(wCAT, FG_FC2, FG_FC4);
       MMA_DONE();
-      epi_dgrad(acc, FG_FC2, FG_HC, ua);                // dY2 -> HC
+      tl.epi_dgrad<true>(acc, FG_FC2, FG_HC, ua);                // dY2 -> HC
       TR_TILE(13);
       OPERANDS_READY();                                 // d_fc1 = dY2 @ W_m1 ; wgrad mid1
 #pragma unroll
       for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, ua + 4 * ks, mm.w_mn(um::IMG_WM1, ks), ks > 0);
       mm.wgrad32(wM1, FG_FC1, FG_HC);
       MMA_DONE();
-      epi_dgrad(acc, FG_FC1, FG_FC3, ua);               // dY1 -> FC3
+      tl.epi_dgrad<true>(acc, FG_FC1, FG_FC3, ua);               // dY1 -> FC3
       TR_TILE(14);
       // d_emb1 = dY3 @ W_cat[:, 32:] + dY1 @ W_in (32 columns at a time), d_emb2 = dYc @ W_cl[:, 32:] ; wgrad in_layer
       OPERANDS_READY();
@@ -671,7 +785,7 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
 #pragma unroll
         for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, ua + 4 * ks, mm.w_mn(um::IMG_WIN + 4 * c * 512, ks), 1u);
         MMA_DONE();
-        eg_store(acc, 8 * c);
+        tl.eg_store(acc, 8 * c);
         ptx::wgmma_fence();
       }
 #pragma unroll
@@ -681,79 +795,17 @@ k_step_fused(StepParams a, FusedExtra x, VmbLayout L, const unsigned char* image
       mm.wgrad32(wIN, FG_E1, FG_FC3);
       MMA_DONE();
       TR_TILE(15);
-      eg_store(acc, EG_E2);
-      eg_store(hacc, EG_E2 + 8);
+      tl.eg_store(acc, EG_E2);
+      tl.eg_store(hacc, EG_E2 + 8);
       __syncthreads();                                  // embedding-gradient tile: fragment layout -> point layout
       TR_TILE(16);
       // ---- PE backward: dproj_d = pi * sum_k 2^k g_{k,d} cos(pi 2^k proj_d), written as an fp16 block --------------
       {
-        const int q0 = hsel ? 3 : 0, q1 = hsel ? 5 : 3;
-        float jt0 = 0.f, jt1 = 0.f, jt2 = 0.f;         // JOINT: this half's dL/dt
-        if constexpr (JOINT) {
-          if (!hsel) {                                  // emb1 cols 1..3 = d/d[x y z]
-            const float4 e0 = *reinterpret_cast<const float4*>(eg + p * 16);
-            jt0 = e0.y * INV_LS; jt1 = e0.z * INV_LS; jt2 = e0.w * INV_LS;
-          }
-        }
-        uint64_t c01, c23;
-        {
-          uint64_t pj01, pj23;
-          um::project4(Bd, q0, tp0, tp1, tp2, pj01, pj23);
-          um::cos4_x2(pj01, pj23, c01, c23);
-        }
-#pragma unroll 1
-        for (int q = q0; q < q1; ++q) {
-          float g1a[8], g1b[8], g2[8];
-          eg_load8(4 * q + 2, g1a);                    // emb1 cols of directions 4q, 4q+1 (k = 0..3)
-          eg_load8(4 * q + 4, g1b);                    //                          4q+2, 4q+3
-          eg_load8(EG_E2 + 2 * q, g2);                 // emb2 cols (k = 4, 5)
-          float cv[4][6], dp[4];
-          uint64_t nc01 = 0, nc23 = 0;
-          if (q + 1 < q1) {                            // next chunk's front half before this chunk's recurrence
-            uint64_t pj01, pj23;
-            um::project4(Bd, q + 1, tp0, tp1, tp2, pj01, pj23);
-            um::cos4_x2(pj01, pj23, nc01, nc23);
-          }
-          um::cos_doubling4_x2(c01, c23, cv);
-          c01 = nc01; c23 = nc23;
-#pragma unroll
-          for (int dd = 0; dd < 4; ++dd) {
-            const float* g1 = (dd < 2) ? (g1a + dd * 4) : (g1b + (dd - 2) * 4);
-            float d = g1[0] * cv[dd][0];
-            d = fmaf(2.f * g1[1], cv[dd][1], d);
-            d = fmaf(4.f * g1[2], cv[dd][2], d);
-            d = fmaf(8.f * g1[3], cv[dd][3], d);
-            d = fmaf(16.f * g2[dd * 2], cv[dd][4], d);
-            d = fmaf(32.f * g2[dd * 2 + 1], cv[dd][5], d);
-            dp[dd] = d * VMB_PI_F;
-            if constexpr (JOINT) {
-              const int dir = 4 * q + dd;
-              const float g = dp[dd] * INV_LS;
-              jt0 = fmaf(g, Bd[dir], jt0); jt1 = fmaf(g, Bd[um::DIRS_PITCH + dir], jt1); jt2 = fmaf(g, Bd[2 * um::DIRS_PITCH + dir], jt2);
-            }
-          }
-          // directions 4q..4q+3 = columns (4q)%8.. of feature group q/2
-          *reinterpret_cast<uint2*>(act + (FG_DPR + (q >> 1)) * FGB + p * 16 + (q & 1) * 8) =
-              make_uint2(um::pack_h2(dp[0], dp[1]), um::pack_h2(dp[2], dp[3]));
-        }
-        if (hsel) {                                     // direction 20: emb1 cols 4..7, emb2 cols 40, 41
-          float g1[8], g2[8], c[6];
-          eg_load8(0, g1);
-          eg_load8(EG_E2 + 10, g2);
-          um::cos_ladder(fmaf(Bd[2 * um::DIRS_PITCH + 20], t2x, fmaf(Bd[um::DIRS_PITCH + 20], t1x, Bd[20] * t0x)), c);
-          float d = g1[4] * c[0];
-          d = fmaf(2.f * g1[5], c[1], d); d = fmaf(4.f * g1[6], c[2], d); d = fmaf(8.f * g1[7], c[3], d);
-          d = fmaf(16.f * g2[0], c[4], d); d = fmaf(32.f * g2[1], c[5], d);
-          *reinterpret_cast<uint2*>(act + (FG_DPR + 2) * FGB + p * 16 + 8) = make_uint2(um::pack_h2(d * VMB_PI_F, 0.f), 0u);
-          if constexpr (JOINT) {
-            const float g = (d * VMB_PI_F) * INV_LS;
-            jt0 = fmaf(g, Bd[20], jt0); jt1 = fmaf(g, Bd[um::DIRS_PITCH + 20], jt1); jt2 = fmaf(g, Bd[2 * um::DIRS_PITCH + 20], jt2);
-          }
-        }
+        const float3 jt = tl.pe_backward<true>(tin);
         if constexpr (JOINT) {
           if (live) {
             float* o = jdt + (((size_t)b * R + ray) * S + sidx) * 6 + 3 * hsel;
-            o[0] = jt0; o[1] = jt1; o[2] = jt2;
+            o[0] = jt.x; o[1] = jt.y; o[2] = jt.z;
           }
         }
       }

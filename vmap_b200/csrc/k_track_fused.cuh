@@ -10,15 +10,16 @@
 //   Weights  object b reads the fp16 weight image row rows[b] ([n_rows][um::IMG_BYTES], as the AdamW launch writes it)
 //            with one bulk async copy: the fp16 matrices, the fp32 biases and the PE directions.  rows[] stays a device
 //            array (capturable); a row outside [0, n_rows) contributes zero rows and sets VMB_TRACK_ST_BAD_ROW, as K10.
-//   Tile     the fused step's: one CTA = whole rays of one object (blockIdx.y), up to 128 points, 256 threads = two
+//   Tile     uf::Tile, the fused step's (k_step_fused.cuh): one CTA = whole rays of one object (blockIdx.y), up to 128 points, 256 threads = two
 //            warpgroups; rays never straddle a warp (32 / S rays per warp, S <= 32), so a tile is 4 (32 / S) rays.  Not
-//            cooperative and no CTA waits on another: each CTA counts its object's mask slice in its prologue.
+//            cooperative and no CTA waits on another: each CTA counts its object's mask slice in its prologue
+//            (load_object, shared with k_reloc_fused).
 //   Points   pose_point: p = R q + t from an fp32 copy of the fp64 pose, then p / scale.  K11: the pose of the ray's draw
 //            frame (ba_draw_frame); a ray whose frame is outside the table contributes nothing and sets
 //            VMB_BA_ST_BAD_FRAME.
-//   Forward  the fused step's E0 (positional embedding) and its six forward wgmma stages (in_layer, mid1, cat_layer,
-//            mid2, color_linear + out_alpha, out_color) with the same operand layout and the same fp16 rounding points:
-//            fp16 embedding, fp16 image weights, fp32 accumulation, fp16 ReLU activations, fp32 heads.
+//   Forward  forward_tile: uf::Tile::embed (E0) and the six forward wgmma stages (in_layer, mid1, cat_layer, mid2,
+//            color_linear + out_alpha, out_color) with uf::Tile::epi_relu, the step's operand layout and fp16 rounding
+//            points: fp16 embedding, fp16 image weights, fp32 accumulation, fp16 ReLU activations, fp32 heads.
 //   Render   one lane per sample, the ray's lanes adjacent in a warp: the heads' sigmoids in fp32, then K10's render in
 //            fp64 in sample order (1 - occ as sigmoid(-alpha)) and ray_loss on it, with the object's own mask counts.
 //            Each ray's three loss terms stay in fp64.  d(raw alpha) and d(raw colour) in fp32 as K10, scaled by
@@ -26,12 +27,14 @@
 //            on the clamped values (and VMB_TRACK_ST_CLAMP is set when it is not 0): exactly the dhead values (the
 //            four per point: LS d(raw alpha), LS d(raw colour)[3]) whose magnitude passes 60000; the saturating fp16
 //            packs of the d_hc .. d_fc1 epilogues are not counted.
-//   Backward the input-gradient chain of the fused step only: d_hc, d_fc4 (with the dhead . W_a term), d_fc3, d_fc2,
-//            d_fc1, d_emb, each gated dY passed to the next wgmma in registers.  No weight-gradient wgmmas, no dB, no
-//            partial rows of weights, no finish and no AdamW.
-//   Pose     per point dL/dt = INV_LS (dE_xyz + sum_d dproj_d B_d) from the PE backward's cosines, formed as the fused
-//            step's JOINT instantiation forms it (warpgroup 0: dE_xyz, directions 0..11; warpgroup 1: 12..20; the two
-//            halves added in that order), then pose_terms ((R q) x g, g), g = dL/dt / scale, in fp64 from the fp64 pose.
+//   Backward the fused step's input-gradient chain without its weight gradients: d_hc, d_fc4 (with the dhead . W_a
+//            term), d_fc3, d_fc2, d_fc1, d_emb, each gated dY (uf::Tile::epi_dgrad) passed to the next wgmma in
+//            registers, d_emb to the eg tile (uf::Tile::eg_store).  No dB, no partial rows of weights, no finish and no
+//            AdamW.
+//   Pose     per point dL/dt = INV_LS (dE_xyz + sum_d dproj_d B_d) from uf::Tile::pe_backward, the half sums the
+//            fused step's JOINT instantiation stores (warpgroup 0: dE_xyz, directions 0..11; warpgroup 1: 12..20; the
+//            two halves added in that order), then pose_terms ((R q) x g, g), g = dL/dt / scale, in fp64 from the fp64
+//            pose.
 //   Rows     one row per ray, its samples summed in sample order: K11's rows [B][R][VMB_TRACK_PART] (BA flavour).  The
 //            track flavour writes the same per-ray terms to the workspace and k_tf_reduce sums them per K10 tile
 //            (vmb_track_tiles' tile of 128 / S rays, which the fused tile matches only at S = 10 and 32) in ray order
@@ -85,74 +88,39 @@ struct Workspace {
   }
 };
 
-// cvt + ReLU in one instruction (as the fused step's epilogue)
-__device__ __forceinline__ uint32_t pack_relu_h2(float lo, float hi) {
-  uint32_t r;
-  asm("cvt.rn.relu.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  return r;
+// The start of k_track_fused and k_reloc_fused once the object's image row is known to be valid: the weight image on
+// its way behind the barrier at SM_BAR (image_ready waits for it) while the object's slice mask counts
+// (loss.py:16-18,38) go to red -- every CTA of the object counts the same rays.  Returns the tile (quad: this thread's
+// warp within its warpgroup); its embedding-gradient tile aliases the activations, which nothing reads after d_fc1.
+__device__ __forceinline__ uf::Tile load_object(unsigned char* smem, const unsigned char* image, int row,
+                                                const TrackParams& a, int (&red)[3][NT / 32], int quad) {
+  const int tid = threadIdx.x, b = blockIdx.y, R = a.R;
+  uint64_t* wbar = reinterpret_cast<uint64_t*>(smem + SM_BAR);
+  if (tid == 0) { ptx::mbar_init(wbar, 1); ptx::mbar_init_fence(); }
+  __syncthreads();
+  if (tid == 0) {
+    ptx::mbar_arrive_expect_tx(wbar, um::IMG_BYTES);
+    ptx::bulk_g2s(smem + SM_W, image + (size_t)row * um::IMG_BYTES, um::IMG_BYTES, wbar);
+  }
+  const unsigned char* sv = a.sem + (size_t)b * a.sem_stride;
+  const unsigned char* mv = a.mask + (size_t)b * a.mask_stride;
+  int nd = 0, no = 0, ns = 0;
+  for (int r = tid; r < R; r += NT) slice_mask_count(sv, mv, r, nd, no, ns);
+  warp_mask_counts(tid, nd, no, ns, red);
+  return uf::Tile(smem + SM_ACT, smem + SM_ACT, smem + SM_W, reinterpret_cast<float*>(smem + SM_HD), quad);
 }
 
-// E0 and the six forward stages of one tile (the fused step's code, layout and fp16 rounding points) at this thread's
-// network input t: the embedding blocks and hidden activations to `act`, the heads (raw alpha, raw colour[3]) in point
-// layout to `hd` and zeroed dhead rows.  The weight image is in shared memory.  Ends before the CTA barrier that makes
-// the heads tile visible.  Shared by k_track_fused and the forward-only relocalisation tile (k_reloc.cuh).
-__device__ __forceinline__ void forward_tile(unsigned char* act, float* hd, const float* wf, const float* Bd,
-                                             const uf::Mma& mm, float3 t, int p, int hsel, int cq, int fr0,
-                                             uint32_t (&ua)[8]) {
-  const float t0x = t.x, t1x = t.y, t2x = t.z;
-  const uint64_t tp0 = um::pk2(t0x, t0x), tp1 = um::pk2(t1x, t1x), tp2 = um::pk2(t2x, t2x);
-  // ---- E0: positional embedding (embedding.py:82-91), the fused step's code and layout ------------------------------
-  {
-    uint4* e1 = reinterpret_cast<uint4*>(act + uf::FG_E1 * FGB + p * 16);
-    uint4* e2 = reinterpret_cast<uint4*>(act + uf::FG_E2 * FGB + p * 16);
-    const int q0 = hsel ? 3 : 0, q1 = hsel ? 5 : 3;
-    uint64_t s01, s23, c01, c23;
-    {
-      uint64_t pj01, pj23;
-      um::project4(Bd, q0, tp0, tp1, tp2, pj01, pj23);
-      um::sincos4_x2(pj01, pj23, s01, s23, c01, c23);
-    }
-#pragma unroll 1
-    for (int qq = q0; qq < q1; ++qq) {                 // directions 4qq .. 4qq+3
-      float sv[4][6];
-      uint64_t ns01 = 0, ns23 = 0, nc01 = 0, nc23 = 0;
-      if (qq + 1 < q1) {
-        uint64_t pj01, pj23;
-        um::project4(Bd, qq + 1, tp0, tp1, tp2, pj01, pj23);
-        um::sincos4_x2(pj01, pj23, ns01, ns23, nc01, nc23);
-      }
-      um::sin_doubling4_x2(s01, s23, c01, c23, sv);
-      s01 = ns01; s23 = ns23; c01 = nc01; c23 = nc23;
-      const uint4 ua = make_uint4(um::pack_h2(sv[0][0], sv[0][1]), um::pack_h2(sv[0][2], sv[0][3]), um::pack_h2(sv[1][0], sv[1][1]), um::pack_h2(sv[1][2], sv[1][3]));
-      const uint4 ub = make_uint4(um::pack_h2(sv[2][0], sv[2][1]), um::pack_h2(sv[2][2], sv[2][3]), um::pack_h2(sv[3][0], sv[3][1]), um::pack_h2(sv[3][2], sv[3][3]));
-      const uint4 uc = make_uint4(um::pack_h2(sv[0][4], sv[0][5]), um::pack_h2(sv[1][4], sv[1][5]), um::pack_h2(sv[2][4], sv[2][5]), um::pack_h2(sv[3][4], sv[3][5]));
-      e1[(2 * qq + 1) * 128] = ua; e1[(2 * qq + 2) * 128] = ub; e2[qq * 128] = uc;
-    }
-    if (hsel) {
-      // direction 20 shares chunk 0 of emb1 with [1, x, y, z] and chunk 5 of emb2 with the const-1 column
-      float s[6];
-      um::sin_ladder(fmaf(Bd[2 * um::DIRS_PITCH + 20], t2x, fmaf(Bd[um::DIRS_PITCH + 20], t1x, Bd[20] * t0x)), s);
-      e1[0] = make_uint4(um::pack_h2(1.0f, t0x), um::pack_h2(t1x, t2x), um::pack_h2(s[0], s[1]), um::pack_h2(s[2], s[3]));
-      e2[5 * 128] = make_uint4(um::pack_h2(s[4], s[5]), um::pack_h2(1.0f, 0.f), 0u, 0u);
-      e1[11 * 128] = make_uint4(0u, 0u, 0u, 0u);
-      uint4* dh = reinterpret_cast<uint4*>(act + uf::FG_DH * FGB + p * 16);   // this point's dhead row: 0 until the render
-      dh[0] = make_uint4(0u, 0u, 0u, 0u); dh[128] = make_uint4(0u, 0u, 0u, 0u);
-    }
-  }
+__device__ __forceinline__ void image_ready(unsigned char* smem) {
+  um::mbar_wait_or_trap(reinterpret_cast<uint64_t*>(smem + SM_BAR), 0);
+}
 
-  // hidden-layer epilogue on the fragment: acc + bias -> ReLU -> fp16 into block fg (read back by the dgrad gates) and
-  // into u, the A operand of the next stage
-  auto epi_relu = [&](const float (&v)[16], int bias_off, int fg, uint32_t (&u)[8]) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 bb = *reinterpret_cast<const float2*>(wf + bias_off + 8 * j + 2 * cq);
-      unsigned char* dst = act + (fg + j) * FGB + fr0 * 16 + cq * 4;
-      u[2 * j] = pack_relu_h2(v[4 * j] + bb.x, v[4 * j + 1] + bb.y);
-      u[2 * j + 1] = pack_relu_h2(v[4 * j + 2] + bb.x, v[4 * j + 3] + bb.y);
-      *reinterpret_cast<uint32_t*>(dst) = u[2 * j];
-      *reinterpret_cast<uint32_t*>(dst + 128) = u[2 * j + 1];
-    }
-  };
+// E0 (uf::Tile::embed) and the six forward stages of one tile (the fused step's layout and fp16 rounding points) at this
+// thread's network input: the embedding blocks and hidden activations to `act`, the heads (raw alpha, raw colour[3]) in
+// point layout to `hd` and zeroed dhead rows.  The weight image is in shared memory.  Ends before the CTA barrier that makes
+// the heads tile visible.  Shared by k_track_fused and the forward-only relocalisation tile (k_reloc.cuh).
+__device__ __forceinline__ void forward_tile(const uf::Tile& tl, const uf::PeIn& in, uint32_t (&ua)[8]) {
+  tl.embed(in);
+
 #define MMA_DONE() do { ptx::wgmma_commit(); ptx::wgmma_wait<0>(); } while (0)
 
   // ---- forward: the fused step's six stages.  Only the embedding blocks cross warpgroups (SS A operand): one CTA
@@ -162,42 +130,42 @@ __device__ __forceinline__ void forward_tile(unsigned char* act, float* hd, cons
   __syncthreads();
   ptx::wgmma_fence();                                 // in_layer: emb1 (K = 96)
 #pragma unroll
-  for (int ks = 0; ks < 6; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(uf::FG_E1, ks), mm.w_k(um::IMG_WIN, ks), ks > 0);
+  for (int ks = 0; ks < 6; ++ks) ptx::wgmma_n32<0, 0>(acc, tl.mm.a_k(uf::FG_E1, ks), tl.mm.w_k(um::IMG_WIN, ks), ks > 0);
   MMA_DONE();
-  epi_relu(acc, um::F_BIN, uf::FG_FC1, ua);
+  tl.epi_relu(acc, um::F_BIN, uf::FG_FC1, ua);
   ptx::wgmma_fence();                                 // mid1: fc1
 #pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WM1, ks), ks > 0);
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, tl.mm.w_k(um::IMG_WM1, ks), ks > 0);
   MMA_DONE();
-  epi_relu(acc, um::F_BM1, uf::FG_FC2, ua);
+  tl.epi_relu(acc, um::F_BM1, uf::FG_FC2, ua);
   ptx::wgmma_fence();                                 // cat_layer: [fc2 | emb1] (K = 128)
 #pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WCAT, ks), ks > 0);
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, tl.mm.w_k(um::IMG_WCAT, ks), ks > 0);
 #pragma unroll
-  for (int ks = 2; ks < 8; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(uf::FG_FC2, ks), mm.w_k(um::IMG_WCAT, ks), 1u);
+  for (int ks = 2; ks < 8; ++ks) ptx::wgmma_n32<0, 0>(acc, tl.mm.a_k(uf::FG_FC2, ks), tl.mm.w_k(um::IMG_WCAT, ks), 1u);
   MMA_DONE();
-  epi_relu(acc, um::F_BCAT, uf::FG_FC3, ua);
+  tl.epi_relu(acc, um::F_BCAT, uf::FG_FC3, ua);
   ptx::wgmma_fence();                                 // mid2: fc3
 #pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WM2, ks), ks > 0);
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, tl.mm.w_k(um::IMG_WM2, ks), ks > 0);
   MMA_DONE();
-  epi_relu(acc, um::F_BM2, uf::FG_FC4, ua);
+  tl.epi_relu(acc, um::F_BM2, uf::FG_FC4, ua);
   ptx::wgmma_fence();                                 // color_linear: [fc4 | emb2] (K = 80) ; out_alpha: fc4 -> column 0
 #pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, mm.w_k(um::IMG_WCL, ks), ks > 0);
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<0>(acc, ua + 4 * ks, tl.mm.w_k(um::IMG_WCL, ks), ks > 0);
 #pragma unroll
-  for (int ks = 2; ks < 5; ++ks) ptx::wgmma_n32<0, 0>(acc, mm.a_k(uf::FG_FC4, ks), mm.w_k(um::IMG_WCL, ks), 1u);
+  for (int ks = 2; ks < 5; ++ks) ptx::wgmma_n32<0, 0>(acc, tl.mm.a_k(uf::FG_FC4, ks), tl.mm.w_k(um::IMG_WCL, ks), 1u);
 #pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<0>(hacc, ua + 4 * ks, mm.w16_k(um::IMG_WA16, ks), ks > 0);
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<0>(hacc, ua + 4 * ks, tl.mm.w16_k(um::IMG_WA16, ks), ks > 0);
   MMA_DONE();
-  epi_relu(acc, um::F_BCL, uf::FG_HC, ua);
-  if (cq == 0) { hd[fr0 * 4] = hacc[0]; hd[(fr0 + 8) * 4] = hacc[2]; }
+  tl.epi_relu(acc, um::F_BCL, uf::FG_HC, ua);
+  if (tl.cq == 0) { tl.hd[tl.fr0 * 4] = hacc[0]; tl.hd[(tl.fr0 + 8) * 4] = hacc[2]; }
   ptx::wgmma_fence();                                 // out_color: hc -> columns 1..3
 #pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<0>(hacc, ua + 4 * ks, mm.w16_k(um::IMG_WOC16, ks), ks > 0);
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<0>(hacc, ua + 4 * ks, tl.mm.w16_k(um::IMG_WOC16, ks), ks > 0);
   MMA_DONE();
-  if (cq == 0) { hd[fr0 * 4 + 1] = hacc[1]; hd[(fr0 + 8) * 4 + 1] = hacc[3]; }
-  if (cq == 1) { hd[fr0 * 4 + 2] = hacc[0]; hd[fr0 * 4 + 3] = hacc[1]; hd[(fr0 + 8) * 4 + 2] = hacc[2]; hd[(fr0 + 8) * 4 + 3] = hacc[3]; }
+  if (tl.cq == 0) { tl.hd[tl.fr0 * 4 + 1] = hacc[1]; tl.hd[(tl.fr0 + 8) * 4 + 1] = hacc[3]; }
+  if (tl.cq == 1) { tl.hd[tl.fr0 * 4 + 2] = hacc[0]; tl.hd[tl.fr0 * 4 + 3] = hacc[1]; tl.hd[(tl.fr0 + 8) * 4 + 2] = hacc[2]; tl.hd[(tl.fr0 + 8) * 4 + 3] = hacc[3]; }
 #undef MMA_DONE
 }
 
@@ -261,7 +229,7 @@ __global__ void __launch_bounds__(NT, 2) k_track_fused(TrackParams a, BaRays x, 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.y, S = a.S, R = a.R;
   const unsigned FULL = 0xffffffffu;
-  // thread roles as the fused step: point layout (one thread pair per point) and accumulator-fragment layout
+  // point layout (one thread pair per point) and this thread's sample; uf::Tile holds the fragment layout
   const int p = tid & 127, hsel = tid >> 7, quad = warp & 3;
   const int rw = lane / S, sidx = lane - rw * S, seg_lo = lane - sidx;
   const int ray = blockIdx.x * nr + quad * rpw + rw;
@@ -280,21 +248,7 @@ __global__ void __launch_bounds__(NT, 2) k_track_fused(TrackParams a, BaRays x, 
     if (tid == 0 && a.status) atomicOr(a.status, VMB_TRACK_ST_BAD_ROW);
     return;
   }
-  uint64_t* wbar = reinterpret_cast<uint64_t*>(smem + SM_BAR);
-  if (tid == 0) { ptx::mbar_init(wbar, 1); ptx::mbar_init_fence(); }
-  __syncthreads();
-  if (tid == 0) {                                     // the object's weight image: in flight while the mask counts run
-    ptx::mbar_arrive_expect_tx(wbar, um::IMG_BYTES);
-    ptx::bulk_g2s(smem + SM_W, image + (size_t)row * um::IMG_BYTES, um::IMG_BYTES, wbar);
-  }
-  // ---- the object's mask counts of this slice (loss.py:16-18,38): every CTA of the object counts the same rays ------
-  {
-    const unsigned char* sv = a.sem + (size_t)b * a.sem_stride;
-    const unsigned char* mv = a.mask + (size_t)b * a.mask_stride;
-    int nd = 0, no = 0, ns = 0;
-    for (int r = tid; r < R; r += NT) slice_mask_count(sv, mv, r, nd, no, ns);
-    warp_mask_counts(tid, nd, no, ns, red);
-  }
+  const uf::Tile tl = load_object(smem, image, row, a, red, quad);
 
   // ---- points: p = R q + t (fp32 copy of the fp64 pose), network input p / scale ------------------------------------
   const double* T = a.pose;
@@ -314,54 +268,18 @@ __global__ void __launch_bounds__(NT, 2) k_track_fused(TrackParams a, BaRays x, 
   float zv = 0.f;
   if (hsel == 0 && live) zv = a.z[(size_t)b * a.z_stride + (size_t)ray * S + sidx];
 
-  unsigned char* act = smem + SM_ACT;
-  unsigned char* eg = smem + SM_ACT;                  // aliases act from the d_emb stage on
-  float* hd = reinterpret_cast<float*>(smem + SM_HD);
-  const float* wf = reinterpret_cast<const float*>(smem + SM_W + um::IMG_F32);
-  const float* Bd = wf + um::F_DIRS;
-  const int cq = lane & 3, fr0 = 64 * hsel + 16 * quad + (lane >> 2);
-  uf::Mma mm;
-  mm.a16 = ptx::smem_u32(act) >> 4;
-  mm.w16 = ptx::smem_u32(smem + SM_W) >> 4;
-  mm.mh = hsel;
-  um::mbar_wait_or_trap(wbar, 0);
+  image_ready(smem);
 
-  const float t0x = t.x, t1x = t.y, t2x = t.z;
-  const uint64_t tp0 = um::pk2(t0x, t0x), tp1 = um::pk2(t1x, t1x), tp2 = um::pk2(t2x, t2x);
+  const uf::PeIn tin(t);
   uint32_t ua[8];
-  forward_tile(act, hd, wf, Bd, mm, t, p, hsel, cq, fr0, ua);
-  // dgrad epilogue: dY = (h > 0) * fp16(acc), h from its block; dY only in registers (no weight gradient reads it)
-  auto epi_dgrad = [&](const float (&v)[16], int fg_h, uint32_t (&u)[8]) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int off = (fg_h + j) * FGB + fr0 * 16 + cq * 4;
-      const uint32_t h0 = *reinterpret_cast<const uint32_t*>(act + off);
-      const uint32_t h1 = *reinterpret_cast<const uint32_t*>(act + off + 128);
-      u[2 * j] = um::gate_h2(um::pack_h2(v[4 * j], v[4 * j + 1]), h0);
-      u[2 * j + 1] = um::gate_h2(um::pack_h2(v[4 * j + 2], v[4 * j + 3]), h1);
-    }
-  };
-  auto eg_store = [&](const auto& v, int blk0) {
-    constexpr int NJ = (int)(sizeof(v) / 16);
-#pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      float* d = reinterpret_cast<float*>(eg + (blk0 + 2 * j + (cq >> 1)) * FGB + fr0 * 16 + (cq & 1) * 8);
-      *reinterpret_cast<float2*>(d) = make_float2(v[4 * j], v[4 * j + 1]);
-      *reinterpret_cast<float2*>(d + 32) = make_float2(v[4 * j + 2], v[4 * j + 3]);
-    }
-  };
-  auto eg_load8 = [&](int blk, float (&o)[8]) {
-    const float4 u0 = *reinterpret_cast<const float4*>(eg + blk * FGB + p * 16);
-    const float4 u1 = *reinterpret_cast<const float4*>(eg + (blk + 1) * FGB + p * 16);
-    o[0] = u0.x; o[1] = u0.y; o[2] = u0.z; o[3] = u0.w; o[4] = u1.x; o[5] = u1.y; o[6] = u1.z; o[7] = u1.w;
-  };
+  forward_tile(tl, tin, ua);
 #define MMA_DONE() do { ptx::wgmma_commit(); ptx::wgmma_wait<0>(); } while (0)
   float acc[16], hacc[8];
   __syncthreads();                                    // heads tile (fragment layout -> point layout); mask counts
 
   // ---- render + loss + d(raw alpha, raw colour): K10's rule, one lane per sample in the warps of warpgroup 0 ---------
   if (hsel == 0) {                                    // warp-uniform
-    const RayRender rr = render_ray(hd, wf, zv, p, S, sidx, seg_lo);
+    const RayRender rr = render_ray(tl.hd, tl.wf, zv, p, S, sidx, seg_lo);
     const float al = rr.al, oc = rr.oc, c0 = rr.c0, c1 = rr.c1, c2 = rr.c2, Ts = rr.Ts, wgt = rr.wgt;
     const double D = rr.D, O = rr.O, C0 = rr.C0, C1 = rr.C1, C2 = rr.C2, V = rr.V;
     int cnt[3];
@@ -397,7 +315,7 @@ __global__ void __launch_bounds__(NT, 2) k_track_fused(TrackParams a, BaRays x, 
         n_clamp += fabsf(d[c]) > 60000.f;
         d[c] = fminf(fmaxf(d[c], -60000.f), 60000.f);
       }
-      *reinterpret_cast<uint2*>(act + uf::FG_DH * FGB + p * 16) = make_uint2(um::pack_h2(d[0], d[1]), um::pack_h2(d[2], d[3]));
+      *reinterpret_cast<uint2*>(tl.act + uf::FG_DH * FGB + p * 16) = make_uint2(um::pack_h2(d[0], d[1]), um::pack_h2(d[2], d[3]));
     }
     for (int o = 16; o > 0; o >>= 1) n_clamp += __shfl_xor_sync(FULL, n_clamp, o);
     if (lane == 0 && n_clamp && a.status) { atomicOr(a.status, VMB_TRACK_ST_CLAMP); atomicAdd(a.status + 1, n_clamp); }
@@ -408,116 +326,63 @@ __global__ void __launch_bounds__(NT, 2) k_track_fused(TrackParams a, BaRays x, 
   ptx::fence_async_smem();
   __syncthreads();
   ptx::wgmma_fence();                                 // d_hc = dhead @ W_oc
-  ptx::wgmma_n32<0, 1>(acc, mm.a_k(uf::FG_DH, 0), mm.w16_mn(um::IMG_WOC16), 0u);
+  ptx::wgmma_n32<0, 1>(acc, tl.mm.a_k(uf::FG_DH, 0), tl.mm.w16_mn(um::IMG_WOC16), 0u);
   MMA_DONE();
-  epi_dgrad(acc, uf::FG_HC, uyc);
+  tl.epi_dgrad<false>(acc, uf::FG_HC, 0, uyc);
   ptx::wgmma_fence();                                 // d_fc4 = dYc @ W_cl[:, :32] + dhead @ W_a
 #pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, uyc + 4 * ks, mm.w_mn(um::IMG_WCL, ks), ks > 0);
-  ptx::wgmma_n32<0, 1>(acc, mm.a_k(uf::FG_DH, 0), mm.w16_mn(um::IMG_WA16), 1u);
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, uyc + 4 * ks, tl.mm.w_mn(um::IMG_WCL, ks), ks > 0);
+  ptx::wgmma_n32<0, 1>(acc, tl.mm.a_k(uf::FG_DH, 0), tl.mm.w16_mn(um::IMG_WA16), 1u);
   MMA_DONE();
-  epi_dgrad(acc, uf::FG_FC4, ua);
+  tl.epi_dgrad<false>(acc, uf::FG_FC4, 0, ua);
   ptx::wgmma_fence();                                 // d_fc3 = dY4 @ W_m2
 #pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, ua + 4 * ks, mm.w_mn(um::IMG_WM2, ks), ks > 0);
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, ua + 4 * ks, tl.mm.w_mn(um::IMG_WM2, ks), ks > 0);
   MMA_DONE();
-  epi_dgrad(acc, uf::FG_FC3, uy3);
+  tl.epi_dgrad<false>(acc, uf::FG_FC3, 0, uy3);
   ptx::wgmma_fence();                                 // d_fc2 = dY3 @ W_cat[:, :32]
 #pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, uy3 + 4 * ks, mm.w_mn(um::IMG_WCAT, ks), ks > 0);
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, uy3 + 4 * ks, tl.mm.w_mn(um::IMG_WCAT, ks), ks > 0);
   MMA_DONE();
-  epi_dgrad(acc, uf::FG_FC2, ua);
+  tl.epi_dgrad<false>(acc, uf::FG_FC2, 0, ua);
   ptx::wgmma_fence();                                 // d_fc1 = dY2 @ W_m1
 #pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, ua + 4 * ks, mm.w_mn(um::IMG_WM1, ks), ks > 0);
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, ua + 4 * ks, tl.mm.w_mn(um::IMG_WM1, ks), ks > 0);
   MMA_DONE();
-  epi_dgrad(acc, uf::FG_FC1, ua);
+  tl.epi_dgrad<false>(acc, uf::FG_FC1, 0, ua);
   __syncthreads();                                    // every read of the activations is done: eg may overwrite them
   // d_emb1 = dY3 @ W_cat[:, 32:] + dY1 @ W_in (32 columns at a time), d_emb2 = dYc @ W_cl[:, 32:]
   ptx::wgmma_fence();
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
 #pragma unroll
-    for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, uy3 + 4 * ks, mm.w_mn(um::IMG_WCAT + (4 + 4 * c) * 512, ks), ks > 0);
+    for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, uy3 + 4 * ks, tl.mm.w_mn(um::IMG_WCAT + (4 + 4 * c) * 512, ks), ks > 0);
 #pragma unroll
-    for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, ua + 4 * ks, mm.w_mn(um::IMG_WIN + 4 * c * 512, ks), 1u);
+    for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, ua + 4 * ks, tl.mm.w_mn(um::IMG_WIN + 4 * c * 512, ks), 1u);
     MMA_DONE();
-    eg_store(acc, 8 * c);
+    tl.eg_store(acc, 8 * c);
     ptx::wgmma_fence();
   }
 #pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, uyc + 4 * ks, mm.w_mn(um::IMG_WCL + 4 * 512, ks), ks > 0);
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n32_rs<1>(acc, uyc + 4 * ks, tl.mm.w_mn(um::IMG_WCL + 4 * 512, ks), ks > 0);
 #pragma unroll
-  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<1>(hacc, uyc + 4 * ks, mm.w_mn(um::IMG_WCL + 8 * 512, ks), ks > 0);
+  for (int ks = 0; ks < 2; ++ks) ptx::wgmma_n16_rs<1>(hacc, uyc + 4 * ks, tl.mm.w_mn(um::IMG_WCL + 8 * 512, ks), ks > 0);
   MMA_DONE();
-  eg_store(acc, uf::EG_E2);
-  eg_store(hacc, uf::EG_E2 + 8);
+  tl.eg_store(acc, uf::EG_E2);
+  tl.eg_store(hacc, uf::EG_E2 + 8);
 #undef MMA_DONE
   __syncthreads();                                    // embedding-gradient tile: fragment layout -> point layout
 
-  // ---- PE backward: this warpgroup's half of dL/dt (the JOINT instantiation's sums) ----------------------------------
-  float jt0 = 0.f, jt1 = 0.f, jt2 = 0.f;
-  {
-    const int q0 = hsel ? 3 : 0, q1 = hsel ? 5 : 3;
-    if (!hsel) {                                      // emb1 cols 1..3 = d/d[x y z]
-      const float4 e0 = *reinterpret_cast<const float4*>(eg + p * 16);
-      jt0 = e0.y * INV_LS; jt1 = e0.z * INV_LS; jt2 = e0.w * INV_LS;
-    }
-    uint64_t c01, c23;
-    {
-      uint64_t pj01, pj23;
-      um::project4(Bd, q0, tp0, tp1, tp2, pj01, pj23);
-      um::cos4_x2(pj01, pj23, c01, c23);
-    }
-#pragma unroll 1
-    for (int qq = q0; qq < q1; ++qq) {
-      float g1a[8], g1b[8], g2[8];
-      eg_load8(4 * qq + 2, g1a);                      // emb1 cols of directions 4qq, 4qq+1 (k = 0..3)
-      eg_load8(4 * qq + 4, g1b);                      //                          4qq+2, 4qq+3
-      eg_load8(uf::EG_E2 + 2 * qq, g2);               // emb2 cols (k = 4, 5)
-      float cv[4][6];
-      uint64_t nc01 = 0, nc23 = 0;
-      if (qq + 1 < q1) {
-        uint64_t pj01, pj23;
-        um::project4(Bd, qq + 1, tp0, tp1, tp2, pj01, pj23);
-        um::cos4_x2(pj01, pj23, nc01, nc23);
-      }
-      um::cos_doubling4_x2(c01, c23, cv);
-      c01 = nc01; c23 = nc23;
-#pragma unroll
-      for (int dd = 0; dd < 4; ++dd) {
-        const float* g1 = (dd < 2) ? (g1a + dd * 4) : (g1b + (dd - 2) * 4);
-        float d = g1[0] * cv[dd][0];
-        d = fmaf(2.f * g1[1], cv[dd][1], d);
-        d = fmaf(4.f * g1[2], cv[dd][2], d);
-        d = fmaf(8.f * g1[3], cv[dd][3], d);
-        d = fmaf(16.f * g2[dd * 2], cv[dd][4], d);
-        d = fmaf(32.f * g2[dd * 2 + 1], cv[dd][5], d);
-        const int dir = 4 * qq + dd;
-        const float g = (d * VMB_PI_F) * INV_LS;
-        jt0 = fmaf(g, Bd[dir], jt0); jt1 = fmaf(g, Bd[um::DIRS_PITCH + dir], jt1); jt2 = fmaf(g, Bd[2 * um::DIRS_PITCH + dir], jt2);
-      }
-    }
-    if (hsel) {                                       // direction 20: emb1 cols 4..7, emb2 cols 40, 41
-      float g1[8], g2[8], c[6];
-      eg_load8(0, g1);
-      eg_load8(uf::EG_E2 + 10, g2);
-      um::cos_ladder(fmaf(Bd[2 * um::DIRS_PITCH + 20], t2x, fmaf(Bd[um::DIRS_PITCH + 20], t1x, Bd[20] * t0x)), c);
-      float d = g1[4] * c[0];
-      d = fmaf(2.f * g1[5], c[1], d); d = fmaf(4.f * g1[6], c[2], d); d = fmaf(8.f * g1[7], c[3], d);
-      d = fmaf(16.f * g2[0], c[4], d); d = fmaf(32.f * g2[1], c[5], d);
-      const float g = (d * VMB_PI_F) * INV_LS;
-      jt0 = fmaf(g, Bd[20], jt0); jt1 = fmaf(g, Bd[um::DIRS_PITCH + 20], jt1); jt2 = fmaf(g, Bd[2 * um::DIRS_PITCH + 20], jt2);
-      *reinterpret_cast<float4*>(smem + SM_DT + p * 16) = make_float4(jt0, jt1, jt2, 0.f);
-    }
-  }
+  // ---- PE backward: this warpgroup's half of dL/dt, warpgroup 1's to shared memory ------------------------------------
+  const float3 jt = tl.pe_backward<false>(tin);
+  if (hsel) *reinterpret_cast<float4*>(smem + SM_DT + p * 16) = make_float4(jt.x, jt.y, jt.z, 0.f);
   __syncthreads();
 
   // ---- pose terms in fp64 per point, the ray's samples summed in order into its row ---------------------------------
   if (hsel == 0) {
     const float4 h1 = *reinterpret_cast<const float4*>(smem + SM_DT + p * 16);
     double c6[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-    if (pok) pose_terms(T, make_double3(q.x, q.y, q.z), make_float3(jt0 + h1.x, jt1 + h1.y, jt2 + h1.z), sc, c6);
+    if (pok) pose_terms(T, make_double3(q.x, q.y, q.z), make_float3(jt.x + h1.x, jt.y + h1.y, jt.z + h1.z), sc, c6);
     double s6[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
     for (int s = 0; s < S; ++s)
 #pragma unroll
