@@ -1,10 +1,12 @@
 """Relocalisation without a GPU: the hypothesis set, the selection order's restatement and the C declarations."""
+import contextlib
 import math
 import os
 import re
 
 import numpy as np
 import pytest
+import torch
 
 from vmap_b200 import reloc
 
@@ -59,3 +61,75 @@ def test_declarations_match_the_binding():
     src = open(reloc.__file__).read()
     assert "vmb_reloc_score(" in src and "vmb_reloc_select(" in src
     assert math.isclose(reloc.ROUND2_SHRINK, 0.25)
+
+
+def test_select_order_all_non_finite_infinities_and_signed_zeros():
+    nan, inf = float("nan"), float("inf")
+    assert select_order([nan] * 5, 5) == [0, 1, 2, 3, 4]
+    assert select_order([inf, -inf, 2.0, nan, -inf, -1.0], 6) == [5, 2, 0, 1, 3, 4]
+    assert select_order([0.0, -0.0, 1.0, -0.0, 0.0, -1.0], 6) == [5, 0, 1, 3, 4, 2]
+    assert select_order([7.0], 1) == [0]
+
+
+# ---- Relocalizer's argument checks, on a stand-in group whose library must never be reached ------------------------
+
+class _NoLaunch:
+    def __getattr__(self, name):
+        raise AssertionError(f"{name} was called")
+
+
+class _Ens:
+    device, hidden, colour_scaling, opacity_scaling = torch.device("cpu"), 32, 5.0, 10.0
+    lib, image, _handle = _NoLaunch(), None, None
+
+    def _on_device(self):
+        return contextlib.nullcontext()
+
+
+class _Group:
+    path, ens, active = "fused", _Ens(), [0, 1, 2]
+
+    def bind(self, g, it):
+        pass
+
+
+def _reloc(n_groups=1):
+    return reloc.Relocalizer([_Group() for _ in range(n_groups)], n_hyp=16, top_k=4)
+
+
+def test_score_checks_its_arguments_before_any_launch():
+    from vmap_b200 import _lib
+    rl = _reloc()
+    P = torch.eye(4, dtype=torch.float64).repeat(6, 1, 1)
+    f64 = dict(dtype=torch.float64)
+    bad = [(P[:, :, :3], None), (P.reshape(6, 16), None), (P.reshape(2, 3, 4, 4), None), (P.long(), None),
+           (P[:0], None), (P[:1].expand(_lib.RELOC_MAX_HYP + 1, 4, 4), None), (P.numpy(), None),
+           (P, torch.zeros(6, 3, 4)), (P, torch.zeros(6, 2, 4, **f64)), (P, torch.zeros(5, 3, 4, **f64)),
+           (P, torch.zeros(6, 3, 5, **f64)), (P, torch.zeros(4, 3, 6, **f64).permute(2, 1, 0)),
+           (P, torch.zeros(72, **f64)), (P, np.zeros((6, 3, 4)))]
+    for poses, terms in bad:
+        with pytest.raises(_lib.VmbError):
+            rl.score(poses, terms)
+    with pytest.raises(_lib.VmbError, match="one group"):       # one buffer of terms cannot hold two groups' rows
+        _reloc(2).score(P, torch.zeros(6, 3, 4, **f64))
+    for poses, terms in ((P, None), (P[0], None), (P, torch.zeros(6, 3, 4, **f64)), (P.float(), None)):
+        with pytest.raises(AssertionError, match="vmb_reloc_score"):   # well-formed: they reach the library
+            rl.score(poses, terms)
+
+
+def test_select_checks_its_arguments_before_any_launch():
+    from vmap_b200 import _lib
+    rl = _reloc()
+    s = torch.arange(6, dtype=torch.float64)
+    P = torch.eye(4, dtype=torch.float64).repeat(6, 1, 1)
+    big = _lib.RELOC_MAX_HYP + 1
+    bad = [(s.float(), P, 2), (s[None], P, 2), (s[:0], P[:0], 1), (s.numpy(), P, 2), (s, P[:5], 2), (s, P.float(), 2),
+           (s, P.reshape(6, 16), 2), (s, P.numpy(), 2), (s, P, 0), (s, P, 7), (s, P, 2.5), (s, P, True),
+           (torch.zeros(big, dtype=torch.float64), torch.zeros(big, 4, 4, dtype=torch.float64), 2),
+           (torch.zeros(100, dtype=torch.float64), torch.zeros(100, 4, 4, dtype=torch.float64), _lib.RELOC_MAX_K + 1)]
+    for scores, poses, k in bad:
+        with pytest.raises(_lib.VmbError):
+            rl.select(scores, poses, k)
+    for k in (1, 6):
+        with pytest.raises(AssertionError, match="vmb_reloc_select"):
+            rl.select(s, P, k)

@@ -110,14 +110,35 @@ class Relocalizer:
                                     f"(a hidden-{g.ens.hidden} group takes path {g.path!r})")
         return live
 
+    def _on_device(self, t) -> bool:
+        dev = torch.device(self.device)
+        if dev.type == "cuda" and dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        return torch.is_tensor(t) and t.device == dev
+
+    def _poses(self, poses, who: str) -> torch.Tensor:
+        if not self._on_device(poses) or not poses.is_floating_point() or poses.dim() not in (2, 3) \
+                or tuple(poses.shape[-2:]) != (4, 4):
+            raise _lib.VmbError(f"{who}: poses must be a floating-point [H, 4, 4] tensor on {self.device}")
+        return poses.reshape(-1, 4, 4).to(torch.float64).contiguous()
+
     def score(self, poses: torch.Tensor, terms: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Slice-0 tracking loss [H] fp64 of each pose of ``poses`` [H, 4, 4] (device, fp64); ``terms``: optional
-        [H, B, 4] fp64 per-object terms of a one-group tracker."""
+        [H, B, 4] contiguous fp64 device tensor of per-object terms (L_d, L_c, L_o, total), one group only (a second
+        group's call would overwrite the first's rows).  Arguments are checked before any launch."""
         live = self._groups()
-        poses = poses.reshape(-1, 4, 4).to(torch.float64).contiguous()
+        poses = self._poses(poses, "Relocalizer.score")
         H = poses.shape[0]
         if not 1 <= H <= _lib.RELOC_MAX_HYP:
             raise _lib.VmbError(f"Relocalizer.score: 1 .. {_lib.RELOC_MAX_HYP} poses")
+        if terms is not None:
+            if len(live) != 1:
+                raise _lib.VmbError(f"Relocalizer.score: terms need exactly one group ({len(live)} are live)")
+            B = len(live[0].active)
+            if not (self._on_device(terms) and terms.dtype == torch.float64 and tuple(terms.shape) == (H, B, 4)
+                    and terms.is_contiguous()):
+                raise _lib.VmbError(f"Relocalizer.score: terms must be a contiguous fp64 [{H}, {B}, 4] tensor on "
+                                    f"{self.device}")
         scores = torch.zeros(H, dtype=torch.float64, device=poses.device)
         a = _lib.TrackArgs()
         a.n_groups, a.n_iter, a.iter = len(live), 1, 1
@@ -134,12 +155,23 @@ class Relocalizer:
         return scores
 
     def select(self, scores: torch.Tensor, poses: torch.Tensor, k: int) -> Tuple[torch.Tensor, torch.Tensor]:
-        """The ``k`` best (lowest score, ties to the lower index, non-finite last): (indices [k] int32, poses [k,4,4])."""
+        """The ``k`` best (lowest score, ties to the lower index, non-finite last): (indices [k] int32, poses [k,4,4]).
+        ``scores`` [n] and ``poses`` [n, 4, 4]: fp64 tensors on the groups' device; 1 <= k <= min(n, RELOC_MAX_K)."""
+        if not (self._on_device(scores) and scores.dtype == torch.float64 and scores.dim() == 1):
+            raise _lib.VmbError(f"Relocalizer.select: scores must be a 1-D fp64 tensor on {self.device}")
         n = scores.numel()
+        if not 1 <= n <= _lib.RELOC_MAX_HYP:
+            raise _lib.VmbError(f"Relocalizer.select: 1 .. {_lib.RELOC_MAX_HYP} scores")
+        if not (self._on_device(poses) and poses.dtype == torch.float64 and tuple(poses.shape) == (n, 4, 4)):
+            raise _lib.VmbError(f"Relocalizer.select: poses must be an fp64 [{n}, 4, 4] tensor on {self.device}")
+        if not isinstance(k, (int, np.integer)) or isinstance(k, bool) or not 1 <= k <= min(n, _lib.RELOC_MAX_K):
+            raise _lib.VmbError(f"Relocalizer.select: k must be in [1, min(n, {_lib.RELOC_MAX_K})]")
+        k = int(k)
+        scores = scores.contiguous()
         idx = torch.empty(k, dtype=torch.int32, device=scores.device)
         out = torch.empty(k, 4, 4, dtype=torch.float64, device=scores.device)
         e = self._groups()[0].ens
-        poses = poses.reshape(-1, 4, 4).contiguous()
+        poses = poses.contiguous()
         with e._on_device():
             _lib.check(e._handle, e.lib.vmb_reloc_select(e._handle, n, _ptr(scores), _ptr(poses), k, _ptr(idx),
                                                          _ptr(out), _stream()), "vmb_reloc_select")
