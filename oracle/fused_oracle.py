@@ -222,7 +222,10 @@ def fused_step(params: Dict[str, torch.Tensor], scale, batch: Dict[str, torch.Te
     batch: the six step inputs; counts: [B,4] mask counts (default: from this batch); signs: [B,R,5] residual signs;
     emb: (E1 [B,R*S,87], E2 [B,R*S,42]) to use as the embedding (the kernel's own, see ``tests/test_fused_faithful_gpu``);
     var: [B,R] ray variances for the depth-loss weight 1 / (sqrt(var) + 1e-4) (e.g. the kernel's: the fp32 sum
-    cancels on rays whose weight sits on one sample, and the weight amplifies that); ls: the loss scale; aux: a dict that receives ``dh`` (``ls * dh`` before its fp16 pack, [B,P,4]).
+    cancels on rays whose weight sits on one sample, and the weight amplifies that); ls: the loss scale; aux: a dict
+    that receives ``dh`` (``ls * dh`` before its fp16 pack, [B,P,4]), ``dproj`` ([B,P,21], before its fp16 pack) and
+    ``dt`` (each point's dL/dt = ``INV_LS (dE1_xyz + dproj @ dirs)`` [B,P,3] from that unrounded dproj, as the joint
+    step's ``pe_backward`` forms it).
     Returns ``(render, loss_terms, grads)`` as ``oracle.lw_oracle.lw_step`` does; all fp64."""
     dev = batch["pcs"].device
     f64 = dict(dtype=torch.float64, device=dev)
@@ -327,6 +330,9 @@ def fused_step(params: Dict[str, torch.Tensor], scale, batch: Dict[str, torch.Te
     cb = cos_bands(proj, rnd.cos32)
     pi = PI_F if rnd.cos32 else math.pi
     dproj = sum(dband[..., k * N_DIRS:(k + 1) * N_DIRS] * (2.0 ** k) * cb[k] for k in range(N_BANDS)) * pi
+    if aux is not None:                                                                # pe_backward: from fp32 dproj
+        aux["dproj"] = dproj
+        aux["dt"] = inv_ls * (dE1[..., :3] + mm(dproj, p[PE_KEY]))
     dproj = _half(dproj, rnd.dproj)
     tt = emb1[..., :3] if (rnd.t16 and emb is not None) else _half(t, rnd.t16)
     g[PE_KEY] = inv_ls * mm(tr(dproj), tt)
