@@ -68,7 +68,12 @@ const char* vmb_version(void);
 /* ---- lifetime ------------------------------------------------------------------------ */
 /* Allocates per-handle scratch only (mask counts etc.).  Replaces nothing in the
  * reference; it is the moral equivalent of `optimiser = torch.optim.AdamW(...)`
- * (train.py:67) + `update_vmap` (utils.py:30-34) creating the stacked state.             */
+ * (train.py:67) + `update_vmap` (utils.py:30-34) creating the stacked state.
+ * Scratch rule: every scratch buffer on the handle grows on demand, sized by the calls
+ * that use it, and is freed by vmb_destroy.  A buffer is never moved once a CUDA graph
+ * captured on a stream holds it (and never grows during a capture), so after a capture a
+ * call that needs it larger fails with VMB_E_CUDA ("operation not permitted when stream
+ * is capturing"): run the largest shape eagerly before capturing.                        */
 int vmb_create(vmb_handle** out, int device, int max_obj, int hidden, int n_freq);
 void vmb_destroy(vmb_handle* h);
 const char* vmb_last_error(const vmb_handle* h);
@@ -754,8 +759,8 @@ int vmb_ba_step_fused(vmb_handle* h, const vmb_ba_args* a, int group, const void
  * a NULL image, hyps, scores or idx.  VMB_E_UNSUPPORTED: hidden != 32 or n_freq != 6, n_samples > 32.  On the device: a
  * row outside [0, n_rows) contributes 0 and sets VMB_TRACK_ST_BAD_ROW.  No floating-point atomics: bitwise reproducible,
  * and a hypothesis's score does not depend on n_hyp.  The per-ray scratch ([n_hyp][n_obj][n_rays][3] fp64 on the
- * handle) grows on demand and is never moved once a captured graph holds it: after a capture, a call with a larger
- * n_hyp * n_obj * n_rays fails with VMB_E_CUDA (run the largest shape eagerly first).  Registers as in k_reloc.cuh. */
+ * handle) follows the scratch rule (vmb_create): after a capture, a call with a larger n_hyp * n_obj * n_rays fails
+ * with VMB_E_CUDA.  Registers as in k_reloc.cuh. */
 #define VMB_RELOC_MAX_HYP 4096
 #define VMB_RELOC_MAX_K 64
 int vmb_reloc_score(vmb_handle* h, const vmb_track_args* a, int group, int n_hyp, const double* hyps, double* scores,

@@ -321,31 +321,12 @@ __global__ void k_fin_relabel(FinParams q) {
 // Handle-owned, grow-only scratch.  The classify outputs (flags, sorted selection) are read by voxel and finalize,
 // so the three calls of one frame must use the same handle in order.
 struct Workspace {
-  unsigned char* pix = nullptr; size_t pix_cap = 0;     // flags | rowok | sel_key | sel_key_out | sel_val | sel_val_out
-  unsigned char* ids = nullptr; size_t ids_cap = 0;     // new_off | seg_off | minb | status | ext
-  unsigned char* el = nullptr; size_t el_cap = 0;       // elem | ekey | ekey_out | eidx | eidx_out | head
-  void* cub_tmp = nullptr; size_t cub_cap = 0;
+  DeviceBuffer<unsigned char> pix;      // flags | rowok | sel_key | sel_key_out | sel_val | sel_val_out
+  DeviceBuffer<unsigned char> ids;      // new_off | seg_off | minb | status | ext
+  DeviceBuffer<unsigned char> el;       // elem | ekey | ekey_out | eidx | eidx_out | head
+  DeviceBuffer<void> cub_tmp;
   Params last{};
   bool classified = false;
-
-  static cudaError_t grow(void** p, size_t* cap, size_t need) {
-    if (*cap >= need) return cudaSuccess;
-    if (*p) cudaFree(*p);
-    *p = nullptr; *cap = 0;
-    const cudaError_t e = cudaMalloc(p, need);
-    if (e == cudaSuccess) *cap = need;
-    return e;
-  }
-  cudaError_t tmp(size_t need) { return grow(&cub_tmp, &cub_cap, need); }
-  void release() {
-    if (pix) cudaFree(pix);
-    if (ids) cudaFree(ids);
-    if (el) cudaFree(el);
-    if (cub_tmp) cudaFree(cub_tmp);
-    pix = ids = el = nullptr; cub_tmp = nullptr;
-    pix_cap = ids_cap = el_cap = cub_cap = 0;
-    classified = false;
-  }
 };
 
 inline size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }

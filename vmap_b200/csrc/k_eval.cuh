@@ -353,43 +353,26 @@ __global__ void __launch_bounds__(128) k_nn_query(NnParams q) {
 // Handle-owned, grow-only scratch of the evaluation kernels; the crop scan is kept apart from the rest so sampling or a
 // nearest-neighbour query between a crop count and its emit does not disturb the counts.
 struct Workspace {
-  int* clip_scan = nullptr; size_t clip_cap = 0;
-  double* cum = nullptr; size_t cum_cap = 0;            // surface sampling: areas / prefix, then a flag int
-  unsigned char* nn = nullptr; size_t nn_cap = 0;        // keys | grid | cell_start | pt_cell | pt_rank | sorted
-  void* cub_tmp = nullptr; size_t cub_cap = 0;
+  DeviceBuffer<int> clip_scan;
+  DeviceBuffer<double> cum;                              // surface sampling: areas / prefix, then a flag int
+  DeviceBuffer<unsigned char> nn;                        // keys | grid | cell_start | pt_cell | pt_rank | sorted
+  DeviceBuffer<void> cub_tmp;
   ClipParams last{};                                     // the last crop count (emit must match it)
   bool counted = false;
 
-  static cudaError_t grow(void** p, size_t* cap, size_t need) {
-    if (*cap >= need) return cudaSuccess;
-    if (*p) cudaFree(*p);
-    *p = nullptr; *cap = 0;
-    const cudaError_t e = cudaMalloc(p, need);
-    if (e == cudaSuccess) *cap = need;
-    return e;
-  }
-  cudaError_t exclusive_sum(int* d, long long n, cudaStream_t st) {
+  cudaError_t exclusive_sum(int* d, long long n, bool capturing, cudaStream_t st) {
     size_t need = 0;
     cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, need, d, (int)n, st);
-    if (e == cudaSuccess) e = grow(&cub_tmp, &cub_cap, need);
+    if (e == cudaSuccess) e = cub_tmp.grow(need, capturing);
     if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(cub_tmp, need, d, (int)n, st);
     return e;
   }
-  cudaError_t inclusive_sum(double* d, long long n, cudaStream_t st) {
+  cudaError_t inclusive_sum(double* d, long long n, bool capturing, cudaStream_t st) {
     size_t need = 0;
     cudaError_t e = cub::DeviceScan::InclusiveSum(nullptr, need, d, d, (int)n, st);
-    if (e == cudaSuccess) e = grow(&cub_tmp, &cub_cap, need);
+    if (e == cudaSuccess) e = cub_tmp.grow(need, capturing);
     if (e == cudaSuccess) e = cub::DeviceScan::InclusiveSum(cub_tmp, need, d, d, (int)n, st);
     return e;
-  }
-  void release() {
-    if (clip_scan) cudaFree(clip_scan);
-    if (cum) cudaFree(cum);
-    if (nn) cudaFree(nn);
-    if (cub_tmp) cudaFree(cub_tmp);
-    clip_scan = nullptr; cum = nullptr; nn = nullptr; cub_tmp = nullptr;
-    clip_cap = cum_cap = nn_cap = cub_cap = 0;
-    counted = false;
   }
 };
 

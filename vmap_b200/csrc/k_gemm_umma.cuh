@@ -530,24 +530,18 @@ struct Operand { const void* base; long long rows, cols, ld; };
 template <int A_MN, int B_MN, int EPI>
 static cudaError_t launch_gemm(const Operand& a1, const Operand& a2, const Operand& b, GemmArgs g, int m_tiles, int n_tiles,
                                int z, cudaStream_t st) {
-  static bool attr[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (!attr[dev & 63]) {
-    cudaError_t e = cudaFuncSetAttribute(k_gemm_umma<A_MN, B_MN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM);
-    if (e != cudaSuccess) return e;
-    attr[dev & 63] = true;
-  }
+  const cudaError_t e = smem_limit_once<k_gemm_umma<A_MN, B_MN, EPI>>(dev, GEMM_SMEM);
+  if (e != cudaSuccess) return e;
   CUtensorMap mA1, mA2, mB;
   if (!make_operand_map(&mA1, a1.base, a1.rows, a1.cols, a1.ld, A_MN)) return cudaErrorInvalidValue;
   if (a2.base) { if (!make_operand_map(&mA2, a2.base, a2.rows, a2.cols, a2.ld, A_MN)) return cudaErrorInvalidValue; }
   else mA2 = mA1;
   if (!make_operand_map(&mB, b.base, b.rows, b.cols, b.ld, B_MN)) return cudaErrorInvalidValue;
-  static int n_sm[64] = {};
-  if (!n_sm[dev & 63]) cudaDeviceGetAttribute(&n_sm[dev & 63], cudaDevAttrMultiProcessorCount, dev);
   g.mt = m_tiles; g.nt = n_tiles; g.zt = z;
   const long long total = (long long)m_tiles * n_tiles * z;
-  const int grid = (int)std::min<long long>(total, (long long)n_sm[dev & 63]);
+  const int grid = (int)std::min<long long>(total, (long long)sm_count(dev));
   return launch_k(k_gemm_umma<A_MN, B_MN, EPI>, dim3(grid), dim3(GEMM_THREADS), GEMM_SMEM, st, mA1, mA2, mB, g);
 }
 
@@ -567,12 +561,9 @@ static cudaError_t launch_gemm_ws(const Operand& a1, const Operand& a2, const Op
   int dev = 0;
   cudaGetDevice(&dev);
   auto kern = g.N > 128 ? k_gemm_ws<B_MN, EPI, 2> : k_gemm_ws<B_MN, EPI, 1>;
-  static bool attr[64][2] = {};
-  if (!attr[dev & 63][g.N > 128]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, WS_SMEM);
-    if (e != cudaSuccess) return e;
-    attr[dev & 63][g.N > 128] = true;
-  }
+  const cudaError_t e = g.N > 128 ? smem_limit_once<k_gemm_ws<B_MN, EPI, 2>>(dev, WS_SMEM)
+                                   : smem_limit_once<k_gemm_ws<B_MN, EPI, 1>>(dev, WS_SMEM);
+  if (e != cudaSuccess) return e;
   CUtensorMap mA1, mA2, mB;
   if (!make_operand_map(&mA1, a1.base, a1.rows, a1.cols, a1.ld, 0)) return cudaErrorInvalidValue;
   if (a2.base) { if (!make_operand_map(&mA2, a2.base, a2.rows, a2.cols, a2.ld, 0)) return cudaErrorInvalidValue; }
@@ -581,10 +572,8 @@ static cudaError_t launch_gemm_ws(const Operand& a1, const Operand& a2, const Op
   CUtensorMap mB2 = mB;
   g.b_two = 0;
   if (b2) { if (!make_operand_map(&mB2, b2->base, b2->rows, b2->cols, b2->ld, B_MN)) return cudaErrorInvalidValue; g.b_two = 1; }
-  static int n_sm[64] = {};
-  if (!n_sm[dev & 63]) cudaDeviceGetAttribute(&n_sm[dev & 63], cudaDevAttrMultiProcessorCount, dev);
   g.mt = m_tiles; g.nt = 1; g.zt = 1;
-  const int grid = std::min(m_tiles, n_sm[dev & 63]);
+  const int grid = std::min(m_tiles, sm_count(dev));
   return launch_k(kern, dim3(grid), dim3(WS_THREADS), WS_SMEM, st, mA1, mA2, mB, mB2, g, geo);
 }
 

@@ -714,27 +714,11 @@ __global__ void __launch_bounds__(NT) k_obb_pick(ObbParams q) {
   *q.box_status = ST_OK;
 }
 
-// ---- handle scratch (grow-only) -------------------------------------------------------------------------------------
+// ---- handle scratch (DeviceBuffer's rule) -------------------------------------------------------------------------
 struct Workspace {
-  unsigned char* buf = nullptr; size_t cap = 0;
-  void* cub_tmp = nullptr; size_t cub_cap = 0;
-  double* obb = nullptr; size_t obb_cap = 0;
-
-  static cudaError_t grow(void** p, size_t* cap, size_t need) {
-    if (*cap >= need) return cudaSuccess;
-    if (*p) cudaFree(*p);
-    *p = nullptr; *cap = 0;
-    const cudaError_t e = cudaMalloc(p, need);
-    if (e == cudaSuccess) *cap = need;
-    return e;
-  }
-  void release() {
-    if (buf) cudaFree(buf);
-    if (cub_tmp) cudaFree(cub_tmp);
-    if (obb) cudaFree(obb);
-    buf = nullptr; cub_tmp = nullptr; obb = nullptr;
-    cap = cub_cap = obb_cap = 0;
-  }
+  DeviceBuffer<unsigned char> buf;
+  DeviceBuffer<void> cub_tmp;
+  DeviceBuffer<double> obb;
 };
 
 inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }

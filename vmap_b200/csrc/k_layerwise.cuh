@@ -44,31 +44,12 @@ static void fill_image_index(const VmbLayout& L, int* idx) {
   }
 }
 
-// multiprocessors of the current device (launch sizing)
-static int sm_count() {
-  static int n[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (!n[dev & 63]) cudaDeviceGetAttribute(&n[dev & 63], cudaDevAttrMultiProcessorCount, dev);
-  return n[dev & 63] > 0 ? n[dev & 63] : 132;
-}
+// point counts of the workspaces' per-point buffers are rounded up to whole 128-point blocks
+inline long long pad_points(long long P) { return (P + 127) / 128 * 128; }
 
 struct Workspace {
-  long long cap_points = 0; int H = 0;
-  __half *E = nullptr, *X1 = nullptr, *X2 = nullptr, *X3 = nullptr, *X4 = nullptr, *XC = nullptr;
-  __half *dYa = nullptr, *dYb = nullptr, *dYc = nullptr, *dh16 = nullptr;
-  float *dalpha_s = nullptr, *dE = nullptr;
-  void release() {
-    void* ptrs[] = {E, X1, X2, X3, X4, XC, dYa, dYb, dYc, dh16, dalpha_s, dE};
-    for (void* q : ptrs) if (q) cudaFree(q);
-    cudaStream_t keep_s = side; cudaEvent_t km[5], ks[2];
-    for (int i = 0; i < 5; ++i) km[i] = ev_main[i];
-    for (int i = 0; i < 2; ++i) ks[i] = ev_side[i];
-    *this = Workspace();
-    side = keep_s;
-    for (int i = 0; i < 5; ++i) ev_main[i] = km[i];
-    for (int i = 0; i < 2; ++i) ev_side[i] = ks[i];
-  }
+  DeviceBuffer<__half> E, X1, X2, X3, X4, XC, dYa, dYb, dYc, dh16;
+  DeviceBuffer<float> dalpha_s, dE;
   // side stream of the backward pass: the weight-gradient GEMMs of a layer depend only on that layer's dY, so they run
   // beside the input-gradient chain (fork / join with events; inside a stream capture they become parallel graph branches)
   cudaStream_t side = nullptr;
@@ -80,33 +61,21 @@ struct Workspace {
     for (auto& v : ev_side) if (e == cudaSuccess) e = cudaEventCreateWithFlags(&v, cudaEventDisableTiming);
     return e;
   }
-  void destroy_streams() {
-    for (auto& v : ev_main) if (v) { cudaEventDestroy(v); v = nullptr; }
-    for (auto& v : ev_side) if (v) { cudaEventDestroy(v); v = nullptr; }
-    if (side) { cudaStreamDestroy(side); side = nullptr; }
+  ~Workspace() {
+    for (auto v : ev_main) if (v) cudaEventDestroy(v);
+    for (auto v : ev_side) if (v) cudaEventDestroy(v);
+    if (side) cudaStreamDestroy(side);
   }
-  bool in_graph = false;       // a captured CUDA graph holds these pointers: the buffers must never move again
-  // Grow-only.  Never reallocates while the stream is capturing or after a capture has baked the pointers
-  // into a graph (kernel arguments and TMA tensor maps): that would be a use-after-free at the next replay.
-  cudaError_t ensure(long long P, int H_, cudaStream_t st) {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(st, &cs);
-    const bool capturing = cs != cudaStreamCaptureStatusNone;
-    if (P <= cap_points && H_ == H) { in_graph |= capturing; return cudaSuccess; }
-    if (capturing || in_graph) return cudaErrorStreamCaptureUnsupported;
-    release();
-    const long long Pp = (P + 127) / 128 * 128;
-    cudaError_t e = cudaSuccess;
-    auto al = [&](void** q, size_t bytes) { if (e == cudaSuccess) e = cudaMalloc(q, bytes); };
-    al((void**)&E, Pp * EW * 2);
-    __half** hs[] = {&X1, &X2, &X3, &X4, &XC, &dYa, &dYb, &dYc};
-    for (auto q : hs) al((void**)q, Pp * H_ * 2);
-    al((void**)&dh16, Pp * 8 * 2);
-    al((void**)&dalpha_s, Pp * 4);
-    al((void**)&dE, Pp * EW * 4);
-    if (e != cudaSuccess) { release(); return e; }
-    cap_points = Pp; H = H_;
-    return cudaSuccess;
+  // every buffer for P points of a hidden-H model
+  cudaError_t grow(long long P, int H, bool capturing) {
+    const size_t Pp = (size_t)pad_points(P);
+    cudaError_t e = E.grow(Pp * EW * 2, capturing);
+    for (auto* x : {&X1, &X2, &X3, &X4, &XC, &dYa, &dYb, &dYc})
+      if (e == cudaSuccess) e = x->grow(Pp * H * 2, capturing);
+    if (e == cudaSuccess) e = dh16.grow(Pp * 8 * 2, capturing);
+    if (e == cudaSuccess) e = dalpha_s.grow(Pp * 4, capturing);
+    if (e == cudaSuccess) e = dE.grow(Pp * EW * 4, capturing);
+    return e;
   }
 };
 
@@ -557,7 +526,7 @@ static cudaError_t demb1_gemm(Workspace& ws, const __half* dY3, const __half* dY
   return e;
 }
 
-#define LW_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return -2; } } while (0)
+#define LW_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return VMB_E_CUDA; } } while (0)
 
 template <int H>
 static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, const __half* image, int b, cudaStream_t st,
@@ -596,26 +565,22 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
   ra.mask = sp.mask + (size_t)b * sp.mask_stride; ra.counts = sp.counts; ra.cs = sp.cs; ra.os = sp.os; ra.backward = sp.backward;
   ra.loss_terms = sp.loss_terms; ra.r_depth = sp.r_depth; ra.r_var = sp.r_var; ra.r_colour = sp.r_colour; ra.r_opacity = sp.r_opacity;
   // heads + render + loss (+ head gradients when training) in one launch
-  {
-    static bool attr_set[64] = {};
-    int dev = 0; cudaGetDevice(&dev);
-    if (!attr_set[dev & 63]) {
-      LW_TRY(cudaFuncSetAttribute(k_lw_heads_render<H>, cudaFuncAttributeMaxDynamicSharedMemorySize, hr_smem<H>()));
-      attr_set[dev & 63] = true;
-    }
-  }
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const int n_sm = sm_count(dev);
+  LW_TRY(smem_limit_once<k_lw_heads_render<H>>(dev, hr_smem<H>()));
   const int hr_per_sm = std::max(1, std::min(8, (int)(227 * 1024 / (hr_smem<H>() + 6 * 1024))));
   arm();
-  LW_TRY(launch_k(k_lw_heads_render<H>, dim3(std::min((sp.R + 3) / 4, sm_count() * hr_per_sm)), dim3(128), (size_t)hr_smem<H>(), st, ra,
+  LW_TRY(launch_k(k_lw_heads_render<H>, dim3(std::min((sp.R + 3) / 4, n_sm * hr_per_sm)), dim3(128), (size_t)hr_smem<H>(), st, ra,
                   (const __half*)ws.X4, (const __half*)ws.XC, Pb, L, ws.dYc, ws.dh16, ws.dalpha_s, G));
   if (!sp.backward) return 0;
 
   // ---- backward ----
   // split over points: enough z slices that the widest weight-gradient GEMM (2 x 2 output tiles) fills the machine
   // (one resident CTA per SM) at any point count, bounded below so a slice still amortises its pipeline fill
-  const int ksplit = (int)std::min<long long>(4096, std::max<long long>(512, ((np * 4 / sm_count() + BK - 1) / BK) * BK));
+  const int ksplit = (int)std::min<long long>(4096, std::max<long long>(512, ((np * 4 / n_sm + BK - 1) / BK) * BK));
   const int zs = (int)((np + ksplit - 1) / ksplit);
-  const int cs_rows = (int)std::max<long long>(64, (np + 4 * sm_count() - 1) / (4 * sm_count()));       // bias column sums: ~4 blocks per SM
+  const int cs_rows = (int)std::max<long long>(64, (np + 4 * n_sm - 1) / (4 * n_sm));       // bias column sums: ~4 blocks per SM
   // weight gradient: G[o*ldm + n] += sum_p dY[p][o] * X[p][n]   (A = dY^T, B = X, both MN-major, split over points)
   LW_TRY(ws.ensure_streams());
   cudaStream_t sd = ws.side;
@@ -673,15 +638,8 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
   LW_TRY(wgrad(ws.dYc, opE1, E1W, L.o_Win, VMB_E1, VMB_E1, ONES1, L.o_bin));
   LW_TRY(cudaEventRecord(ws.ev_side[1], sd));
   LW_TRY(demb1_gemm<H>(ws, ws.dYb, ws.dYc, Wi, np, st));                                        // d emb1 (dY3, dY1)
-  {
-    static bool attr_set[64] = {};
-    int dev = 0; cudaGetDevice(&dev);
-    if (!attr_set[dev & 63]) {
-      LW_TRY(cudaFuncSetAttribute(k_lw_pe_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, PEB_SMEM));
-      attr_set[dev & 63] = true;
-    }
-  }
-  arm();                                          // follows the embedding-gradient GEMM directly on `st`
+  LW_TRY(smem_limit_once<k_lw_pe_bwd>(dev, PEB_SMEM));
+  arm();                                         // follows the embedding-gradient GEMM directly on `st`
   LW_TRY(launch_k(k_lw_pe_bwd, dim3(nblk), dim3(128), (size_t)PEB_SMEM, st, pcs, dirs, scale_p, np, (const float*)ws.dE, G + L.o_B));
   LW_TRY(cudaStreamWaitEvent(st, ws.ev_side[1], 0));    // join: every weight-gradient GEMM of this object has been enqueued before what follows
   LW_TRY(cudaGetLastError());
@@ -691,9 +649,9 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
 // forward only (vmb_forward): chunks of FWD_CHUNK points so the activation workspace stays bounded for 256^3 grids
 constexpr long long FWD_CHUNK = 1LL << 18;
 static int launch_forward(Workspace& ws, const VmbLayout& L, const StepParams& sp, const void* image, cudaStream_t st, std::string& err) {
-  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return -2; }
+  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return VMB_E_CUDA; }
   const long long N = sp.R;
-  LW_TRY(ws.ensure(std::min(N, FWD_CHUNK), L.H, st));
+  LW_TRY(ws.grow(std::min(N, FWD_CHUNK), L.H, stream_capturing(st)));
   for (int b = 0; b < sp.B; ++b)
     for (long long p0 = 0; p0 < N; p0 += FWD_CHUNK) {
       const long long n = std::min(FWD_CHUNK, N - p0);
@@ -702,7 +660,7 @@ static int launch_forward(Workspace& ws, const VmbLayout& L, const StepParams& s
         case 64:  rc = step_object<64>(ws, L, sp, (const __half*)image, b, st, err, p0, n); break;
         case 128: rc = step_object<128>(ws, L, sp, (const __half*)image, b, st, err, p0, n); break;
         case 256: rc = step_object<256>(ws, L, sp, (const __half*)image, b, st, err, p0, n); break;
-        default: err = "layer-wise path: hidden must be 64, 128 or 256"; return -4;
+        default: err = "layer-wise path: hidden must be 64, 128 or 256"; return VMB_E_UNSUPPORTED;
       }
       if (rc) return rc;
     }
@@ -710,16 +668,16 @@ static int launch_forward(Workspace& ws, const VmbLayout& L, const StepParams& s
 }
 
 static int launch_step(Workspace& ws, const VmbLayout& L, const StepParams& sp, const void* image, cudaStream_t st, std::string& err) {
-  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return -2; }
-  if (sp.S > 32) { err = "layer-wise path: n_samples > 32"; return -4; }
-  LW_TRY(ws.ensure((long long)sp.R * sp.S, L.H, st));
+  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return VMB_E_CUDA; }
+  if (sp.S > 32) { err = "layer-wise path: n_samples > 32"; return VMB_E_UNSUPPORTED; }
+  LW_TRY(ws.grow((long long)sp.R * sp.S, L.H, stream_capturing(st)));
   for (int b = 0; b < sp.B; ++b) {
     int rc;
     switch (L.H) {
       case 64:  rc = step_object<64>(ws, L, sp, (const __half*)image, b, st, err); break;
       case 128: rc = step_object<128>(ws, L, sp, (const __half*)image, b, st, err); break;
       case 256: rc = step_object<256>(ws, L, sp, (const __half*)image, b, st, err); break;
-      default: err = "layer-wise path: hidden must be 64, 128 or 256"; return -4;
+      default: err = "layer-wise path: hidden must be 64, 128 or 256"; return VMB_E_UNSUPPORTED;
     }
     if (rc) return rc;
   }

@@ -29,28 +29,10 @@ namespace rl {
 constexpr int NT = tf::NT;
 
 // per-(hypothesis, object, ray) loss terms [n_hyp][B][R][3] before K10's tile sums, sized by the call's n_hyp B R:
-// grow-only, and never moved once a captured graph holds them (tf::Workspace's rule), so after a capture a larger
-// call is refused (VMB_E_CUDA, cudaErrorStreamCaptureUnsupported): run the largest shape eagerly before capturing
+// handle scratch (DeviceBuffer's rule), so after a capture a larger call is refused (VMB_E_CUDA): run the largest shape
+// eagerly before capturing
 struct Workspace {
-  double* lray = nullptr;
-  long long cap = 0;
-  bool in_graph = false;
-  void release() {
-    if (lray) cudaFree(lray);
-    lray = nullptr; cap = 0; in_graph = false;
-  }
-  cudaError_t ensure(long long rays, cudaStream_t st) {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(st, &cs);
-    const bool capturing = cs != cudaStreamCaptureStatusNone;
-    if (rays <= cap) { in_graph |= capturing; return cudaSuccess; }
-    if (capturing || in_graph) return cudaErrorStreamCaptureUnsupported;
-    release();
-    cudaError_t e = cudaMalloc((void**)&lray, (size_t)rays * 3 * sizeof(double));
-    if (e != cudaSuccess) { release(); return e; }
-    cap = rays;
-    return cudaSuccess;
-  }
+  DeviceBuffer<double> lray;
 };
 
 // One CTA = fused tile blockIdx.x of object blockIdx.y, hypotheses [blockIdx.z * chunk, +chunk) of n_hyp.
@@ -179,8 +161,8 @@ __global__ void __launch_bounds__(256) k_reloc_select(int n, const double* __res
 static int launch_reloc_fused(Workspace& ws, const VmbLayout& L, const TrackParams& tp, const void* image,
                               const double* hyps, int n_hyp, double* scores, double* terms, int nr10, int n_sm,
                               cudaStream_t st, std::string& err) {
-  if (L.H != 32 || L.nfreq != 6) { err = "relocalisation scoring: hidden must be 32 and n_freq 6"; return -4; }
-  if (tp.S < 1 || tp.S > 32) { err = "relocalisation scoring: n_samples must be in [1, 32]"; return -4; }
+  if (L.H != 32 || L.nfreq != 6) { err = "relocalisation scoring: hidden must be 32 and n_freq 6"; return VMB_E_UNSUPPORTED; }
+  if (tp.S < 1 || tp.S > 32) { err = "relocalisation scoring: n_samples must be in [1, 32]"; return VMB_E_UNSUPPORTED; }
   const int rpw = 32 / tp.S, nr = 4 * rpw;
   const int tiles = (tp.R + nr - 1) / nr;
   // chunks of hypotheses: enough CTAs for about four waves of two per SM, each CTA reusing its image and counts
@@ -190,14 +172,14 @@ static int launch_reloc_fused(Workspace& ws, const VmbLayout& L, const TrackPara
   int dev = 0;
   cudaGetDevice(&dev);
   cudaError_t e = smem_limit_once<k_reloc_fused>(dev, tf::SMEM);
-  if (e == cudaSuccess) e = ws.ensure((long long)n_hyp * tp.B * tp.R, st);
-  if (e != cudaSuccess) { err = std::string("relocalisation scoring: ") + cudaGetErrorString(e); return -2; }
+  if (e == cudaSuccess) e = ws.lray.grow((size_t)n_hyp * tp.B * tp.R * 3 * sizeof(double), stream_capturing(st));
+  if (e != cudaSuccess) { err = std::string("relocalisation scoring: ") + cudaGetErrorString(e); return VMB_E_CUDA; }
   k_reloc_fused<<<dim3((unsigned)tiles, (unsigned)tp.B, (unsigned)n_chunks), NT, tf::SMEM, st>>>(
       tp, (const unsigned char*)image, hyps, n_hyp, chunk, nr, rpw, ws.lray);
   k_reloc_reduce<<<(unsigned)n_hyp, 256, 0, st>>>(tp.B, tp.R, nr10, (double)tp.cs, (double)tp.os, ws.lray, scores,
                                                   terms);
   e = cudaGetLastError();
-  if (e != cudaSuccess) { err = std::string("relocalisation scoring launch: ") + cudaGetErrorString(e); return -2; }
+  if (e != cudaSuccess) { err = std::string("relocalisation scoring launch: ") + cudaGetErrorString(e); return VMB_E_CUDA; }
   return 0;
 }
 

@@ -263,29 +263,12 @@ __global__ void __launch_bounds__(128) k_composite(Params q) {
 }
 
 struct Workspace {
-  double* boxes = nullptr; size_t boxes_cap = 0;
-  int* obj_id = nullptr; size_t id_cap = 0;
-  int* ints = nullptr; size_t ints_cap = 0;          // keys | keys_alt | vals | vals_alt | cnt | scan | wbase
-  void* cub_tmp = nullptr; size_t cub_cap = 0;
+  DeviceBuffer<double> boxes;
+  DeviceBuffer<int> obj_id;
+  DeviceBuffer<int> ints;                             // keys | keys_alt | vals | vals_alt | cnt | scan | wbase
+  DeviceBuffer<void> cub_tmp;
   Params last{};                                      // the last count (emit must match it)
   bool counted = false;
-
-  static cudaError_t grow(void** p, size_t* cap, size_t need) {
-    if (*cap >= need) return cudaSuccess;
-    if (*p) cudaFree(*p);
-    *p = nullptr; *cap = 0;
-    const cudaError_t e = cudaMalloc(p, need);
-    if (e == cudaSuccess) *cap = need;
-    return e;
-  }
-  void release() {
-    if (boxes) cudaFree(boxes);
-    if (obj_id) cudaFree(obj_id);
-    if (ints) cudaFree(ints);
-    if (cub_tmp) cudaFree(cub_tmp);
-    boxes = nullptr; obj_id = nullptr; ints = nullptr; cub_tmp = nullptr;
-    boxes_cap = id_cap = ints_cap = cub_cap = 0;
-  }
 };
 
 inline unsigned blocks_for(long long n, int bs) { return (unsigned)((n + bs - 1) / bs); }

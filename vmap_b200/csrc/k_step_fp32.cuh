@@ -524,13 +524,3 @@ __global__ void __launch_bounds__(128) k_step_fp32(StepParams a, VmbLayout L) {
     atomicAdd(G + L.o_B + tid, s);
   }
 }
-
-// host: raise kernel K's dynamic shared-memory limit to `bytes` on device `dev`, the first time only
-template <auto K>
-static cudaError_t smem_limit_once(int dev, int bytes) {
-  static bool set[64] = {};      // per device (one process may drive several GPUs)
-  if (set[dev & 63]) return cudaSuccess;
-  const cudaError_t e = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) set[dev & 63] = true;
-  return e;
-}

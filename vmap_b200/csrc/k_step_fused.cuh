@@ -1104,30 +1104,32 @@ static void fused_partition(int B, int tpo, int G, uf::Ranges& rg) {
 static int fused_launch_step(const VmbLayout& L, const StepParams& sp, const FusedExtra& fx, const void* image, int n_sm,
                              cudaStream_t st, std::string& err, float* jdt = nullptr, unsigned long long* trace = nullptr) {
   using namespace uf;
-  if (L.H != 32 || L.nfreq != 6) { err = "fused step kernel: hidden must be 32 and n_freq 6"; return -4; }
-  if (sp.S < 1 || sp.S > 32) { err = "fused step kernel: n_samples must be in [1, 32]"; return -4; }
-  if (!sp.fwd_only && sp.B > MAX_OBJ_SMEM) { err = "fused step kernel: too many objects for the in-kernel mask counts"; return -4; }
-  if (jdt && (sp.fwd_only || !sp.backward)) { err = "fused step kernel: the joint step needs the backward"; return -4; }
-  if (trace && (jdt || sp.fwd_only || !sp.backward || sp.S != 10)) {
-    err = "fused step kernel: the phase trace covers the training step at n_samples 10 only"; return -4;
+  if (L.H != 32 || L.nfreq != 6) { err = "fused step kernel: hidden must be 32 and n_freq 6"; return VMB_E_UNSUPPORTED; }
+  if (sp.S < 1 || sp.S > 32) { err = "fused step kernel: n_samples must be in [1, 32]"; return VMB_E_UNSUPPORTED; }
+  if (!sp.fwd_only && sp.B > MAX_OBJ_SMEM) {
+    err = "fused step kernel: too many objects for the in-kernel mask counts"; return VMB_E_UNSUPPORTED;
   }
-  static bool attr_set[64] = {};
+  if (jdt && (sp.fwd_only || !sp.backward)) { err = "fused step kernel: the joint step needs the backward"; return VMB_E_UNSUPPORTED; }
+  if (trace && (jdt || sp.fwd_only || !sp.backward || sp.S != 10)) {
+    err = "fused step kernel: the phase trace covers the training step at n_samples 10 only"; return VMB_E_UNSUPPORTED;
+  }
   int dev = 0;
   cudaGetDevice(&dev);
   const int smem_bytes = SM_CNT + (sp.fwd_only ? 0 : sp.B * 12) + SMEM_SLACK;
-  if (!attr_set[dev & 63]) {
+  {
     cudaError_t e = cudaSuccess;
-    for (auto k : {k_step_fused<0, false>, k_step_fused<10, false>, k_step_fused<14, false>,
-                   k_step_fused<0, true>, k_step_fused<10, true>, k_step_fused<14, true>, k_step_fused<10, false, true>})
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
-    if (e != cudaSuccess) { err = std::string("cudaFuncSetAttribute(k_step_fused): ") + cudaGetErrorString(e); return -2; }
-    attr_set[dev & 63] = true;
+    for (auto raise : {smem_limit_once<k_step_fused<0, false>>, smem_limit_once<k_step_fused<10, false>>,
+                       smem_limit_once<k_step_fused<14, false>>, smem_limit_once<k_step_fused<0, true>>,
+                       smem_limit_once<k_step_fused<10, true>>, smem_limit_once<k_step_fused<14, true>>,
+                       smem_limit_once<k_step_fused<10, false, true>>})
+      if (e == cudaSuccess) e = raise(dev, SMEM_MAX);
+    if (e != cudaSuccess) { err = std::string("cudaFuncSetAttribute(k_step_fused): ") + cudaGetErrorString(e); return VMB_E_CUDA; }
   }
   const int rpw = 32 / sp.S;                  // whole rays per warp: the sample axis never crosses a warp
   const int nr = 4 * rpw;
   const int tpo = (sp.R + nr - 1) / nr;       // tiles per object
   const long long T = (long long)tpo * sp.B;
-  if (T > 0x7fffffffLL) { err = "fused step kernel: too many tiles"; return -1; }
+  if (T > 0x7fffffffLL) { err = "fused step kernel: too many tiles"; return VMB_E_ARG; }
   long long grid = T;
   if (grid > n_sm) grid = n_sm;
   if (grid > MAX_CTAS) grid = MAX_CTAS;
@@ -1150,6 +1152,6 @@ static int fused_launch_step(const VmbLayout& L, const StepParams& sp, const Fus
   else if (jdt) e = kern(sp.S == 10 ? k_step_fused<10, true> : sp.S == 14 ? k_step_fused<14, true> : k_step_fused<0, true>);
   else     e = kern(sp.S == 10 ? k_step_fused<10, false> : sp.S == 14 ? k_step_fused<14, false> : k_step_fused<0, false>);
   if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) { err = std::string("k_step_fused launch: ") + cudaGetErrorString(e); return -2; }
+  if (e != cudaSuccess) { err = std::string("k_step_fused launch: ") + cudaGetErrorString(e); return VMB_E_CUDA; }
   return 0;
 }

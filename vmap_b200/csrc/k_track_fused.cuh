@@ -59,33 +59,13 @@ constexpr int DT_BYTES = 128 * 16;                    // warpgroup 1's half of d
 constexpr int SM_BAR = SM_DT + DT_BYTES, SMEM = SM_BAR + 16;
 constexpr float LS = um::LS, INV_LS = um::INV_LS;
 
-// per-ray pose terms and loss terms of the track flavour (k_tf_reduce's input): grow-only, never moved once a captured
-// graph holds them (TrackWorkspace's rule).  Sized for the handle's max_obj objects (not the B of the call: the tracked
-// set changes from frame to frame, and a frame that tracks more objects than the captured one must still run), so only
-// a larger n_rays than any call before a capture is refused.
+// per-ray pose terms and loss terms of the track flavour (k_tf_reduce's input), handle scratch (DeviceBuffer's rule).
+// Sized for the handle's max_obj objects (not the B of the call: the tracked set changes from frame to frame, and a
+// frame that tracks more objects than the captured one must still run), so only a larger n_rays than any call before a
+// capture is refused.
 struct Workspace {
-  double* gray = nullptr;      // [B][R][6]
-  double* lray = nullptr;      // [B][R][3]
-  long long cap_rays = 0;
-  bool in_graph = false;
-  void release() {
-    if (gray) cudaFree(gray);
-    if (lray) cudaFree(lray);
-    gray = lray = nullptr; cap_rays = 0; in_graph = false;
-  }
-  cudaError_t ensure(long long rays, cudaStream_t st) {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(st, &cs);
-    const bool capturing = cs != cudaStreamCaptureStatusNone;
-    if (rays <= cap_rays) { in_graph |= capturing; return cudaSuccess; }
-    if (capturing || in_graph) return cudaErrorStreamCaptureUnsupported;
-    release();
-    cudaError_t e = cudaMalloc((void**)&gray, (size_t)rays * 6 * sizeof(double));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&lray, (size_t)rays * 3 * sizeof(double));
-    if (e != cudaSuccess) { release(); return e; }
-    cap_rays = rays;
-    return cudaSuccess;
-  }
+  DeviceBuffer<double> gray;   // [B][R][6]
+  DeviceBuffer<double> lray;   // [B][R][3]
 };
 
 // The start of k_track_fused and k_reloc_fused once the object's image row is known to be valid: the weight image on
@@ -412,15 +392,20 @@ __global__ void __launch_bounds__(128) k_tf_reduce(int R, int nr10, int n_out, c
 template <bool BA>
 static int launch_track_fused(Workspace& ws, const VmbLayout& L, const TrackParams& tp, const BaRays& x, const void* image,
                               int nr10, int cap_obj, cudaStream_t st, std::string& err) {
-  if (L.H != 32 || L.nfreq != 6) { err = "fused tracking step: hidden must be 32 and n_freq 6"; return -4; }
-  if (tp.S < 1 || tp.S > 32) { err = "fused tracking step: n_samples must be in [1, 32]"; return -4; }
+  if (L.H != 32 || L.nfreq != 6) { err = "fused tracking step: hidden must be 32 and n_freq 6"; return VMB_E_UNSUPPORTED; }
+  if (tp.S < 1 || tp.S > 32) { err = "fused tracking step: n_samples must be in [1, 32]"; return VMB_E_UNSUPPORTED; }
   const int rpw = 32 / tp.S, nr = 4 * rpw;
   const int tiles = (tp.R + nr - 1) / nr;
   int dev = 0;
   cudaGetDevice(&dev);
   cudaError_t e = smem_limit_once<k_track_fused<BA>>(dev, SMEM);
-  if (e == cudaSuccess && !BA) e = ws.ensure((long long)std::max(cap_obj, tp.B) * tp.R, st);
-  if (e != cudaSuccess) { err = std::string("fused tracking step: ") + cudaGetErrorString(e); return -2; }
+  if (e == cudaSuccess && !BA) {
+    const size_t rays = (size_t)std::max(cap_obj, tp.B) * tp.R;
+    const bool capturing = stream_capturing(st);
+    e = ws.gray.grow(rays * 6 * sizeof(double), capturing);
+    if (e == cudaSuccess) e = ws.lray.grow(rays * 3 * sizeof(double), capturing);
+  }
+  if (e != cudaSuccess) { err = std::string("fused tracking step: ") + cudaGetErrorString(e); return VMB_E_CUDA; }
   k_track_fused<BA><<<dim3((unsigned)tiles, (unsigned)tp.B), NT, SMEM, st>>>(tp, x, (const unsigned char*)image, nr, rpw,
                                                                             ws.gray, ws.lray);
   if (!BA) {
@@ -429,7 +414,7 @@ static int launch_track_fused(Workspace& ws, const VmbLayout& L, const TrackPara
                                                                                       tp.partials);
   }
   e = cudaGetLastError();
-  if (e != cudaSuccess) { err = std::string("fused tracking step launch: ") + cudaGetErrorString(e); return -2; }
+  if (e != cudaSuccess) { err = std::string("fused tracking step launch: ") + cudaGetErrorString(e); return VMB_E_CUDA; }
   return 0;
 }
 

@@ -38,46 +38,14 @@
 
 namespace lw {
 
-// the path's own buffers next to the training step's: grow-only, never moved once a captured graph holds them
+// the path's own buffers next to the training step's (handle scratch, DeviceBuffer's rule)
 struct TrackWorkspace {
-  Workspace w;                 // E, X1..X4, XC, dYa..dYc, dalpha_s, dE (dh16 unused)
-  float* prow = nullptr;       // [stride] the object's fp32 param row
-  __half* wimg = nullptr;      // [img_halves] its fp16 image row
-  int* ctl = nullptr;          // [8]: mask counts nd, no, ns; row ok; scale (float bits)
-  double* lossr = nullptr;     // [R][3] per-ray loss terms
-  double* gpt = nullptr;       // [P][6] per-point pose terms
-  long long cap_rays = 0, cap_points = 0; int H = 0;
-  bool in_graph = false;
-  void release() {
-    void* ptrs[] = {prow, wimg, ctl, lossr, gpt};
-    for (void* q : ptrs) if (q) cudaFree(q);
-    prow = nullptr; wimg = nullptr; ctl = nullptr; lossr = nullptr; gpt = nullptr;
-    cap_rays = cap_points = 0; H = 0; in_graph = false;
-    w.release();
-    w.destroy_streams();
-  }
-  cudaError_t ensure(long long R, long long P, int H_, int stride, cudaStream_t st) {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(st, &cs);
-    const bool capturing = cs != cudaStreamCaptureStatusNone;
-    cudaError_t e = w.ensure(P, H_, st);
-    if (e != cudaSuccess) return e;
-    if (R <= cap_rays && P <= cap_points && H_ == H) { in_graph |= capturing; return cudaSuccess; }
-    if (capturing || in_graph) return cudaErrorStreamCaptureUnsupported;
-    void* ptrs[] = {prow, wimg, ctl, lossr, gpt};
-    for (void* q : ptrs) if (q) cudaFree(q);
-    prow = nullptr; wimg = nullptr; ctl = nullptr; lossr = nullptr; gpt = nullptr; cap_rays = cap_points = 0;
-    const long long Pp = (P + 127) / 128 * 128;
-    auto al = [&](void** q, size_t bytes) { if (e == cudaSuccess) e = cudaMalloc(q, bytes); };
-    al((void**)&prow, (size_t)stride * 4);
-    al((void**)&wimg, (size_t)img_halves(H_) * 2);
-    al((void**)&ctl, 8 * sizeof(int));
-    al((void**)&lossr, (size_t)R * 3 * sizeof(double));
-    al((void**)&gpt, (size_t)Pp * 6 * sizeof(double));
-    if (e != cudaSuccess) return e;
-    cap_rays = R; cap_points = Pp; H = H_;
-    return cudaSuccess;
-  }
+  Workspace w;                          // E, X1..X4, XC, dYa..dYc, dalpha_s, dE (dh16 unused)
+  DeviceBuffer<float> prow;             // [stride] the object's fp32 param row
+  DeviceBuffer<__half> wimg;            // [img_halves] its fp16 image row
+  DeviceBuffer<int> ctl;                // [8]: mask counts nd, no, ns; row ok; scale (float bits)
+  DeviceBuffer<double> lossr;           // [R][3] per-ray loss terms
+  DeviceBuffer<double> gpt;             // [P][6] per-point pose terms
 };
 
 // What the path reads for one object b of the group (TrackParams / BaRays of k_track.cuh carry the rest)
@@ -381,7 +349,7 @@ struct TlwGroup {
   int nr;                        // track flavour: rays per K10 tile
 };
 
-#define TLW_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return -2; } } while (0)
+#define TLW_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return VMB_E_CUDA; } } while (0)
 
 template <int H, bool BA>
 static int track_object_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGroup& G, int b, cudaStream_t st, std::string& err) {
@@ -400,20 +368,21 @@ static int track_object_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGrou
   const unsigned char* sem = a.sem + (size_t)b * a.sem_stride;
   const unsigned char* mask = a.mask + (size_t)b * a.mask_stride;
   const long long halves = img_halves(H);
-  TLW_TRY(launch_k(k_tlw_gather, dim3((unsigned)std::min<long long>(2 * sm_count(), (halves / 8 + 255) / 256)), dim3(256), 0, st, o,
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const int n_sm = sm_count(dev);
+  TLW_TRY(launch_k(k_tlw_gather, dim3((unsigned)std::min<long long>(2 * n_sm, (halves / 8 + 255) / 256)), dim3(256), 0, st, o,
                    a.params, a.scale, G.image, sem, mask, L.stride, halves, tw.prow, tw.wimg, tw.ctl));
   arm();
   TLW_TRY(launch_k(k_tlw_pe<BA>, dim3(nblk), dim3(128), 0, st, o, (const float*)tw.prow, (const int*)tw.ctl, L.o_B, ws.E));
   TLW_TRY(forward_gemms<H>(ws, L, tw.prow, tw.wimg, np, pdl_ok, st));
-  int dev = 0;
-  cudaGetDevice(&dev);
   TLW_TRY((smem_limit_once<k_tlw_render<H, BA>>(dev, hr_smem<H>())));
   TlwRender ra;
   ra.z = a.z + (size_t)b * a.z_stride; ra.gt_depth = a.gt_depth + (size_t)b * a.gt_depth_stride;
   ra.gt_colour = a.gt_colour + (size_t)b * a.gt_colour_stride; ra.sem = sem; ra.mask = mask; ra.cs = a.cs; ra.os = a.os;
   const int hr_per_sm = std::max(1, std::min(8, (int)(227 * 1024 / (hr_smem<H>() + 6 * 1024))));
   arm();
-  TLW_TRY(launch_k(k_tlw_render<H, BA>, dim3(std::min((a.R + 3) / 4, sm_count() * hr_per_sm)), dim3(128), (size_t)hr_smem<H>(), st,
+  TLW_TRY(launch_k(k_tlw_render<H, BA>, dim3(std::min((a.R + 3) / 4, n_sm * hr_per_sm)), dim3(128), (size_t)hr_smem<H>(), st,
                    o, ra, (const __half*)ws.X4, (const __half*)ws.XC, (const float*)tw.prow, L, (const int*)tw.ctl, ws.dYc,
                    ws.dalpha_s, tw.lossr));
   // backward to the embedding only, the input-gradient chain of step_object
@@ -444,15 +413,22 @@ static int track_object_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGrou
 
 template <bool BA>
 static int launch_track_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGroup& G, cudaStream_t st, std::string& err) {
-  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return -2; }
-  TLW_TRY(tw.ensure(G.tp.R, (long long)G.tp.R * G.tp.S, L.H, L.stride, st));
+  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return VMB_E_CUDA; }
+  const long long R = G.tp.R, P = R * G.tp.S;
+  const bool capturing = stream_capturing(st);
+  TLW_TRY(tw.w.grow(P, L.H, capturing));
+  TLW_TRY(tw.prow.grow((size_t)L.stride * 4, capturing));
+  TLW_TRY(tw.wimg.grow((size_t)img_halves(L.H) * 2, capturing));
+  TLW_TRY(tw.ctl.grow(8 * sizeof(int), capturing));
+  TLW_TRY(tw.lossr.grow((size_t)R * 3 * sizeof(double), capturing));
+  TLW_TRY(tw.gpt.grow((size_t)pad_points(P) * 6 * sizeof(double), capturing));
   for (int b = 0; b < G.tp.B; ++b) {
     int rc;
     switch (L.H) {
       case 64:  rc = track_object_lw<64, BA>(tw, L, G, b, st, err); break;
       case 128: rc = track_object_lw<128, BA>(tw, L, G, b, st, err); break;
       case 256: rc = track_object_lw<256, BA>(tw, L, G, b, st, err); break;
-      default: err = "layer-wise tracking: hidden must be 64, 128 or 256"; return -4;
+      default: err = "layer-wise tracking: hidden must be 64, 128 or 256"; return VMB_E_UNSUPPORTED;
     }
     if (rc) return rc;
   }
@@ -470,36 +446,11 @@ static int launch_track_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGrou
 //                  because the pose terms read the PE directions from the fp32 param row and must see them before the update.
 //   k_tlw_pose / k_tlw_reduce (BA flavour) on the training workspace's dE: one row per ray, loss columns 0.
 // ---------------------------------------------------------------------------------------------------------------------
-struct JointWorkspace {        // grow-only, never moved once a captured graph holds it (as TrackWorkspace)
-  float* pw = nullptr;         // [P][3] world points of the current object (fused step: of all B objects)
-  int* ctl = nullptr;          // [8] as TrackWorkspace::ctl (only row ok and scale are read)
-  double* gpt = nullptr;       // [P][6] per-point pose terms (layer-wise step)
-  float* jdt = nullptr;        // [P][2][3] the fused step's per-point dL/dt halves
-  long long cap_points = 0;
-  bool in_graph = false;
-  void release() {
-    void* ptrs[] = {pw, ctl, gpt, jdt};
-    for (void* q : ptrs) if (q) cudaFree(q);
-    pw = nullptr; ctl = nullptr; gpt = nullptr; jdt = nullptr; cap_points = 0; in_graph = false;
-  }
-  cudaError_t ensure(long long P, cudaStream_t st) {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(st, &cs);
-    const bool capturing = cs != cudaStreamCaptureStatusNone;
-    if (P <= cap_points) { in_graph |= capturing; return cudaSuccess; }
-    if (capturing || in_graph) return cudaErrorStreamCaptureUnsupported;
-    release();
-    const long long Pp = (P + 127) / 128 * 128;
-    cudaError_t e = cudaSuccess;
-    auto al = [&](void** q, size_t bytes) { if (e == cudaSuccess) e = cudaMalloc(q, bytes); };
-    al((void**)&pw, (size_t)Pp * 3 * sizeof(float));
-    al((void**)&ctl, 8 * sizeof(int));
-    al((void**)&gpt, (size_t)Pp * 6 * sizeof(double));
-    al((void**)&jdt, (size_t)Pp * 6 * sizeof(float));
-    if (e != cudaSuccess) { release(); return e; }
-    cap_points = Pp;
-    return cudaSuccess;
-  }
+struct JointWorkspace {        // handle scratch (DeviceBuffer's rule); each step grows the buffers it uses
+  DeviceBuffer<float> pw;      // [P][3] world points of the current object (fused step: of all B objects)
+  DeviceBuffer<int> ctl;       // [8] as TrackWorkspace::ctl (only row ok and scale are read; layer-wise step)
+  DeviceBuffer<double> gpt;    // [P][6] per-point pose terms (layer-wise step)
+  DeviceBuffer<float> jdt;     // [P][2][3] the fused step's per-point dL/dt halves
 };
 
 // object o.b + blockIdx.y of a batched launch (the fused joint step: all B objects in one grid; the layer-wise step
@@ -599,17 +550,20 @@ static int joint_object_lw(Workspace& ws, JointWorkspace& jw, const VmbLayout& L
 static int launch_joint_lw(Workspace& ws, JointWorkspace& jw, const VmbLayout& L, const StepParams& sp, const BaRays& x,
                            const double* poses, int* status, const void* image, float* pw_out, cudaStream_t st,
                            std::string& err) {
-  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return -2; }
-  const long long np = (long long)sp.R * sp.S;
-  TLW_TRY(ws.ensure(np, L.H, st));
-  TLW_TRY(jw.ensure(np, st));
+  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return VMB_E_CUDA; }
+  const long long np = (long long)sp.R * sp.S, Pp = pad_points(np);
+  const bool capturing = stream_capturing(st);
+  TLW_TRY(ws.grow(np, L.H, capturing));
+  TLW_TRY(jw.pw.grow((size_t)Pp * 3 * sizeof(float), capturing));
+  TLW_TRY(jw.ctl.grow(8 * sizeof(int), capturing));
+  TLW_TRY(jw.gpt.grow((size_t)Pp * 6 * sizeof(double), capturing));
   for (int b = 0; b < sp.B; ++b) {
     int rc;
     switch (L.H) {
       case 64:  rc = joint_object_lw<64>(ws, jw, L, sp, x, poses, status, (const __half*)image, b, pw_out, st, err); break;
       case 128: rc = joint_object_lw<128>(ws, jw, L, sp, x, poses, status, (const __half*)image, b, pw_out, st, err); break;
       case 256: rc = joint_object_lw<256>(ws, jw, L, sp, x, poses, status, (const __half*)image, b, pw_out, st, err); break;
-      default: err = "joint step: hidden must be 64, 128 or 256"; return -4;
+      default: err = "joint step: hidden must be 64, 128 or 256"; return VMB_E_UNSUPPORTED;
     }
     if (rc) return rc;
   }

@@ -32,17 +32,19 @@ struct vmb_handle {
   int device, max_obj, H, nfreq;
   int n_sm;
   VmbLayout L;
-  int* d_counts;          // [max_obj][4]
-  int* d_img_index;       // [P] param index -> half index inside the fp16 image (or -1)
-  unsigned int* d_ticket; // last-block ticket of the fused AdamW (device step counter mode)
-  unsigned int* d_smax;   // [max_obj] sampler: per-object max sampled depth (order-preserving key)
-  float* d_partials;      // fused step: [(max_obj + n_sm)][stride] per-(CTA, object) gradient partials (allocated on first use)
-  unsigned int* d_finish_sync; // fused step: finish sync words + per-object readiness counts and skip flags (uf::SY_*)
-  float2* d_bc;           // AdamW bias corrections per step number for (bc_b1, bc_b2), built on the host in double precision
-  double bc_b1, bc_b2;
-  int img_halves;
-  bool umma_ok;           // hidden 32: fused wgmma kernel + its pre-arranged fp16 image
-  bool lw_ok;             // hidden 64/128/256: layer-wise wgmma GEMM path + row-major fp16 image
+  // Scratch of the entry points: device buffers that grow on demand and never move once a captured graph holds them
+  // (DeviceBuffer), freed with the handle.
+  DeviceBuffer<int> d_counts;          // [max_obj][4]
+  DeviceBuffer<int> d_img_index;       // [P] param index -> half index inside the fp16 image (or -1)
+  DeviceBuffer<unsigned int> d_ticket; // last-block ticket of the fused AdamW (device step counter mode)
+  DeviceBuffer<unsigned int> d_smax;   // [max_obj] sampler: per-object max sampled depth (order-preserving key)
+  DeviceBuffer<float> d_partials;      // fused step: [(max_obj + n_sm)][stride] per-(CTA, object) gradient partials (allocated on first use)
+  DeviceBuffer<unsigned int> d_finish_sync; // fused step: finish sync words + per-object readiness counts and skip flags (uf::SY_*)
+  DeviceBuffer<float2> d_bc;           // AdamW bias corrections per step number for (bc_b1, bc_b2), built on the host in double precision
+  double bc_b1 = -1.0, bc_b2 = -1.0;
+  int img_halves = 0;
+  bool umma_ok = false;   // hidden 32: fused wgmma kernel + its pre-arranged fp16 image
+  bool lw_ok = false;     // hidden 64/128/256: layer-wise wgmma GEMM path + row-major fp16 image
   lw::Workspace ws;       // training-step activations (may be baked into a captured graph)
   lw::Workspace ws_fwd;   // forward-only queries (vmb_forward): separate, so eval_points never moves the step's buffers
   mesh::Workspace ws_mesh;// marching cubes / unprojection scratch (grow-only)
@@ -139,30 +141,28 @@ int vmb_create(vmb_handle** out, int device, int max_obj, int hidden, int n_freq
   CUDA_TRY(nullptr, cudaSetDevice(device));
   vmb_handle* h = new vmb_handle();
   h->device = device; h->max_obj = max_obj; h->H = hidden; h->nfreq = n_freq;
-  h->n_sm = 132;
-  cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, device);
+  h->n_sm = sm_count(device);
   h->L = vmb_make_layout(hidden, n_freq);
-  h->d_counts = nullptr; h->d_img_index = nullptr; h->d_ticket = nullptr; h->d_smax = nullptr; h->d_partials = nullptr; h->d_finish_sync = nullptr; h->d_bc = nullptr; h->bc_b1 = h->bc_b2 = -1.0; h->img_halves = 0; h->umma_ok = false; h->lw_ok = false;
-  cudaError_t e = cudaMalloc(&h->d_counts, sizeof(int) * 4 * max_obj);
-  if (e == cudaSuccess) e = cudaMalloc(&h->d_ticket, sizeof(unsigned int));
+  cudaError_t e = h->d_counts.grow(sizeof(int) * 4 * max_obj, false);
+  if (e == cudaSuccess) e = h->d_ticket.grow(sizeof(unsigned int), false);
   if (e == cudaSuccess) e = cudaMemset(h->d_ticket, 0, sizeof(unsigned int));
-  if (e == cudaSuccess) e = cudaMalloc(&h->d_smax, sizeof(unsigned int) * (size_t)max_obj);
+  if (e == cudaSuccess) e = h->d_smax.grow(sizeof(unsigned int) * (size_t)max_obj, false);
   if (e != cudaSuccess) { delete h; return fail(nullptr, VMB_E_NOMEM, cudaGetErrorString(e)); }
   if (hidden == 32 && n_freq == 6) {
     std::vector<int> idx(h->L.P);
     umma_fill_image_index(h->L, idx.data());
     h->img_halves = umma_image_bytes() / 2;
-    e = cudaMalloc(&h->d_img_index, sizeof(int) * h->L.P);
+    e = h->d_img_index.grow(sizeof(int) * h->L.P, false);
     if (e == cudaSuccess) e = cudaMemcpy(h->d_img_index, idx.data(), sizeof(int) * h->L.P, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { cudaFree(h->d_counts); delete h; return fail(nullptr, VMB_E_CUDA, cudaGetErrorString(e)); }
+    if (e != cudaSuccess) { delete h; return fail(nullptr, VMB_E_CUDA, cudaGetErrorString(e)); }
     h->umma_ok = true;
   } else if ((hidden == 64 || hidden == 128 || hidden == 256) && n_freq == 6) {
     std::vector<int> idx(h->L.P);
     lw::fill_image_index(h->L, idx.data());
     h->img_halves = (int)lw::img_halves(hidden);
-    e = cudaMalloc(&h->d_img_index, sizeof(int) * h->L.P);
+    e = h->d_img_index.grow(sizeof(int) * h->L.P, false);
     if (e == cudaSuccess) e = cudaMemcpy(h->d_img_index, idx.data(), sizeof(int) * h->L.P, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { cudaFree(h->d_counts); delete h; return fail(nullptr, VMB_E_CUDA, cudaGetErrorString(e)); }
+    if (e != cudaSuccess) { delete h; return fail(nullptr, VMB_E_CUDA, cudaGetErrorString(e)); }
     h->lw_ok = true;
   }
   *out = h;
@@ -172,25 +172,6 @@ int vmb_create(vmb_handle** out, int device, int max_obj, int hidden, int n_freq
 void vmb_destroy(vmb_handle* h) {
   if (!h) return;
   cudaSetDevice(h->device);
-  if (h->d_counts) cudaFree(h->d_counts);
-  if (h->d_img_index) cudaFree(h->d_img_index);
-  if (h->d_ticket) cudaFree(h->d_ticket);
-  if (h->d_smax) cudaFree(h->d_smax);
-  if (h->d_partials) cudaFree(h->d_partials);
-  if (h->d_finish_sync) cudaFree(h->d_finish_sync);
-  if (h->d_bc) cudaFree(h->d_bc);
-  h->ws.release(); h->ws.destroy_streams();
-  h->ws_fwd.release(); h->ws_fwd.destroy_streams();
-  h->ws_mesh.release();
-  h->ws_eval.release();
-  h->ws_assoc.release();
-  h->ws_hull.release();
-  h->ws_render.release();
-  h->ws_track.release();
-  h->ws_ba.release();
-  h->ws_joint.release();
-  h->ws_tf.release();
-  h->ws_reloc.release();
   delete h;
 }
 
@@ -220,19 +201,18 @@ static AdamScalars adam_scalars(float lr_f, float b1_f, float b2_f, float wd_f, 
   return q;
 }
 
-// scratch of the fused step kernel (gradient partial rows + finish sync words and skip flags): allocated on first use,
-// never while a stream capture is in progress (a captured graph bakes the pointers in)
+// scratch of the fused step kernel (gradient partial rows + finish sync words and skip flags): a fixed size, allocated
+// on the first use and kept from then on, so later steps make no runtime call for it
 static int fused_scratch(vmb_handle* h, cudaStream_t st) {
-  if (h->d_partials) return VMB_OK;
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  cudaStreamIsCapturing(st, &cs);
-  if (cs != cudaStreamCaptureStatusNone)
-    return fail(h, VMB_E_CUDA, "vmb_step: first fused step of a handle must run outside stream capture (scratch allocation)");
+  if (h->d_finish_sync) return VMB_OK;
+  const bool capturing = stream_capturing(st);
   const size_t rows = (size_t)fused_rows_needed(h->max_obj, h->n_sm);
-  cudaError_t e = cudaMalloc(&h->d_partials, rows * h->L.stride * sizeof(float));
   const size_t sync_bytes = sizeof(unsigned int) * (uf::SY_OBJ + 2 * (size_t)h->max_obj);
-  if (e == cudaSuccess) e = cudaMalloc(&h->d_finish_sync, sync_bytes);
+  cudaError_t e = h->d_partials.grow(rows * h->L.stride * sizeof(float), capturing);
+  if (e == cudaSuccess) e = h->d_finish_sync.grow(sync_bytes, capturing);
   if (e == cudaSuccess) e = cudaMemset(h->d_finish_sync, 0, sync_bytes);
+  if (e == cudaErrorStreamCaptureUnsupported)
+    return fail(h, VMB_E_CUDA, "vmb_step: first fused step of a handle must run outside stream capture (scratch allocation)");
   if (e != cudaSuccess) return fail(h, VMB_E_NOMEM, cudaGetErrorString(e));
   return VMB_OK;
 }
@@ -243,11 +223,9 @@ static int fused_scratch(vmb_handle* h, cudaStream_t st) {
 constexpr int BC_N = 20480;
 static int ensure_bc_table(vmb_handle* h, double b1, double b2, cudaStream_t st) {
   if (h->d_bc && h->bc_b1 == b1 && h->bc_b2 == b2) return VMB_OK;
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  cudaStreamIsCapturing(st, &cs);
-  if (cs != cudaStreamCaptureStatusNone)
+  if (stream_capturing(st))
     return fail(h, VMB_E_CUDA, "AdamW bias-correction table must be built outside stream capture (run one step eagerly first)");
-  if (!h->d_bc) CUDA_TRY(h, cudaMalloc(&h->d_bc, sizeof(float2) * BC_N));
+  CUDA_TRY(h, h->d_bc.grow(sizeof(float2) * BC_N, false));
   std::vector<float2> tab(BC_N);
   for (int t = 0; t < BC_N; ++t) {
     const double tt = t < 1 ? 1.0 : (double)t;
@@ -437,7 +415,7 @@ int vmb_step_trace(vmb_handle* h, const vmb_step_args* a, unsigned long long* tr
   if (rc1 != VMB_OK) return rc1;
   std::string err;
   const int rc = fused_launch_step(h->L, sp, fx, a->image, h->n_sm, st, err, nullptr, trace);
-  if (rc != VMB_OK) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, err);
+  if (rc != VMB_OK) return fail(h, rc, err);
   return VMB_OK;
 }
 
@@ -459,13 +437,13 @@ int vmb_forward(vmb_handle* h, const vmb_forward_args* a, void* stream) {
     FusedExtra fx;
     memset(&fx, 0, sizeof(fx));
     const int rc = fused_launch_step(h->L, sp, fx, a->image, h->n_sm, (cudaStream_t)stream, err);
-    if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, err);
+    if (rc != VMB_OK) return fail(h, rc, err);
     return VMB_OK;
   }
   if (a->image && h->lw_ok) {
     std::string err;
     const int rc = lw::launch_forward(h->ws_fwd, h->L, sp, a->image, (cudaStream_t)stream, err);
-    if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, err);
+    if (rc != VMB_OK) return fail(h, rc, err);
     return VMB_OK;
   }
   return dispatch_fp32(h, sp, (cudaStream_t)stream);
@@ -533,13 +511,9 @@ int vmb_sample(vmb_handle* h, const vmb_sample_args* a, void* stream) {
   CUDA_TRY(h, cudaMemsetAsync(h->d_smax, 0, sizeof(unsigned int) * a->n_obj, st));
   k_sample_gather<<<dim3(chunks, a->n_obj), 256, 0, st>>>(p, h->d_smax);
   const int smem_pts = 256 * (a->n_bins_cam2surface + a->n_bins) * 16;      // staged z + points of 256 rays
-  static bool attr_set[64] = {};
-  if (!attr_set[h->device & 63]) {
-    CUDA_TRY(h, cudaFuncSetAttribute(k_sample_points<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 256 * 32 * 16));
-    CUDA_TRY(h, cudaFuncSetAttribute(k_sample_points<1, 9>, cudaFuncAttributeMaxDynamicSharedMemorySize, 256 * 32 * 16));
-    CUDA_TRY(h, cudaFuncSetAttribute(k_sample_points<5, 9>, cudaFuncAttributeMaxDynamicSharedMemorySize, 256 * 32 * 16));
-    attr_set[h->device & 63] = true;
-  }
+  CUDA_TRY(h, (smem_limit_once<k_sample_points<0, 0>>(h->device, 256 * 32 * 16)));
+  CUDA_TRY(h, (smem_limit_once<k_sample_points<1, 9>>(h->device, 256 * 32 * 16)));
+  CUDA_TRY(h, (smem_limit_once<k_sample_points<5, 9>>(h->device, 256 * 32 * 16)));
   const dim3 grid2(chunks, a->n_obj);
   if (a->n_bins_cam2surface == 1 && a->n_bins == 9)      k_sample_points<1, 9><<<grid2, 256, smem_pts, st>>>(p, h->d_smax);   // objects
   else if (a->n_bins_cam2surface == 5 && a->n_bins == 9) k_sample_points<5, 9><<<grid2, 256, smem_pts, st>>>(p, h->d_smax);   // background
@@ -621,16 +595,17 @@ int vmb_mc_count(vmb_handle* h, const vmb_mc_args* a, void* stream) {
   if (!a->totals) return fail(h, VMB_E_ARG, "vmb_mc_count: totals is NULL");
   cudaStream_t st = (cudaStream_t)stream;
   mesh::Workspace& w = h->ws_mesh;
+  const bool capturing = stream_capturing(st);
   const size_t n1 = (size_t)q.n + 1;
-  CUDA_TRY(h, mesh::Workspace::grow((void**)&w.mc_bytes, &w.mc_cap, 2 * n1 * sizeof(int) + 2 * (size_t)q.n));
-  q.pt_scan = reinterpret_cast<int*>(w.mc_bytes);
+  CUDA_TRY(h, w.mc_bytes.grow(2 * n1 * sizeof(int) + 2 * (size_t)q.n, capturing));
+  q.pt_scan = reinterpret_cast<int*>(w.mc_bytes.get());
   q.cell_scan = q.pt_scan + n1;
   q.pt_mask = reinterpret_cast<unsigned char*>(q.cell_scan + n1);
   q.cell_case = q.pt_mask + q.n;
   mesh::k_mc_count<<<mesh::blocks_for((long long)n1), 256, 0, st>>>(q);
   CUDA_TRY(h, cudaGetLastError());
-  CUDA_TRY(h, w.scan(q.pt_scan, (long long)n1, st));
-  CUDA_TRY(h, w.scan(q.cell_scan, (long long)n1, st));
+  CUDA_TRY(h, w.scan(q.pt_scan, (long long)n1, capturing, st));
+  CUDA_TRY(h, w.scan(q.cell_scan, (long long)n1, capturing, st));
   mesh::k_mc_totals<<<1, 1, 0, st>>>(q.pt_scan, q.cell_scan, q.n, a->totals);
   CUDA_TRY(h, cudaGetLastError());
   w.last = q;
@@ -677,11 +652,12 @@ int vmb_unproject(vmb_handle* h, const vmb_unproject_args* a, void* stream) {
   q.out = a->points; q.max_points = a->points ? a->max_points : 0;
   mesh::Workspace& w = h->ws_mesh;
   cudaStream_t st = (cudaStream_t)stream;
-  CUDA_TRY(h, mesh::Workspace::grow((void**)&w.up_scan, &w.up_cap, (size_t)(q.n + 1) * sizeof(int)));
+  const bool capturing = stream_capturing(st);
+  CUDA_TRY(h, w.up_scan.grow((size_t)(q.n + 1) * sizeof(int), capturing));
   q.scan = w.up_scan;
   mesh::k_unproj_flag<<<mesh::blocks_for(q.n + 1), 256, 0, st>>>(q);
   CUDA_TRY(h, cudaGetLastError());
-  CUDA_TRY(h, w.scan(q.scan, q.n + 1, st));
+  CUDA_TRY(h, w.scan(q.scan, q.n + 1, capturing, st));
   CUDA_TRY(h, cudaMemcpyAsync(a->count, q.scan + q.n, sizeof(int), cudaMemcpyDeviceToDevice, st));
   if (q.max_points > 0 && q.n > 0) {
     mesh::k_unproj_emit<<<mesh::blocks_for(q.n), 256, 0, st>>>(q);
@@ -714,11 +690,12 @@ int vmb_clip_count(vmb_handle* h, const vmb_clip_args* a, void* stream) {
   if (!a->count) return fail(h, VMB_E_ARG, "vmb_clip_count: count is NULL");
   cudaStream_t st = (cudaStream_t)stream;
   eval3d::Workspace& w = h->ws_eval;
-  CUDA_TRY(h, eval3d::Workspace::grow((void**)&w.clip_scan, &w.clip_cap, (size_t)(q.nf + 1) * sizeof(int)));
+  const bool capturing = stream_capturing(st);
+  CUDA_TRY(h, w.clip_scan.grow((size_t)(q.nf + 1) * sizeof(int), capturing));
   q.scan = w.clip_scan;
   eval3d::k_clip_count<<<eval3d::blocks_for(q.nf + 1, 128), 128, 0, st>>>(q);
   CUDA_TRY(h, cudaGetLastError());
-  CUDA_TRY(h, w.exclusive_sum(q.scan, q.nf + 1, st));
+  CUDA_TRY(h, w.exclusive_sum(q.scan, q.nf + 1, capturing, st));
   CUDA_TRY(h, cudaMemcpyAsync(a->count, q.scan + q.nf, sizeof(int), cudaMemcpyDeviceToDevice, st));
   w.last = q;
   w.counted = true;
@@ -754,13 +731,14 @@ int vmb_surface_sample(vmb_handle* h, const vmb_surface_sample_args* a, void* st
   q.n = a->n_points; q.seed = a->seed; q.uniforms = a->uniforms; q.points = a->points; q.face_index = a->face_index;
   cudaStream_t st = (cudaStream_t)stream;
   eval3d::Workspace& w = h->ws_eval;
-  CUDA_TRY(h, eval3d::Workspace::grow((void**)&w.cum, &w.cum_cap, (size_t)q.nf * sizeof(double) + sizeof(double)));
+  const bool capturing = stream_capturing(st);
+  CUDA_TRY(h, w.cum.grow((size_t)q.nf * sizeof(double) + sizeof(double), capturing));
   q.cum = w.cum;
   q.bad = reinterpret_cast<int*>(w.cum + q.nf);
   CUDA_TRY(h, cudaMemsetAsync(q.bad, 0, sizeof(int), st));
   eval3d::k_face_area<<<eval3d::blocks_for(q.nf, 256), 256, 0, st>>>(q);
   CUDA_TRY(h, cudaGetLastError());
-  CUDA_TRY(h, w.inclusive_sum(q.cum, q.nf, st));
+  CUDA_TRY(h, w.inclusive_sum(q.cum, q.nf, capturing, st));
   double total = 0.0;
   int bad = 0;
   CUDA_TRY(h, cudaMemcpyAsync(&total, q.cum + q.nf - 1, sizeof(double), cudaMemcpyDeviceToHost, st));
@@ -792,8 +770,9 @@ int vmb_nn_dist(vmb_handle* h, const vmb_nn_args* a, void* stream) {
   const size_t need = off_sorted + (size_t)q.n_ref * sizeof(float4);
   eval3d::Workspace& w = h->ws_eval;
   cudaStream_t st = (cudaStream_t)stream;
-  CUDA_TRY(h, eval3d::Workspace::grow((void**)&w.nn, &w.nn_cap, need));
-  q.keys = reinterpret_cast<unsigned int*>(w.nn);
+  const bool capturing = stream_capturing(st);
+  CUDA_TRY(h, w.nn.grow(need, capturing));
+  q.keys = reinterpret_cast<unsigned int*>(w.nn.get());
   q.grid = reinterpret_cast<eval3d::Grid*>(w.nn + off_grid);
   q.cell_start = reinterpret_cast<int*>(w.nn + off_cells);
   q.pt_cell = reinterpret_cast<int*>(w.nn + off_cell_pt);
@@ -806,7 +785,7 @@ int vmb_nn_dist(vmb_handle* h, const vmb_nn_args* a, void* stream) {
   eval3d::k_nn_grid<<<1, 1, 0, st>>>(q);
   eval3d::k_nn_count<<<eval3d::blocks_for(q.n_ref, 256), 256, 0, st>>>(q);
   CUDA_TRY(h, cudaGetLastError());
-  CUDA_TRY(h, w.exclusive_sum(q.cell_start, q.max_cells + 1, st));
+  CUDA_TRY(h, w.exclusive_sum(q.cell_start, q.max_cells + 1, capturing, st));
   eval3d::k_nn_scatter<<<eval3d::blocks_for(q.n_ref, 256), 256, 0, st>>>(q);
   eval3d::k_nn_query<<<eval3d::blocks_for(q.n_q, 128), 128, 0, st>>>(q);
   CUDA_TRY(h, cudaGetLastError());
@@ -814,7 +793,7 @@ int vmb_nn_dist(vmb_handle* h, const vmb_nn_args* a, void* stream) {
 }
 
 // ---- K7: ScanNet instance association (classify -> voxel -> finalize) ------------------------------
-static int assoc_params(vmb_handle* h, const vmb_assoc_args* a, assoc::Params& q, const char* who) {
+static int assoc_params(vmb_handle* h, const vmb_assoc_args* a, assoc::Params& q, bool capturing, const char* who) {
   if (!h || !a || a->width <= 0 || a->height <= 0 || !a->inst || !a->depth || !a->stats || !a->boxes)
     return fail(h, VMB_E_ARG, std::string(who) + ": bad arguments");
   if (a->max_id < 1 || a->max_id > 65536) return fail(h, VMB_E_ARG, std::string(who) + ": max_id must be in [1, 65536]");
@@ -835,24 +814,24 @@ static int assoc_params(vmb_handle* h, const vmb_assoc_args* a, assoc::Params& q
   q.boxes = a->boxes; q.pool = a->pool; q.cloud_off = a->cloud_off; q.cloud_cnt = a->cloud_cnt;
   q.stats = a->stats;
   q.bound = a->n_pool + q.n;
-  // scratch carving (grow-only; pixel, id and element regions)
+  // scratch carving (pixel, id and element regions)
   assoc::Workspace& w = h->ws_assoc;
   const size_t n = (size_t)q.n, ni = (size_t)q.max_id + 1, nb = (size_t)q.bound;
   const size_t o_row = assoc::align16(n), o_k = o_row + assoc::align16(n), o_ko = o_k + 4 * n, o_v = o_ko + 4 * n,
                o_vo = o_v + 4 * n, pix_need = o_vo + 4 * n;
-  CUDA_TRY(h, assoc::Workspace::grow((void**)&w.pix, &w.pix_cap, pix_need));
+  CUDA_TRY(h, w.pix.grow(pix_need, capturing));
   q.flags = w.pix; q.rowok = w.pix + o_row;
   q.sel_key = (int*)(w.pix + o_k); q.sel_key_out = (int*)(w.pix + o_ko);
   q.sel_val = (int*)(w.pix + o_v); q.sel_val_out = (int*)(w.pix + o_vo);
   const size_t i_seg = assoc::align16(4 * ni), i_min = i_seg + assoc::align16(4 * ni), i_st = i_min + 24 * ni,
                i_ext = i_st + 16, ids_need = i_ext + 20 * ni;
-  CUDA_TRY(h, assoc::Workspace::grow((void**)&w.ids, &w.ids_cap, ids_need));
-  q.new_off = (int*)w.ids; q.seg_off = (int*)(w.ids + i_seg);
+  CUDA_TRY(h, w.ids.grow(ids_need, capturing));
+  q.new_off = (int*)w.ids.get(); q.seg_off = (int*)(w.ids + i_seg);
   q.minb = (unsigned long long*)(w.ids + i_min); q.status = (int*)(w.ids + i_st);
   const size_t e_k = 24 * nb, e_ko = e_k + 8 * nb, e_i = e_ko + 8 * nb, e_io = e_i + 4 * nb,
                e_h = e_io + assoc::align16(4 * nb), el_need = e_h + 4 * (nb + 1);
-  CUDA_TRY(h, assoc::Workspace::grow((void**)&w.el, &w.el_cap, el_need));
-  q.elem = (double*)w.el; q.ekey = (unsigned long long*)(w.el + e_k); q.ekey_out = (unsigned long long*)(w.el + e_ko);
+  CUDA_TRY(h, w.el.grow(el_need, capturing));
+  q.elem = (double*)w.el.get(); q.ekey = (unsigned long long*)(w.el + e_k); q.ekey_out = (unsigned long long*)(w.el + e_ko);
   q.eidx = (int*)(w.el + e_i); q.eidx_out = (int*)(w.el + e_io); q.head = (int*)(w.el + e_h);
   return VMB_OK;
 }
@@ -863,10 +842,11 @@ static bool assoc_same(const assoc::Params& a, const assoc::Params& b) {
 }
 
 int vmb_assoc_classify(vmb_handle* h, const vmb_assoc_args* a, void* stream) {
-  assoc::Params q;
-  const int rc = assoc_params(h, a, q, "vmb_assoc_classify");
-  if (rc != VMB_OK) return rc;
   cudaStream_t st = (cudaStream_t)stream;
+  const bool capturing = stream_capturing(st);
+  assoc::Params q;
+  const int rc = assoc_params(h, a, q, capturing, "vmb_assoc_classify");
+  if (rc != VMB_OK) return rc;
   const unsigned gi = assoc::grid_for(q.max_id + 1, 256, 1 << 20), gp = assoc::grid_for(q.n, 256, 8 * h->n_sm);
   assoc::k_init<<<gi, 256, 0, st>>>(q);
   assoc::k_stats<<<gp, 256, 0, st>>>(q);
@@ -881,7 +861,7 @@ int vmb_assoc_classify(vmb_handle* h, const vmb_assoc_args* a, void* stream) {
   size_t need = 0;
   CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(nullptr, need, q.sel_key, q.sel_key_out, q.sel_val, q.sel_val_out,
                                               (int)q.n, 0, end_bit, st));
-  CUDA_TRY(h, w.tmp(need));
+  CUDA_TRY(h, w.cub_tmp.grow(need, capturing));
   CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(w.cub_tmp, need, q.sel_key, q.sel_key_out, q.sel_val, q.sel_val_out,
                                               (int)q.n, 0, end_bit, st));
   w.last = q;
@@ -890,21 +870,22 @@ int vmb_assoc_classify(vmb_handle* h, const vmb_assoc_args* a, void* stream) {
 }
 
 int vmb_assoc_voxel(vmb_handle* h, const vmb_assoc_args* a, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool capturing = stream_capturing(st);
   assoc::Params q;
-  const int rc = assoc_params(h, a, q, "vmb_assoc_voxel");
+  const int rc = assoc_params(h, a, q, capturing, "vmb_assoc_voxel");
   if (rc != VMB_OK) return rc;
   assoc::Workspace& w = h->ws_assoc;
   if (!w.classified || !assoc_same(w.last, q))
     return fail(h, VMB_E_ARG, "vmb_assoc_voxel: no matching vmb_assoc_classify on this handle");
   if (!a->cloud_out || a->max_cloud_out < q.bound)
     return fail(h, VMB_E_ARG, "vmb_assoc_voxel: cloud_out must hold n_pool + width * height points");
-  cudaStream_t st = (cudaStream_t)stream;
   const unsigned gi = assoc::grid_for(q.max_id + 1, 256, 1 << 20), ge = assoc::grid_for(q.bound, 256, 8 * h->n_sm);
   assoc::k_seg_len<<<gi, 256, 0, st>>>(q);
   CUDA_TRY(h, cudaGetLastError());
   size_t need = 0;
   CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(nullptr, need, q.seg_off, q.max_id + 1, st));
-  CUDA_TRY(h, w.tmp(need));
+  CUDA_TRY(h, w.cub_tmp.grow(need, capturing));
   CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(w.cub_tmp, need, q.seg_off, q.max_id + 1, st));
   CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(w.cub_tmp, need, q.new_off, q.max_id + 1, st));
   assoc::k_elements<<<ge, 256, 0, st>>>(q);
@@ -912,13 +893,13 @@ int vmb_assoc_voxel(vmb_handle* h, const vmb_assoc_args* a, void* stream) {
   CUDA_TRY(h, cudaGetLastError());
   need = 0;
   CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(nullptr, need, q.ekey, q.ekey_out, q.eidx, q.eidx_out, (int)q.bound, 0, 64, st));
-  CUDA_TRY(h, w.tmp(need));
+  CUDA_TRY(h, w.cub_tmp.grow(need, capturing));
   CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(w.cub_tmp, need, q.ekey, q.ekey_out, q.eidx, q.eidx_out, (int)q.bound, 0, 64, st));
   assoc::k_heads<<<ge, 256, 0, st>>>(q);
   CUDA_TRY(h, cudaGetLastError());
   need = 0;
   CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(nullptr, need, q.head, (int)(q.bound + 1), st));
-  CUDA_TRY(h, w.tmp(need));
+  CUDA_TRY(h, w.cub_tmp.grow(need, capturing));
   CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(w.cub_tmp, need, q.head, (int)(q.bound + 1), st));
   assoc::k_voxel_mean<<<ge, 256, 0, st>>>(q, a->cloud_out);
   CUDA_TRY(h, cudaGetLastError());
@@ -930,8 +911,10 @@ int vmb_assoc_voxel(vmb_handle* h, const vmb_assoc_args* a, void* stream) {
 }
 
 int vmb_assoc_finalize(vmb_handle* h, const vmb_assoc_args* a, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool capturing = stream_capturing(st);
   assoc::Params q;
-  const int rc = assoc_params(h, a, q, "vmb_assoc_finalize");
+  const int rc = assoc_params(h, a, q, capturing, "vmb_assoc_finalize");
   if (rc != VMB_OK) return rc;
   assoc::Workspace& w = h->ws_assoc;
   if (!w.classified || !assoc_same(w.last, q))
@@ -942,8 +925,7 @@ int vmb_assoc_finalize(vmb_handle* h, const vmb_assoc_args* a, void* stream) {
   f.W = q.W; f.H = q.H; f.max_id = q.max_id; f.n = q.n;
   f.inst = q.inst; f.depth = q.depth; f.stats = q.stats; f.flags = q.flags; f.final_label = a->final_label;
   f.labels = a->labels; f.bbox = a->bbox; f.half_scale = q.half_scale;
-  f.ext = (int*)(w.ids + ((size_t)((char*)q.status - (char*)w.ids) + 16));
-  cudaStream_t st = (cudaStream_t)stream;
+  f.ext = (int*)(w.ids + ((size_t)((unsigned char*)q.status - w.ids) + 16));
   const unsigned gi = assoc::grid_for(q.max_id + 1, 256, 1 << 20), gp = assoc::grid_for(q.n, 256, 8 * h->n_sm);
   assoc::k_fin_init<<<gi, 256, 0, st>>>(f);
   assoc::k_fin_label<<<gp, 256, 0, st>>>(f);
@@ -981,7 +963,9 @@ int vmb_hull(vmb_handle* h, const vmb_hull_args* a, void* stream) {
                fi = align256(4 * (size_t)fcap);
   const size_t need = 11 * si + 256 + 2 * pb + 4 * pi + 12 * fi;
   Workspace& w = h->ws_hull;
-  CUDA_TRY(h, Workspace::grow((void**)&w.buf, &w.cap, need));
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool capturing = stream_capturing(st);
+  CUDA_TRY(h, w.buf.grow(need, capturing));
   unsigned char* c = w.buf;
   auto take = [&](size_t bytes) { unsigned char* r = c; c += bytes; return r; };
   q.size = (int*)take(si); q.start = (int*)take(si);
@@ -995,15 +979,14 @@ int vmb_hull(vmb_handle* h, const vmb_hull_args* a, void* stream) {
   q.start_at = (int*)take(pi); q.end_at = (int*)take(pi);
   q.fv = (int*)take(3 * fi); q.fn = (int*)take(3 * fi); q.fs = (int*)take(fi); q.vis = (int*)take(fi);
   q.fre = (int*)take(fi); q.hz = (int*)take(3 * fi);
-  cudaStream_t st = (cudaStream_t)stream;
   const int ni = (int)std::max<long long>(n, 1);
   size_t t1 = 0, t2 = 0, t3 = 0;
   CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(nullptr, t1, q.size, q.start, ns + 1, st));
   CUDA_TRY(h, cub::DeviceSelect::Flagged(nullptr, t2, q.list[0], q.keep, q.list[1], q.n_sel, ni, st));
   CUDA_TRY(h, cub::DeviceSelect::Flagged(nullptr, t3, thrust::counting_iterator<int>(0), q.is_vertex, q.list[1],
                                          q.n_sel, ni, st));
-  CUDA_TRY(h, Workspace::grow(&w.cub_tmp, &w.cub_cap, std::max(t1, std::max(t2, t3))));
-  size_t tb = w.cub_cap;
+  CUDA_TRY(h, w.cub_tmp.grow(std::max(t1, std::max(t2, t3)), capturing));
+  size_t tb = w.cub_tmp.bytes();
   const unsigned gs = grid_of(ns + 1, 256, 4096), gn = grid_of(n, 256, 8 * (long long)h->n_sm);
   k_sizes<<<gs, 256, 0, st>>>(q, q.cnt[0]);
   CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(w.cub_tmp, tb, q.size, q.start, ns + 1, st));
@@ -1047,13 +1030,13 @@ int vmb_obb_minvol(vmb_handle* h, const vmb_obb_args* a, void* stream) {
     return fail(h, VMB_E_ARG, "vmb_obb_minvol: bad arguments");
   const long long cap = std::max<long long>(a->max_facets, 1);
   Workspace& w = h->ws_hull;
-  CUDA_TRY(h, Workspace::grow((void**)&w.obb, &w.obb_cap, 15 * sizeof(double) * (size_t)cap));
+  cudaStream_t st = (cudaStream_t)stream;
+  CUDA_TRY(h, w.obb.grow(15 * sizeof(double) * (size_t)cap, stream_capturing(st)));
   ObbParams q;
   q.pts = a->points; q.facets = a->facets; q.facet_nbr = a->facet_nbr; q.facet_count = a->facet_count;
   q.vertices = a->vertices; q.vertex_count = a->vertex_count; q.status = a->status;
   q.box = a->box; q.box_status = a->box_status;
   q.nr = w.obb; q.nu = w.obb + 3 * cap; q.res = w.obb + 6 * cap;
-  cudaStream_t st = (cudaStream_t)stream;
   k_obb_normals<<<grid_of(cap, 256, 8 * (long long)h->n_sm), 256, 0, st>>>(q);
   k_obb_eval<<<grid_of(cap, 1, 8 * (long long)h->n_sm), NT, 0, st>>>(q);
   k_obb_pick<<<1, NT, 0, st>>>(q);
@@ -1069,7 +1052,7 @@ static bool finite_all(const double* v, int n) {
 }
 
 // checks shared by the three render entry points; fills the geometry part of q and uploads the source table
-static int render_params(vmb_handle* h, const vmb_render_args* a, render::Params& q, const char* who) {
+static int render_params(vmb_handle* h, const vmb_render_args* a, render::Params& q, bool capturing, const char* who) {
   const std::string w(who);
   if (!h || !a) return fail(h, VMB_E_ARG, w + ": null argument");
   if (a->width <= 0 || a->height <= 0) return fail(h, VMB_E_ARG, w + ": width and height must be >= 1");
@@ -1109,8 +1092,8 @@ static int render_params(vmb_handle* h, const vmb_render_args* a, render::Params
   q.hit_src = a->hit_src; q.hit_t = a->hit_t; q.hit_count = a->hit_count;
   q.overflow = a->overflow; q.src_total = a->src_total; q.zstar = a->zstar; q.surf = a->surf;
   render::Workspace& ws = h->ws_render;
-  CUDA_TRY(h, render::Workspace::grow((void**)&ws.boxes, &ws.boxes_cap, (size_t)a->n_src * VMB_RENDER_BOX * sizeof(double)));
-  CUDA_TRY(h, render::Workspace::grow((void**)&ws.obj_id, &ws.id_cap, (size_t)a->n_src * sizeof(int)));
+  CUDA_TRY(h, ws.boxes.grow((size_t)a->n_src * VMB_RENDER_BOX * sizeof(double), capturing));
+  CUDA_TRY(h, ws.obj_id.grow((size_t)a->n_src * sizeof(int), capturing));
   q.boxes = ws.boxes; q.obj_id = ws.obj_id;
   return VMB_OK;
 }
@@ -1131,17 +1114,18 @@ static bool render_same(const render::Params& x, const render::Params& y) {
 }
 
 int vmb_render_count(vmb_handle* h, const vmb_render_args* a, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool capturing = stream_capturing(st);
   render::Params q;
-  int rc = render_params(h, a, q, "vmb_render_count");
+  int rc = render_params(h, a, q, capturing, "vmb_render_count");
   if (rc != VMB_OK) return rc;
   if (!a->overflow || !a->src_total) return fail(h, VMB_E_ARG, "vmb_render_count: overflow / src_total missing");
   if (a->pass == 1 && !a->zstar) return fail(h, VMB_E_ARG, "vmb_render_count: pass 1 needs zstar");
-  cudaStream_t st = (cudaStream_t)stream;
   if ((rc = render_upload(h, a, st)) != VMB_OK) return rc;
   render::Workspace& ws = h->ws_render;
   const long long n_e = (long long)q.n_rays * VMB_RENDER_MAX_HITS;
   const size_t n1 = (size_t)n_e + 1;
-  CUDA_TRY(h, render::Workspace::grow((void**)&ws.ints, &ws.ints_cap, 7 * n1 * sizeof(int)));
+  CUDA_TRY(h, ws.ints.grow(7 * n1 * sizeof(int), capturing));
   q.keys = ws.ints; q.keys_alt = q.keys + n1; q.vals = q.keys_alt + n1; q.vals_alt = q.vals + n1;
   q.cnt = q.vals_alt + n1;
   int* scan = q.cnt + n1;
@@ -1158,7 +1142,7 @@ int vmb_render_count(vmb_handle* h, const vmb_render_args* a, void* stream) {
   size_t need = 0, need_scan = 0;
   CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(nullptr, need, q.keys, q.keys_alt, q.vals, q.vals_alt, (int)n_e, 0, 11, st));
   CUDA_TRY(h, cub::DeviceScan::ExclusiveSum(nullptr, need_scan, scan, (int)n1, st));
-  CUDA_TRY(h, render::Workspace::grow(&ws.cub_tmp, &ws.cub_cap, std::max(need, need_scan)));
+  CUDA_TRY(h, ws.cub_tmp.grow(std::max(need, need_scan), capturing));
   CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(ws.cub_tmp, need, q.keys, q.keys_alt, q.vals, q.vals_alt, (int)n_e, 0, 11, st));
   render::k_gather_counts<<<render::blocks_for(n_e + 1, 256), 256, 0, st>>>(q, q.vals_alt, q.cnt, scan);
   CUDA_TRY(h, cudaGetLastError());
@@ -1172,7 +1156,7 @@ int vmb_render_count(vmb_handle* h, const vmb_render_args* a, void* stream) {
 
 int vmb_render_emit(vmb_handle* h, const vmb_render_args* a, void* stream) {
   render::Params q;
-  const int rc = render_params(h, a, q, "vmb_render_emit");
+  const int rc = render_params(h, a, q, stream_capturing((cudaStream_t)stream), "vmb_render_emit");
   if (rc != VMB_OK) return rc;
   render::Workspace& ws = h->ws_render;
   if (!ws.counted || !render_same(q, ws.last))
@@ -1187,8 +1171,9 @@ int vmb_render_emit(vmb_handle* h, const vmb_render_args* a, void* stream) {
 }
 
 int vmb_render_composite(vmb_handle* h, const vmb_render_args* a, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   render::Params q;
-  int rc = render_params(h, a, q, "vmb_render_composite");
+  int rc = render_params(h, a, q, stream_capturing(st), "vmb_render_composite");
   if (rc != VMB_OK) return rc;
   const bool images = a->pass == 1 || a->n_fine == 0;
   if (!a->z_coarse || !a->alpha_coarse || !a->colour_coarse || !a->base_coarse)
@@ -1198,7 +1183,6 @@ int vmb_render_composite(vmb_handle* h, const vmb_render_args* a, void* stream) 
   if (!a->zstar || (a->pass == 0 && !a->surf)) return fail(h, VMB_E_ARG, "vmb_render_composite: zstar / surf missing");
   if (images && (!a->depth || !a->colour || !a->opacity || !a->instance))
     return fail(h, VMB_E_ARG, "vmb_render_composite: output images missing");
-  cudaStream_t st = (cudaStream_t)stream;
   if ((rc = render_upload(h, a, st)) != VMB_OK) return rc;
   q.z_c = a->z_coarse; q.alpha_c = a->alpha_coarse; q.colour_c = a->colour_coarse; q.base_c = a->base_coarse;
   q.z_f = a->z_fine; q.alpha_f = a->alpha_fine; q.colour_f = a->colour_fine; q.base_f = a->base_fine;
@@ -1357,13 +1341,13 @@ static int pose_step(vmb_handle* h, const Args* a, int group, const void* image,
     std::string err;
     const int rc = tf::launch_track_fused<BA>(h->ws_tf, h->L, tp, x, image, fp32_tile(32) / g.n_samples, h->max_obj,
                                               st, err);
-    if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, std::string(who) + ": " + err);
+    if (rc != VMB_OK) return fail(h, rc, std::string(who) + ": " + err);
     return VMB_OK;
   } else if constexpr (PATH == POSE_LW) {
     const lw::TlwGroup G{tp, x, (const __half*)image, BA ? 1 : fp32_tile(g.hidden) / g.n_samples};
     std::string err;
     const int rc = lw::launch_track_lw<BA>(BA ? h->ws_ba : h->ws_track, h->L, G, st, err);
-    if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, std::string(who) + ": " + err);
+    if (rc != VMB_OK) return fail(h, rc, std::string(who) + ": " + err);
     return VMB_OK;
   } else {
     switch (h->H) {
@@ -1439,7 +1423,7 @@ int vmb_reloc_score(vmb_handle* h, const vmb_track_args* a, int group, int n_hyp
   std::string err;
   const int rc = rl::launch_reloc_fused(h->ws_reloc, h->L, tp, image, hyps, n_hyp, scores, terms,
                                         fp32_tile(32) / g.n_samples, h->n_sm, (cudaStream_t)stream, err);
-  if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, std::string(who) + ": " + err);
+  if (rc != VMB_OK) return fail(h, rc, std::string(who) + ": " + err);
   return VMB_OK;
 }
 
@@ -1547,7 +1531,7 @@ int vmb_joint_step_lw(vmb_handle* h, const vmb_step_args* s, const vmb_ba_args* 
   if (rcc != VMB_OK) return rcc;
   std::string err;
   const int rc = lw::launch_joint_lw(h->ws, h->ws_joint, h->L, sp, x, a->poses, a->status, s->image, pcs_world_out, st, err);
-  if (rc) return fail(h, rc == -4 ? VMB_E_UNSUPPORTED : VMB_E_CUDA, std::string(who) + ": " + err);
+  if (rc != VMB_OK) return fail(h, rc, std::string(who) + ": " + err);
   if (s->loss_sum) { k_loss_sum<<<1, 32, 0, st>>>(s->loss_terms, s->n_obj, s->loss_sum); CUDA_TRY(h, cudaGetLastError()); }
   return VMB_OK;
 }
@@ -1568,7 +1552,10 @@ int vmb_joint_step_fused(vmb_handle* h, const vmb_step_args* s, const vmb_ba_arg
   if (rc1 != VMB_OK) return rc1;
   cudaStream_t st = (cudaStream_t)stream;
   const long long np = (long long)s->n_rays * s->n_samples;
-  CUDA_TRY(h, h->ws_joint.ensure(np * s->n_obj, st));
+  const size_t Pp = (size_t)lw::pad_points(np * s->n_obj);
+  const bool capturing = stream_capturing(st);
+  CUDA_TRY(h, h->ws_joint.pw.grow(Pp * 3 * sizeof(float), capturing));
+  CUDA_TRY(h, h->ws_joint.jdt.grow(Pp * 6 * sizeof(float), capturing));
   lw::TlwObj o;
   memset(&o, 0, sizeof(o));
   o.R = s->n_rays; o.S = s->n_samples; o.n_rows = s->n_obj; o.pcs = s->pcs; o.pose = a->poses; o.status = a->status;
