@@ -45,7 +45,9 @@ def evaluate(params: Dict[str, torch.Tensor], scale, batch: Dict[str, torch.Tens
 
     Returns a dict of fp64 tensors: ``rows`` [B,R,6] each ray's pose terms ((R q) x g, g) summed over its samples,
     ``ray_terms`` [B,R,3] each ray's (L_d, L_c, L_o) share, ``terms`` [B,4] per-object loss terms and weighted total,
-    ``grad`` [F,6] the per-pose tangent gradient, ``loss`` the scalar loss, ``var`` [B,R] the rendered variance."""
+    ``grad`` [F,6] the per-pose tangent gradient, ``loss`` the scalar loss, ``var`` [B,R] the rendered variance,
+    and before the fp16 clamp: ``dyc_pre`` [B,P,H] the gated, loss-scaled dYc and ``rank1`` [B,P,H] dY4's loss-scaled
+    d_alpha w_a term (the values the kernel counts into status[1])."""
     f64 = dict(dtype=torch.float64)
     rnd = rounding
     p = {k: v.to(**f64) for k, v in params.items()}
@@ -123,12 +125,14 @@ def evaluate(params: Dict[str, torch.Tensor], scale, batch: Dict[str, torch.Tens
     docc = Gs * Tr - suffix / om
     dh_a = (10.0 * docc * oc * fr).reshape(B, P)
     dh_c = (gC[..., None, :] * w[..., None] * col * (1.0 - col)).reshape(B, P, 3)
-    dYc = _half((XC > 0) * mm(LS * dh_c, W_oc), rnd.dyc, DH_CLAMP)
+    dyc_pre = (XC > 0) * mm(LS * dh_c, W_oc)                                            # before the +-60000 clamp
+    dYc = _half(dyc_pre, rnd.dyc, DH_CLAMP)
 
     # ---- backward to the embedding only ----
     def gate(acc, x_prev):
         return _half(acc, rnd.dgrad) * (x_prev > 0)
-    dY4 = gate(mm(dYc, W_cl[..., :H]) + (LS * dh_a)[..., None] * w_a[:, None, :], X4)
+    rank1 = (LS * dh_a)[..., None] * w_a[:, None, :]                                      # dY4's d_alpha term
+    dY4 = gate(mm(dYc, W_cl[..., :H]) + rank1, X4)
     dY3 = gate(mm(dY4, W_m2), X3)
     dY2 = gate(mm(dY3, W_cat[..., :H]), X2)
     dY1 = gate(mm(dY2, W_m1), X1)
@@ -145,4 +149,4 @@ def evaluate(params: Dict[str, torch.Tensor], scale, batch: Dict[str, torch.Tens
     grad = torch.zeros(T.shape[0], 6, **f64)
     grad.index_add_(0, f.reshape(-1), rows.reshape(-1, 6))
     return {"rows": rows, "ray_terms": ray_terms, "terms": terms, "grad": grad, "loss": float(terms[:, 3].sum()),
-            "var": V, "abs_sum": pt.abs().sum((1, 2))}
+            "var": V, "abs_sum": pt.abs().sum((1, 2)), "dyc_pre": dyc_pre, "rank1": rank1}

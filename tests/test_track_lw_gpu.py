@@ -1,6 +1,6 @@
 """Tracking and bundle adjustment on the layer-wise tensor-core path (vmb_track_step_lw / vmb_ba_step_lw): parity with
-K10 / K11 and the fp64 oracle, K10's partial-row layout, the BA rows, bitwise reproducibility, the guards, localisation
-on a trained iMAP map and online SLAM in iMAP mode, and the vMAP background opt-in."""
+K10 / K11 and the fp64 oracle, K10's partial-row layout, the BA rows, bitwise reproducibility, the fp16 clamp count,
+the guards, localisation on a trained iMAP map and online SLAM in iMAP mode, and the vMAP background opt-in."""
 import ctypes as C
 import math
 
@@ -182,6 +182,49 @@ def test_ba_bad_frame_and_empty_masks():
     r0, _ = _ba_once(ens, rows, batch, P, kf_draw, np.array([[1, 1]] * 2, np.int32), 10, "layerwise")
     assert np.all(r2[1, :, 6] == 0.0) and np.array_equal(r2[0], r0[0])
     assert np.abs(r2[1, :, 7:9]).sum() > 0
+
+
+def _saturating(params):
+    """fused_oracle.saturation_batch alone stays far below the fp16 clamp at hidden 64 / 128 (the restatement's largest
+    |2^8 dYc| is about 10 and |2^8 d_alpha w_a| about 1e3), so the out_color weights are raised: colour unit 0 is made a
+    constant 2^-10 (a zero color_linear row, bias 2^-10), its out_color weights are set to 2^16, and the colour biases
+    drop by the 2^6 that adds.  Its dYc column, 2^16 sum_c 2^8 dh_c, then passes 60000 at about a hundred points per
+    object.  Its color_linear row is zero, so that column reaches no other gradient."""
+    params["color_linear.0.weight"][:, 0] = 0.0
+    params["color_linear.0.bias"][:, 0] = 2.0 ** -10
+    params["out_color.weight"][:, :, 0] = 2.0 ** 16
+    params["out_color.bias"] -= 2.0 ** 6
+    return params
+
+
+@pytest.mark.parametrize("hidden", [64, 128])
+def test_clamp_count(hidden):
+    """status[1]: the track and BA flavours count the same clamped values, between the restatement's counts of values
+    clearly past and clearly within +-60000; an ordinary batch on the unmodified network counts none."""
+    from oracle import fused_oracle as fo
+    from vmap_b200 import _lib
+    from vmap_b200.ensemble import VmapEnsemble
+    B, R, S = 2, 64, 10
+    rows = [1, 2]
+    params = _saturating(vo.init_params(B + 2, hidden, seed=hidden))
+    ens = VmapEnsemble(B + 2, hidden=hidden, scale=2.0, impl="fp32")
+    ens.load_stacked(params)
+    batch = fo.saturation_batch(B, R, S, seed=hidden + 1)
+    T = _rand_pose(hidden, 5, 0.05)
+    st = _track_once(ens, rows, batch, T, "layerwise")[3]["status"].cpu().numpy()
+    assert st[0] & _lib.TRACK_ST_CLAMP and st[1] > 0, st
+    # one draw of R rays per object, every ray at the frame whose pose is T
+    _, out = _ba_once(ens, rows, batch, np.stack([np.eye(4), T]), np.zeros((B, 1), np.int32), np.ones((B, 1), np.int32),
+                      R, "layerwise")
+    assert int(out["status"][1]) == int(st[1])
+    f = tlo.evaluate({k: v[rows] for k, v in params.items()}, torch.full((B,), 2.0), batch, T)
+    lo = sum(int((f[k].abs() > 60000 * 1.05).sum()) for k in ("dyc_pre", "rank1"))
+    hi = sum(int((f[k].abs() > 60000 / 1.05).sum()) for k in ("dyc_pre", "rank1"))
+    print(f"H{hidden}: status[1] {int(st[1])}, restatement {lo} past 63000, {hi} past 57143")
+    assert 0 < lo <= int(st[1]) <= hi
+    ens0, rows0, batch0, _ = _stack(hidden, B, R, S, seed=hidden)
+    st0 = _track_once(ens0, rows0, batch0, T, "layerwise")[3]["status"].cpu().numpy()
+    assert st0[1] == 0 and not st0[0] & _lib.TRACK_ST_CLAMP, st0
 
 
 def _bind_lw(ens, rows, batch, S_override=None):

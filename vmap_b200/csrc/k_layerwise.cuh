@@ -6,6 +6,9 @@
 // gradients, PE gradient) are small CUDA-core kernels.  Same arithmetic and the same reference lines
 // as k_step_fp32.cuh / k_step_fused.cuh: embedding.py:82-91, model.py:54-85, render_rays.py:4-96,
 // loss.py:5-62 and their backward.
+// The pose step (k_track_lw.cuh) runs the same network through the pieces written here once: the embedding block
+// (pe_block), a warp's head rows (HeadRows: staging, the heads, the dYc gate) and the GEMM chains (forward_gemms,
+// InputGrads).  Each step keeps its own render and loss.
 //
 // Workspace row layouts (fp16 unless noted), P = R*S points of the object:
 //   E  [P][144]: cols 0..86 = emb[0..86] (xyz/scale, sin k=0..3), 87 = 1, 88..95 = 0,
@@ -16,6 +19,7 @@
 //   W_in [H][96] | W_m1 [H][H] | W_cat [H][H+96] | W_m2 [H][H] | W_cl [H][H+48]   (zero under pad / ones columns)
 #pragma once
 #include <string>
+#include <type_traits>
 #include "common.cuh"
 #include "k_step_fp32.cuh"
 #include "k_gemm_umma.cuh"
@@ -95,8 +99,12 @@ __device__ __forceinline__ void sincos_ladder6(float proj, float (&s)[6], float 
 // ---------------------------------------------------------------------------------------------
 // positional embedding: 128 points per block, rows assembled in shared memory, written coalesced
 // ---------------------------------------------------------------------------------------------
-// one E row (EW halves) of the point t = p / scale: xyz, the sin bands, the constant-1 and zero columns
-__device__ __forceinline__ void pe_row(__half* r, float t0, float t1, float t2, const float* __restrict__ dirs) {
+// The E rows (EW halves each) of this block's 128 points of P, this thread's at the network input t (p / scale, or the
+// posed point of k_tlw_pe): xyz, the sin bands, the constant-1 and zero columns
+__device__ __forceinline__ void pe_block(float t0, float t1, float t2, const float* __restrict__ dirs, long long P,
+                                         __half* __restrict__ E) {
+  __shared__ __align__(16) __half row[128 * EW];
+  __half* r = row + threadIdx.x * EW;
   r[0] = __float2half_rn(t0); r[1] = __float2half_rn(t1); r[2] = __float2half_rn(t2);
   for (int d = 0; d < VMB_NDIRS; ++d) {
     float s[6], c[6];
@@ -110,6 +118,13 @@ __device__ __forceinline__ void pe_row(__half* r, float t0, float t1, float t2, 
   for (int j = ONES1 + 1; j < E1W; ++j) r[j] = __float2half_rn(0.f);
   r[E1W + ONES2] = __float2half_rn(1.0f);
   for (int j = E1W + ONES2 + 1; j < EW; ++j) r[j] = __float2half_rn(0.f);
+  __syncthreads();
+  // 128 rows x 288 B are contiguous in E
+  const long long p0 = (long long)blockIdx.x * 128;
+  const uint4* src = reinterpret_cast<const uint4*>(row);
+  uint4* dst = reinterpret_cast<uint4*>(E + p0 * EW);
+  const long long n16 = min(128LL, P - p0) * (EW * 2 / 16);
+  for (long long i = threadIdx.x; i < n16; i += 128) dst[i] = src[i];
 }
 
 __global__ void __launch_bounds__(128) k_lw_pe(const float* __restrict__ pcs, const float* __restrict__ dirs,
@@ -117,18 +132,10 @@ __global__ void __launch_bounds__(128) k_lw_pe(const float* __restrict__ pcs, co
   ptx::pdl_wait();
   ptx::pdl_launch_dependents();
   const float scale = *scale_ptr;
-  __shared__ __align__(16) __half row[128 * EW];
-  const long long p0 = (long long)blockIdx.x * 128, p = p0 + threadIdx.x;
-  __half* r = row + threadIdx.x * EW;
+  const long long p = (long long)blockIdx.x * 128 + threadIdx.x;
   float t0 = 0.f, t1 = 0.f, t2 = 0.f;
   if (p < P) { t0 = pcs[p * 3] / scale; t1 = pcs[p * 3 + 1] / scale; t2 = pcs[p * 3 + 2] / scale; }
-  pe_row(r, t0, t1, t2, dirs);
-  __syncthreads();
-  // 128 rows x 288 B are contiguous in E
-  const uint4* src = reinterpret_cast<const uint4*>(row);
-  uint4* dst = reinterpret_cast<uint4*>(E + p0 * EW);
-  const long long n16 = min(128LL, P - p0) * (EW * 2 / 16);
-  for (long long i = threadIdx.x; i < n16; i += 128) dst[i] = src[i];
+  pe_block(t0, t1, t2, dirs, P, E);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -178,6 +185,112 @@ struct RenderArgs {
   const int* counts; float cs, os; int backward;
   float* loss_terms; float* r_depth; float* r_var; float* r_colour; float* r_opacity;
 };
+template <int H> constexpr int hr_pitch() { return H * 2 + 16; }
+template <int H> constexpr int hr_smem() { return 4 * 32 * hr_pitch<H>(); }         // 4 warps x 32 rows (fc4, then hc)
+__device__ __forceinline__ void cp_async16(void* dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(ptx::smem_u32(dst)), "l"(src) : "memory");
+}
+// One warp's ray in the heads / render kernels (k_lw_heads_render, k_tlw_render), lane = sample: the heads forward on
+// the staged fc4 / hc rows and the head backward into dY_c.  A warp stages its ray's fc4 rows, then its hc rows, in ONE
+// shared-memory buffer with coalesced 16 B asynchronous copies (a lane walking its own 2H-byte row straight from global
+// memory is a chain of dependent L2 round trips); the row pitch of 2H + 16 B makes the per-lane 16 B reads
+// conflict-free, and one buffer per warp keeps three blocks resident per SM at H = 256 so the copies of one warp hide
+// behind the arithmetic of the others.
+template <int H>
+struct HeadRows {
+  static constexpr int PITCH = hr_pitch<H>(), LPR = H / 8, RPP = 32 / LPR;      // lanes per row, rows per copy pass
+  float* w;                 // the block's head weights in shared memory: [0,H) out_alpha row, [H,4H) out_color rows
+  unsigned char* srow;      // this warp's 32 rows
+  int lane, S;
+
+  // every thread of the block; the caller synchronises before the first read
+  __device__ __forceinline__ void load(const float* __restrict__ P, const VmbLayout& L) {
+    for (int i = threadIdx.x; i < H; i += 128) w[i] = P[L.o_Wa + i];
+    for (int i = threadIdx.x; i < 3 * H; i += 128) w[H + i] = P[L.o_Woc + i];
+  }
+  __device__ __forceinline__ uint4* row() const { return reinterpret_cast<uint4*>(srow + lane * PITCH); }
+  // the ray's S rows [pb, pb + S) of X, once the rows staged before are no longer read
+  __device__ __forceinline__ void stage(const __half* X, long long pb) {
+    __syncwarp();
+#pragma unroll 4
+    for (int r0 = 0; r0 < S; r0 += RPP) {
+      const int r = r0 + lane / LPR, cq = lane % LPR;
+      if (r < S) cp_async16(srow + r * PITCH + cq * 16, X + (pb + r) * H + cq * 8);
+    }
+    asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
+    __syncwarp();
+  }
+  // w_a . fc4 of the staged fc4 row, in two chains: the dot product is FMA-latency bound otherwise
+  __device__ __forceinline__ float alpha() const {
+    const uint4* xrow = row();
+    float ha = 0.f, hb = 0.f;
+#pragma unroll 4
+    for (int q = 0; q < H / 8; ++q) {
+      const uint4 u = xrow[q];
+      const __half* hu = reinterpret_cast<const __half*>(&u);
+#pragma unroll
+      for (int j = 0; j < 8; j += 2) {
+        ha = fmaf(__half2float(hu[j]), w[q * 8 + j], ha);
+        hb = fmaf(__half2float(hu[j + 1]), w[q * 8 + j + 1], hb);
+      }
+    }
+    return ha + hb;
+  }
+  // W_oc hc of the staged hc row
+  __device__ __forceinline__ void colour(float& h0, float& h1, float& h2) const {
+    const uint4* xrow = row();
+    h0 = h1 = h2 = 0.f;
+#pragma unroll 4
+    for (int q = 0; q < H / 8; ++q) {
+      const uint4 v = xrow[q];
+      const __half* hv = reinterpret_cast<const __half*>(&v);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float fc = __half2float(hv[j]);
+        const int o = q * 8 + j;
+        h0 = fmaf(fc, w[H + o], h0); h1 = fmaf(fc, w[2 * H + o], h1); h2 = fmaf(fc, w[3 * H + o], h2);
+      }
+    }
+  }
+  // The staged hc row gated IN PLACE into dY_c = relu'(hc) * (d @ W_oc), clamped to the fp16 range +-60000, from the
+  // loss-scaled d(raw colour) d0..d2.  Returns how many values pass 60000: the clamped dY_c elements, and the elements
+  // where dY4's rank-1 term da w_a (da the loss-scaled d(raw alpha)) does on its own.
+  __device__ __forceinline__ int gate(float d0, float d1, float d2, float da) {
+    uint4* xc = row();
+    int n = 0;
+#pragma unroll 4
+    for (int q = 0; q < H / 8; ++q) {
+      const uint4 v = xc[q];
+      const __half* hv = reinterpret_cast<const __half*>(&v);
+      uint32_t r[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int o = q * 8 + 2 * j;
+        float x0 = fmaf(d2, w[3 * H + o], fmaf(d1, w[2 * H + o], d0 * w[H + o]));
+        float x1 = fmaf(d2, w[3 * H + o + 1], fmaf(d1, w[2 * H + o + 1], d0 * w[H + o + 1]));
+        const bool g0 = __half2float(hv[2 * j]) > 0.f, g1 = __half2float(hv[2 * j + 1]) > 0.f;
+        n += (g0 && fabsf(x0) > 60000.f) + (g1 && fabsf(x1) > 60000.f);
+        n += (fabsf(da * w[o]) > 60000.f) + (fabsf(da * w[o + 1]) > 60000.f);
+        x0 = g0 ? fminf(fmaxf(x0, -60000.f), 60000.f) : 0.f;
+        x1 = g1 ? fminf(fmaxf(x1, -60000.f), 60000.f) : 0.f;
+        __half2 hh = __floats2half2_rn(x0, x1);
+        r[j] = *reinterpret_cast<uint32_t*>(&hh);
+      }
+      xc[q] = make_uint4(r[0], r[1], r[2], r[3]);
+    }
+    return n;
+  }
+  // the ray's dY_c rows out as whole 2H-byte rows (the mirror image of stage), once every lane has gated its row
+  __device__ __forceinline__ void store(__half* __restrict__ dYc, long long pb) const {
+    __syncwarp();
+#pragma unroll 4
+    for (int r0 = 0; r0 < S; r0 += RPP) {
+      const int r = r0 + lane / LPR, cq = lane % LPR;
+      if (r < S) *reinterpret_cast<uint4*>(dYc + (pb + r) * H + cq * 8) = *reinterpret_cast<const uint4*>(srow + r * PITCH + cq * 16);
+    }
+  }
+};
+
 // Heads + render + loss + head gradients in ONE kernel, one warp per ray, lane = sample (n_samples <= 32):
 //   forward   alpha / colour heads of the lane's point (the fc4 / hc rows are read once),
 //   render    transmittance as a warp product scan, the ray sums as warp reductions,
@@ -185,15 +298,6 @@ struct RenderArgs {
 //             (fp16, x2^8), the scaled copies of d_alpha for the rank-1 term / the head wgrad GEMMs, and the bias
 //             gradients of the two heads.
 // Replaces three launches (heads, render, head gradients) and the round trip of occupancy / colour / dhead through HBM.
-// A warp stages its ray's fc4 rows, then its hc rows, in ONE shared-memory buffer with coalesced 16 B asynchronous
-// copies (a lane walking its own 2H-byte row straight from global memory is a chain of dependent L2 round trips); the
-// row pitch of 2H + 16 B makes the per-lane 16 B reads conflict-free, and one buffer per warp keeps three blocks
-// resident per SM at H = 256 so the copies of one warp hide behind the arithmetic of the others.
-template <int H> constexpr int hr_pitch() { return H * 2 + 16; }
-template <int H> constexpr int hr_smem() { return 4 * 32 * hr_pitch<H>(); }         // 4 warps x 32 rows (fc4, then hc)
-__device__ __forceinline__ void cp_async16(void* dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(ptx::smem_u32(dst)), "l"(src) : "memory");
-}
 template <int H>
 __global__ void __launch_bounds__(128) k_lw_heads_render(RenderArgs a, const __half* __restrict__ X4, const __half* __restrict__ XC,
                                                          const float* __restrict__ P, VmbLayout L, __half* __restrict__ dYc,
@@ -202,12 +306,12 @@ __global__ void __launch_bounds__(128) k_lw_heads_render(RenderArgs a, const __h
   ptx::pdl_wait();
   ptx::pdl_launch_dependents();
   extern __shared__ __align__(16) unsigned char hr_rows[];
-  __shared__ float w[4 * H];                          // [0,H) out_alpha row, [H,4H) out_color rows
+  __shared__ float w[4 * H];
   __shared__ int s_on[3];
   __shared__ float s_loss[3], s_b[4];
-  constexpr int PITCH = hr_pitch<H>(), LPR = H / 8, RPP = 32 / LPR;      // lanes per row, rows per copy pass
-  for (int i = threadIdx.x; i < H; i += 128) w[i] = P[L.o_Wa + i];
-  for (int i = threadIdx.x; i < 3 * H; i += 128) w[H + i] = P[L.o_Woc + i];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, S = a.S, b = a.b;
+  HeadRows<H> hr{w, hr_rows + warp * (32 * HeadRows<H>::PITCH), lane, S};
+  hr.load(P, L);
   if (threadIdx.x < 3) {
     int on = 1;
     for (int i = 0; i < a.B; ++i) on &= (a.counts[i * 4 + threadIdx.x] != 0);
@@ -215,7 +319,6 @@ __global__ void __launch_bounds__(128) k_lw_heads_render(RenderArgs a, const __h
   }
   if (threadIdx.x < 4) s_b[threadIdx.x] = 0.f;
   __syncthreads();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, S = a.S, b = a.b;
   const unsigned FULL = 0xffffffffu;
   const float b_a = P[L.o_ba], b_c0 = P[L.o_boc], b_c1 = P[L.o_boc + 1], b_c2 = P[L.o_boc + 2];
   const float inv_nd = 1.f / ((float)a.counts[b * 4 + 0] + 1e-10f);
@@ -223,53 +326,17 @@ __global__ void __launch_bounds__(128) k_lw_heads_render(RenderArgs a, const __h
   const float inv_ns = 1.f / ((float)a.counts[b * 4 + 2] + 1e-10f);
   const float on_d = s_on[0] ? 1.f : 0.f, on_c = s_on[1] ? 1.f : 0.f, on_o = s_on[2] ? 1.f : 0.f;
   const bool in = lane < S;
-  unsigned char* srow = hr_rows + warp * (32 * PITCH);          // this warp's row buffer
   float l_d = 0.f, l_c = 0.f, l_o = 0.f;              // every lane carries the same per-ray values; lane 0's are used
   float sb0 = 0.f, sb1 = 0.f, sb2 = 0.f, sb3 = 0.f;   // this lane's share of the head bias gradients
-  auto stage_rows = [&](const __half* X, long long pb) {
-#pragma unroll 4
-    for (int r0 = 0; r0 < S; r0 += RPP) {
-      const int r = r0 + lane / LPR, cq = lane % LPR;
-      if (r < S) cp_async16(srow + r * PITCH + cq * 16, X + (pb + r) * H + cq * 8);
-    }
-    asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
-    __syncwarp();
-  };
-  const uint4* xrow = reinterpret_cast<const uint4*>(srow + lane * PITCH);
   for (int ray = blockIdx.x * 4 + warp; ray < a.R; ray += gridDim.x * 4) {
     const long long pb = (long long)ray * S, pi = pb + lane;
-    __syncwarp();                                     // the previous ray's rows are no longer read
-    stage_rows(X4, pb);
+    hr.stage(X4, pb);
     float ha = 0.f, h0 = 0.f, h1 = 0.f, h2 = 0.f;
-    if (in) {
-      float hb = 0.f;                                 // two chains: the dot product is FMA-latency bound otherwise
-#pragma unroll 4
-      for (int q = 0; q < H / 8; ++q) {
-        const uint4 u = xrow[q];
-        const __half* hu = reinterpret_cast<const __half*>(&u);
-#pragma unroll
-        for (int j = 0; j < 8; j += 2) {
-          ha = fmaf(__half2float(hu[j]), w[q * 8 + j], ha);
-          hb = fmaf(__half2float(hu[j + 1]), w[q * 8 + j + 1], hb);
-        }
-      }
-      ha += hb;
-    }
-    __syncwarp();
-    stage_rows(XC, pb);                               // hc stays staged for the backward half
+    if (in) ha = hr.alpha();
+    hr.stage(XC, pb);                                 // hc stays staged for the backward half
     float oc = 0.f, zz = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f;
     if (in) {
-#pragma unroll 4
-      for (int q = 0; q < H / 8; ++q) {
-        const uint4 v = xrow[q];
-        const __half* hv = reinterpret_cast<const __half*>(&v);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float fc = __half2float(hv[j]);
-          const int o = q * 8 + j;
-          h0 = fmaf(fc, w[H + o], h0); h1 = fmaf(fc, w[2 * H + o], h1); h2 = fmaf(fc, w[3 * H + o], h2);
-        }
-      }
+      hr.colour(h0, h1, h2);
       oc = vmb_sigmoid((ha + b_a) * 10.0f);
       c0 = vmb_sigmoid(h0 + b_c0); c1 = vmb_sigmoid(h1 + b_c1); c2 = vmb_sigmoid(h2 + b_c2);
       zz = a.z[pi];
@@ -320,33 +387,9 @@ __global__ void __launch_bounds__(128) k_lw_heads_render(RenderArgs a, const __h
       __half2 h01 = __floats2half2_rn(fminf(fmaxf(LS * dh.x, -60000.f), 60000.f), fminf(fmaxf(LS * dh.y, -60000.f), 60000.f));
       __half2 h23 = __floats2half2_rn(fminf(fmaxf(LS * dh.z, -60000.f), 60000.f), fminf(fmaxf(LS * dh.w, -60000.f), 60000.f));
       reinterpret_cast<uint4*>(dh16)[pi] = make_uint4(*reinterpret_cast<uint32_t*>(&h01), *reinterpret_cast<uint32_t*>(&h23), 0u, 0u);
-      uint4* xc = const_cast<uint4*>(xrow);             // second pass over the staged hc row, gated IN PLACE
-      const float d0 = LS * dh.y, d1 = LS * dh.z, d2 = LS * dh.w;
-#pragma unroll 4
-      for (int q = 0; q < H / 8; ++q) {
-        const uint4 v = xc[q];
-        const __half* hv = reinterpret_cast<const __half*>(&v);
-        uint32_t r[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int o = q * 8 + 2 * j;
-          float x0 = fmaf(d2, w[3 * H + o], fmaf(d1, w[2 * H + o], d0 * w[H + o]));
-          float x1 = fmaf(d2, w[3 * H + o + 1], fmaf(d1, w[2 * H + o + 1], d0 * w[H + o + 1]));
-          x0 = (__half2float(hv[2 * j]) > 0.f) ? fminf(fmaxf(x0, -60000.f), 60000.f) : 0.f;
-          x1 = (__half2float(hv[2 * j + 1]) > 0.f) ? fminf(fmaxf(x1, -60000.f), 60000.f) : 0.f;
-          __half2 hh = __floats2half2_rn(x0, x1);
-          r[j] = *reinterpret_cast<uint32_t*>(&hh);
-        }
-        xc[q] = make_uint4(r[0], r[1], r[2], r[3]);
-      }
+      hr.gate(LS * dh.y, LS * dh.z, LS * dh.w, LS * dh.x);     // the clamp count is the pose step's
     }
-    __syncwarp();
-    // the ray's dYc rows leave as whole 2H-byte rows (the mirror image of the staging copies)
-#pragma unroll 4
-    for (int r0 = 0; r0 < S; r0 += RPP) {
-      const int r = r0 + lane / LPR, cq = lane % LPR;
-      if (r < S) *reinterpret_cast<uint4*>(dYc + (pb + r) * H + cq * 8) = *reinterpret_cast<const uint4*>(srow + r * PITCH + cq * 16);
-    }
+    hr.store(dYc, pb);
   }
   if (lane == 0) { atomicAdd(&s_loss[0], l_d); atomicAdd(&s_loss[1], l_c); atomicAdd(&s_loss[2], l_o); }
   if (a.backward) {
@@ -461,14 +504,42 @@ __global__ void __launch_bounds__(128) k_lw_pe_bwd(const float* __restrict__ pcs
 // ---------------------------------------------------------------------------------------------
 // host orchestration: one object at a time (wide ensembles have one or very few objects)
 // ---------------------------------------------------------------------------------------------
+// (k_track_lw.cuh uses it too, and undefines it)
+#define LW_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return VMB_E_CUDA; } } while (0)
+
+// f(std::integral_constant<int, H>) for the layer-wise widths, once the driver's tensor-map encoder is there; `what`
+// names the path in the error
+template <class F>
+static int for_hidden(int H, const char* what, std::string& err, F&& f) {
+  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return VMB_E_CUDA; }
+  switch (H) {
+    case 64:  return f(std::integral_constant<int, 64>());
+    case 128: return f(std::integral_constant<int, 128>());
+    case 256: return f(std::integral_constant<int, 256>());
+  }
+  err = std::string(what) + ": hidden must be 64, 128 or 256";
+  return VMB_E_UNSUPPORTED;
+}
+
+// programmatic dependent launch pays where the step is a chain of short single-wave kernels (background model, iMAP
+// shards: -3..5 %); at the full iMAP shape the kernels are HBM-bound for tens of microseconds and the early launch of
+// the successor only takes resources from them (+1 %): armed below 64 K points only
+static bool pdl_ok(long long np) { return np <= 65536; }
+
+// blocks of a heads / render launch over R rays: four rays each, no more than stay resident with their row buffers
+template <int H>
+static int hr_blocks(int R, int n_sm) {
+  const int hr_per_sm = std::max(1, std::min(8, (int)(227 * 1024 / (hr_smem<H>() + 6 * 1024))));
+  return std::min((R + 3) / 4, n_sm * hr_per_sm);
+}
+
 // ---------------------------------------------------------------------------------------------
 // GEMM launches of one object, shared by the training step (step_object) and the tracking path (k_track_lw.cuh)
 // ---------------------------------------------------------------------------------------------
 // forward: the five layers E -> X1 -> X2 -> X3 -> X4 -> XC (model.py:54-85); Pb = the object's fp32 param row (biases),
 // Wi = its fp16 image.  Each launch follows its predecessor directly on `st` (k_lw_pe first): armed when pdl_ok.
 template <int H>
-static cudaError_t forward_gemms(Workspace& ws, const VmbLayout& L, const float* Pb, const __half* Wi, long long np, bool pdl_ok,
-                                 cudaStream_t st) {
+static cudaError_t forward_gemms(Workspace& ws, const VmbLayout& L, const float* Pb, const __half* Wi, long long np, cudaStream_t st) {
   const int mt = (int)((np + BM - 1) / BM);
   const Operand none{nullptr, 0, 0, 0};
   auto opX = [&](const __half* x) { return Operand{x, np, H, H}; };
@@ -476,7 +547,7 @@ static cudaError_t forward_gemms(Workspace& ws, const VmbLayout& L, const float*
   auto fwd = [&](const Operand& a1, const Operand& a2, int K1, int K2, long long woff, int ldw, int boff, __half* out) {
     GemmArgs g; memset(&g, 0, sizeof(g));
     g.M = (int)np; g.N = H; g.K1 = K1; g.K2 = K2; g.bias = Pb + boff; g.out16 = out; g.ldo = H; g.scale = 1.0f;
-    if (pdl_ok) pdl_arm();                          // follows k_lw_pe / the previous layer directly on `st`
+    if (pdl_ok(np)) pdl_arm();                      // follows k_lw_pe / the previous layer directly on `st`
     return launch_gemm_auto<0, EPI_RELU_F16>(a1, a2, Operand{Wi + woff, H, ldw, ldw}, g, mt, (H + BN - 1) / BN, st);
   };
   cudaError_t e = fwd(opE1, none, E1W, 0, 0, 96, L.o_bin, ws.X1);
@@ -487,46 +558,56 @@ static cudaError_t forward_gemms(Workspace& ws, const VmbLayout& L, const float*
   return e;
 }
 
-// input gradient through a weight block: out = gate(x_prev) * (dY @ W[:, c0:c0+N] (+ rank-1 r1row x r1col))
+// The input-gradient chain from dYc (and dalpha_s) to the embedding gradient dE, one GEMM per member, in this order:
+// de_colour (the colour block of dE), dy4 (with the rank-1 d_alpha w_a term) -> dYa, dy3 -> dYb, dy2 -> dYa, dy1 -> dYc, demb1
+// (the emb1 block of dE from dY3 and dY1).  Wi = the object's fp16 image, w_a its fp32 out_alpha row.  Each member
+// launches on `st`; the caller arms it, or puts its own work in between.
 template <int H>
-static cudaError_t dgrad_gate_gemm(const __half* dY, const __half* Wi, long long woff, int ldw, long long np, const __half* xprev,
-                                   __half* out, const float* r1row, const float* r1col, cudaStream_t st) {
-  GemmArgs g; memset(&g, 0, sizeof(g));
-  g.M = (int)np; g.N = H; g.K1 = H; g.out16 = out; g.ldo = H; g.gate = xprev; g.ldg = H; g.r1_row = r1row; g.r1_col = r1col;
-  g.r1_stride = 1; g.scale = 1.0f;
-  const Operand none{nullptr, 0, 0, 0};
-  return launch_gemm_auto<1, EPI_GATE_F16>(Operand{dY, np, H, H}, none, Operand{Wi + woff, H, H, ldw}, g,
-                                           (int)((np + BM - 1) / BM), (H + BN - 1) / BN, st);
-}
+struct InputGrads {
+  Workspace& ws;
+  const __half* Wi;
+  const float* w_a;
+  long long np;
+  cudaStream_t st;
 
-// input gradient into the fp32 embedding gradient: dE[:, ecol:ecol+N] (=|+=) dY @ W[:, c0:c0+N]
-template <int H>
-static cudaError_t dgrad_emb_gemm(Workspace& ws, const __half* dY, const __half* Wi, long long woff, int ldw, int N, int ecol,
-                                  int accumulate, long long np, cudaStream_t st) {
-  GemmArgs g; memset(&g, 0, sizeof(g));
-  g.M = (int)np; g.N = N; g.K1 = H; g.out32 = ws.dE + ecol; g.ld32 = EW; g.accumulate = accumulate; g.scale = 1.0f;
-  const Operand none{nullptr, 0, 0, 0};
-  return launch_gemm_auto<1, EPI_F32>(Operand{dY, np, H, H}, none, Operand{Wi + woff, H, N, ldw}, g, (int)((np + BM - 1) / BM), 1, st);
-}
-
-// d emb1 = dY3 @ W_cat[:, H:] + dY1 @ W_in in ONE launch: A = [dY3 | dY1] along K, B = the two weight blocks
-// (two launches, the second accumulating, where the weight-stationary kernel does not fit)
-template <int H>
-static cudaError_t demb1_gemm(Workspace& ws, const __half* dY3, const __half* dY1, const __half* Wi, long long np, cudaStream_t st) {
-  GemmArgs g; memset(&g, 0, sizeof(g));
-  g.M = (int)np; g.N = E1W; g.K1 = H; g.K2 = H; g.out32 = ws.dE; g.ld32 = EW; g.accumulate = 0; g.scale = 1.0f;
-  const Operand bcat{Wi + off_cat(H) + H, H, E1W, H + 96}, bin{Wi, H, E1W, 96};
-  cudaError_t e = launch_gemm_ws<1, EPI_F32>(Operand{dY3, np, H, H}, Operand{dY1, np, H, H}, bcat, g, (int)((np + BM - 1) / BM),
-                                              st, &bin);
-  if (e == cudaErrorNotSupported) {
-    (void)cudaGetLastError();
-    e = dgrad_emb_gemm<H>(ws, dY3, Wi, off_cat(H) + H, H + 96, E1W, 0, 0, np, st);
-    if (e == cudaSuccess) e = dgrad_emb_gemm<H>(ws, dY1, Wi, 0, 96, E1W, 0, 1, np, st);
+  // out = gate(x_prev) * (dY @ W[:, woff block] (+ rank-1 r1row x r1col))
+  cudaError_t gate(const __half* dY, long long woff, int ldw, const __half* xprev, __half* out, const float* r1row = nullptr,
+                   const float* r1col = nullptr) const {
+    GemmArgs g; memset(&g, 0, sizeof(g));
+    g.M = (int)np; g.N = H; g.K1 = H; g.out16 = out; g.ldo = H; g.gate = xprev; g.ldg = H; g.r1_row = r1row; g.r1_col = r1col;
+    g.r1_stride = 1; g.scale = 1.0f;
+    const Operand none{nullptr, 0, 0, 0};
+    return launch_gemm_auto<1, EPI_GATE_F16>(Operand{dY, np, H, H}, none, Operand{Wi + woff, H, H, ldw}, g,
+                                             (int)((np + BM - 1) / BM), (H + BN - 1) / BN, st);
   }
-  return e;
-}
-
-#define LW_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return VMB_E_CUDA; } } while (0)
+  // dE[:, ecol:ecol+N] (=|+=) dY @ W[:, woff block]
+  cudaError_t emb(const __half* dY, long long woff, int ldw, int N, int ecol, int accumulate) const {
+    GemmArgs g; memset(&g, 0, sizeof(g));
+    g.M = (int)np; g.N = N; g.K1 = H; g.out32 = ws.dE + ecol; g.ld32 = EW; g.accumulate = accumulate; g.scale = 1.0f;
+    const Operand none{nullptr, 0, 0, 0};
+    return launch_gemm_auto<1, EPI_F32>(Operand{dY, np, H, H}, none, Operand{Wi + woff, H, N, ldw}, g, (int)((np + BM - 1) / BM), 1, st);
+  }
+  cudaError_t de_colour() const { return emb(ws.dYc, off_cl(H) + H, H + 48, E2W, E1W, 0); }
+  cudaError_t dy4() const { return gate(ws.dYc, off_cl(H), H + 48, ws.X4, ws.dYa, ws.dalpha_s, w_a); }
+  cudaError_t dy3() const { return gate(ws.dYa, off_m2(H), H, ws.X3, ws.dYb); }
+  cudaError_t dy2() const { return gate(ws.dYb, off_cat(H), H + 96, ws.X2, ws.dYa); }
+  cudaError_t dy1() const { return gate(ws.dYa, off_m1(H), H, ws.X1, ws.dYc); }
+  // d emb1 = dY3 @ W_cat[:, H:] + dY1 @ W_in in ONE launch: A = [dY3 | dY1] along K, B = the two weight blocks
+  // (two launches, the second accumulating, where the weight-stationary kernel does not fit)
+  cudaError_t demb1() const {
+    GemmArgs g; memset(&g, 0, sizeof(g));
+    g.M = (int)np; g.N = E1W; g.K1 = H; g.K2 = H; g.out32 = ws.dE; g.ld32 = EW; g.accumulate = 0; g.scale = 1.0f;
+    const Operand bcat{Wi + off_cat(H) + H, H, E1W, H + 96}, bin{Wi, H, E1W, 96};
+    cudaError_t e = launch_gemm_ws<1, EPI_F32>(Operand{ws.dYb, np, H, H}, Operand{ws.dYc, np, H, H}, bcat, g,
+                                                (int)((np + BM - 1) / BM), st, &bin);
+    if (e == cudaErrorNotSupported) {
+      (void)cudaGetLastError();
+      e = emb(ws.dYb, off_cat(H) + H, H + 96, E1W, 0, 0);
+      if (e == cudaSuccess) e = emb(ws.dYc, 0, 96, E1W, 0, 1);
+    }
+    return e;
+  }
+};
 
 template <int H>
 static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, const __half* image, int b, cudaStream_t st,
@@ -541,17 +622,13 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
   const float* scale_p = sp.scale + b;
   const int nblk = (int)((np + 127) / 128);
   const Operand none{nullptr, 0, 0, 0};
-  // programmatic dependent launch pays where the step is a chain of short single-wave kernels (background model, iMAP
-  // shards: -3..5 %); at the full iMAP shape the kernels are HBM-bound for tens of microseconds and the early launch of
-  // the successor only takes resources from them (+1 %): armed below 64 K points only
-  const bool pdl_ok = np <= 65536;
-  auto arm = [&]() { if (pdl_ok) pdl_arm(); };
+  auto arm = [&]() { if (pdl_ok(np)) pdl_arm(); };
   auto opX = [&](const __half* x) { return Operand{x, np, H, H}; };
   const Operand opE1{ws.E, np, E1W, EW}, opE2{ws.E + E1W, np, E2W, EW};
 
   // ---- forward ----
   LW_TRY(launch_k(k_lw_pe, dim3(nblk), dim3(128), 0, st, pcs, dirs, scale_p, np, ws.E));
-  LW_TRY(forward_gemms<H>(ws, L, Pb, Wi, np, pdl_ok, st));
+  LW_TRY(forward_gemms<H>(ws, L, Pb, Wi, np, st));
   if (sp.fwd_only) {
     arm();
     LW_TRY(launch_k(k_lw_heads<H>, dim3(nblk), dim3(128), 0, st, (const __half*)ws.X4, (const __half*)ws.XC, Pb, L, np,
@@ -569,9 +646,8 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
   cudaGetDevice(&dev);
   const int n_sm = sm_count(dev);
   LW_TRY(smem_limit_once<k_lw_heads_render<H>>(dev, hr_smem<H>()));
-  const int hr_per_sm = std::max(1, std::min(8, (int)(227 * 1024 / (hr_smem<H>() + 6 * 1024))));
   arm();
-  LW_TRY(launch_k(k_lw_heads_render<H>, dim3(std::min((sp.R + 3) / 4, n_sm * hr_per_sm)), dim3(128), (size_t)hr_smem<H>(), st, ra,
+  LW_TRY(launch_k(k_lw_heads_render<H>, dim3(hr_blocks<H>(sp.R, n_sm)), dim3(128), (size_t)hr_smem<H>(), st, ra,
                   (const __half*)ws.X4, (const __half*)ws.XC, Pb, L, ws.dYc, ws.dh16, ws.dalpha_s, G));
   if (!sp.backward) return 0;
 
@@ -591,9 +667,7 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
     g.n_valid = n_valid; g.ones_col = ones_col; g.gbias = boff >= 0 ? G + boff : nullptr; g.scale = INV_LS;
     return launch_gemm<1, 1, EPI_ATOMIC>(Operand{dY, np, H, H}, none, xb, g, (H + BM - 1) / BM, (N + BN - 1) / BN, zs, sd);
   };
-  auto dgrad_gate = [&](const __half* dY, long long woff, int ldw, const __half* xprev, __half* out, const float* r1row, const float* r1col) {
-    return dgrad_gate_gemm<H>(dY, Wi, woff, ldw, np, xprev, out, r1row, r1col, st);
-  };
+  const InputGrads<H> ig{ws, Wi, Pb + L.o_Wa, np, st};
   // heads: dW_a[o] = sum_p d_a fc4[p][o]; dW_oc[c][o] = sum_p d_rc[c] hc[p][o]   (B = dh16 [P][8], columns 0 / 1..3)
   {
     GemmArgs g; memset(&g, 0, sizeof(g));
@@ -610,34 +684,34 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
   LW_TRY(wgrad(ws.dYc, opX(ws.X4), H, L.o_Wcl, H + L.e2, H, -1, -1));
   arm();
   LW_TRY(wgrad(ws.dYc, opE2, E2W, L.o_Wcl + H, H + L.e2, L.e2, ONES2, L.o_bcl));
-  LW_TRY(dgrad_emb_gemm<H>(ws, ws.dYc, Wi, off_cl(H) + H, H + 48, E2W, E1W, 0, np, st));          // first kernel on `st` after the fork: not armed
+  LW_TRY(ig.de_colour());                                     // first kernel on `st` after the fork: not armed
   arm();
-  LW_TRY(dgrad_gate(ws.dYc, off_cl(H), H + 48, ws.X4, ws.dYa, ws.dalpha_s, Pb + L.o_Wa));          // dY4 -> dYa
+  LW_TRY(ig.dy4());
   // mid2
   LW_TRY(fork(1));
   LW_TRY(wgrad(ws.dYa, opX(ws.X3), H, L.o_Wm2, H, H, -1, -1));
   arm();                                          // follows this layer's weight-gradient GEMM directly on the side stream
   LW_TRY(launch_k(k_lw_colsum, dim3((unsigned)((np + cs_rows - 1) / cs_rows)), dim3(256), 0, sd, (const __half*)ws.dYa, np, H, cs_rows, G + L.o_bm2));
   LW_TRY(cudaEventRecord(ws.ev_side[0], sd));           // the side stream is done reading dYc (dY of color_linear) and dYa (dY4)
-  LW_TRY(dgrad_gate(ws.dYa, off_m2(H), H, ws.X3, ws.dYb, nullptr, nullptr));                        // dY3 -> dYb
+  LW_TRY(ig.dy3());
   // cat_layer
   LW_TRY(fork(2));
   LW_TRY(wgrad(ws.dYb, opX(ws.X2), H, L.o_Wcat, H + VMB_E1, H, -1, -1));
   arm();
   LW_TRY(wgrad(ws.dYb, opE1, E1W, L.o_Wcat + H, H + VMB_E1, VMB_E1, ONES1, L.o_bcat));
   LW_TRY(cudaStreamWaitEvent(st, ws.ev_side[0], 0));    // dYa / dYc are about to be overwritten
-  LW_TRY(dgrad_gate(ws.dYb, off_cat(H), H + 96, ws.X2, ws.dYa, nullptr, nullptr));                  // dY2 -> dYa (dY3 stays in dYb)
+  LW_TRY(ig.dy2());                                     // dY3 stays in dYb
   // mid1
   LW_TRY(fork(3));
   LW_TRY(wgrad(ws.dYa, opX(ws.X1), H, L.o_Wm1, H, H, -1, -1));
   arm();                                          // follows this layer's weight-gradient GEMM directly on the side stream
   LW_TRY(launch_k(k_lw_colsum, dim3((unsigned)((np + cs_rows - 1) / cs_rows)), dim3(256), 0, sd, (const __half*)ws.dYa, np, H, cs_rows, G + L.o_bm1));
-  LW_TRY(dgrad_gate(ws.dYa, off_m1(H), H, ws.X1, ws.dYc, nullptr, nullptr));                        // dY1 -> dYc (free since color_linear)
+  LW_TRY(ig.dy1());                                     // dYc is free since color_linear
   // in_layer
   LW_TRY(fork(4));
   LW_TRY(wgrad(ws.dYc, opE1, E1W, L.o_Win, VMB_E1, VMB_E1, ONES1, L.o_bin));
   LW_TRY(cudaEventRecord(ws.ev_side[1], sd));
-  LW_TRY(demb1_gemm<H>(ws, ws.dYb, ws.dYc, Wi, np, st));                                        // d emb1 (dY3, dY1)
+  LW_TRY(ig.demb1());
   LW_TRY(smem_limit_once<k_lw_pe_bwd>(dev, PEB_SMEM));
   arm();                                         // follows the embedding-gradient GEMM directly on `st`
   LW_TRY(launch_k(k_lw_pe_bwd, dim3(nblk), dim3(128), (size_t)PEB_SMEM, st, pcs, dirs, scale_p, np, (const float*)ws.dE, G + L.o_B));
@@ -649,40 +723,25 @@ static int step_object(Workspace& ws, const VmbLayout& L, const StepParams& sp, 
 // forward only (vmb_forward): chunks of FWD_CHUNK points so the activation workspace stays bounded for 256^3 grids
 constexpr long long FWD_CHUNK = 1LL << 18;
 static int launch_forward(Workspace& ws, const VmbLayout& L, const StepParams& sp, const void* image, cudaStream_t st, std::string& err) {
-  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return VMB_E_CUDA; }
-  const long long N = sp.R;
-  LW_TRY(ws.grow(std::min(N, FWD_CHUNK), L.H, stream_capturing(st)));
-  for (int b = 0; b < sp.B; ++b)
-    for (long long p0 = 0; p0 < N; p0 += FWD_CHUNK) {
-      const long long n = std::min(FWD_CHUNK, N - p0);
-      int rc;
-      switch (L.H) {
-        case 64:  rc = step_object<64>(ws, L, sp, (const __half*)image, b, st, err, p0, n); break;
-        case 128: rc = step_object<128>(ws, L, sp, (const __half*)image, b, st, err, p0, n); break;
-        case 256: rc = step_object<256>(ws, L, sp, (const __half*)image, b, st, err, p0, n); break;
-        default: err = "layer-wise path: hidden must be 64, 128 or 256"; return VMB_E_UNSUPPORTED;
-      }
-      if (rc) return rc;
-    }
-  return 0;
+  return for_hidden(L.H, "layer-wise path", err, [&](auto h) -> int {
+    const long long N = sp.R;
+    LW_TRY(ws.grow(std::min(N, FWD_CHUNK), L.H, stream_capturing(st)));
+    for (int b = 0; b < sp.B; ++b)
+      for (long long p0 = 0; p0 < N; p0 += FWD_CHUNK)
+        if (const int rc = step_object<decltype(h)::value>(ws, L, sp, (const __half*)image, b, st, err, p0, std::min(FWD_CHUNK, N - p0)))
+          return rc;
+    return 0;
+  });
 }
 
 static int launch_step(Workspace& ws, const VmbLayout& L, const StepParams& sp, const void* image, cudaStream_t st, std::string& err) {
-  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return VMB_E_CUDA; }
-  if (sp.S > 32) { err = "layer-wise path: n_samples > 32"; return VMB_E_UNSUPPORTED; }
-  LW_TRY(ws.grow((long long)sp.R * sp.S, L.H, stream_capturing(st)));
-  for (int b = 0; b < sp.B; ++b) {
-    int rc;
-    switch (L.H) {
-      case 64:  rc = step_object<64>(ws, L, sp, (const __half*)image, b, st, err); break;
-      case 128: rc = step_object<128>(ws, L, sp, (const __half*)image, b, st, err); break;
-      case 256: rc = step_object<256>(ws, L, sp, (const __half*)image, b, st, err); break;
-      default: err = "layer-wise path: hidden must be 64, 128 or 256"; return VMB_E_UNSUPPORTED;
-    }
-    if (rc) return rc;
-  }
-  return 0;
+  return for_hidden(L.H, "layer-wise path", err, [&](auto h) -> int {
+    if (sp.S > 32) { err = "layer-wise path: n_samples > 32"; return VMB_E_UNSUPPORTED; }
+    LW_TRY(ws.grow((long long)sp.R * sp.S, L.H, stream_capturing(st)));
+    for (int b = 0; b < sp.B; ++b)
+      if (const int rc = step_object<decltype(h)::value>(ws, L, sp, (const __half*)image, b, st, err)) return rc;
+    return 0;
+  });
 }
-#undef LW_TRY
 
 }  // namespace lw

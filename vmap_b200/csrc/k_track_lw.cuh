@@ -9,20 +9,22 @@
 //   Weights  object b reads params row rows[b] and the fp16 image row rows[b] (as the AdamW launch writes it).  Both
 //            are copied on the device into this path's workspace first, so rows[] stays a device array (capturable);
 //            a row outside [0, n_rows) contributes nothing and sets VMB_TRACK_ST_BAD_ROW, as K10.
-//   Points   pose_point: p = R q + t from an fp32 copy of the fp64 pose, then p / scale; the embedding row
-//            is k_lw_pe's (fp16, sin by sincos_ladder6, constant-1 columns).  K11: the ray's pose is its draw's frame
-//            (ba_draw_frame); a ray whose frame is outside the table contributes nothing and sets VMB_BA_ST_BAD_FRAME.
+//   Points   pose_point: p = R q + t from an fp32 copy of the fp64 pose, then p / scale; the embedding block is
+//            k_lw_pe's pe_block (fp16, sin by sincos_ladder6, constant-1 columns).  K11: the ray's pose is its draw's
+//            frame (ba_draw_frame); a ray whose frame is outside the table contributes nothing and sets
+//            VMB_BA_ST_BAD_FRAME.
 //   Network  the five forward GEMMs of step_object (fp16 operands, fp32 accumulation, fp16 activations).
-//   Render   one warp per ray, lane = sample (S <= 32): the heads in fp32 from the fp16 activations; the composite,
-//            render in fp64 in sample order exactly as K10 (1 - occ as sigmoid(-alpha)) and ray_loss on it; mask counts
-//            of this slice per object (integers); the backward to (raw alpha, raw colour) in fp32 as K10.  Each ray's three
-//            loss terms go to an fp64 per-ray buffer.  d(raw alpha) and dYc are loss-scaled by LS = 2^8 and clamped to
-//            the fp16 range +-60000 as in the training kernel.  status[1] gets a LOWER BOUND on the clamped values
-//            (and VMB_TRACK_ST_CLAMP is set when it is not 0): every clamped dYc element, plus every element where the
-//            rank-1 term LS d(raw alpha) W_a of dY4 passes 60000 on its own; the saturating packs of the dY4..dY1
-//            GEMM epilogues are not counted.  No head weight gradients.
-//   Backward the input-gradient GEMM chain of step_object only (colour-block dE, dY4 with the rank-1 d_alpha term, dY3,
-//            dY2, dY1, the fused dE GEMM): no weight-gradient GEMMs, no column sums, no side stream.
+//   Render   one warp per ray, lane = sample (S <= 32): the training kernel's HeadRows (row staging, the heads in fp32
+//            from the fp16 activations, the dYc gate and its store); the composite, render in fp64 in sample order
+//            exactly as K10 (1 - occ as sigmoid(-alpha)) and ray_loss on it; mask counts of this slice per object
+//            (integers); the backward to (raw alpha, raw colour) in fp32 as K10.  Each ray's three loss terms go to an
+//            fp64 per-ray buffer.  d(raw alpha) and dYc are loss-scaled by LS = 2^8 and clamped to the fp16 range
+//            +-60000 as in the training kernel.  status[1] gets a LOWER BOUND on the clamped values (and
+//            VMB_TRACK_ST_CLAMP is set when it is not 0), the count HeadRows::gate returns: every clamped dYc element,
+//            plus every element where the rank-1 term LS d(raw alpha) W_a of dY4 passes 60000 on its own; the
+//            saturating packs of the dY4..dY1 GEMM epilogues are not counted.  No head weight gradients.
+//   Backward step_object's input-gradient chain (InputGrads: colour-block dE, dY4 with the rank-1 d_alpha term, dY3,
+//            dY2, dY1, the fused dE GEMM) back to back: no weight-gradient GEMMs, no column sums, no side stream.
 //   Pose     per point dL/dt = INV_LS (dE_xyz + sum_{k,d} dE_{k,d} pi 2^k cos(pi 2^k proj_d) B_d) in fp32 (the cosines
 //            of sincos_ladder6, as k_lw_pe_bwd), then pose_terms: ((R q) x g, g), g = dL/dt / scale, in fp64 from the
 //            fp64 pose.  Track flavour: the terms are summed in point order over the rays of each of K10's tiles
@@ -30,8 +32,9 @@
 //            partial rows.  BA flavour: one row per ray (its samples in order), as K11.
 // No floating-point atomics anywhere on this path (the GEMM epilogues used here store): bitwise reproducible.
 // Registers (ptxas -v, sm_90a; track / BA flavour), no spills in any of them:
-//   k_tlw_gather 32; k_tlw_pe 74 / 74; k_tlw_render H 64: 67 / 68, H 128: 67 / 68, H 256: 67 / 68;
-//   k_tlw_pose 62 / 62; k_tlw_reduce 40 / 40; the joint step's k_joint_world 32 (it runs k_tlw_pose / k_tlw_reduce<true>).
+//   k_tlw_gather 32; k_tlw_pe 74 / 74; k_tlw_render 67 / 68 at every H; k_tlw_pose 62 / 62; k_tlw_reduce 40 / 40;
+//   the joint step's k_joint_world 32 (it runs k_tlw_pose / k_tlw_reduce<true>).  The training step's kernels on the
+//   same helpers: k_lw_pe 74, k_lw_heads_render 62 / 62 / 61 at H 64 / 128 / 256 (it drops HeadRows::gate's count).
 #pragma once
 #include "k_layerwise.cuh"
 #include "k_track.cuh"
@@ -114,19 +117,11 @@ __global__ void __launch_bounds__(128) k_tlw_pe(TlwObj o, const float* __restric
   ptx::pdl_launch_dependents();
   const long long P = (long long)o.R * o.S;
   const float sc = __int_as_float(ctl[4]);
-  const float* dirs = prow + o_B;
-  __shared__ __align__(16) __half row[128 * EW];
-  const long long p0 = (long long)blockIdx.x * 128, p = p0 + threadIdx.x;
-  __half* r = row + threadIdx.x * EW;
+  const long long p = (long long)blockIdx.x * 128 + threadIdx.x;
   float3 q, t = make_float3(0.f, 0.f, 0.f);
   const double* T;
   if (p < P) tlw_point<BA>(o, p, sc, q, t, T);
-  pe_row(r, t.x, t.y, t.z, dirs);                    // k_lw_pe's row
-  __syncthreads();
-  const uint4* src = reinterpret_cast<const uint4*>(row);
-  uint4* dst = reinterpret_cast<uint4*>(E + p0 * EW);
-  const long long n16 = min(128LL, P - p0) * (EW * 2 / 16);
-  for (long long i = threadIdx.x; i < n16; i += 128) dst[i] = src[i];
+  pe_block(t.x, t.y, t.z, prow + o_B, P, E);
 }
 
 // ---- 3: heads + fp64 render + loss + d(raw alpha, raw colour) -> dalpha_s, dYc; one warp per ray, lane = sample ------
@@ -141,62 +136,25 @@ __global__ void __launch_bounds__(128) k_tlw_render(TlwObj o, TlwRender a, const
   ptx::pdl_wait();
   ptx::pdl_launch_dependents();
   extern __shared__ __align__(16) unsigned char hr_rows[];
-  __shared__ float w[4 * H];                          // [0,H) out_alpha row, [H,4H) out_color rows
-  constexpr int PITCH = hr_pitch<H>(), LPR = H / 8, RPP = 32 / LPR;
-  for (int i = threadIdx.x; i < H; i += 128) w[i] = P[L.o_Wa + i];
-  for (int i = threadIdx.x; i < 3 * H; i += 128) w[H + i] = P[L.o_Woc + i];
-  __syncthreads();
+  __shared__ float w[4 * H];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, S = o.S;
+  HeadRows<H> hr{w, hr_rows + warp * (32 * HeadRows<H>::PITCH), lane, S};
+  hr.load(P, L);
+  __syncthreads();
   const unsigned FULL = 0xffffffffu;
   const float b_a = P[L.o_ba], b_c0 = P[L.o_boc], b_c1 = P[L.o_boc + 1], b_c2 = P[L.o_boc + 2];
   const int cnt[3] = {ctl[0], ctl[1], ctl[2]};
   const bool in = lane < S;
-  unsigned char* srow = hr_rows + warp * (32 * PITCH);
   int n_clamp = 0;
-  auto stage_rows = [&](const __half* X, long long pb) {
-#pragma unroll 4
-    for (int r0 = 0; r0 < S; r0 += RPP) {
-      const int r = r0 + lane / LPR, cq = lane % LPR;
-      if (r < S) cp_async16(srow + r * PITCH + cq * 16, X + (pb + r) * H + cq * 8);
-    }
-    asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
-    __syncwarp();
-  };
-  const uint4* xrow = reinterpret_cast<const uint4*>(srow + lane * PITCH);
   for (int ray = blockIdx.x * 4 + warp; ray < o.R; ray += gridDim.x * 4) {
     const long long pb = (long long)ray * S, pi = pb + lane;
-    __syncwarp();
-    stage_rows(X4, pb);
+    hr.stage(X4, pb);
     float ha = 0.f, h0 = 0.f, h1 = 0.f, h2 = 0.f;
-    if (in) {
-      float hb = 0.f;
-#pragma unroll 4
-      for (int q = 0; q < H / 8; ++q) {
-        const uint4 u = xrow[q];
-        const __half* hu = reinterpret_cast<const __half*>(&u);
-#pragma unroll
-        for (int j = 0; j < 8; j += 2) {
-          ha = fmaf(__half2float(hu[j]), w[q * 8 + j], ha);
-          hb = fmaf(__half2float(hu[j + 1]), w[q * 8 + j + 1], hb);
-        }
-      }
-      ha += hb;
-    }
-    __syncwarp();
-    stage_rows(XC, pb);
+    if (in) ha = hr.alpha();
+    hr.stage(XC, pb);
     float al = 0.f, oc = 0.f, zz = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f;
     if (in) {
-#pragma unroll 4
-      for (int q = 0; q < H / 8; ++q) {
-        const uint4 v = xrow[q];
-        const __half* hv = reinterpret_cast<const __half*>(&v);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float fc = __half2float(hv[j]);
-          const int oo = q * 8 + j;
-          h0 = fmaf(fc, w[H + oo], h0); h1 = fmaf(fc, w[2 * H + oo], h1); h2 = fmaf(fc, w[3 * H + oo], h2);
-        }
-      }
+      hr.colour(h0, h1, h2);
       al = (ha + b_a) * 10.0f;                        // model.py:77
       oc = vmb_sigmoid(al);                           // render_rays.py:6
       c0 = vmb_sigmoid(h0 + b_c0); c1 = vmb_sigmoid(h1 + b_c1); c2 = vmb_sigmoid(h2 + b_c2);
@@ -238,35 +196,9 @@ __global__ void __launch_bounds__(128) k_tlw_render(TlwObj o, TlwRender a, const
       const float dy0 = gC0 * wf * c0 * (1.f - c0), dy1 = gC1 * wf * c1 * (1.f - c1), dy2 = gC2 * wf * c2 * (1.f - c2);
       const float da = LS * dx;
       dalpha_s[pi] = da;
-      uint4* xc = const_cast<uint4*>(xrow);           // the staged hc row, gated in place
-      const float d0 = LS * dy0, d1 = LS * dy1, d2 = LS * dy2;
-#pragma unroll 4
-      for (int q = 0; q < H / 8; ++q) {
-        const uint4 v = xc[q];
-        const __half* hv = reinterpret_cast<const __half*>(&v);
-        uint32_t r[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int oo = q * 8 + 2 * j;
-          float x0 = fmaf(d2, w[3 * H + oo], fmaf(d1, w[2 * H + oo], d0 * w[H + oo]));
-          float x1 = fmaf(d2, w[3 * H + oo + 1], fmaf(d1, w[2 * H + oo + 1], d0 * w[H + oo + 1]));
-          const bool g0 = __half2float(hv[2 * j]) > 0.f, g1 = __half2float(hv[2 * j + 1]) > 0.f;
-          n_clamp += (g0 && fabsf(x0) > 60000.f) + (g1 && fabsf(x1) > 60000.f);
-          n_clamp += (fabsf(da * w[oo]) > 60000.f) + (fabsf(da * w[oo + 1]) > 60000.f);
-          x0 = g0 ? fminf(fmaxf(x0, -60000.f), 60000.f) : 0.f;
-          x1 = g1 ? fminf(fmaxf(x1, -60000.f), 60000.f) : 0.f;
-          __half2 hh = __floats2half2_rn(x0, x1);
-          r[j] = *reinterpret_cast<uint32_t*>(&hh);
-        }
-        xc[q] = make_uint4(r[0], r[1], r[2], r[3]);
-      }
+      n_clamp += hr.gate(LS * dy0, LS * dy1, LS * dy2, da);
     }
-    __syncwarp();
-#pragma unroll 4
-    for (int r0 = 0; r0 < S; r0 += RPP) {
-      const int r = r0 + lane / LPR, cq = lane % LPR;
-      if (r < S) *reinterpret_cast<uint4*>(dYc + (pb + r) * H + cq * 8) = *reinterpret_cast<const uint4*>(srow + r * PITCH + cq * 16);
-    }
+    hr.store(dYc, pb);
   }
   for (int d = 16; d > 0; d >>= 1) n_clamp += __shfl_xor_sync(FULL, n_clamp, d);
   if (lane == 0 && n_clamp && o.status) { atomicOr(o.status, VMB_TRACK_ST_CLAMP); atomicAdd(o.status + 1, n_clamp); }
@@ -349,16 +281,13 @@ struct TlwGroup {
   int nr;                        // track flavour: rays per K10 tile
 };
 
-#define TLW_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return VMB_E_CUDA; } } while (0)
-
 template <int H, bool BA>
 static int track_object_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGroup& G, int b, cudaStream_t st, std::string& err) {
   const TrackParams& a = G.tp;
   Workspace& ws = tw.w;
   const long long np = (long long)a.R * a.S;
   const int nblk = (int)((np + 127) / 128);
-  const bool pdl_ok = np <= 65536;                   // step_object's rule
-  auto arm = [&]() { if (pdl_ok) pdl_arm(); };
+  auto arm = [&]() { if (pdl_ok(np)) pdl_arm(); };
   TlwObj o;
   o.b = b; o.R = a.R; o.S = a.S; o.n_rows = a.n_rows; o.rows = a.rows;
   o.pcs = a.pcs + (size_t)b * a.pcs_stride; o.pose = a.pose; o.status = a.status;
@@ -371,68 +300,61 @@ static int track_object_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGrou
   int dev = 0;
   cudaGetDevice(&dev);
   const int n_sm = sm_count(dev);
-  TLW_TRY(launch_k(k_tlw_gather, dim3((unsigned)std::min<long long>(2 * n_sm, (halves / 8 + 255) / 256)), dim3(256), 0, st, o,
-                   a.params, a.scale, G.image, sem, mask, L.stride, halves, tw.prow, tw.wimg, tw.ctl));
+  LW_TRY(launch_k(k_tlw_gather, dim3((unsigned)std::min<long long>(2 * n_sm, (halves / 8 + 255) / 256)), dim3(256), 0, st, o,
+                  a.params, a.scale, G.image, sem, mask, L.stride, halves, tw.prow, tw.wimg, tw.ctl));
   arm();
-  TLW_TRY(launch_k(k_tlw_pe<BA>, dim3(nblk), dim3(128), 0, st, o, (const float*)tw.prow, (const int*)tw.ctl, L.o_B, ws.E));
-  TLW_TRY(forward_gemms<H>(ws, L, tw.prow, tw.wimg, np, pdl_ok, st));
-  TLW_TRY((smem_limit_once<k_tlw_render<H, BA>>(dev, hr_smem<H>())));
+  LW_TRY(launch_k(k_tlw_pe<BA>, dim3(nblk), dim3(128), 0, st, o, (const float*)tw.prow, (const int*)tw.ctl, L.o_B, ws.E));
+  LW_TRY(forward_gemms<H>(ws, L, tw.prow, tw.wimg, np, st));
+  LW_TRY((smem_limit_once<k_tlw_render<H, BA>>(dev, hr_smem<H>())));
   TlwRender ra;
   ra.z = a.z + (size_t)b * a.z_stride; ra.gt_depth = a.gt_depth + (size_t)b * a.gt_depth_stride;
   ra.gt_colour = a.gt_colour + (size_t)b * a.gt_colour_stride; ra.sem = sem; ra.mask = mask; ra.cs = a.cs; ra.os = a.os;
-  const int hr_per_sm = std::max(1, std::min(8, (int)(227 * 1024 / (hr_smem<H>() + 6 * 1024))));
   arm();
-  TLW_TRY(launch_k(k_tlw_render<H, BA>, dim3(std::min((a.R + 3) / 4, n_sm * hr_per_sm)), dim3(128), (size_t)hr_smem<H>(), st,
-                   o, ra, (const __half*)ws.X4, (const __half*)ws.XC, (const float*)tw.prow, L, (const int*)tw.ctl, ws.dYc,
-                   ws.dalpha_s, tw.lossr));
-  // backward to the embedding only, the input-gradient chain of step_object
+  LW_TRY(launch_k(k_tlw_render<H, BA>, dim3(hr_blocks<H>(a.R, n_sm)), dim3(128), (size_t)hr_smem<H>(), st,
+                  o, ra, (const __half*)ws.X4, (const __half*)ws.XC, (const float*)tw.prow, L, (const int*)tw.ctl, ws.dYc,
+                  ws.dalpha_s, tw.lossr));
+  // backward to the embedding only: step_object's input-gradient chain, each GEMM following the last directly
+  const InputGrads<H> ig{ws, tw.wimg, tw.prow + L.o_Wa, np, st};
   arm();
-  TLW_TRY(dgrad_emb_gemm<H>(ws, ws.dYc, tw.wimg, off_cl(H) + H, H + 48, E2W, E1W, 0, np, st));        // colour block of dE
+  LW_TRY(ig.de_colour());
   arm();
-  TLW_TRY(dgrad_gate_gemm<H>(ws.dYc, tw.wimg, off_cl(H), H + 48, np, ws.X4, ws.dYa, ws.dalpha_s, tw.prow + L.o_Wa, st));  // dY4
+  LW_TRY(ig.dy4());
   arm();
-  TLW_TRY(dgrad_gate_gemm<H>(ws.dYa, tw.wimg, off_m2(H), H, np, ws.X3, ws.dYb, nullptr, nullptr, st));    // dY3 -> dYb
+  LW_TRY(ig.dy3());
   arm();
-  TLW_TRY(dgrad_gate_gemm<H>(ws.dYb, tw.wimg, off_cat(H), H + 96, np, ws.X2, ws.dYa, nullptr, nullptr, st));  // dY2 -> dYa
+  LW_TRY(ig.dy2());
   arm();
-  TLW_TRY(dgrad_gate_gemm<H>(ws.dYa, tw.wimg, off_m1(H), H, np, ws.X1, ws.dYc, nullptr, nullptr, st));    // dY1 -> dYc
+  LW_TRY(ig.dy1());
   arm();
-  TLW_TRY(demb1_gemm<H>(ws, ws.dYb, ws.dYc, tw.wimg, np, st));                                           // d emb1
-  TLW_TRY(smem_limit_once<k_tlw_pose<BA>>(dev, PEB_SMEM));
+  LW_TRY(ig.demb1());
+  LW_TRY(smem_limit_once<k_tlw_pose<BA>>(dev, PEB_SMEM));
   arm();
-  TLW_TRY(launch_k(k_tlw_pose<BA>, dim3(nblk), dim3(128), (size_t)PEB_SMEM, st, o, (const float*)tw.prow, (const int*)tw.ctl, L.o_B,
+  LW_TRY(launch_k(k_tlw_pose<BA>, dim3(nblk), dim3(128), (size_t)PEB_SMEM, st, o, (const float*)tw.prow, (const int*)tw.ctl, L.o_B,
                    (const float*)ws.dE, tw.gpt));
   const int n_out = BA ? a.R : (a.R + G.nr - 1) / G.nr;
   double* out = BA ? G.x.rows + (size_t)b * a.R * VMB_TRACK_PART : a.partials + (size_t)b * n_out * VMB_TRACK_PART;
   arm();
-  TLW_TRY(launch_k(k_tlw_reduce<BA>, dim3((n_out + 127) / 128), dim3(128), 0, st, o, G.nr, n_out, (const int*)tw.ctl,
-                   (const double*)tw.gpt, (const double*)tw.lossr, out));
-  TLW_TRY(cudaGetLastError());
+  LW_TRY(launch_k(k_tlw_reduce<BA>, dim3((n_out + 127) / 128), dim3(128), 0, st, o, G.nr, n_out, (const int*)tw.ctl,
+                  (const double*)tw.gpt, (const double*)tw.lossr, out));
+  LW_TRY(cudaGetLastError());
   return 0;
 }
 
 template <bool BA>
 static int launch_track_lw(TrackWorkspace& tw, const VmbLayout& L, const TlwGroup& G, cudaStream_t st, std::string& err) {
-  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return VMB_E_CUDA; }
-  const long long R = G.tp.R, P = R * G.tp.S;
-  const bool capturing = stream_capturing(st);
-  TLW_TRY(tw.w.grow(P, L.H, capturing));
-  TLW_TRY(tw.prow.grow((size_t)L.stride * 4, capturing));
-  TLW_TRY(tw.wimg.grow((size_t)img_halves(L.H) * 2, capturing));
-  TLW_TRY(tw.ctl.grow(8 * sizeof(int), capturing));
-  TLW_TRY(tw.lossr.grow((size_t)R * 3 * sizeof(double), capturing));
-  TLW_TRY(tw.gpt.grow((size_t)pad_points(P) * 6 * sizeof(double), capturing));
-  for (int b = 0; b < G.tp.B; ++b) {
-    int rc;
-    switch (L.H) {
-      case 64:  rc = track_object_lw<64, BA>(tw, L, G, b, st, err); break;
-      case 128: rc = track_object_lw<128, BA>(tw, L, G, b, st, err); break;
-      case 256: rc = track_object_lw<256, BA>(tw, L, G, b, st, err); break;
-      default: err = "layer-wise tracking: hidden must be 64, 128 or 256"; return VMB_E_UNSUPPORTED;
-    }
-    if (rc) return rc;
-  }
-  return 0;
+  return for_hidden(L.H, "layer-wise tracking", err, [&](auto h) -> int {
+    const long long R = G.tp.R, P = R * G.tp.S;
+    const bool capturing = stream_capturing(st);
+    LW_TRY(tw.w.grow(P, L.H, capturing));
+    LW_TRY(tw.prow.grow((size_t)L.stride * 4, capturing));
+    LW_TRY(tw.wimg.grow((size_t)img_halves(L.H) * 2, capturing));
+    LW_TRY(tw.ctl.grow(8 * sizeof(int), capturing));
+    LW_TRY(tw.lossr.grow((size_t)R * 3 * sizeof(double), capturing));
+    LW_TRY(tw.gpt.grow((size_t)pad_points(P) * 6 * sizeof(double), capturing));
+    for (int b = 0; b < G.tp.B; ++b)
+      if (const int rc = track_object_lw<decltype(h)::value, BA>(tw, L, G, b, st, err)) return rc;
+    return 0;
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -528,47 +450,42 @@ static int joint_object_lw(Workspace& ws, JointWorkspace& jw, const VmbLayout& L
   o.n_pix_draw = x.n_pix_draw; o.n_poses = x.n_poses; o.kf_stride = x.kf_stride;
   o.kf_draw = x.kf_draw + (size_t)b * x.kf_draw_stride;
   o.kf_frame = x.kf_frame + (size_t)b * x.kf_stride;
-  TLW_TRY(launch_k(k_joint_world, dim3((unsigned)((np + 255) / 256)), dim3(256), 0, st, o, 0LL, 0LL, sp.scale, jw.pw,
-                   pw_out ? pw_out + (size_t)b * np * 3 : nullptr, jw.ctl));
+  LW_TRY(launch_k(k_joint_world, dim3((unsigned)((np + 255) / 256)), dim3(256), 0, st, o, 0LL, 0LL, sp.scale, jw.pw,
+                  pw_out ? pw_out + (size_t)b * np * 3 : nullptr, jw.ctl));
   StepParams s1 = sp;
   s1.pcs = jw.pw; s1.pcs_stride = 0;                // step_object reads object b's points at pcs + b * pcs_stride
   const int rc = step_object<H>(ws, L, s1, image, b, st, err);
   if (rc) return rc;
   int dev = 0;
   cudaGetDevice(&dev);
-  TLW_TRY(smem_limit_once<k_tlw_pose<true>>(dev, PEB_SMEM));
+  LW_TRY(smem_limit_once<k_tlw_pose<true>>(dev, PEB_SMEM));
   // after step_object's join with its side stream: an ordinary launch
-  TLW_TRY(launch_k(k_tlw_pose<true>, dim3((unsigned)((np + 127) / 128)), dim3(128), (size_t)PEB_SMEM, st, o,
-                   sp.params + (size_t)b * L.stride, (const int*)jw.ctl, L.o_B, (const float*)ws.dE, jw.gpt));
-  if (np <= 65536) pdl_arm();                       // step_object's rule
-  TLW_TRY(launch_k(k_tlw_reduce<true>, dim3((sp.R + 127) / 128), dim3(128), 0, st, o, 1, sp.R, (const int*)jw.ctl,
-                   (const double*)jw.gpt, (const double*)nullptr, x.rows + (size_t)b * sp.R * VMB_TRACK_PART));
-  TLW_TRY(cudaGetLastError());
+  LW_TRY(launch_k(k_tlw_pose<true>, dim3((unsigned)((np + 127) / 128)), dim3(128), (size_t)PEB_SMEM, st, o,
+                  sp.params + (size_t)b * L.stride, (const int*)jw.ctl, L.o_B, (const float*)ws.dE, jw.gpt));
+  if (pdl_ok(np)) pdl_arm();
+  LW_TRY(launch_k(k_tlw_reduce<true>, dim3((sp.R + 127) / 128), dim3(128), 0, st, o, 1, sp.R, (const int*)jw.ctl,
+                  (const double*)jw.gpt, (const double*)nullptr, x.rows + (size_t)b * sp.R * VMB_TRACK_PART));
+  LW_TRY(cudaGetLastError());
   return 0;
 }
 
 static int launch_joint_lw(Workspace& ws, JointWorkspace& jw, const VmbLayout& L, const StepParams& sp, const BaRays& x,
                            const double* poses, int* status, const void* image, float* pw_out, cudaStream_t st,
                            std::string& err) {
-  if (!get_encode()) { err = "cuTensorMapEncodeTiled not available from the driver"; return VMB_E_CUDA; }
-  const long long np = (long long)sp.R * sp.S, Pp = pad_points(np);
-  const bool capturing = stream_capturing(st);
-  TLW_TRY(ws.grow(np, L.H, capturing));
-  TLW_TRY(jw.pw.grow((size_t)Pp * 3 * sizeof(float), capturing));
-  TLW_TRY(jw.ctl.grow(8 * sizeof(int), capturing));
-  TLW_TRY(jw.gpt.grow((size_t)Pp * 6 * sizeof(double), capturing));
-  for (int b = 0; b < sp.B; ++b) {
-    int rc;
-    switch (L.H) {
-      case 64:  rc = joint_object_lw<64>(ws, jw, L, sp, x, poses, status, (const __half*)image, b, pw_out, st, err); break;
-      case 128: rc = joint_object_lw<128>(ws, jw, L, sp, x, poses, status, (const __half*)image, b, pw_out, st, err); break;
-      case 256: rc = joint_object_lw<256>(ws, jw, L, sp, x, poses, status, (const __half*)image, b, pw_out, st, err); break;
-      default: err = "joint step: hidden must be 64, 128 or 256"; return VMB_E_UNSUPPORTED;
-    }
-    if (rc) return rc;
-  }
-  return 0;
+  return for_hidden(L.H, "joint step", err, [&](auto h) -> int {
+    const long long np = (long long)sp.R * sp.S, Pp = pad_points(np);
+    const bool capturing = stream_capturing(st);
+    LW_TRY(ws.grow(np, L.H, capturing));
+    LW_TRY(jw.pw.grow((size_t)Pp * 3 * sizeof(float), capturing));
+    LW_TRY(jw.ctl.grow(8 * sizeof(int), capturing));
+    LW_TRY(jw.gpt.grow((size_t)Pp * 6 * sizeof(double), capturing));
+    for (int b = 0; b < sp.B; ++b)
+      if (const int rc = joint_object_lw<decltype(h)::value>(ws, jw, L, sp, x, poses, status, (const __half*)image, b, pw_out,
+                                                             st, err))
+        return rc;
+    return 0;
+  });
 }
-#undef TLW_TRY
+#undef LW_TRY
 
 }  // namespace lw
